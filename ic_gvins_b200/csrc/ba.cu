@@ -10,10 +10,11 @@
 //
 // Per window: n = 15K+7 camera-side columns laid out [pose_0..pose_{K-1} (6 each) | extrinsic 6 | td 1 | mix_0..mix_{K-1} (9 each)];
 // the vision factors only touch the first NCV = 6K+7 ("vision columns").  Landmarks (inverse depths) are eliminated:
-//   lin_vis    : thread / reprojection factor -> residual, local Jacobians, Huber correction -> 40-double record
-//   lin_lm     : warp / landmark -> h_l, g_l and the dense coupling row w_l (A_W, landmark-major)
-//   pair_gram  : factors grouped by (reference node, observing node): 20x20 Gram matrix per group on the FP64 tensor cores
-//                (DMMA.8x8x4), then a one-writer-per-entry gather into the vision part of H_cc and g_c
+//   lin_vis    : CTA / run of landmarks of one reference node: thread / reprojection factor -> residual, local Jacobians, Huber
+//                correction -> record in shared memory; per (reference node, observing node) pair the 20x20 Gram matrix of the run's
+//                records on the FP64 tensor cores (DMMA.8x8x4), summed over the node's runs in run order;
+//                lanes / landmark -> h_l, g_l and the dense coupling row w_l (A_W, landmark-major)
+//   pair_gram  : one-writer-per-entry gather of the pair Gram matrices into the vision part of H_cc and g_c
 //   schur_dmma : sum_l phi_l w_l w_l^T with phi_l = s_l^2 / (s_l^2 h_l + D_l^2) on the FP64 tensor cores
 //   lin_cam    : one CTA / window (second stream, beside the vision chain) -> IMU preintegration, GNSS, bias, prior and
 //                marginalization factors -> H_c, g_c
@@ -49,6 +50,7 @@ constexpr int BA_MAX_NODES = 32;  // icg_ba_create: max_K <= 32
 struct BaCaps {
     int NW, K, L, F, G, R;     // capacities
     int NCV, N, NS, NCA, RJ, LP, NVB;  // derived strides: NCV = 6K+7, N = 15K+7, NS = N padded, NCA = roundup4(NCV+1), RJ = 2F padded, LP = L padded
+    int GQ;                            // Gram partials per window: one per (lin_vis run, observing node) <= min(F, runs x (K - 1))
 };
 
 struct WinDims {  // per-window actual sizes
@@ -85,14 +87,21 @@ struct BaDev {  // device pointers (flat, capacity-strided by window)
     uint8_t *f_active_0;                     // pristine copies of what the two-pass protocol mutates (restart re-solves the UPLOADED problem)
     double *gnss_std_0;
     uint8_t *f_active;                       // by factor id
-    int *lm_off;  // CSR offsets of the factor records by landmark
-    int *vb_lm0;  // [NW][NVB] first landmark of every lin_vis run (runs hold whole landmarks, <= 128 factors); last entry = run count
+    // landmark POSITIONS: the window's landmarks ordered by reference node, stable by id (landmarks without factors last); record slots
+    // follow that order.  Arrays indexed by landmark id (rho, h_l, g_l, scale_l, A_W rows) keep the id.
+    int *lm_off;  // CSR offsets of the factor records by landmark position
+    int *lm_perm; // [NW][L] landmark id at each position
+    int *vb_lm0;  // [NW][NVB] first landmark position of every lin_vis run (whole landmarks of ONE reference node, <= 128 factors); last entry = run count
+    int *ref_nrun;       // [NW][K] lin_vis runs per reference node
     int *f_meta_s;       // per record slot: (landmark, reference node, observing node, factor id)
     double *f_const_s;   // per record slot: the factor's 14 constants (copy of f_const in slot order)
-    int *pair_off, *pair_ro, *pair_fidx, *npairs;  // factors grouped by (reference node, observing node)
+    int *vis_ord;        // per record slot: the run's slots ordered by observing node (stable): run-local slot | Gram partial index << 8
+    int *part_off, *pair_ro, *npairs;  // (reference node, observing node) pairs: CSR offsets of their Gram partials (in run order), (ref << 8 | obs), count
+    double *gpart;       // [NW][GQ][210] Gram partial of one (run, observing node): packed upper 20x20
+    int *vis_cnt;        // [NW][K] lin_vis runs of the reference node arrived (the last one resets it)
     double *Mp;                                    // per-pair 20x20 Gram matrices (upper, 210 entries)
     double *AW, *CJ, *CW;  // Schur SYRK input; vision Gram matrix; Schur partials
-    double *jcomp, *costf;  // per-factor record (40 doubles, landmark-CSR order), cost
+    double *costf;         // per-factor cost
     double *hl, *gl, *scale_l, *scale_c;
     double *Hc, *gc;
     double *Hs;  // H_c + vision Gram - Schur term (lower triangle, ld NS): the operand ba_solve scales and factorises
@@ -120,19 +129,33 @@ __device__ __forceinline__ int col_mix(int K, int k) { return 6 * K + 7 + 9 * k;
 // ------------------------------------------------------------------------------------------------ lin_vis (+ landmark rows)
 __device__ __forceinline__ int jc_off(int a) { return a < 18 ? (a / 6) * 12 + (a % 6) : 36 + 2 * (a - 18); }  // row 0 offset in a record
 __device__ __forceinline__ int jc_row1(int a) { return a < 18 ? 6 : 1; }                                           // + this for row 1
-// One CTA linearises a run of WHOLE landmarks (<= 128 reprojection factors; the host packs the runs at upload).
-//  phase 1: thread / factor, in record (landmark-CSR slot) order -> residual, local Jacobians, Huber correction -> 40-double record
+__device__ __forceinline__ int tri20(int la, int lb) {  // index of (la <= lb) in the packed upper 20x20
+    return la * 20 - la * (la - 1) / 2 + (lb - la);
+}
+__device__ __forceinline__ void dmma884(double &c0, double &c1, double a, double b) {
+    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
+}
+// One CTA linearises a run of WHOLE landmarks of ONE reference node (<= 128 reprojection factors; the host packs the runs at upload).
+//  phase 1: thread / factor, in record slot order -> residual, local Jacobians, Huber correction -> 40-double record
 //           [Ji 12 | Jj 12 | Je 12 | Jt 2 | r 2] + [j_rho 2 | observing node | reference node], staged in shared memory;
-//  phase 2: the records leave as contiguous, fully used 128-byte lines (a thread-per-record store pattern costs 32 sectors per
-//           instruction and made the store pipe the bottleneck) -- ba_pair_gram1 consumes them;
+//  phase 2: the Gram matrices of the run.  Within a (reference node, observing node) pair every factor has the same 19 camera-side columns
+//           [ref pose 6 | obs pose 6 | extrinsic 6 | td 1] (+ the residual as a 20th column), so the pair's contribution is the dense
+//           20x20 Gram matrix X^T X of its stacked 2x20 rows: one warp per observing node of the run, 4 rows (2 factors) per DMMA.8x8x4
+//           k-step.  With the m8n8k4 fragment layout (A: lane -> (row lane/4, k lane%4); B: lane -> (k lane%4, col lane/4)) the A and
+//           B operands of X^T X are the SAME register: lane loads X[k = lane%4][8 t + lane/4] for the three column tiles t and issues
+//           the six upper-triangular tile products.  The packed result is the run's partial of that pair (D.gpart);
 //  phase 3: eight lanes per landmark reduce its records, straight from shared memory, to h_l, g_l and the coupling row
 //           w_l[c] = sum_f J_f[:, c]^T j_rho,f of A_W (landmark-major [l][NCA]: zeroed, then the <= 13 + 6 n_obs non-zeros).  All
 //           factors of a landmark share the reference node, the extrinsic and td (accumulated); each observing node appears once
-//           (written directly; icg_ba_upload checks it).
+//           (written directly; icg_ba_upload checks it);
+//  phase 4: the last run of the reference node to arrive (arrival counter) sums the node's partials of every pair in run order -> Mp.
+//           No floating-point atomics: the result does not depend on which CTA arrives last, nor on the other windows of the batch.
+// The Jacobians never leave the SM: per factor only the cost is stored.
 constexpr int LV_LD = 45;  // shared-memory record row: 44 doubles padded to an odd length (conflict-free)
 constexpr size_t LV_SMEM = sizeof(double) * (128 * LV_LD + (BA_MAX_NODES + 1) * NODE_FRAME_LD);  // records + node frames (49.5 KB: dynamic, opted in at create)
 __global__ void __launch_bounds__(128, 4) ba_lin_vis(BaCaps C, BaDev D) {
     extern __shared__ double lv_sm[];
+    __shared__ int s_ord[128], s_gbeg[BA_MAX_NODES], s_gend[BA_MAX_NODES], s_last, s_p0, s_np;
     double (*s_rec)[LV_LD] = (double (*)[LV_LD]) lv_sm;
     double (*s_frame)[NODE_FRAME_LD] = (double (*)[NODE_FRAME_LD]) (lv_sm + 128 * LV_LD);
     const int w = blockIdx.y;
@@ -143,10 +166,12 @@ __global__ void __launch_bounds__(128, 4) ba_lin_vis(BaCaps C, BaDev D) {
     const WinDims dm = D.dims[w];
     const int tid = threadIdx.x;
     const int *off = D.lm_off + (size_t) w * (C.L + 1);
-    const int lmA = vb[blockIdx.x], lmB = vb[blockIdx.x + 1];
-    const int s0 = off[lmA], nslot = off[lmB] - s0;
+    const int pA = vb[blockIdx.x], pB = vb[blockIdx.x + 1];  // landmark positions of the run
+    const int s0 = off[pA], nslot = off[pB] - s0;
     // ---- phase 0: the window's K + 1 node frames (rotation matrix | position of every pose and of the extrinsic), once per CTA
     if (tid <= dm.K) node_frame(tid < dm.K ? D.pose + ((size_t) w * C.K + tid) * 7 : D.ext + (size_t) w * 8, s_frame[tid]);
+    if (tid < BA_MAX_NODES) s_gbeg[tid] = s_gend[tid] = 0;
+    if (tid == 0) s_np = 0;
     __syncthreads();
     // ---- phase 1
     if (tid < nslot) {
@@ -183,14 +208,63 @@ __global__ void __launch_bounds__(128, 4) ba_lin_vis(BaCaps C, BaDev D) {
     }
     __syncthreads();
     // ---- phase 2
-    {
-        double *gj = D.jcomp + ((size_t) w * C.F + s0) * 40;
-        for (int idx = tid; idx < nslot * 40; idx += 128) {
-            const int rr = idx / 40, k = idx - 40 * rr;
-            gj[idx] = s_rec[rr][k];
+    const int lane = tid & 31, warp = tid >> 5;
+    if (nslot > 0) {
+        if (tid < nslot) {  // slots [s_gbeg[o], s_gend[o]) of s_ord observe from node o
+            const int *ord = D.vis_ord + (size_t) w * C.F + s0;
+            const int v = ord[tid], ob = (int) s_rec[v & 255][42];
+            s_ord[tid] = v;
+            if (tid == 0 || (int) s_rec[ord[tid - 1] & 255][42] != ob) s_gbeg[ob] = tid;
+            if (tid == nslot - 1 || (int) s_rec[ord[tid + 1] & 255][42] != ob) s_gend[ob] = tid + 1;
         }
+        __syncthreads();
+        const int kk = lane & 3, g = lane >> 2;  // k index inside the step (factor kk/2, residual row kk%2), column inside the tile
+        int o[3];
+#pragma unroll
+        for (int t = 0; t < 3; t++) {
+            const int a = 8 * t + g;
+            o[t] = a < 20 ? jc_off(a) + (kk & 1) * jc_row1(a) : -1;
+        }
+        for (int ob = warp; ob < dm.K; ob += 4) {
+            const int beg = s_gbeg[ob], end = s_gend[ob];
+            if (beg == end) continue;
+            double c00[2] = {0, 0}, c01[2] = {0, 0}, c02[2] = {0, 0}, c11[2] = {0, 0}, c12[2] = {0, 0}, c22[2] = {0, 0};
+            constexpr int UNR = 2;  // k-steps in flight (4 factors)
+            for (int base = beg; base < end; base += 2 * UNR) {
+                double x[UNR][3];
+#pragma unroll
+                for (int u = 0; u < UNR; u++) {
+                    const int q = base + 2 * u + (kk >> 1);
+                    const bool ok = q < end;
+                    const double *rec = s_rec[ok ? s_ord[q] & 255 : 0];
+#pragma unroll
+                    for (int t = 0; t < 3; t++) x[u][t] = (ok && o[t] >= 0) ? rec[o[t]] : 0.0;
+                }
+#pragma unroll
+                for (int u = 0; u < UNR; u++) {
+                    dmma884(c00[0], c00[1], x[u][0], x[u][0]);
+                    dmma884(c01[0], c01[1], x[u][0], x[u][1]);
+                    dmma884(c02[0], c02[1], x[u][0], x[u][2]);
+                    dmma884(c11[0], c11[1], x[u][1], x[u][1]);
+                    dmma884(c12[0], c12[1], x[u][1], x[u][2]);
+                    dmma884(c22[0], c22[1], x[u][2], x[u][2]);
+                }
+            }
+            // C fragment: lane holds (row lane/4, cols 2 (lane%4) + {0,1}) of each 8x8 tile
+            double *pp = D.gpart + ((size_t) w * C.GQ + (s_ord[beg] >> 8)) * 210;
+            auto put = [&](int ti, int tj, const double *c) {
+#pragma unroll
+                for (int e = 0; e < 2; e++) {
+                    const int la = 8 * ti + g, lb = 8 * tj + 2 * kk + e;
+                    if (la <= lb && lb < 20) pp[tri20(la, lb)] = c[e];
+                }
+            };
+            put(0, 0, c00), put(0, 1, c01), put(0, 2, c02), put(1, 1, c11), put(1, 2, c12), put(2, 2, c22);
+        }
+        __threadfence();  // the partials are visible device-wide before this run is counted (phase 4)
     }
     // ---- phase 3
+    const int *perm = D.lm_perm + (size_t) w * C.L;
     const int K = dm.K, NCV = 6 * K + 7, NCA = 4 * ((NCV + 1 + 3) / 4);
     const int grp = tid >> 3, sl = tid & 7;
     int o0[3], o1[3];
@@ -199,8 +273,8 @@ __global__ void __launch_bounds__(128, 4) ba_lin_vis(BaCaps C, BaDev D) {
         const int c = sl + 8 * t;  // 0..23; 19 -> residual pair (g_l); 20 -> h_l from j_rho; > 20 unused
         o0[t] = c < 19 ? jc_off(c) : 38, o1[t] = c < 19 ? o0[t] + jc_row1(c) : 39;
     }
-    for (int l = lmA + grp; l < lmB; l += 16) {
-        const int f0 = off[l] - s0, nf = off[l + 1] - off[l];
+    for (int pl = pA + grp; pl < pB; pl += 16) {
+        const int l = perm[pl], f0 = off[pl] - s0, nf = off[pl + 1] - off[pl];
         double *row = D.AW + ((size_t) w * C.LP + l) * C.NCA;
         for (int c = sl; c < NCA; c += 8) row[c] = 0.0;
         __syncwarp(0xffu << (tid & 24));  // the landmark's eight lanes: zeros land before the values
@@ -241,77 +315,46 @@ __global__ void __launch_bounds__(128, 4) ba_lin_vis(BaCaps C, BaDev D) {
             }
         }
     }
+    // ---- phase 4
+    if (nslot == 0) return;  // a run of landmarks without factors: no pair
+    const int rn = (int) s_rec[0][43];
+    __syncthreads();
+    if (tid == 0) s_last = atomicAdd(D.vis_cnt + (size_t) w * C.K + rn, 1) == D.ref_nrun[(size_t) w * C.K + rn] - 1;
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    if (tid == 0) D.vis_cnt[(size_t) w * C.K + rn] = 0;
+    const int PM = C.K * (C.K - 1), P = D.npairs[w];
+    const int *pro = D.pair_ro + (size_t) w * PM, *poff = D.part_off + (size_t) w * (PM + 1);
+    for (int p = tid; p < P; p += 128)  // the node's pairs are consecutive (pairs are ordered by reference node)
+        if ((pro[p] >> 8) == rn) {
+            atomicAdd(&s_np, 1);
+            if (p == 0 || (pro[p - 1] >> 8) != rn) s_p0 = p;
+        }
+    __syncthreads();
+    const double *part = D.gpart + (size_t) w * C.GQ * 210;
+    double *Mp = D.Mp + (size_t) w * PM * 210;
+    for (int p = s_p0 + warp; p < s_p0 + s_np; p += 4) {  // warp / pair: the 7 entries of a lane in flight together
+        const int k0 = poff[p], k1 = poff[p + 1];
+        double acc[7];
+#pragma unroll
+        for (int j = 0; j < 7; j++) acc[j] = lane + 32 * j < 210 ? __ldcg(part + (size_t) k0 * 210 + lane + 32 * j) : 0.0;
+        for (int k = k0 + 1; k < k1; k++) {
+            double v[7];
+#pragma unroll
+            for (int j = 0; j < 7; j++) v[j] = lane + 32 * j < 210 ? __ldcg(part + (size_t) k * 210 + lane + 32 * j) : 0.0;
+#pragma unroll
+            for (int j = 0; j < 7; j++) acc[j] += v[j];
+        }
+#pragma unroll
+        for (int j = 0; j < 7; j++)
+            if (lane + 32 * j < 210) Mp[(size_t) p * 210 + lane + 32 * j] = acc[j];
+    }
 }
 
 // ------------------------------------------------------------------------------------------------ pair_gram: vision part of H_cc, g_c
-// Factors are grouped by (reference node, observing node).  Within a group every factor has the same 19 camera-side columns
-// [ref pose 6 | obs pose 6 | extrinsic 6 | td 1] (+ the residual as a 20th column), so the group's contribution is the dense
-// 20x20 Gram matrix of its stacked 2x20 rows: stage 1 (warp / group) computes it, stage 2 (thread / output entry) gathers the
-// groups into the symmetric (NCV+1)^2 matrix [H_vis g_vis; g_vis^T r^T r].  No atomics: every output has one writer.
-__device__ __forceinline__ int tri20(int la, int lb) {  // index of (la <= lb) in the packed upper 20x20
-    return la * 20 - la * (la - 1) / 2 + (lb - la);
-}
-// stage 1: one warp per (window, group): the group's packed 20x20 Gram matrix -> Mp (global, L2 resident).
-// FP64 tensor cores (DMMA.8x8x4): the stacked 2x20 rows X of the group are multiplied as X^T X, 4 rows (2 factors) per k-step.
-// With the m8n8k4 fragment layout (A: lane -> (row lane/4, k lane%4); B: lane -> (k lane%4, col lane/4)) the A operand of
-// X^T X and the B operand are the SAME register: lane loads X[k = lane%4][8 t + lane/4] for the three column tiles t and issues
-// the six upper-triangular tile products.  Records are read straight from L2 (each 320-byte record is consumed whole by the warp).
-__device__ __forceinline__ void dmma884(double &c0, double &c1, double a, double b) {
-    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
-}
-__device__ __forceinline__ void gram1_body(const BaCaps &C, const BaDev &D, int w, int pblock) {
-    const LmState &st = D.st[w];
-    if (st.done || !st.need_lin) return;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int PM = C.K * (C.K - 1);
-    const int P = D.npairs[w];
-    const int p = pblock * 8 + warp;
-    if (p >= P) return;
-    const int *poff = D.pair_off + (size_t) w * (PM + 1), *pfidx = D.pair_fidx + (size_t) w * C.F;
-    double *Mp = D.Mp + (size_t) w * PM * 210;
-    const int kk = lane & 3, g = lane >> 2;  // k index inside the step (factor kk/2, residual row kk%2), column inside the tile
-    int o[3];
-#pragma unroll
-    for (int t = 0; t < 3; t++) {
-        const int a = 8 * t + g;
-        o[t] = a < 20 ? jc_off(a) + (kk & 1) * jc_row1(a) : -1;
-    }
-    double c00[2] = {0, 0}, c01[2] = {0, 0}, c02[2] = {0, 0}, c11[2] = {0, 0}, c12[2] = {0, 0}, c22[2] = {0, 0};
-    const int pbeg = poff[p], pend = poff[p + 1];
-    const double *rec = D.jcomp + (size_t) w * C.F * 40;
-    constexpr int UNR = 4;  // k-steps in flight (8 factors)
-    for (int base = pbeg; base < pend; base += 2 * UNR) {
-        double x[UNR][3];
-#pragma unroll
-        for (int u = 0; u < UNR; u++) {
-            const int q = base + 2 * u + (kk >> 1);
-            const bool ok = q < pend;
-            const int f = ok ? pfidx[q] : 0;
-#pragma unroll
-            for (int t = 0; t < 3; t++) x[u][t] = (ok && o[t] >= 0) ? rec[(size_t) f * 40 + o[t]] : 0.0;
-        }
-#pragma unroll
-        for (int u = 0; u < UNR; u++) {
-            dmma884(c00[0], c00[1], x[u][0], x[u][0]);
-            dmma884(c01[0], c01[1], x[u][0], x[u][1]);
-            dmma884(c02[0], c02[1], x[u][0], x[u][2]);
-            dmma884(c11[0], c11[1], x[u][1], x[u][1]);
-            dmma884(c12[0], c12[1], x[u][1], x[u][2]);
-            dmma884(c22[0], c22[1], x[u][2], x[u][2]);
-        }
-    }
-    // C fragment: lane holds (row lane/4, cols 2 (lane%4) + {0,1}) of each 8x8 tile
-    auto put = [&](int ti, int tj, const double *c) {
-#pragma unroll
-        for (int e = 0; e < 2; e++) {
-            const int la = 8 * ti + g, lb = 8 * tj + 2 * kk + e;
-            if (la <= lb && lb < 20) Mp[(size_t) p * 210 + tri20(la, lb)] = c[e];
-        }
-    };
-    put(0, 0, c00), put(0, 1, c01), put(0, 2, c02), put(1, 1, c11), put(1, 2, c12), put(2, 2, c22);
-}
-
-__global__ void __launch_bounds__(256) ba_pair_gram1(BaCaps C, BaDev D) { gram1_body(C, D, blockIdx.y, blockIdx.x); }
+// ba_lin_vis leaves one packed 20x20 Gram matrix per (reference node, observing node) pair in Mp; the gather (thread / output entry)
+// assembles the pairs into the symmetric (NCV+1)^2 matrix [H_vis g_vis; g_vis^T r^T r].  No atomics: every output has one writer.
 
 // stage 2: one thread per output entry gathers the groups that touch both of its blocks (one writer per entry, no atomics)
 // gather of one entry (A <= B) of the symmetric (NCV+1)^2 matrix [H_vis g_vis; g_vis^T r^T r] from the per-pair Gram matrices
@@ -388,7 +431,7 @@ __global__ void __launch_bounds__(256) ba_pair_gram2(BaCaps C, BaDev D) {
 // ------------------------------------------------------------------------------------------------ Schur term
 // Schur SYRK on the FP64 tensor cores: CW[split] = sum over the split's landmarks of phi_l w_l w_l^T (stored symmetric), with
 // phi_l = s_l^2 / (s_l^2 h_l + clamp(s_l^2 h_l) / radius) the LM-damped landmark pivot.  DMMA.8x8x4 with k = 4 landmarks per step; as in
-// ba_pair_gram1 the A and B fragments of X^T X share one layout: lane reads A_W[l0 + lane%4][8 t + lane/4].  The CTA stages its
+// ba_lin_vis's Gram phase the A and B fragments of X^T X share one layout: lane reads A_W[l0 + lane%4][8 t + lane/4].  The CTA stages its
 // landmark rows (and phi) in shared memory once per pass -- leading dimension = 8 mod 16 doubles, so a fragment read is the minimal
 // two wavefronts -- and every warp accumulates two 16x16 super-tiles (2x2 DMMA tiles each) of the upper triangle per pass.
 // The BA_SPLIT_W landmark splits are separate CTAs whose partials ba_pack1 sums in fixed order (deterministic).
@@ -1784,9 +1827,9 @@ struct icg_ba {
     HostDev<LmState> st;
     HostDev<double> pose, mix, ext, rho, imu_blob, imu_U, gnss_blh, gnss_std, lever, pose_prior, pose_prior_sinfo, mix_prior, mix_prior_std, marg_x0,
         marg_H0, marg_b0, marg_c0;
-    HostDev<int> f_slot, f_meta_s, vb_lm0;  // f_slot / lm_fidx: host-side packing helpers only (factor id <-> record slot)
+    HostDev<int> f_meta_s, vb_lm0, ref_nrun;  // lm_fidx: host-side packing helper only (record slot -> factor id)
     HostDev<double> f_const_s;
-    HostDev<int> lm_off, lm_fidx, gnss_node, marg_type, marg_node, pair_off, pair_ro, pair_fidx, npairs;
+    HostDev<int> lm_off, lm_perm, lm_fidx, gnss_node, marg_type, marg_node, part_off, pair_ro, vis_ord, npairs;
     HostDev<uint8_t> f_active;
     std::vector<void *> dev_only;
     HostDev<double> scratch;  // single-factor evaluation
@@ -1953,7 +1996,9 @@ static int ba_create_body(icg_ba *h, int max_windows, int max_K, int max_L, int 
     C.NW = max_windows, C.K = max_K, C.L = max_L, C.F = max_F, C.G = std::max(1, max_gnss), C.R = std::max(1, max_marg_r);
     C.NCV = 6 * max_K + 7, C.N = 15 * max_K + 7, C.NS = (C.N + 3) & ~3, C.NCA = 4 * ((C.NCV + 1 + 3) / 4);
     C.RJ = (2 * max_F + 31) & ~31, C.LP = (max_L + 31) & ~31;
-    C.NVB = (max_F + 127 - max_K) / (128 - max_K) + max_L / 128 + 4;  // worst case: every run is cut short by one landmark's K - 1 factors
+    // worst case: every run is cut short by one landmark's K - 1 factors, plus one more run per reference node (runs never span two)
+    C.NVB = (max_F + 127 - max_K) / (128 - max_K) + max_L / 128 + 4 + max_K;
+    C.GQ = std::max(1, std::min(max_F, (C.NVB - 2) * (max_K - 1)));  // a partial holds >= 1 factor; a run observes from <= K - 1 nodes
     h->nblk_vis = (max_F + 255) / 256;
     const size_t NW = max_windows;
 #define HD(field, count)                                                       \
@@ -1965,17 +2010,17 @@ static int ba_create_body(icg_ba *h, int max_windows, int max_K, int max_L, int 
     HD(imu_blob, NW * C.K * ICG_IMU_BLOB_DOUBLES) HD(imu_U, NW * C.K * 225) HD(gnss_blh, NW * C.G * 3) HD(gnss_std, NW * C.G * 3) HD(lever, NW * 3)
     HD(pose_prior, NW * 7) HD(pose_prior_sinfo, NW * 6) HD(mix_prior, NW * 9) HD(mix_prior_std, NW * 9) HD(marg_x0, NW * BA_MARG_MAXB * 9)
     HD(marg_H0, NW * C.R * C.R) HD(marg_b0, NW * C.R) HD(marg_c0, NW)
-    HD(lm_off, NW * (C.L + 1)) HD(lm_fidx, NW * C.F) HD(gnss_node, NW * C.G) HD(marg_type, NW * BA_MARG_MAXB) HD(marg_node, NW * BA_MARG_MAXB) HD(f_active, NW * C.F)
-    HD(scratch, 1024) HD(st_save, NW) HD(cull_counters, 2 * NW) HD(f_slot, NW * C.F) HD(f_meta_s, NW * C.F * 4) HD(vb_lm0, NW * C.NVB) HD(f_const_s, NW * C.F * 14)
-    HD(pair_off, NW * ((size_t) C.K * (C.K - 1) + 1)) HD(pair_ro, NW * (size_t) C.K * (C.K - 1)) HD(pair_fidx, NW * C.F) HD(npairs, NW)
+    HD(lm_off, NW * (C.L + 1)) HD(lm_perm, NW * C.L) HD(lm_fidx, NW * C.F) HD(gnss_node, NW * C.G) HD(marg_type, NW * BA_MARG_MAXB) HD(marg_node, NW * BA_MARG_MAXB) HD(f_active, NW * C.F)
+    HD(scratch, 1024) HD(st_save, NW) HD(cull_counters, 2 * NW) HD(f_meta_s, NW * C.F * 4) HD(vb_lm0, NW * C.NVB) HD(ref_nrun, NW * C.K) HD(f_const_s, NW * C.F * 14)
+    HD(part_off, NW * ((size_t) C.K * (C.K - 1) + 1)) HD(pair_ro, NW * (size_t) C.K * (C.K - 1)) HD(vis_ord, NW * C.F) HD(npairs, NW)
 #undef HD
     BaDev &D = h->D;
     D.rank = 0, D.world = 1;
     D.dims = h->dims.d, D.st = h->st.d, D.pose = h->pose.d, D.mix = h->mix.d, D.ext = h->ext.d, D.rho = h->rho.d;
     D.f_active = h->f_active.d;
-    D.pair_off = h->pair_off.d, D.pair_ro = h->pair_ro.d, D.pair_fidx = h->pair_fidx.d, D.npairs = h->npairs.d;
-    D.f_meta_s = h->f_meta_s.d, D.vb_lm0 = h->vb_lm0.d, D.f_const_s = h->f_const_s.d;
-    D.lm_off = h->lm_off.d, D.imu_blob = h->imu_blob.d, D.imu_U = h->imu_U.d;
+    D.part_off = h->part_off.d, D.pair_ro = h->pair_ro.d, D.vis_ord = h->vis_ord.d, D.npairs = h->npairs.d;
+    D.f_meta_s = h->f_meta_s.d, D.vb_lm0 = h->vb_lm0.d, D.ref_nrun = h->ref_nrun.d, D.f_const_s = h->f_const_s.d;
+    D.lm_off = h->lm_off.d, D.lm_perm = h->lm_perm.d, D.imu_blob = h->imu_blob.d, D.imu_U = h->imu_U.d;
     D.gnss_node = h->gnss_node.d, D.gnss_blh = h->gnss_blh.d, D.gnss_std = h->gnss_std.d, D.lever = h->lever.d;
     D.pose_prior = h->pose_prior.d, D.pose_prior_sinfo = h->pose_prior_sinfo.d, D.mix_prior = h->mix_prior.d, D.mix_prior_std = h->mix_prior_std.d;
     D.marg_type = h->marg_type.d, D.marg_node = h->marg_node.d, D.marg_x0 = h->marg_x0.d, D.marg_H0 = h->marg_H0.d, D.marg_b0 = h->marg_b0.d, D.marg_c0 = h->marg_c0.d;
@@ -1985,10 +2030,15 @@ static int ba_create_body(icg_ba *h, int max_windows, int max_K, int max_L, int 
     DM(pose_c, NW * C.K * 7) DM(mix_c, NW * C.K * 9) DM(ext_c, NW * 8) DM(rho_c, NW * C.L)
     DM(pose_0, NW * C.K * 7) DM(mix_0, NW * C.K * 9) DM(ext_0, NW * 8) DM(rho_0, NW * C.L)
     DM(AW, NW * C.NCA * C.LP) DM(Mp, NW * (size_t) C.K * (C.K - 1) * 210) DM(CJ, NW * BA_SPLIT_J * C.NCA * C.NCA) DM(CW, NW * BA_SPLIT_W * C.NCA * C.NCA)
-    DM(jcomp, NW * C.F * 40) DM(costf, NW * C.F) DM(hl, NW * C.L) DM(gl, NW * C.L) DM(scale_l, NW * C.L) DM(scale_c, NW * C.NS)
+    DM(gpart, NW * (size_t) C.GQ * 210) DM(costf, NW * C.F) DM(hl, NW * C.L) DM(gl, NW * C.L) DM(scale_l, NW * C.L) DM(scale_c, NW * C.NS)
     DM(Hc, NW * C.NS * C.NS) DM(gc, NW * C.NS) DM(Hs, NW * C.NS * C.NS) DM(cost_part, NW * (h->nblk_vis + 1)) DM(red, NW * (2 * (size_t) C.NCA * C.NCA + 8)) DM(redmax, NW) DM(red2, NW * 4) DM(step_c, NW * C.NS) DM(step_l, NW * C.L)
 #undef DM
     if (rc == ICG_OK) rc = dmalloc(h, &D.gnss_std_0, NW * C.G * 3);
+    if (rc == ICG_OK) {
+        double *cnt = nullptr;
+        rc = dmalloc(h, &cnt, (NW * C.K + 1) / 2);  // zeroed: the arrival counters start at 0 and every lin_vis launch leaves them at 0
+        D.vis_cnt = (int *) cnt;
+    }
     if (rc == ICG_OK) {
         double *fa0 = nullptr;
         rc = dmalloc(h, &fa0, (NW * C.F + 7) / 8 + 1);
@@ -2031,8 +2081,8 @@ void icg_ba_destroy(icg_ba *h) {
     h->dims.release(), h->st.release(), h->pose.release(), h->mix.release(), h->ext.release(), h->rho.release();
     h->imu_blob.release(), h->imu_U.release(), h->gnss_blh.release(), h->gnss_std.release(), h->lever.release(), h->pose_prior.release();
     h->pose_prior_sinfo.release(), h->mix_prior.release(), h->mix_prior_std.release(), h->marg_x0.release(), h->marg_H0.release(), h->marg_b0.release();
-    h->marg_c0.release(), h->lm_off.release(), h->lm_fidx.release(), h->gnss_node.release();
-    h->f_slot.release(), h->f_meta_s.release(), h->vb_lm0.release(), h->f_const_s.release(), h->marg_type.release(), h->marg_node.release(), h->f_active.release(), h->scratch.release(), h->st_save.release(), h->cull_counters.release(), h->pair_off.release(), h->pair_ro.release(), h->pair_fidx.release(), h->npairs.release();
+    h->marg_c0.release(), h->lm_off.release(), h->lm_perm.release(), h->lm_fidx.release(), h->gnss_node.release();
+    h->f_meta_s.release(), h->vb_lm0.release(), h->ref_nrun.release(), h->f_const_s.release(), h->marg_type.release(), h->marg_node.release(), h->f_active.release(), h->scratch.release(), h->st_save.release(), h->cull_counters.release(), h->part_off.release(), h->pair_ro.release(), h->vis_ord.release(), h->npairs.release();
     if (h->comm) nccl_api().CommDestroy((ncclComm_t) h->comm);
     split_release(h);
     if (h->marg_ready) h->marg_map.release(), h->marg_oJ0.release(), h->marg_oe0.release(), h->marg_oHp.release(), h->marg_obp.release();
@@ -2083,8 +2133,8 @@ int icg_ba_upload(icg_ba *h, int n, const icg_ba_problem *P) {
                 PK_FAIL(ICG_EINVAL, "icg_ba_upload: window %d factor %d has invalid indices", w, f);
             }
         }
+        std::vector<int> refof(p.L, -1);  // reference node of every landmark (-1: no factor)
         {   // a map point has one reference frame and at most one observation per keyframe (IG/ic_gvins.cc:1777-1834): lin_lm relies on it
-            std::vector<int> refof(p.L, -1);
             std::vector<unsigned> seen((size_t) p.L, 0u);
             for (int f = 0; f < p.F; f++) {
                 const int l = p.f_lm[f];
@@ -2099,28 +2149,40 @@ int icg_ba_upload(icg_ba *h, int n, const icg_ba_problem *P) {
             memcpy(h->f_active.h + (size_t) w * C.F, p.f_active, p.F);
         else
             memset(h->f_active.h + (size_t) w * C.F, 1, p.F);
-        // CSR by landmark
+        // landmark positions: ordered by reference node, stable by id, landmarks without factors last
+        int *perm = h->lm_perm.h + (size_t) w * C.L;
+        std::vector<int> pos_of(p.L);
+        {
+            std::vector<int> kcur(p.K + 2, 0);
+            for (int l = 0; l < p.L; l++) kcur[(refof[l] < 0 ? p.K : refof[l]) + 1]++;
+            for (int k = 0; k <= p.K; k++) kcur[k + 1] += kcur[k];
+            for (int l = 0; l < p.L; l++) pos_of[l] = kcur[refof[l] < 0 ? p.K : refof[l]]++, perm[pos_of[l]] = l;
+        }
+        // CSR by landmark position: the record slots
         int *off = h->lm_off.h + (size_t) w * (C.L + 1), *fidx = h->lm_fidx.h + (size_t) w * C.F;
         for (int l = 0; l <= p.L; l++) off[l] = 0;
-        for (int f = 0; f < p.F; f++) off[p.f_lm[f] + 1]++;
+        for (int f = 0; f < p.F; f++) off[pos_of[p.f_lm[f]] + 1]++;
         for (int l = 0; l < p.L; l++) off[l + 1] += off[l];
-        int *fslot = h->f_slot.h + (size_t) w * C.F;
+        int *vbh = h->vb_lm0.h + (size_t) w * C.NVB, *meta = h->f_meta_s.h + (size_t) w * C.F * 4;
+        int nrun = 0;
         {
             std::vector<int> cur(off, off + p.L);
-            for (int f = 0; f < p.F; f++) fslot[f] = cur[p.f_lm[f]], fidx[cur[p.f_lm[f]]++] = f;
-            // lin_vis runs: greedy packing of whole landmarks into <= 128 record slots
-            int *vbh = h->vb_lm0.h + (size_t) w * C.NVB;
-            int nrun = 0, l0 = 0;
+            for (int f = 0; f < p.F; f++) fidx[cur[pos_of[p.f_lm[f]]]++] = f;
+            // lin_vis runs: greedy packing of whole landmarks of one reference node into <= 128 record slots
+            int *nrun_of = h->ref_nrun.h + (size_t) w * C.K;
+            for (int k = 0; k < C.K; k++) nrun_of[k] = 0;
+            int l0 = 0;
             while (l0 < p.L) {
+                const int ref = refof[perm[l0]];
                 int l1 = l0;
-                while (l1 < p.L && off[l1 + 1] - off[l0] <= 128) l1++;
-                if (l1 == l0 || nrun >= C.NVB - 2) PK_FAIL(ICG_EINVAL, "icg_ba_upload: window %d: landmark %d has more than 128 factors or the run table overflows", w, l0);
+                while (l1 < p.L && refof[perm[l1]] == ref && off[l1 + 1] - off[l0] <= 128) l1++;
+                if (l1 == l0 || nrun >= C.NVB - 2) PK_FAIL(ICG_EINVAL, "icg_ba_upload: window %d: landmark %d has more than 128 factors or the run table overflows", w, perm[l0]);
+                if (ref >= 0) nrun_of[ref]++;
                 vbh[nrun++] = l0;
                 l0 = l1;
             }
             vbh[nrun] = p.L;
             vbh[C.NVB - 1] = nrun;
-            int *meta = h->f_meta_s.h + (size_t) w * C.F * 4;
             double *fcs = h->f_const_s.h + (size_t) w * C.F * 14;
             for (int q = 0; q < p.F; q++) {
                 const int f = fidx[q];
@@ -2128,23 +2190,42 @@ int icg_ba_upload(icg_ba *h, int n, const icg_ba_problem *P) {
                 memcpy(fcs + (size_t) q * 14, p.f_const + (size_t) f * 14, sizeof(double) * 14);
             }
         }
-        // CSR by (reference node, observing node) pair
+        // (reference node, observing node) pairs and their Gram partials: one per (run, observing node of the run), numbered pair by pair
+        // and, within a pair, in run order (the order ba_lin_vis sums them in); every run's slots ordered by observing node (stable)
         {
             const int PM = C.K * (C.K - 1);
-            int *poff = h->pair_off.h + (size_t) w * (PM + 1), *pro = h->pair_ro.h + (size_t) w * PM, *pfidx = h->pair_fidx.h + (size_t) w * C.F;
-            std::vector<int> cnt((size_t) p.K * p.K, 0), slot((size_t) p.K * p.K, -1);
-            for (int f = 0; f < p.F; f++) cnt[(size_t) p.f_ref[f] * p.K + p.f_obs[f]]++;
+            int *poff = h->part_off.h + (size_t) w * (PM + 1), *pro = h->pair_ro.h + (size_t) w * PM, *ord = h->vis_ord.h + (size_t) w * C.F;
+            std::vector<int> slot((size_t) p.K * p.K, -1);
+            for (int f = 0; f < p.F; f++) slot[(size_t) p.f_ref[f] * p.K + p.f_obs[f]] = 0;
             int P = 0;
-            poff[0] = 0;
             for (int key = 0; key < p.K * p.K; key++)
-                if (cnt[key]) {
-                    slot[key] = P;
-                    pro[P] = ((key / p.K) << 8) | (key % p.K);
-                    poff[P + 1] = poff[P] + cnt[key];
-                    P++;
+                if (slot[key] == 0) slot[key] = P, pro[P++] = ((key / p.K) << 8) | (key % p.K);
+            std::vector<int> npart(P, 0);
+            for (int r = 0; r < nrun; r++) {
+                unsigned seen = 0u;
+                for (int q = off[vbh[r]]; q < off[vbh[r + 1]]; q++) seen |= 1u << meta[4 * q + 2];
+                for (int k = 0; k < p.K; k++)
+                    if ((seen >> k) & 1u) npart[slot[(size_t) refof[perm[vbh[r]]] * p.K + k]]++;
+            }
+            poff[0] = 0;
+            for (int i = 0; i < P; i++) poff[i + 1] = poff[i] + npart[i];
+            std::vector<int> cur(poff, poff + P), start(p.K), pidx(p.K);
+            for (int r = 0; r < nrun; r++) {
+                const int a = off[vbh[r]], b = off[vbh[r + 1]];
+                if (a == b) continue;
+                const int ref = meta[4 * a + 1];
+                std::fill(start.begin(), start.end(), 0);
+                for (int q = a; q < b; q++) start[meta[4 * q + 2]]++;
+                for (int k = 0, t = 0; k < p.K; k++) {
+                    const int c = start[k];
+                    start[k] = t, t += c;
+                    if (c) pidx[k] = cur[slot[(size_t) ref * p.K + k]]++;
                 }
-            std::vector<int> cur(poff, poff + P);
-            for (int f = 0; f < p.F; f++) pfidx[cur[slot[(size_t) p.f_ref[f] * p.K + p.f_obs[f]]]++] = fslot[f];  // record slots, not factor ids
+                for (int q = a; q < b; q++) {
+                    const int k = meta[4 * q + 2];
+                    ord[a + start[k]++] = (q - a) | (pidx[k] << 8);
+                }
+            }
             h->npairs.h[w] = P;
         }
         for (int k = 0; k < p.n_imu; k++) {
@@ -2238,7 +2319,7 @@ int icg_ba_upload(icg_ba *h, int n, const icg_ba_problem *P) {
 #define UP(field, stride) ICG_CUDA(h->field.up(s, nn * (size_t) (stride)))
         UP(dims, 1); UP(pose, C.K * 7); UP(mix, C.K * 9); UP(ext, 8); UP(rho, C.L);
         UP(f_active, C.F);  // factor constants and indices travel once, in record-slot order (f_meta_s / f_const_s)
-        UP(f_meta_s, C.F * 4); UP(vb_lm0, C.NVB); UP(f_const_s, C.F * 14); UP(lm_off, C.L + 1); UP(pair_off, PM + 1); UP(pair_ro, PM); UP(pair_fidx, C.F);
+        UP(f_meta_s, C.F * 4); UP(vb_lm0, C.NVB); UP(f_const_s, C.F * 14); UP(lm_off, C.L + 1); UP(lm_perm, C.L); UP(ref_nrun, C.K); UP(part_off, PM + 1); UP(pair_ro, PM); UP(vis_ord, C.F);
         UP(npairs, 1); UP(imu_blob, C.K * ICG_IMU_BLOB_DOUBLES); UP(imu_U, C.K * 225);
         UP(gnss_node, C.G); UP(gnss_blh, C.G * 3); UP(gnss_std, C.G * 3); UP(lever, 3);
         UP(pose_prior, 7); UP(pose_prior_sinfo, 6); UP(mix_prior, 9); UP(mix_prior_std, 9);
@@ -2259,7 +2340,7 @@ int icg_ba_upload(icg_ba *h, int n, const icg_ba_problem *P) {
 }
 
 // ---- in-situ stage timing
-static const char *PROF_NAMES[16] = {"(gap/other)", "lin_vis", "lin_lm", "pair_gram1", "pair_gram2", "schur_dmma", "join lin_cam + lin_done",
+static const char *PROF_NAMES[16] = {"(gap/other)", "lin_vis", "lin_lm", "", "pair_gram2", "schur_dmma", "join lin_cam + lin_done",
                                      "pack1 / export + signal", "solve", "cost (+cost_cam)", "pack2 / exchange", "accept", "hsum / reduce", "join gram chain", "step_lm", ""};
 static void prof_mark(icg_ba *h, int tag) {
     if (!h->prof) return;
@@ -2358,8 +2439,6 @@ static int enqueue_lm(icg_ba *h, int max_num_iterations) {
         //  Gram warps when they share SMs)
         ba_schur_dmma<<<dim3(BA_SPLIT_W, n), 256, h->smem_schur, s>>>(C, D, h->ld_schur);
         prof_mark(h, 5);
-        ba_pair_gram1<<<dim3((C.K * (C.K - 1) + 7) / 8, n), 256, 0, s>>>(C, D);
-        prof_mark(h, 3);
         if (h->comm) {
             ba_pair_gram2<<<dim3(((C.NCV + 1) * (C.NCV + 1) + 255) / 256, n), 256, 0, s>>>(C, D);
             prof_mark(h, 4);
@@ -2378,7 +2457,7 @@ static int enqueue_lm(icg_ba *h, int max_num_iterations) {
         prof_mark(h, 12);
         ba_solve<<<n, SOLVE_THREADS, h->smem_solve, s>>>(C, D);
         prof_mark(h, 8);
-        count_launch(h->comm ? 8 : 6);
+        count_launch(h->comm ? 7 : 5);
         if (it == max_num_iterations) break;
         ICG_CUDA(cudaEventRecord(h->ev_fork, s));
         ICG_CUDA(cudaStreamWaitEvent(h->stream_cam, h->ev_fork, 0));
@@ -2518,8 +2597,6 @@ static int enqueue_lm_split(icg_ba *h, int max_num_iterations) {
         prof_mark(h, 1);
         ba_schur_dmma<<<dim3(BA_SPLIT_W, n), 256, h->smem_schur, s>>>(C, D, h->ld_schur);
         prof_mark(h, 5);
-        ba_pair_gram1<<<dim3((C.K * (C.K - 1) + 7) / 8, n), 256, 0, s>>>(C, D);
-        prof_mark(h, 3);
         ba_export<<<g_nn, 256, 0, s>>>(C, D);
         ba_signal<<<1, 32, 0, s>>>(D, epoch);
         prof_mark(h, 7);
@@ -2532,7 +2609,7 @@ static int enqueue_lm_split(icg_ba *h, int max_num_iterations) {
         prof_mark(h, 8);
         ba_step_lm<<<dim3(n, STEP_SLICES), SOLVE_THREADS, h->smem_step_lm, s>>>(C, D, epoch);
         prof_mark(h, 14);
-        count_launch(9);
+        count_launch(8);
         if (it == max_num_iterations) break;
         ICG_CUDA(cudaEventRecord(h->ev_fork, s));
         ICG_CUDA(cudaStreamWaitEvent(h->stream_cam, h->ev_fork, 0));
@@ -2834,7 +2911,6 @@ static int marginalize_body(icg_ba *h, int n_windows, const icg_ba_problem *prob
     const size_t smem = sizeof(double) * (8 * 480 + 2 * (size_t) C.R) + sizeof(int) * (size_t) C.R + 64;
     marg_prepare<<<(n + 127) / 128, 128, 0, s>>>(D, M, n, 0);
     ba_lin_vis<<<dim3(C.NVB - 2, n), 128, LV_SMEM, s>>>(C, D);
-    ba_pair_gram1<<<dim3((C.K * (C.K - 1) + 7) / 8, n), 256, 0, s>>>(C, D);
     marg_assemble<<<n, 256, smem, s>>>(C, D, M);
     // eigendecompositions: on-chip cluster-pair kernel when every block of the batch fits (n <= MARG_PAIR_MAXN), global-memory kernel otherwise
     int max_m = 0, max_r = 0;
@@ -2868,7 +2944,7 @@ static int marginalize_body(icg_ba *h, int n_windows, const icg_ba_problem *prob
     marg_finish<<<n, MARG_THREADS, 0, s>>>(M);
     marg_prepare<<<(n + 127) / 128, 128, 0, s>>>(D, M, n, 1);
     ICG_CHECK_LAUNCH();
-    count_launch(10);
+    count_launch(9);
     // D2H: every window's r x r result sits at the start of its rcap^2 slot -- move the used prefix of each slot only (one strided copy)
     {
         const size_t pitch = sizeof(double) * (size_t) M.rcap * M.rcap, used = sizeof(double) * (size_t) max_r * max_r;

@@ -9,8 +9,8 @@
 // J0 = S^1/2 V^T, e0 = -S^-1/2 V^T bp of the Schur complement Hp = Hrr - Hrm Hmm^+ Hmr (eigen-pseudo-inverse, EPS 1e-8).
 //
 // Device plan (batched over windows, one CTA per window per stage):
-//   lin_vis / pair_gram1            (the solve's own kernels, loss + constant-block masks switched off) -> per-factor Jacobians,
-//                                    per-landmark coupling rows (lin_vis phase 3), per-(ref,obs) 20x20 Gram matrices
+//   lin_vis                         (the solve's own kernel, loss + constant-block masks switched off) -> per-landmark coupling
+//                                    rows (lin_vis phase 3), per-(ref,obs) 20x20 Gram matrices
 //   marg_assemble                   dense H0, b0 in the [marginalized | remained] column order (one writer per entry per stage)
 //   marg_jacobi(Hmm)                one-sided (Hestenes) Jacobi: columns of G = Hmm V orthogonalised by plane rotations, one warp per
 //                                    column pair, round-robin ordering; lambda_i = v_i . g_i

@@ -3,7 +3,7 @@
 //
 // One LM attempt, rank g of G (G = 1: everything is local), windows w = 0 .. W-1, owner(w) = w mod G:
 //
-//   every rank   ba_lin_vis / ba_schur_dmma / ba_pair_gram1     its landmark shard of every window (the kernels of the fused pipeline)
+//   every rank   ba_lin_vis / ba_schur_dmma                     its landmark shard of every window (the kernels of the fused pipeline)
 //   every rank   ba_export        packs [tri(H_vis - Schur) | diag H_vis | g_vis | W phi g_l | cost, sum rho^2, max |g_l|] of window w and
 //                                 STORES it into the inbox of owner(w) -- peer memory over NVLink (P2P stores), slot [w / G][g]
 //                ba_signal        release-flag "my partials of this epoch have landed" on every peer
