@@ -14,14 +14,17 @@
 //                correction -> record in shared memory; per (reference node, observing node) pair the 20x20 Gram matrix of the run's
 //                records on the FP64 tensor cores (DMMA.8x8x4), summed over the node's runs in run order;
 //                lanes / landmark -> h_l, g_l and the dense coupling row w_l (A_W, landmark-major)
-//   pair_gram  : one-writer-per-entry gather of the pair Gram matrices into the vision part of H_cc and g_c
-//   schur_dmma : sum_l phi_l w_l w_l^T with phi_l = s_l^2 / (s_l^2 h_l + D_l^2) on the FP64 tensor cores
+//   schur_dmma : cluster of 4 CTAs / window: sum_l phi_l w_l w_l^T with phi_l = s_l^2 / (s_l^2 h_l + D_l^2) on the FP64 tensor cores, one
+//                landmark split per CTA, the partials summed over DSMEM; epilogue: one-writer-per-entry gather of the pair Gram matrices
+//                into the vision part of H_cc and g_c -> Hs = H_c + H_vis - Schur term and the solve's vision vectors (or the export /
+//                all-reduce payload of a landmark shard)
 //   lin_cam    : one CTA / window (second stream, beside the vision chain) -> IMU preintegration, GNSS, bias, prior and
 //                marginalization factors -> H_c, g_c
 //   solve      : one CTA / window -> Jacobi scaling, LM diagonal, S = s(H - Schur)s + D^2, packed Cholesky in shared memory
 //                (panel updates on DMMA), triangular solves, landmark back-substitution, model cost change, candidate x (+) delta
 //   cost       : candidate cost (all factors, residuals only);   accept : Ceres step acceptance + radius update
 //   ba_marg.cuh: sliding-window marginalization (MarginalizationInfo) on the same device-resident linearisation
+#include <cooperative_groups.h>
 #include <dlfcn.h>
 #include <unistd.h>
 #include <math.h>
@@ -40,9 +43,9 @@
 
 namespace icg {
 using namespace bam;
+namespace cg = cooperative_groups;
 
-constexpr int BA_SPLIT_J = 1;   // the vision Gram matrix is produced whole by ba_pair_gram
-constexpr int BA_SPLIT_W = 4;   // row splits of the Schur SYRK (partials summed in fixed order -> deterministic)
+constexpr int BA_SPLIT_W = 4;   // row splits of the Schur SYRK = CTAs of its cluster (partials summed in fixed order -> deterministic)
 constexpr int BA_CHOL_NB = 8;   // Cholesky block width
 constexpr int BA_MARG_MAXB = 72;  // remained blocks of a prior: <= 2 max_K + 2 = 66 at max_K = 32 (table stride)
 constexpr int BA_MAX_NODES = 32;  // icg_ba_create: max_K <= 32
@@ -100,11 +103,12 @@ struct BaDev {  // device pointers (flat, capacity-strided by window)
     double *gpart;       // [NW][GQ][210] Gram partial of one (run, observing node): packed upper 20x20
     int *vis_cnt;        // [NW][K] lin_vis runs of the reference node arrived (the last one resets it)
     double *Mp;                                    // per-pair 20x20 Gram matrices (upper, 210 entries)
-    double *AW, *CJ, *CW;  // Schur SYRK input; vision Gram matrix; Schur partials
+    double *AW;            // Schur SYRK input
     double *costf;         // per-factor cost
     double *hl, *gl, *scale_l, *scale_c;
     double *Hc, *gc;
     double *Hs;  // H_c + vision Gram - Schur term (lower triangle, ld NS): the operand ba_solve scales and factorises
+    double *visv;  // [NW][3 NCV] diag H_vis | g_vis | W phi g_l (window NCV): ba_solve's other operands (single GPU)
     double *imu_blob, *imu_U;
     int *gnss_node;
     double *gnss_blh, *gnss_std, *lever;
@@ -353,11 +357,11 @@ __global__ void __launch_bounds__(128, 4) ba_lin_vis(BaCaps C, BaDev D) {
 }
 
 // ------------------------------------------------------------------------------------------------ pair_gram: vision part of H_cc, g_c
-// ba_lin_vis leaves one packed 20x20 Gram matrix per (reference node, observing node) pair in Mp; the gather (thread / output entry)
-// assembles the pairs into the symmetric (NCV+1)^2 matrix [H_vis g_vis; g_vis^T r^T r].  No atomics: every output has one writer.
+// ba_lin_vis leaves one packed 20x20 Gram matrix per (reference node, observing node) pair in Mp; the epilogue of ba_schur_dmma gathers
+// them (thread / output entry) into the symmetric (NCV+1)^2 matrix [H_vis g_vis; g_vis^T r^T r].  No atomics: every output has one writer.
 
-// stage 2: one thread per output entry gathers the groups that touch both of its blocks (one writer per entry, no atomics)
-// gather of one entry (A <= B) of the symmetric (NCV+1)^2 matrix [H_vis g_vis; g_vis^T r^T r] from the per-pair Gram matrices
+// gather of one entry (A <= B) of the symmetric (NCV+1)^2 matrix [H_vis g_vis; g_vis^T r^T r] from the per-pair Gram matrices: the groups
+// that touch both of its blocks
 __device__ __forceinline__ void gram2_slots(const BaCaps &C, const BaDev &D, int w, int K, short *s_slot) {
     const int PM = C.K * (C.K - 1), P = D.npairs[w];
     const int *pro = D.pair_ro + (size_t) w * PM;
@@ -374,33 +378,35 @@ __device__ __forceinline__ double gram2_entry(const BaCaps &C, const BaDev &D, i
     const int ga = 12 + a, gb = 12 + b;          // local column of a global-block column
     double sum = 0;
     if (bA == K) {  // (global, global): every group
-        // up to K (K - 1) groups: eight loads in flight and four partial sums in a fixed order (these 36 entries are the tail of the kernel:
-        // a serial sum is 90 dependent L2 round trips)
+        // up to K (K - 1) groups: sixteen loads in flight and four partial sums in a fixed order, group p into sum p mod 4 (these 36 entries
+        // are the tail of the epilogue: a serial sum is 90 dependent L2 round trips)
         const int idx = tri20(ga, gb);
         double s4[4] = {0, 0, 0, 0};
         int p = 0;
-        for (; p + 8 <= P; p += 8) {
-            double v[8];
+        for (; p + 16 <= P; p += 16) {
+            double v[16];
 #pragma unroll
-            for (int u = 0; u < 8; u++) v[u] = Mp[(size_t) (p + u) * 210 + idx];
+            for (int u = 0; u < 16; u++) v[u] = Mp[(size_t) (p + u) * 210 + idx];
 #pragma unroll
-            for (int u = 0; u < 8; u++) s4[u & 3] += v[u];
+            for (int u = 0; u < 16; u++) s4[u & 3] += v[u];
         }
         for (; p < P; p++) s4[p & 3] += Mp[(size_t) p * 210 + idx];
         sum = (s4[0] + s4[1]) + (s4[2] + s4[3]);
     } else if (bB == K || bB == bA) {  // (pose, global) or the pose's diagonal block
         const int i1 = tri20(a, bB == K ? gb : b), i2 = tri20(6 + a, bB == K ? gb : 6 + b);
-        for (int o0 = 0; o0 < K; o0 += 4) {  // 8 loads in flight; same summation order as a serial loop
-            double v1[4], v2[4];
+        // 16 loads in flight; same summation order as a serial loop (a missing pair or o >= K adds +0.0, which leaves a sum that started
+        // at +0.0 unchanged)
+        for (int o0 = 0; o0 < K; o0 += 8) {
+            double v1[8], v2[8];
 #pragma unroll
-            for (int u = 0; u < 4; u++) {
+            for (int u = 0; u < 8; u++) {
                 const int o = o0 + u;
                 const int p1 = o < K ? s_slot[bA * K + o] : -1, p2 = o < K ? s_slot[o * K + bA] : -1;  // bA as reference node / as observing node
                 v1[u] = p1 >= 0 ? Mp[(size_t) p1 * 210 + i1] : 0.0;
                 v2[u] = p2 >= 0 ? Mp[(size_t) p2 * 210 + i2] : 0.0;
             }
 #pragma unroll
-            for (int u = 0; u < 4; u++) sum += v1[u], sum += v2[u];
+            for (int u = 0; u < 8; u++) sum += v1[u], sum += v2[u];
         }
     } else {  // two different poses: the (bA -> bB) and (bB -> bA) groups
         const int p1 = s_slot[bA * K + bB], p2 = s_slot[bB * K + bA];
@@ -409,48 +415,111 @@ __device__ __forceinline__ double gram2_entry(const BaCaps &C, const BaDev &D, i
     }
     return sum;
 }
-// stage 2 as its own kernel: landmark-sharded solves only (the vision Gram matrix must exist before the all-reduce)
-__global__ void __launch_bounds__(256) ba_pair_gram2(BaCaps C, BaDev D) {
-    __shared__ short s_slot[32 * 32];
-    const int w = blockIdx.y;
-    const LmState &st = D.st[w];
-    if (st.done || !st.need_lin) return;
-    const int K = D.dims[w].K, NCV = 6 * K + 7, nn = NCV + 1;
-    if ((int) blockIdx.x * 256 >= nn * nn) return;
-    gram2_slots(C, D, w, K, s_slot);
-    const int t = blockIdx.x * 256 + threadIdx.x;
-    if (t >= nn * nn) return;
-    const int A = t / nn, B = t - A * nn;
-    if (B < A) return;
-    const double sum = gram2_entry(C, D, w, K, s_slot, A, B);
-    double *Cout = D.CJ + (size_t) w * C.NCA * C.NCA;
-    Cout[(size_t) A * C.NCA + B] = sum;
-    Cout[(size_t) B * C.NCA + A] = sum;
+
+// ------------------------------------------------------------------------------------------------ Schur term + reduced camera system
+__device__ __forceinline__ double block_sum(double v, double *s_red);
+__device__ __forceinline__ double block_max(double v, double *s_red);
+__device__ __forceinline__ double *x_inbox(const BaDev &D, int peer, int w, int from);  // ba_split.cuh
+__device__ __forceinline__ int tri_idx(int A, int B, int ncv);
+
+// Entry (A <= B <= NCV) of the vision Gram matrix (cj, gathered here from Mp) and of the Schur term (cw): stores what the solve of the
+// pipeline that drives the handle reads.
+//   single GPU (fused pipeline): Hs = H_c + (cj - cw) on the vision rows (lower triangle) and D.visv = [diag H_vis | g_vis | W phi g_l];
+//   split pipeline: [tri(H_vis - Schur) | diag H_vis | g_vis | W phi g_l] straight into the owner's inbox (P2P stores; ba_signal publishes
+//                   them, the owner's ba_reduce sums the ranks);
+//   NCCL landmark shards: [H_vis g_vis | Schur term] stored symmetric in D.red, all-reduced, then turned into Hs by ba_hsum.
+__device__ __forceinline__ void schur_store(const BaCaps &C, const BaDev &D, int w, int K, const short *s_slot, int A, int B, double cw) {
+    const int NCV = 6 * K + 7;
+    const bool nccl = !D.S.split && D.world > 1;
+    if (A == NCV && !nccl) return;  // the r^T r corner: only the all-reduced buffer carries it
+    const size_t e = (size_t) w * C.NS * C.NS + (size_t) B * C.NS + A;
+    const double hc = !D.S.split && !nccl && B < NCV ? D.Hc[e] : 0.0;  // in flight during the gather
+    const double cj = gram2_entry(C, D, w, K, s_slot, A, B);
+    if (D.S.split) {
+        double *P = x_inbox(D, w % D.world, w, D.rank);
+        const int TRI = NCV * (NCV + 1) / 2;
+        if (B < NCV) {
+            P[tri_idx(A, B, NCV)] = cj - cw;
+            if (A == B) P[TRI + A] = cj;
+        } else {
+            P[TRI + NCV + A] = cj;       // g_vis
+            P[TRI + 2 * NCV + A] = cw;   // W phi g_l
+        }
+    } else if (nccl) {
+        const size_t NN = (size_t) C.NCA * C.NCA;
+        double *R = D.red + (size_t) w * (2 * NN + 8);
+        R[(size_t) A * C.NCA + B] = R[(size_t) B * C.NCA + A] = cj;
+        R[NN + (size_t) A * C.NCA + B] = R[NN + (size_t) B * C.NCA + A] = cw;
+    } else {
+        double *V = D.visv + (size_t) w * 3 * C.NCV;
+        if (B < NCV) {
+            D.Hs[e] = hc + (cj - cw);
+            if (A == B) V[A] = cj;
+        } else {
+            V[NCV + A] = cj, V[2 * NCV + A] = cw;
+        }
+    }
 }
 
-// ------------------------------------------------------------------------------------------------ Schur term
-// Schur SYRK on the FP64 tensor cores: CW[split] = sum over the split's landmarks of phi_l w_l w_l^T (stored symmetric), with
+// the scalars of the split / NCCL payloads: vision cost, sum rho^2 and max |g_l| over this rank's factors and landmarks (one CTA)
+__device__ __forceinline__ void schur_scalars(const BaCaps &C, const BaDev &D, int w, const WinDims &dm, double *s_red) {
+    const int tid = threadIdx.x;
+    double c = 0, q = 0, gm = 0;
+    for (int f = tid; f < dm.F; f += 256) c += D.costf[(size_t) w * C.F + f];
+    for (int l = tid; l < dm.L; l += 256) {
+        const double r = D.rho[(size_t) w * C.L + l];
+        q += r * r;
+        gm = fmax(gm, fabs(D.gl[(size_t) w * C.L + l]));
+    }
+    c = block_sum(c, s_red);
+    q = block_sum(q, s_red);
+    gm = block_max(gm, s_red);
+    if (tid != 0) return;
+    if (D.S.split) {
+        const int NCV = 6 * dm.K + 7, TRI = NCV * (NCV + 1) / 2;
+        double *P = x_inbox(D, w % D.world, w, D.rank);
+        P[TRI + 3 * NCV] = c, P[TRI + 3 * NCV + 1] = q, P[TRI + 3 * NCV + 2] = gm;
+    } else {
+        const size_t NN = (size_t) C.NCA * C.NCA;
+        double *R = D.red + (size_t) w * (2 * NN + 8);
+        R[2 * NN] = c, R[2 * NN + 1] = q;
+        for (int k = 2; k < 8; k++) R[2 * NN + k] = 0;
+        D.redmax[w] = gm;
+    }
+}
+
+// Schur SYRK on the FP64 tensor cores: the sum over the window's landmarks of phi_l w_l w_l^T, with
 // phi_l = s_l^2 / (s_l^2 h_l + clamp(s_l^2 h_l) / radius) the LM-damped landmark pivot.  DMMA.8x8x4 with k = 4 landmarks per step; as in
 // ba_lin_vis's Gram phase the A and B fragments of X^T X share one layout: lane reads A_W[l0 + lane%4][8 t + lane/4].  The CTA stages its
 // landmark rows (and phi) in shared memory once per pass -- leading dimension = 8 mod 16 doubles, so a fragment read is the minimal
 // two wavefronts -- and every warp accumulates two 16x16 super-tiles (2x2 DMMA tiles each) of the upper triangle per pass.
-// The BA_SPLIT_W landmark splits are separate CTAs whose partials ba_pack1 sums in fixed order (deterministic).
+// One thread-block CLUSTER of BA_SPLIT_W CTAs per window: CTA k accumulates the partial of landmark split k.  After each pass (16
+// super-tiles) every CTA puts its partials in shared memory over its staging rows, which the pass no longer needs; after a cluster barrier
+// each CTA owns a quarter of the pass's super-tiles, sums the BA_SPLIT_W partials of an entry over DSMEM in split order starting from 0.0
+// (deterministic) and hands the entry to schur_store.  The partials never leave the cluster.
 constexpr int SCHUR_RCH = 80;  // landmark rows staged per chunk (multiple of 4)
-__device__ __forceinline__ void schur_body(const BaCaps &C, const BaDev &D, int w, int split, int ld, double *sA /* [SCHUR_RCH][ld] rows, then phi[SCHUR_RCH] */) {
+constexpr int SCHUR_PASS = 16;  // super-tiles per pass
+__global__ void __cluster_dims__(BA_SPLIT_W, 1, 1) __launch_bounds__(256) ba_schur_dmma(BaCaps C, BaDev D, int ld) {
+    extern __shared__ double sA[];  // [SCHUR_RCH][ld] rows, then phi[SCHUR_RCH]; between passes: [SCHUR_PASS][256] partials
+    __shared__ short s_slot[32 * 32];
+    __shared__ double s_red[40];
+    cg::cluster_group cluster = cg::this_cluster();
+    const int w = blockIdx.y, split = blockIdx.x;  // cluster rank = split
     const LmState &st = D.st[w];
-    if (st.done) return;
+    if (st.done) return;  // per window: the whole cluster leaves
     const WinDims dm = D.dims[w];
     const int NCV = 6 * dm.K + 7, NCA = 4 * ((NCV + 1 + 3) / 4);
     const int T2 = (NCA + 15) / 16, nsuper = T2 * (T2 + 1) / 2;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, kk = lane & 3;
     double *sphi = sA + (size_t) SCHUR_RCH * ld;
     const double *A = D.AW + (size_t) w * C.LP * C.NCA;
-    double *Cout = D.CW + ((size_t) w * BA_SPLIT_W + split) * C.NCA * C.NCA;
     const double radius = st.radius;
     const int nsteps = (dm.L + 3) / 4;
     const int r_beg = 4 * (int) ((long long) nsteps * split / BA_SPLIT_W), r_end = min(dm.L, 4 * (int) ((long long) nsteps * (split + 1) / BA_SPLIT_W));
-    const int npass = (nsuper + 15) / 16;
+    const int npass = (nsuper + SCHUR_PASS - 1) / SCHUR_PASS;
+    gram2_slots(C, D, w, dm.K, s_slot);
     for (int pass = 0; pass < npass; pass++) {
+        if (pass > 0) cluster.barrier_wait();  // the peers have read this CTA's partials of the previous pass: its staging rows are free
         int si[2], sj[2];
         bool on[2];
 #pragma unroll
@@ -520,39 +589,45 @@ __device__ __forceinline__ void schur_body(const BaCaps &C, const BaDev &D, int 
                 }
             }
         }
+        __syncthreads();  // every warp is done with the staged rows
+        // super-tile (2 pass + h2) * 8 + warp -> slot h2 * 8 + warp, in C-fragment order: position 64 q + 32 e + lane holds (row g, col
+        // 2 kk + e) of DMMA tile q (conflict-free stores, and reads below)
 #pragma unroll
         for (int h2 = 0; h2 < 2; h2++) {
             if (!on[h2]) continue;
 #pragma unroll
-            for (int q = 0; q < 4; q++) {  // C fragment: (row g, cols 2 kk + {0, 1}) of tile (2 si + q/2, 2 sj + q%2)
+            for (int q = 0; q < 4; q++)
 #pragma unroll
-                for (int e = 0; e < 2; e++) {
-                    const int r = 8 * (2 * si[h2] + (q >> 1)) + g, cc = 8 * (2 * sj[h2] + (q & 1)) + 2 * kk + e;
-                    if (r <= cc && cc < NCA) {
-                        Cout[(size_t) r * C.NCA + cc] = acc[h2][q][e];
-                        Cout[(size_t) cc * C.NCA + r] = acc[h2][q][e];  // stored symmetric: ba_solve reads rows contiguously
-                    }
-                }
-            }
+                for (int e = 0; e < 2; e++) sA[(h2 * 8 + warp) * 256 + 64 * q + 32 * e + lane] = acc[h2][q][e];
+        }
+        cluster.sync();  // every split's partials of this pass are in place
+        // CTA `split` owns slots split, split + 4, ...; thread tid owns position tid of each
+        const int nslot = min(SCHUR_PASS, nsuper - SCHUR_PASS * pass);
+        double cw[SCHUR_PASS / BA_SPLIT_W];
+#pragma unroll
+        for (int j = 0; j < SCHUR_PASS / BA_SPLIT_W; j++) {
+            const int sl = split + BA_SPLIT_W * j;
+            double p[BA_SPLIT_W];
+#pragma unroll
+            for (int k = 0; k < BA_SPLIT_W; k++) p[k] = sl < nslot ? cluster.map_shared_rank(sA, k)[sl * 256 + tid] : 0.0;
+            cw[j] = 0;
+#pragma unroll
+            for (int k = 0; k < BA_SPLIT_W; k++) cw[j] += p[k];
+        }
+        cluster.barrier_arrive();  // done reading the peers (the matching wait comes before this CTA's shared memory is reused or released)
+        const int q = tid >> 6, r_in = 8 * (q >> 1) + ((tid & 31) >> 2), c_in = 8 * (q & 1) + 2 * (tid & 3) + ((tid >> 5) & 1);
+#pragma unroll
+        for (int j = 0; j < SCHUR_PASS / BA_SPLIT_W; j++) {
+            const int sl = split + BA_SPLIT_W * j;
+            if (sl >= nslot) break;
+            int a = 0, e = SCHUR_PASS * pass + sl;
+            while (e >= T2 - a) e -= T2 - a, a++;
+            const int r = 16 * a + r_in, cc = 16 * (a + e) + c_in;
+            if (r <= cc && cc <= NCV) schur_store(C, D, w, dm.K, s_slot, r, cc, cw[j]);
         }
     }
-}
-
-__global__ void __launch_bounds__(256) ba_schur_dmma(BaCaps C, BaDev D, int ld) {
-    extern __shared__ double sA[];
-    schur_body(C, D, blockIdx.y, blockIdx.x, ld, sA);
-}
-
-// symmetric read of the summed SYRK partials (upper tiles hold the data)
-__device__ __forceinline__ double syrk_get(const double *Cp, int nsplit, int NCAcap, int a, int b) {
-    if (a > b) {
-        int t = a;
-        a = b, b = t;
-    }
-    // tiles with ti <= tj are stored; within a diagonal tile both triangles are present
-    double s = 0;
-    for (int k = 0; k < nsplit; k++) s += Cp[(size_t) k * NCAcap * NCAcap + (size_t) a * NCAcap + b];
-    return s;
+    if (split == 0 && (D.S.split || D.world > 1)) schur_scalars(C, D, w, dm, s_red);
+    cluster.barrier_wait();  // no CTA leaves while a peer may still read its shared memory
 }
 
 // ------------------------------------------------------------------------------------------------ camera-only factors
@@ -822,52 +897,9 @@ __global__ void __launch_bounds__(CAM_THREADS) ba_lin_cam(BaCaps C, BaDev D) {
     if (threadIdx.x == 0) st.cost_cam = c;
 }
 
-__device__ __forceinline__ double block_sum(double v, double *s_red);
-__device__ __forceinline__ double block_max(double v, double *s_red);
-
 // ------------------------------------------------------------------------------------------------ reduction operands
-// Everything a landmark shard contributes to the window's reduced camera system goes into ONE contiguous buffer per window, so that
-// a sharded solve needs a single all-reduce (sum) per attempt: [H_vis g_vis | Schur term | vision cost, sum rho^2].
-constexpr int PACK1_SPLIT = 4;  // CTAs per window
-__global__ void __launch_bounds__(256) ba_pack1(BaCaps C, BaDev D) {
-    __shared__ double s_red[40];
-    const int w = blockIdx.x, tid = threadIdx.x, part = blockIdx.y;
-    const LmState &st = D.st[w];
-    if (st.done) return;
-    const WinDims dm = D.dims[w];
-    const int NN = C.NCA * C.NCA;
-    double *R = D.red + (size_t) w * (2 * NN + 8);
-    const double *CJ = D.CJ + (size_t) w * BA_SPLIT_J * NN, *CW = D.CW + (size_t) w * BA_SPLIT_W * NN;
-    const int e0 = (int) ((long long) NN * part / PACK1_SPLIT), e1 = (int) ((long long) NN * (part + 1) / PACK1_SPLIT);
-    for (int e = e0 + tid; e < e1; e += 256) {
-        const double cj = CJ[e];
-        double p[BA_SPLIT_W];
-#pragma unroll
-        for (int k = 0; k < BA_SPLIT_W; k++) p[k] = CW[(size_t) k * NN + e];
-        double s = 0;
-#pragma unroll
-        for (int k = 0; k < BA_SPLIT_W; k++) s += p[k];
-        R[e] = cj;
-        R[NN + e] = s;
-    }
-    if (part != 0) return;
-    double c = 0, q = 0, gm = 0;
-    for (int f = tid; f < dm.F; f += 256) c += D.costf[(size_t) w * C.F + f];
-    for (int l = tid; l < dm.L; l += 256) {
-        const double r = D.rho[(size_t) w * C.L + l];
-        q += r * r;
-        gm = fmax(gm, fabs(D.gl[(size_t) w * C.L + l]));
-    }
-    c = block_sum(c, s_red);
-    q = block_sum(q, s_red);
-    gm = block_max(gm, s_red);
-    if (tid == 0) {
-        R[2 * NN] = c, R[2 * NN + 1] = q;
-        for (int k = 2; k < 8; k++) R[2 * NN + k] = 0;
-        D.redmax[w] = gm;
-    }
-}
-
+// Everything a landmark shard contributes to the window's reduced camera system goes into ONE contiguous buffer per window (written by
+// ba_schur_dmma), so that a sharded solve needs a single all-reduce (sum) per attempt: [H_vis g_vis | Schur term | vision cost, sum rho^2].
 __global__ void ba_pack2(BaCaps C, BaDev D, int n, int nblk_vis) {
     const int w = blockIdx.x * blockDim.x + threadIdx.x;
     if (w >= n) return;
@@ -883,37 +915,20 @@ __global__ void ba_pack2(BaCaps C, BaDev D, int n, int nblk_vis) {
 }
 
 // ------------------------------------------------------------------------------------------------ reduced camera matrix
-// Hs = H_c + H_vis - Schur term, lower triangle, one thread per entry (wide and coalesced; ba_solve then reads ONE operand per entry
-// instead of gathering 2 + BA_SPLIT_W).  Landmark-sharded solve: the vision / Schur operands are the all-reduced buffer.
+// Hs = H_c + H_vis - Schur term of a landmark-sharded window (NCCL transport) from the all-reduced buffer, lower triangle, one thread per
+// entry (ba_solve then reads ONE operand per entry).  A single GPU's Hs is formed by ba_schur_dmma's epilogue.
 __global__ void __launch_bounds__(256) ba_hsum(BaCaps C, BaDev D) {
-    __shared__ short s_slot[32 * 32];
     const int w = blockIdx.y;
     if (D.st[w].done) return;
     const int K = D.dims[w].K, NCV = 6 * K + 7, nn = NCV + 1;
     const int NN = C.NCA * C.NCA;
-    if ((int) blockIdx.x * 256 >= nn * nn) return;
-    const bool sharded = D.world > 1;
-    if (!sharded) gram2_slots(C, D, w, K, s_slot);
     const int t = blockIdx.x * 256 + threadIdx.x;
     if (t >= nn * nn) return;
     const int A = t / nn, B = t - A * nn;  // A <= B: entry (row B, column A) of the lower triangle
-    if (B < A) return;
-    double cj, cw;
-    if (sharded) {
-        const double *RED = D.red + (size_t) w * (2 * NN + 8);
-        cj = RED[(size_t) B * C.NCA + A], cw = RED[NN + (size_t) B * C.NCA + A];
-    } else {
-        // single GPU: the gather of the per-pair Gram matrices (ba_pair_gram2's job) happens here, one kernel less on the path
-        cj = gram2_entry(C, D, w, K, s_slot, A, B);
-        double *Cout = D.CJ + (size_t) w * NN;
-        Cout[(size_t) A * C.NCA + B] = cj;
-        Cout[(size_t) B * C.NCA + A] = cj;
-        const double *CWp = D.CW + (size_t) w * BA_SPLIT_W * NN;
-        cw = 0;
-#pragma unroll
-        for (int k = 0; k < BA_SPLIT_W; k++) cw += CWp[(size_t) k * NN + (size_t) B * C.NCA + A];
-    }
-    if (B < NCV) D.Hs[(size_t) w * C.NS * C.NS + (size_t) B * C.NS + A] = D.Hc[(size_t) w * C.NS * C.NS + (size_t) B * C.NS + A] + (cj - cw);
+    if (B < A || B >= NCV) return;
+    const double *RED = D.red + (size_t) w * (2 * NN + 8);
+    const double cj = RED[(size_t) B * C.NCA + A], cw = RED[NN + (size_t) B * C.NCA + A];
+    D.Hs[(size_t) w * C.NS * C.NS + (size_t) B * C.NS + A] = D.Hc[(size_t) w * C.NS * C.NS + (size_t) B * C.NS + A] + (cj - cw);
 }
 
 // ------------------------------------------------------------------------------------------------ solve (one CTA per window)
@@ -988,20 +1003,14 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
     // pointer that could also be global made every access a generic LD / ST (longer latency, long-scoreboard tracked)
     double *S = s_diag + C.NS;
     const double *Hc = D.Hc + (size_t) w * C.NS * C.NS, *gcam = D.gc + (size_t) w * C.NS, *Hs = D.Hs + (size_t) w * C.NS * C.NS;
-    // Reduction operands.  Landmark-sharded solve: the packed, all-reduced buffer (identical on every shard, written by ba_pack1).
-    // Single GPU: read the producers' outputs directly (vision Gram matrix; the BA_SPLIT_W Schur partials summed in fixed order).
+    // Vision vectors [diag H_vis | g_vis | W phi g_l] (a < NCV).  Landmark-sharded solve: the packed, all-reduced buffer (identical on every
+    // shard).  Single GPU: the vectors ba_schur_dmma's epilogue wrote.
     const bool sharded = D.world > 1;
     const int NN = C.NCA * C.NCA;
-    const double *RED = D.red + (size_t) w * (2 * NN + 8);
-    const double *CJ = sharded ? RED : D.CJ + (size_t) w * BA_SPLIT_J * NN;
-    const double *CWp = sharded ? RED + NN : D.CW + (size_t) w * BA_SPLIT_W * NN;
-    auto cw_get = [&](int a, int b) {  // symmetric storage: any (a, b)
-        if (sharded) return CWp[(size_t) a * C.NCA + b];
-        double s2 = 0;
-#pragma unroll
-        for (int k = 0; k < BA_SPLIT_W; k++) s2 += CWp[(size_t) k * NN + (size_t) a * C.NCA + b];
-        return s2;
-    };
+    const double *RED = D.red + (size_t) w * (2 * NN + 8), *V = D.visv + (size_t) w * 3 * C.NCV;
+    auto hvis_diag = [&](int a) { return sharded ? RED[(size_t) a * C.NCA + a] : V[a]; };
+    auto g_vis = [&](int a) { return sharded ? RED[(size_t) a * C.NCA + NCV] : V[NCV + a]; };
+    auto wphig = [&](int a) { return sharded ? RED[NN + (size_t) a * C.NCA + NCV] : V[2 * NCV + a]; };
     const double camw = D.rank == 0 ? 1.0 : 0.0;       // camera-side partial sums are counted on shard 0 only
     if (tid == 0 && st.need_lin) st.need_lin = 0;      // the linearisation kernels of this iteration have run (stream order)
     double *scale_c = D.scale_c + (size_t) w * C.NS;
@@ -1010,10 +1019,10 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
     // ---- after a fresh linearisation: total cost, gradient, (first time) Jacobi scaling
     for (int a = tid; a < N; a += SOLVE_THREADS) {
         double g = gcam[a];
-        if (a < NCV) g += syrk_get(CJ, 1, C.NCA, a, NCV);
+        if (a < NCV) g += g_vis(a);
         s_g[a] = g;
         if (f_first) {
-            double h = Hc[(size_t) a * C.NS + a] + (a < NCV ? syrk_get(CJ, 1, C.NCA, a, a) : 0.0);
+            double h = Hc[(size_t) a * C.NS + a] + (a < NCV ? hvis_diag(a) : 0.0);
             scale_c[a] = 1.0 / (1.0 + sqrt(h));
         }
     }
@@ -1066,7 +1075,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
     SOLVE_CLK(0)  // gradient, cost, termination tests
 
     // ---- assemble S' = s (H - Schur) s + D^2 (packed lower), rhs' = -s (g - W phi g_l)
-    // The reduced camera matrix (ba_hsum's output, row i contiguous) goes global -> packed shared rows with 8-byte cp.async: every element of
+    // The reduced camera matrix (Hs, row i contiguous) goes global -> packed shared rows with 8-byte cp.async: every element of
     // the lower triangle is in flight at once (one L2 round trip for the whole matrix instead of one per row and warp), the vector part below
     // overlaps the copy, and the Jacobi scaling + LM diagonal are applied in place afterwards.
     constexpr bool async_fill = true;
@@ -1080,10 +1089,10 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
         asm volatile("cp.async.commit_group;" ::: "memory");
     }
     for (int a = tid; a < N; a += SOLVE_THREADS) {
-        double h = Hc[(size_t) a * C.NS + a] + (a < NCV ? syrk_get(CJ, 1, C.NCA, a, a) : 0.0);
+        double h = Hc[(size_t) a * C.NS + a] + (a < NCV ? hvis_diag(a) : 0.0);
         double hs = s_scale[a] * s_scale[a] * h;
         s_d2[a] = fmin(fmax(hs, 1e-6), 1e32) / radius;
-        double gw = a < NCV ? cw_get(a, NCV) : 0.0;
+        double gw = a < NCV ? wphig(a) : 0.0;
         s_rhs[a] = -s_scale[a] * (s_g[a] - gw);
     }
     if (async_fill) asm volatile("cp.async.wait_all;" ::: "memory");
@@ -1108,7 +1117,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
             for (int q = 0; q < MAXQ; q++) {
                 const int j = (tid & 31) + 32 * q;
                 hv[q] = 0;
-                if (q < nq && j <= i) hv[q] = (i < NCV ? Hs : Hc)[(size_t) i * C.NS + j];  // ba_hsum: H_c + vision Gram - Schur (vision rows); row i contiguous
+                if (q < nq && j <= i) hv[q] = (i < NCV ? Hs : Hc)[(size_t) i * C.NS + j];  // Hs: H_c + vision Gram - Schur (vision rows); row i contiguous
             }
 #pragma unroll
             for (int q = 0; q < MAXQ; q++) {
@@ -2029,7 +2038,7 @@ static int ba_create_body(icg_ba *h, int max_windows, int max_K, int max_L, int 
     if (rc == ICG_OK) rc = dmalloc(h, &D.field, count);
     DM(pose_c, NW * C.K * 7) DM(mix_c, NW * C.K * 9) DM(ext_c, NW * 8) DM(rho_c, NW * C.L)
     DM(pose_0, NW * C.K * 7) DM(mix_0, NW * C.K * 9) DM(ext_0, NW * 8) DM(rho_0, NW * C.L)
-    DM(AW, NW * C.NCA * C.LP) DM(Mp, NW * (size_t) C.K * (C.K - 1) * 210) DM(CJ, NW * BA_SPLIT_J * C.NCA * C.NCA) DM(CW, NW * BA_SPLIT_W * C.NCA * C.NCA)
+    DM(AW, NW * C.NCA * C.LP) DM(Mp, NW * (size_t) C.K * (C.K - 1) * 210) DM(visv, NW * 3 * C.NCV)
     DM(gpart, NW * (size_t) C.GQ * 210) DM(costf, NW * C.F) DM(hl, NW * C.L) DM(gl, NW * C.L) DM(scale_l, NW * C.L) DM(scale_c, NW * C.NS)
     DM(Hc, NW * C.NS * C.NS) DM(gc, NW * C.NS) DM(Hs, NW * C.NS * C.NS) DM(cost_part, NW * (h->nblk_vis + 1)) DM(red, NW * (2 * (size_t) C.NCA * C.NCA + 8)) DM(redmax, NW) DM(red2, NW * 4) DM(step_c, NW * C.NS) DM(step_l, NW * C.L)
 #undef DM
@@ -2060,7 +2069,7 @@ static int ba_create_body(icg_ba *h, int max_windows, int max_K, int max_L, int 
         ICG_CUDA(raise_dynamic_smem((const void *) ba_solve, (size_t) (h->smem_solve)));
     }
     h->ld_schur = 16 * ((C.NCA + 15) / 16) + 8;  // = 8 mod 16 doubles: conflict-free fragment reads
-    h->smem_schur = sizeof(double) * ((size_t) SCHUR_RCH * h->ld_schur + SCHUR_RCH);
+    h->smem_schur = sizeof(double) * std::max((size_t) SCHUR_RCH * h->ld_schur + SCHUR_RCH, (size_t) SCHUR_PASS * 256);  // staging | one pass's partials
     ICG_CUDA(raise_dynamic_smem((const void *) ba_schur_dmma, (size_t) (h->smem_schur)));
     ICG_CUDA(cudaFuncSetAttribute(ba_schur_dmma, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     ICG_CUDA(raise_dynamic_smem((const void *) ba_lin_cam, (size_t) (h->smem_cam)));
@@ -2340,8 +2349,8 @@ int icg_ba_upload(icg_ba *h, int n, const icg_ba_problem *P) {
 }
 
 // ---- in-situ stage timing
-static const char *PROF_NAMES[16] = {"(gap/other)", "lin_vis", "lin_lm", "", "pair_gram2", "schur_dmma", "join lin_cam + lin_done",
-                                     "pack1 / export + signal", "solve", "cost (+cost_cam)", "pack2 / exchange", "accept", "hsum / reduce", "join gram chain", "step_lm", ""};
+static const char *PROF_NAMES[16] = {"(gap/other)", "lin_vis", "lin_lm", "", "", "schur_dmma (+ epilogue)", "join lin_cam + lin_done",
+                                     "signal", "solve", "cost (+cost_cam)", "pack2 / exchange", "accept", "hsum / reduce", "join gram chain", "step_lm", ""};
 static void prof_mark(icg_ba *h, int tag) {
     if (!h->prof) return;
     if (h->prof_used == h->prof_ev.size()) {
@@ -2415,8 +2424,9 @@ static int enqueue_lm(icg_ba *h, int max_num_iterations) {
     const dim3 g_vis(C.NVB - 2, n), g_cost(h->nblk_vis, n);
     // iteration 0 linearisation + (max_iter) x [schur syrk, solve, cost, accept, re-linearise]; one extra solve call
     // performs the final termination bookkeeping.
-    // where the camera-only factors are forked: 0 = beside ba_lin_vis (round 1), 1 = behind it, beside the Schur / Gram kernels (ba_lin_vis holds
-    // 128 registers x 4 CTAs: a 320-thread camera CTA on the same SM costs it a resident CTA).  Chosen by measurement (in-kernel phase clocks, ICG_BA_PROFILE).
+    // where the camera-only factors are forked: 0 = beside ba_lin_vis (round 1), 1 = behind it (ba_lin_vis holds 128 registers x 4 CTAs: a
+    // 320-thread camera CTA on the same SM costs it a resident CTA; on a single GPU nothing runs beside it then, the Schur kernel's epilogue
+    // reads H_c).  Chosen by measurement (in-kernel phase clocks, ICG_BA_PROFILE).
     static const int cam_fork = getenv("ICG_BA_CAM_FORK") ? atoi(getenv("ICG_BA_CAM_FORK")) : 0;
     for (int it = 0; it <= max_num_iterations; it++) {
         // fork: IMU / GNSS / prior factors (one latency-bound CTA per window) run beside the vision chain
@@ -2437,27 +2447,25 @@ static int enqueue_lm(icg_ba *h, int max_num_iterations) {
         }
         // (measured: one fused launch or two streams are both slower -- the Schur CTAs' shared memory throttles the latency-bound
         //  Gram warps when they share SMs)
+        if (!h->comm) {  // single GPU: the Schur kernel's epilogue adds H_c
+            ICG_CUDA(cudaStreamWaitEvent(s, h->ev_join, 0));
+            prof_mark(h, 6);
+        }
         ba_schur_dmma<<<dim3(BA_SPLIT_W, n), 256, h->smem_schur, s>>>(C, D, h->ld_schur);
         prof_mark(h, 5);
-        if (h->comm) {
-            ba_pair_gram2<<<dim3(((C.NCV + 1) * (C.NCV + 1) + 255) / 256, n), 256, 0, s>>>(C, D);
-            prof_mark(h, 4);
-        }
-        ICG_CUDA(cudaStreamWaitEvent(s, h->ev_join, 0));
-        prof_mark(h, 6);
         if (h->comm) {  // landmark-sharded window: one sum all-reduce of [H_vis g | Schur | cost, |rho|^2] + one max all-reduce
-            ba_pack1<<<dim3(n, PACK1_SPLIT), 256, 0, s>>>(C, D);
-            prof_mark(h, 7);
+            ICG_CUDA(cudaStreamWaitEvent(s, h->ev_join, 0));
+            prof_mark(h, 6);
             int rc = nccl_allreduce(h, D.red, (size_t) n * (2 * (size_t) C.NCA * C.NCA + 8), 0);
             if (rc != ICG_OK) return rc;
             rc = nccl_allreduce(h, D.redmax, (size_t) n, 1);
             if (rc != ICG_OK) return rc;
+            ba_hsum<<<dim3(((C.NCV + 1) * (C.NCV + 1) + 255) / 256, n), 256, 0, s>>>(C, D);
+            prof_mark(h, 12);
         }
-        ba_hsum<<<dim3(((C.NCV + 1) * (C.NCV + 1) + 255) / 256, n), 256, 0, s>>>(C, D);
-        prof_mark(h, 12);
         ba_solve<<<n, SOLVE_THREADS, h->smem_solve, s>>>(C, D);
         prof_mark(h, 8);
-        count_launch(h->comm ? 7 : 5);
+        count_launch(h->comm ? 5 : 4);
         if (it == max_num_iterations) break;
         ICG_CUDA(cudaEventRecord(h->ev_fork, s));
         ICG_CUDA(cudaStreamWaitEvent(h->stream_cam, h->ev_fork, 0));
@@ -2595,9 +2603,8 @@ static int enqueue_lm_split(icg_ba *h, int max_num_iterations) {
         prof_mark(h, 0);
         ba_lin_vis<<<g_vis, 128, LV_SMEM, s>>>(C, D);
         prof_mark(h, 1);
-        ba_schur_dmma<<<dim3(BA_SPLIT_W, n), 256, h->smem_schur, s>>>(C, D, h->ld_schur);
+        ba_schur_dmma<<<dim3(BA_SPLIT_W, n), 256, h->smem_schur, s>>>(C, D, h->ld_schur);  // + the export into the owner's inbox
         prof_mark(h, 5);
-        ba_export<<<g_nn, 256, 0, s>>>(C, D);
         ba_signal<<<1, 32, 0, s>>>(D, epoch);
         prof_mark(h, 7);
         ICG_CUDA(cudaStreamWaitEvent(s, h->ev_join, 0));
@@ -2609,7 +2616,7 @@ static int enqueue_lm_split(icg_ba *h, int max_num_iterations) {
         prof_mark(h, 8);
         ba_step_lm<<<dim3(n, STEP_SLICES), SOLVE_THREADS, h->smem_step_lm, s>>>(C, D, epoch);
         prof_mark(h, 14);
-        count_launch(8);
+        count_launch(7);
         if (it == max_num_iterations) break;
         ICG_CUDA(cudaEventRecord(h->ev_fork, s));
         ICG_CUDA(cudaStreamWaitEvent(h->stream_cam, h->ev_fork, 0));

@@ -3,9 +3,10 @@
 //
 // One LM attempt, rank g of G (G = 1: everything is local), windows w = 0 .. W-1, owner(w) = w mod G:
 //
-//   every rank   ba_lin_vis / ba_schur_dmma                     its landmark shard of every window (the kernels of the fused pipeline)
-//   every rank   ba_export        packs [tri(H_vis - Schur) | diag H_vis | g_vis | W phi g_l | cost, sum rho^2, max |g_l|] of window w and
-//                                 STORES it into the inbox of owner(w) -- peer memory over NVLink (P2P stores), slot [w / G][g]
+//   every rank   ba_lin_vis / ba_schur_dmma                     its landmark shard of every window (the kernels of the fused pipeline);
+//                                 the Schur kernel's epilogue packs [tri(H_vis - Schur) | diag H_vis | g_vis | W phi g_l | cost, sum rho^2,
+//                                 max |g_l|] of window w and STORES it into the inbox of owner(w) -- peer memory over NVLink (P2P stores),
+//                                 slot [w / G][g]
 //                ba_signal        release-flag "my partials of this epoch have landed" on every peer
 //   owner        ba_reduce        waits for the G flags, sums the G slots in rank order (deterministic, identical regardless of arrival
 //                                 order) into Hs = H_c + sum; the reduction is fused into the assembly of the solve's operand
@@ -73,54 +74,7 @@ __device__ __forceinline__ unsigned long long *x_flagC(const BaDev &D, int peer,
 }
 __device__ __forceinline__ int tri_idx(int A, int B, int ncv) { return A * ncv - A * (A - 1) / 2 + (B - A); }  // A <= B < ncv
 
-// ------------------------------------------------------------------------------------------------ export (every rank)
-// thread per entry (A <= B) of the symmetric (NCV+1)^2 matrix [H_vis g_vis; g_vis^T .]: gathers the per-pair Gram matrices (ba_hsum's job in the
-// fused pipeline), subtracts the Schur partials and stores into the owner's inbox.  Block 0 of a window also reduces the scalars.
-__global__ void __launch_bounds__(256) ba_export(BaCaps C, BaDev D) {
-    __shared__ short s_slot[32 * 32];
-    __shared__ double s_red[40];
-    const int w = blockIdx.y, tid = threadIdx.x;
-    const LmState &st = D.st[w];
-    if (st.done) return;
-    const WinDims dm = D.dims[w];
-    const int K = dm.K, NCV = 6 * K + 7, nn = NCV + 1;
-    if ((int) blockIdx.x * 256 >= nn * nn) return;
-    const int owner = w % D.world;
-    double *P = x_inbox(D, owner, w, D.rank);
-    const int TRI = NCV * (NCV + 1) / 2;
-    gram2_slots(C, D, w, K, s_slot);
-    const int t = blockIdx.x * 256 + tid;
-    if (t < nn * nn) {
-        const int A = t / nn, B = t - A * nn;
-        if (B >= A && A < NCV) {
-            const double cj = gram2_entry(C, D, w, K, s_slot, A, B);
-            const double *CWp = D.CW + (size_t) w * BA_SPLIT_W * C.NCA * C.NCA;
-            double cw = 0;
-#pragma unroll
-            for (int k = 0; k < BA_SPLIT_W; k++) cw += CWp[(size_t) k * C.NCA * C.NCA + (size_t) B * C.NCA + A];
-            if (B < NCV) {
-                P[tri_idx(A, B, NCV)] = cj - cw;
-                if (A == B) P[TRI + A] = cj;
-            } else {
-                P[TRI + NCV + A] = cj;       // g_vis
-                P[TRI + 2 * NCV + A] = cw;   // W phi g_l
-            }
-        }
-    }
-    if (blockIdx.x != 0) return;
-    double c = 0, q = 0, gm = 0;
-    for (int f = tid; f < dm.F; f += 256) c += D.costf[(size_t) w * C.F + f];
-    for (int l = tid; l < dm.L; l += 256) {
-        const double r = D.rho[(size_t) w * C.L + l];
-        q += r * r;
-        gm = fmax(gm, fabs(D.gl[(size_t) w * C.L + l]));
-    }
-    c = block_sum(c, s_red);
-    q = block_sum(q, s_red);
-    gm = block_max(gm, s_red);
-    if (tid == 0) P[TRI + 3 * NCV] = c, P[TRI + 3 * NCV + 1] = q, P[TRI + 3 * NCV + 2] = gm;
-}
-
+// ------------------------------------------------------------------------------------------------ signal (every rank)
 // everything this rank stored for `epoch` has been issued by earlier kernels of the stream: publish (one thread per peer)
 __global__ void ba_signal(BaDev D, unsigned long long epoch) {
     const int q = threadIdx.x;
@@ -140,7 +94,7 @@ __global__ void __launch_bounds__(256) ba_reduce(BaCaps C, BaDev D, unsigned lon
     __syncthreads();
     const int t = blockIdx.x * 256 + tid;
     if (t >= nn * nn) return;
-    const int A = t / nn, B = t - A * nn;  // same thread -> entry map as ba_export
+    const int A = t / nn, B = t - A * nn;
     if (B < A) return;
     const double *P0 = x_inbox(D, D.rank, w, 0);
     const size_t PK = D.S.PK;
