@@ -70,6 +70,9 @@ def _declare(L: C.CDLL) -> None:
     L.icg_detect_blocks.argtypes = [vp, vp, vp, C.c_int, C.c_int, vp, vp, C.c_double, C.c_double, C.c_int, vp, vp]
     L.icg_detect_blocks_dev.argtypes = [vp, C.c_int, vp, C.c_int, C.c_size_t, vp, C.c_int, vp, vp, C.c_double, C.c_double, C.c_int, vp, vp]
     L.icg_corner_subpix.argtypes = [vp, vp, C.c_int, vp, C.c_int]
+    L.icg_detect_features.argtypes = [vp, vp, C.c_int, vp, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]
+    L.icg_detect_features_dev.argtypes = [vp, C.c_int, vp, C.c_int, C.c_size_t, vp, vp, vp, vp, vp, vp, vp, vp, C.c_int, vp, vp]
+    L.icg_detect_mask_dev.argtypes = [vp, C.c_int, C.POINTER(vp), C.POINTER(C.c_int)]
     # ---- camera model (host functions)
     L.icg_camera_undistort_points.argtypes = [vp, vp, C.c_int]
     L.icg_camera_distort_points.argtypes = [vp, vp, C.c_int]
@@ -136,6 +139,7 @@ EXPORTS = [
     "icg_klt_upload_level0", "icg_klt_upload_batch", "icg_klt_slot_level0", "icg_klt_slot_level", "icg_klt_build_pyramids",
     "icg_klt_track_batch_dev", "icg_klt_sync", "icg_klt_download_level",
     "icg_detect_create", "icg_detect_destroy", "icg_detect_blocks", "icg_detect_blocks_dev", "icg_corner_subpix",
+    "icg_detect_features", "icg_detect_features_dev", "icg_detect_mask_dev",
     "icg_camera_undistort_points", "icg_camera_distort_points", "icg_camera_distort_camera_points", "icg_camera_pixel2cam", "icg_camera_world2pixel", "icg_tracking_histogram", "icg_find_fundamental_mat_ransac", "icg_triangulate_points",
     "icg_clahe_create", "icg_clahe_destroy", "icg_clahe_apply", "icg_clahe_apply_dev", "icg_clahe_apply_batch_dev", "icg_geom_create", "icg_geom_destroy", "icg_geom_undistort_points", "icg_geom_distort_points", "icg_geom_find_fundamental_mat_ransac", "icg_geom_triangulate_points", "icg_geom_imu_preintegrate_batch", "icg_clahe_sync",
     "icg_imu_preintegrate", "icg_ba_create", "icg_ba_destroy", "icg_ba_solve", "icg_ba_upload", "icg_ba_run", "icg_ba_download",

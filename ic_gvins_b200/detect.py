@@ -107,3 +107,45 @@ class Detector:
             if len(p):
                 out.append(p + np.array([x0, y0], np.float32))
         return np.concatenate(out, axis=0) if out else np.zeros((0, 2), np.float32)
+
+    def features_detection_points(self, img, feat_xy, new_xy, n_ref=None, ismask=True, max_features=300):
+        """Tracking::featuresDetection (tracking.cc:579-685) driven by the point lists, in one synchronous call (icg_detect_features):
+        feat_xy = the frame's map-point features (undistorted keyPoint()), new_xy = pts2d_new_ (distorted), n_ref = pts2d_ref_.size()
+        (default len(new_xy)); the library counts the points per block, draws the occupancy mask when `ismask` and detects the deficits.
+        Returns the new corners in frame coordinates (block order), or None when the gate skipped the frame (the caller keeps its lists)."""
+        img = np.ascontiguousarray(img, np.uint8)
+        a = np.ascontiguousarray(np.asarray(feat_xy, np.float32).reshape(-1, 2))
+        b = np.ascontiguousarray(np.asarray(new_xy, np.float32).reshape(-1, 2))
+        _, _, _, _, quota, _ = block_grid(self.W, self.H, max_features)
+        out = np.zeros((self.max_blocks * self.cap, 2), np.float32)
+        n = np.zeros(1, np.int32)
+        check(lib().icg_detect_features(self._h, vp(img.ctypes.data), img.strides[0], vp(a.ctypes.data), a.shape[0], vp(b.ctypes.data), b.shape[0],
+                                        len(b) if n_ref is None else int(n_ref), 1 if ismask else 0, int(max_features), vp(out.ctypes.data),
+                                        vp(n.ctypes.data)), "icg_detect_features")
+        return None if n[0] < 0 else out[:n[0]].copy()
+
+    def features_detection_dev(self, n_frames, dev_img, pitch, frame_stride, dev_feat_xy, dev_feat_status, feat_off, dev_new_xy, dev_new_status,
+                               new_off, dev_out_xy, dev_out_n, n_ref=None, ismask=None, max_features=300):
+        """The same for `n_frames` device-resident frames (icg_detect_features_dev; asynchronous on the handle's stream).  Point lists, status
+        bytes (or 0) and outputs are device addresses; feat_off / new_off (n_frames + 1), n_ref and ismask (n_frames) are host sequences.
+        Frame f's corners land at dev_out_xy + f * cols * rows * quota * 2 floats, dev_out_n[f] = their number (-1: gated, -2: capacity)."""
+        fo = np.ascontiguousarray(np.asarray(feat_off, np.int32).reshape(-1))
+        no = np.ascontiguousarray(np.asarray(new_off, np.int32).reshape(-1))
+        if fo.size != n_frames + 1 or no.size != n_frames + 1:
+            raise ValueError("feat_off and new_off need n_frames + 1 entries")
+        nr = np.ascontiguousarray(np.asarray(n_ref, np.int32).reshape(-1)) if n_ref is not None else None
+        im = np.ascontiguousarray(np.asarray(ismask, np.uint8).reshape(-1)) if ismask is not None else None
+        for x in (nr, im):
+            if x is not None and x.size != n_frames:
+                raise ValueError("n_ref and ismask need n_frames entries")
+        check(lib().icg_detect_features_dev(self._h, n_frames, vp(dev_img), pitch, frame_stride, vp(dev_feat_xy) if dev_feat_xy else None,
+                                            vp(dev_feat_status) if dev_feat_status else None, vp(fo.ctypes.data), vp(dev_new_xy) if dev_new_xy else None,
+                                            vp(dev_new_status) if dev_new_status else None, vp(no.ctypes.data),
+                                            vp(nr.ctypes.data) if nr is not None else None, vp(im.ctypes.data) if im is not None else None,
+                                            int(max_features), vp(dev_out_xy), vp(dev_out_n)), "icg_detect_features_dev")
+
+    def mask_dev(self, frame=0):
+        """(device address, row pitch) of frame `frame`'s occupancy mask as the last features_detection_* call built it."""
+        p, pitch = vp(), C.c_int()
+        check(lib().icg_detect_mask_dev(self._h, frame, C.byref(p), C.byref(pitch)), "icg_detect_mask_dev")
+        return p.value, pitch.value

@@ -201,6 +201,37 @@ int icg_detect_blocks(icg_detect *h, const uint8_t *img, const uint8_t *mask, in
 int icg_detect_blocks_dev(icg_detect *h, int n_frames, const uint8_t *dev_img, int pitch, size_t frame_stride, const uint8_t *dev_mask, int n_blocks,
                           const icg_rect *rois, const int32_t *max_corners, double quality, double min_distance, int do_subpix, float *out_xy,
                           int32_t *out_n);
+/*
+ * Tracking::featuresDetection (IG/tracking/tracking.cc:576-685) up to the append into the reference's lists, driven by the point lists:
+ *   gate (:579-582): |feat| + n_ref > max_features - 5 -> the frame is not detected, *out_n = -1 (the caller keeps its lists);
+ *   counts (:591-606): every feat point (undistorted keyPoint(), :598) and every new point (pts2d_new_, distorted, :602) goes into block
+ *     int(y / (float) bh) * cols + int(x / (float) bw) (a col == cols aliases into the next row's first block; indices outside the grid are
+ *     dropped); block k asks for quota - count[k] corners (:629) and is skipped when that is <= 0;
+ *   mask (:609-620, when ismask): 255, and 0 on the disc of radius min_dist around cvRound of every point, clipped to the frame;
+ *   goodFeaturesToTrack(quality 0.01, min_dist) + cornerSubPix per block as icg_detect_blocks (:627-656), then the shift to frame
+ *     coordinates (float) (col * bw) + x (:669-675).
+ * The grid is Tracking::Tracking's (:66-85): cols = lround(W / 200.0), rows = lround(H / 200.0), bw = W / cols, bh = H / rows,
+ * quota = lround(max_features / (double) (cols * rows)), min_dist = (int) round(200 / sqrt(quota * 1.5)).  ICG_EINVAL when quota exceeds the
+ * handle's max_corners_per_block, the frames' blocks exceed max_blocks, a block exceeds max_roi_pixels or the offsets are not monotone.
+ * Host buffers, one frame, synchronous.  out_xy: cols * rows * quota x 2 floats (frame coordinates, block order, OpenCV's order within a block);
+ * *out_n = the number of corners, -1 when the gate skipped the frame.  n_ref < 0 stands for n_new.
+ */
+int icg_detect_features(icg_detect *h, const uint8_t *img, int stride, const float *feat_xy, int n_feat, const float *new_xy, int n_new,
+                        int n_ref, int ismask, int max_features, float *out_xy, int32_t *out_n);
+/* The same for n_frames DEVICE-resident frames in one call (geometry as icg_detect_blocks_dev).  Point lists in DEVICE memory: frame f's feat
+ * points are dev_feat_xy[feat_off[f] .. feat_off[f + 1]), its new points likewise; feat_off / new_off are HOST arrays of n_frames + 1.
+ * dev_feat_status / dev_new_status: DEVICE u8 per point or NULL; a point with status 0 is neither counted nor masked, so the LK status of
+ * icg_klt_track_batch_dev can be passed without compacting.  n_ref: HOST, n_frames, or NULL = the number of valid points of the frame's new
+ * list.  ismask: HOST, n_frames (NULL = all set).  Outputs in DEVICE memory: frame f's corners at dev_out_xy + f * cols * rows * quota * 2,
+ * dev_out_n[f] as *out_n above, or -2 when an internal capacity was exceeded.  Asynchronous on the handle's stream.  The first call allocates
+ * one pitch x height mask plane per frame the handle's max_blocks allows (ICG_ENOMEM if that fails). */
+int icg_detect_features_dev(icg_detect *h, int n_frames, const uint8_t *dev_img, int pitch, size_t frame_stride,
+                            const float *dev_feat_xy, const uint8_t *dev_feat_status, const int32_t *feat_off,
+                            const float *dev_new_xy, const uint8_t *dev_new_status, const int32_t *new_off,
+                            const int32_t *n_ref, const uint8_t *ismask, int max_features, float *dev_out_xy, int32_t *dev_out_n);
+/* device pointer + row pitch of frame f's occupancy mask as the last icg_detect_features[_dev] call built it (parity tests); the mask of a
+ * frame the gate skipped is not written */
+int icg_detect_mask_dev(icg_detect *h, int frame, void **dev_ptr, int *pitch);
 /* Drop-in for cv::cornerSubPix(img, corners, Size(5,5), Size(-1,-1), (COUNT+EPS, 20, 0.01)) on the whole frame; corners in/out */
 int icg_corner_subpix(icg_detect *h, const uint8_t *img, int stride, float *corners_xy, int n);
 
