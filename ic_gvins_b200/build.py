@@ -25,6 +25,7 @@ SOURCES = {
     "camera.cu": ["-fmad=false"],
     "fundamental.cu": ["-fmad=false"],  # host code; no contraction of the reference's double sequence
     "geom.cu": ["-fmad=false"],         # device versions of the camera model / RANSAC gate / triangulation / IMU propagation (same cores)
+    "track.cu": ["-fmad=false"],       # trackMappoint / trackReferenceFrame on the KLT handle (geom_core.cuh arithmetic)
     "ba.cu": [],
 }
 

@@ -1,7 +1,7 @@
 // fundamental.cu -- SURVEY.md 8f rank 3: the fundamental-matrix outlier gate of the front end and two-view triangulation, HOST entry points
 // (the serial reference loop: the iteration bound shrinks as better models are found, the subsets come from one cv::RNG stream).  The
-// arithmetic lives in geom_core.cuh; geom.cu runs the same cores on the device (all hypotheses solved and scored in parallel, the serial
-// acceptance rule replayed on the counts).
+// arithmetic lives in geom_core.cuh; geom.cu runs the same cores on the device (rounds of subsets solved and scored in parallel, the serial
+// acceptance rule replayed on each round's counts).
 //
 // Replaces cv::findFundamentalMat(pts_new_undis, pts_cur_undis, cv::FM_RANSAC, reprojection_error_std_, 0.99, status)
 // (IG/tracking/tracking.cc:547; only `status` is consumed, :549-553).  OpenCV is an un-vendored dependency of the reference; its

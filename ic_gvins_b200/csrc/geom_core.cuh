@@ -55,6 +55,47 @@ GC_HD void distort_point(const icg_camera &c, float *p) {  // Camera::distortPoi
     distort_xy(c, x, y, xd, yd);
     cam2pixel(c, xd, yd, 1.0, p[0], p[1]);
 }
+// Camera::distortCameraPoint (camera.cc:104-117): normalise by z, radtan, the distorted coordinates pass through float (:112-113), cam2pixel
+GC_HD void distort_camera_point(const icg_camera &c, double X, double Y, double Z, float &u, float &v) {
+    const double x = X / Z, y = Y / Z;
+    double xd, yd;
+    distort_xy(c, x, y, xd, yd);
+    cam2pixel(c, (double) (float) xd, (double) (float) yd, 1.0, u, v);
+}
+// Camera::world2cam (camera.cc:145-147): R^T (pw - t), R9 row-major; the products as fixed-order sums (no FMA: the callers build with -fmad=false)
+GC_HD void world2cam(const double *R9, const double *t3, const double *pw, double &x, double &y, double &z) {
+    const double d0 = pw[0] - t3[0], d1 = pw[1] - t3[1], d2 = pw[2] - t3[2];
+    x = R9[0] * d0 + R9[3] * d1 + R9[6] * d2;
+    y = R9[1] * d0 + R9[4] * d1 + R9[7] * d2;
+    z = R9[2] * d0 + R9[5] * d1 + R9[8] * d2;
+}
+// Camera::world2pixel (camera.cc:141-143) = cam2pixel(world2cam(pw, pose))
+GC_HD void world2pixel(const icg_camera &c, const double *R9, const double *t3, const double *pw, float &u, float &v) {
+    double x, y, z;
+    world2cam(R9, t3, pw, x, y, z);
+    cam2pixel(c, x, y, z, u, v);
+}
+// M = A^T B for row-major 3 x 3 A, B (R_cur^T R_pre of tracking.cc:465, pose1.R^T pose0.R of :867): M(i,j) = sum_k A(k,i) B(k,j), k ascending
+GC_HD void rt_mul(const double *A, const double *B, double *M) {
+    for (int i = 0; i < 3; i++)
+        for (int j = 0; j < 3; j++) M[3 * i + j] = A[i] * B[j] + A[3 + i] * B[3 + j] + A[6 + i] * B[6 + j];
+}
+// M v for row-major 3 x 3 M, fixed-order sums
+GC_HD void mat_vec(const double *M, double x, double y, double z, double &ox, double &oy, double &oz) {
+    ox = M[0] * x + M[1] * y + M[2] * z;
+    oy = M[3] * x + M[4] * y + M[5] * z;
+    oz = M[6] * x + M[7] * y + M[8] * z;
+}
+// Tracking::keyPointParallax (tracking.cc:861-871) with Rc1c0 = pose1.R^T pose0.R precomputed (rt_mul):
+//   |(Rc1c0 pixel2cam(pp0)).xy - pixel2cam(pp1).xy| * focalLength(),  focalLength() = (fx + fy) * 0.5 (camera.h:82-84)
+GC_HD double key_point_parallax(const icg_camera &c, const double *Rc1c0, float u0, float v0, float u1, float v1) {
+    double x0, y0, x1, y1, px, py, pz;
+    pixel2cam(c, u0, v0, x0, y0);
+    pixel2cam(c, u1, v1, x1, y1);
+    mat_vec(Rc1c0, x0, y0, 1.0, px, py, pz);
+    const double dx = px - x1, dy = py - y1;
+    return sqrt(dx * dx + dy * dy) * ((c.fx + c.fy) * 0.5);
+}
 
 // ------------------------------------------------------------------------------------------------ cv::findFundamentalMat(FM_RANSAC)
 struct CvRng {  // cv::RNG: multiply-with-carry, CV_RNG_COEFF = 4164903690
@@ -242,7 +283,7 @@ GC_HD bool is_inlier(const float *m1, const float *m2, int i, const double *F, d
     const float err = (float) (e1 > e2 ? e1 : e2);  // std::max(a, b): b unless a > b... max(a, b) = (a < b) ? b : a
     return err <= t;
 }
-inline int update_num_iters(double p, double ep, int model_points, int max_iters) {  // RANSACUpdateNumIters (host: replay loop only)
+GC_HD int update_num_iters(double p, double ep, int model_points, int max_iters) {  // RANSACUpdateNumIters (ptsetreg.cpp)
     p = p < 0. ? 0. : p > 1. ? 1. : p, ep = ep < 0. ? 0. : ep > 1. ? 1. : ep;
     double num = 1. - p > DBL_MIN ? 1. - p : DBL_MIN, denom = 1. - pow(1. - ep, model_points);
     if (denom < DBL_MIN) return 0;
@@ -422,4 +463,20 @@ GC_HD void preintegrate_core(const double *state16, const double *iewn3, const d
 }
 
 }  // namespace gc
+
+// ------------------------------------------------------------------------------------------------ batched device RANSAC (geom.cu)
+constexpr int RS_CTA = 64;      // subsets solved and scored per CTA and round == threads per CTA
+constexpr int RS_CLUSTER = 8;  // CTAs per set when the batch is small (64, then 8 x 64 subsets per round: 1 000 iterations in 3 rounds)
+struct RansacBatch {          // all DEVICE pointers; set s = pairs off[s] .. off[s] + n[s] (n == NULL: off[s + 1] - off[s])
+    const int *off, *n;
+    const float *p1, *p2;
+    const double *thr, *conf;  // per set; NULL = 3 / 0.99
+    int max_iters;
+    uint8_t *mask;             // per pair, at the pair's index
+    int *n_inliers;            // per set
+    double *F;                 // 9 per set, may be NULL
+    long long *stats;          // 3 per set (subsets drawn, clock64 cycles of the draw, of the whole CTA), may be NULL
+};
+int ransac_batch_launch(cudaStream_t st, int n_sets, const RansacBatch &B);
+
 }  // namespace icg

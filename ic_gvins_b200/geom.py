@@ -55,6 +55,22 @@ class Geometry:
               "icg_geom_find_fundamental_mat_ransac")
         return F.reshape(3, 3), st
 
+    def findFundamentalMat_batch_dev(self, set_off, dev_pts1, dev_pts2, dev_mask, dev_n_inliers, thresholds=None, confidences=None, maxIters=1000,
+                                     dev_F=0, dev_stats=0):
+        """cv2.findFundamentalMat(FM_RANSAC) on S device-resident point sets in one asynchronous call (icg_geom_find_fundamental_mat_ransac_batch):
+        set s = pairs set_off[s] .. set_off[s + 1] (host sequence of S + 1) of the float2 device arrays at dev_pts1 / dev_pts2; thresholds /
+        confidences: host sequences of S (None = 3 / 0.99).  Writes one u8 per pair at dev_mask, S int32 inlier counts at dev_n_inliers, and
+        optionally 9 doubles per set at dev_F and 3 int64 per set at dev_stats (subsets drawn, draw cycles, total cycles)."""
+        off = np.ascontiguousarray(np.asarray(set_off, np.int32).reshape(-1))
+        S = off.size - 1
+        th = np.ascontiguousarray(np.broadcast_to(np.asarray(thresholds, np.float64), (S,))) if thresholds is not None else None
+        cf = np.ascontiguousarray(np.broadcast_to(np.asarray(confidences, np.float64), (S,))) if confidences is not None else None
+        check(lib().icg_geom_find_fundamental_mat_ransac_batch(self._h, S, vp(off.ctypes.data), vp(dev_pts1) if dev_pts1 else None,
+                                                               vp(dev_pts2) if dev_pts2 else None, vp(th.ctypes.data) if th is not None else None,
+                                                               vp(cf.ctypes.data) if cf is not None else None, int(maxIters), vp(dev_mask),
+                                                               vp(dev_n_inliers), vp(dev_F) if dev_F else None, vp(dev_stats) if dev_stats else None),
+              "icg_geom_find_fundamental_mat_ransac_batch")
+
     def triangulatePoints(self, Tcw0, Tcw1, pc0, pc1):
         a = np.ascontiguousarray(np.array(Tcw0, np.float64).reshape(-1, 12))
         b = np.ascontiguousarray(np.array(Tcw1, np.float64).reshape(12))

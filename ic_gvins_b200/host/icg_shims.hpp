@@ -91,7 +91,72 @@ public:
               "icg_klt_track_fb");
     }
 
+    // Tracking::trackMappoint (IG/tracking/tracking.cc:351-455) from the prediction to the parallax, one call (icg_klt_track_frame with an
+    // empty reference list).  Inputs in the order :357-370 gathers them: pts2d_map (distortedKeyPoint), pts2d_map_undis (keyPoint),
+    // pw_xyz (mappoint->pos(), 3 doubles per point), ref_kp (the map point's keyPoint() in frame_ref_, NaN when it has none).  p: poses,
+    // camera, dt (prev_slot / cur_slot are set here: the two frames are uploaded into slots 0 and 1).  Outputs: pts2d_matched /
+    // pts2d_matched_undis / velocity_xy (2 doubles per point) of the survivors, src = their input indices (reduce mappoint_matched_ and
+    // mappoint_type with it).  parallax_map / parallax_map_counts are updated as :416-417 and :450 do and left alone when the reference
+    // returns before (:372-375).  Returns the reference's return value.
+    bool trackMappoint(const Mat &pre, const Mat &cur, icg_track_frame p, const std::vector<Point2f> &pts2d_map, const std::vector<Point2f> &pts2d_map_undis,
+                       const std::vector<double> &pw_xyz, const std::vector<Point2f> &ref_kp, std::vector<Point2f> &pts2d_matched,
+                       std::vector<Point2f> &pts2d_matched_undis, std::vector<double> &velocity_xy, std::vector<int32_t> &src, double &parallax_map,
+                       int &parallax_map_counts) {
+        const int n = (int) pts2d_map.size();
+        upload(pre, cur, p);
+        std::vector<Point2f> fwd(n), fwd_undis(n);
+        std::vector<uint8_t> keep(n);
+        pts2d_matched.resize(n), pts2d_matched_undis.resize(n), velocity_xy.resize(2 * (size_t) n), src.resize(n);
+        icg_track_map m{reinterpret_cast<const float *>(pts2d_map.data()), reinterpret_cast<const float *>(pts2d_map_undis.data()), pw_xyz.data(),
+                        reinterpret_cast<const float *>(ref_kp.data()), reinterpret_cast<float *>(fwd.data()), reinterpret_cast<float *>(fwd_undis.data()),
+                        keep.data(), reinterpret_cast<float *>(pts2d_matched.data()), reinterpret_cast<float *>(pts2d_matched_undis.data()), velocity_xy.data(),
+                        src.data()};
+        int32_t n_out[2];
+        double par[2];
+        int32_t par_n[2];
+        check(icg_klt_track_frame(h_, &p, n, &m, 0, nullptr, n_out, par, par_n), "icg_klt_track_frame");
+        pts2d_matched.resize(n_out[0]), pts2d_matched_undis.resize(n_out[0]), velocity_xy.resize(2 * (size_t) n_out[0]), src.resize(n_out[0]);
+        if (par_n[0] >= 0) parallax_map = par[0], parallax_map_counts = par_n[0];
+        return n_out[0] > 0;
+    }
+
+    // Tracking::trackReferenceFrame (IG/tracking/tracking.cc:457-574), one call (icg_klt_track_frame with an empty map list).  pts2d_new,
+    // pts2d_ref, ref_frame_id (pts2d_ref_frame_[k]->id()) and velocity_ref (2 doubles per point) are reduced in place as :507-511 and
+    // :550-554 reduce them, and pts2d_new becomes pts2d_cur_ (:569); src = the input index of every survivor (reduce pts2d_ref_frame_ with it);
+    // velocity_cur (2 doubles per point) = velocity_cur_.  parallax_ref / parallax_ref_counts are left alone when the reference returns before
+    // computing them (:459-462, :513-517).  Returns the reference's return value.  One corner differs: when the RANSAC rejects every survivor,
+    // the reference returns at :557-561 with pts2d_new_ still the gate-reduced list; here pts2d_new comes back empty like pts2d_ref.
+    bool trackReferenceFrame(const Mat &pre, const Mat &cur, icg_track_frame p, std::vector<Point2f> &pts2d_new, std::vector<Point2f> &pts2d_ref,
+                             std::vector<int64_t> &ref_frame_id, std::vector<double> &velocity_ref, std::vector<double> &velocity_cur, std::vector<int32_t> &src,
+                             double &parallax_ref, int &parallax_ref_counts) {
+        const int n = (int) pts2d_new.size();
+        upload(pre, cur, p);
+        std::vector<Point2f> fwd(n), fwd_undis(n), cur_pts(n), cur_undis(n), ref_out(n);
+        std::vector<uint8_t> keep(n);
+        std::vector<int64_t> id_out(n);
+        std::vector<double> vref_out(2 * (size_t) n);
+        velocity_cur.resize(2 * (size_t) n), src.resize(n);
+        icg_track_ref r{reinterpret_cast<const float *>(pts2d_new.data()), reinterpret_cast<const float *>(pts2d_ref.data()), ref_frame_id.data(),
+                        velocity_ref.data(), reinterpret_cast<float *>(fwd.data()), reinterpret_cast<float *>(fwd_undis.data()), keep.data(),
+                        reinterpret_cast<float *>(cur_pts.data()), reinterpret_cast<float *>(cur_undis.data()), velocity_cur.data(),
+                        reinterpret_cast<float *>(ref_out.data()), id_out.data(), vref_out.data(), src.data()};
+        int32_t n_out[2];
+        double par[2];
+        int32_t par_n[2];
+        check(icg_klt_track_frame(h_, &p, 0, nullptr, n, &r, n_out, par, par_n), "icg_klt_track_frame");
+        const int k = n_out[1];
+        cur_pts.resize(k), ref_out.resize(k), id_out.resize(k), vref_out.resize(2 * (size_t) k), velocity_cur.resize(2 * (size_t) k), src.resize(k);
+        pts2d_new.swap(cur_pts), pts2d_ref.swap(ref_out), ref_frame_id.swap(id_out), velocity_ref.swap(vref_out);
+        if (par_n[1] >= 0) parallax_ref = par[1], parallax_ref_counts = par_n[1];
+        return k > 0;
+    }
+
 private:
+    void upload(const Mat &pre, const Mat &cur, icg_track_frame &p) {
+        check(icg_klt_upload(h_, 0, mat_data(pre), mat_stride(pre)), "icg_klt_upload");
+        check(icg_klt_upload(h_, 1, mat_data(cur), mat_stride(cur)), "icg_klt_upload");
+        p.prev_slot = 0, p.cur_slot = 1;
+    }
     icg_klt *h_ = nullptr;
 };
 

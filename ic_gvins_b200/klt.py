@@ -10,6 +10,7 @@ import ctypes as C
 import numpy as np
 
 from ._lib import check, lib, vp
+from .camera import CameraStruct
 
 OPTFLOW_USE_INITIAL_FLOW = 4
 TERM_COUNT, TERM_EPS = 1, 2
@@ -17,6 +18,45 @@ TERM_COUNT, TERM_EPS = 1, 2
 
 def _ptr(a: np.ndarray):
     return C.c_void_p(a.ctypes.data)
+
+
+class TrackFrameStruct(C.Structure):
+    """ctypes image of `icg_track_frame` (per-stream parameters of trackMappoint / trackReferenceFrame)."""
+    _fields_ = [("prev_slot", C.c_int32), ("cur_slot", C.c_int32), ("camera", CameraStruct), ("R_pre", C.c_double * 9), ("R_cur", C.c_double * 9),
+                ("R_ref", C.c_double * 9), ("t_cur", C.c_double * 3), ("dt", C.c_double), ("ref_id", C.c_int64), ("fm_threshold", C.c_double)]
+
+
+MAP_IN = ("prev_xy", "prev_undis_xy", "pw", "ref_kp_xy")
+MAP_OUT = ("fwd_xy", "fwd_undis_xy", "keep", "cur_xy", "cur_undis_xy", "velocity", "src")
+REF_IN = ("new_xy", "ref_xy", "ref_frame_id", "velocity_ref")
+REF_OUT = ("fwd_xy", "fwd_undis_xy", "keep", "cur_xy", "cur_undis_xy", "velocity", "ref_out_xy", "ref_frame_id_out", "velocity_ref_out", "src")
+
+
+class TrackMapStruct(C.Structure):
+    """ctypes image of `icg_track_map` (all pointers)."""
+    _fields_ = [(k, C.c_void_p) for k in MAP_IN + MAP_OUT]
+
+
+class TrackRefStruct(C.Structure):
+    """ctypes image of `icg_track_ref` (all pointers)."""
+    _fields_ = [(k, C.c_void_p) for k in REF_IN + REF_OUT]
+
+
+# numpy (dtype, columns) of every list array; columns 1 = flat
+_SPEC = {"prev_xy": (np.float32, 2), "prev_undis_xy": (np.float32, 2), "pw": (np.float64, 3), "ref_kp_xy": (np.float32, 2),
+         "new_xy": (np.float32, 2), "ref_xy": (np.float32, 2), "ref_frame_id": (np.int64, 1), "velocity_ref": (np.float64, 2),
+         "fwd_xy": (np.float32, 2), "fwd_undis_xy": (np.float32, 2), "keep": (np.uint8, 1), "cur_xy": (np.float32, 2),
+         "cur_undis_xy": (np.float32, 2), "velocity": (np.float64, 2), "ref_out_xy": (np.float32, 2), "ref_frame_id_out": (np.int64, 1),
+         "velocity_ref_out": (np.float64, 2), "src": (np.int32, 1)}
+
+
+def track_frame_params(prev_slot, cur_slot, intrinsic, distortion, R_pre, R_cur, R_ref, t_cur, dt, ref_id, fm_threshold) -> TrackFrameStruct:
+    """icg_track_frame from Camera::createCamera's intrinsic / distortion lists and camera-to-world attitudes (Pose::R, 3 x 3)."""
+    i, d = list(map(float, intrinsic)), list(map(float, distortion))
+    cam = CameraStruct(i[0], i[1], i[2], i[3], i[4] if len(i) == 5 else 0.0, d[0], d[1], d[2], d[3], d[4] if len(d) == 5 else 0.0)
+    m = lambda a, n: (C.c_double * n)(*np.asarray(a, np.float64).reshape(n).tolist())  # noqa: E731
+    return TrackFrameStruct(int(prev_slot), int(cur_slot), cam, m(R_pre, 9), m(R_cur, 9), m(R_ref, 9), m(t_cur, 3), float(dt), int(ref_id),
+                            float(fm_threshold))
 
 
 class KltTracker:
@@ -107,6 +147,53 @@ class KltTracker:
                         status_ptr: int, mode: int = 1):
         check(lib().icg_klt_track_batch_dev(self._h, n_total, vp(slots_ptr), vp(prev_ptr), vp(init_ptr), vp(fwd_ptr),
                                             vp(bwd_ptr) if bwd_ptr else None, vp(status_ptr), mode), "icg_klt_track_batch_dev")
+
+    # ------------------------------------------------------------------ trackMappoint + trackReferenceFrame (tracking.cc:351-574)
+    def track_frame(self, params: TrackFrameStruct, map_lists=None, ref_lists=None):
+        """One stream from host arrays (icg_klt_track_frame, synchronous).  map_lists: dict with prev_xy, prev_undis_xy (n, 2) float32, pw (n, 3),
+        ref_kp_xy (n, 2) float32 (NaN = no feature in frame_ref_); ref_lists: dict with new_xy, ref_xy (m, 2) float32, ref_frame_id (m,) int64,
+        velocity_ref (m, 2).  Either may be None (empty).  Returns (map_out, ref_out, n_out[2], parallax[2], parallax_n[2]); the outputs are the
+        per-input fwd_xy / fwd_undis_xy / keep and the compacted lists cut to their counts."""
+        def prep(lists, names_in, names_out, struct):
+            lists = lists or {}
+            n = len(lists[names_in[0]]) if names_in[0] in lists else 0
+            arrs = {}
+            for k in names_in:
+                dt, c = _SPEC[k]
+                arrs[k] = np.ascontiguousarray(np.asarray(lists[k], dt).reshape(n, c) if n else np.zeros((1, c), dt))
+            for k in names_out:
+                dt, c = _SPEC[k]
+                arrs[k] = np.zeros((max(n, 1), c), dt)
+            return n, arrs, struct(*[a.ctypes.data for a in (arrs[k] for k in names_in + names_out)])
+        nm, am, sm = prep(map_lists, MAP_IN, MAP_OUT, TrackMapStruct)
+        nr, ar, sr = prep(ref_lists, REF_IN, REF_OUT, TrackRefStruct)
+        n_out, par, par_n = np.zeros(2, np.int32), np.zeros(2), np.zeros(2, np.int32)
+        check(lib().icg_klt_track_frame(self._h, C.byref(params), nm, C.byref(sm), nr, C.byref(sr), _ptr(n_out), _ptr(par), _ptr(par_n)),
+              "icg_klt_track_frame")
+
+        def cut(arrs, names_out, n, k_out):
+            out = {}
+            for k in names_out:
+                a = arrs[k][:n] if k in ("fwd_xy", "fwd_undis_xy", "keep") else arrs[k][:k_out]
+                out[k] = a.reshape(-1) if _SPEC[k][1] == 1 else a
+            return out
+        return cut(am, MAP_OUT, nm, int(n_out[0])), cut(ar, REF_OUT, nr, int(n_out[1])), n_out, par, par_n
+
+    def track_frames_dev(self, params, map_off, map_ptrs, ref_off, ref_ptrs, dev_n_out, dev_parallax, dev_parallax_n):
+        """B streams in one asynchronous call (icg_klt_track_frames_dev).  params: sequence of TrackFrameStruct; map_off / ref_off: host sequences
+        of B + 1; map_ptrs / ref_ptrs: dicts name -> device address (MAP_IN + MAP_OUT / REF_IN + REF_OUT; None or {} for a list with no points);
+        dev_n_out / dev_parallax / dev_parallax_n: device addresses of 2 B int32 / float64 / int32."""
+        B = len(params)
+        par = (TrackFrameStruct * B)(*params)
+        mo = np.ascontiguousarray(np.asarray(map_off, np.int32).reshape(-1))
+        ro = np.ascontiguousarray(np.asarray(ref_off, np.int32).reshape(-1))
+        if mo.size != B + 1 or ro.size != B + 1:
+            raise ValueError("map_off and ref_off need len(params) + 1 entries")
+        sm = TrackMapStruct(*[map_ptrs.get(k) for k in MAP_IN + MAP_OUT]) if map_ptrs else None
+        sr = TrackRefStruct(*[ref_ptrs.get(k) for k in REF_IN + REF_OUT]) if ref_ptrs else None
+        check(lib().icg_klt_track_frames_dev(self._h, B, par, _ptr(mo), C.byref(sm) if sm is not None else None, _ptr(ro),
+                                             C.byref(sr) if sr is not None else None, vp(dev_n_out), vp(dev_parallax), vp(dev_parallax_n)),
+              "icg_klt_track_frames_dev")
 
     def sync(self):
         check(lib().icg_klt_sync(self._h), "icg_klt_sync")
