@@ -133,6 +133,8 @@ def _declare_r2(L: C.CDLL) -> None:
     L.icg_geom_find_fundamental_mat_ransac_batch.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp, C.c_int, vp, vp, vp, vp]
     L.icg_klt_track_frames_dev.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp]
     L.icg_klt_track_frame.argtypes = [vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp]
+    L.icg_klt_triangulate_dev.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp, C.c_int, vp, vp, vp]
+    L.icg_klt_triangulate.argtypes = [vp, vp, C.c_int, vp, C.c_int, vp, vp, vp]
 
 
 # every symbol include/icgvins_b200.h declares (checked by tests/test_abi.py against the header text)
@@ -146,6 +148,7 @@ EXPORTS = [
     "icg_camera_undistort_points", "icg_camera_distort_points", "icg_camera_distort_camera_points", "icg_camera_pixel2cam", "icg_camera_world2pixel", "icg_tracking_histogram", "icg_find_fundamental_mat_ransac", "icg_triangulate_points",
     "icg_clahe_create", "icg_clahe_destroy", "icg_clahe_apply", "icg_clahe_apply_dev", "icg_clahe_apply_batch_dev", "icg_geom_create", "icg_geom_destroy", "icg_geom_undistort_points", "icg_geom_distort_points", "icg_geom_find_fundamental_mat_ransac", "icg_geom_triangulate_points", "icg_geom_imu_preintegrate_batch", "icg_clahe_sync",
     "icg_geom_find_fundamental_mat_ransac_batch", "icg_klt_track_frames_dev", "icg_klt_track_frame",
+    "icg_klt_triangulate_dev", "icg_klt_triangulate",
     "icg_imu_preintegrate", "icg_ba_create", "icg_ba_destroy", "icg_ba_solve", "icg_ba_upload", "icg_ba_run", "icg_ba_download",
     "icg_ba_sync", "icg_nccl_unique_id", "icg_ba_set_shard", "icg_ba_shard_export", "icg_ba_shard_connect", "icg_ba_shard_error", "icg_ba_gvins_optimization", "icg_ba_run_gvins", "icg_ba_gvins_optimization_begin", "icg_ba_gvins_optimization_end", "icg_ba_residual_costs", "icg_ba_reproj_evaluate", "icg_ba_imu_evaluate", "icg_ba_marginalize", "icg_ba_marginalize_resident", "icg_ba_gnss_evaluate", "icg_ba_pose_prior_evaluate", "icg_ba_mix_prior_evaluate", "icg_ba_imu_error_evaluate", "icg_ba_marg_factor_evaluate",
 ]

@@ -332,6 +332,25 @@ GC_HD void triangulate_point(const double *P0, const double *P1, const double *p
     }
     for (int k = 0; k < 3; k++) pw[k] = V[best][k] / V[best][3];
 }
+// Tracking::pose2Tcw (tracking.cc:851-859), top 3 rows: T = [R^T | -R^T t], 3 x 4 row-major; -R^T t as the fixed-order sum of world2cam
+GC_HD void pose_tcw(const double *R9, const double *t3, double *T12) {
+    for (int i = 0; i < 3; i++) {
+        T12[4 * i] = R9[i], T12[4 * i + 1] = R9[3 + i], T12[4 * i + 2] = R9[6 + i];
+        T12[4 * i + 3] = -(R9[i] * t3[0] + R9[3 + i] * t3[1] + R9[6 + i] * t3[2]);
+    }
+}
+// Tracking::isGoodToTrack(pp, pose, pw, 1.0, 3.0) (tracking.cc:813-829): isGoodDepth(z, 3) = 1 < z < 200 * 3 (:247-249, mappoint.h:52-53),
+// then |reprojectionError(pose, pw, pp)| <= std (camera.cc:153-157: world2pixel returns a cv::Point2f, so each difference is float - float)
+GC_HD bool good_to_track(const icg_camera &c, float u, float v, const double *R9, const double *t3, const double *pw, double std) {
+    double x, y, z;
+    world2cam(R9, t3, pw, x, y, z);
+    if (!(z > 1.0 && z < 200.0 * 3.0)) return false;
+    float pu, pv;
+    cam2pixel(c, x, y, z, pu, pv);
+    const float ex = pu - u, ey = pv - v;
+    const double dx = ex, dy = ey;
+    return !(sqrt(dx * dx + dy * dy) > std * 1.0);
+}
 
 // ------------------------------------------------------------------------------------------------ IMU preintegration propagation
 // PreintegrationEarth::resetState / integrationProcess / updateJacobianAndCovariance (IG/preintegration/preintegration_earth.cc:205-338) or, with

@@ -51,6 +51,11 @@ struct TrackScratch {
     uint8_t *d_rmask = nullptr;
     // device copies of the single-stream host call (icg_klt_track_frame)
     uint8_t *d_host = nullptr;
+    // triangulation (icg_klt_triangulate_dev): params | kf_off | ref_off | kf staged as one blob (pinned + its device copy, fenced by stage_ev),
+    // and the device copies of the single-stream host call (icg_klt_triangulate)
+    uint8_t *h_tri = nullptr, *d_tri = nullptr;
+    size_t tri_bytes = 0;
+    uint8_t *d_tri_host = nullptr;
 };
 
 void track_scratch_free(TrackScratch *t) {
@@ -58,6 +63,9 @@ void track_scratch_free(TrackScratch *t) {
     cudaFree(t->d_par), cudaFree(t->d_moff), cudaFree(t->d_roff), cudaFree(t->d_thr), cudaFree(t->d_n1), cudaFree(t->d_ninl);
     cudaFree(t->d_nu), cudaFree(t->d_rmask);
     if (t->d_host) cudaFree(t->d_host);
+    if (t->d_tri) cudaFree(t->d_tri);
+    if (t->d_tri_host) cudaFree(t->d_tri_host);
+    if (t->h_tri) cudaFreeHost(t->h_tri);
     if (t->h_stage) cudaFreeHost(t->h_stage);
     if (t->stage_ev) cudaEventDestroy(t->stage_ev);
     delete t;
@@ -294,6 +302,148 @@ __global__ void __launch_bounds__(TRK_THREADS) track_compact_kernel(TrackArgs A)
     if (tid == 0) A.n_out[2 * s + 1] = kept;
 }
 
+// ------------------------------------------------------------------------------------------------ Tracking::triangulation (:690-798)
+constexpr int TRI_MAX_KF = 64;             // table entries per stream
+constexpr double TRI_MIN_PARALLAX = 10.0;  // TRACK_MIN_PARALLAX (tracking.h:114)
+
+struct TriKf {             // one table entry with the products the points need, computed once per CTA
+    double Rck[9];         // R_cur^T R_kf: keyPointParallax with pose0 = the point's reference frame, pose1 = frame_cur_ (:741)
+    double T[12];          // pose2Tcw(pose_kf) (:749)
+    double R[9], t[3];     // pose_kf for world2cam (isGoodToTrack and the depth, :756, :765)
+    int64_t id;
+    int in_map;
+};
+
+struct TriArgs {
+    const icg_tri_frame *par;
+    const int32_t *koff, *roff;
+    const icg_tri_keyframe *kf;
+    const int32_t *n_in;
+    int n_in_stride;
+    icg_tri_list list;
+    icg_tri_new out;
+    int32_t *counts;
+};
+
+// CTA / stream: table -> shared memory, id check over the live list, then chunks of 256 points: thread per point for rules 2-8, two stable
+// block-prefix compactions (kept: in place, as track_compact_kernel; new: into out from the segment start)
+__global__ void __launch_bounds__(TRK_THREADS, 1) tri_kernel(TriArgs A) {
+    __shared__ TriKf s_kf[TRI_MAX_KF];
+    __shared__ double s_T1[12];
+    __shared__ int s_warp[TRK_THREADS / 32];
+    __shared__ int s_cnt[3];  // outlier, reset, outtime
+    const int s = blockIdx.x, tid = threadIdx.x;
+    const icg_tri_frame &P = A.par[s];
+    const icg_camera &cam = P.camera;
+    int32_t *cnt = A.counts + 5 * (size_t) s;
+    const int base = A.roff[s], seg = A.roff[s + 1] - base;
+    if (!P.triangulate) {  // not a keyframe of this stream: untouched
+        if (tid == 0) cnt[0] = -1, cnt[1] = cnt[2] = cnt[3] = cnt[4] = 0;
+        return;
+    }
+    const int n = A.n_in ? A.n_in[(size_t) s * A.n_in_stride] : seg;
+    if (n < 0 || n > seg || n == 0) {  // n == 0: pts2d_cur_.empty() -> return false (:692-694)
+        if (tid == 0) cnt[0] = n == 0 ? -1 : -2, cnt[1] = cnt[2] = cnt[3] = cnt[4] = 0;
+        return;
+    }
+    const int k0 = A.koff[s], nk = A.koff[s + 1] - k0;
+    for (int e = tid; e < nk; e += TRK_THREADS) {
+        const icg_tri_keyframe &K = A.kf[k0 + e];
+        TriKf &E = s_kf[e];
+        gc::rt_mul(P.R_cur, K.R, E.Rck);
+        gc::pose_tcw(K.R, K.t, E.T);
+        for (int q = 0; q < 9; q++) E.R[q] = K.R[q];
+        for (int q = 0; q < 3; q++) E.t[q] = K.t[q];
+        E.id = K.id, E.in_map = K.in_map;
+    }
+    if (tid == 0) {
+        gc::pose_tcw(P.R_cur, P.t_cur, s_T1);
+        s_cnt[0] = s_cnt[1] = s_cnt[2] = 0;
+    }
+    __syncthreads();
+    auto find = [&](int64_t id) {
+        for (int e = 0; e < nk; e++)
+            if (s_kf[e].id == id) return e;
+        return -1;
+    };
+    // every frame a point can name must be in the table; checked before anything is written (the compaction is in place)
+    bool miss = false;
+    for (int li = tid; li < n; li += TRK_THREADS) {
+        const int64_t fid = A.list.ref_frame_id_out[base + li];
+        miss = miss || (fid <= P.ref_id && find(fid) < 0);
+    }
+    if (__syncthreads_or(miss)) {
+        if (tid == 0) cnt[0] = -2, cnt[1] = cnt[2] = cnt[3] = cnt[4] = 0;
+        return;
+    }
+    int kept = 0, made = 0;
+    for (int c = 0; c < n; c += TRK_THREADS) {
+        const int li = c + tid, i = base + li;
+        const bool valid = li < n;
+        bool keep = false, made_pt = false;
+        float2 rp = make_float2(0.f, 0.f), cp = rp, ru = rp, cu = rp;
+        int64_t fid = 0;
+        double vr0 = 0, vr1 = 0, pw[3] = {0, 0, 0}, depth = 0;
+        if (valid) {
+            rp = ((const float2 *) A.list.ref_out_xy)[i], cp = ((const float2 *) A.list.cur_xy)[i];
+            fid = A.list.ref_frame_id_out[i];
+            vr0 = A.list.velocity_ref_out[2 * (size_t) i], vr1 = A.list.velocity_ref_out[2 * (size_t) i + 1];
+            float r[2] = {rp.x, rp.y}, q[2] = {cp.x, cp.y};
+            gc::undistort_point(cam, r);  // :708-713
+            gc::undistort_point(cam, q);
+            ru = make_float2(r[0], r[1]), cu = make_float2(q[0], q[1]);
+            if (fid > P.ref_id) {  // :723-730, before the window test
+                keep = true;
+                rp = cp, fid = P.cur_id;
+                atomicAdd(&s_cnt[1], 1);
+            } else {
+                const TriKf &E = s_kf[find(fid)];
+                if (P.window_normal && !E.in_map) {  // :733-737
+                    atomicAdd(&s_cnt[2], 1);
+                } else if (gc::key_point_parallax(cam, E.Rck, ru.x, ru.y, cu.x, cu.y) < TRI_MIN_PARALLAX) {  // :740-745
+                    keep = true;
+                } else {
+                    double pc0[2], pc1[2];
+                    gc::pixel2cam(cam, ru.x, ru.y, pc0[0], pc0[1]);  // :750-751
+                    gc::pixel2cam(cam, cu.x, cu.y, pc1[0], pc1[1]);
+                    gc::triangulate_point(E.T, s_T1, pc0, pc1, pw);  // :753
+                    if (gc::good_to_track(cam, ru.x, ru.y, E.R, E.t, pw, P.reprojection_error_std) &&
+                        gc::good_to_track(cam, cu.x, cu.y, P.R_cur, P.t_cur, pw, P.reprojection_error_std)) {  // :756-760
+                        double x, y;
+                        gc::world2cam(E.R, E.t, pw, x, y, depth);  // :764-765
+                        if (depth < 1.0 || depth > 200.0) depth = 10.0;  // MapPoint's constructor (mappoint.cc:39-42)
+                        made_pt = true;
+                    } else {
+                        atomicAdd(&s_cnt[0], 1);
+                    }
+                }
+            }
+        }
+        int tot_k, tot_m;
+        const int j = base + kept + block_prefix(keep, s_warp, &tot_k);  // contains the barriers that order the reads before the writes
+        const int o = base + made + block_prefix(made_pt, s_warp, &tot_m);
+        if (keep) {  // reduceVector (:788-791)
+            ((float2 *) A.list.ref_out_xy)[j] = rp, ((float2 *) A.list.cur_xy)[j] = cp;
+            A.list.ref_frame_id_out[j] = fid;
+            A.list.velocity_ref_out[2 * (size_t) j] = vr0, A.list.velocity_ref_out[2 * (size_t) j + 1] = vr1;
+            A.list.src[j] = li;
+        }
+        if (made_pt) {  // :761-784
+            const icg_tri_new &O = A.out;
+            O.pw[3 * (size_t) o] = pw[0], O.pw[3 * (size_t) o + 1] = pw[1], O.pw[3 * (size_t) o + 2] = pw[2];
+            O.depth[o] = depth;
+            ((float2 *) O.ref_undis_xy)[o] = ru, ((float2 *) O.ref_xy)[o] = rp;
+            ((float2 *) O.cur_undis_xy)[o] = cu, ((float2 *) O.cur_xy)[o] = cp;
+            O.velocity_cur[2 * (size_t) o] = A.list.velocity[2 * (size_t) i], O.velocity_cur[2 * (size_t) o + 1] = A.list.velocity[2 * (size_t) i + 1];
+            O.velocity_ref[2 * (size_t) o] = vr0, O.velocity_ref[2 * (size_t) o + 1] = vr1;
+            O.ref_frame_id[o] = fid, O.src[o] = li;
+        }
+        kept += tot_k, made += tot_m;
+    }
+    __syncthreads();
+    if (tid == 0) cnt[0] = kept, cnt[1] = made, cnt[2] = s_cnt[0], cnt[3] = s_cnt[1], cnt[4] = s_cnt[2];
+}
+
 }  // namespace icg
 
 using namespace icg;
@@ -425,9 +575,161 @@ int track_launch(icg_klt *h, const char *who, int n_streams, const icg_track_fra
     return ICG_OK;
 }
 
+bool tri_list_ptrs(const icg_tri_list *l) { return l && l->ref_out_xy && l->ref_frame_id_out && l->cur_xy && l->velocity_ref_out && l->velocity && l->src; }
+bool tri_new_ptrs(const icg_tri_new *o) {
+    return o && o->pw && o->depth && o->ref_undis_xy && o->ref_xy && o->cur_undis_xy && o->cur_xy && o->velocity_cur && o->velocity_ref && o->ref_frame_id &&
+           o->src;
+}
+
+// the triangulation launch; every pointer of list / out and dev_n_in / dev_counts are device pointers
+int tri_launch(icg_klt *h, const char *who, int n_streams, const icg_tri_frame *params, const int32_t *kf_off, const icg_tri_keyframe *kf,
+               const int32_t *ref_off, const int32_t *dev_n_in, int n_in_stride, const icg_tri_list *list, const icg_tri_new *out, int32_t *dev_counts) {
+    if (!h || n_streams < 1 || !params || !kf_off || !ref_off || !dev_counts || (dev_n_in && n_in_stride < 1)) {
+        set_error("%s: bad arguments", who);
+        return ICG_EINVAL;
+    }
+    int n_kf, n_pts;
+    if (bad_lists(who, n_streams, kf_off, kf != nullptr, &n_kf)) return ICG_EINVAL;
+    if (bad_lists(who, n_streams, ref_off, tri_list_ptrs(list) && tri_new_ptrs(out), &n_pts)) return ICG_EINVAL;
+    for (int s = 0; s < n_streams; s++) {
+        const icg_tri_frame &P = params[s];
+        if (!(P.camera.fx != 0.0) || !(P.camera.fy != 0.0)) {
+            set_error("%s: bad camera in stream %d", who, s);
+            return ICG_EINVAL;
+        }
+        const int k0 = kf_off[s], nk = kf_off[s + 1] - k0;
+        if (nk > TRI_MAX_KF) {
+            set_error("%s: %d keyframes in stream %d exceed %d", who, nk, s, TRI_MAX_KF);
+            return ICG_EINVAL;
+        }
+        for (int a = 0; a < nk; a++)
+            for (int b = 0; b < a; b++)
+                if (kf[k0 + a].id == kf[k0 + b].id) {
+                    set_error("%s: duplicate keyframe id %lld in stream %d", who, (long long) kf[k0 + a].id, s);
+                    return ICG_EINVAL;
+                }
+    }
+    ICG_CUDA(cudaSetDevice(h->device));
+    int rc = track_reserve(h, 1);  // creates the handle's scratch (stage event) on first use
+    if (rc != ICG_OK) return rc;
+    TrackScratch &t = *h->track;
+    const size_t S = n_streams, pb = (sizeof(icg_tri_frame) * S + 15) & ~(size_t) 15, ob = (4 * (S + 1) + 15) & ~(size_t) 15;
+    const size_t bytes = pb + 2 * ob + sizeof(icg_tri_keyframe) * (size_t) n_kf;
+    if (t.stage_pending) ICG_CUDA(cudaEventSynchronize(t.stage_ev));
+    t.stage_pending = false;
+    if (t.tri_bytes < bytes) {
+        ICG_CUDA(cudaStreamSynchronize(h->stream));  // the old device blob may still be read by an enqueued call
+        if (t.h_tri) cudaFreeHost(t.h_tri);
+        if (t.d_tri) cudaFree(t.d_tri);
+        t.h_tri = t.d_tri = nullptr, t.tri_bytes = 0;
+        if (cudaMallocHost(&t.h_tri, bytes) != cudaSuccess || cudaMalloc(&t.d_tri, bytes) != cudaSuccess) {
+            set_error("%s: staging allocation of %zu bytes failed", who, bytes);
+            return ICG_ENOMEM;
+        }
+        t.tri_bytes = bytes;
+    }
+    memcpy(t.h_tri, params, sizeof(icg_tri_frame) * S);
+    memcpy(t.h_tri + pb, kf_off, 4 * (S + 1));
+    memcpy(t.h_tri + pb + ob, ref_off, 4 * (S + 1));
+    if (n_kf) memcpy(t.h_tri + pb + 2 * ob, kf, sizeof(icg_tri_keyframe) * (size_t) n_kf);
+    ICG_CUDA(cudaMemcpyAsync(t.d_tri, t.h_tri, bytes, cudaMemcpyHostToDevice, h->stream));
+    ICG_CUDA(cudaEventRecord(t.stage_ev, h->stream));
+    t.stage_pending = true;
+
+    static const icg_tri_list no_list = {};
+    static const icg_tri_new no_new = {};
+    TriArgs A;
+    A.par = (const icg_tri_frame *) t.d_tri, A.koff = (const int32_t *) (t.d_tri + pb), A.roff = (const int32_t *) (t.d_tri + pb + ob);
+    A.kf = (const icg_tri_keyframe *) (t.d_tri + pb + 2 * ob);
+    A.n_in = dev_n_in, A.n_in_stride = n_in_stride;
+    A.list = n_pts ? *list : no_list, A.out = n_pts ? *out : no_new;
+    A.counts = dev_counts;
+    tri_kernel<<<n_streams, TRK_THREADS, 0, h->stream>>>(A);
+    ICG_CHECK_LAUNCH();
+    count_launch();
+    return ICG_OK;
+}
+
 }  // namespace
 
 extern "C" {
+
+int icg_klt_triangulate_dev(icg_klt *h, int n_streams, const icg_tri_frame *params, const int32_t *kf_off, const icg_tri_keyframe *kf,
+                            const int32_t *ref_off, const int32_t *dev_n_in, int n_in_stride, const icg_tri_list *list, const icg_tri_new *out,
+                            int32_t *dev_counts) {
+    return tri_launch(h, "icg_klt_triangulate_dev", n_streams, params, kf_off, kf, ref_off, dev_n_in, n_in_stride, list, out, dev_counts);
+}
+
+int icg_klt_triangulate(icg_klt *h, const icg_tri_frame *params, int n_kf, const icg_tri_keyframe *kf, int n, const icg_tri_list *list,
+                        const icg_tri_new *out, int32_t *counts) {
+    const char *who = "icg_klt_triangulate";
+    if (!h || !params || n_kf < 0 || (n_kf > 0 && !kf) || n < 0 || !counts || (n > 0 && (!tri_list_ptrs(list) || !tri_new_ptrs(out)))) {
+        set_error("%s: bad arguments", who);
+        return ICG_EINVAL;
+    }
+    if (n > h->max_pts) {
+        set_error("%s: %d points exceed max_points=%d of the handle", who, n, h->max_pts);
+        return ICG_EINVAL;
+    }
+    ICG_CUDA(cudaSetDevice(h->device));
+    int rc = track_reserve(h, 1);
+    if (rc != ICG_OK) return rc;
+    TrackScratch &t = *h->track;
+    // device copies, max_points entries each: list 60 bytes / point, out 108, + the 5 counts
+    const size_t P = h->max_pts;
+    if (!t.d_tri_host && cudaMalloc(&t.d_tri_host, P * 168 + 32) != cudaSuccess) {
+        t.d_tri_host = nullptr;
+        set_error("%s: scratch allocation failed", who);
+        return ICG_ENOMEM;
+    }
+    uint8_t *q = t.d_tri_host;
+    auto take = [&](size_t bytes) {
+        uint8_t *p = q;
+        q += bytes;
+        return p;
+    };
+    icg_tri_list dl;
+    icg_tri_new dn;
+    dl.ref_frame_id_out = (int64_t *) take(8 * P), dl.velocity_ref_out = (double *) take(16 * P), dl.velocity = (const double *) take(16 * P);
+    dn.pw = (double *) take(24 * P), dn.depth = (double *) take(8 * P), dn.velocity_cur = (double *) take(16 * P), dn.velocity_ref = (double *) take(16 * P);
+    dn.ref_frame_id = (int64_t *) take(8 * P);
+    dl.ref_out_xy = (float *) take(8 * P), dl.cur_xy = (float *) take(8 * P);
+    dn.ref_undis_xy = (float *) take(8 * P), dn.ref_xy = (float *) take(8 * P), dn.cur_undis_xy = (float *) take(8 * P), dn.cur_xy = (float *) take(8 * P);
+    dl.src = (int32_t *) take(4 * P), dn.src = (int32_t *) take(4 * P);
+    int32_t *d_cnt = (int32_t *) take(32);
+    auto h2d = [&](const void *dst, const void *src, size_t bytes) -> int {
+        if (bytes) ICG_CUDA(cudaMemcpyAsync((void *) dst, src, bytes, cudaMemcpyHostToDevice, h->stream));
+        return ICG_OK;
+    };
+    auto d2h = [&](void *dst, const void *src, size_t bytes) -> int {
+        if (bytes) ICG_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, h->stream));
+        return ICG_OK;
+    };
+    const size_t N = n;
+    if (N && ((rc = h2d(dl.ref_out_xy, list->ref_out_xy, 8 * N)) || (rc = h2d(dl.ref_frame_id_out, list->ref_frame_id_out, 8 * N)) ||
+              (rc = h2d(dl.cur_xy, list->cur_xy, 8 * N)) || (rc = h2d(dl.velocity_ref_out, list->velocity_ref_out, 16 * N)) ||
+              (rc = h2d(dl.velocity, list->velocity, 16 * N))))
+        return rc;
+    const int32_t koff[2] = {0, n_kf}, roff[2] = {0, n};
+    rc = tri_launch(h, who, 1, params, koff, kf, roff, nullptr, 1, &dl, &dn, d_cnt);
+    if (rc != ICG_OK) return rc;
+    if ((rc = d2h(counts, d_cnt, 20))) return rc;
+    ICG_CUDA(cudaStreamSynchronize(h->stream));
+    const size_t K = counts[0] > 0 ? counts[0] : 0, M = counts[0] >= 0 ? counts[1] : 0;
+    if (K && ((rc = d2h(list->ref_out_xy, dl.ref_out_xy, 8 * K)) || (rc = d2h(list->ref_frame_id_out, dl.ref_frame_id_out, 8 * K)) ||
+              (rc = d2h(list->cur_xy, dl.cur_xy, 8 * K)) || (rc = d2h(list->velocity_ref_out, dl.velocity_ref_out, 16 * K)) ||
+              (rc = d2h(list->src, dl.src, 4 * K))))
+        return rc;
+    if (M && ((rc = d2h(out->pw, dn.pw, 24 * M)) || (rc = d2h(out->depth, dn.depth, 8 * M)) || (rc = d2h(out->ref_undis_xy, dn.ref_undis_xy, 8 * M)) ||
+              (rc = d2h(out->ref_xy, dn.ref_xy, 8 * M)) || (rc = d2h(out->cur_undis_xy, dn.cur_undis_xy, 8 * M)) ||
+              (rc = d2h(out->cur_xy, dn.cur_xy, 8 * M)) || (rc = d2h(out->velocity_cur, dn.velocity_cur, 16 * M)) ||
+              (rc = d2h(out->velocity_ref, dn.velocity_ref, 16 * M)) || (rc = d2h(out->ref_frame_id, dn.ref_frame_id, 8 * M)) ||
+              (rc = d2h(out->src, dn.src, 4 * M))))
+        return rc;
+    ICG_CUDA(cudaStreamSynchronize(h->stream));
+    return ICG_OK;
+}
+
 
 int icg_klt_track_frames_dev(icg_klt *h, int n_streams, const icg_track_frame *params, const int32_t *map_off, const icg_track_map *map,
                              const int32_t *ref_off, const icg_track_ref *ref, int32_t *dev_n_out, double *dev_parallax, int32_t *dev_parallax_n) {

@@ -151,6 +151,59 @@ public:
         return k > 0;
     }
 
+    // One new map point of Tracking::triangulation (IG/tracking/tracking.cc:761-784): what MapPoint::createMapPoint and the two
+    // Feature::createFeature calls take.  depth already carries MapPoint's clamp (mappoint.cc:39-42); src = the point's index in the input list.
+    struct NewMapPoint {
+        double pw[3], depth;
+        Point2f ref_undis, ref, cur_undis, cur;
+        double velocity_cur[2], velocity_ref[2];
+        int64_t ref_frame_id;
+        int32_t src;
+    };
+
+    // Tracking::triangulation (IG/tracking/tracking.cc:690-798), one call (icg_klt_triangulate).  frames: every frame pts2d_ref_frame_ can
+    // name with id <= frame_ref_->id(), with its pose and map_->isKeyFrameInMap (at most 64).  pts2d_ref, ref_frame_id (pts2d_ref_frame_[k]->id()),
+    // pts2d_cur and velocity_ref (2 doubles per point) are reduced in place as :788-791 reduces them; pts2d_new becomes pts2d_cur (:793);
+    // src = the input index of every kept point (reduce pts2d_ref_frame_ with it).  velocity_cur (2 doubles per point) is read only.  points
+    // receives the new map points in creation order: create the MapPoint / Feature objects in this order.  counts (may be NULL): kept,
+    // succeeded, outlier, reset, outtime (:795).  Returns the reference's return value.
+    bool triangulation(const icg_tri_frame &p, const std::vector<icg_tri_keyframe> &frames, std::vector<Point2f> &pts2d_ref, std::vector<int64_t> &ref_frame_id,
+                       std::vector<Point2f> &pts2d_cur, std::vector<double> &velocity_ref, const std::vector<double> &velocity_cur, std::vector<Point2f> &pts2d_new,
+                       std::vector<int32_t> &src, std::vector<NewMapPoint> &points, int32_t *counts = nullptr) {
+        const int n = (int) pts2d_cur.size();
+        const size_t N = n > 0 ? n : 1;
+        src.resize(N);
+        std::vector<double> pw(3 * N), depth(N), vcur(2 * N), vref(2 * N);
+        std::vector<Point2f> ru(N), rp(N), cu(N), cp(N);
+        std::vector<int64_t> fid(N);
+        std::vector<int32_t> nsrc(N);
+        icg_tri_list l{reinterpret_cast<float *>(pts2d_ref.data()), ref_frame_id.data(), reinterpret_cast<float *>(pts2d_cur.data()), velocity_ref.data(),
+                       velocity_cur.data(), src.data()};
+        icg_tri_new o{pw.data(), depth.data(), reinterpret_cast<float *>(ru.data()), reinterpret_cast<float *>(rp.data()), reinterpret_cast<float *>(cu.data()),
+                      reinterpret_cast<float *>(cp.data()), vcur.data(), vref.data(), fid.data(), nsrc.data()};
+        int32_t c[5];
+        check(icg_klt_triangulate(h_, &p, (int) frames.size(), frames.data(), n, &l, &o, c), "icg_klt_triangulate");
+        if (c[0] == -2) throw std::runtime_error("KltContext::triangulation: a reference frame of the list is missing from `frames`");
+        if (counts)
+            for (int k = 0; k < 5; k++) counts[k] = c[k];
+        points.clear();
+        src.resize(c[0] >= 0 ? c[0] : 0);
+        if (c[0] < 0) return false;  // :692-694 (or triangulate == 0): nothing changes
+        const int k = c[0];
+        pts2d_ref.resize(k), ref_frame_id.resize(k), pts2d_cur.resize(k), velocity_ref.resize(2 * (size_t) k);
+        pts2d_new = pts2d_cur;
+        for (int m = 0; m < c[1]; m++) {
+            NewMapPoint q;
+            for (int d = 0; d < 3; d++) q.pw[d] = pw[3 * (size_t) m + d];
+            q.depth = depth[m], q.ref_undis = ru[m], q.ref = rp[m], q.cur_undis = cu[m], q.cur = cp[m];
+            q.velocity_cur[0] = vcur[2 * (size_t) m], q.velocity_cur[1] = vcur[2 * (size_t) m + 1];
+            q.velocity_ref[0] = vref[2 * (size_t) m], q.velocity_ref[1] = vref[2 * (size_t) m + 1];
+            q.ref_frame_id = fid[m], q.src = nsrc[m];
+            points.push_back(q);
+        }
+        return true;
+    }
+
 private:
     void upload(const Mat &pre, const Mat &cur, icg_track_frame &p) {
         check(icg_klt_upload(h_, 0, mat_data(pre), mat_stride(pre)), "icg_klt_upload");

@@ -50,6 +50,58 @@ _SPEC = {"prev_xy": (np.float32, 2), "prev_undis_xy": (np.float32, 2), "pw": (np
          "velocity_ref_out": (np.float64, 2), "src": (np.int32, 1)}
 
 
+class TriFrameStruct(C.Structure):
+    """ctypes image of `icg_tri_frame` (per-stream parameters of Tracking::triangulation)."""
+    _fields_ = [("camera", CameraStruct), ("R_cur", C.c_double * 9), ("t_cur", C.c_double * 3), ("cur_id", C.c_int64), ("ref_id", C.c_int64),
+                ("window_normal", C.c_int32), ("triangulate", C.c_int32), ("reprojection_error_std", C.c_double)]
+
+
+class TriKeyframeStruct(C.Structure):
+    """ctypes image of `icg_tri_keyframe` (a frame the reference list can name)."""
+    _fields_ = [("id", C.c_int64), ("R", C.c_double * 9), ("t", C.c_double * 3), ("in_map", C.c_int32)]
+
+
+TRI_LIST = ("ref_out_xy", "ref_frame_id_out", "cur_xy", "velocity_ref_out", "velocity", "src")
+TRI_NEW = ("pw", "depth", "ref_undis_xy", "ref_xy", "cur_undis_xy", "cur_xy", "velocity_cur", "velocity_ref", "ref_frame_id", "src")
+TRI_COUNTS = ("kept", "succeeded", "outlier", "reset", "outtime")
+
+
+class TriListStruct(C.Structure):
+    """ctypes image of `icg_tri_list` (all pointers)."""
+    _fields_ = [(k, C.c_void_p) for k in TRI_LIST]
+
+
+class TriNewStruct(C.Structure):
+    """ctypes image of `icg_tri_new` (all pointers)."""
+    _fields_ = [(k, C.c_void_p) for k in TRI_NEW]
+
+
+# numpy (dtype, columns) of the new map points' arrays (the list arrays are in _SPEC)
+_TRI_NEW_SPEC = {"pw": (np.float64, 3), "depth": (np.float64, 1), "ref_undis_xy": (np.float32, 2), "ref_xy": (np.float32, 2),
+                 "cur_undis_xy": (np.float32, 2), "cur_xy": (np.float32, 2), "velocity_cur": (np.float64, 2), "velocity_ref": (np.float64, 2),
+                 "ref_frame_id": (np.int64, 1), "src": (np.int32, 1)}
+
+
+def tri_frame_params(intrinsic, distortion, R_cur, t_cur, cur_id, ref_id, window_normal, reprojection_error_std, triangulate=True) -> TriFrameStruct:
+    """icg_tri_frame from Camera::createCamera's lists and frame_cur_'s camera-to-world pose"""
+    i, d = list(map(float, intrinsic)), list(map(float, distortion))
+    cam = CameraStruct(i[0], i[1], i[2], i[3], i[4] if len(i) == 5 else 0.0, d[0], d[1], d[2], d[3], d[4] if len(d) == 5 else 0.0)
+    m = lambda a, n: (C.c_double * n)(*np.asarray(a, np.float64).reshape(n).tolist())  # noqa: E731
+    return TriFrameStruct(cam, m(R_cur, 9), m(t_cur, 3), int(cur_id), int(ref_id), int(bool(window_normal)), int(bool(triangulate)),
+                          float(reprojection_error_std))
+
+
+def tri_keyframes(frames) -> C.Array:
+    """icg_tri_keyframe array from an iterable of (id, R (3 x 3 camera-to-world), t (3), in_map)"""
+    frames = list(frames)
+    arr = (TriKeyframeStruct * max(len(frames), 1))()
+    for e, (fid, R, t, in_map) in enumerate(frames):
+        arr[e].id, arr[e].in_map = int(fid), int(bool(in_map))
+        arr[e].R[:] = np.asarray(R, np.float64).reshape(9).tolist()
+        arr[e].t[:] = np.asarray(t, np.float64).reshape(3).tolist()
+    return arr
+
+
 def track_frame_params(prev_slot, cur_slot, intrinsic, distortion, R_pre, R_cur, R_ref, t_cur, dt, ref_id, fm_threshold) -> TrackFrameStruct:
     """icg_track_frame from Camera::createCamera's intrinsic / distortion lists and camera-to-world attitudes (Pose::R, 3 x 3)."""
     i, d = list(map(float, intrinsic)), list(map(float, distortion))
@@ -194,6 +246,50 @@ class KltTracker:
         check(lib().icg_klt_track_frames_dev(self._h, B, par, _ptr(mo), C.byref(sm) if sm is not None else None, _ptr(ro),
                                              C.byref(sr) if sr is not None else None, vp(dev_n_out), vp(dev_parallax), vp(dev_parallax_n)),
               "icg_klt_track_frames_dev")
+
+    # ------------------------------------------------------------------ Tracking::triangulation (tracking.cc:690-798)
+    def triangulate(self, params: TriFrameStruct, keyframes, lists):
+        """One stream from host arrays (icg_klt_triangulate, synchronous).  keyframes: iterable of (id, R, t, in_map); lists: dict with
+        ref_out_xy, cur_xy (n, 2) float32, ref_frame_id_out (n,) int64, velocity_ref_out, velocity (n, 2) float64 (None or {} = empty).
+        Returns (list_out, new, counts): list_out = the compacted ref_out_xy / ref_frame_id_out / cur_xy / velocity_ref_out / src cut to the
+        kept count, new = the new map points (TRI_NEW) cut to the succeeded count, counts = int32[5] (TRI_COUNTS)."""
+        kfs = list(keyframes)
+        kf = tri_keyframes(kfs)
+        lists = lists or {}
+        n = len(lists["cur_xy"]) if "cur_xy" in lists else 0
+        la = {}
+        for k in TRI_LIST:
+            dt, c = _SPEC[k]
+            la[k] = np.ascontiguousarray(np.asarray(lists[k], dt).reshape(n, c)).copy() if (n and k != "src") else np.zeros((max(n, 1), c), dt)
+        na = {k: np.zeros((max(n, 1), c), dt) for k, (dt, c) in _TRI_NEW_SPEC.items()}
+        sl = TriListStruct(*[la[k].ctypes.data for k in TRI_LIST])
+        sn = TriNewStruct(*[na[k].ctypes.data for k in TRI_NEW])
+        counts = np.zeros(5, np.int32)
+        check(lib().icg_klt_triangulate(self._h, C.byref(params), len(kfs), kf, n, C.byref(sl), C.byref(sn), _ptr(counts)), "icg_klt_triangulate")
+        k_out, m_out = max(int(counts[0]), 0), max(int(counts[1]), 0) if counts[0] >= 0 else 0
+        flat = lambda a, c: a.reshape(-1) if c == 1 else a  # noqa: E731
+        lo = {k: flat(la[k][:k_out], _SPEC[k][1]) for k in TRI_LIST if k != "velocity"}
+        no = {k: flat(na[k][:m_out], _TRI_NEW_SPEC[k][1]) for k in TRI_NEW}
+        return lo, no, counts
+
+    def triangulate_dev(self, params, kf_off, keyframes, ref_off, dev_n_in, n_in_stride, list_ptrs, new_ptrs, dev_counts):
+        """B streams in one asynchronous call (icg_klt_triangulate_dev).  params: sequence of TriFrameStruct; kf_off: host sequence of B + 1;
+        keyframes: iterable of (id, R, t, in_map) for all streams in kf_off order (or a prebuilt tri_keyframes array; params likewise may be a
+        prebuilt TriFrameStruct array); ref_off: host sequence of B + 1; dev_n_in: device address of
+        the live counts (dev_n_in[s * n_in_stride]) or 0 for the segment lengths; list_ptrs / new_ptrs: dicts name -> device address (TRI_LIST /
+        TRI_NEW; None when no stream has points); dev_counts: device address of 5 B int32."""
+        B = len(params)
+        par = params if isinstance(params, C.Array) else (TriFrameStruct * B)(*params)
+        ko = np.ascontiguousarray(np.asarray(kf_off, np.int32).reshape(-1))
+        ro = np.ascontiguousarray(np.asarray(ref_off, np.int32).reshape(-1))
+        if ko.size != B + 1 or ro.size != B + 1:
+            raise ValueError("kf_off and ref_off need len(params) + 1 entries")
+        kf = keyframes if isinstance(keyframes, C.Array) else tri_keyframes(list(keyframes))
+        sl = TriListStruct(*[list_ptrs.get(k) for k in TRI_LIST]) if list_ptrs else None
+        sn = TriNewStruct(*[new_ptrs.get(k) for k in TRI_NEW]) if new_ptrs else None
+        check(lib().icg_klt_triangulate_dev(self._h, B, par, _ptr(ko), kf if ko[-1] else None, _ptr(ro), vp(dev_n_in) if dev_n_in else None,
+                                            int(n_in_stride), C.byref(sl) if sl is not None else None, C.byref(sn) if sn is not None else None,
+                                            vp(dev_counts)), "icg_klt_triangulate_dev")
 
     def sync(self):
         check(lib().icg_klt_sync(self._h), "icg_klt_sync")

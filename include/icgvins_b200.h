@@ -239,6 +239,73 @@ int icg_klt_track_frames_dev(icg_klt *h, int n_streams, const icg_track_frame *p
 int icg_klt_track_frame(icg_klt *h, const icg_track_frame *params, int n_map, const icg_track_map *map, int n_ref, const icg_track_ref *ref,
                         int32_t *n_out, double *parallax, int32_t *parallax_n);
 
+/* ----- Tracking::triangulation (IG/tracking/tracking.cc:690-798) on the KLT handle (csrc/track.cu) ----- */
+/* Per-stream parameters.  Attitudes are camera-to-world rotations (Pose::R), row-major, as in icg_track_frame. */
+typedef struct icg_tri_frame {
+    icg_camera camera;
+    double R_cur[9], t_cur[3];     /* frame_cur_->pose() (:699) */
+    int64_t cur_id, ref_id;        /* frame_cur_->id(), frame_ref_->id() (:723) */
+    int32_t window_normal;         /* map_->isWindowNormal() (:733) */
+    int32_t triangulate;           /* the host's keyframe decision (:215-217); 0: the stream is left untouched, kept = -1 */
+    double reprojection_error_std; /* reprojection_error_std_ (isGoodToTrack, :813-829) */
+} icg_tri_frame;
+/* A frame a point of the stream can name as pts2d_ref_frame_[k]: its id, pose (Pose::R row-major, Pose::t) and whether
+ * map_->isKeyFrameInMap(frame) holds (:733). */
+typedef struct icg_tri_keyframe {
+    int64_t id;
+    double R[9], t[3];
+    int32_t in_map;
+} icg_tri_keyframe;
+/* The reference list as icg_klt_track_frames_dev leaves it (the same pointers can be passed).  ref_out_xy = pts2d_ref_, ref_frame_id_out =
+ * pts2d_ref_frame_[k]->id(), cur_xy = pts2d_cur_, velocity_ref_out = velocity_ref_ (2 doubles): compacted IN PLACE in list order by the
+ * status of :788-791 (reduceVector).  velocity = velocity_cur_ (2 doubles), read only (:791 does not reduce it).  src: the input index of
+ * every kept point. */
+typedef struct icg_tri_list {
+    float *ref_out_xy;
+    int64_t *ref_frame_id_out;
+    float *cur_xy;
+    double *velocity_ref_out;
+    const double *velocity;
+    int32_t *src;
+} icg_tri_list;
+/* The new map points in creation order (MapPoint ids are issued in this order, mappoint.cc:45-49; :761-784): pw (3 doubles), depth =
+ * world2cam(pw, frame_ref->pose()).z with MapPoint's clamp (outside [1, 200] -> 10, mappoint.cc:39-42), the reference feature
+ * (ref_undis_xy = undistort(pts2d_ref_[k]), ref_xy = pts2d_ref_[k], velocity_ref = velocity_ref_[k] (2 doubles), ref_frame_id), the current
+ * feature (cur_undis_xy, cur_xy = pts2d_cur_[k], velocity_cur = velocity_cur_[k] (2 doubles)) and src = the point's input index. */
+typedef struct icg_tri_new {
+    double *pw, *depth;
+    float *ref_undis_xy, *ref_xy, *cur_undis_xy, *cur_xy;
+    double *velocity_cur, *velocity_ref;
+    int64_t *ref_frame_id;
+    int32_t *src;
+} icg_tri_new;
+/*
+ * Tracking::triangulation for n_streams streams in one asynchronous call on the KLT handle's stream (stream-ordered after
+ * icg_klt_track_frames_dev).  Per point k, in list order:
+ *   reset      ref_frame_id > ref_id: ref_frame_id := cur_id, ref_xy := cur_xy, kept; velocity_ref untouched (:723-730)
+ *   outtime    window_normal && !in_map(ref frame): dropped (:733-737)
+ *   parallax   keyPointParallax(undistort(ref), undistort(cur), ref frame pose, pose_cur) < 10 (TRACK_MIN_PARALLAX, tracking.h:114): kept (:740-745)
+ *   triangulate pw = triangulatePoint(Tcw(ref frame), Tcw(pose_cur), pixel2cam(ref_undis), pixel2cam(cur_undis)), Tcw = [R^T | -R^T t] (:747-753, :851-859)
+ *   outlier    unless isGoodToTrack(ref_undis, pose_ref, pw, 1, 3) && isGoodToTrack(cur_undis, pose_cur, pw, 1, 3): 1 < z < 600 and
+ *              |world2pixel(pw) - pp| <= reprojection_error_std, the difference taken in float (camera.cc:153-157): dropped (:756-760, :813-829)
+ *   succeeded  dropped from the list, written to `out` as a new map point (:761-784)
+ * kf_off (n_streams + 1, starting at 0) and kf: HOST CSR of each stream's frames, at most 64 per stream with distinct ids (ICG_EINVAL
+ * otherwise).  Every ref_frame_id <= ref_id in a stream's live list must be in its table (frames that left the map with in_map = 0),
+ * otherwise the stream reports -2 and nothing of it is written.  ref_off (HOST, n_streams + 1): stream s owns list entries ref_off[s] ..
+ * ref_off[s + 1] and writes its new points from out index ref_off[s].  The live count of stream s is read ON THE DEVICE from
+ * dev_n_in[s * n_in_stride] (icg_klt_track_frames_dev's dev_n_out + 1 with stride 2 chains both calls without a host sync); dev_n_in NULL:
+ * the segment length; a count outside [0, segment] gives -2.  dev_counts (DEVICE, 5 int32 per stream): kept (-1: the reference's
+ * `return false` for an empty list, and streams with triangulate == 0; -2: see above), succeeded, outlier, reset, outtime (:795).
+ * Parameters, offsets and tables are staged through the handle's pinned buffer; list and out pointers are DEVICE pointers.
+ */
+int icg_klt_triangulate_dev(icg_klt *h, int n_streams, const icg_tri_frame *params, const int32_t *kf_off, const icg_tri_keyframe *kf,
+                            const int32_t *ref_off, const int32_t *dev_n_in, int n_in_stride, const icg_tri_list *list, const icg_tri_new *out,
+                            int32_t *dev_counts);
+/* The same for one stream from HOST buffers (n points, n_kf table entries; out needs room for n points; counts: 5 int32, host);
+ * synchronous.  A thin wrapper over the launch of icg_klt_triangulate_dev.  n <= the handle's max_points. */
+int icg_klt_triangulate(icg_klt *h, const icg_tri_frame *params, int n_kf, const icg_tri_keyframe *kf, int n, const icg_tri_list *list,
+                        const icg_tri_new *out, int32_t *counts);
+
 /* ----- pre-pass of path A: cv::CLAHE (IG/tracking/tracking.cc:62 createCLAHE(3.0, Size(21, 21)); :141 clahe_->apply(img, img)) ----- */
 typedef struct icg_clahe icg_clahe;
 int icg_clahe_create(icg_clahe **h, int width, int height, int tiles_x, int tiles_y, double clip_limit, int device, void *stream);
