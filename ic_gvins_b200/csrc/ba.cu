@@ -22,7 +22,8 @@
 //                marginalization factors -> H_c, g_c
 //   solve      : one CTA / window -> Jacobi scaling, LM diagonal, S = s(H - Schur)s + D^2, packed Cholesky in shared memory
 //                (panel updates on DMMA), triangular solves, landmark back-substitution, model cost change, candidate x (+) delta
-//   cost       : candidate cost (all factors, residuals only);   accept : Ceres step acceptance + radius update
+//   single GPU : lin_vis + lin_cam at the candidate, into the window's second linearisation buffer (its costs are the candidate cost)
+//   cost       : candidate cost (all factors, residuals only) of the split / NCCL pipelines;   accept : Ceres step acceptance + radius update
 //   ba_marg.cuh: sliding-window marginalization (MarginalizationInfo) on the same device-resident linearisation
 #include <cooperative_groups.h>
 #include <dlfcn.h>
@@ -63,8 +64,10 @@ struct WinDims {  // per-window actual sizes
 };
 
 struct LmState {
-    double radius, decrease_factor, x_cost, x_norm, cand_cost, model_cost_change, step_norm, gmax, initial_cost, cost_cam;
+    double radius, decrease_factor, x_cost, x_norm, cand_cost, model_cost_change, step_norm, gmax, initial_cost;
+    double cost_cam[2];  // camera-only cost of each linearisation buffer
     int iter, n_success, n_invalid, done, need_lin, last_success, first, step_valid, fresh_lin, max_iter, chol_ok;
+    int lin_buf;  // linearisation buffer that holds the linearisation at x (the other one receives the candidate's)
 };
 
 // Exchange state of the split pipeline (ba_split.cuh): one buffer per rank holding the inbox of reduction operands, the step broadcast, the
@@ -102,11 +105,15 @@ struct BaDev {  // device pointers (flat, capacity-strided by window)
     int *part_off, *pair_ro, *npairs;  // (reference node, observing node) pairs: CSR offsets of their Gram partials (in run order), (ref << 8 | obs), count
     double *gpart;       // [NW][GQ][210] Gram partial of one (run, observing node): packed upper 20x20
     int *vis_cnt;        // [NW][K] lin_vis runs of the reference node arrived (the last one resets it)
-    double *Mp;                                    // per-pair 20x20 Gram matrices (upper, 210 entries)
-    double *AW;            // Schur SYRK input
-    double *costf;         // per-factor cost
-    double *hl, *gl, *scale_l, *scale_c;
-    double *Hc, *gc;
+    // Linearisation buffers: everything a linearisation writes and a later iteration reads comes in two copies, selected per window by
+    // LmState::lin_buf through the lin_* helpers below.  The single-GPU pipeline linearises the candidate into the copy the window is not
+    // using and flips lin_buf when ba_accept takes the step; the split and NCCL pipelines never flip it and have copy 0 only.
+    double *Mp[2];         // per-pair 20x20 Gram matrices (upper, 210 entries)
+    double *AW[2];         // Schur SYRK input
+    double *costf[2];      // per-factor cost
+    double *hl[2], *gl[2];
+    double *Hc[2], *gc[2];
+    double *scale_l, *scale_c;
     double *Hs;  // H_c + vision Gram - Schur term (lower triangle, ld NS): the operand ba_solve scales and factorises
     double *visv;  // [NW][3 NCV] diag H_vis | g_vis | W phi g_l (window NCV): ba_solve's other operands (single GPU)
     double *imu_blob, *imu_U;
@@ -124,6 +131,15 @@ struct BaDev {  // device pointers (flat, capacity-strided by window)
     double *Sglobal;    // fallback Cholesky workspace when the packed system does not fit shared memory
     unsigned long long *clk;  // ICG_BA_PROFILE: SM-clock totals of ba_solve's phases for window 0 (nullptr otherwise)
 };
+
+// window w's part of linearisation buffer b
+__device__ __forceinline__ double *lin_Mp(const BaCaps &C, const BaDev &D, int b, int w) { return D.Mp[b] + (size_t) w * C.K * (C.K - 1) * 210; }
+__device__ __forceinline__ double *lin_AW(const BaCaps &C, const BaDev &D, int b, int w) { return D.AW[b] + (size_t) w * C.LP * C.NCA; }
+__device__ __forceinline__ double *lin_costf(const BaCaps &C, const BaDev &D, int b, int w) { return D.costf[b] + (size_t) w * C.F; }
+__device__ __forceinline__ double *lin_hl(const BaCaps &C, const BaDev &D, int b, int w) { return D.hl[b] + (size_t) w * C.L; }
+__device__ __forceinline__ double *lin_gl(const BaCaps &C, const BaDev &D, int b, int w) { return D.gl[b] + (size_t) w * C.L; }
+__device__ __forceinline__ double *lin_Hc(const BaCaps &C, const BaDev &D, int b, int w) { return D.Hc[b] + (size_t) w * C.NS * C.NS; }
+__device__ __forceinline__ double *lin_gc(const BaCaps &C, const BaDev &D, int b, int w) { return D.gc[b] + (size_t) w * C.NS; }
 
 __device__ __forceinline__ int col_pose(int k) { return 6 * k; }
 __device__ __forceinline__ int col_ext(int K) { return 6 * K; }
@@ -155,16 +171,20 @@ __device__ __forceinline__ void dmma884(double &c0, double &c1, double a, double
 //  phase 4: the last run of the reference node to arrive (arrival counter) sums the node's partials of every pair in run order -> Mp.
 //           No floating-point atomics: the result does not depend on which CTA arrives last, nor on the other windows of the batch.
 // The Jacobians never leave the SM: per factor only the cost is stored.
+// at_cand = 0: at x (windows that need a linearisation) into buffer lin_buf; at_cand = 1: at the candidate of a valid step into buffer
+// 1 - lin_buf (its per-factor costs are the candidate cost ba_accept tests).
 constexpr int LV_LD = 45;  // shared-memory record row: 44 doubles padded to an odd length (conflict-free)
 constexpr size_t LV_SMEM = sizeof(double) * (128 * LV_LD + (BA_MAX_NODES + 1) * NODE_FRAME_LD);  // records + node frames (49.5 KB: dynamic, opted in at create)
-__global__ void __launch_bounds__(128, 4) ba_lin_vis(BaCaps C, BaDev D) {
+__global__ void __launch_bounds__(128, 4) ba_lin_vis(BaCaps C, BaDev D, int at_cand) {
     extern __shared__ double lv_sm[];
     __shared__ int s_ord[128], s_gbeg[BA_MAX_NODES], s_gend[BA_MAX_NODES], s_last, s_p0, s_np;
     double (*s_rec)[LV_LD] = (double (*)[LV_LD]) lv_sm;
     double (*s_frame)[NODE_FRAME_LD] = (double (*)[NODE_FRAME_LD]) (lv_sm + 128 * LV_LD);
     const int w = blockIdx.y;
     const LmState &st = D.st[w];
-    if (st.done || !st.need_lin) return;
+    if (st.done || !(at_cand ? st.step_valid : st.need_lin)) return;
+    const int b = at_cand ? 1 - st.lin_buf : st.lin_buf;
+    const double *pose = at_cand ? D.pose_c : D.pose, *xext = at_cand ? D.ext_c : D.ext, *rho = at_cand ? D.rho_c : D.rho;
     const int *vb = D.vb_lm0 + (size_t) w * C.NVB;
     if ((int) blockIdx.x >= vb[C.NVB - 1]) return;  // last entry = number of runs of this window
     const WinDims dm = D.dims[w];
@@ -173,7 +193,7 @@ __global__ void __launch_bounds__(128, 4) ba_lin_vis(BaCaps C, BaDev D) {
     const int pA = vb[blockIdx.x], pB = vb[blockIdx.x + 1];  // landmark positions of the run
     const int s0 = off[pA], nslot = off[pB] - s0;
     // ---- phase 0: the window's K + 1 node frames (rotation matrix | position of every pose and of the extrinsic), once per CTA
-    if (tid <= dm.K) node_frame(tid < dm.K ? D.pose + ((size_t) w * C.K + tid) * 7 : D.ext + (size_t) w * 8, s_frame[tid]);
+    if (tid <= dm.K) node_frame(tid < dm.K ? pose + ((size_t) w * C.K + tid) * 7 : xext + (size_t) w * 8, s_frame[tid]);
     if (tid < BA_MAX_NODES) s_gbeg[tid] = s_gend[tid] = 0;
     if (tid == 0) s_np = 0;
     __syncthreads();
@@ -184,8 +204,8 @@ __global__ void __launch_bounds__(128, 4) ba_lin_vis(BaCaps C, BaDev D) {
         const int4 meta = ((const int4 *) D.f_meta_s)[(size_t) w * C.F + q];  // (landmark, reference node, observing node, factor id)
         const int i = meta.y, j = meta.z, f = meta.w;
         if (D.f_active[(size_t) w * C.F + f] != 0) {
-            const double *ext = D.ext + (size_t) w * 8;
-            reproj_eval_frames(s_frame[i], s_frame[j], s_frame[dm.K], D.rho[(size_t) w * C.L + meta.x], ext[7],
+            const double *ext = xext + (size_t) w * 8;
+            reproj_eval_frames(s_frame[i], s_frame[j], s_frame[dm.K], rho[(size_t) w * C.L + meta.x], ext[7],
                                D.f_const_s + ((size_t) w * C.F + q) * 14, dm.reproj_sinv, true, r, Ji, Jj, Je, Jr, Jt);
             if (dm.ext_const)
                 for (int k = 0; k < 12; k++) Je[k] = 0;
@@ -203,7 +223,7 @@ __global__ void __launch_bounds__(128, 4) ba_lin_vis(BaCaps C, BaDev D) {
             for (int k = 0; k < 12; k++) Ji[k] = Jj[k] = Je[k] = 0;
             Jr[0] = Jr[1] = Jt[0] = Jt[1] = r[0] = r[1] = 0;
         }
-        D.costf[(size_t) w * C.F + f] = cost;
+        lin_costf(C, D, b, w)[f] = cost;
         double *sr = s_rec[tid];
 #pragma unroll
         for (int k = 0; k < 12; k++) sr[k] = Ji[k], sr[12 + k] = Jj[k], sr[24 + k] = Je[k];
@@ -279,7 +299,7 @@ __global__ void __launch_bounds__(128, 4) ba_lin_vis(BaCaps C, BaDev D) {
     }
     for (int pl = pA + grp; pl < pB; pl += 16) {
         const int l = perm[pl], f0 = off[pl] - s0, nf = off[pl + 1] - off[pl];
-        double *row = D.AW + ((size_t) w * C.LP + l) * C.NCA;
+        double *row = lin_AW(C, D, b, w) + (size_t) l * C.NCA;
         for (int c = sl; c < NCA; c += 8) row[c] = 0.0;
         __syncwarp(0xffu << (tid & 24));  // the landmark's eight lanes: zeros land before the values
         double acc[3] = {0, 0, 0};
@@ -312,9 +332,9 @@ __global__ void __launch_bounds__(128, 4) ba_lin_vis(BaCaps C, BaDev D) {
             }
             if (c == 19) {
                 row[NCV] = acc[t];
-                D.gl[(size_t) w * C.L + l] = acc[t];
+                lin_gl(C, D, b, w)[l] = acc[t];
             } else if (c == 20) {
-                D.hl[(size_t) w * C.L + l] = acc[t];
+                lin_hl(C, D, b, w)[l] = acc[t];
                 if (st.first) D.scale_l[(size_t) w * C.L + l] = 1.0 / (1.0 + sqrt(acc[t]));  // jacobi_scaling, once (iteration 0)
             }
         }
@@ -337,7 +357,7 @@ __global__ void __launch_bounds__(128, 4) ba_lin_vis(BaCaps C, BaDev D) {
         }
     __syncthreads();
     const double *part = D.gpart + (size_t) w * C.GQ * 210;
-    double *Mp = D.Mp + (size_t) w * PM * 210;
+    double *Mp = lin_Mp(C, D, b, w);
     for (int p = s_p0 + warp; p < s_p0 + s_np; p += 4) {  // warp / pair: the 7 entries of a lane in flight together
         const int k0 = poff[p], k1 = poff[p + 1];
         double acc[7];
@@ -370,9 +390,9 @@ __device__ __forceinline__ void gram2_slots(const BaCaps &C, const BaDev &D, int
     for (int p = threadIdx.x; p < P; p += blockDim.x) s_slot[(pro[p] >> 8) * K + (pro[p] & 255)] = (short) p;
     __syncthreads();
 }
-__device__ __forceinline__ double gram2_entry(const BaCaps &C, const BaDev &D, int w, int K, const short *s_slot, int A, int B) {
-    const int PM = C.K * (C.K - 1), P = D.npairs[w];
-    const double *Mp = D.Mp + (size_t) w * PM * 210;
+__device__ __forceinline__ double gram2_entry(const BaCaps &C, const BaDev &D, int buf, int w, int K, const short *s_slot, int A, int B) {
+    const int P = D.npairs[w];
+    const double *Mp = lin_Mp(C, D, buf, w);
     const int bA = A < 6 * K ? A / 6 : K, bB = B < 6 * K ? B / 6 : K;
     const int a = A - 6 * bA, b = B - 6 * bB;  // offsets inside the block (global block: 0..7 = ext 6, td, residual)
     const int ga = 12 + a, gb = 12 + b;          // local column of a global-block column
@@ -428,13 +448,13 @@ __device__ __forceinline__ int tri_idx(int A, int B, int ncv);
 //   split pipeline: [tri(H_vis - Schur) | diag H_vis | g_vis | W phi g_l] straight into the owner's inbox (P2P stores; ba_signal publishes
 //                   them, the owner's ba_reduce sums the ranks);
 //   NCCL landmark shards: [H_vis g_vis | Schur term] stored symmetric in D.red, all-reduced, then turned into Hs by ba_hsum.
-__device__ __forceinline__ void schur_store(const BaCaps &C, const BaDev &D, int w, int K, const short *s_slot, int A, int B, double cw) {
+__device__ __forceinline__ void schur_store(const BaCaps &C, const BaDev &D, int buf, int w, int K, const short *s_slot, int A, int B, double cw) {
     const int NCV = 6 * K + 7;
     const bool nccl = !D.S.split && D.world > 1;
     if (A == NCV && !nccl) return;  // the r^T r corner: only the all-reduced buffer carries it
     const size_t e = (size_t) w * C.NS * C.NS + (size_t) B * C.NS + A;
-    const double hc = !D.S.split && !nccl && B < NCV ? D.Hc[e] : 0.0;  // in flight during the gather
-    const double cj = gram2_entry(C, D, w, K, s_slot, A, B);
+    const double hc = !D.S.split && !nccl && B < NCV ? lin_Hc(C, D, buf, w)[(size_t) B * C.NS + A] : 0.0;  // in flight during the gather
+    const double cj = gram2_entry(C, D, buf, w, K, s_slot, A, B);
     if (D.S.split) {
         double *P = x_inbox(D, w % D.world, w, D.rank);
         const int TRI = NCV * (NCV + 1) / 2;
@@ -465,11 +485,12 @@ __device__ __forceinline__ void schur_store(const BaCaps &C, const BaDev &D, int
 __device__ __forceinline__ void schur_scalars(const BaCaps &C, const BaDev &D, int w, const WinDims &dm, double *s_red) {
     const int tid = threadIdx.x;
     double c = 0, q = 0, gm = 0;
-    for (int f = tid; f < dm.F; f += 256) c += D.costf[(size_t) w * C.F + f];
+    const double *costf = lin_costf(C, D, 0, w), *gl = lin_gl(C, D, 0, w);  // these pipelines use buffer 0 only
+    for (int f = tid; f < dm.F; f += 256) c += costf[f];
     for (int l = tid; l < dm.L; l += 256) {
         const double r = D.rho[(size_t) w * C.L + l];
         q += r * r;
-        gm = fmax(gm, fabs(D.gl[(size_t) w * C.L + l]));
+        gm = fmax(gm, fabs(gl[l]));
     }
     c = block_sum(c, s_red);
     q = block_sum(q, s_red);
@@ -512,7 +533,8 @@ __global__ void __cluster_dims__(BA_SPLIT_W, 1, 1) __launch_bounds__(256) ba_sch
     const int T2 = (NCA + 15) / 16, nsuper = T2 * (T2 + 1) / 2;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, kk = lane & 3;
     double *sphi = sA + (size_t) SCHUR_RCH * ld;
-    const double *A = D.AW + (size_t) w * C.LP * C.NCA;
+    const int b = st.lin_buf;
+    const double *A = lin_AW(C, D, b, w), *hl = lin_hl(C, D, b, w);
     const double radius = st.radius;
     const int nsteps = (dm.L + 3) / 4;
     const int r_beg = 4 * (int) ((long long) nsteps * split / BA_SPLIT_W), r_end = min(dm.L, 4 * (int) ((long long) nsteps * (split + 1) / BA_SPLIT_W));
@@ -568,7 +590,7 @@ __global__ void __cluster_dims__(BA_SPLIT_W, 1, 1) __launch_bounds__(256) ba_sch
                 double ph = 0;
                 if (rr < nr) {
                     const int l = r0 + rr;
-                    const double sl = D.scale_l[(size_t) w * C.L + l], hs = sl * sl * D.hl[(size_t) w * C.L + l];
+                    const double sl = D.scale_l[(size_t) w * C.L + l], hs = sl * sl * hl[l];
                     ph = sl * sl / (hs + fmin(fmax(hs, 1e-6), 1e32) / radius);
                 }
                 sphi[rr] = ph;
@@ -623,7 +645,7 @@ __global__ void __cluster_dims__(BA_SPLIT_W, 1, 1) __launch_bounds__(256) ba_sch
             int a = 0, e = SCHUR_PASS * pass + sl;
             while (e >= T2 - a) e -= T2 - a, a++;
             const int r = 16 * a + r_in, cc = 16 * (a + e) + c_in;
-            if (r <= cc && cc <= NCV) schur_store(C, D, w, dm.K, s_slot, r, cc, cw[j]);
+            if (r <= cc && cc <= NCV) schur_store(C, D, b, w, dm.K, s_slot, r, cc, cw[j]);
         }
     }
     if (split == 0 && (D.S.split || D.world > 1)) schur_scalars(C, D, w, dm, s_red);
@@ -698,7 +720,7 @@ __device__ void marg_dx(const BaCaps &C, const BaDev &D, int w, const WinDims &d
     }
 }
 
-// cost of all camera-only factors at (pose, mix, ext); optionally the linearisation (H_c, g_c).  One CTA (256 threads).
+// cost of all camera-only factors at (pose, mix, ext); optionally the linearisation (H_c, g_c of buffer b).  One CTA (256 threads).
 // smem: per IMU factor 30 + 450 doubles; GNSS 3 + 18 each; misc.
 // x += v on a global accumulator whose value the thread does not need back: one fire-and-forget reduction at the L2 (RED.ADD.F64) instead of a
 // load -> add -> store chain (a dependent L2 round trip per entry: measured 50 k of ba_lin_cam's 123 k cycles in the IMU block accumulation).
@@ -706,10 +728,10 @@ __device__ void marg_dx(const BaCaps &C, const BaDev &D, int w, const WinDims &d
 __device__ __forceinline__ void red_add(double *p, double v) { asm volatile("red.global.add.f64 [%0], %1;" ::"l"(p), "d"(v) : "memory"); }
 
 __device__ double cam_factors(const BaCaps &C, const BaDev &D, int w, const WinDims &dm, const double *pose, const double *mix, const double *ext,
-                              bool lin, double *smem) {
+                              bool lin, int b, double *smem) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
     const int K = dm.K, N = 15 * K + 7;
-    double *Hc = D.Hc + (size_t) w * C.NS * C.NS, *gc = D.gc + (size_t) w * C.NS;
+    double *Hc = lin_Hc(C, D, b, w), *gc = lin_gc(C, D, b, w);
     double *s_imu = smem;                              // n_imu * 480
     double *s_gnss = s_imu + (size_t) C.K * 480;       // G * 24 : r[3] J[18] cost scale
     double *s_misc = s_gnss + (size_t) C.G * 24;       // pose prior r[6] J[36] | mix prior r[9] | marg dx[R] y[R] | costs
@@ -886,15 +908,18 @@ __device__ double cam_factors(const BaCaps &C, const BaDev &D, int w, const WinD
 }
 
 constexpr int CAM_THREADS = 320;  // 10 warps: the K - 1 = 9 IMU factors of a 10-node window are evaluated in one round (warp per factor)
-__global__ void __launch_bounds__(CAM_THREADS) ba_lin_cam(BaCaps C, BaDev D) {
+// at_cand: as ba_lin_vis
+__global__ void __launch_bounds__(CAM_THREADS) ba_lin_cam(BaCaps C, BaDev D, int at_cand) {
     extern __shared__ double smem[];
     const int w = blockIdx.x;
     LmState &st = D.st[w];
-    if (st.done || !st.need_lin) return;
+    if (st.done || !(at_cand ? st.step_valid : st.need_lin)) return;
     if (D.S.split && (w % D.world) != D.rank) return;  // split pipeline: the window's owner handles the camera-only factors
     const WinDims dm = D.dims[w];
-    double c = cam_factors(C, D, w, dm, D.pose + (size_t) w * C.K * 7, D.mix + (size_t) w * C.K * 9, D.ext + (size_t) w * 8, true, smem);
-    if (threadIdx.x == 0) st.cost_cam = c;
+    const int b = at_cand ? 1 - st.lin_buf : st.lin_buf;
+    const double *pose = at_cand ? D.pose_c : D.pose, *mix = at_cand ? D.mix_c : D.mix, *ext = at_cand ? D.ext_c : D.ext;
+    double c = cam_factors(C, D, w, dm, pose + (size_t) w * C.K * 7, mix + (size_t) w * C.K * 9, ext + (size_t) w * 8, true, b, smem);
+    if (threadIdx.x == 0) st.cost_cam[b] = c;
 }
 
 // ------------------------------------------------------------------------------------------------ reduction operands
@@ -928,7 +953,7 @@ __global__ void __launch_bounds__(256) ba_hsum(BaCaps C, BaDev D) {
     if (B < A || B >= NCV) return;
     const double *RED = D.red + (size_t) w * (2 * NN + 8);
     const double cj = RED[(size_t) B * C.NCA + A], cw = RED[NN + (size_t) B * C.NCA + A];
-    D.Hs[(size_t) w * C.NS * C.NS + (size_t) B * C.NS + A] = D.Hc[(size_t) w * C.NS * C.NS + (size_t) B * C.NS + A] + (cj - cw);
+    D.Hs[(size_t) w * C.NS * C.NS + (size_t) B * C.NS + A] = lin_Hc(C, D, 0, w)[(size_t) B * C.NS + A] + (cj - cw);
 }
 
 // ------------------------------------------------------------------------------------------------ solve (one CTA per window)
@@ -1002,7 +1027,8 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
     // packed lower triangle, N + 1 rows, ALWAYS in shared memory (systems that do not fit are driven by the split pipeline, ba_solve_cam): a
     // pointer that could also be global made every access a generic LD / ST (longer latency, long-scoreboard tracked)
     double *S = s_diag + C.NS;
-    const double *Hc = D.Hc + (size_t) w * C.NS * C.NS, *gcam = D.gc + (size_t) w * C.NS, *Hs = D.Hs + (size_t) w * C.NS * C.NS;
+    const int b = st.lin_buf;
+    const double *Hc = lin_Hc(C, D, b, w), *gcam = lin_gc(C, D, b, w), *Hs = D.Hs + (size_t) w * C.NS * C.NS;
     // Vision vectors [diag H_vis | g_vis | W phi g_l] (a < NCV).  Landmark-sharded solve: the packed, all-reduced buffer (identical on every
     // shard).  Single GPU: the vectors ba_schur_dmma's epilogue wrote.
     const bool sharded = D.world > 1;
@@ -1014,7 +1040,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
     const double camw = D.rank == 0 ? 1.0 : 0.0;       // camera-side partial sums are counted on shard 0 only
     if (tid == 0 && st.need_lin) st.need_lin = 0;      // the linearisation kernels of this iteration have run (stream order)
     double *scale_c = D.scale_c + (size_t) w * C.NS;
-    const double *hl = D.hl + (size_t) w * C.L, *gl = D.gl + (size_t) w * C.L, *scale_l = D.scale_l + (size_t) w * C.L;
+    const double *hl = lin_hl(C, D, b, w), *gl = lin_gl(C, D, b, w), *scale_l = D.scale_l + (size_t) w * C.L;
 
     // ---- after a fresh linearisation: total cost, gradient, (first time) Jacobi scaling
     for (int a = tid; a < N; a += SOLVE_THREADS) {
@@ -1036,7 +1062,8 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
             gml = D.redmax[w];
         } else {
             double cs = 0, gq = 0;
-            for (int f = tid; f < dm.F; f += SOLVE_THREADS) cs += D.costf[(size_t) w * C.F + f];
+            const double *costf = lin_costf(C, D, b, w);
+            for (int f = tid; f < dm.F; f += SOLVE_THREADS) cs += costf[f];
             for (int l = tid; l < L; l += SOLVE_THREADS) gq = fmax(gq, fabs(gl[l]));
             c = block_sum(cs, s_red);
             gml = block_max(gq, s_red);
@@ -1046,7 +1073,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
         gm = fmax(block_max(gm, s_red), gml);
         gmax_now = gm;
         if (tid == 0) {
-            st.x_cost = c + st.cost_cam;
+            st.x_cost = c + st.cost_cam[b];
             st.gmax = gm;
             if (f_first) st.initial_cost = st.x_cost;
             st.fresh_lin = 0;
@@ -1340,7 +1367,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
     // ---- landmark back-substitution + model cost change  (-1/2 step'.g' + 1/2 step'.D^2 step', exact identity of
     //      Ceres' -(J' step)^T (r + J' step / 2) for the damped normal-equation solution)
     double *step_l = D.step_l + (size_t) w * C.L;
-    const double *AW = D.AW + (size_t) w * C.LP * C.NCA;  // landmark-major
+    const double *AW = lin_AW(C, D, b, w);  // landmark-major
     double part = 0;
     bool finite = true;
     double *R2 = D.red2 + (size_t) w * 4;
@@ -1468,7 +1495,8 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
 #undef SOLVE_CLK_ADD
 }
 
-// ------------------------------------------------------------------------------------------------ candidate cost
+// ------------------------------------------------------------------------------------------------ candidate cost (split / NCCL pipelines)
+// The single-GPU pipeline takes the candidate cost from the linearisation at the candidate instead (ba_accept).
 // camera-only factors at the candidate point (one CTA per window; runs beside the vision blocks on the handle's second stream)
 __global__ void __launch_bounds__(CAM_THREADS) ba_cost_cam(BaCaps C, BaDev D, int nblk_vis) {
     extern __shared__ double smem[];
@@ -1477,7 +1505,7 @@ __global__ void __launch_bounds__(CAM_THREADS) ba_cost_cam(BaCaps C, BaDev D, in
     if (st.done || !st.step_valid) return;
     if (D.S.split && (w % D.world) != D.rank) return;
     const WinDims dm = D.dims[w];
-    double c = cam_factors(C, D, w, dm, D.pose_c + (size_t) w * C.K * 7, D.mix_c + (size_t) w * C.K * 9, D.ext_c + (size_t) w * 8, false, smem);
+    double c = cam_factors(C, D, w, dm, D.pose_c + (size_t) w * C.K * 7, D.mix_c + (size_t) w * C.K * 9, D.ext_c + (size_t) w * 8, false, 0, smem);
     if (threadIdx.x == 0) D.cost_part[(size_t) w * (nblk_vis + 1) + nblk_vis] = c;
 }
 __global__ void __launch_bounds__(256) ba_cost(BaCaps C, BaDev D, int nblk_vis) {
@@ -1510,7 +1538,7 @@ __global__ void __launch_bounds__(256) ba_cost(BaCaps C, BaDev D, int nblk_vis) 
 }
 
 // ------------------------------------------------------------------------------------------------ accept / reject
-__global__ void __launch_bounds__(128) ba_accept(BaCaps C, BaDev D, int nblk_vis) {
+__global__ void __launch_bounds__(128) ba_accept(BaCaps C, BaDev D) {
     __shared__ int s_accept;
     __shared__ double s_camsq, s_rhosq;
     __shared__ double s_red[40];
@@ -1538,17 +1566,39 @@ __global__ void __launch_bounds__(128) ba_accept(BaCaps C, BaDev D, int nblk_vis
         }
         if (tid == 0) s_camsq = s, s_rhosq = q;
     }
+    // Single GPU: the candidate cost from the linearisation at the candidate (buffer 1 - lin_buf), summed in ba_cost's order -- per 256 record
+    // slots block_sum's tree (warp k sums slots [32 k, 32 k + 32) of the block, then the eight warp sums in order), the blocks in order, then
+    // the camera-only cost -- so that every decision below matches the sum of ba_cost's partials bit for bit.  Landmark shards receive the
+    // all-reduced candidate cost in R2[3] (ba_pack2).
+    // s_warp (dynamic, 8 per 256 slots): the sums of the 32-slot groups; warp k of this CTA reduces groups k, k + 4, ... with no barrier in
+    // between, so that the loads of several groups are in flight together.
+    extern __shared__ double s_warp[];
+    const int lane = tid & 31, warp = tid >> 5, ngrp = (dm.F + 31) / 32;
+    const bool cand_here = D.world == 1 && st.step_valid;
+    if (cand_here) {
+        const double *costf = lin_costf(C, D, 1 - st.lin_buf, w);
+        const int4 *meta = (const int4 *) D.f_meta_s + (size_t) w * C.F;  // (landmark, reference node, observing node, factor id) per slot
+#pragma unroll 4
+        for (int g = warp; g < ngrp; g += 4) {
+            const int q = 32 * g + lane;
+            double v = q < dm.F ? costf[meta[q].w] : 0.0;  // lin_vis leaves 0 for an inactive factor
+            for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+            if (lane == 0) s_warp[g] = v;
+        }
+    }
     __syncthreads();
     if (tid == 0) {
         s_accept = 0;
         const double mcc = R2[0], sn = R2[1], nfin = R2[2];
         double cand = R2[3];
-        if (D.world == 1 && st.step_valid) {  // single GPU: sum the candidate-cost partials here (ba_pack2 does it before the all-reduce otherwise)
-            const double *part = D.cost_part + (size_t) w * (nblk_vis + 1);
+        if (cand_here) {
             cand = 0;
-            const int nb = (dm.F + 255) / 256;
-            for (int b = 0; b < nb; b++) cand += part[b];
-            cand += part[nblk_vis];
+            for (int g0 = 0; g0 < ngrp; g0 += 8) {
+                double t = 0;
+                for (int k = 0; k < 8; k++) t += g0 + k < ngrp ? s_warp[g0 + k] : 0.0;
+                cand += t;
+            }
+            cand += st.cost_cam[1 - st.lin_buf];
         }
         if (!chol_ok || nfin != 0.0 || !(mcc > 0.0)) {
             // HandleInvalidStep + LevenbergMarquardtStrategy::StepIsInvalid
@@ -1578,8 +1628,11 @@ __global__ void __launch_bounds__(128) ba_accept(BaCaps C, BaDev D, int nblk_vis
                     st.radius = fmin(1e16, st.radius / fmax(1.0 / 3.0, 1.0 - t * t * t));
                     st.decrease_factor = 2.0;
                     st.last_success = 1;
-                    st.need_lin = 1;
                     st.fresh_lin = 1;
+                    if (D.world == 1)
+                        st.lin_buf ^= 1;  // the candidate's linearisation is now the one at x
+                    else
+                        st.need_lin = 1;
                 } else {
                     // StepRejected
                     st.radius = st.radius / st.decrease_factor;
@@ -2038,9 +2091,9 @@ static int ba_create_body(icg_ba *h, int max_windows, int max_K, int max_L, int 
     if (rc == ICG_OK) rc = dmalloc(h, &D.field, count);
     DM(pose_c, NW * C.K * 7) DM(mix_c, NW * C.K * 9) DM(ext_c, NW * 8) DM(rho_c, NW * C.L)
     DM(pose_0, NW * C.K * 7) DM(mix_0, NW * C.K * 9) DM(ext_0, NW * 8) DM(rho_0, NW * C.L)
-    DM(AW, NW * C.NCA * C.LP) DM(Mp, NW * (size_t) C.K * (C.K - 1) * 210) DM(visv, NW * 3 * C.NCV)
-    DM(gpart, NW * (size_t) C.GQ * 210) DM(costf, NW * C.F) DM(hl, NW * C.L) DM(gl, NW * C.L) DM(scale_l, NW * C.L) DM(scale_c, NW * C.NS)
-    DM(Hc, NW * C.NS * C.NS) DM(gc, NW * C.NS) DM(Hs, NW * C.NS * C.NS) DM(cost_part, NW * (h->nblk_vis + 1)) DM(red, NW * (2 * (size_t) C.NCA * C.NCA + 8)) DM(redmax, NW) DM(red2, NW * 4) DM(step_c, NW * C.NS) DM(step_l, NW * C.L)
+    DM(AW[0], NW * C.NCA * C.LP) DM(Mp[0], NW * (size_t) C.K * (C.K - 1) * 210) DM(visv, NW * 3 * C.NCV)
+    DM(gpart, NW * (size_t) C.GQ * 210) DM(costf[0], NW * C.F) DM(hl[0], NW * C.L) DM(gl[0], NW * C.L) DM(scale_l, NW * C.L) DM(scale_c, NW * C.NS)
+    DM(Hc[0], NW * C.NS * C.NS) DM(gc[0], NW * C.NS) DM(Hs, NW * C.NS * C.NS) DM(cost_part, NW * (h->nblk_vis + 1)) DM(red, NW * (2 * (size_t) C.NCA * C.NCA + 8)) DM(redmax, NW) DM(red2, NW * 4) DM(step_c, NW * C.NS) DM(step_l, NW * C.L)
 #undef DM
     if (rc == ICG_OK) rc = dmalloc(h, &D.gnss_std_0, NW * C.G * 3);
     if (rc == ICG_OK) {
@@ -2349,7 +2402,7 @@ int icg_ba_upload(icg_ba *h, int n, const icg_ba_problem *P) {
 }
 
 // ---- in-situ stage timing
-static const char *PROF_NAMES[16] = {"(gap/other)", "lin_vis", "lin_lm", "", "", "schur_dmma (+ epilogue)", "join lin_cam + lin_done",
+static const char *PROF_NAMES[16] = {"(gap/other)", "lin_vis", "lin_lm", "lin at candidate", "","schur_dmma (+ epilogue)", "join lin_cam + lin_done",
                                      "signal", "solve", "cost (+cost_cam)", "pack2 / exchange", "accept", "hsum / reduce", "join gram chain", "step_lm", ""};
 static void prof_mark(icg_ba *h, int tag) {
     if (!h->prof) return;
@@ -2415,41 +2468,74 @@ static void prof_print(icg_ba *h) {
 
 static int enqueue_lm_split(icg_ba *h, int max_num_iterations);
 
+// The second linearisation buffer (BaDev::Mp etc.), allocated on the first LM sequence of the single-GPU pipeline: handles that the split
+// or NCCL pipelines drive never linearise a candidate and do not pay for it (~80 MB for 148 windows at K = 10, L = 300).
+static int alloc_lin_buf2(icg_ba *h) {
+    BaDev &D = h->D;
+    if (D.Mp[1]) return ICG_OK;
+    const BaCaps &C = h->C;
+    const size_t NW = C.NW;
+    int rc = ICG_OK;
+#define DM(field, count) \
+    if (rc == ICG_OK) rc = dmalloc(h, &D.field, count);
+    DM(AW[1], NW * C.NCA * C.LP) DM(Mp[1], NW * (size_t) C.K * (C.K - 1) * 210) DM(costf[1], NW * C.F) DM(hl[1], NW * C.L) DM(gl[1], NW * C.L)
+    DM(Hc[1], NW * C.NS * C.NS) DM(gc[1], NW * C.NS)
+#undef DM
+    return rc;
+}
+
 static int enqueue_lm(icg_ba *h, int max_num_iterations) {
     if (h->D.S.split) return enqueue_lm_split(h, max_num_iterations);
+    if (!h->comm) {
+        const int rc = alloc_lin_buf2(h);
+        if (rc != ICG_OK) return rc;
+    }
     const BaCaps &C = h->C;
     const BaDev &D = h->D;
     const int n = h->cur_windows;
     cudaStream_t s = h->stream;
     const dim3 g_vis(C.NVB - 2, n), g_cost(h->nblk_vis, n);
-    // iteration 0 linearisation + (max_iter) x [schur syrk, solve, cost, accept, re-linearise]; one extra solve call
-    // performs the final termination bookkeeping.
+    // Single GPU: linearisation at x (iteration 0) + (max_iter) x [schur syrk, solve, linearisation at the candidate, accept]; one extra
+    // schur + solve performs the final termination bookkeeping.  The linearisation at the candidate goes into the window's other buffer:
+    // its per-factor costs are the candidate cost ba_accept tests, and an accepted step flips the buffers instead of linearising again at
+    // the new x; a rejected one leaves the linearisation at x untouched.
+    // Landmark shards (NCCL): the candidate cost crosses the ranks before the accept step, so they evaluate it on its own (ba_cost,
+    // ba_cost_cam) and re-linearise at x after an accepted step.
     // where the camera-only factors are forked: 0 = beside ba_lin_vis (round 1), 1 = behind it (ba_lin_vis holds 128 registers x 4 CTAs: a
     // 320-thread camera CTA on the same SM costs it a resident CTA; on a single GPU nothing runs beside it then, the Schur kernel's epilogue
     // reads H_c).  Chosen by measurement (in-kernel phase clocks, ICG_BA_PROFILE).
     static const int cam_fork = getenv("ICG_BA_CAM_FORK") ? atoi(getenv("ICG_BA_CAM_FORK")) : 0;
-    for (int it = 0; it <= max_num_iterations; it++) {
+    // the linearisation (at x or at the candidate); the single GPU joins the camera-only factors before the next kernel reads H_c
+    auto enqueue_lin = [&](int at_cand) -> int {
         // fork: IMU / GNSS / prior factors (one latency-bound CTA per window) run beside the vision chain
         if (cam_fork == 0) {
             ICG_CUDA(cudaEventRecord(h->ev_fork, s));
             ICG_CUDA(cudaStreamWaitEvent(h->stream_cam, h->ev_fork, 0));
-            ba_lin_cam<<<n, h->cam_threads, h->smem_cam, h->stream_cam>>>(C, D);
+            ba_lin_cam<<<n, h->cam_threads, h->smem_cam, h->stream_cam>>>(C, D, at_cand);
             ICG_CUDA(cudaEventRecord(h->ev_join, h->stream_cam));
         }
         prof_mark(h, 0);
-        ba_lin_vis<<<g_vis, 128, LV_SMEM, s>>>(C, D);
-        prof_mark(h, 1);
+        ba_lin_vis<<<g_vis, 128, LV_SMEM, s>>>(C, D, at_cand);
+        prof_mark(h, at_cand ? 3 : 1);
         if (cam_fork != 0) {
             ICG_CUDA(cudaEventRecord(h->ev_fork, s));
             ICG_CUDA(cudaStreamWaitEvent(h->stream_cam, h->ev_fork, 0));
-            ba_lin_cam<<<n, h->cam_threads, h->smem_cam, h->stream_cam>>>(C, D);
+            ba_lin_cam<<<n, h->cam_threads, h->smem_cam, h->stream_cam>>>(C, D, at_cand);
             ICG_CUDA(cudaEventRecord(h->ev_join, h->stream_cam));
         }
         // (measured: one fused launch or two streams are both slower -- the Schur CTAs' shared memory throttles the latency-bound
         //  Gram warps when they share SMs)
-        if (!h->comm) {  // single GPU: the Schur kernel's epilogue adds H_c
+        if (!h->comm) {
             ICG_CUDA(cudaStreamWaitEvent(s, h->ev_join, 0));
-            prof_mark(h, 6);
+            prof_mark(h, at_cand ? 3 : 6);
+        }
+        count_launch(2);
+        return ICG_OK;
+    };
+    for (int it = 0; it <= max_num_iterations; it++) {
+        if (it == 0 || h->comm) {
+            const int rc = enqueue_lin(0);
+            if (rc != ICG_OK) return rc;
         }
         ba_schur_dmma<<<dim3(BA_SPLIT_W, n), 256, h->smem_schur, s>>>(C, D, h->ld_schur);
         prof_mark(h, 5);
@@ -2465,24 +2551,28 @@ static int enqueue_lm(icg_ba *h, int max_num_iterations) {
         }
         ba_solve<<<n, SOLVE_THREADS, h->smem_solve, s>>>(C, D);
         prof_mark(h, 8);
-        count_launch(h->comm ? 5 : 4);
+        count_launch(h->comm ? 3 : 2);
         if (it == max_num_iterations) break;
-        ICG_CUDA(cudaEventRecord(h->ev_fork, s));
-        ICG_CUDA(cudaStreamWaitEvent(h->stream_cam, h->ev_fork, 0));
-        ba_cost_cam<<<n, h->cam_threads, h->smem_cam, h->stream_cam>>>(C, D, h->nblk_vis);
-        ICG_CUDA(cudaEventRecord(h->ev_join, h->stream_cam));
-        ba_cost<<<g_cost, 256, 0, s>>>(C, D, h->nblk_vis);
-        ICG_CUDA(cudaStreamWaitEvent(s, h->ev_join, 0));
-        prof_mark(h, 9);
         if (h->comm) {
+            ICG_CUDA(cudaEventRecord(h->ev_fork, s));
+            ICG_CUDA(cudaStreamWaitEvent(h->stream_cam, h->ev_fork, 0));
+            ba_cost_cam<<<n, h->cam_threads, h->smem_cam, h->stream_cam>>>(C, D, h->nblk_vis);
+            ICG_CUDA(cudaEventRecord(h->ev_join, h->stream_cam));
+            ba_cost<<<g_cost, 256, 0, s>>>(C, D, h->nblk_vis);
+            ICG_CUDA(cudaStreamWaitEvent(s, h->ev_join, 0));
+            prof_mark(h, 9);
             ba_pack2<<<(n + 127) / 128, 128, 0, s>>>(C, D, n, h->nblk_vis);
             prof_mark(h, 10);
             int rc = nccl_allreduce(h, D.red2, (size_t) n * 4, 0);
             if (rc != ICG_OK) return rc;
+            count_launch(3);
+        } else {
+            const int rc = enqueue_lin(1);
+            if (rc != ICG_OK) return rc;
         }
-        ba_accept<<<n, 128, 0, s>>>(C, D, h->nblk_vis);
+        ba_accept<<<n, 128, sizeof(double) * 8 * h->nblk_vis, s>>>(C, D);  // one double per 32 record slots
         prof_mark(h, 11);
-        count_launch(h->comm ? 4 : 3);
+        count_launch();
     }
     ICG_CHECK_LAUNCH();
     return ICG_OK;
@@ -2598,10 +2688,10 @@ static int enqueue_lm_split(icg_ba *h, int max_num_iterations) {
         const unsigned long long epoch = ++h->epoch;
         ICG_CUDA(cudaEventRecord(h->ev_fork, s));
         ICG_CUDA(cudaStreamWaitEvent(h->stream_cam, h->ev_fork, 0));
-        ba_lin_cam<<<n, h->cam_threads, h->smem_cam, h->stream_cam>>>(C, D);
+        ba_lin_cam<<<n, h->cam_threads, h->smem_cam, h->stream_cam>>>(C, D, 0);
         ICG_CUDA(cudaEventRecord(h->ev_join, h->stream_cam));
         prof_mark(h, 0);
-        ba_lin_vis<<<g_vis, 128, LV_SMEM, s>>>(C, D);
+        ba_lin_vis<<<g_vis, 128, LV_SMEM, s>>>(C, D, 0);
         prof_mark(h, 1);
         ba_schur_dmma<<<dim3(BA_SPLIT_W, n), 256, h->smem_schur, s>>>(C, D, h->ld_schur);  // + the export into the owner's inbox
         prof_mark(h, 5);
@@ -2917,7 +3007,7 @@ static int marginalize_body(icg_ba *h, int n_windows, const icg_ba_problem *prob
     const BaDev &D = h->D;
     const size_t smem = sizeof(double) * (8 * 480 + 2 * (size_t) C.R) + sizeof(int) * (size_t) C.R + 64;
     marg_prepare<<<(n + 127) / 128, 128, 0, s>>>(D, M, n, 0);
-    ba_lin_vis<<<dim3(C.NVB - 2, n), 128, LV_SMEM, s>>>(C, D);
+    ba_lin_vis<<<dim3(C.NVB - 2, n), 128, LV_SMEM, s>>>(C, D, 0);
     marg_assemble<<<n, 256, smem, s>>>(C, D, M);
     // eigendecompositions: on-chip cluster-pair kernel when every block of the batch fits (n <= MARG_PAIR_MAXN), global-memory kernel otherwise
     int max_m = 0, max_r = 0;

@@ -178,7 +178,7 @@ __global__ void __launch_bounds__(256) marg_assemble(BaCaps C, BaDev D, MargDev 
     {
         const int PM = C.K * (C.K - 1), P = D.npairs[w];
         const int *pro = D.pair_ro + (size_t) w * PM;
-        const double *Mp = D.Mp + (size_t) w * PM * 210;
+        const double *Mp = lin_Mp(C, D, D.st[w].lin_buf, w);
         int la = 0, lb = 0;
         if (tid < 210) {
             int e = tid;
@@ -203,13 +203,15 @@ __global__ void __launch_bounds__(256) marg_assemble(BaCaps C, BaDev D, MargDev 
         }
     }
     // ---- landmark rows: h_l on the diagonal, coupling row w_l, g_l  (thread per (landmark, vision column))
+    const int buf = D.st[w].lin_buf;  // the linearisation ba_lin_vis just made at x
+    const double *AW = lin_AW(C, D, buf, w), *hl = lin_hl(C, D, buf, w);
     for (int e = tid; e < dm.L * (NCV + 1); e += blockDim.x) {
         const int l = e / (NCV + 1), c = e - l * (NCV + 1);
         const int cl = lm_col[l];
         if (cl < 0) continue;
-        const double v = D.AW[((size_t) w * C.LP + l) * C.NCA + c];
+        const double v = AW[(size_t) l * C.NCA + c];
         if (c == NCV) {
-            H0[(size_t) cl * n0 + cl] = D.hl[(size_t) w * C.L + l];
+            H0[(size_t) cl * n0 + cl] = hl[l];
             b0[cl] = -v;
         } else {
             const int mc = c < 6 * K ? (pose_col[c / 6] < 0 ? -1 : pose_col[c / 6] + c % 6) : c < 6 * K + 6 ? ext_col + c - 6 * K : td_col;

@@ -105,7 +105,7 @@ __global__ void __launch_bounds__(256) ba_reduce(BaCaps C, BaDev D, unsigned lon
     };
     double *rv = D.S.redv + (size_t) w * D.S.RV;
     if (A < NCV && B < NCV) {
-        D.Hs[(size_t) w * C.NS * C.NS + (size_t) B * C.NS + A] = D.Hc[(size_t) w * C.NS * C.NS + (size_t) B * C.NS + A] + rsum(tri_idx(A, B, NCV));
+        D.Hs[(size_t) w * C.NS * C.NS + (size_t) B * C.NS + A] = lin_Hc(C, D, 0, w)[(size_t) B * C.NS + A] + rsum(tri_idx(A, B, NCV));
         if (A == B) rv[A] = rsum(TRI + A);
     } else if (A < NCV) {  // B == NCV: the gradient column
         rv[NCV + A] = rsum(TRI + NCV + A);
@@ -138,7 +138,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS) ba_solve_cam(BaCaps C, BaDev D,
     const int CT = CL * SOLVE_THREADS, ctid = cr * SOLVE_THREADS + tid, cwarp = ctid >> 5, ncwarps = CT / 32;
     // snapshot of the LM state (CTA 0 updates it after the first cluster barrier)
     const int f_first = st.first, f_fresh = st.fresh_lin, f_last = st.last_success, f_iter = st.iter, f_maxit = st.max_iter;
-    const double radius = st.radius, cost_cam = st.cost_cam, gmax_old = st.gmax, xcost_old = st.x_cost, init_old = st.initial_cost;
+    const double radius = st.radius, cost_cam = st.cost_cam[0], gmax_old = st.gmax, xcost_old = st.x_cost, init_old = st.initial_cost;
     double *s_red = sm;                  // 40
     double *s_scale = s_red + 40;        // N
     double *s_g = s_scale + C.NS;        // N
@@ -146,7 +146,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS) ba_solve_cam(BaCaps C, BaDev D,
     double *s_d2 = s_rhs + C.NS;         // N
     double *s_blk = s_d2 + C.NS;         // SPLIT_BS_ROWS x (NS + 1): row block of L for the back-substitution (CTA 0)
     double *S = D.Sglobal + (size_t) (w / D.world) * split_S_stride(C);  // one workspace per OWNED window: packed triangle | pivot reciprocals
-    const double *Hc = D.Hc + (size_t) w * C.NS * C.NS, *gcam = D.gc + (size_t) w * C.NS, *Hs = D.Hs + (size_t) w * C.NS * C.NS;
+    const double *Hc = lin_Hc(C, D, 0, w), *gcam = lin_gc(C, D, 0, w), *Hs = D.Hs + (size_t) w * C.NS * C.NS;
     const double *rv = D.S.redv + (size_t) w * D.S.RV;   // [diag H_vis | g_vis | W phi g_l | cost, sum rho^2, max |g_l|]
     double *scale_c = D.scale_c + (size_t) w * C.NS;
     // ---- gradient, Jacobi scaling (first linearisation), LM diagonal, rhs: every CTA keeps its own copy (no DSMEM traffic)
@@ -572,7 +572,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 1) ba_solve_cam_dsm(BaCaps C, B
     const int nt = dsm_ntiles(NR), npan = (N + 7) / 8;   // this window: tile rows (incl. the rhs row), column panels
     const int Tn = N >> 3, rn = N & 7;                   // tile row / row in the tile of the augmented right-hand-side row
     const int f_first = st.first, f_fresh = st.fresh_lin, f_last = st.last_success, f_iter = st.iter, f_maxit = st.max_iter;
-    const double radius = st.radius, cost_cam = st.cost_cam, gmax_old = st.gmax, xcost_old = st.x_cost, init_old = st.initial_cost;
+    const double radius = st.radius, cost_cam = st.cost_cam[0], gmax_old = st.gmax, xcost_old = st.x_cost, init_old = st.initial_cost;
     double *s_red = sm;                       // 40
     double *s_scale = s_red + 40;             // VL each
     double *s_g = s_scale + VL;
@@ -591,7 +591,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 1) ba_solve_cam_dsm(BaCaps C, B
     double *s_dg = s_xT + 16;                 // [ntc][64] replicated diagonal tiles
     double *s_P = s_dg + (size_t) ntc * 64;   // [2][ntc][64] panel column, by panel parity
     double *s_tiles = s_P + (size_t) 2 * ntc * 64;
-    const double *Hc = D.Hc + (size_t) w * C.NS * C.NS, *gcam = D.gc + (size_t) w * C.NS, *Hs = D.Hs + (size_t) w * C.NS * C.NS;
+    const double *Hc = lin_Hc(C, D, 0, w), *gcam = lin_gc(C, D, 0, w), *Hs = D.Hs + (size_t) w * C.NS * C.NS;
     const double *rv = D.S.redv + (size_t) w * D.S.RV;   // [diag H_vis | g_vis | W phi g_l | cost, sum rho^2, max |g_l|]
     double *scale_c = D.scale_c + (size_t) w * C.NS;
     // ---- gradient, Jacobi scaling (first linearisation), LM diagonal, rhs: every CTA keeps its own copy
@@ -1074,9 +1074,9 @@ __global__ void __launch_bounds__(SOLVE_THREADS) ba_step_lm(BaCaps C, BaDev D, u
     for (int a = tid; a < N; a += SOLVE_THREADS) s_dl[a] = __ldcg(BC + SPLIT_HDR + a);
     __syncthreads();
     const double radius = st.radius;
-    const double *hl = D.hl + (size_t) w * C.L, *gl = D.gl + (size_t) w * C.L, *scale_l = D.scale_l + (size_t) w * C.L;
+    const double *hl = lin_hl(C, D, 0, w), *gl = lin_gl(C, D, 0, w), *scale_l = D.scale_l + (size_t) w * C.L;
     double *step_l = D.step_l + (size_t) w * C.L;
-    const double *AW = D.AW + (size_t) w * C.LP * C.NCA;
+    const double *AW = lin_AW(C, D, 0, w);
     const double *rho = D.rho + (size_t) w * C.L;
     double *rho_c = D.rho_c + (size_t) w * C.L;
     constexpr int LB = 4;
