@@ -45,6 +45,41 @@ class BaSummary(C.Structure):
                 ("initial_cost", C.c_double), ("final_cost", C.c_double), ("final_radius", C.c_double)]
 
 
+fp = C.POINTER(C.c_float)
+
+
+class CullWindow(C.Structure):
+    """ctypes image of `icg_ba_cull_window`."""
+    _fields_ = [("R_bc", C.c_double * 9), ("t_bc", C.c_double * 3), ("td_bc", C.c_double), ("estimate_ext", C.c_int32), ("estimate_td", C.c_int32),
+                ("lm_ref_node", ip), ("lm_ref_kp", fp), ("obs_off", ip), ("obs_node", ip), ("obs_kp", fp), ("obs_factor", ip),
+                ("R_bc_out", C.c_double * 9), ("t_bc_out", C.c_double * 3), ("td_bc_out", C.c_double), ("ext_accepted", C.c_int32),
+                ("cam_pose", dp), ("lm_pw", dp), ("lm_depth", dp), ("lm_outlier", bp), ("obs_outlier", bp), ("counts", C.c_int32 * 5)]
+
+
+_CULL_IN = dict(lm_ref_node=(np.int32, ip), lm_ref_kp=(np.float32, fp), obs_off=(np.int32, ip), obs_node=(np.int32, ip), obs_kp=(np.float32, fp),
+                obs_factor=(np.int32, ip))
+
+
+def cull_struct(prob: dict, ci: dict) -> CullWindow:
+    """The icg_ba_cull_window of one window over the arrays of `ci` (made contiguous in place; output arrays are added to it)."""
+    s = CullWindow()
+    K, L = int(prob["K"]), int(prob["L"])
+    for k, v in zip(("R_bc", "t_bc"), (np.asarray(ci["R_bc"], np.float64).reshape(-1), np.asarray(ci["t_bc"], np.float64).reshape(-1))):
+        getattr(s, k)[:] = [float(x) for x in v]
+    s.td_bc, s.estimate_ext, s.estimate_td = float(ci.get("td_bc", 0.0)), int(ci.get("estimate_ext", 1)), int(ci.get("estimate_td", 1))
+    for k, (dt, pt) in _CULL_IN.items():
+        if ci.get(k) is None:
+            continue
+        a = np.ascontiguousarray(ci[k], dtype=dt)
+        ci[k] = a
+        setattr(s, k, a.ctypes.data_as(pt) if a.size else pt())
+    n_obs = int(ci["obs_off"][L]) if L > 0 else 0
+    ci.update(cam_pose=np.zeros((K, 12)), lm_pw=np.zeros((L, 3)), lm_depth=np.zeros(L), lm_outlier=np.zeros(L, np.uint8), obs_outlier=np.zeros(n_obs, np.uint8))
+    s.cam_pose, s.lm_pw, s.lm_depth = (ci[k].ctypes.data_as(dp) for k in ("cam_pose", "lm_pw", "lm_depth"))
+    s.lm_outlier, s.obs_outlier = ci["lm_outlier"].ctypes.data_as(bp), ci["obs_outlier"].ctypes.data_as(bp)
+    return s
+
+
 _ARR = dict(pose=np.float64, mix=np.float64, ext=np.float64, invdepth=np.float64, f_lm=np.int32, f_ref=np.int32, f_obs=np.int32,
             f_const=np.float64, f_active=np.uint8, imu_blob=np.float64, pose_prior=np.float64, pose_prior_std=np.float64,
             mix_prior=np.float64, mix_prior_std=np.float64, gnss_node=np.int32, gnss_blh=np.float64, gnss_std=np.float64,
@@ -249,16 +284,52 @@ class WindowSolver:
         s2 = self.solve(prob, second)[0]
         return dict(pass1=s1, pass2=s2, reproj_removed=int(out.sum()), gnss_reweighted=n_gnss_out)
 
-    def marginalize(self, problems, num_marg=1, want_schur=True, resident=False):
+    def marginalize(self, problems, num_marg=1, want_schur=True, resident=False, culled=None, node_in_map=None):
         """MarginalizationInfo::marginalization as GVINS::gvinsMarginalization drives it (IG/ic_gvins.cc:1412-1640) on a list of
         windows: removes the `num_marg` oldest nodes + the landmarks anchored in them.  Returns one dict per window with the new
         prior in the layout the problem dict's marg_* entries use (node indices already shifted).  resident=True: the windows are the
-        ones this handle has just solved (icg_ba_marginalize_resident: nothing is uploaded again)."""
+        ones this handle has just solved (icg_ba_marginalize_resident: nothing is uploaded again).  culled (resident only): the list
+        update_and_cull returned, with `obs_factor` in each dict; the factor set is then the map after the culling
+        (icg_ba_marginalize_resident_culled), node_in_map[w] (K flags) naming the keyframes still in the map (all of them when None)."""
         if isinstance(problems, dict):
             problems = [problems]
         call = self.marg_prepare(problems, num_marg, want_schur)
-        self.marg_run(call, resident)
+        if culled is None:
+            self.marg_run(call, resident)
+        else:
+            if not resident:
+                raise ValueError("culled= applies to the resident marginalization")
+            if node_in_map is None:
+                node_in_map = [np.ones(p["K"], np.uint8) for p in problems]
+            nim = [np.ascontiguousarray(m, np.uint8) for m in node_in_map]
+            keep = [dict(c) for c in culled]
+            cw = (CullWindow * len(problems))(*[cull_struct(p, c) for p, c in zip(problems, keep)])
+            for w, (c, k) in enumerate(zip(culled, keep)):  # the culling's flags, as that call returned them
+                k["flags"] = [np.ascontiguousarray(c["lm_outlier"], np.uint8), np.ascontiguousarray(c["obs_outlier"], np.uint8)]
+                cw[w].lm_outlier, cw[w].obs_outlier = (a.ctypes.data_as(bp) for a in k["flags"])
+            ptrs = (vp * len(nim))(*[vp(m.ctypes.data) for m in nim])
+            check(lib().icg_ba_marginalize_resident_culled(self._h, call["n"], call["arr"], vp(call["nm"].ctypes.data), cw, ptrs, call["pri"]),
+                  "icg_ba_marginalize_resident_culled")
         return self.marg_collect(call)
+
+    def update_and_cull(self, problems, camera, std, cull_inputs):
+        """updateParametersFromOptimizer + gvinsOutlierCulling (IG/ic_gvins.cc:1299-1389, 1035-1128) on the windows this handle has just
+        solved (icg_ba_update_and_cull_resident).  camera: a camera.Camera or CameraStruct; std: reprojection_error_std_.  cull_inputs: one
+        dict per window with R_bc (3x3), t_bc, td_bc, estimate_ext, estimate_td, lm_ref_node (L), lm_ref_kp (L x 2), obs_off (L + 1),
+        obs_node, obs_kp (x 2) and optionally obs_factor.  Returns one dict per window: the inputs plus R_bc_out, t_bc_out, td_bc_out,
+        ext_accepted, cam_pose (K x 12), lm_pw (L x 3), lm_depth, lm_outlier, obs_outlier and counts (5)."""
+        if isinstance(problems, dict):
+            problems, cull_inputs = [problems], [cull_inputs]
+        n = len(problems)
+        arr = (BaProblem * n)(*[to_struct(p) for p in problems])
+        outs = [dict(c) for c in cull_inputs]
+        cw = (CullWindow * n)(*[cull_struct(p, c) for p, c in zip(problems, outs)])
+        cam = camera.c if hasattr(camera, "c") else camera
+        check(lib().icg_ba_update_and_cull_resident(self._h, n, arr, C.byref(cam), float(std), cw), "icg_ba_update_and_cull_resident")
+        for c, s in zip(outs, cw):
+            c.update(R_bc_out=np.array(s.R_bc_out[:]).reshape(3, 3), t_bc_out=np.array(s.t_bc_out[:]), td_bc_out=s.td_bc_out, ext_accepted=s.ext_accepted,
+                     counts=np.array(s.counts[:], np.int32))
+        return outs
 
     def marg_prepare(self, problems, num_marg=1, want_schur=True):
         """The argument block of one icg_ba_marginalize call (struct array over the problems' host arrays + caller-allocated output arrays):

@@ -27,6 +27,7 @@ SOURCES = {
     "geom.cu": ["-fmad=false"],         # device versions of the camera model / RANSAC gate / triangulation / IMU propagation (same cores)
     "track.cu": ["-fmad=false"],       # trackMappoint / trackReferenceFrame on the KLT handle (geom_core.cuh arithmetic)
     "ba.cu": [],
+    "ba_cull.cu": ["-fmad=false"],     # post-solve map update and outlier culling (fixed-order sums, as the numpy restatement)
 }
 
 

@@ -38,6 +38,7 @@
 #include <thread>
 #include <vector>
 
+#include "ba_cull.cuh"
 #include "ba_math.cuh"
 #include "common.cuh"
 #include "geom_core.cuh"
@@ -1923,6 +1924,10 @@ struct icg_ba {
     MargDev M;
     HostDev<int> marg_map;
     HostDev<double> marg_oJ0, marg_oe0, marg_oHp, marg_obp;
+    HostDev<uint8_t> marg_fmask;  // factor set of icg_ba_marginalize_resident_culled (ba_lin_vis reads it in place of f_active)
+    // post-solve update + culling: one pinned staging buffer and its device twin, [inputs | outputs], grown on demand
+    unsigned char *cull_h = nullptr, *cull_d = nullptr;
+    size_t cull_cap = 0;
 };
 
 extern "C" {
@@ -2147,7 +2152,9 @@ void icg_ba_destroy(icg_ba *h) {
     h->f_meta_s.release(), h->vb_lm0.release(), h->ref_nrun.release(), h->f_const_s.release(), h->marg_type.release(), h->marg_node.release(), h->f_active.release(), h->scratch.release(), h->st_save.release(), h->cull_counters.release(), h->part_off.release(), h->pair_ro.release(), h->vis_ord.release(), h->npairs.release();
     if (h->comm) nccl_api().CommDestroy((ncclComm_t) h->comm);
     split_release(h);
-    if (h->marg_ready) h->marg_map.release(), h->marg_oJ0.release(), h->marg_oe0.release(), h->marg_oHp.release(), h->marg_obp.release();
+    if (h->marg_ready) h->marg_map.release(), h->marg_oJ0.release(), h->marg_oe0.release(), h->marg_oHp.release(), h->marg_obp.release(), h->marg_fmask.release();
+    if (h->cull_h) cudaFreeHost(h->cull_h);
+    if (h->cull_d) cudaFree(h->cull_d);
     for (void *p : h->dev_only) cudaFree(p);
     if (h->stream_cam) cudaStreamSynchronize(h->stream_cam), cudaStreamDestroy(h->stream_cam);
     if (h->ev_fork) cudaEventDestroy(h->ev_fork);
@@ -2894,7 +2901,7 @@ static int marg_alloc(icg_ba *h) {
     }
     M.map_stride = MARG_MAP_HDR + 2 * C.K + C.L;
     if (h->marg_map.alloc(NW * M.map_stride) != ICG_OK || h->marg_oJ0.alloc(NW * (size_t) M.rcap * M.rcap) != ICG_OK || h->marg_oe0.alloc(NW * M.rcap) != ICG_OK ||
-        h->marg_oHp.alloc(NW * (size_t) M.rcap * M.rcap) != ICG_OK || h->marg_obp.alloc(NW * M.rcap) != ICG_OK) {
+        h->marg_oHp.alloc(NW * (size_t) M.rcap * M.rcap) != ICG_OK || h->marg_obp.alloc(NW * M.rcap) != ICG_OK || h->marg_fmask.alloc(NW * C.F) != ICG_OK) {
         set_error("icg_ba_marginalize: workspace allocation failed");
         return ICG_ENOMEM;
     }
@@ -2915,7 +2922,10 @@ static int marg_alloc(icg_ba *h) {
     return ICG_OK;
 }
 
-static int marginalize_body(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg, icg_ba_prior *out, bool resident) {
+// fmask (resident only, may be NULL): per window, the factor set to marginalize in place of the problem's activity (F bytes each); it reaches
+// ba_lin_vis through a copy of the device view, so the handle's own f_active is never written
+static int marginalize_body(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg, icg_ba_prior *out, bool resident,
+                            const uint8_t *const *fmask = nullptr) {
     if (!h || !problems || !num_marg || !out || n_windows < 1 || n_windows > h->C.NW) {
         set_error("icg_ba_marginalize: bad arguments");
         return ICG_EINVAL;
@@ -2956,16 +2966,18 @@ static int marginalize_body(icg_ba *h, int n_windows, const icg_ba_problem *prob
         int *map = h->marg_map.h + (size_t) w * M.map_stride;
         int *pose_col = map + MARG_MAP_HDR, *mix_col = pose_col + C.K, *lm_col = mix_col + C.K;
         std::vector<char> tp(p.K, 0), tm(p.K, 0), tl(p.L, 0);
+        const uint8_t *act = fmask ? fmask[w] : p.f_active;
+        if (fmask) memcpy(h->marg_fmask.h + (size_t) w * C.F, act, p.F);
         bool any_vis = false;
         for (int f = 0; f < p.F; f++) {
-            if ((p.f_active && !p.f_active[f]) || p.f_ref[f] >= nm) continue;
+            if ((act && !act[f]) || p.f_ref[f] >= nm) continue;
             tl[p.f_lm[f]] = 1, tp[p.f_obs[f]] = 1, any_vis = true;
         }
         bool has_ext = any_vis, has_td = any_vis;
         // a block exists in the marginalization problem only if some factor touches it (MarginalizationInfo::addResidualBlockInfo,
         // marginalization_info.h:103-121): removed nodes without any factor get no columns
         for (int f = 0; f < p.F; f++)
-            if (!(p.f_active && !p.f_active[f]) && p.f_ref[f] < nm) tp[p.f_ref[f]] = 1;
+            if (!(act && !act[f]) && p.f_ref[f] < nm) tp[p.f_ref[f]] = 1;
         for (int k = 0; k < nm && k < p.n_imu; k++) tp[k] = tm[k] = tp[k + 1] = tm[k + 1] = 1;  // factor k joins node k and node k + 1
         for (int g = 0; g < p.n_gnss; g++)
             if (p.gnss_node[g] < nm) tp[p.gnss_node[g]] = 1;
@@ -3004,7 +3016,11 @@ static int marginalize_body(icg_ba *h, int n_windows, const icg_ba_problem *prob
     }
     cudaStream_t s = h->stream;
     ICG_CUDA(h->marg_map.up(s, (size_t) n * M.map_stride));
-    const BaDev &D = h->D;
+    BaDev D = h->D;
+    if (fmask) {
+        ICG_CUDA(h->marg_fmask.up(s, (size_t) n * C.F));
+        D.f_active = h->marg_fmask.d;
+    }
     const size_t smem = sizeof(double) * (8 * 480 + 2 * (size_t) C.R) + sizeof(int) * (size_t) C.R + 64;
     marg_prepare<<<(n + 127) / 128, 128, 0, s>>>(D, M, n, 0);
     ba_lin_vis<<<dim3(C.NVB - 2, n), 128, LV_SMEM, s>>>(C, D, 0);
@@ -3091,6 +3107,183 @@ int icg_ba_marginalize(icg_ba *h, int n_windows, const icg_ba_problem *problems,
 
 int icg_ba_marginalize_resident(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg, icg_ba_prior *out) {
     return marginalize_body(h, n_windows, problems, num_marg, out, true);
+}
+
+// ---- post-solve map update + outlier culling (ba_cull.cu)
+static int resident_single_rank(icg_ba *h, int n_windows, const icg_ba_problem *problems, const char *what) {
+    if (!h || !problems || n_windows < 1) {
+        set_error("%s: bad arguments", what);
+        return ICG_EINVAL;
+    }
+    if (h->comm || h->D.world > 1) {
+        set_error("%s: not available on a landmark-sharded handle (icg_ba_set_shard(world = 1) first)", what);
+        return ICG_EUNSUPPORTED;
+    }
+    if (h->cur_windows != n_windows) {
+        set_error("%s: the handle holds %d uploaded windows, the call names %d", what, h->cur_windows, n_windows);
+        return ICG_EINVAL;
+    }
+    return ICG_OK;
+}
+
+int icg_ba_update_and_cull_resident(icg_ba *h, int n_windows, const icg_ba_problem *problems, const icg_camera *cam, double reprojection_error_std,
+                                    icg_ba_cull_window *io) {
+    int rc = resident_single_rank(h, n_windows, problems, "icg_ba_update_and_cull_resident");
+    if (rc != ICG_OK) return rc;
+    if (!cam || !io) {
+        set_error("icg_ba_update_and_cull_resident: bad arguments");
+        return ICG_EINVAL;
+    }
+    const BaCaps &C = h->C;
+    const int n = n_windows;
+    // layout of the staging buffer: inputs [windows | lm_ref_node | obs_off | obs_node | lm_ref_kp | obs_kp], then outputs
+    // [windows | cam_pose | lm_pw | lm_depth | lm_outlier | obs_outlier], every array 16-byte aligned
+    std::vector<CullWin> win(n);
+    size_t nL = 0, nO = 0, nK = 0;
+    for (int w = 0; w < n; w++) {
+        const icg_ba_problem &p = problems[w];
+        const icg_ba_cull_window &c = io[w];
+        if (p.K < 2 || p.K > C.K || p.L < 0 || p.L > C.L || !c.cam_pose ||
+            (p.L > 0 && (!c.lm_ref_node || !c.lm_ref_kp || !c.obs_off || !c.lm_pw || !c.lm_depth || !c.lm_outlier))) {
+            set_error("icg_ba_update_and_cull_resident: window %d: sizes out of range or arrays missing", w);
+            return ICG_EINVAL;
+        }
+        const int no = p.L > 0 ? c.obs_off[p.L] : 0;
+        if (p.L > 0 && (c.obs_off[0] != 0 || no < 0 || no > INT32_MAX - (int64_t) nO || (no > 0 && (!c.obs_node || !c.obs_kp || !c.obs_outlier)))) {
+            set_error("icg_ba_update_and_cull_resident: window %d: obs_off must start at 0 and observation arrays must be given", w);
+            return ICG_EINVAL;
+        }
+        for (int l = 0; l < p.L; l++) {
+            if (c.obs_off[l + 1] < c.obs_off[l] || c.lm_ref_node[l] < 0 || c.lm_ref_node[l] >= p.K) {
+                set_error("icg_ba_update_and_cull_resident: window %d landmark %d: obs_off not monotone or reference node out of range", w, l);
+                return ICG_EINVAL;
+            }
+        }
+        for (int o = 0; o < no; o++)
+            if (c.obs_node[o] < 0 || c.obs_node[o] >= p.K) {
+                set_error("icg_ba_update_and_cull_resident: window %d observation %d: node %d out of range", w, o, c.obs_node[o]);
+                return ICG_EINVAL;
+            }
+        CullWin &W = win[w];
+        memcpy(W.R_bc, c.R_bc, sizeof(W.R_bc)), memcpy(W.t_bc, c.t_bc, sizeof(W.t_bc));
+        W.td_bc = c.td_bc, W.K = p.K, W.L = p.L, W.estimate_ext = c.estimate_ext != 0, W.estimate_td = c.estimate_td != 0;
+        W.lm0 = (int) nL, W.off0 = (int) (nL + w), W.obs0 = (int) nO, W.node0 = (int) nK;
+        nL += p.L, nO += no, nK += p.K;
+    }
+    auto al = [](size_t b) { return (b + 15) & ~(size_t) 15; };
+    size_t at = 0;
+    auto take = [&](size_t bytes) {
+        const size_t o = at;
+        at += al(bytes);
+        return o;
+    };
+    const size_t i_win = take(sizeof(CullWin) * n), i_ref = take(4 * nL), i_off = take(4 * (nL + n)), i_node = take(4 * nO), i_rkp = take(8 * nL),
+                 i_kp = take(8 * nO);
+    const size_t in_bytes = at;
+    const size_t o_win = take(sizeof(CullOut) * n), o_pose = take(96 * nK), o_pw = take(24 * nL), o_depth = take(8 * nL), o_lmo = take(nL), o_obso = take(nO);
+    const size_t out_bytes = at - in_bytes;
+    ICG_CUDA(cudaSetDevice(h->device));
+    cudaStream_t s = h->stream;
+    if (at > h->cull_cap) {
+        ICG_CUDA(cudaStreamSynchronize(s));
+        if (h->cull_h) cudaFreeHost(h->cull_h), h->cull_h = nullptr;
+        if (h->cull_d) cudaFree(h->cull_d), h->cull_d = nullptr;
+        h->cull_cap = 0;
+        const size_t cap = at + at / 4;
+        if (cudaMallocHost(&h->cull_h, cap) != cudaSuccess || cudaMalloc(&h->cull_d, cap) != cudaSuccess) {
+            set_error("icg_ba_update_and_cull_resident: staging allocation of %zu bytes failed", cap);
+            return ICG_ENOMEM;
+        }
+        h->cull_cap = cap;
+    }
+    unsigned char *H = h->cull_h, *Dv = h->cull_d;
+    memcpy(H + i_win, win.data(), sizeof(CullWin) * n);
+    for (int w = 0; w < n; w++) {
+        const icg_ba_problem &p = problems[w];
+        const icg_ba_cull_window &c = io[w];
+        const CullWin &W = win[w];
+        if (p.L == 0) {
+            ((int *) (H + i_off))[W.off0] = 0;
+            continue;
+        }
+        const int no = c.obs_off[p.L];
+        memcpy(H + i_ref + 4 * (size_t) W.lm0, c.lm_ref_node, 4 * (size_t) p.L);
+        memcpy(H + i_off + 4 * (size_t) W.off0, c.obs_off, 4 * ((size_t) p.L + 1));
+        memcpy(H + i_rkp + 8 * (size_t) W.lm0, c.lm_ref_kp, 8 * (size_t) p.L);
+        if (no > 0) memcpy(H + i_node + 4 * (size_t) W.obs0, c.obs_node, 4 * (size_t) no), memcpy(H + i_kp + 8 * (size_t) W.obs0, c.obs_kp, 8 * (size_t) no);
+    }
+    ICG_CUDA(cudaMemcpyAsync(Dv, H, in_bytes, cudaMemcpyHostToDevice, s));
+    CullArgs a;
+    a.cam = *cam, a.std = reprojection_error_std;
+    a.pose = h->D.pose, a.ext = h->D.ext, a.rho = h->D.rho, a.pose_stride = C.K * 7, a.rho_stride = C.L;
+    a.win = (const CullWin *) (Dv + i_win), a.lm_ref_node = (const int *) (Dv + i_ref), a.obs_off = (const int *) (Dv + i_off);
+    a.obs_node = (const int *) (Dv + i_node), a.lm_ref_kp = (const float *) (Dv + i_rkp), a.obs_kp = (const float *) (Dv + i_kp);
+    a.out = (CullOut *) (Dv + o_win), a.cam_pose = (double *) (Dv + o_pose), a.lm_pw = (double *) (Dv + o_pw), a.lm_depth = (double *) (Dv + o_depth);
+    a.lm_outlier = Dv + o_lmo, a.obs_outlier = Dv + o_obso;
+    ICG_CUDA(launch_update_cull(a, n, s));
+    count_launch();
+    ICG_CUDA(cudaMemcpyAsync(H + in_bytes, Dv + in_bytes, out_bytes, cudaMemcpyDeviceToHost, s));
+    ICG_CUDA(cudaStreamSynchronize(s));
+    for (int w = 0; w < n; w++) {
+        const icg_ba_problem &p = problems[w];
+        icg_ba_cull_window &c = io[w];
+        const CullWin &W = win[w];
+        const CullOut &O = ((const CullOut *) (H + o_win))[w];
+        memcpy(c.R_bc_out, O.R_bc, sizeof(c.R_bc_out)), memcpy(c.t_bc_out, O.t_bc, sizeof(c.t_bc_out));
+        c.td_bc_out = O.td_bc, c.ext_accepted = O.ext_accepted;
+        memcpy(c.counts, O.counts, sizeof(c.counts));
+        memcpy(c.cam_pose, H + o_pose + 96 * (size_t) W.node0, 96 * (size_t) p.K);
+        if (p.L == 0) continue;
+        const int no = c.obs_off[p.L];
+        memcpy(c.lm_pw, H + o_pw + 24 * (size_t) W.lm0, 24 * (size_t) p.L);
+        memcpy(c.lm_depth, H + o_depth + 8 * (size_t) W.lm0, 8 * (size_t) p.L);
+        memcpy(c.lm_outlier, H + o_lmo + W.lm0, p.L);
+        if (no > 0) memcpy(c.obs_outlier, H + o_obso + W.obs0, no);
+    }
+    return ICG_OK;
+}
+
+int icg_ba_marginalize_resident_culled(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg,
+                                       const icg_ba_cull_window *culled, const uint8_t *const *node_in_map, icg_ba_prior *out) {
+    int rc = resident_single_rank(h, n_windows, problems, "icg_ba_marginalize_resident_culled");
+    if (rc != ICG_OK) return rc;
+    if (!culled || !node_in_map) {
+        set_error("icg_ba_marginalize_resident_culled: bad arguments");
+        return ICG_EINVAL;
+    }
+    // the factor set of gvinsMarginalization (IG/ic_gvins.cc:1558-1609) from the culling's flags: on the host, beside the structure loop
+    // of marginalize_body, which reads the factor set on the host as well
+    std::vector<std::vector<uint8_t>> masks(n_windows);
+    std::vector<const uint8_t *> mp(n_windows);
+    for (int w = 0; w < n_windows; w++) {
+        const icg_ba_problem &p = problems[w];
+        const icg_ba_cull_window &c = culled[w];
+        if (!node_in_map[w] || (p.L > 0 && (!c.lm_ref_node || !c.obs_off || !c.lm_outlier)) || p.K > h->C.K || p.L > h->C.L || p.F > h->C.F ||
+            (p.L > 0 && c.obs_off[p.L] > 0 && (!c.obs_node || !c.obs_factor || !c.obs_outlier))) {
+            set_error("icg_ba_marginalize_resident_culled: window %d: arrays missing", w);
+            return ICG_EINVAL;
+        }
+        std::vector<uint8_t> &m = masks[w];
+        m.assign(p.F, 1);
+        std::vector<uint8_t> lm_bad(p.L, 0);
+        for (int l = 0; l < p.L; l++) {
+            lm_bad[l] = c.lm_outlier[l] != 0;
+            for (int o = c.obs_off[l]; o < c.obs_off[l + 1]; o++) {
+                const int f = c.obs_factor[o], k = c.obs_node[o];
+                if (f < -1 || f >= p.F || (f >= 0 && (p.f_lm[f] != l || p.f_obs[f] != k))) {
+                    set_error("icg_ba_marginalize_resident_culled: window %d landmark %d: observation %d names factor %d of another landmark or node", w, l, o, f);
+                    return ICG_EINVAL;
+                }
+                if (!c.obs_outlier[o]) continue;
+                if (k == c.lm_ref_node[l]) lm_bad[l] = 1;
+                if (f >= 0) m[f] = 0;
+            }
+        }
+        for (int f = 0; f < p.F; f++)
+            if (lm_bad[p.f_lm[f]] || !node_in_map[w][p.f_obs[f]]) m[f] = 0;
+        mp[w] = m.data();
+    }
+    return marginalize_body(h, n_windows, problems, num_marg, out, true, mp.data());
 }
 
 int icg_nccl_unique_id(uint8_t *id128) {

@@ -187,7 +187,9 @@ __global__ void __launch_bounds__(256) marg_assemble(BaCaps C, BaDev D, MargDev 
         }
         for (int p = 0; p < P; p++) {
             const int ref = pro[p] >> 8, obs = pro[p] & 255;
-            if (ref >= nm) continue;  // uniform over the CTA
+            // uniform over the CTA.  A node without columns has no marginalized factor, so the pair's Gram matrix is zero: a pair whose
+            // factors were all left out of the factor set (culled landmarks, a keyframe gone from the map) adds nothing and is skipped
+            if (ref >= nm || pose_col[ref] < 0 || pose_col[obs] < 0) continue;
             if (tid < 210) {
                 auto gcol = [&](int c) { return c < 6 ? pose_col[ref] + c : c < 12 ? pose_col[obs] + c - 6 : c < 18 ? ext_col + c - 12 : td_col; };
                 const double v = Mp[(size_t) p * 210 + tid];

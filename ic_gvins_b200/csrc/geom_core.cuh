@@ -351,6 +351,21 @@ GC_HD bool good_to_track(const icg_camera &c, float u, float v, const double *R9
     const double dx = ex, dy = ey;
     return !(sqrt(dx * dx + dy * dy) > std * 1.0);
 }
+// Tracking::isGoodToTrack(pp, pose, pw, scale, depth_scale): 1 < z < 200 * depth_scale, then |reprojectionError| <= std * scale.  err receives
+// the error when the depth passes (gvinsOutlierCulling sums it, IG/ic_gvins.cc:1066-1081).  Every test keeps the reference's sense: a NaN
+// depth fails.
+GC_HD bool good_to_track_scaled(const icg_camera &c, float u, float v, const double *R9, const double *t3, const double *pw, double std, double scale,
+                                double depth_scale, double &err) {
+    double x, y, z;
+    world2cam(R9, t3, pw, x, y, z);
+    if (!(z > 1.0 && z < 200.0 * depth_scale)) return false;
+    float pu, pv;
+    cam2pixel(c, x, y, z, pu, pv);
+    const float ex = pu - u, ey = pv - v;
+    const double dx = ex, dy = ey;
+    err = sqrt(dx * dx + dy * dy);
+    return !(err > std * scale);
+}
 
 // ------------------------------------------------------------------------------------------------ IMU preintegration propagation
 // PreintegrationEarth::resetState / integrationProcess / updateJacobianAndCovariance (IG/preintegration/preintegration_earth.cc:205-338) or, with

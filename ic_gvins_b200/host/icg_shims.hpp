@@ -242,6 +242,28 @@ public:
         std::vector<double> x0, J0, e0;               // remainedBlockData(), linearizedJacobians() (r x r row-major), linearizedResiduals()
     };
     Prior marginalization(const icg_ba_problem &problem, int num_marg, bool after_solve = false) {  // after_solve: the window this solver just optimised (no re-upload)
+        return marginalize(problem, num_marg, [&](const int32_t *nm, icg_ba_prior *o) {
+            return after_solve ? icg_ba_marginalize_resident(h_, 1, &problem, nm, o) : icg_ba_marginalize(h_, 1, &problem, nm, o);
+        });
+    }
+    // The same on the window this solver just optimised, with the factor set of the map after updateAndCull (IG/ic_gvins.cc:1558-1609):
+    // culled = that call's io (obs_factor set), node_in_map = K flags, 0 for the keyframes gvinsRemoveAllSecondNewFrame took out of the map.
+    Prior marginalization(const icg_ba_problem &problem, int num_marg, const icg_ba_cull_window &culled, const uint8_t *node_in_map) {
+        return marginalize(problem, num_marg, [&](const int32_t *nm, icg_ba_prior *o) {
+            return icg_ba_marginalize_resident_culled(h_, 1, &problem, nm, &culled, &node_in_map, o);
+        });
+    }
+
+    // updateParametersFromOptimizer + gvinsOutlierCulling (IG/ic_gvins.cc:1232-1236) on the window this solver just optimised: io carries the
+    // observation lists the caller gathered and receives pose_b_c_ / td_b_c_, every node's frame->pose(), every landmark's pos() / depth and
+    // the outlier flags (see icg_ba_cull_window); the caller applies them to its object graph.
+    void updateAndCull(const icg_ba_problem &problem, const icg_camera &camera, double reprojection_error_std, icg_ba_cull_window &io) {
+        check(icg_ba_update_and_cull_resident(h_, 1, &problem, &camera, reprojection_error_std, &io), "icg_ba_update_and_cull_resident");
+    }
+
+private:
+    template <typename Call>
+    Prior marginalize(const icg_ba_problem &problem, int num_marg, Call call) {
         Prior P;
         const int rcap = 15 * problem.K + 7;
         P.block_type.resize(2 * problem.K + 2), P.block_node.resize(2 * problem.K + 2);
@@ -249,14 +271,13 @@ public:
         icg_ba_prior o{};
         o.rcap = rcap, o.block_type = P.block_type.data(), o.block_node = P.block_node.data(), o.x0 = P.x0.data(), o.J0 = P.J0.data(), o.e0 = P.e0.data();
         const int32_t nm = num_marg;
-        check(after_solve ? icg_ba_marginalize_resident(h_, 1, &problem, &nm, &o) : icg_ba_marginalize(h_, 1, &problem, &nm, &o), "icg_ba_marginalize");
+        check(call(&nm, &o), "icg_ba_marginalize");
         P.m = o.m, P.r = o.r;
         P.block_type.resize(o.nblocks), P.block_node.resize(o.nblocks);
         P.J0.resize((size_t) o.r * o.r), P.e0.resize(o.r);
         return P;
     }
 
-private:
     icg_ba *h_ = nullptr;
 };
 

@@ -524,6 +524,58 @@ int icg_ba_marginalize(icg_ba *h, int n_windows, const icg_ba_problem *problems,
  * of that solve (n_windows equal to the uploaded count; read for the factor structure and x0 only). */
 int icg_ba_marginalize_resident(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg, icg_ba_prior *out);
 /*
+ * The rest of GVINS::gvinsOptimization after the second Solve (IG/ic_gvins.cc:1232-1236), on the windows the handle holds:
+ *   updateParametersFromOptimizer (:1299-1389)
+ *     td_b_c = ext[7] when estimate_td;  when estimate_ext: R = toRotationMatrix(Quaterniond(ext[6], ext[3..5]).normalized()), t = ext[0..2],
+ *     dt = |t - t_bc|, dr = |Quaterniond(R R_bc^T).vec()| 180 / pi; (R, t) replaces (R_bc, t_bc) unless dt > 1 || dr > 5
+ *     node k: R_c = R(q_k normalised) R_bc, t_c = p_k + R(q_k) t_bc (MISC::stateToCameraPose with the gated extrinsic, misc.cc:102-108)
+ *     landmark l: depth = 1 / invdepth (no clamp), pw = R_c(ref) (pixel2cam(ref_kp) depth) + t_c(ref)
+ *   gvinsOutlierCulling (:1035-1128), per landmark, its observations in list order:
+ *     an observation fails unless isGoodToTrack(kp, pose, pw, 3.0): 1 < z < 200 and |float(world2pixel) - kp| <= 3 std (a NaN or infinite
+ *     depth fails); a failing observation is a feature outlier; if it is in the landmark's reference node the landmark is an outlier
+ *     (reason 1) and the walk stops there.  Then, whatever the walk did: fewer than two passing observations -> reason 2, otherwise
+ *     mean of their errors (summed in list order) > std -> reason 3.
+ * Arithmetic: fixed-order sums without FMA; parity with Eigen's products and its Quaterniond(Matrix3d) is not pinned.
+ * The caller gathers, per landmark, the observations the culling visits (mappoint->observations() in that order, skipping features that
+ * are already outliers and frames that are not keyframes in the map; the reference observation included, the factors the chi-square
+ * pass removed included).  Every keyframe in the map has a time node (addNewKeyFrameTimeNode, IG/ic_gvins.cc:724-752), so every
+ * observation names a node.  Landmarks are in the problem's order (the order of invdepth); outputs are in that order too.
+ */
+typedef struct icg_ba_cull_window {
+    /* in */
+    double R_bc[9], t_bc[3], td_bc;    /* pose_b_c_ (R row-major) and td_b_c_ before the update */
+    int32_t estimate_ext, estimate_td; /* optimize_estimate_extrinsic_, optimize_estimate_td_ */
+    const int32_t *lm_ref_node;        /* L: node of mappoint->referenceFrame() */
+    const float *lm_ref_kp;            /* L x 2: mappoint->referenceKeypoint() */
+    const int32_t *obs_off;            /* L + 1, obs_off[0] = 0: landmark l owns observations obs_off[l] .. obs_off[l + 1] */
+    const int32_t *obs_node;           /* node of the observing keyframe (every keyframe in the map has one) */
+    const float *obs_kp;               /* x 2: feat->keyPoint() */
+    const int32_t *obs_factor;         /* reprojection factor (problem row) of the observation, -1 for none (the reference observation);
+                                          read by icg_ba_marginalize_resident_culled only, may be NULL for the culling */
+    /* out */
+    double R_bc_out[9], t_bc_out[3], td_bc_out; /* pose_b_c_ / td_b_c_ after the update */
+    int32_t ext_accepted;              /* 1: the estimate replaced pose_b_c_, 0: the 1 m / 5 deg gate rejected it, -1: estimate_ext is 0 */
+    double *cam_pose;                  /* K x 12: frame->pose() of every node, R row-major | t */
+    double *lm_pw, *lm_depth;          /* L x 3, L: mappoint->pos(), the depth of updateDepth */
+    uint8_t *lm_outlier;               /* L: bit 0 reason 1, bit 1 reason 2, bit 2 reason 3 (0: kept) */
+    uint8_t *obs_outlier;              /* per observation: feat->setOutlier(true) (observations after a reason-1 stop stay 0) */
+    int32_t counts[5];                 /* outliers_[0], outliers_[1], num1, num2, num3 as the reference counts them (a landmark with reason 1
+                                          and reason 2 or 3 counts twice in outliers_[0]) */
+} icg_ba_cull_window;
+/* One CTA per window; the observation lists go up in one copy through pinned staging and the outputs come back in one copy; synchronous.
+ * `problems` is the array of the solve (n_windows equal to the uploaded count; K and L are read).  The handle's state (parameters,
+ * factor activity, GNSS sigmas) is not changed.  ICG_EUNSUPPORTED on a landmark-sharded handle. */
+int icg_ba_update_and_cull_resident(icg_ba *h, int n_windows, const icg_ba_problem *problems, const icg_camera *cam, double reprojection_error_std,
+                                    icg_ba_cull_window *io);
+/* icg_ba_marginalize_resident on the map after the culling: reprojection factor f of a landmark anchored in a removed node is marginalized
+ * iff its landmark is not a culling outlier, neither its observation nor the landmark's reference observation is a feature outlier, and
+ * node_in_map[w][f_obs[f]] is set (the keyframes gvinsRemoveAllSecondNewFrame left in the map, IG/ic_gvins.cc:1391-1410): the factor set
+ * gvinsMarginalization builds (:1558-1609).  The chi-square activity plays no part (removeReprojectionFactorsByChi2 never marks a feature).
+ * culled: the io array of icg_ba_update_and_cull_resident after that call (obs_factor must be set); node_in_map: K bytes per window.  The
+ * handle's factor activity is not changed. */
+int icg_ba_marginalize_resident_culled(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg,
+                                       const icg_ba_cull_window *culled, const uint8_t *const *node_in_map, icg_ba_prior *out);
+/*
  * Landmark sharding of the window solve across the GPUs of one box (SURVEY.md 8e): every process (one per GPU) uploads the same
  * camera-side problem but only ITS landmarks and their reprojection factors; per LM attempt one NCCL sum all-reduce of the packed
  * [vision Gram matrix + gradient | Schur term | vision cost, sum rho^2] buffer (+ an n-double max / 4n-double sum) makes the
