@@ -56,6 +56,12 @@ class CullWindow(C.Structure):
                 ("cam_pose", dp), ("lm_pw", dp), ("lm_depth", dp), ("lm_outlier", bp), ("obs_outlier", bp), ("counts", C.c_int32 * 5)]
 
 
+class ReintWindow(C.Structure):
+    """ctypes image of `icg_ba_reint_window`."""
+    _fields_ = [("reintegrate", C.c_int32), ("imu", dp), ("imu_off", ip), ("status", C.POINTER(C.c_int8)), ("blob_out", dp), ("end_state10", dp),
+                ("count", C.c_int32)]
+
+
 _CULL_IN = dict(lm_ref_node=(np.int32, ip), lm_ref_kp=(np.float32, fp), obs_off=(np.int32, ip), obs_node=(np.int32, ip), obs_kp=(np.float32, fp),
                 obs_factor=(np.int32, ip))
 
@@ -329,6 +335,50 @@ class WindowSolver:
         for c, s in zip(outs, cw):
             c.update(R_bc_out=np.array(s.R_bc_out[:]).reshape(3, 3), t_bc_out=np.array(s.t_bc_out[:]), td_bc_out=s.td_bc_out, ext_accepted=s.ext_accepted,
                      counts=np.array(s.counts[:], np.int32))
+        return outs
+
+    def reintegrate(self, problems, noise5, station, imu_rows, reintegrate=None):
+        """GVINS::doReintegration (IG/ic_gvins.cc:1680-1695) on the windows this handle has just solved (icg_ba_reintegrate_resident).  noise5 =
+        gyr_arw, acc_vrw, gyr_bias_std, acc_bias_std, corr_time; station = parameters_->station (the reference leaves it at (0, 0, 0));
+        imu_rows[w] = the n_imu row arrays (m_k, 7) of window w's factors (None for a window left alone); reintegrate: per-window flags
+        (None = all).  Returns one dict per window: status (n_imu int8: 1 reintegrated, 0 gate closed, -1 not positive definite), count,
+        end_states (n_imu x 10, zero where the gate was closed) and blobs (n_imu x 480: the window's blobs with the reintegrated ones
+        replaced).  The reintegrated blobs are written into problem["imu_blob"], as the reference mutates preintegrationlist_.  A factor with
+        status -1 raises IcgError after the call; the exception's `results` holds the dicts."""
+        from ._lib import IcgError
+        if isinstance(problems, dict):
+            problems, imu_rows = [problems], [imu_rows]
+        n = len(problems)
+        flags = [1] * n if reintegrate is None else [int(bool(x)) for x in reintegrate]
+        arr = (BaProblem * n)(*[to_struct(p) for p in problems])
+        io = (ReintWindow * n)()
+        outs, keep = [], []
+        for w, p in enumerate(problems):
+            m = int(p["n_imu"])
+            o = dict(status=np.zeros(m, np.int8), count=0, end_states=np.zeros((m, 10)),
+                     blobs=np.array(np.asarray(p["imu_blob"], np.float64)[:m * IMU_BLOB].reshape(m, IMU_BLOB), copy=True))
+            outs.append(o)
+            io[w].reintegrate = flags[w] if m > 0 else 0
+            io[w].status, io[w].blob_out = o["status"].ctypes.data_as(C.POINTER(C.c_int8)), o["blobs"].ctypes.data_as(dp)
+            io[w].end_state10 = o["end_states"].ctypes.data_as(dp)
+            if io[w].reintegrate:
+                rows = [np.asarray(x, np.float64).reshape(-1, 7) for x in imu_rows[w]]
+                off = np.zeros(m + 1, np.int32)
+                off[1:] = np.cumsum([len(x) for x in rows])
+                imu = np.ascontiguousarray(np.concatenate(rows, axis=0)) if rows else np.zeros((0, 7))
+                keep.append((imu, off))
+                io[w].imu, io[w].imu_off = imu.ctypes.data_as(dp), off.ctypes.data_as(ip)
+        nz = np.ascontiguousarray(noise5, np.float64)
+        stn = np.ascontiguousarray(station, np.float64)
+        rc = lib().icg_ba_reintegrate_resident(self._h, n, arr, vp(nz.ctypes.data), vp(stn.ctypes.data), io)
+        for w, (p, o) in enumerate(zip(problems, outs)):
+            o["count"] = int(io[w].count)
+            if (o["status"] == 1).any():
+                p["imu_blob"].reshape(-1, IMU_BLOB)[:len(o["status"])][o["status"] == 1] = o["blobs"][o["status"] == 1]
+        if rc != 0:
+            err = IcgError(f"icg_ba_reintegrate_resident failed with code {rc}: {lib().icg_last_error().decode('utf-8', 'replace')}")
+            err.code, err.results = rc, outs
+            raise err
         return outs
 
     def marg_prepare(self, problems, num_marg=1, want_schur=True):

@@ -28,6 +28,7 @@ SOURCES = {
     "track.cu": ["-fmad=false"],       # trackMappoint / trackReferenceFrame on the KLT handle (geom_core.cuh arithmetic)
     "ba.cu": [],
     "ba_cull.cu": ["-fmad=false"],     # post-solve map update and outlier culling (fixed-order sums, as the numpy restatement)
+    "preint.cu": ["-fmad=false"],      # IMU propagation, warp per interval: the sums of geom_core.cuh's preintegrate_core, bit for bit
 }
 
 

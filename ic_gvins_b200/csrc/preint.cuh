@@ -1,0 +1,43 @@
+// preint.cuh -- the IMU propagation of PreintegrationEarth / PreintegrationNormal on the device, one warp per interval (preint.cu), and its
+// two front ends: the plain batch of icg_geom_imu_preintegrate_batch (geom.cu: states from the caller) and the reintegration of the factors
+// an icg_ba handle holds (ba.cu: icg_ba_reintegrate_resident, doReintegration of IG/ic_gvins.cc:1680-1695).
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+namespace icg {
+
+constexpr int PREINT_WARPS = 2;  // intervals (warps) per CTA
+
+struct PreintBatch {  // all DEVICE pointers; interval k = rows off[k] .. off[k + 1] of imu
+    int n;
+    const double *state16;  // n x 16
+    const double *iewn3;    // 3 shared, NULL: PreintegrationNormal
+    const double *gravity3, *noise5, *imu;
+    const int *off;
+    double *blobs, *ends;   // n x ICG_IMU_BLOB_DOUBLES, n x 10 (ends may be NULL)
+};
+
+struct ReintItem {  // one factor of a window the caller asked to reintegrate
+    int win, fac;    // window, factor (joins nodes fac and fac + 1)
+    int row0, nrow;  // its rows in the staged IMU rows (row0 = the sample at its start)
+};
+struct PreintResident {
+    int n;                    // items
+    const ReintItem *item;    // DEVICE
+    const double *imu;        // DEVICE, staged rows of every item
+    const double *pose, *mix; // the handle's parameters, capacity-strided by window: K x 7, K x 9
+    double *blob, *U;         // the handle's factors: K x ICG_IMU_BLOB_DOUBLES, K x 225 per window
+    int K;                    // the handle's max_K
+    double noise5[5], station[3];
+    int8_t *status;           // per item: 1 reintegrated, 0 gate closed, -1 not positive definite (factor kept)
+    double *ends;             // per item x 10: end state where status != 0
+    double *out_blob;         // compact: the status-1 blobs in completion order ...
+    int *out_item;            // ... and the item each one belongs to
+    int *counter;             // number of status-1 items (zero before the launch)
+};
+
+cudaError_t preint_batch_launch(const PreintBatch &a, cudaStream_t stream);
+cudaError_t preint_resident_launch(const PreintResident &a, cudaStream_t stream);
+
+}  // namespace icg

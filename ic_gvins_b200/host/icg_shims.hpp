@@ -261,6 +261,26 @@ public:
         check(icg_ba_update_and_cull_resident(h_, 1, &problem, &camera, reprojection_error_std, &io), "icg_ba_update_and_cull_resident");
     }
 
+    // GVINS::doReintegration (IG/ic_gvins.cc:1680-1695) on the window this solver just optimised, as gvinsOptimization calls it while the
+    // window is not full (:1223-1227).  imu = the rows (dt, dtheta[3], dvel[3]) of every factor's imu_buffer_, imu_off = n_imu + 1 offsets
+    // into them; noise5 = gyr_arw, acc_vrw, gyr_bias_std, acc_bias_std, corr_time; station = parameters_->station ((0, 0, 0) in the
+    // reference).  blobs (n_imu x ICG_IMU_BLOB_DOUBLES) is updated in place where status == 1 (the solver holds the same factors from then on);
+    // end_states (n_imu x 10, may be NULL) receives currentState() of every reintegrated factor.  Returns cnt (the factors whose gate opened).
+    int doReintegration(const icg_ba_problem &problem, const double noise5[5], const double station[3], const std::vector<double> &imu,
+                        const std::vector<int32_t> &imu_off, std::vector<int8_t> &status, std::vector<double> &blobs,
+                        std::vector<double> *end_states = nullptr) {
+        const size_t m = problem.n_imu > 0 ? (size_t) problem.n_imu : 0;
+        status.assign(m, 0);
+        blobs.resize(m * ICG_IMU_BLOB_DOUBLES);
+        if (end_states) end_states->assign(10 * m, 0.0);
+        icg_ba_reint_window io{};
+        io.reintegrate = 1, io.imu = imu.data(), io.imu_off = imu_off.data(), io.status = status.data(), io.blob_out = blobs.data();
+        io.end_state10 = end_states ? end_states->data() : nullptr;
+        if (m > 0 && imu_off.size() != m + 1) throw std::runtime_error("WindowSolver::doReintegration: imu_off needs n_imu + 1 entries");
+        check(icg_ba_reintegrate_resident(h_, 1, &problem, noise5, station, &io), "icg_ba_reintegrate_resident");
+        return io.count;
+    }
+
 private:
     template <typename Call>
     Prior marginalize(const icg_ba_problem &problem, int num_marg, Call call) {

@@ -576,6 +576,40 @@ int icg_ba_update_and_cull_resident(icg_ba *h, int n_windows, const icg_ba_probl
 int icg_ba_marginalize_resident_culled(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg,
                                        const icg_ba_cull_window *culled, const uint8_t *const *node_in_map, icg_ba_prior *out);
 /*
+ * GVINS::doReintegration (IG/ic_gvins.cc:1680-1695), which gvinsOptimization runs after the second Solve while the window is not full
+ * (:1223-1227), on the IMU factors the handle holds.  For factor k of a window (joining nodes k and k + 1):
+ *   state    stateFromData(statedatalist_[k]): node k's resident pose with q normalised (q / sqrt(x^2 + y^2 + z^2 + w^2), summed in that
+ *            order; parity with Eigen's norm reduction is not pinned) and mix (v, bg, ba), i.e. the values the last solve left
+ *   gate     |blob.bg - mix.bg| > 6 noise5[2] or |blob.ba - mix.ba| > 6 noise5[3] (blob[11..16] = deltaState().bg / ba; strict; each norm
+ *            the sqrt of the fixed-order sum of squares)
+ *   replay   reintegration(state): the whole imu_buffer_ from the new state with the factor's own form (blob[477]) and gravity
+ *            (blob[17..19]); the Earth form recomputes iewn = Earth::iewn(station3, p_k) (resetState, preintegration_earth.cc:305-324),
+ *            the Normal form keeps iewn = 0.  station3 is parameters_->station, which the reference never assigns: make_shared value-
+ *            initialises it (IG/ic_gvins.cc:91), so a faithful caller passes (0, 0, 0).
+ * A status-1 factor's blob and square-root information are replaced on the device, so every later icg_ba_marginalize_resident[_culled]
+ * and icg_ba_run[_gvins](restart = 1) sees the reintegrated factor, as the reference's next Evaluate does; the square-root information is
+ * the one icg_ba_upload computes (same code, same result bit for bit).  Parameters, factor activity and GNSS sigmas are not changed.
+ * One warp per factor; the rows go up in one copy through pinned staging, and the statuses, end states and reintegrated blobs come back
+ * (unchanged blobs do not).  Synchronous.  `problems` is the array of the solve (n_windows equal to the uploaded count; K and n_imu are
+ * read).  ICG_EINVAL before anything is launched when imu_off is not increasing by at least one row per factor; ICG_EINVAL after the call,
+ * naming the first such factor, when a reintegrated covariance is not positive definite (status -1: that factor is kept, every other one
+ * is processed).  ICG_EUNSUPPORTED on a landmark-sharded handle.
+ */
+typedef struct icg_ba_reint_window {
+    /* in */
+    int32_t reintegrate;    /* 0: the window is left alone (the reference reintegrates only while !map_->isMaximumKeframes(), :1223) */
+    const double *imu;      /* rows (dt, dtheta[3], dvel[3]) of every factor's interval (imu_buffer_ of preintegrationlist_[k]) */
+    const int32_t *imu_off; /* n_imu + 1: factor k = rows imu_off[k] .. imu_off[k + 1] - 1, row imu_off[k] = imu0 (the sample at its start) */
+    /* out */
+    int8_t *status;         /* n_imu: 1 reintegrated, 0 gate closed, -1 reintegrated covariance not positive definite (factor NOT replaced) */
+    double *blob_out;       /* n_imu x ICG_IMU_BLOB_DOUBLES: written where status == 1 only */
+    double *end_state10;    /* n_imu x 10 or NULL: currentState() p, q_xyzw, v after the replay, where status != 0 (addNewTimeNode reads the
+                               last one, :923) */
+    int32_t count;          /* cnt of :1689: factors whose gate opened (0 for windows left alone) */
+} icg_ba_reint_window;
+int icg_ba_reintegrate_resident(icg_ba *h, int n_windows, const icg_ba_problem *problems, const double *noise5, const double *station3,
+                                icg_ba_reint_window *io);
+/*
  * Landmark sharding of the window solve across the GPUs of one box (SURVEY.md 8e): every process (one per GPU) uploads the same
  * camera-side problem but only ITS landmarks and their reprojection factors; per LM attempt one NCCL sum all-reduce of the packed
  * [vision Gram matrix + gradient | Schur term | vision cost, sum rho^2] buffer (+ an n-double max / 4n-double sum) makes the
