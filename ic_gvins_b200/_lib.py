@@ -99,11 +99,10 @@ def _declare(L: C.CDLL) -> None:
     L.icg_ba_run.argtypes = [vp, C.c_int, C.c_int]
     L.icg_ba_download.argtypes = [vp, C.c_int, vp, vp]
     L.icg_ba_sync.argtypes = [vp]
-    L.icg_nccl_unique_id.argtypes = [vp]
-    L.icg_ba_set_shard.argtypes = [vp, C.c_int, C.c_int, vp]
     L.icg_ba_shard_export.argtypes = [vp, C.c_int, C.c_int, vp]
     L.icg_ba_shard_connect.argtypes = [vp, vp]
     L.icg_ba_shard_error.argtypes = [vp]
+    L.icg_ba_shard_leave.argtypes = [vp]
     L.icg_ba_gvins_optimization.argtypes = [vp, C.c_int, vp, C.c_int, vp, vp]
     L.icg_ba_run_gvins.argtypes = [vp, C.c_int, C.c_int]
     L.icg_ba_gvins_optimization_begin.argtypes = [vp, C.c_int, vp, C.c_int]
@@ -153,5 +152,5 @@ EXPORTS = [
     "icg_geom_find_fundamental_mat_ransac_batch", "icg_klt_track_frames_dev", "icg_klt_track_frame",
     "icg_klt_triangulate_dev", "icg_klt_triangulate",
     "icg_imu_preintegrate", "icg_ba_create", "icg_ba_destroy", "icg_ba_solve", "icg_ba_upload", "icg_ba_run", "icg_ba_download",
-    "icg_ba_sync", "icg_nccl_unique_id", "icg_ba_set_shard", "icg_ba_shard_export", "icg_ba_shard_connect", "icg_ba_shard_error", "icg_ba_gvins_optimization", "icg_ba_run_gvins", "icg_ba_gvins_optimization_begin", "icg_ba_gvins_optimization_end", "icg_ba_residual_costs", "icg_ba_reproj_evaluate", "icg_ba_imu_evaluate", "icg_ba_marginalize", "icg_ba_marginalize_resident", "icg_ba_update_and_cull_resident", "icg_ba_marginalize_resident_culled", "icg_ba_reintegrate_resident", "icg_ba_gnss_evaluate", "icg_ba_pose_prior_evaluate", "icg_ba_mix_prior_evaluate", "icg_ba_imu_error_evaluate", "icg_ba_marg_factor_evaluate",
+    "icg_ba_sync", "icg_ba_shard_export", "icg_ba_shard_connect", "icg_ba_shard_error", "icg_ba_shard_leave", "icg_ba_gvins_optimization", "icg_ba_run_gvins", "icg_ba_gvins_optimization_begin", "icg_ba_gvins_optimization_end", "icg_ba_residual_costs", "icg_ba_reproj_evaluate", "icg_ba_imu_evaluate", "icg_ba_marginalize", "icg_ba_marginalize_resident", "icg_ba_update_and_cull_resident", "icg_ba_marginalize_resident_culled", "icg_ba_reintegrate_resident", "icg_ba_gnss_evaluate", "icg_ba_pose_prior_evaluate", "icg_ba_mix_prior_evaluate", "icg_ba_imu_error_evaluate", "icg_ba_marg_factor_evaluate",
 ]

@@ -139,27 +139,16 @@ def merge_shard(prob: dict, shard: dict) -> None:
 
 
 def connect_shards(solver: "WindowSolver", rank: int, world: int, transport: str, dist) -> None:
-    """Join `solver` to the landmark-shard group of `world` processes (one per GPU).  `dist` is an initialised torch.distributed module
-    (any backend): it only carries the rendezvous blobs -- the ncclUniqueId for transport "nccl", the CUDA IPC handles of the exchange
-    buffers for transport "p2p" (peer-memory stores over NVLink, no NCCL on the data path)."""
-    if transport == "nccl":
-        ids = [nccl_unique_id() if rank == 0 else None]
-        dist.broadcast_object_list(ids, src=0)
-        solver.set_shard(rank, world, ids[0])
-    elif transport == "p2p":
-        mine = solver.shard_export(rank, world)
-        blobs = [None] * world
-        dist.all_gather_object(blobs, mine)
-        solver.shard_connect(blobs)
-        dist.barrier()
-    else:
-        raise ValueError(transport)
-
-
-def nccl_unique_id() -> bytes:
-    buf = (C.c_uint8 * 128)()
-    check(lib().icg_nccl_unique_id(buf), "icg_nccl_unique_id")
-    return bytes(buf)
+    """Join `solver` to the landmark-shard group of `world` processes (one per GPU) over peer memory (transport "p2p": each rank stores
+    its reduction operand into the window owner's buffer over NVLink; the only transport).  `dist` is an initialised torch.distributed
+    module (any backend): it only carries the rendezvous blobs, the CUDA IPC handles of the exchange buffers."""
+    if transport != "p2p":
+        raise ValueError(f"unknown landmark-shard transport {transport!r} (only 'p2p')")
+    mine = solver.shard_export(rank, world)
+    blobs = [None] * world
+    dist.all_gather_object(blobs, mine)
+    solver.shard_connect(blobs)
+    dist.barrier()
 
 
 def imu_preintegrate(state16, iewn, gravity, noise5, imu):
@@ -194,11 +183,6 @@ class WindowSolver:
         except Exception:
             pass
 
-    def set_shard(self, rank: int, world: int, unique_id: bytes | None = None):
-        """Make this handle solve landmark shard `rank` of `world` (one process per GPU; NCCL all-reduce per LM attempt)."""
-        buf = (C.c_uint8 * 128)(*unique_id) if unique_id else None
-        check(lib().icg_ba_set_shard(self._h, rank, world, buf), "icg_ba_set_shard")
-
     def shard_export(self, rank: int, world: int) -> bytes:
         """Allocate this rank's peer-memory exchange buffer for a group of `world` ranks; returns the blob the other ranks need."""
         buf = (C.c_uint8 * 128)()
@@ -210,6 +194,10 @@ class WindowSolver:
         raw = b"".join(blobs)
         buf = (C.c_uint8 * len(raw)).from_buffer_copy(raw)
         check(lib().icg_ba_shard_connect(self._h, buf), "icg_ba_shard_connect")
+
+    def shard_leave(self) -> None:
+        """Leave the landmark-shard group: the handle solves whole windows on its own GPU again, like a fresh handle of its capacities."""
+        check(lib().icg_ba_shard_leave(self._h), "icg_ba_shard_leave")
 
     def solve(self, problems, max_num_iterations: int):
         """ceres::Solver::Solve on a list of problem dicts (updated in place).  Returns a list of summaries."""

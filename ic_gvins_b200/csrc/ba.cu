@@ -16,20 +16,18 @@
 //                lanes / landmark -> h_l, g_l and the dense coupling row w_l (A_W, landmark-major)
 //   schur_dmma : cluster of 4 CTAs / window: sum_l phi_l w_l w_l^T with phi_l = s_l^2 / (s_l^2 h_l + D_l^2) on the FP64 tensor cores, one
 //                landmark split per CTA, the partials summed over DSMEM; epilogue: one-writer-per-entry gather of the pair Gram matrices
-//                into the vision part of H_cc and g_c -> Hs = H_c + H_vis - Schur term and the solve's vision vectors (or the export /
-//                all-reduce payload of a landmark shard)
+//                into the vision part of H_cc and g_c -> Hs = H_c + H_vis - Schur term and the solve's vision vectors (or the split
+//                pipeline's export payload)
 //   lin_cam    : one CTA / window (second stream, beside the vision chain) -> IMU preintegration, GNSS, bias, prior and
 //                marginalization factors -> H_c, g_c
 //   solve      : one CTA / window -> Jacobi scaling, LM diagonal, S = s(H - Schur)s + D^2, packed Cholesky in shared memory
 //                (panel updates on DMMA), triangular solves, landmark back-substitution, model cost change, candidate x (+) delta
 //   single GPU : lin_vis + lin_cam at the candidate, into the window's second linearisation buffer (its costs are the candidate cost)
-//   cost       : candidate cost (all factors, residuals only) of the split / NCCL pipelines;   accept : Ceres step acceptance + radius update
+//   cost       : candidate cost (all factors, residuals only) of the split pipeline;   accept : Ceres step acceptance + radius update
 //   ba_marg.cuh: sliding-window marginalization (MarginalizationInfo) on the same device-resident linearisation
 #include <cooperative_groups.h>
-#include <dlfcn.h>
 #include <unistd.h>
 #include <math.h>
-#include <nccl.h>
 #include <stdlib.h>
 #include <string.h>
 
@@ -109,7 +107,7 @@ struct BaDev {  // device pointers (flat, capacity-strided by window)
     int *vis_cnt;        // [NW][K] lin_vis runs of the reference node arrived (the last one resets it)
     // Linearisation buffers: everything a linearisation writes and a later iteration reads comes in two copies, selected per window by
     // LmState::lin_buf through the lin_* helpers below.  The single-GPU pipeline linearises the candidate into the copy the window is not
-    // using and flips lin_buf when ba_accept takes the step; the split and NCCL pipelines never flip it and have copy 0 only.
+    // using and flips lin_buf when ba_accept takes the step; the split pipeline never flips it and has copy 0 only.
     double *Mp[2];         // per-pair 20x20 Gram matrices (upper, 210 entries)
     double *AW[2];         // Schur SYRK input
     double *costf[2];      // per-factor cost
@@ -125,9 +123,7 @@ struct BaDev {  // device pointers (flat, capacity-strided by window)
     int *marg_type, *marg_node;
     double *marg_x0, *marg_H0, *marg_b0, *marg_c0;
     double *cost_part;  // [NW][ncost_blocks]
-    double *red;        // [NW][2*NCA*NCA + 8]: vision Gram | Schur term | scalars -- the operand of the landmark-shard all-reduce
-    double *redmax;     // [NW] max |g_l| over the local landmarks (max-reduced)
-    double *red2;       // [NW][4]: model cost change, step norm^2, non-finite count, candidate cost (sum-reduced)
+    double *red2;       // [NW][4]: model cost change, step norm^2, non-finite count of the step (+ the split pipeline's fourth exchanged partial)
     int rank, world;    // landmark shard of this process (camera-only terms are counted on rank 0 only)
     double *step_c, *step_l;
     double *Sglobal;    // fallback Cholesky workspace when the packed system does not fit shared memory
@@ -448,14 +444,12 @@ __device__ __forceinline__ int tri_idx(int A, int B, int ncv);
 // pipeline that drives the handle reads.
 //   single GPU (fused pipeline): Hs = H_c + (cj - cw) on the vision rows (lower triangle) and D.visv = [diag H_vis | g_vis | W phi g_l];
 //   split pipeline: [tri(H_vis - Schur) | diag H_vis | g_vis | W phi g_l] straight into the owner's inbox (P2P stores; ba_signal publishes
-//                   them, the owner's ba_reduce sums the ranks);
-//   NCCL landmark shards: [H_vis g_vis | Schur term] stored symmetric in D.red, all-reduced, then turned into Hs by ba_hsum.
+//                   them, the owner's ba_reduce sums the ranks).
 __device__ __forceinline__ void schur_store(const BaCaps &C, const BaDev &D, int buf, int w, int K, const short *s_slot, int A, int B, double cw) {
     const int NCV = 6 * K + 7;
-    const bool nccl = !D.S.split && D.world > 1;
-    if (A == NCV && !nccl) return;  // the r^T r corner: only the all-reduced buffer carries it
+    if (A == NCV) return;  // the r^T r corner: no solve reads it
     const size_t e = (size_t) w * C.NS * C.NS + (size_t) B * C.NS + A;
-    const double hc = !D.S.split && !nccl && B < NCV ? lin_Hc(C, D, buf, w)[(size_t) B * C.NS + A] : 0.0;  // in flight during the gather
+    const double hc = !D.S.split && B < NCV ? lin_Hc(C, D, buf, w)[(size_t) B * C.NS + A] : 0.0;  // in flight during the gather
     const double cj = gram2_entry(C, D, buf, w, K, s_slot, A, B);
     if (D.S.split) {
         double *P = x_inbox(D, w % D.world, w, D.rank);
@@ -467,11 +461,6 @@ __device__ __forceinline__ void schur_store(const BaCaps &C, const BaDev &D, int
             P[TRI + NCV + A] = cj;       // g_vis
             P[TRI + 2 * NCV + A] = cw;   // W phi g_l
         }
-    } else if (nccl) {
-        const size_t NN = (size_t) C.NCA * C.NCA;
-        double *R = D.red + (size_t) w * (2 * NN + 8);
-        R[(size_t) A * C.NCA + B] = R[(size_t) B * C.NCA + A] = cj;
-        R[NN + (size_t) A * C.NCA + B] = R[NN + (size_t) B * C.NCA + A] = cw;
     } else {
         double *V = D.visv + (size_t) w * 3 * C.NCV;
         if (B < NCV) {
@@ -483,11 +472,11 @@ __device__ __forceinline__ void schur_store(const BaCaps &C, const BaDev &D, int
     }
 }
 
-// the scalars of the split / NCCL payloads: vision cost, sum rho^2 and max |g_l| over this rank's factors and landmarks (one CTA)
+// the scalars of the split payload: vision cost, sum rho^2 and max |g_l| over this rank's factors and landmarks (one CTA)
 __device__ __forceinline__ void schur_scalars(const BaCaps &C, const BaDev &D, int w, const WinDims &dm, double *s_red) {
     const int tid = threadIdx.x;
     double c = 0, q = 0, gm = 0;
-    const double *costf = lin_costf(C, D, 0, w), *gl = lin_gl(C, D, 0, w);  // these pipelines use buffer 0 only
+    const double *costf = lin_costf(C, D, 0, w), *gl = lin_gl(C, D, 0, w);  // the split pipeline uses buffer 0 only
     for (int f = tid; f < dm.F; f += 256) c += costf[f];
     for (int l = tid; l < dm.L; l += 256) {
         const double r = D.rho[(size_t) w * C.L + l];
@@ -498,17 +487,9 @@ __device__ __forceinline__ void schur_scalars(const BaCaps &C, const BaDev &D, i
     q = block_sum(q, s_red);
     gm = block_max(gm, s_red);
     if (tid != 0) return;
-    if (D.S.split) {
-        const int NCV = 6 * dm.K + 7, TRI = NCV * (NCV + 1) / 2;
-        double *P = x_inbox(D, w % D.world, w, D.rank);
-        P[TRI + 3 * NCV] = c, P[TRI + 3 * NCV + 1] = q, P[TRI + 3 * NCV + 2] = gm;
-    } else {
-        const size_t NN = (size_t) C.NCA * C.NCA;
-        double *R = D.red + (size_t) w * (2 * NN + 8);
-        R[2 * NN] = c, R[2 * NN + 1] = q;
-        for (int k = 2; k < 8; k++) R[2 * NN + k] = 0;
-        D.redmax[w] = gm;
-    }
+    const int NCV = 6 * dm.K + 7, TRI = NCV * (NCV + 1) / 2;
+    double *P = x_inbox(D, w % D.world, w, D.rank);
+    P[TRI + 3 * NCV] = c, P[TRI + 3 * NCV + 1] = q, P[TRI + 3 * NCV + 2] = gm;
 }
 
 // Schur SYRK on the FP64 tensor cores: the sum over the window's landmarks of phi_l w_l w_l^T, with
@@ -650,7 +631,7 @@ __global__ void __cluster_dims__(BA_SPLIT_W, 1, 1) __launch_bounds__(256) ba_sch
             if (r <= cc && cc <= NCV) schur_store(C, D, b, w, dm.K, s_slot, r, cc, cw[j]);
         }
     }
-    if (split == 0 && (D.S.split || D.world > 1)) schur_scalars(C, D, w, dm, s_red);
+    if (split == 0 && D.S.split) schur_scalars(C, D, w, dm, s_red);
     cluster.barrier_wait();  // no CTA leaves while a peer may still read its shared memory
 }
 
@@ -924,40 +905,6 @@ __global__ void __launch_bounds__(CAM_THREADS) ba_lin_cam(BaCaps C, BaDev D, int
     if (threadIdx.x == 0) st.cost_cam[b] = c;
 }
 
-// ------------------------------------------------------------------------------------------------ reduction operands
-// Everything a landmark shard contributes to the window's reduced camera system goes into ONE contiguous buffer per window (written by
-// ba_schur_dmma), so that a sharded solve needs a single all-reduce (sum) per attempt: [H_vis g_vis | Schur term | vision cost, sum rho^2].
-__global__ void ba_pack2(BaCaps C, BaDev D, int n, int nblk_vis) {
-    const int w = blockIdx.x * blockDim.x + threadIdx.x;
-    if (w >= n) return;
-    const LmState &st = D.st[w];
-    if (st.done || !st.step_valid) return;
-    const WinDims dm = D.dims[w];
-    const double *part = D.cost_part + (size_t) w * (nblk_vis + 1);
-    double cand = 0;
-    const int nb = (dm.F + 255) / 256;
-    for (int b = 0; b < nb; b++) cand += part[b];
-    if (D.rank == 0) cand += part[nblk_vis];  // camera-only factors are replicated on every shard: count them once
-    D.red2[(size_t) w * 4 + 3] = cand;
-}
-
-// ------------------------------------------------------------------------------------------------ reduced camera matrix
-// Hs = H_c + H_vis - Schur term of a landmark-sharded window (NCCL transport) from the all-reduced buffer, lower triangle, one thread per
-// entry (ba_solve then reads ONE operand per entry).  A single GPU's Hs is formed by ba_schur_dmma's epilogue.
-__global__ void __launch_bounds__(256) ba_hsum(BaCaps C, BaDev D) {
-    const int w = blockIdx.y;
-    if (D.st[w].done) return;
-    const int K = D.dims[w].K, NCV = 6 * K + 7, nn = NCV + 1;
-    const int NN = C.NCA * C.NCA;
-    const int t = blockIdx.x * 256 + threadIdx.x;
-    if (t >= nn * nn) return;
-    const int A = t / nn, B = t - A * nn;  // A <= B: entry (row B, column A) of the lower triangle
-    if (B < A || B >= NCV) return;
-    const double *RED = D.red + (size_t) w * (2 * NN + 8);
-    const double cj = RED[(size_t) B * C.NCA + A], cw = RED[NN + (size_t) B * C.NCA + A];
-    D.Hs[(size_t) w * C.NS * C.NS + (size_t) B * C.NS + A] = lin_Hc(C, D, 0, w)[(size_t) B * C.NS + A] + (cj - cw);
-}
-
 // ------------------------------------------------------------------------------------------------ solve (one CTA per window)
 constexpr int SOLVE_THREADS = 256;  // 2 CTAs (windows) per SM: 107 KB shared memory and <= 128 registers each
 
@@ -1031,15 +978,8 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
     double *S = s_diag + C.NS;
     const int b = st.lin_buf;
     const double *Hc = lin_Hc(C, D, b, w), *gcam = lin_gc(C, D, b, w), *Hs = D.Hs + (size_t) w * C.NS * C.NS;
-    // Vision vectors [diag H_vis | g_vis | W phi g_l] (a < NCV).  Landmark-sharded solve: the packed, all-reduced buffer (identical on every
-    // shard).  Single GPU: the vectors ba_schur_dmma's epilogue wrote.
-    const bool sharded = D.world > 1;
-    const int NN = C.NCA * C.NCA;
-    const double *RED = D.red + (size_t) w * (2 * NN + 8), *V = D.visv + (size_t) w * 3 * C.NCV;
-    auto hvis_diag = [&](int a) { return sharded ? RED[(size_t) a * C.NCA + a] : V[a]; };
-    auto g_vis = [&](int a) { return sharded ? RED[(size_t) a * C.NCA + NCV] : V[NCV + a]; };
-    auto wphig = [&](int a) { return sharded ? RED[NN + (size_t) a * C.NCA + NCV] : V[2 * NCV + a]; };
-    const double camw = D.rank == 0 ? 1.0 : 0.0;       // camera-side partial sums are counted on shard 0 only
+    // Vision vectors [diag H_vis | g_vis | W phi g_l] (a < NCV), as ba_schur_dmma's epilogue wrote them.
+    const double *V = D.visv + (size_t) (3 * C.NCV) * w;
     if (tid == 0 && st.need_lin) st.need_lin = 0;      // the linearisation kernels of this iteration have run (stream order)
     double *scale_c = D.scale_c + (size_t) w * C.NS;
     const double *hl = lin_hl(C, D, b, w), *gl = lin_gl(C, D, b, w), *scale_l = D.scale_l + (size_t) w * C.L;
@@ -1047,10 +987,10 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
     // ---- after a fresh linearisation: total cost, gradient, (first time) Jacobi scaling
     for (int a = tid; a < N; a += SOLVE_THREADS) {
         double g = gcam[a];
-        if (a < NCV) g += g_vis(a);
+        if (a < NCV) g += V[NCV + a];
         s_g[a] = g;
         if (f_first) {
-            double h = Hc[(size_t) a * C.NS + a] + (a < NCV ? hvis_diag(a) : 0.0);
+            double h = Hc[(size_t) a * C.NS + a] + (a < NCV ? V[a] : 0.0);
             scale_c[a] = 1.0 / (1.0 + sqrt(h));
         }
     }
@@ -1058,18 +998,11 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
     for (int a = tid; a < N; a += SOLVE_THREADS) s_scale[a] = scale_c[a];
     double gmax_now = st.gmax;
     if (f_fresh) {
-        double c, gml;
-        if (sharded) {
-            c = RED[2 * NN];  // vision cost, summed over the landmark shards
-            gml = D.redmax[w];
-        } else {
-            double cs = 0, gq = 0;
-            const double *costf = lin_costf(C, D, b, w);
-            for (int f = tid; f < dm.F; f += SOLVE_THREADS) cs += costf[f];
-            for (int l = tid; l < L; l += SOLVE_THREADS) gq = fmax(gq, fabs(gl[l]));
-            c = block_sum(cs, s_red);
-            gml = block_max(gq, s_red);
-        }
+        double cs = 0, gq = 0;
+        const double *costf = lin_costf(C, D, b, w);
+        for (int f = tid; f < dm.F; f += SOLVE_THREADS) cs += costf[f];
+        for (int l = tid; l < L; l += SOLVE_THREADS) gq = fmax(gq, fabs(gl[l]));
+        const double c = block_sum(cs, s_red), gml = block_max(gq, s_red);
         double gm = 0;
         for (int a = tid; a < N; a += SOLVE_THREADS) gm = fmax(gm, fabs(s_g[a]));
         gm = fmax(block_max(gm, s_red), gml);
@@ -1118,10 +1051,10 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
         asm volatile("cp.async.commit_group;" ::: "memory");
     }
     for (int a = tid; a < N; a += SOLVE_THREADS) {
-        double h = Hc[(size_t) a * C.NS + a] + (a < NCV ? hvis_diag(a) : 0.0);
+        double h = Hc[(size_t) a * C.NS + a] + (a < NCV ? V[a] : 0.0);
         double hs = s_scale[a] * s_scale[a] * h;
         s_d2[a] = fmin(fmax(hs, 1e-6), 1e32) / radius;
-        double gw = a < NCV ? wphig(a) : 0.0;
+        double gw = a < NCV ? V[2 * NCV + a] : 0.0;
         s_rhs[a] = -s_scale[a] * (s_g[a] - gw);
     }
     if (async_fill) asm volatile("cp.async.wait_all;" ::: "memory");
@@ -1374,17 +1307,17 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
     bool finite = true;
     double *R2 = D.red2 + (size_t) w * 4;
     if (!valid) {
-        // Cholesky breakdown (identical on every shard): the step is invalid; ba_accept applies HandleInvalidStep
+        // Cholesky breakdown: the step is invalid; ba_accept applies HandleInvalidStep
         if (tid == 0) {
             st.chol_ok = 0, st.step_valid = 0;
-            R2[0] = 0, R2[1] = 0, R2[2] = 1, R2[3] = 0;
+            R2[0] = 0, R2[1] = 0, R2[2] = 1;
         }
         return;
     }
     for (int a = tid; a < N; a += SOLVE_THREADS) {
         double sp = s_rhs[a];
         finite = finite && isfinite(sp);
-        part += camw * (-0.5 * sp * (s_scale[a] * s_g[a]) + 0.5 * s_d2[a] * sp * sp);
+        part += -0.5 * sp * (s_scale[a] * s_g[a]) + 0.5 * s_d2[a] * sp * sp;
     }
     // landmark back-substitution: one warp per landmark, the coupling row is read coalesced (two landmarks in flight per warp)
     double *s_sx = s_diag;  // s_diag is dead after the back-substitution: scaled camera step s_c * step'_c
@@ -1448,7 +1381,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
     SOLVE_CLK(4)  // landmark back-substitution
     const double mcc = block_sum(part, s_red);
     const double nfin = block_sum(finite ? 0.0 : 1.0, s_red);
-    // ---- candidate point x (+) delta, delta = step' * scale; |x - x_cand|^2 over active blocks (camera part counted on shard 0)
+    // ---- candidate point x (+) delta, delta = step' * scale; |x - x_cand|^2 over active blocks
     const double *pose = D.pose + (size_t) w * C.K * 7, *mix = D.mix + (size_t) w * C.K * 9, *ext = D.ext + (size_t) w * 8, *rho = D.rho + (size_t) w * C.L;
     double *pose_c = D.pose_c + (size_t) w * C.K * 7, *mix_c = D.mix_c + (size_t) w * C.K * 9, *ext_c = D.ext_c + (size_t) w * 8, *rho_c = D.rho_c + (size_t) w * C.L;
     double sn = 0;
@@ -1463,14 +1396,14 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
             double d[6];
             for (int e = 0; e < 6; e++) d[e] = s_rhs[c0 + e] * s_scale[c0 + e];
             pose_plus(x, d, xc);
-            for (int e = 0; e < 7; e++) sn += camw * (x[e] - xc[e]) * (x[e] - xc[e]);
+            for (int e = 0; e < 7; e++) sn += (x[e] - xc[e]) * (x[e] - xc[e]);
         }
     }
     for (int e = tid; e < K * 9; e += SOLVE_THREADS) {
         int k = e / 9, q = e - 9 * k, c = col_mix(K, k) + q;
         double v = mix[e] + s_rhs[c] * s_scale[c];
         mix_c[e] = v;
-        sn += camw * (mix[e] - v) * (mix[e] - v);
+        sn += (mix[e] - v) * (mix[e] - v);
     }
     if (tid == 0) {
         if (dm.td_const) {
@@ -1478,7 +1411,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
         } else {
             double v = ext[7] + s_rhs[col_td(K)] * s_scale[col_td(K)];
             ext_c[7] = v;
-            sn += camw * (ext[7] - v) * (ext[7] - v);
+            sn += (ext[7] - v) * (ext[7] - v);
         }
     }
     for (int l = tid; l < L; l += SOLVE_THREADS) {
@@ -1489,7 +1422,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
     sn = block_sum(sn, s_red);
     if (tid == 0) {
         st.chol_ok = 1, st.step_valid = 1;  // provisional: ba_accept validates with the reduced model cost change
-        R2[0] = mcc, R2[1] = sn, R2[2] = nfin, R2[3] = 0;
+        R2[0] = mcc, R2[1] = sn, R2[2] = nfin;
     }
     SOLVE_CLK(5)  // candidate point, reductions
 #undef SOLVE_CLK
@@ -1497,7 +1430,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
 #undef SOLVE_CLK_ADD
 }
 
-// ------------------------------------------------------------------------------------------------ candidate cost (split / NCCL pipelines)
+// ------------------------------------------------------------------------------------------------ candidate cost (split pipeline)
 // The single-GPU pipeline takes the candidate cost from the linearisation at the candidate instead (ba_accept).
 // camera-only factors at the candidate point (one CTA per window; runs beside the vision blocks on the handle's second stream)
 __global__ void __launch_bounds__(CAM_THREADS) ba_cost_cam(BaCaps C, BaDev D, int nblk_vis) {
@@ -1548,9 +1481,8 @@ __global__ void __launch_bounds__(128) ba_accept(BaCaps C, BaDev D) {
     LmState &st = D.st[w];
     if (st.done) return;
     const WinDims dm = D.dims[w];
-    const int chol_ok = st.chol_ok;
     const double *R2 = D.red2 + (size_t) w * 4;
-    // |x|^2 of the camera-side blocks (replicated on every shard); the landmark part comes from the reduced operand
+    // |x|^2 of the camera-side blocks and of the landmarks
     {
         const double *pose = D.pose + (size_t) w * C.K * 7, *mix = D.mix + (size_t) w * C.K * 9, *ext = D.ext + (size_t) w * 8;
         double s = 0;
@@ -1559,25 +1491,19 @@ __global__ void __launch_bounds__(128) ba_accept(BaCaps C, BaDev D) {
         if (tid < 7 && !dm.ext_const) s += ext[tid] * ext[tid];
         if (tid == 7 && !dm.td_const) s += ext[7] * ext[7];
         s = block_sum(s, s_red);
-        double q = 0;  // |rho|^2: from the reduced operand when the landmarks are sharded
-        if (D.world == 1) {
-            for (int l = tid; l < dm.L; l += 128) q += D.rho[(size_t) w * C.L + l] * D.rho[(size_t) w * C.L + l];
-            q = block_sum(q, s_red);
-        } else {
-            q = D.red[(size_t) w * (2 * C.NCA * C.NCA + 8) + 2 * C.NCA * C.NCA + 1];
-        }
+        double q = 0;  // |rho|^2
+        for (int l = tid; l < dm.L; l += 128) q += D.rho[(size_t) w * C.L + l] * D.rho[(size_t) w * C.L + l];
+        q = block_sum(q, s_red);
         if (tid == 0) s_camsq = s, s_rhosq = q;
     }
-    // Single GPU: the candidate cost from the linearisation at the candidate (buffer 1 - lin_buf), summed in ba_cost's order -- per 256 record
-    // slots block_sum's tree (warp k sums slots [32 k, 32 k + 32) of the block, then the eight warp sums in order), the blocks in order, then
-    // the camera-only cost -- so that every decision below matches the sum of ba_cost's partials bit for bit.  Landmark shards receive the
-    // all-reduced candidate cost in R2[3] (ba_pack2).
+    // The candidate cost from the linearisation at the candidate (buffer 1 - lin_buf), summed in ba_cost's order -- per 256 record slots
+    // block_sum's tree (warp k sums slots [32 k, 32 k + 32) of the block, then the eight warp sums in order), the blocks in order, then the
+    // camera-only cost -- so that every decision below matches the sum of ba_cost's partials bit for bit.
     // s_warp (dynamic, 8 per 256 slots): the sums of the 32-slot groups; warp k of this CTA reduces groups k, k + 4, ... with no barrier in
     // between, so that the loads of several groups are in flight together.
     extern __shared__ double s_warp[];
     const int lane = tid & 31, warp = tid >> 5, ngrp = (dm.F + 31) / 32;
-    const bool cand_here = D.world == 1 && st.step_valid;
-    if (cand_here) {
+    if (st.step_valid) {
         const double *costf = lin_costf(C, D, 1 - st.lin_buf, w);
         const int4 *meta = (const int4 *) D.f_meta_s + (size_t) w * C.F;  // (landmark, reference node, observing node, factor id) per slot
 #pragma unroll 4
@@ -1592,9 +1518,8 @@ __global__ void __launch_bounds__(128) ba_accept(BaCaps C, BaDev D) {
     if (tid == 0) {
         s_accept = 0;
         const double mcc = R2[0], sn = R2[1], nfin = R2[2];
-        double cand = R2[3];
-        if (cand_here) {
-            cand = 0;
+        double cand = 0;
+        if (st.step_valid) {
             for (int g0 = 0; g0 < ngrp; g0 += 8) {
                 double t = 0;
                 for (int k = 0; k < 8; k++) t += g0 + k < ngrp ? s_warp[g0 + k] : 0.0;
@@ -1602,7 +1527,7 @@ __global__ void __launch_bounds__(128) ba_accept(BaCaps C, BaDev D) {
             }
             cand += st.cost_cam[1 - st.lin_buf];
         }
-        if (!chol_ok || nfin != 0.0 || !(mcc > 0.0)) {
+        if (!st.chol_ok || nfin != 0.0 || !(mcc > 0.0)) {
             // HandleInvalidStep + LevenbergMarquardtStrategy::StepIsInvalid
             st.step_valid = 0;
             st.n_invalid++;
@@ -1631,10 +1556,7 @@ __global__ void __launch_bounds__(128) ba_accept(BaCaps C, BaDev D) {
                     st.decrease_factor = 2.0;
                     st.last_success = 1;
                     st.fresh_lin = 1;
-                    if (D.world == 1)
-                        st.lin_buf ^= 1;  // the candidate's linearisation is now the one at x
-                    else
-                        st.need_lin = 1;
+                    st.lin_buf ^= 1;  // the candidate's linearisation is now the one at x
                 } else {
                     // StepRejected
                     st.radius = st.radius / st.decrease_factor;
@@ -1861,7 +1783,6 @@ struct icg_ba {
     HostDev<double> scratch;  // single-factor evaluation
     HostDev<LmState> st_save;   // pass-1 LM state of the two-pass protocol
     HostDev<int> cull_counters; // per window: reprojection factors removed, GNSS fixes re-weighted
-    void *comm = nullptr;       // ncclComm_t when this handle solves a landmark shard (transport "nccl")
     // split pipeline (ba_split.cuh): exchange buffer of this rank, peers' buffers opened through CUDA IPC, epoch counter of the flags
     double *xbuf = nullptr;
     size_t xbuf_doubles = 0;
@@ -1908,42 +1829,6 @@ static int dmalloc(icg_ba *h, double **p, size_t n) {
     }
     cudaMemsetAsync(*p, 0, sizeof(double) * n, h->stream);
     h->dev_only.push_back(*p);
-    return ICG_OK;
-}
-
-// ---- NCCL, loaded at run time (only landmark-sharded solves need it; the KLT / single-GPU paths never touch it)
-namespace {
-struct NcclApi {
-    void *lib = nullptr;
-    ncclResult_t (*GetUniqueId)(ncclUniqueId *) = nullptr;
-    ncclResult_t (*CommInitRank)(ncclComm_t *, int, ncclUniqueId, int) = nullptr;
-    ncclResult_t (*AllReduce)(const void *, void *, size_t, ncclDataType_t, ncclRedOp_t, ncclComm_t, cudaStream_t) = nullptr;
-    ncclResult_t (*CommDestroy)(ncclComm_t) = nullptr;
-    const char *(*GetErrorString)(ncclResult_t) = nullptr;
-};
-NcclApi &nccl_api() {
-    static NcclApi api;
-    if (!api.lib) {
-        api.lib = dlopen("libnccl.so.2", RTLD_NOW | RTLD_GLOBAL);
-        if (api.lib) {
-            api.GetUniqueId = (decltype(api.GetUniqueId)) dlsym(api.lib, "ncclGetUniqueId");
-            api.CommInitRank = (decltype(api.CommInitRank)) dlsym(api.lib, "ncclCommInitRank");
-            api.AllReduce = (decltype(api.AllReduce)) dlsym(api.lib, "ncclAllReduce");
-            api.CommDestroy = (decltype(api.CommDestroy)) dlsym(api.lib, "ncclCommDestroy");
-            api.GetErrorString = (decltype(api.GetErrorString)) dlsym(api.lib, "ncclGetErrorString");
-        }
-    }
-    return api;
-}
-}  // namespace
-
-static int nccl_allreduce(icg_ba *h, double *buf, size_t count, int op_max) {
-    NcclApi &a = nccl_api();
-    ncclResult_t r = a.AllReduce(buf, buf, count, ncclDouble, op_max ? ncclMax : ncclSum, (ncclComm_t) h->comm, h->stream);
-    if (r != ncclSuccess) {
-        set_error("ncclAllReduce failed: %s", a.GetErrorString ? a.GetErrorString(r) : "?");
-        return ICG_ENCCL;
-    }
     return ICG_OK;
 }
 
@@ -2067,7 +1952,7 @@ static int ba_create_body(icg_ba *h, int max_windows, int max_K, int max_L, int 
     DM(pose_0, NW * C.K * 7) DM(mix_0, NW * C.K * 9) DM(ext_0, NW * 8) DM(rho_0, NW * C.L)
     DM(AW[0], NW * C.NCA * C.LP) DM(Mp[0], NW * (size_t) C.K * (C.K - 1) * 210) DM(visv, NW * 3 * C.NCV)
     DM(gpart, NW * (size_t) C.GQ * 210) DM(costf[0], NW * C.F) DM(hl[0], NW * C.L) DM(gl[0], NW * C.L) DM(scale_l, NW * C.L) DM(scale_c, NW * C.NS)
-    DM(Hc[0], NW * C.NS * C.NS) DM(gc[0], NW * C.NS) DM(Hs, NW * C.NS * C.NS) DM(cost_part, NW * (h->nblk_vis + 1)) DM(red, NW * (2 * (size_t) C.NCA * C.NCA + 8)) DM(redmax, NW) DM(red2, NW * 4) DM(step_c, NW * C.NS) DM(step_l, NW * C.L)
+    DM(Hc[0], NW * C.NS * C.NS) DM(gc[0], NW * C.NS) DM(Hs, NW * C.NS * C.NS) DM(cost_part, NW * (h->nblk_vis + 1)) DM(red2, NW * 4) DM(step_c, NW * C.NS) DM(step_l, NW * C.L)
 #undef DM
     if (rc == ICG_OK) rc = dmalloc(h, &D.gnss_std_0, NW * C.G * 3);
     if (rc == ICG_OK) {
@@ -2119,7 +2004,6 @@ void icg_ba_destroy(icg_ba *h) {
     h->pose_prior_sinfo.release(), h->mix_prior.release(), h->mix_prior_std.release(), h->marg_x0.release(), h->marg_H0.release(), h->marg_b0.release();
     h->marg_c0.release(), h->lm_off.release(), h->lm_perm.release(), h->lm_fidx.release(), h->gnss_node.release();
     h->f_meta_s.release(), h->vb_lm0.release(), h->ref_nrun.release(), h->f_const_s.release(), h->marg_type.release(), h->marg_node.release(), h->f_active.release(), h->scratch.release(), h->st_save.release(), h->cull_counters.release(), h->part_off.release(), h->pair_ro.release(), h->vis_ord.release(), h->npairs.release();
-    if (h->comm) nccl_api().CommDestroy((ncclComm_t) h->comm);
     split_release(h);
     if (h->marg_ready) h->marg_map.release(), h->marg_oJ0.release(), h->marg_oe0.release(), h->marg_oHp.release(), h->marg_obp.release(), h->marg_fmask.release();
     if (h->cull_h) cudaFreeHost(h->cull_h);
@@ -2381,7 +2265,7 @@ int icg_ba_upload(icg_ba *h, int n, const icg_ba_problem *P) {
 
 // ---- in-situ stage timing
 static const char *PROF_NAMES[16] = {"(gap/other)", "lin_vis", "lin_lm", "lin at candidate", "","schur_dmma (+ epilogue)", "join lin_cam + lin_done",
-                                     "signal", "solve", "cost (+cost_cam)", "pack2 / exchange", "accept", "hsum / reduce", "join gram chain", "step_lm", ""};
+                                     "signal", "solve", "cost (+cost_cam)", "exchange", "accept", "reduce", "join gram chain", "step_lm", ""};
 static void prof_mark(icg_ba *h, int tag) {
     if (!h->prof) return;
     if (h->prof_used == h->prof_ev.size()) {
@@ -2447,7 +2331,7 @@ static void prof_print(icg_ba *h) {
 static int enqueue_lm_split(icg_ba *h, int max_num_iterations);
 
 // The second linearisation buffer (BaDev::Mp etc.), allocated on the first LM sequence of the single-GPU pipeline: handles that the split
-// or NCCL pipelines drive never linearise a candidate and do not pay for it (~80 MB for 148 windows at K = 10, L = 300).
+// pipeline drives never linearise a candidate and do not pay for it (~80 MB for 148 windows at K = 10, L = 300).
 static int alloc_lin_buf2(icg_ba *h) {
     BaDev &D = h->D;
     if (D.Mp[1]) return ICG_OK;
@@ -2464,26 +2348,22 @@ static int alloc_lin_buf2(icg_ba *h) {
 
 static int enqueue_lm(icg_ba *h, int max_num_iterations) {
     if (h->D.S.split) return enqueue_lm_split(h, max_num_iterations);
-    if (!h->comm) {
-        const int rc = alloc_lin_buf2(h);
-        if (rc != ICG_OK) return rc;
-    }
+    int rc = alloc_lin_buf2(h);
+    if (rc != ICG_OK) return rc;
     const BaCaps &C = h->C;
     const BaDev &D = h->D;
     const int n = h->cur_windows;
     cudaStream_t s = h->stream;
-    const dim3 g_vis(C.NVB - 2, n), g_cost(h->nblk_vis, n);
-    // Single GPU: linearisation at x (iteration 0) + (max_iter) x [schur syrk, solve, linearisation at the candidate, accept]; one extra
-    // schur + solve performs the final termination bookkeeping.  The linearisation at the candidate goes into the window's other buffer:
-    // its per-factor costs are the candidate cost ba_accept tests, and an accepted step flips the buffers instead of linearising again at
-    // the new x; a rejected one leaves the linearisation at x untouched.
-    // Landmark shards (NCCL): the candidate cost crosses the ranks before the accept step, so they evaluate it on its own (ba_cost,
-    // ba_cost_cam) and re-linearise at x after an accepted step.
+    const dim3 g_vis(C.NVB - 2, n);
+    // Linearisation at x (iteration 0) + (max_iter) x [schur syrk, solve, linearisation at the candidate, accept]; one extra schur + solve
+    // performs the final termination bookkeeping.  The linearisation at the candidate goes into the window's other buffer: its per-factor
+    // costs are the candidate cost ba_accept tests, and an accepted step flips the buffers instead of linearising again at the new x; a
+    // rejected one leaves the linearisation at x untouched.
     // where the camera-only factors are forked: 0 = beside ba_lin_vis (round 1), 1 = behind it (ba_lin_vis holds 128 registers x 4 CTAs: a
     // 320-thread camera CTA on the same SM costs it a resident CTA; on a single GPU nothing runs beside it then, the Schur kernel's epilogue
     // reads H_c).  Chosen by measurement (in-kernel phase clocks, ICG_BA_PROFILE).
     static const int cam_fork = getenv("ICG_BA_CAM_FORK") ? atoi(getenv("ICG_BA_CAM_FORK")) : 0;
-    // the linearisation (at x or at the candidate); the single GPU joins the camera-only factors before the next kernel reads H_c
+    // the linearisation (at x or at the candidate); the camera-only factors are joined before the next kernel reads H_c
     auto enqueue_lin = [&](int at_cand) -> int {
         // fork: IMU / GNSS / prior factors (one latency-bound CTA per window) run beside the vision chain
         if (cam_fork == 0) {
@@ -2503,51 +2383,22 @@ static int enqueue_lm(icg_ba *h, int max_num_iterations) {
         }
         // (measured: one fused launch or two streams are both slower -- the Schur CTAs' shared memory throttles the latency-bound
         //  Gram warps when they share SMs)
-        if (!h->comm) {
-            ICG_CUDA(cudaStreamWaitEvent(s, h->ev_join, 0));
-            prof_mark(h, at_cand ? 3 : 6);
-        }
+        ICG_CUDA(cudaStreamWaitEvent(s, h->ev_join, 0));
+        prof_mark(h, at_cand ? 3 : 6);
         count_launch(2);
         return ICG_OK;
     };
+    rc = enqueue_lin(0);
+    if (rc != ICG_OK) return rc;
     for (int it = 0; it <= max_num_iterations; it++) {
-        if (it == 0 || h->comm) {
-            const int rc = enqueue_lin(0);
-            if (rc != ICG_OK) return rc;
-        }
         ba_schur_dmma<<<dim3(BA_SPLIT_W, n), 256, h->smem_schur, s>>>(C, D, h->ld_schur);
         prof_mark(h, 5);
-        if (h->comm) {  // landmark-sharded window: one sum all-reduce of [H_vis g | Schur | cost, |rho|^2] + one max all-reduce
-            ICG_CUDA(cudaStreamWaitEvent(s, h->ev_join, 0));
-            prof_mark(h, 6);
-            int rc = nccl_allreduce(h, D.red, (size_t) n * (2 * (size_t) C.NCA * C.NCA + 8), 0);
-            if (rc != ICG_OK) return rc;
-            rc = nccl_allreduce(h, D.redmax, (size_t) n, 1);
-            if (rc != ICG_OK) return rc;
-            ba_hsum<<<dim3(((C.NCV + 1) * (C.NCV + 1) + 255) / 256, n), 256, 0, s>>>(C, D);
-            prof_mark(h, 12);
-        }
         ba_solve<<<n, SOLVE_THREADS, h->smem_solve, s>>>(C, D);
         prof_mark(h, 8);
-        count_launch(h->comm ? 3 : 2);
+        count_launch(2);
         if (it == max_num_iterations) break;
-        if (h->comm) {
-            ICG_CUDA(cudaEventRecord(h->ev_fork, s));
-            ICG_CUDA(cudaStreamWaitEvent(h->stream_cam, h->ev_fork, 0));
-            ba_cost_cam<<<n, h->cam_threads, h->smem_cam, h->stream_cam>>>(C, D, h->nblk_vis);
-            ICG_CUDA(cudaEventRecord(h->ev_join, h->stream_cam));
-            ba_cost<<<g_cost, 256, 0, s>>>(C, D, h->nblk_vis);
-            ICG_CUDA(cudaStreamWaitEvent(s, h->ev_join, 0));
-            prof_mark(h, 9);
-            ba_pack2<<<(n + 127) / 128, 128, 0, s>>>(C, D, n, h->nblk_vis);
-            prof_mark(h, 10);
-            int rc = nccl_allreduce(h, D.red2, (size_t) n * 4, 0);
-            if (rc != ICG_OK) return rc;
-            count_launch(3);
-        } else {
-            const int rc = enqueue_lin(1);
-            if (rc != ICG_OK) return rc;
-        }
+        rc = enqueue_lin(1);
+        if (rc != ICG_OK) return rc;
         ba_accept<<<n, 128, sizeof(double) * 8 * h->nblk_vis, s>>>(C, D);  // one double per 32 record slots
         prof_mark(h, 11);
         count_launch();
@@ -2901,8 +2752,8 @@ static int marginalize_body(icg_ba *h, int n_windows, const icg_ba_problem *prob
         set_error("icg_ba_marginalize: bad arguments");
         return ICG_EINVAL;
     }
-    if (h->comm || h->D.world > 1) {
-        set_error("icg_ba_marginalize: not available on a landmark-sharded handle (icg_ba_set_shard(world = 1) first)");
+    if (h->D.world > 1) {
+        set_error("icg_ba_marginalize: not available on a landmark-sharded handle (icg_ba_shard_leave first)");
         return ICG_EUNSUPPORTED;
     }
     int rc = ICG_OK;
@@ -3086,8 +2937,8 @@ static int resident_single_rank(icg_ba *h, int n_windows, const icg_ba_problem *
         set_error("%s: bad arguments", what);
         return ICG_EINVAL;
     }
-    if (h->comm || h->D.world > 1) {
-        set_error("%s: not available on a landmark-sharded handle (icg_ba_set_shard(world = 1) first)", what);
+    if (h->D.world > 1) {
+        set_error("%s: not available on a landmark-sharded handle (icg_ba_shard_leave first)", what);
         return ICG_EUNSUPPORTED;
     }
     if (h->cur_windows != n_windows) {
@@ -3392,60 +3243,6 @@ int icg_ba_marginalize_resident_culled(icg_ba *h, int n_windows, const icg_ba_pr
     return marginalize_body(h, n_windows, problems, num_marg, out, true, mp.data());
 }
 
-int icg_nccl_unique_id(uint8_t *id128) {
-    NcclApi &a = nccl_api();
-    if (!a.lib || !a.GetUniqueId) {
-        set_error("icg_nccl_unique_id: libnccl.so.2 not loadable");
-        return ICG_ENCCL;
-    }
-    ncclUniqueId id;
-    ncclResult_t r = a.GetUniqueId(&id);
-    if (r != ncclSuccess) {
-        set_error("ncclGetUniqueId failed: %s", a.GetErrorString(r));
-        return ICG_ENCCL;
-    }
-    static_assert(sizeof(ncclUniqueId) == 128, "ncclUniqueId size");
-    memcpy(id128, &id, 128);
-    return ICG_OK;
-}
-
-int icg_ba_set_shard(icg_ba *h, int rank, int world, const uint8_t *id128) {
-    if (!h || rank < 0 || world < 1 || rank >= world) {
-        set_error("icg_ba_set_shard: bad arguments");
-        return ICG_EINVAL;
-    }
-    ICG_CUDA(cudaSetDevice(h->device));
-    NcclApi &a = nccl_api();
-    if (h->comm) {
-        a.CommDestroy((ncclComm_t) h->comm);
-        h->comm = nullptr;
-    }
-    if (h->D.S.split && h->x_world > 1) {  // leaving a peer-memory shard group
-        int rc = h->use_global_S ? split_setup(h, 0, 1) : (split_release(h), ICG_OK);
-        if (rc != ICG_OK) return rc;
-    }
-    if (world > 1 && h->use_global_S) {
-        set_error("icg_ba_set_shard: windows of this size (max_K = %d) are solved by the split pipeline; use icg_ba_shard_export / icg_ba_shard_connect (transport p2p)", h->C.K);
-        return ICG_EUNSUPPORTED;
-    }
-    h->D.rank = rank, h->D.world = world;
-    if (world == 1) return ICG_OK;
-    if (!id128 || !a.lib || !a.CommInitRank) {
-        set_error("icg_ba_set_shard: libnccl.so.2 not loadable or null id");
-        return ICG_ENCCL;
-    }
-    ncclUniqueId id;
-    memcpy(&id, id128, 128);
-    ncclComm_t comm;
-    ncclResult_t r = a.CommInitRank(&comm, world, id, rank);
-    if (r != ncclSuccess) {
-        set_error("ncclCommInitRank failed: %s", a.GetErrorString(r));
-        return ICG_ENCCL;
-    }
-    h->comm = comm;
-    return ICG_OK;
-}
-
 // ---- landmark shards over peer memory (transport "p2p")
 struct ShardBlob {  // what a rank publishes to the others (ICG_SHARD_BLOB_BYTES)
     uint64_t magic, pid, ptr, doubles;
@@ -3458,10 +3255,6 @@ int icg_ba_shard_export(icg_ba *h, int rank, int world, uint8_t *blob) {
     if (!h || !blob) {
         set_error("icg_ba_shard_export: bad arguments");
         return ICG_EINVAL;
-    }
-    if (h->comm) {
-        nccl_api().CommDestroy((ncclComm_t) h->comm);
-        h->comm = nullptr;
     }
     int rc = split_setup(h, rank, world);
     if (rc != ICG_OK) return rc;
@@ -3510,6 +3303,28 @@ int icg_ba_shard_connect(icg_ba *h, const uint8_t *blobs) {
             h->D.S.peer[r] = (double *) p;
         }
     }
+    return ICG_OK;
+}
+
+// Leave the peer-memory shard group: the exchange buffers and the peers' mappings are released and the handle returns to the pipeline
+// its window size selects, on this GPU alone -- the fused single-GPU pipeline, or the split pipeline for systems that do not fit one CTA.
+int icg_ba_shard_leave(icg_ba *h) {
+    if (!h) {
+        set_error("icg_ba_shard_leave: bad arguments");
+        return ICG_EINVAL;
+    }
+    ICG_CUDA(cudaSetDevice(h->device));
+    ICG_CUDA(cudaStreamSynchronize(h->stream));
+    if (h->use_global_S) {
+        if (h->x_world > 1) {
+            const int rc = split_setup(h, 0, 1);
+            if (rc != ICG_OK) return rc;
+        }
+    } else {
+        split_release(h);
+        if (!getenv("ICG_BA_CAM_THREADS")) h->cam_threads = 160;  // split_setup sizes it by the group
+    }
+    h->D.rank = 0, h->D.world = 1;
     return ICG_OK;
 }
 

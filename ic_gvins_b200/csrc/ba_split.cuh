@@ -20,7 +20,7 @@
 //   every rank   ba_accept_split  waits for the G slots, sums them in rank order: identical inputs -> identical accept / reject, radius and
 //                                 termination decisions on every rank, no broadcast of the LM state
 //
-// Three flag synchronisations per attempt, no NCCL on the data path, no host round trip.  The flags are monotonically increasing epoch
+// Three flag synchronisations per attempt, no collective library on the data path, no host round trip.  The flags are monotonically increasing epoch
 // counters (one per LM attempt over the life of the handle); a consumer that does not see its flag within ~2 s raises the handle's
 // device-side error word instead of hanging the GPU.
 #pragma once

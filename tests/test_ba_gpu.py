@@ -490,16 +490,35 @@ def test_small_factor_seams_match_oracle(olib, solver):
         col += l
 
 
-def test_nccl_transport_is_refused_for_split_pipeline_sizes():
-    """windows whose reduced camera system does not fit one CTA (max_K = 20) are sharded over peer memory only: icg_ba_set_shard(world > 1)
-    must say so instead of building an NCCL communicator it cannot use"""
-    from ic_gvins_b200._lib import IcgError, check, lib
+@pytest.mark.parametrize("K,L", [(10, 300), (20, 2000)])
+def test_shard_leave_restores_a_fresh_handle(olib, K, L):
+    """After icg_ba_shard_leave, a handle that was rank 0 of a peer-memory shard group (two handles on cuda:0, exported and connected)
+    behaves like a fresh handle of the same capacities: the whole windows it solves are bitwise equal to the fresh handle's, and at K = 10
+    (fused single-GPU pipeline) the marginalization it refused inside the group runs and matches the fresh handle's bit for bit."""
+    from ic_gvins_b200._lib import IcgError
     from ic_gvins_b200.ba import WindowSolver
-    s = WindowSolver(max_windows=1, max_K=20, max_L=64, max_F=256, max_gnss=4, max_marg_r=1)
+    probs = [make(olib, K=K, L=L, seed=3200 + 10 * K + w, with_marg=(w == 1))[0] for w in range(2)]
+    caps = dict(max_windows=2, max_K=K, max_L=L, max_F=max(p["F"] for p in probs), max_gnss=16, max_marg_r=64)
+    group = [WindowSolver(**caps) for _ in range(2)]
+    fresh = WindowSolver(**caps)
     try:
-        import ctypes as C
-        idbuf = (C.c_uint8 * 128)()
-        with pytest.raises(IcgError, match="split pipeline"):
-            check(lib().icg_ba_set_shard(s._h, 0, 2, idbuf), "icg_ba_set_shard")
+        blobs = [sv.shard_export(r, 2) for r, sv in enumerate(group)]
+        for sv in group:
+            sv.shard_connect(blobs)
+        if K == 10:
+            with pytest.raises(IcgError, match="landmark-sharded"):
+                group[0].marginalize(copy.deepcopy(probs[0]), 1)
+        for sv in group:
+            sv.shard_leave()
+        left, ref = copy.deepcopy(probs), copy.deepcopy(probs)
+        out_left, out_ref = group[0].solve(left, 20), fresh.solve(ref, 20)
+        assert out_left == out_ref
+        for a, b in zip(left, ref):
+            for key in ("pose", "mix", "ext", "invdepth"):
+                assert np.array_equal(a[key], b[key]), key
+        if K == 10:
+            m_left, m_ref = group[0].marginalize(copy.deepcopy(ref[0]), 1)[0], fresh.marginalize(copy.deepcopy(ref[0]), 1)[0]
+            assert m_left["r"] == m_ref["r"] and np.array_equal(m_left["Hp"], m_ref["Hp"])
     finally:
-        s.close()
+        for sv in group + [fresh]:
+            sv.close()

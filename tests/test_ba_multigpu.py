@@ -1,6 +1,6 @@
 """Landmark-sharded window solve (SURVEY.md 8e, BASELINE cfg 4) on the GPUs of one box vs the single-process CPU oracle.
 
-One process per GPU (torch.multiprocessing spawn, NCCL rendezvous on 127.0.0.1); every rank uploads the camera-side problem and ITS
+One process per GPU (torch.multiprocessing spawn, torch.distributed rendezvous on 127.0.0.1, peer-memory transport); every rank uploads the camera-side problem and ITS
 block of landmarks, the ranks solve together, rank 0 merges the landmark results and compares with the oracle's solution of the
 whole window: same LM trajectory, solution within 1e-6 relative.  Skipped on boxes with fewer than 2 GPUs; the same sharded code path
 runs with two ranks on ONE GPU in tests/test_ba_gpu.py (peer-memory transport, in-process)."""
@@ -23,7 +23,7 @@ def _ngpu():
         return 0
 
 
-def _worker(rank, world, port, cfg, transport, q):
+def _worker(rank, world, port, cfg, q):
     try:
         os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world), LOCAL_RANK=str(rank))
         import torch
@@ -47,7 +47,7 @@ def _worker(rank, world, port, cfg, transport, q):
         shards = [shard_window(p, rank, world) for p in probs]
         s = WindowSolver(max_windows=nwin, max_K=K, max_L=max(1, max(sh["L"] for sh in shards)), max_F=max(1, max(sh["F"] for sh in shards)),
                          max_gnss=16, max_marg_r=64, device=rank)
-        connect_shards(s, rank, world, transport, dist)
+        connect_shards(s, rank, world, "p2p", dist)
         summ = s.solve(shards, 20)
         parts = [None] * world
         dist.all_gather_object(parts, [(sh["lm_lo"], sh["lm_hi"], sh["invdepth"], sh["pose"], sh["mix"], sh["ext"]) for sh in shards])
@@ -75,7 +75,7 @@ def _worker(rank, world, port, cfg, transport, q):
         q.put((rank, "FAIL: " + repr(e) + "\n" + traceback.format_exc()))
 
 
-def _run(world, cfg, transport):
+def _run(world, cfg):
     import torch.multiprocessing as mp
     s = socket.socket()
     s.bind(("127.0.0.1", 0))
@@ -83,7 +83,7 @@ def _run(world, cfg, transport):
     s.close()
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, cfg, transport, q)) for r in range(world)]
+    procs = [ctx.Process(target=_worker, args=(r, world, port, cfg, q)) for r in range(world)]
     for p in procs:
         p.start()
     res = []
@@ -100,14 +100,13 @@ def _run(world, cfg, transport):
 @pytest.mark.skipif(_ngpu() < 2, reason="needs >= 2 GPUs")
 @pytest.mark.parametrize("world", [2, 0])  # 0 = min(8, all GPUs of the box)
 def test_sharded_cfg4_matches_oracle(world):
-    """cfg 4 (20 KF / 2000 landmarks): the reduced camera system does not fit one CTA, so the handle runs the split pipeline and the shards talk
-    over peer memory (CUDA IPC, transport p2p); the NCCL transport is refused for these sizes (tests/test_ba_gpu.py)."""
+    """cfg 4 (20 KF / 2000 landmarks): the reduced camera system does not fit one CTA, so the handle runs the split pipeline with its
+    cluster solve on the window owner; the shards talk over peer memory (CUDA IPC, transport p2p)."""
     n = _ngpu()
     world = world or min(8, n)
-    _run(world, (20, 2000, 3), "p2p")
+    _run(world, (20, 2000, 3))
 
 
 @pytest.mark.skipif(_ngpu() < 2, reason="needs >= 2 GPUs")
-@pytest.mark.parametrize("transport", ["p2p", "nccl"])
-def test_sharded_cfg3_matches_oracle(transport):
-    _run(2, (10, 300, 2), transport)
+def test_sharded_cfg3_matches_oracle():
+    _run(2, (10, 300, 2))
