@@ -84,7 +84,10 @@ def imu_samples(t0, t1, rate, rng, bg, ba, yaw_rate=5.0 * D2R, earth=True):
 
 # ---------------------------------------------------------------------------------------------- problem
 def make_window(preintegrate, K=10, L=300, seed=2024, full_visibility=False, perturb=True, with_marg=False, pixel_noise=0.5, with_priors=False,
-                gnss_every=2, earth=True):
+                gnss_every=2, earth=True, n_ref=5):
+    """n_ref: landmark j is anchored in node j mod n_ref (j mod (K - 1) when K <= n_ref).  A larger n_ref spreads the landmarks over more
+    nodes, so fewer of them are marginalized with node 0.  The anchor itself draws no random numbers: the default (5) generates the same
+    arrays as before the keyword existed."""
     rng = np.random.Generator(np.random.PCG64(seed))
     dtk, rate = 0.5, 200.0
     times = np.arange(K) * dtk
@@ -110,7 +113,7 @@ def make_window(preintegrate, K=10, L=300, seed=2024, full_visibility=False, per
         return Rbc.T @ (pb - ext_t[:3])
 
     for j in range(L):
-        r = j % 5 if K > 5 else j % max(1, K - 1)
+        r = j % n_ref if K > n_ref else j % max(1, K - 1)
         depth = rng.uniform(5.0, 60.0)
         uv = np.array([rng.uniform(-0.7, 0.7), rng.uniform(-0.3, 0.3), 1.0])
         pc0 = uv * depth

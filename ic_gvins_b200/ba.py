@@ -284,7 +284,9 @@ class WindowSolver:
         prior in the layout the problem dict's marg_* entries use (node indices already shifted).  resident=True: the windows are the
         ones this handle has just solved (icg_ba_marginalize_resident: nothing is uploaded again).  culled (resident only): the list
         update_and_cull returned, with `obs_factor` in each dict; the factor set is then the map after the culling
-        (icg_ba_marginalize_resident_culled), node_in_map[w] (K flags) naming the keyframes still in the map (all of them when None)."""
+        (icg_ba_marginalize_resident_culled), node_in_map[w] (K flags) naming the keyframes still in the map (all of them when None).
+        Any handle marginalizes (cfg-4 windows included); a window whose marginalized or remained block exceeds 512 rows raises IcgError
+        (ICG_EUNSUPPORTED) before anything runs.  To consume its own prior, a handle of max_K nodes needs max_marg_r >= 15 (max_K - 1) + 7."""
         if isinstance(problems, dict):
             problems = [problems]
         call = self.marg_prepare(problems, num_marg, want_schur)

@@ -1803,9 +1803,12 @@ struct icg_ba {
     int prof_skip = 1;  // LM sequences to discard first (lazy module loading puts a one-off multi-ms cost on every kernel's first launch)
     double prof_ms[16] = {0};
     long prof_cnt[16] = {0};
-    // marginalization workspace (allocated on the first icg_ba_marginalize call)
+    // marginalization workspace (allocated on the first icg_ba_marginalize call).  The parts sized by the marginalized block (H0, b0, G1,
+    // V1, lam1, Z) follow the largest batch seen so far: marg_nw windows at the strides M.n0cap / M.mcap, grown on demand
     bool marg_ready = false;
-    MargDev M;
+    MargDev M{};
+    int marg_nw = 0;
+    int marg_cluster_ok = -1;  // -1 not checked yet; 1: an 8-CTA marg_jacobi_cluster with its largest shared memory can be scheduled
     HostDev<int> marg_map;
     HostDev<double> marg_oJ0, marg_oe0, marg_oHp, marg_obp;
     HostDev<uint8_t> marg_fmask;  // factor set of icg_ba_marginalize_resident_culled (ba_lin_vis reads it in place of f_active)
@@ -2006,6 +2009,8 @@ void icg_ba_destroy(icg_ba *h) {
     h->f_meta_s.release(), h->vb_lm0.release(), h->ref_nrun.release(), h->f_const_s.release(), h->marg_type.release(), h->marg_node.release(), h->f_active.release(), h->scratch.release(), h->st_save.release(), h->cull_counters.release(), h->part_off.release(), h->pair_ro.release(), h->vis_ord.release(), h->npairs.release();
     split_release(h);
     if (h->marg_ready) h->marg_map.release(), h->marg_oJ0.release(), h->marg_oe0.release(), h->marg_oHp.release(), h->marg_obp.release(), h->marg_fmask.release();
+    for (double *p : {h->M.H0, h->M.b0, h->M.G1, h->M.V1, h->M.lam1, h->M.Z})
+        if (p) cudaFree(p);
     if (h->cull_h) cudaFreeHost(h->cull_h);
     if (h->cull_d) cudaFree(h->cull_d);
     if (h->reint_h) cudaFreeHost(h->reint_h);
@@ -2711,16 +2716,16 @@ int icg_ba_gvins_optimization(icg_ba *h, int n_windows, const icg_ba_problem *pr
 }
 
 // ---- marginalization (B10)
+constexpr int MARG_MAXN = 512;  // rows of the largest block an eigensolver takes (marg_jacobi: RPL = 16 rows per lane)
+
+// The parts of the workspace that do not depend on the batch: the structure map, the outputs (rcap = N per window), the Jacobi workspace
+// of Hp (n = r <= N) and the saved flags
 static int marg_alloc(icg_ba *h) {
     if (h->marg_ready) return ICG_OK;
     const BaCaps &C = h->C;
     MargDev &M = h->M;
     const size_t NW = C.NW;
-    M.rcap = C.N, M.mcap = 15 * C.K + C.L, M.n0cap = C.N + C.L;
-    if (M.mcap > 512) {
-        set_error("icg_ba_marginalize: max_K=%d / max_L=%d exceed the Jacobi kernel's 512-row limit", C.K, C.L);
-        return ICG_EUNSUPPORTED;
-    }
+    M.rcap = C.N, M.mcap = 0, M.n0cap = 0;
     M.map_stride = MARG_MAP_HDR + 2 * C.K + C.L;
     if (h->marg_map.alloc(NW * M.map_stride) != ICG_OK || h->marg_oJ0.alloc(NW * (size_t) M.rcap * M.rcap) != ICG_OK || h->marg_oe0.alloc(NW * M.rcap) != ICG_OK ||
         h->marg_oHp.alloc(NW * (size_t) M.rcap * M.rcap) != ICG_OK || h->marg_obp.alloc(NW * M.rcap) != ICG_OK || h->marg_fmask.alloc(NW * C.F) != ICG_OK) {
@@ -2732,15 +2737,41 @@ static int marg_alloc(icg_ba *h) {
     double *fl = nullptr;
 #define DM(ptr, count) \
     if (rc == ICG_OK) rc = dmalloc(h, &ptr, count);
-    DM(M.H0, NW * (size_t) M.n0cap * M.n0cap) DM(M.b0, NW * M.n0cap) DM(M.G1, NW * (size_t) M.mcap * M.mcap) DM(M.V1, NW * (size_t) M.mcap * M.mcap)
-    DM(M.G2, NW * (size_t) M.rcap * M.rcap) DM(M.V2, NW * (size_t) M.rcap * M.rcap) DM(M.lam1, NW * M.mcap) DM(M.lam2, NW * M.rcap)
-    DM(M.Z, NW * (size_t) M.mcap * (M.rcap + 1)) DM(fl, NW * 2)
+    DM(M.G2, NW * (size_t) M.rcap * M.rcap) DM(M.V2, NW * (size_t) M.rcap * M.rcap) DM(M.lam2, NW * M.rcap) DM(fl, NW * 2)
 #undef DM
     if (rc != ICG_OK) return rc;
     M.flags = (int *) fl;
     const size_t smem = sizeof(double) * (8 * 480 + 2 * (size_t) C.R) + sizeof(int) * (size_t) C.R + 64;
     ICG_CUDA(raise_dynamic_smem((const void *) marg_assemble, (size_t) (smem)));
     h->marg_ready = true;
+    return ICG_OK;
+}
+
+// The parts sized by the marginalized block: H0 / b0 (n0 = m + r), G1 / V1 / lam1 (m), Z (m (rcap + 1)) for n windows.  They grow to the
+// batch's maxima when a batch needs more than the last allocation (strides only: the kernels index window w's slot by them and touch the
+// n0^2 / m^2 leading entries, so the results do not depend on them).
+static int marg_grow(icg_ba *h, int n, int max_m, int max_n0) {
+    MargDev &M = h->M;
+    if (n <= h->marg_nw && max_m <= M.mcap && max_n0 <= M.n0cap) return ICG_OK;
+    const int nw = std::max(n, h->marg_nw), mcap = std::max(max_m, M.mcap), n0cap = std::max(max_n0, M.n0cap);
+    ICG_CUDA(cudaStreamSynchronize(h->stream));  // earlier launches on the handle's stream may still read the old buffers
+    for (double **p : {&M.H0, &M.b0, &M.G1, &M.V1, &M.lam1, &M.Z}) {
+        if (*p) cudaFree(*p);
+        *p = nullptr;
+    }
+    h->marg_nw = 0, M.mcap = 0, M.n0cap = 0;
+    const size_t NW = nw;
+    const size_t count[6] = {NW * n0cap * n0cap, NW * n0cap, NW * mcap * mcap, NW * mcap * mcap, NW * mcap, NW * mcap * (M.rcap + 1)};
+    double **ptr[6] = {&M.H0, &M.b0, &M.G1, &M.V1, &M.lam1, &M.Z};
+    for (int k = 0; k < 6; k++) {
+        if (cudaMalloc(ptr[k], sizeof(double) * std::max<size_t>(1, count[k])) != cudaSuccess) {
+            *ptr[k] = nullptr;
+            set_error("icg_ba_marginalize: workspace allocation of %zu doubles failed (%d windows, m <= %d, m + r <= %d)", count[k], nw, mcap, n0cap);
+            return ICG_ENOMEM;
+        }
+        ICG_CUDA(cudaMemsetAsync(*ptr[k], 0, sizeof(double) * std::max<size_t>(1, count[k]), h->stream));
+    }
+    h->marg_nw = nw, M.mcap = mcap, M.n0cap = n0cap;
     return ICG_OK;
 }
 
@@ -2835,8 +2866,32 @@ static int marginalize_body(icg_ba *h, int n_windows, const icg_ba_problem *prob
         if (td_col < 0) td_col = 0;
         map[0] = m, map[1] = idx - m, map[2] = idx, map[3] = nm, map[4] = ext_col, map[5] = td_col, map[6] = map[7] = 0;
         o.m = m, o.r = idx - m, o.nblocks = nb;
+        // checked before anything is launched: a rejected call leaves the device state of the handle as it was
+        if (m > MARG_MAXN || idx - m > MARG_MAXN) {
+            set_error("icg_ba_marginalize: window %d: %s=%d exceeds the %d rows of the largest eigensolver kernel", w, m > MARG_MAXN ? "m" : "r",
+                      m > MARG_MAXN ? m : idx - m, MARG_MAXN);
+            return ICG_EUNSUPPORTED;
+        }
     }
+    int max_m = 0, max_r = 0, max_n0 = 0;
+    for (int w = 0; w < n; w++) max_m = std::max(max_m, out[w].m), max_r = std::max(max_r, out[w].r), max_n0 = std::max(max_n0, out[w].m + out[w].r);
+    rc = marg_grow(h, n, max_m, max_n0);
+    if (rc != ICG_OK) return rc;
     cudaStream_t s = h->stream;
+    if (h->marg_cluster_ok < 0) {  // once per handle: can an 8-CTA marg_jacobi_cluster with the largest shared-memory slices be placed at all?
+        const size_t csm = marg_cluster_smem(MARG_CLUSTER_MAXN);
+        ICG_CUDA(raise_dynamic_smem((const void *) marg_jacobi_cluster, csm));
+        cudaLaunchConfig_t cfg;
+        memset(&cfg, 0, sizeof(cfg));
+        cfg.gridDim = dim3(MARG_CLUSTER_CTAS), cfg.blockDim = dim3(MARG_CLUSTER_THREADS), cfg.dynamicSmemBytes = csm, cfg.stream = s;
+        cudaLaunchAttribute at[1];
+        at[0].id = cudaLaunchAttributeClusterDimension;
+        at[0].val.clusterDim.x = MARG_CLUSTER_CTAS, at[0].val.clusterDim.y = 1, at[0].val.clusterDim.z = 1;
+        cfg.attrs = at, cfg.numAttrs = 1;
+        int nclusters = 0;
+        h->marg_cluster_ok = cudaOccupancyMaxActiveClusters(&nclusters, marg_jacobi_cluster, &cfg) == cudaSuccess && nclusters > 0 ? 1 : 0;
+        cudaGetLastError();  // a refused query is an answer (the global kernel takes those blocks), not an error of this call
+    }
     ICG_CUDA(h->marg_map.up(s, (size_t) n * M.map_stride));
     BaDev D = h->D;
     if (fmask) {
@@ -2847,11 +2902,23 @@ static int marginalize_body(icg_ba *h, int n_windows, const icg_ba_problem *prob
     marg_prepare<<<(n + 127) / 128, 128, 0, s>>>(D, M, n, 0);
     ba_lin_vis<<<dim3(C.NVB - 2, n), 128, LV_SMEM, s>>>(C, D, 0);
     marg_assemble<<<n, 256, smem, s>>>(C, D, M);
-    // eigendecompositions: on-chip cluster-pair kernel when every block of the batch fits (n <= MARG_PAIR_MAXN), global-memory kernel otherwise
-    int max_m = 0, max_r = 0;
-    for (int w = 0; w < n; w++) max_m = std::max(max_m, out[w].m), max_r = std::max(max_r, out[w].r);
+    // eigendecompositions: one kernel per stage serves the whole batch, chosen by the batch's largest block --
+    //   n <= MARG_CTA_MAXN: one CTA;  n <= MARG_PAIR_MAXN: cluster pair;  n <= MARG_CLUSTER_MAXN: 8-CTA cluster;  otherwise: global memory.
+    // ICG_MARG_GLOBAL_JACOBI forces the global kernel, ICG_MARG_PAIR_JACOBI skips the one-CTA kernel, ICG_MARG_CLUSTER_JACOBI takes the
+    // 8-CTA cluster for any n it supports.
     auto jacobi = [&](int which, int nmax) -> int {
-        if (nmax <= MARG_CTA_MAXN && !getenv("ICG_MARG_GLOBAL_JACOBI") && !getenv("ICG_MARG_PAIR_JACOBI")) {
+        const bool cluster_ok = nmax <= MARG_CLUSTER_MAXN && h->marg_cluster_ok == 1;
+        if (cluster_ok && !getenv("ICG_MARG_GLOBAL_JACOBI") && (getenv("ICG_MARG_CLUSTER_JACOBI") || nmax > MARG_PAIR_MAXN)) {
+            const size_t smem = marg_cluster_smem(nmax);
+            cudaLaunchConfig_t cfg;
+            memset(&cfg, 0, sizeof(cfg));
+            cfg.gridDim = dim3((unsigned) (MARG_CLUSTER_CTAS * n)), cfg.blockDim = dim3(MARG_CLUSTER_THREADS), cfg.dynamicSmemBytes = smem, cfg.stream = s;
+            cudaLaunchAttribute at[1];
+            at[0].id = cudaLaunchAttributeClusterDimension;
+            at[0].val.clusterDim.x = MARG_CLUSTER_CTAS, at[0].val.clusterDim.y = 1, at[0].val.clusterDim.z = 1;
+            cfg.attrs = at, cfg.numAttrs = 1;
+            ICG_CUDA(cudaLaunchKernelEx(&cfg, marg_jacobi_cluster, M, which));
+        } else if (nmax <= MARG_CTA_MAXN && !getenv("ICG_MARG_GLOBAL_JACOBI") && !getenv("ICG_MARG_PAIR_JACOBI")) {
             const size_t smem = sizeof(double) * 2 * (size_t) nmax * nmax;
             ICG_CUDA(raise_dynamic_smem((const void *) marg_jacobi_cta, smem));
             marg_jacobi_cta<<<n, MARG_CTA_THREADS, smem, s>>>(M, which);

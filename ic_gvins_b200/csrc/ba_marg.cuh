@@ -563,6 +563,140 @@ __global__ void __launch_bounds__(MARG_CTA_THREADS) marg_jacobi_cta(MargDev M, i
     }
 }
 
+// The same eigensolver for MARG_PAIR_MAXN < n <= MARG_CLUSTER_MAXN (a cfg-4 window's remained block, r = 15 * 19 + 7 = 292): a CLUSTER OF
+// EIGHT CTAs per window, G and V distributed over their shared memory by rows.  CTA k holds rows [k R8, (k + 1) R8), R8 = ceil(n / 8) <= 40,
+// of every column of G and of V (column-major inside the slice): 2 * 40 * 320 doubles = 204.8 KB at n = 320, plus the partial-sum slots.
+// A round-robin step:
+//   1. four lanes per column pair form the pair's three partial dot products (al, be, ga) over the CTA's rows, into a local slot;
+//   2. one cluster barrier;
+//   3. every CTA reads the eight CTAs' slots over DSMEM and sums them in rank order 0..7, so every CTA gets the same (al, be, ga), the same
+//      rotation and the same "any rotation this sweep" decision (the sweep loop exits uniformly with no broadcast);
+//   4. every CTA rotates its own rows of G and V; a block barrier separates them from the next step's partials.
+// The slots are double-buffered by step parity: a slot is rewritten two steps later, after every CTA has passed the barrier that follows its
+// reads, so one cluster barrier per step is enough.  lambda_j = v_j . g_j is summed from rank-ordered per-CTA partials.
+constexpr int MARG_CLUSTER_MAXN = 320;
+constexpr int MARG_CLUSTER_CTAS = 8;                       // portable maximum cluster size
+constexpr int MARG_CLUSTER_THREADS = 640;                  // 160 four-lane groups: one per pair of a step at n = 320
+constexpr int MARG_CLUSTER_SLOT = 3 * (MARG_CLUSTER_MAXN / 2);  // (al, be, ga) per pair
+__host__ __device__ constexpr int marg_cluster_rows(int n) { return (n + MARG_CLUSTER_CTAS - 1) / MARG_CLUSTER_CTAS; }
+__host__ __device__ constexpr size_t marg_cluster_smem(int n) {
+    return sizeof(double) * (2 * (size_t) marg_cluster_rows(n) * n + 2 * (size_t) MARG_CLUSTER_SLOT);
+}
+__global__ void __launch_bounds__(MARG_CLUSTER_THREADS) marg_jacobi_cluster(MargDev M, int which) {
+    extern __shared__ double sm_mat[];  // G slice | V slice (n columns of R8 rows each) | partial slots [2][MARG_CLUSTER_SLOT]
+    __shared__ int s_any[2];
+    cg::cluster_group cluster = cg::this_cluster();
+    const int cr = (int) cluster.block_rank();
+    const int w = blockIdx.x / MARG_CLUSTER_CTAS, tid = threadIdx.x, lane = tid & 31, sl = lane & 3;
+    const int *map = M.map + (size_t) w * M.map_stride;
+    const int m = map[0], r = map[1], n0 = map[2];
+    if (m <= 0) return;  // uniform over the cluster
+    const int n = which == 0 ? m : r;
+    const double *src = which == 0 ? M.H0 + (size_t) w * M.n0cap * M.n0cap : M.Hp + (size_t) w * M.rcap * M.rcap;
+    const int lds = which == 0 ? n0 : r;
+    double *Vout = which == 0 ? M.V1 + (size_t) w * M.mcap * M.mcap : M.V2 + (size_t) w * M.rcap * M.rcap;
+    double *lam = which == 0 ? M.lam1 + (size_t) w * M.mcap : M.lam2 + (size_t) w * M.rcap;
+    const int R8 = marg_cluster_rows(n), r0 = cr * R8;
+    double *G = sm_mat, *V = sm_mat + (size_t) R8 * n, *slot = V + (size_t) R8 * n;
+    for (int e = tid; e < R8 * n; e += MARG_CLUSTER_THREADS) {
+        const int j = e / R8, i = r0 + (e - j * R8);  // column j, row i (rows past n are zero: they add nothing to any sum)
+        G[e] = i < n ? 0.5 * (src[(size_t) i * lds + j] + src[(size_t) j * lds + i]) : 0.0;
+        V[e] = i == j ? 1.0 : 0.0;
+    }
+    if (tid < 2) s_any[tid] = 0;
+    // this lane's two remote slots in the rank-ordered sum: ranks 2 sl and 2 sl + 1
+    const double *slot_a = cluster.map_shared_rank(slot, 2 * sl), *slot_b = cluster.map_shared_rank(slot, 2 * sl + 1);
+    cluster.sync();
+    const int ne = (n + 1) & ~1, half = ne / 2;
+    const int i = tid >> 2;                                  // pair slot of this four-lane group
+    const unsigned gmask = 0xFu << (lane & ~3);
+    constexpr int RPL = (MARG_CLUSTER_MAXN / MARG_CLUSTER_CTAS + 3) / 4;  // rows per lane: R8 <= 40
+    int gstep = 0;                                           // steps over all sweeps: the slot parity (ne - 1 is odd)
+    for (int sweep = 0; sweep < 40; sweep++) {
+        for (int step = 0; step < ne - 1; step++, gstep++) {
+            const int buf = gstep & 1;
+            int p = i == 0 ? ne - 1 : (step + i) % (ne - 1);
+            int q = (step + ne - 1 - i) % (ne - 1);
+            const bool active = i < half && p < n && q < n;  // uniform over the four lanes
+            if (p > q) {
+                const int t = p;
+                p = q, q = t;
+            }
+            double *gp = G + (size_t) p * R8, *gq = G + (size_t) q * R8;
+            if (active) {
+                double al = 0, be = 0, ga = 0;
+#pragma unroll
+                for (int k = 0; k < RPL; k++) {
+                    const int row = sl + 4 * k;
+                    const double a = row < R8 ? gp[row] : 0.0, b = row < R8 ? gq[row] : 0.0;
+                    al += a * a, be += b * b, ga += a * b;
+                }
+#pragma unroll
+                for (int o = 2; o > 0; o >>= 1) {
+                    al += __shfl_xor_sync(gmask, al, o);
+                    be += __shfl_xor_sync(gmask, be, o);
+                    ga += __shfl_xor_sync(gmask, ga, o);
+                }
+                if (sl == 0) {
+                    double *s = slot + (size_t) buf * MARG_CLUSTER_SLOT + 3 * i;
+                    s[0] = al, s[1] = be, s[2] = ga;
+                }
+            }
+            cluster.sync();  // every CTA's partials of this step are in place
+            if (active) {
+                const size_t o = (size_t) buf * MARG_CLUSTER_SLOT + 3 * i;
+                const double xa[3] = {slot_a[o], slot_a[o + 1], slot_a[o + 2]}, xb[3] = {slot_b[o], slot_b[o + 1], slot_b[o + 2]};
+                double t3[3] = {0, 0, 0};
+#pragma unroll
+                for (int rk = 0; rk < MARG_CLUSTER_CTAS; rk++) {
+                    const int src_lane = (lane & ~3) | (rk >> 1);
+#pragma unroll
+                    for (int c = 0; c < 3; c++) t3[c] += __shfl_sync(gmask, (rk & 1) ? xb[c] : xa[c], src_lane);
+                }
+                double c, s;
+                if (jacobi_rotation(t3[0], t3[1], t3[2], c, s)) {
+                    double *vp = V + (size_t) p * R8, *vq = V + (size_t) q * R8;
+#pragma unroll
+                    for (int k = 0; k < RPL; k++) {
+                        const int row = sl + 4 * k;
+                        if (row < R8) {
+                            const double a = gp[row], b = gq[row];
+                            gp[row] = c * a - s * b;
+                            gq[row] = s * a + c * b;
+                            const double x = vp[row], y = vq[row];
+                            vp[row] = c * x - s * y;
+                            vq[row] = s * x + c * y;
+                        }
+                    }
+                    if (sl == 0) s_any[sweep & 1] = 1;
+                }
+            }
+            __syncthreads();  // this step's rotations land before the next step's partials read the columns
+        }
+        const int any = s_any[sweep & 1];  // the same value in every CTA of the cluster
+        if (tid == 0) s_any[(sweep + 1) & 1] = 0;
+        if (!any) break;
+    }
+    // ---- results: this CTA's rows of V; lambda_j from the eight CTAs' partials of v_j . g_j, summed in rank order
+    for (int e = tid; e < R8 * n; e += MARG_CLUSTER_THREADS) {
+        const int j = e / R8, il = e - j * R8;
+        if (r0 + il < n) Vout[(size_t) j * n + r0 + il] = V[e];
+    }
+    cluster.sync();  // the other CTAs have read this CTA's slots of the last step: the slot area is free
+    for (int j = tid; j < n; j += MARG_CLUSTER_THREADS) {
+        double s = 0;
+        for (int il = 0; il < R8; il++) s += V[(size_t) j * R8 + il] * G[(size_t) j * R8 + il];
+        slot[j] = s;  // n <= 2 * MARG_CLUSTER_SLOT
+    }
+    cluster.sync();
+    for (int j = cr + MARG_CLUSTER_CTAS * tid; j < n; j += MARG_CLUSTER_CTAS * MARG_CLUSTER_THREADS) {
+        double s = 0;
+        for (int rk = 0; rk < MARG_CLUSTER_CTAS; rk++) s += cluster.map_shared_rank(slot, rk)[j];
+        lam[j] = s;
+    }
+    cluster.sync();  // every CTA's shared memory stays alive until the others have read its partials
+}
+
 // Hp = Hrr - Hrm Hmm^+ Hmr, bp = br - Hrm Hmm^+ bm with Hmm^+ = V diag(1/lambda > EPS) V^T  (schurElimination)
 __global__ void __launch_bounds__(MARG_THREADS) marg_schur(MargDev M) {
     const int w = blockIdx.x, tid = threadIdx.x;

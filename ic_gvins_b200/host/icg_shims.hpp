@@ -214,6 +214,8 @@ private:
 };
 
 // The window solve seam: what GVINS::gvinsOptimization hands to ceres::Solver::Solve (IG/ic_gvins.cc:1130-1239).
+// Any max_K / max_L marginalizes (a block beyond 512 rows throws ICG_EUNSUPPORTED); to consume its own prior the handle needs
+// max_marg_r >= 15 (max_K - 1) + 7, e.g. 292 for a 20-keyframe window.
 class WindowSolver {
 public:
     WindowSolver(int max_K, int max_L, int max_F, int max_gnss = 16, int max_marg_r = 160, int device = 0) {

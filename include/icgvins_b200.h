@@ -508,6 +508,10 @@ int icg_ba_sync(icg_ba *h);
  * e0/bp rcap doubles with rcap >= 15*(K - num_marg) + 7.  Column order inside the marginalized / remained groups is
  * [pose_k, mix_k ascending k | landmarks ascending] / [pose_k, mix_k (touched blocks only) | ext | td]; the reference's order is that of
  * an unordered_map (implementation-defined) and only permutes rows / columns.
+ * Sizes: the device workspace follows the batch (its largest m and m + r), not the handle's max_K / max_L, so any handle marginalizes,
+ * cfg-4 windows (max_K = 20, max_L = 2000) included.  A window whose m or r exceeds 512 rows (the largest eigensolver) returns
+ * ICG_EUNSUPPORTED naming the window, before anything runs on the device.  Landmark-sharded handles return ICG_EUNSUPPORTED.  The next
+ * window consumes the prior through icg_ba_problem.marg_r <= max_marg_r: a window of K nodes can need 15 (K - 1) + 7 rows (292 at K = 20).
  */
 typedef struct icg_ba_prior {
     int32_t m, r, nblocks;            /* out: marginalizedSize(), remainedSize(), number of remained blocks */
