@@ -371,6 +371,42 @@ class WindowSolver:
             raise err
         return outs
 
+    def slide(self, next_problems, carry, prior_from_marg=True):
+        """The next keyframe's windows from the ones this handle holds (icg_ba_slide_resident): rows whose source is carried stay on the device,
+        the rest are read from `next_problems` (dicts as upload() takes them; carried value rows may be stale).  carry: one dict per window
+        with int32 arrays node_src (K), lm_src (L), f_src (F), imu_src (n_imu), gnss_src (n_gnss) -- old row or -1; a missing key carries
+        nothing of that kind.  prior_from_marg (one flag, or one per window): the prior is the one the last resident marginalization left.
+        Follow with run_gvins() and gvins_optimization_end(next_problems)."""
+        from ._lib import SlideWindow
+        n = len(next_problems)
+        flags = [prior_from_marg] * n if np.isscalar(prior_from_marg) else list(prior_from_marg)
+        arr = (BaProblem * n)(*[to_struct(p) for p in next_problems])
+        cw = (SlideWindow * n)()
+        keep = []
+        for w, c in enumerate(carry):
+            for k in ("node_src", "lm_src", "f_src", "imu_src", "gnss_src"):
+                if c.get(k) is None:
+                    continue
+                a = np.ascontiguousarray(c[k], np.int32)
+                keep.append(a)
+                setattr(cw[w], k, a.ctypes.data_as(ip))
+            cw[w].prior_from_marg = 1 if flags[w] else 0
+        check(lib().icg_ba_slide_resident(self._h, n, arr, cw), "icg_ba_slide_resident")
+        self._keep, self._n = arr, n
+
+    def gvins_optimization_end(self, problems):
+        """icg_ba_gvins_optimization_end after run_gvins(): synchronises, writes the parameters, f_active and gnss_std back into the problem
+        dicts and returns the two-pass results in the layout of gvins_optimization_batch."""
+        n = len(problems)
+        arr = (BaProblem * n)(*[to_struct(p) for p in problems])
+        summ = (BaSummary * (2 * n))()
+        culled = (C.c_int32 * (2 * n))()
+        check(lib().icg_ba_gvins_optimization_end(self._h, n, arr, summ, culled), "icg_ba_gvins_optimization_end")
+        f = lambda s: dict(iterations=s.iterations, num_successful_steps=s.num_successful_steps, termination=s.termination,
+                           initial_cost=s.initial_cost, final_cost=s.final_cost, final_radius=s.final_radius)
+        return [dict(pass1=f(summ[2 * w]), pass2=f(summ[2 * w + 1]), reproj_removed=culled[2 * w], gnss_reweighted=culled[2 * w + 1])
+                for w in range(n)]
+
     def marg_prepare(self, problems, num_marg=1, want_schur=True):
         """The argument block of one icg_ba_marginalize call (struct array over the problems' host arrays + caller-allocated output arrays):
         what a C++ caller keeps alive across keyframes.  marg_run issues the call, marg_collect turns the outputs into dicts."""

@@ -29,6 +29,7 @@ SOURCES = {
     "ba.cu": [],
     "ba_cull.cu": ["-fmad=false"],     # post-solve map update and outlier culling (fixed-order sums, as the numpy restatement)
     "preint.cu": ["-fmad=false"],      # IMU propagation, warp per interval: the sums of geom_core.cuh's preintegrate_core, bit for bit
+    "ba_slide.cu": ["-fmad=false"],    # slide to the next window: the prior's normal equations are icg_ba_upload's host sums, bit for bit
 }
 
 

@@ -283,6 +283,33 @@ public:
         return io.count;
     }
 
+    // The next gvinsOptimization's problem (IG/ic_gvins.cc:1130-1239, 1697-1837) from the window this solver holds, without re-uploading what
+    // carries over.  next = the problem as Solve would take it; carry = per row of next its row in the old window or -1 (an empty vector: none
+    // of that kind carries): node_src from timelist_ before and after gvinsMarginalization / removeUnusedTimeNode, lm_src from the old
+    // invdepthlist_ keys (a re-anchored map point is -1), f_src by (map point, observing keyframe), imu_src by preintegrationlist_ element (a
+    // merged factor is -1), gnss_src by gnsslist_ element.  prior_from_marginalization: the prior is the one marginalization(..., culled, ...)
+    // or marginalization(..., true) just built on this solver.  Then gvinsOptimizationResident(next, ...) solves it.
+    struct Carry {
+        std::vector<int32_t> node_src, lm_src, f_src, imu_src, gnss_src;
+    };
+    void slideWindow(const icg_ba_problem &next, const Carry &carry, bool prior_from_marginalization) {
+        auto ptr = [](const std::vector<int32_t> &v, int32_t n, const char *what) -> const int32_t * {
+            if (v.empty()) return nullptr;
+            if (v.size() != (size_t) (n > 0 ? n : 0)) throw std::runtime_error(std::string("WindowSolver::slideWindow: ") + what + " needs one entry per row of next");
+            return v.data();
+        };
+        icg_ba_slide_window c{};
+        c.node_src = ptr(carry.node_src, next.K, "node_src"), c.lm_src = ptr(carry.lm_src, next.L, "lm_src"), c.f_src = ptr(carry.f_src, next.F, "f_src");
+        c.imu_src = ptr(carry.imu_src, next.n_imu, "imu_src"), c.gnss_src = ptr(carry.gnss_src, next.n_gnss, "gnss_src");
+        c.prior_from_marg = prior_from_marginalization ? 1 : 0;
+        check(icg_ba_slide_resident(h_, 1, &next, &c), "icg_ba_slide_resident");
+    }
+    // the two-pass body of gvinsOptimization on the window slideWindow left (nothing is uploaded); results as gvinsOptimization gives them
+    void gvinsOptimizationResident(const icg_ba_problem &next, int num_iterations, icg_ba_summary out[2], int32_t culled[2]) {
+        check(icg_ba_run_gvins(h_, num_iterations, 0), "icg_ba_run_gvins");
+        check(icg_ba_gvins_optimization_end(h_, 1, &next, out, culled), "icg_ba_gvins_optimization_end");
+    }
+
 private:
     template <typename Call>
     Prior marginalize(const icg_ba_problem &problem, int num_marg, Call call) {

@@ -613,6 +613,33 @@ typedef struct icg_ba_reint_window {
 int icg_ba_reintegrate_resident(icg_ba *h, int n_windows, const icg_ba_problem *problems, const double *noise5, const double *station3,
                                 icg_ba_reint_window *io);
 /*
+ * The next keyframe's windows from the ones the handle holds, without re-uploading what the device already has.  GVINS rebuilds the problem
+ * every keyframe (IG/ic_gvins.cc:1130-1239, 1697-1837); between two windows most of it carries over: node states (the values the solve left),
+ * inverse depths (through depth = 1 / invdepth and back: rho' = 1.0 / (1.0 / rho)), reprojection factor constants, IMU blobs (reintegrated
+ * ones included) with their square-root information, GNSS fixes with their re-weighted std, and the prior gvinsMarginalization just built.
+ * `next` is the next window exactly as icg_ba_upload would take it; per window, `carry` names for every row of next its source row in the old
+ * window, or -1 for a row read from next (a NULL map: no row of that kind is carried).  Carried value rows of next are not read.  The structure
+ * (indices, f_active -- NULL: all active --, sizes, flags, ext, lever, first-window priors, the prior's block tables and x0) is read from next.
+ * prior_from_marg = 1: the prior is the one the last icg_ba_marginalize_resident[_culled] call left for this window (it must be the last
+ * marginalization on the handle, over the same n_windows, with no upload or slide since, and next.marg_r / marg_nblocks must be its r / nblocks);
+ * 0: next.marg_J0 / marg_e0.  H0 = J0^T J0, b0 = J0^T e0, c0 = e0.e0 are formed on the device in icg_ba_upload's summation order.
+ * Afterwards the handle is indistinguishable from one that called icg_ba_upload(next) with the carried values filled in: icg_ba_run[_gvins]
+ * (restart included), icg_ba_download / icg_ba_gvins_optimization_end(next) and the resident calls give the same bits.  Every check (map ranges
+ * against the old window, the upload's checks of next, a new blob's positive-definite covariance, the prior's origin) runs before the device is
+ * written; a rejected call (ICG_EINVAL with a message) leaves the handle as it was.  n_windows must equal the uploaded count.  Asynchronous on the
+ * handle's stream.  ICG_EUNSUPPORTED on a landmark-sharded handle.
+ */
+typedef struct icg_ba_slide_window {
+    const int32_t *node_src;  /* next.K: old node whose pose / mix carries over, or -1 (next.pose / next.mix row) */
+    const int32_t *lm_src;    /* next.L: old landmark whose inverse depth carries over as 1.0 / (1.0 / rho), or -1 (next.invdepth) */
+    const int32_t *f_src;     /* next.F: old reprojection factor whose 14 constants carry over, or -1 (next.f_const row) */
+    const int32_t *imu_src;   /* next.n_imu: old IMU factor whose blob and square-root information carry over, or -1 (next.imu_blob row) */
+    const int32_t *gnss_src;  /* next.n_gnss: old GNSS fix whose blh and current (re-weighted) std carry over, or -1 (next rows) */
+    int32_t prior_from_marg;  /* 1: the prior the last icg_ba_marginalize_resident[_culled] call computed for this window;
+                                 0: next.marg_* (J0 / e0 uploaded, H0 / b0 / c0 formed on the device) */
+} icg_ba_slide_window;
+int icg_ba_slide_resident(icg_ba *h, int n_windows, const icg_ba_problem *next, const icg_ba_slide_window *carry);
+/*
  * Landmark sharding of the window solve across the GPUs of one box (SURVEY.md 8e), over PEER MEMORY (transport "p2p"): every process
  * (one per GPU) uploads the same camera-side problem but only ITS landmarks and their reprojection factors; window w of the batch is
  * owned by rank w mod world.  Every rank STORES its packed reduction operand straight into the owner's inbox over NVLink; the owner sums
