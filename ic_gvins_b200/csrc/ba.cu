@@ -1767,8 +1767,6 @@ struct icg_ba {
     bool own_stream = false;
     int nblk_vis = 0;
     int cur_windows = 0;
-    int cam_threads = 160;  // CTA size of the camera-only factor kernels (<= CAM_THREADS; ICG_BA_CAM_THREADS): 160 x 168 registers leave room for two
-                            // ba_lin_vis CTAs on the SM (320 threads take 82 % of the register file: nothing else fits beside them)
     size_t smem_cam, smem_solve, smem_schur;
     int ld_schur;
     int use_global_S;
@@ -1791,10 +1789,8 @@ struct icg_ba {
     void *ipc_opened[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     unsigned long long epoch = 0;
     size_t smem_solve_cam = 0, smem_step_lm = 0;
-    bool solve_cam_stage_a = false;  // per-warp shared-memory strips for the DMMA A operand (ba_solve_cam)
-    bool solve_cam_dsm = false;      // the packed system fits the cluster's shared memory: ba_solve_cam_dsm (max_K <= 22)
+    bool solve_cam_dsm = false;      // the packed system fits the cluster's shared memory: ba_solve_cam_dsm (max_K <= 23)
     size_t smem_solve_cam_dsm = 0;
-    int dsm_variant = 0;             // ba_solve_cam_dsm: DSM_V_* bits (ICG_BA_DSM_VARIANT)
     // in-situ stage timing (ICG_BA_PROFILE=1): events between the kernels of the LM sequence on the main stream, read back in
     // icg_ba_sync / icg_ba_download and printed by icg_ba_destroy (warm caches, real launch gaps -- unlike an ncu replay)
     bool prof = false;
@@ -1845,6 +1841,11 @@ static int dmalloc(icg_ba *h, double **p, size_t n) {
     return ICG_OK;
 }
 
+// CTA size of the camera-only factor kernels (ba_lin_cam, ba_cost_cam).  160 threads x 168 registers leave room for two ba_lin_vis CTAs on
+// the SM (320 threads take 82 % of the register file: nothing else fits beside them).  With four or more landmark shards the owner's
+// camera-only kernels are on the attempt's critical path (the vision kernels shrink with the shard -- 410 us at one rank, ~100 at four --,
+// the per-window IMU chain of ~118 us does not): all 10 warps, two rounds of IMU factors at K = 20 instead of four.
+static int cam_threads(const icg_ba *h) { return h->D.world >= 4 ? CAM_THREADS : 160; }
 
 extern "C" {
 static int split_setup(icg_ba *h, int rank, int world);
@@ -1915,7 +1916,6 @@ static int ba_create_body(icg_ba *h, int max_windows, int max_K, int max_L, int 
     ICG_CUDA(cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming));
     ICG_CUDA(cudaEventCreateWithFlags(&h->ev_join, cudaEventDisableTiming));
     h->prof = getenv("ICG_BA_PROFILE") != nullptr;
-    if (getenv("ICG_BA_CAM_THREADS")) h->cam_threads = std::min(CAM_THREADS, std::max(128, atoi(getenv("ICG_BA_CAM_THREADS")) & ~31));
     if (h->prof) {
         double *ck = nullptr;
         if (dmalloc(h, &ck, 48) != ICG_OK) return ICG_ENOMEM;
@@ -2367,7 +2367,7 @@ static void prof_print(icg_ba *h) {
                 fprintf(stderr, "[icg_ba profile] %s phases of window 0 (SM cycles, mean):\n", h->solve_cam_dsm ? "ba_solve_cam_dsm" : "ba_solve_cam");
                 for (int k = 0; k < 6; k++)
                     if (ck[8 + k]) fprintf(stderr, "  %-34s %9.0f cycles\n", sn[k], (double) ck[k] / (double) ck[8 + k]);
-                static const char *sn2[5] = {"per panel: wait for the panel column", "(unused)", "per panel: warp 0 diagonal-tile update", "per panel: warp 0 loads + 8x8 factorisation", "per panel: warp 0 write-back"};
+                static const char *sn2[5] = {"(unused)", "(unused)", "per panel: warp 0 diagonal-tile update", "per panel: warp 0 loads + 8x8 factorisation", "per panel: warp 0 write-back"};
                 for (int k = 0; k < 5 && h->solve_cam_dsm; k++)
                     if (ck[40 + k]) fprintf(stderr, "  %-50s %9.0f cycles\n", sn2[k], (double) ck[32 + k] / (double) ck[40 + k]);
             }
@@ -2411,28 +2411,17 @@ static int enqueue_lm(icg_ba *h, int max_num_iterations) {
     // performs the final termination bookkeeping.  The linearisation at the candidate goes into the window's other buffer: its per-factor
     // costs are the candidate cost ba_accept tests, and an accepted step flips the buffers instead of linearising again at the new x; a
     // rejected one leaves the linearisation at x untouched.
-    // where the camera-only factors are forked: 0 = beside ba_lin_vis (round 1), 1 = behind it (ba_lin_vis holds 128 registers x 4 CTAs: a
-    // 320-thread camera CTA on the same SM costs it a resident CTA; on a single GPU nothing runs beside it then, the Schur kernel's epilogue
-    // reads H_c).  Chosen by measurement (in-kernel phase clocks, ICG_BA_PROFILE).
-    static const int cam_fork = getenv("ICG_BA_CAM_FORK") ? atoi(getenv("ICG_BA_CAM_FORK")) : 0;
     // the linearisation (at x or at the candidate); the camera-only factors are joined before the next kernel reads H_c
     auto enqueue_lin = [&](int at_cand) -> int {
-        // fork: IMU / GNSS / prior factors (one latency-bound CTA per window) run beside the vision chain
-        if (cam_fork == 0) {
-            ICG_CUDA(cudaEventRecord(h->ev_fork, s));
-            ICG_CUDA(cudaStreamWaitEvent(h->stream_cam, h->ev_fork, 0));
-            ba_lin_cam<<<n, h->cam_threads, h->smem_cam, h->stream_cam>>>(C, D, at_cand);
-            ICG_CUDA(cudaEventRecord(h->ev_join, h->stream_cam));
-        }
+        // fork: IMU / GNSS / prior factors (one latency-bound CTA per window) run beside the vision chain -- forked ahead of ba_lin_vis, so
+        // that the two overlap (measured against a fork behind it with in-kernel phase clocks, ICG_BA_PROFILE)
+        ICG_CUDA(cudaEventRecord(h->ev_fork, s));
+        ICG_CUDA(cudaStreamWaitEvent(h->stream_cam, h->ev_fork, 0));
+        ba_lin_cam<<<n, cam_threads(h), h->smem_cam, h->stream_cam>>>(C, D, at_cand);
+        ICG_CUDA(cudaEventRecord(h->ev_join, h->stream_cam));
         prof_mark(h, 0);
         ba_lin_vis<<<g_vis, 128, LV_SMEM, s>>>(C, D, at_cand);
         prof_mark(h, at_cand ? 3 : 1);
-        if (cam_fork != 0) {
-            ICG_CUDA(cudaEventRecord(h->ev_fork, s));
-            ICG_CUDA(cudaStreamWaitEvent(h->stream_cam, h->ev_fork, 0));
-            ba_lin_cam<<<n, h->cam_threads, h->smem_cam, h->stream_cam>>>(C, D, at_cand);
-            ICG_CUDA(cudaEventRecord(h->ev_join, h->stream_cam));
-        }
         // (measured: one fused launch or two streams are both slower -- the Schur CTAs' shared memory throttles the latency-bound
         //  Gram warps when they share SMs)
         ICG_CUDA(cudaStreamWaitEvent(s, h->ev_join, 0));
@@ -2515,23 +2504,17 @@ static int split_setup(icg_ba *h, int rank, int world) {
     S.split = 1;
     h->D.rank = rank, h->D.world = world;
     h->x_world = world;
-    // four or more landmark shards: the owner's camera-only kernels are on the attempt's critical path (the vision kernels shrink with the
-    // shard -- 410 us at one rank, ~100 at four --, the per-window IMU chain of ~118 us does not): all 10 warps, two rounds of IMU factors at
-    // K = 20 instead of four
-    if (!getenv("ICG_BA_CAM_THREADS")) h->cam_threads = world >= 4 ? CAM_THREADS : 160;
     h->epoch = 0;
-    {   // ba_solve_cam: vectors + the larger of the back-substitution staging and [B rows | 8 x 8 hand-over | one A strip per warp]; the A strips are
-        // dropped when they do not fit (max_K > 20)
+    {   // ba_solve_cam: vectors + the larger of the back-substitution staging and [B rows | 8 x 8 hand-over]
         const size_t ldbp = ((size_t) (C.N + 15) / 16) * 16 + 8;
-        const size_t bs = (size_t) SPLIT_BS_ROWS * (C.NS + 1), base = 8 * ldbp + 64, strips = (size_t) (SOLVE_THREADS / 32) * 8 * ldbp;
-        h->solve_cam_stage_a = sizeof(double) * (40 + 4 * (size_t) C.NS + std::max(bs, base + strips)) <= 220 * 1024;
-        h->smem_solve_cam = sizeof(double) * (40 + 4 * (size_t) C.NS + std::max(bs, base + (h->solve_cam_stage_a ? strips : 0)));
+        const size_t bs = (size_t) SPLIT_BS_ROWS * (C.NS + 1), base = 8 * ldbp + 64;
+        h->smem_solve_cam = sizeof(double) * (40 + 4 * (size_t) C.NS + std::max(bs, base));
     }
     h->smem_step_lm = sizeof(double) * (40 + (size_t) C.NS);
     h->smem_solve_cam_dsm = sizeof(double) * dsm_smem_doubles(C);
-    h->solve_cam_dsm = h->smem_solve_cam_dsm <= 227 * 1024 && C.N <= 32 * 11 && !getenv("ICG_BA_SOLVE_CAM_L2");  // (the assembly stages <= 11 chunks of 32 columns per row)
+    // the shared-memory form wherever it fits, max_K <= 23 (the assembly stages <= 11 chunks of 32 columns per row); ba_solve_cam beyond
+    h->solve_cam_dsm = h->smem_solve_cam_dsm <= 227 * 1024 && C.N <= 32 * 11;
     if (h->solve_cam_dsm) ICG_CUDA(raise_dynamic_smem((const void *) ba_solve_cam_dsm, h->smem_solve_cam_dsm));
-    h->dsm_variant = getenv("ICG_BA_DSM_VARIANT") ? atoi(getenv("ICG_BA_DSM_VARIANT")) : DSM_V_MBAR_BSUB;
     ICG_CUDA(raise_dynamic_smem((const void *) ba_solve_cam, (size_t) (h->smem_solve_cam)));
     ICG_CUDA(cudaFuncSetAttribute(ba_solve_cam, cudaFuncAttributeNonPortableClusterSizeAllowed, 0));
     ICG_CUDA(raise_dynamic_smem((const void *) ba_step_lm, (size_t) (h->smem_step_lm)));
@@ -2547,8 +2530,8 @@ static int launch_solve_cam(icg_ba *h, int n, unsigned long long epoch) {
     at[0].id = cudaLaunchAttributeClusterDimension;
     at[0].val.clusterDim.x = SPLIT_CLUSTER, at[0].val.clusterDim.y = 1, at[0].val.clusterDim.z = 1;
     cfg.attrs = at, cfg.numAttrs = 1;
-    if (h->solve_cam_dsm) ICG_CUDA(cudaLaunchKernelEx(&cfg, ba_solve_cam_dsm, h->C, h->D, epoch, h->dsm_variant));
-    else ICG_CUDA(cudaLaunchKernelEx(&cfg, ba_solve_cam, h->C, h->D, epoch, (int) h->solve_cam_stage_a));
+    if (h->solve_cam_dsm) ICG_CUDA(cudaLaunchKernelEx(&cfg, ba_solve_cam_dsm, h->C, h->D, epoch));
+    else ICG_CUDA(cudaLaunchKernelEx(&cfg, ba_solve_cam, h->C, h->D, epoch));
     return ICG_OK;
 }
 
@@ -2569,7 +2552,7 @@ static int enqueue_lm_split(icg_ba *h, int max_num_iterations) {
         const unsigned long long epoch = ++h->epoch;
         ICG_CUDA(cudaEventRecord(h->ev_fork, s));
         ICG_CUDA(cudaStreamWaitEvent(h->stream_cam, h->ev_fork, 0));
-        ba_lin_cam<<<n, h->cam_threads, h->smem_cam, h->stream_cam>>>(C, D, 0);
+        ba_lin_cam<<<n, cam_threads(h), h->smem_cam, h->stream_cam>>>(C, D, 0);
         ICG_CUDA(cudaEventRecord(h->ev_join, h->stream_cam));
         prof_mark(h, 0);
         ba_lin_vis<<<g_vis, 128, LV_SMEM, s>>>(C, D, 0);
@@ -2591,7 +2574,7 @@ static int enqueue_lm_split(icg_ba *h, int max_num_iterations) {
         if (it == max_num_iterations) break;
         ICG_CUDA(cudaEventRecord(h->ev_fork, s));
         ICG_CUDA(cudaStreamWaitEvent(h->stream_cam, h->ev_fork, 0));
-        ba_cost_cam<<<n, h->cam_threads, h->smem_cam, h->stream_cam>>>(C, D, h->nblk_vis);
+        ba_cost_cam<<<n, cam_threads(h), h->smem_cam, h->stream_cam>>>(C, D, h->nblk_vis);
         ICG_CUDA(cudaEventRecord(h->ev_join, h->stream_cam));
         ba_cost<<<g_cost, 256, 0, s>>>(C, D, h->nblk_vis);
         ICG_CUDA(cudaStreamWaitEvent(s, h->ev_join, 0));
@@ -3664,7 +3647,6 @@ int icg_ba_shard_leave(icg_ba *h) {
         }
     } else {
         split_release(h);
-        if (!getenv("ICG_BA_CAM_THREADS")) h->cam_threads = 160;  // split_setup sizes it by the group
     }
     h->D.rank = 0, h->D.world = 1;
     return ICG_OK;

@@ -125,7 +125,7 @@ __host__ __device__ inline size_t split_S_stride(const BaCaps &C) { return (size
 // The camera-side half of ba_solve for systems that do not fit one CTA: S lives packed in global memory (L2-resident, written and read by all
 // CTAs of the cluster between cluster barriers -- cluster.sync orders the global accesses at cluster scope and invalidates L1).
 // Row i of the packed lower triangle starts at i (i + 1) / 2; the augmented row N carries the right-hand side.
-__global__ void __launch_bounds__(SOLVE_THREADS) ba_solve_cam(BaCaps C, BaDev D, unsigned long long epoch, int stage_a) {
+__global__ void __launch_bounds__(SOLVE_THREADS) ba_solve_cam(BaCaps C, BaDev D, unsigned long long epoch) {
     extern __shared__ double sm[];
     cg::cluster_group cluster = cg::this_cluster();
     const int CL = (int) cluster.num_blocks(), cr = (int) cluster.block_rank();
@@ -249,60 +249,28 @@ __global__ void __launch_bounds__(SOLVE_THREADS) ba_solve_cam(BaCaps C, BaDev D,
         CAMS_CLK(0, tc0)  // staging of the B operand
         const unsigned long long tc1 = CAMS_NOW();
         (void) tc1;
-        // one 8-row tile: S[rows, J0 : J0 + 8] -= L[rows, : J0] L[J0 : J0 + 8, : J0]^T.
-        // stage_a (the launch gave every warp an 8 x ldbp shared-memory strip): the tile's A rows come in with 8-byte cp.async, ALL columns in
-        // flight at once (one L2 round trip per tile; measured 2 k cycles per 64-column pass when the operand is read from L2 in the k loop),
-        // then both DMMA operands are conflict-free shared-memory reads.  Without the strips (max_K beyond the shared-memory budget): 64 columns
-        // (16 loads per lane) in flight per pass.
+        // one 8-row tile: S[rows, J0 : J0 + 8] -= L[rows, : J0] L[J0 : J0 + 8, : J0]^T; the A operand is read from L2, 64 columns (16 loads per
+        // lane) in flight per pass.  (This form runs only where the system is too large for the cluster's shared memory, max_K >= 24: per-warp
+        // shared-memory strips for the A rows do not fit beside the vectors there.)
         auto tile_update = [&](int tI) {
             const int ia = J0 + 8 * tI + g;
             const bool oka = ia < NR;
             const double *ra = S + (oka ? (size_t) ia * (ia + 1) / 2 : 0);
             const double *sb = s_b + g * ldbp;
             double c0 = 0, c1 = 0, d0 = 0, d1 = 0, e0 = 0, e1 = 0, f0 = 0, f1 = 0;
-            if (stage_a) {
-                double *sw = s_b + 8 * ldbp + 64 + (size_t) warp * 8 * ldbp;  // this warp's strip (behind the B rows and the 8 x 8 hand-over buffer)
-                __syncwarp();  // the strip's previous tile has been consumed
-#pragma unroll 1
-                for (int r = 0; r < 8; r++) {
-                    const int row = J0 + 8 * tI + r;
-                    if (row < NR) {
-                        const double *src = S + (size_t) row * (row + 1) / 2;
-                        const unsigned dst = (unsigned) __cvta_generic_to_shared(sw + r * ldbp);
-                        for (int c = lane; c < J0; c += 32) asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(dst + 8u * c), "l"(src + c) : "memory");
-                    }
-                }
-                asm volatile("cp.async.commit_group;" ::: "memory");
-                asm volatile("cp.async.wait_all;" ::: "memory");
-                __syncwarp();
-                const double *sa = sw + g * ldbp;
-                int k0 = 0;
-                for (; k0 + 16 <= J0; k0 += 16) {
-                    const double a0 = oka ? sa[k0 + kk] : 0.0, a1 = oka ? sa[k0 + 4 + kk] : 0.0, a2 = oka ? sa[k0 + 8 + kk] : 0.0, a3 = oka ? sa[k0 + 12 + kk] : 0.0;
-                    dmma884(c0, c1, a0, sb[k0 + kk]);
-                    dmma884(d0, d1, a1, sb[k0 + 4 + kk]);
-                    dmma884(e0, e1, a2, sb[k0 + 8 + kk]);
-                    dmma884(f0, f1, a3, sb[k0 + 12 + kk]);
-                }
-                for (; k0 + 4 <= J0; k0 += 4) {
-                    const double a0 = oka ? sa[k0 + kk] : 0.0;
-                    dmma884(c0, c1, a0, sb[k0 + kk]);
-                }
-            } else {
-                for (int k0 = 0; k0 < J0; k0 += 64) {
-                    double a[16];
+            for (int k0 = 0; k0 < J0; k0 += 64) {
+                double a[16];
 #pragma unroll
-                    for (int u = 0; u < 16; u++) a[u] = (oka && k0 + 4 * u < J0) ? ra[k0 + 4 * u + kk] : 0.0;
+                for (int u = 0; u < 16; u++) a[u] = (oka && k0 + 4 * u < J0) ? ra[k0 + 4 * u + kk] : 0.0;
 #pragma unroll
-                    for (int u = 0; u < 16; u += 4) {
-                        if (k0 + 4 * u < J0) {  // J0 is a multiple of 8: k-steps come in pairs; zero-padded beyond J0
-                            const double b0 = sb[k0 + 4 * u + kk], b1 = k0 + 4 * u + 4 < J0 ? sb[k0 + 4 * u + 4 + kk] : 0.0;
-                            const double b2 = k0 + 4 * u + 8 < J0 ? sb[k0 + 4 * u + 8 + kk] : 0.0, b3 = k0 + 4 * u + 12 < J0 ? sb[k0 + 4 * u + 12 + kk] : 0.0;
-                            dmma884(c0, c1, a[u], b0);
-                            dmma884(d0, d1, a[u + 1], b1);
-                            dmma884(e0, e1, a[u + 2], b2);
-                            dmma884(f0, f1, a[u + 3], b3);
-                        }
+                for (int u = 0; u < 16; u += 4) {
+                    if (k0 + 4 * u < J0) {  // J0 is a multiple of 8: k-steps come in pairs; zero-padded beyond J0
+                        const double b0 = sb[k0 + 4 * u + kk], b1 = k0 + 4 * u + 4 < J0 ? sb[k0 + 4 * u + 4 + kk] : 0.0;
+                        const double b2 = k0 + 4 * u + 8 < J0 ? sb[k0 + 4 * u + 8 + kk] : 0.0, b3 = k0 + 4 * u + 12 < J0 ? sb[k0 + 4 * u + 12 + kk] : 0.0;
+                        dmma884(c0, c1, a[u], b0);
+                        dmma884(d0, d1, a[u + 1], b1);
+                        dmma884(e0, e1, a[u + 2], b2);
+                        dmma884(f0, f1, a[u + 3], b3);
                     }
                 }
             }
@@ -481,8 +449,8 @@ __global__ void __launch_bounds__(SOLVE_THREADS) ba_solve_cam(BaCaps C, BaDev D,
 
 // ------------------------------------------------------------------------------------------------ solve_cam, distributed-shared-memory form
 // The same job as ba_solve_cam with the packed system RESIDENT IN THE CLUSTER'S SHARED MEMORY: nothing of the factorisation touches L2.
-// (The L2 form above spends each 8-column panel on 2 cluster barriers, the B operand, the A strips and the factored block all
-// fetched from L2 behind them.)
+// (The L2 form above spends each 8-column panel on 2 cluster barriers, both DMMA operands and the factored block all fetched from L2
+// behind them.)
 //
 // Layout.  The (N + 1) x (N + 1) augmented lower triangle (row N = right-hand side) is cut into 8 x 8 tiles, each stored row-major (64 doubles:
 // the DMMA C fragment of lane l is the 16 bytes at 2 l -- one conflict-free 128-bit access per lane).  Tile row T lives on CTA T mod 4; a CTA
@@ -499,7 +467,8 @@ __global__ void __launch_bounds__(SOLVE_THREADS) ba_solve_cam(BaCaps C, BaDev D,
 //   (3) cluster barrier (the stores have landed); the right-hand-side row's entries of the panel are y = L^-1 rhs.
 // Backward substitution L^T x = y, distributed: tile rows last to first; the owner of tile row T solves the 8 x 8 triangle (one warp), adds the
 // row's contributions to its own partial sums for the columns on the left and pushes the partial sums of the next three tile rows (final by
-// construction: its next own tile row is T - 4) to their owners' inboxes; one cluster barrier per tile row.
+// construction: its next own tile row is T - 4) to their owners' inboxes with st.async, each inbox counted by an mbarrier (point to point, no
+// cluster barrier on the chain).
 constexpr int DSM_CL = 4;
 static_assert(SOLVE_THREADS == 256 && DSM_CL == SPLIT_CLUSTER, "ba_solve_cam_dsm: warp r assembles row r of a tile row; one launch geometry for both forms");
 __host__ __device__ inline int dsm_tile_off(int cr, int m) { return m * cr + 2 * m * (m - 1); }  // tiles ahead of local tile row m (T = cr + 4 m)
@@ -527,9 +496,6 @@ __device__ __forceinline__ void dsm_mbar_arrive_local(unsigned bar) { asm volati
 __device__ __forceinline__ void dsm_mbar_arrive_expect_tx_remote(unsigned bar_cluster, unsigned tx) {
     asm volatile("mbarrier.arrive.expect_tx.release.cluster.shared::cluster.b64 _, [%0], %1;" ::"r"(bar_cluster), "r"(tx) : "memory");
 }
-__device__ __forceinline__ void st_async_v2(unsigned dst_cluster, double a, double b, unsigned bar_cluster) {
-    asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v2.f64 [%0], {%1, %2}, [%3];" ::"r"(dst_cluster), "d"(a), "d"(b), "r"(bar_cluster) : "memory");
-}
 __device__ __forceinline__ void st_async_f64(unsigned dst_cluster, double a, unsigned bar_cluster) {
     asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.f64 [%0], %1, [%2];" ::"r"(dst_cluster), "d"(a), "r"(bar_cluster) : "memory");
 }
@@ -552,11 +518,10 @@ __device__ __forceinline__ void dsm_mbar_wait(unsigned bar, unsigned parity, vol
     }
 }
 
-// variant: hand-over with asynchronous stores (st.async) + mbarriers carrying transaction counts instead of a cluster barrier -- bit 0: of the
-// panel column, bit 1: of the back-substitution's partial sums.  Measured with phase clocks: the panel hand-over is bound by the
-// SM-to-SM bandwidth either way and the cluster barrier is the cheaper form there; the back-substitution chain gains from the point-to-point form.
-constexpr int DSM_V_MBAR_PANEL = 1, DSM_V_MBAR_BSUB = 2;
-__global__ void __launch_bounds__(SOLVE_THREADS, 1) ba_solve_cam_dsm(BaCaps C, BaDev D, unsigned long long epoch, int variant) {
+// The panel column is handed over at one cluster barrier: the hand-over is bound by the SM-to-SM bandwidth either way, and the barrier is the
+// cheaper form; the back-substitution chain gains from point-to-point messages (st.async + an mbarrier carrying the transaction count), measured
+// with phase clocks against a cluster barrier per tile row.
+__global__ void __launch_bounds__(SOLVE_THREADS, 1) ba_solve_cam_dsm(BaCaps C, BaDev D, unsigned long long epoch) {
     extern __shared__ double sm[];
     cg::cluster_group cluster = cg::this_cluster();
     constexpr int CL = DSM_CL;
@@ -565,7 +530,6 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 1) ba_solve_cam_dsm(BaCaps C, B
     if (w % D.world != D.rank) return;   // uniform over the cluster
     LmState &st = D.st[w];
     if (st.done) return;
-    const bool use_mbar = variant & DSM_V_MBAR_PANEL, bsub_mbar = variant & DSM_V_MBAR_BSUB;
     const WinDims dm = D.dims[w];
     const int K = dm.K, NCV = 6 * K + 7, N = 15 * K + 7, NR = N + 1;
     const int ntc = dsm_ntiles(C.N + 1), VL = ntc * 8;   // capacity: tiles per side, vector length
@@ -586,8 +550,8 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 1) ba_solve_cam_dsm(BaCaps C, B
     double *s_dv = s_Lf + 64;                 // 8: its reciprocal pivots
     double *s_inbox = s_dv + 8;               // [CL][8]
     double *s_xT = s_inbox + 8 * CL;          // 8
-    int *s_fail = (int *) (s_xT + 8);         // [0] breakdown, [1] a bounded wait ran out; then the mbarriers (8 doubles reserved)
-    unsigned long long *s_bar = (unsigned long long *) (s_xT + 12);  // [0], [1]: panel column by parity; [2]: back-substitution inbox
+    int *s_fail = (int *) (s_xT + 8);         // [0] breakdown, [1] a bounded wait ran out; then the mbarrier (8 doubles reserved)
+    unsigned long long *s_bar = (unsigned long long *) (s_xT + 12);  // the back-substitution inbox
     double *s_dg = s_xT + 16;                 // [ntc][64] replicated diagonal tiles
     double *s_P = s_dg + (size_t) ntc * 64;   // [2][ntc][64] panel column, by panel parity
     double *s_tiles = s_P + (size_t) 2 * ntc * 64;
@@ -611,7 +575,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 1) ba_solve_cam_dsm(BaCaps C, B
     if (tid < 8 * CL) s_inbox[tid] = 0;
     if (tid == 0) {
         s_fail[0] = 0, s_fail[1] = 0;
-        dsm_mbar_init(smem_u32(s_bar), CL), dsm_mbar_init(smem_u32(s_bar + 1), CL), dsm_mbar_init(smem_u32(s_bar + 2), CL - 1);
+        dsm_mbar_init(smem_u32(s_bar), CL - 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -722,13 +686,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 1) ba_solve_cam_dsm(BaCaps C, B
     for (int J = 0; J < npan; J++) {
         const int nb = min(8, N - 8 * J);
         const double *PJ = s_P + (size_t) ((J - 1) & 1) * ntc * 64;   // panel J - 1's solved rows (J > 0)
-        const unsigned long long tc0 = DSM_NOW();
-        (void) tc0;
-        if (J > 0) {
-            if (use_mbar) dsm_mbar_wait(smem_u32(s_bar + ((J - 1) & 1)), ((J - 1) >> 1) & 1, s_dead, D.S.err);   // panel J - 1's column has landed
-            if (tid < 8 && Tn > J - 1) s_y[8 * (J - 1) + tid] = PJ[(size_t) Tn * 64 + rn * 8 + tid];         // its right-hand-side entries: y
-        }
-        DSM_CLK2(0, tc0)  // wait for the panel column
+        if (J > 0 && tid < 8 && Tn > J - 1) s_y[8 * (J - 1) + tid] = PJ[(size_t) Tn * 64 + rn * 8 + tid];   // its right-hand-side entries: y
         const unsigned long long tc1 = DSM_NOW();
         (void) tc1;
         if (J > 0 && worker) {
@@ -885,33 +843,14 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 1) ba_solve_cam_dsm(BaCaps C, B
                 double *dstP = s_P + (size_t) (J & 1) * ntc * 64 + (size_t) T * 64 + r * 8;
 #pragma unroll
                 for (int c = 0; c < 8; c += 2) *(double2 *) (tp + c) = make_double2(x[c], x[c + 1]);
-                if (use_mbar) {
-                    const unsigned a0 = smem_u32(dstP), b0 = smem_u32(s_bar + (J & 1));
 #pragma unroll
-                    for (int q = 0; q < CL; q++) {
-                        const unsigned ap = mapa_u32(a0, q), ab = mapa_u32(b0, q);
+                for (int q = 0; q < CL; q++) {
+                    double *rp = cluster.map_shared_rank(dstP, q);
 #pragma unroll
-                        for (int c = 0; c < 8; c += 2) st_async_v2(ap + 8u * c, x[c], x[c + 1], ab);
-                    }
-                } else {
-#pragma unroll
-                    for (int q = 0; q < CL; q++) {
-                        double *rp = cluster.map_shared_rank(dstP, q);
-#pragma unroll
-                        for (int c = 0; c < 8; c += 2) *(double2 *) (rp + c) = make_double2(x[c], x[c + 1]);
-                    }
+                    for (int c = 0; c < 8; c += 2) *(double2 *) (rp + c) = make_double2(x[c], x[c + 1]);
                 }
             }
-            if (use_mbar) {
-                // every CTA arrives on every CTA's barrier of this panel (also with nothing sent: the arrival says "I am done reading the
-                // buffer of panel J - 1", which the receiver's next-but-one panel overwrites) and announces its bytes
-                if (tid < CL) {
-                    const int nloc = cr + CL * m0 < nt ? (nt - 1 - (cr + CL * m0)) / CL + 1 : 0;   // local tile rows below the panel
-                    dsm_mbar_arrive_expect_tx_remote(mapa_u32(smem_u32(s_bar + (J & 1)), tid), 512u * nloc);
-                }
-            } else {
-                cluster.sync();
-            }
+            cluster.sync();
         }
         DSM_CLK(3, tc2)  // row solves + hand-over
     }
@@ -922,7 +861,6 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 1) ba_solve_cam_dsm(BaCaps C, B
     if (valid) {
         {   // the last panel's column (only the right-hand-side row can be below it)
             const int J = npan - 1;
-            if (use_mbar) dsm_mbar_wait(smem_u32(s_bar + (J & 1)), (J >> 1) & 1, s_dead, D.S.err);
             if (tid < 8 && Tn > J) s_y[8 * J + tid] = s_P[(size_t) (J & 1) * ntc * 64 + (size_t) Tn * 64 + rn * 8 + tid];
         }
         if (rn > 0 && tid == 0) {   // the right-hand-side row shares the last diagonal tile with the last rn columns
@@ -959,12 +897,10 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 1) ba_solve_cam_dsm(BaCaps C, B
 #pragma unroll
                         for (int r = 0; r < 8; r++) tcr[r] = 0;
                     }
-                    if (bsub_mbar) {
-                        // three messages per tile row (from the owners of T + 1 .. T + 3); the ones that do not exist are arrived here
-                        const int nmiss = max(0, 3 - (npan - 1 - T));
-                        if (lane < nmiss) dsm_mbar_arrive_local(smem_u32(s_bar + 2));
-                        dsm_mbar_wait(smem_u32(s_bar + 2), ((npan - 1 - T) / CL) & 1, s_dead, D.S.err);
-                    }
+                    // three messages per tile row (from the owners of T + 1 .. T + 3); the ones that do not exist are arrived here
+                    const int nmiss = max(0, 3 - (npan - 1 - T));
+                    if (lane < nmiss) dsm_mbar_arrive_local(smem_u32(s_bar));
+                    dsm_mbar_wait(smem_u32(s_bar), ((npan - 1 - T) / CL) & 1, s_dead, D.S.err);
                     double v = 0;
                     if (lane < nbT) {
                         v = s_y[8 * T + c] - s_contrib[8 * T + c];
@@ -984,13 +920,9 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 1) ba_solve_cam_dsm(BaCaps C, B
                     if (lane < ncrit) {
                         s_contrib[col] = acc;
                         const int q = (col >> 3) % CL;
-                        if (bsub_mbar) {
-                            const unsigned abar = mapa_u32(smem_u32(s_bar + 2), q);
-                            st_async_f64(mapa_u32(smem_u32(s_inbox + cr * 8 + (col & 7)), q), acc, abar);
-                            if ((col & 7) == 0) dsm_mbar_arrive_expect_tx_remote(abar, 64u);
-                        } else {
-                            cluster.map_shared_rank(s_inbox, q)[cr * 8 + (col & 7)] = acc;
-                        }
+                        const unsigned abar = mapa_u32(smem_u32(s_bar), q);
+                        st_async_f64(mapa_u32(smem_u32(s_inbox + cr * 8 + (col & 7)), q), acc, abar);
+                        if ((col & 7) == 0) dsm_mbar_arrive_expect_tx_remote(abar, 64u);
                     }
                 }
                 __syncthreads();
@@ -1003,7 +935,6 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 1) ba_solve_cam_dsm(BaCaps C, B
                 }
                 __syncthreads();
             }
-            if (!bsub_mbar) cluster.sync();
         }
     }
     cluster.sync();  // the solution has landed on CTA 0; no CTA leaves while its shared memory may still be written

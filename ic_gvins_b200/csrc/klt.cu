@@ -618,10 +618,9 @@ __device__ __forceinline__ void lk_track_point(const KltMaps &maps, const KltArg
     if (err_out != nullptr) *err_out = status ? err_val : 0.f;
 }
 
-// MINB = resident CTAs per SM the register allocation is held to: 5 (<= 102 registers, a few spills) or 4 (128 registers, no spills, fewer
-// instructions); the host picks (ICG_KLT_MINB, default 4)
-template <int MINB>
-__global__ void __launch_bounds__(KLT_WPB * 32, MINB) klt_track_kernel(const __grid_constant__ KltMaps maps, const KltArgs A) {
+// held to 4 resident CTAs per SM (<= 128 registers, no spills): measured faster than the 5-CTA bound, whose register cap (<= 102) costs
+// more instructions
+__global__ void __launch_bounds__(KLT_WPB * 32, 4) klt_track_kernel(const __grid_constant__ KltMaps maps, const KltArgs A) {
     __shared__ __align__(128) uint8_t s_iw[KLT_WPB][KLT_BOXW * KLT_BOXH_I];
     __shared__ __align__(128) uint8_t s_jw[KLT_WPB][KLT_BOXW * KLT_BOXH_J];
     __shared__ __align__(16) int s_pg[KLT_WPB][26 * 24];
@@ -950,11 +949,7 @@ static int launch_track(icg_klt *h, int n_total, const int32_t *d_slots, const f
     A.status = d_status;
     A.err = d_err;
     int grid = (n_total + KLT_WPB - 1) / KLT_WPB;
-    static const int minb = getenv("ICG_KLT_MINB") ? atoi(getenv("ICG_KLT_MINB")) : 4;
-    if (minb == 5)
-        klt_track_kernel<5><<<grid, KLT_WPB * 32, 0, h->stream>>>(h->maps, A);
-    else
-        klt_track_kernel<4><<<grid, KLT_WPB * 32, 0, h->stream>>>(h->maps, A);
+    klt_track_kernel<<<grid, KLT_WPB * 32, 0, h->stream>>>(h->maps, A);
     ICG_CHECK_LAUNCH();
     count_launch();
     return ICG_OK;

@@ -256,6 +256,30 @@ def test_cfg4_window_solve_matches_oracle(olib, solver_cfg4, name):
     _compare_solution(pg, po)
 
 
+@pytest.fixture(scope="module")
+def solver_k24():
+    from ic_gvins_b200.ba import WindowSolver
+    s = WindowSolver(max_windows=1, max_K=24, max_L=300, max_F=4000, max_gnss=16, max_marg_r=64)
+    yield s
+    s.close()
+
+
+def test_l2_cluster_solve_matches_oracle(olib, solver_k24):
+    """max_K = 24 (n = 367): the packed system no longer fits the cluster's shared memory, so the split pipeline solves it with
+    ba_solve_cam (packed S in L2) instead of ba_solve_cam_dsm.  Landmarks anchored over 20 nodes, so that the vision blocks reach across the
+    window.  Solution within 1e-6 relative of the oracle, same LM trajectory."""
+    prob, _ = make(olib, K=24, L=300, seed=2031, n_ref=20)
+    assert prob["F"] <= 4000
+    po, pg = copy.deepcopy(prob), copy.deepcopy(prob)
+    so = oa.ba_solve(olib, po, 20)
+    sg = solver_k24.solve(pg, 20)[0]
+    assert sg["iterations"] == so["iterations"] and sg["num_successful_steps"] == so["num_successful_steps"]
+    assert sg["termination"] == so["termination"]
+    assert abs(sg["initial_cost"] - so["initial_cost"]) <= 1e-9 * so["initial_cost"]
+    assert abs(sg["final_cost"] - so["final_cost"]) <= 1e-7 * so["final_cost"]
+    _compare_solution(pg, po)
+
+
 def test_cfg4_two_pass_protocol_matches_oracle(olib, solver_cfg4):
     prob, _ = make(olib, K=20, L=2000, seed=2030)
     fc = prob["f_const"].reshape(-1, 14)

@@ -3,11 +3,10 @@
 Not a test of the CUDA code (tests/test_ba_gpu.py compares the kernel with the oracle through the C ABI): this pins the ALGORITHM the kernel
 implements -- the tile layout (tile row T on CTA T mod 4, strictly-lower tiles, replicated diagonal tiles), the right-looking panel loop with the
 panel column all-gathered into every CTA, the right-hand side carried as an augmented row, and the distributed backward substitution whose
-partial sums travel point to point -- and the two invariants its barriers rely on:
-  * every panel, every CTA announces itself to every CTA (4 arrivals per panel barrier) and the bytes it announces are the bytes it sends;
+partial sums travel point to point -- and the invariant its back-substitution mbarrier relies on:
   * every tile row of the backward substitution receives exactly three partial-sum messages, counting the local arrivals that stand in for
     senders that do not exist (the mbarrier's arrival count is 3).
-A schedule that violates either would not give wrong numbers on the GPU, it would hang a cluster (the kernel bounds its waits and raises the
+A schedule that violates it would not give wrong numbers on the GPU, it would hang a cluster (the kernel bounds its waits and raises the
 handle's error word instead).  Reference for what is solved: Ceres' DENSE_SCHUR reduced camera system of IG/ic_gvins.cc:1130-1239 at 20
 keyframes (n = 15 K + 7 = 307).
 """
@@ -59,24 +58,15 @@ def solve_dsm(S, rhs):
             Lf = Lc
             if cr == 0:
                 dinv[8 * J:8 * J + nb] = 1.0 / np.diag(Lc)[:nb]
-        arrivals, announced, sent = np.zeros(CL, int), np.zeros(CL, int), np.zeros(CL, int)
         for cr in range(CL):  # row solves; every solved row goes to all four CTAs
             m0 = (J + 1 - cr + CL - 1) // CL
             nloc = (nt - 1 - (cr + CL * m0)) // CL + 1 if cr + CL * m0 < nt else 0
-            rows = 0
             for m in range(m0, m0 + nloc):
                 T = cr + CL * m
                 x = np.linalg.solve(Lf, tiles[cr][tile_off(cr, m) + J].T).T
                 tiles[cr][tile_off(cr, m) + J] = x
                 for q in range(CL):
                     P[q][J & 1][T] = x
-                    sent[q] += 512
-                rows += 1
-            assert rows == nloc
-            for q in range(CL):
-                arrivals[q] += 1
-                announced[q] += 512 * nloc
-        assert (arrivals == CL).all() and (announced == sent).all()
         if Tn > J:
             y[8 * J:8 * J + 8] = P[0][J & 1][Tn][rn]
     if rn > 0:  # the right-hand-side row shares the last diagonal tile with the last rn columns
