@@ -394,6 +394,72 @@ class WindowSolver:
         check(lib().icg_ba_slide_resident(self._h, n, arr, cw), "icg_ba_slide_resident")
         self._keep, self._n = arr, n
 
+    def slide_integrate(self, next_problems, carry, integrate, noise5, station=(0.0, 0.0, 0.0), prior_from_marg=True):
+        """slide() whose new IMU factors, new node rows and aligned GNSS fixes are computed on the device from the states this handle holds
+        (icg_ba_slide_integrate_resident: the host halves of addNewTimeNode, removeUnusedTimeNode and insertNewGnssTimeNode, IG/ic_gvins.cc:754-928).
+        Only rows that `carry` leaves to next_problems are read.  integrate: one dict per window (None: nothing integrated) with
+          imu_from       n_imu int32: -1 next's blob, i >= 0 from old node i's state, SLIDE_CHAIN from the previous factor's end, SLIDE_ROW from state16
+          imu_rows       n_imu entries: the (m, 7) rows (dt, dtheta, dvel) of an integrated factor, None otherwise
+                         (or `imu` + `imu_off` as the C call takes them)
+          gravity        3, or n_imu x 3;  normal: one flag or n_imu (PreintegrationNormal; default Earth);  state16: n_imu x 16 (SLIDE_ROW)
+          node_from_imu  K flags: node j is the end state of integrated factor j - 1
+          gnss_node, gnss_dt  n_gnss: old node whose velocity moves the fix by dt (-1: none)
+        noise5 = gyr_arw, acc_vrw, gyr_bias_std, acc_bias_std, corr_time; station = parameters_->station.  Returns one dict per window: status
+        (n_imu int8: 1 integrated, 0 not, -1 not positive definite), blobs (n_imu x 480) and end_states (n_imu x 10), zero where status is 0.
+        A rejected call raises IcgError with the handle unchanged; after the integration its `results` holds the dicts."""
+        from ._lib import IcgError, SlideIntegrate, SlideWindow, u8p
+        n = len(next_problems)
+        flags = [prior_from_marg] * n if np.isscalar(prior_from_marg) else list(prior_from_marg)
+        arr = (BaProblem * n)(*[to_struct(p) for p in next_problems])
+        cw = (SlideWindow * n)()
+        iw = (SlideIntegrate * n)()
+        keep, outs = [], []
+
+        def arg(a, dtype, ptr):
+            a = np.ascontiguousarray(a, dtype)
+            keep.append(a)
+            return a.ctypes.data_as(ptr)
+
+        for w, (p, c, g) in enumerate(zip(next_problems, carry, integrate)):
+            for k in ("node_src", "lm_src", "f_src", "imu_src", "gnss_src"):
+                if c.get(k) is not None:
+                    setattr(cw[w], k, arg(c[k], np.int32, ip))
+            cw[w].prior_from_marg = 1 if flags[w] else 0
+            m = int(p["n_imu"])
+            o = dict(status=np.zeros(m, np.int8), blobs=np.zeros((m, IMU_BLOB)), end_states=np.zeros((m, 10)))
+            outs.append(o)
+            iw[w].status, iw[w].blob_out = o["status"].ctypes.data_as(C.POINTER(C.c_int8)), o["blobs"].ctypes.data_as(dp)
+            iw[w].end_state10 = o["end_states"].ctypes.data_as(dp)
+            if not g:
+                continue
+            if g.get("imu_from") is not None:
+                iw[w].imu_from = arg(g["imu_from"], np.int32, ip)
+                if "imu_off" in g:
+                    imu, off = g["imu"], g["imu_off"]
+                else:
+                    rows = [np.zeros((0, 7)) if r is None else np.asarray(r, np.float64).reshape(-1, 7) for r in g["imu_rows"]]
+                    off = np.zeros(m + 1, np.int32)
+                    off[1:] = np.cumsum([len(r) for r in rows])
+                    imu = np.concatenate(rows, axis=0) if rows else np.zeros((0, 7))
+                iw[w].imu, iw[w].imu_off = arg(imu, np.float64, dp), arg(off, np.int32, ip)
+                iw[w].gravity3 = arg(np.broadcast_to(np.asarray(g["gravity"], np.float64), (m, 3)), np.float64, dp)
+                iw[w].normal = arg(np.broadcast_to(np.asarray(g.get("normal", False), np.uint8), (m,)), np.uint8, u8p)
+                if g.get("state16") is not None:
+                    iw[w].state16 = arg(g["state16"], np.float64, dp)
+            if g.get("node_from_imu") is not None:
+                iw[w].node_from_imu = arg(g["node_from_imu"], np.uint8, u8p)
+            if g.get("gnss_node") is not None:
+                iw[w].gnss_node, iw[w].gnss_dt = arg(g["gnss_node"], np.int32, ip), arg(g["gnss_dt"], np.float64, dp)
+        nz = np.ascontiguousarray(noise5, np.float64)
+        stn = np.ascontiguousarray(station, np.float64)
+        rc = lib().icg_ba_slide_integrate_resident(self._h, n, arr, cw, iw, vp(nz.ctypes.data), vp(stn.ctypes.data))
+        if rc != 0:
+            err = IcgError(f"icg_ba_slide_integrate_resident failed with code {rc}: {lib().icg_last_error().decode('utf-8', 'replace')}")
+            err.code, err.results = rc, outs
+            raise err
+        self._keep, self._n = arr, n
+        return outs
+
     def gvins_optimization_end(self, problems):
         """icg_ba_gvins_optimization_end after run_gvins(): synchronises, writes the parameters, f_active and gnss_std back into the problem
         dicts and returns the two-pass results in the layout of gvins_optimization_batch."""

@@ -3347,12 +3347,14 @@ int icg_ba_marginalize_resident_culled(icg_ba *h, int n_windows, const icg_ba_pr
 }
 
 // ---- the next keyframe's windows from the resident ones (ba_slide.cu): the structure is packed on the host as icg_ba_upload packs it, the
-//      values of the carried rows never leave the device
-int icg_ba_slide_resident(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba_slide_window *carry) {
-    int rc = resident_single_rank(h, n, next, "icg_ba_slide_resident");
+//      values of the carried rows never leave the device.  With `integ`, the new factors, node rows and aligned fixes it names are computed on
+//      the device (preint.cu) into the staged value rows before the gather reads them.
+static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba_slide_window *carry, const icg_ba_slide_integrate *integ,
+                      const double *noise5, const double *station3, const char *fn) {
+    int rc = resident_single_rank(h, n, next, fn);
     if (rc != ICG_OK) return rc;
-    if (!carry) {
-        set_error("icg_ba_slide_resident: bad arguments");
+    if (!carry || (integ && (!noise5 || !station3))) {
+        set_error("%s: bad arguments", fn);
         return ICG_EINVAL;
     }
     ICG_CUDA(cudaSetDevice(h->device));
@@ -3362,12 +3364,12 @@ int icg_ba_slide_resident(icg_ba *h, int n, const icg_ba_problem *next, const ic
         const icg_ba_problem &p = next[w];
         if (!carry[w].prior_from_marg) continue;
         if (h->marg_res_n != n) {
-            set_error("icg_ba_slide_resident: window %d takes its prior from the marginalization, but no resident marginalization of these %d windows "
-                      "ran since the last upload or slide", w, n);
+            set_error("%s: window %d takes its prior from the marginalization, but no resident marginalization of these %d windows "
+                      "ran since the last upload or slide", fn, w, n);
             return ICG_EINVAL;
         }
         if (h->marg_res_m[w] <= 0 || p.marg_r != h->marg_res_r[w] || p.marg_nblocks != h->marg_res_nb[w]) {
-            set_error("icg_ba_slide_resident: window %d: marg_r=%d / marg_nblocks=%d, but the resident marginalization left m=%d, r=%d / nblocks=%d", w,
+            set_error("%s: window %d: marg_r=%d / marg_nblocks=%d, but the resident marginalization left m=%d, r=%d / nblocks=%d", fn, w,
                       p.marg_r, p.marg_nblocks, h->marg_res_m[w], h->marg_res_r[w], h->marg_res_nb[w]);
             return ICG_EINVAL;
         }
@@ -3378,7 +3380,7 @@ int icg_ba_slide_resident(icg_ba *h, int n, const icg_ba_problem *next, const ic
     if (!h->slide_old && (cudaMalloc(&h->slide_old, sizeof(double) * n_old) != cudaSuccess ||
                           cudaMalloc(&h->fc_alt, sizeof(double) * NW * C.F * 14) != cudaSuccess)) {
         if (h->slide_old) cudaFree(h->slide_old), h->slide_old = nullptr;
-        set_error("icg_ba_slide_resident: allocation of the slide buffers failed");
+        set_error("%s: allocation of the slide buffers failed", fn);
         return ICG_ENOMEM;
     }
     // the old windows: sizes, and every factor's record slot (the inverse of the last packing's slot -> factor table)
@@ -3417,7 +3419,7 @@ int icg_ba_slide_resident(icg_ba *h, int n, const icg_ba_problem *next, const ic
         for (int t = 0; t < 5; t++)
             for (int i = 0; maps[t] && i < cnt[t]; i++) {
                 if (maps[t][i] < -1 || maps[t][i] >= lim[t]) {
-                    set_error("icg_ba_slide_resident: window %d: %s[%d] = %d is out of range of the old window (%d)", w, names[t], i, maps[t][i], lim[t]);
+                    set_error("%s: window %d: %s[%d] = %d is out of range of the old window (%d)", fn, w, names[t], i, maps[t][i], lim[t]);
                     return fail(ICG_EINVAL);
                 }
                 if (maps[t][i] >= 0) continue;
@@ -3434,13 +3436,93 @@ int icg_ba_slide_resident(icg_ba *h, int n, const icg_ba_problem *next, const ic
         max_elems = std::max(max_elems, SLIDE_NODE * p.K + p.L + 14 * p.F + SLIDE_IMU * p.n_imu + SLIDE_GNSS * p.n_gnss);
         max_r = std::max(max_r, W.r);
     }
-    if (n_val >= (size_t) INT32_MAX || n_map >= (size_t) INT32_MAX) {
-        set_error("icg_ba_slide_resident: too many new value rows in one call");
+    // the integration's arrays (only rows the carry maps leave to next are read): every check before anything is staged
+    std::vector<std::vector<int>> item_of(integ ? n : 0);  // per window and new factor: its item, or -1
+    std::vector<int> iwin_of(integ ? n : 0, -1);           // per window: its entry of iwins, or -1
+    std::vector<SlideIntWin> iwins;                         // the windows with device work, one warp each
+    std::vector<size_t> row_base(integ ? n : 0), state_base(integ ? n : 0);
+    size_t n_item = 0, n_align = 0, n_row = 0, n_state = 0;
+    bool want_blob = false;
+    for (int w = 0; integ && w < n; w++) {
+        const icg_ba_problem &p = next[w];
+        const icg_ba_slide_window &c = carry[w];
+        const icg_ba_slide_integrate &g = integ[w];
+        const int oK = old_dims[w].K;
+        std::vector<int> &io = item_of[w];
+        io.assign(p.n_imu, -1);
+        const size_t item0 = n_item, align0 = n_align;
+        row_base[w] = n_row, state_base[w] = n_state;
+        for (int k = 0; g.imu_from && k < p.n_imu; k++) {
+            const int src = g.imu_from[k];
+            if ((c.imu_src && c.imu_src[k] >= 0) || src == -1) continue;
+            if (src >= oK || (src < 0 && src != ICG_SLIDE_CHAIN && src != ICG_SLIDE_ROW)) {
+                set_error("%s: window %d: imu_from[%d] = %d is out of range of the old window (%d)", fn, w, k, src, oK);
+                return fail(ICG_EINVAL);
+            }
+            if (src == ICG_SLIDE_CHAIN && (k == 0 || io[k - 1] < 0)) {
+                set_error("%s: window %d: imu_from[%d] is ICG_SLIDE_CHAIN, but no integrated factor precedes it", fn, w, k);
+                return fail(ICG_EINVAL);
+            }
+            if (!g.gravity3 || !g.imu || !g.imu_off || (src == ICG_SLIDE_ROW && !g.state16)) {
+                set_error("%s: window %d: arrays missing", fn, w);
+                return fail(ICG_EINVAL);
+            }
+            if (g.imu_off[k] < 0 || (long long) g.imu_off[k + 1] - g.imu_off[k] < 1) {
+                set_error("%s: window %d factor %d: imu_off must give every integrated interval at least one row", fn, w, k);
+                return fail(ICG_EINVAL);
+            }
+            io[k] = (int) n_item++;
+            n_row += (size_t) (g.imu_off[k + 1] - g.imu_off[k]);
+            n_state += src == ICG_SLIDE_ROW;
+        }
+        for (int j = 0; g.node_from_imu && j < p.K; j++) {
+            if ((c.node_src && c.node_src[j] >= 0) || !g.node_from_imu[j]) continue;
+            if (j == 0 || j - 1 >= p.n_imu || io[j - 1] < 0) {
+                set_error("%s: window %d: node_from_imu[%d] is set, but factor %d is not integrated", fn, w, j, j - 1);
+                return fail(ICG_EINVAL);
+            }
+        }
+        for (int q = 0; g.gnss_node && q < p.n_gnss; q++) {
+            if ((c.gnss_src && c.gnss_src[q] >= 0) || g.gnss_node[q] == -1) continue;
+            if (g.gnss_node[q] < -1 || g.gnss_node[q] >= oK) {
+                set_error("%s: window %d: gnss_node[%d] = %d is out of range of the old window (%d)", fn, w, q, g.gnss_node[q], oK);
+                return fail(ICG_EINVAL);
+            }
+            if (!g.gnss_dt) {
+                set_error("%s: window %d: arrays missing", fn, w);
+                return fail(ICG_EINVAL);
+            }
+            n_align++;
+        }
+        if (n_item == item0 && n_align == align0) continue;
+        iwin_of[w] = (int) iwins.size();
+        iwins.push_back(SlideIntWin{w, (int) item0, (int) (n_item - item0), (int) align0, (int) (n_align - align0)});
+        want_blob = want_blob || (g.blob_out && n_item > item0);
+    }
+    if (n_val >= (size_t) INT32_MAX || n_map >= (size_t) INT32_MAX || n_row >= (size_t) INT32_MAX / 8 || n_item >= (size_t) INT32_MAX / 8) {
+        set_error("%s: too many new value rows in one call", fn);
         return fail(ICG_EINVAL);
     }
-    // staging: [windows | maps | new value rows] in one pinned buffer, one H2D
+    // staging: [windows | maps | new value rows] in one pinned buffer, one H2D; with device work also [its windows | items | alignments |
+    // IMU rows | ICG_SLIDE_ROW states] (up to in_end) and the outputs that come back, [status | end states | blobs]
     auto al = [](size_t b) { return (b + 15) & ~(size_t) 15; };
-    const size_t b_map = al(sizeof(SlideWin) * n), b_val = b_map + al(sizeof(int) * n_map), total = b_val + sizeof(double) * n_val;
+    const size_t b_map = al(sizeof(SlideWin) * n), b_val = b_map + al(sizeof(int) * n_map);
+    size_t total = b_val + sizeof(double) * n_val;
+    auto take = [&](size_t bytes) {
+        const size_t o = al(total);
+        total = o + bytes;
+        return o;
+    };
+    size_t b_iw = 0, b_item = 0, b_align = 0, b_rows = 0, b_state = 0, b_status = 0, b_ends = 0, b_blob = 0;
+    if (!iwins.empty()) {
+        b_iw = take(sizeof(SlideIntWin) * iwins.size()), b_item = take(sizeof(SlideItem) * n_item), b_align = take(sizeof(SlideAlign) * n_align);
+        b_rows = take(56 * n_row), b_state = take(128 * n_state);
+    }
+    const size_t in_end = total;
+    if (!iwins.empty()) {
+        b_status = take(n_item), b_ends = take(80 * n_item);
+        if (want_blob) b_blob = take(sizeof(double) * ICG_IMU_BLOB_DOUBLES * n_item);
+    }
     cudaStream_t s = h->stream;
     if (total > h->slide_cap) {
         ICG_CUDA(cudaStreamSynchronize(s));  // an earlier slide's copy may still read the old buffer
@@ -3449,7 +3531,7 @@ int icg_ba_slide_resident(icg_ba *h, int n, const icg_ba_problem *next, const ic
         h->slide_cap = 0;
         const size_t cap = total + total / 4;
         if (cudaMallocHost(&h->slide_h, cap) != cudaSuccess || cudaMalloc(&h->slide_d, cap) != cudaSuccess) {
-            set_error("icg_ba_slide_resident: staging allocation of %zu bytes failed", cap);
+            set_error("%s: staging allocation of %zu bytes failed", fn, cap);
             return fail(ICG_ENOMEM);
         }
         h->slide_cap = cap;
@@ -3459,11 +3541,16 @@ int icg_ba_slide_resident(icg_ba *h, int n, const icg_ba_problem *next, const ic
     if (!h->slide_ev) ICG_CUDA(cudaEventCreateWithFlags(&h->slide_ev, cudaEventDisableTiming));
     int *map = (int *) (h->slide_h + b_map);
     double *val = (double *) (h->slide_h + b_val);
-    // per window: its slices of the maps and of the values are disjoint, so the windows are staged on a few host threads, as pack_windows packs
-    // them (the square-root information of every new blob is a 15 x 15 factorisation)
+    SlideItem *items = (SlideItem *) (h->slide_h + b_item);
+    SlideAlign *aligns = (SlideAlign *) (h->slide_h + b_align);
+    double *rows = (double *) (h->slide_h + b_rows), *states = (double *) (h->slide_h + b_state);
+    // per window: its slices of the maps, the values and the integration's inputs are disjoint, so the windows are staged on a few host
+    // threads, as pack_windows packs them (the square-root information of every new blob is a 15 x 15 factorisation).  A row the device
+    // computes gets its value slot here and is written there.
     auto stage_window = [&](int w, std::string &err) -> int {
         const icg_ba_problem &p = next[w];
         const icg_ba_slide_window &c = carry[w];
+        const icg_ba_slide_integrate *g = integ && iwin_of[w] >= 0 ? &integ[w] : nullptr;
         SlideWin &W = wins[w];
         int vo = (int) vbase[w];
         auto stage = [&](const double *src, int count) {
@@ -3472,9 +3559,14 @@ int icg_ba_slide_resident(icg_ba *h, int n, const icg_ba_problem *next, const ic
             vo += count;
             return -(at + 1);
         };
+        std::vector<int> node_at(g ? p.K + 1 : 0, -1);  // value offset of a node row the device writes
         for (int k = 0; k < p.K; k++) {
             if (c.node_src && c.node_src[k] >= 0) {
                 map[W.node_map + k] = c.node_src[k];
+                continue;
+            }
+            if (g && g->node_from_imu && g->node_from_imu[k]) {
+                node_at[k] = vo, map[W.node_map + k] = -(vo + 1), vo += SLIDE_NODE;
                 continue;
             }
             map[W.node_map + k] = stage(p.pose + 7 * (size_t) k, 7);
@@ -3486,28 +3578,46 @@ int icg_ba_slide_resident(icg_ba *h, int n, const icg_ba_problem *next, const ic
             const int f = fidx[q];
             map[W.slot_map + q] = c.f_src && c.f_src[f] >= 0 ? old_slot[w][c.f_src[f]] : stage(p.f_const + 14 * (size_t) f, 14);
         }
+        size_t row_at = g ? row_base[w] : 0, state_at = g ? state_base[w] : 0;
         for (int k = 0; k < p.n_imu; k++) {
             if (c.imu_src && c.imu_src[k] >= 0) {
                 map[W.imu_map + k] = c.imu_src[k];
+                continue;
+            }
+            if (g && item_of[w][k] >= 0) {
+                SlideItem &it = items[item_of[w][k]];
+                const int r0 = g->imu_off[k], nr = g->imu_off[k + 1] - r0;
+                it.src = g->imu_from[k], it.row0 = (int) row_at, it.nrow = nr, it.state = -1, it.blob = vo, it.node = node_at[k + 1];
+                it.normal = g->normal && g->normal[k] ? 1 : 0;
+                for (int i = 0; i < 3; i++) it.grav[i] = g->gravity3[3 * (size_t) k + i];
+                memcpy(rows + 7 * row_at, g->imu + 7 * (size_t) r0, 56 * (size_t) nr);
+                row_at += nr;
+                if (it.src == ICG_SLIDE_ROW) {
+                    memcpy(states + 16 * state_at, g->state16 + 16 * (size_t) k, 128);
+                    it.state = (int) (16 * state_at++);
+                }
+                map[W.imu_map + k] = -(vo + 1), vo += SLIDE_IMU;
                 continue;
             }
             const double *b = p.imu_blob + (size_t) k * ICG_IMU_BLOB_DOUBLES;
             map[W.imu_map + k] = stage(b, ICG_IMU_BLOB_DOUBLES);
             if (!host_imu_sqrt_info(b + 252, val + vo)) {
                 char eb[256];
-                snprintf(eb, sizeof(eb), "icg_ba_slide_resident: window %d IMU factor %d has a non positive-definite covariance", w, k);
+                snprintf(eb, sizeof(eb), "%s: window %d IMU factor %d has a non positive-definite covariance", fn, w, k);
                 err = eb;
                 return ICG_EINVAL;
             }
             vo += 225;
         }
-        for (int g = 0; g < p.n_gnss; g++) {
-            if (c.gnss_src && c.gnss_src[g] >= 0) {
-                map[W.gnss_map + g] = c.gnss_src[g];
+        int align_at = g ? iwins[iwin_of[w]].align0 : 0;
+        for (int q = 0; q < p.n_gnss; q++) {
+            if (c.gnss_src && c.gnss_src[q] >= 0) {
+                map[W.gnss_map + q] = c.gnss_src[q];
                 continue;
             }
-            map[W.gnss_map + g] = stage(p.gnss_blh + 3 * (size_t) g, 3);
-            stage(p.gnss_std + 3 * (size_t) g, 3);
+            map[W.gnss_map + q] = stage(p.gnss_blh + 3 * (size_t) q, 3);
+            stage(p.gnss_std + 3 * (size_t) q, 3);
+            if (g && g->gnss_node && g->gnss_node[q] >= 0) aligns[align_at++] = SlideAlign{-(map[W.gnss_map + q] + 1), g->gnss_node[q], g->gnss_dt[q]};
         }
         if (W.r > 0 && !W.from_marg) {
             W.j0 = -(stage(p.marg_J0, W.r * W.r) + 1);
@@ -3533,9 +3643,50 @@ int icg_ba_slide_resident(icg_ba *h, int n, const icg_ba_problem *next, const ic
             }
     }
     memcpy(h->slide_h, wins.data(), sizeof(SlideWin) * n);
+    if (integ) {
+        // the device work writes the staging only; a covariance that is not positive definite is known after it, so the call waits for it
+        if (!iwins.empty()) {
+            memcpy(h->slide_h + b_iw, iwins.data(), sizeof(SlideIntWin) * iwins.size());
+            PreintSlide a;
+            a.n = (int) iwins.size(), a.win = (const SlideIntWin *) (h->slide_d + b_iw), a.item = (const SlideItem *) (h->slide_d + b_item);
+            a.align = (const SlideAlign *) (h->slide_d + b_align), a.imu = (const double *) (h->slide_d + b_rows);
+            a.state = (const double *) (h->slide_d + b_state), a.pose = h->D.pose, a.mix = h->D.mix, a.K = C.K, a.val = (double *) (h->slide_d + b_val);
+            for (int k = 0; k < 5; k++) a.noise5[k] = noise5[k];
+            for (int k = 0; k < 3; k++) a.station[k] = station3[k];
+            a.status = (int8_t *) (h->slide_d + b_status), a.ends = (double *) (h->slide_d + b_ends);
+            a.out_blob = want_blob ? (double *) (h->slide_d + b_blob) : nullptr;
+            cudaError_t e = cudaMemcpyAsync(h->slide_d, h->slide_h, in_end, cudaMemcpyHostToDevice, s);
+            if (e == cudaSuccess) e = preint_slide_launch(a, s);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(h->slide_h + b_status, h->slide_d + b_status, total - b_status, cudaMemcpyDeviceToHost, s);
+            if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+            if (e != cudaSuccess) {
+                set_error("%s: the integration on the device failed: %s", fn, cudaGetErrorString(e));
+                return fail(ICG_ECUDA);
+            }
+            count_launch();
+        }
+        const int8_t *st = (const int8_t *) (h->slide_h + b_status);
+        const double *ends = (const double *) (h->slide_h + b_ends), *blobs = (const double *) (h->slide_h + b_blob);
+        int bad_w = -1, bad_k = -1;
+        for (int w = 0; w < n; w++) {
+            const icg_ba_slide_integrate &g = integ[w];
+            for (int k = 0; k < next[w].n_imu; k++) {
+                const int q = item_of[w][k];
+                if (g.status) g.status[k] = q >= 0 ? st[q] : 0;
+                if (q < 0) continue;
+                if (g.end_state10) memcpy(g.end_state10 + 10 * (size_t) k, ends + 10 * (size_t) q, 80);
+                if (g.blob_out) memcpy(g.blob_out + (size_t) ICG_IMU_BLOB_DOUBLES * k, blobs + (size_t) ICG_IMU_BLOB_DOUBLES * q, 8 * ICG_IMU_BLOB_DOUBLES);
+                if (st[q] < 0 && bad_w < 0) bad_w = w, bad_k = k;
+            }
+        }
+        if (bad_w >= 0) {
+            set_error("%s: window %d IMU factor %d: the integrated covariance is not positive definite", fn, bad_w, bad_k);
+            return fail(ICG_EINVAL);
+        }
+    }
     // every check has passed: from here on the device is written
     h->marg_res_n = 0;
-    ICG_CUDA(cudaMemcpyAsync(h->slide_d, h->slide_h, total, cudaMemcpyHostToDevice, s));
+    if (iwins.empty()) ICG_CUDA(cudaMemcpyAsync(h->slide_d, h->slide_h, in_end, cudaMemcpyHostToDevice, s));
     ICG_CUDA(cudaEventRecord(h->slide_ev, s));
     rc = upload_structure(h, n);
     if (rc != ICG_OK) return rc;
@@ -3566,6 +3717,19 @@ int icg_ba_slide_resident(icg_ba *h, int n, const icg_ba_problem *next, const ic
     if (rc != ICG_OK) return rc;
     h->cur_windows = n;
     return ICG_OK;
+}
+
+int icg_ba_slide_resident(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba_slide_window *carry) {
+    return slide_body(h, n, next, carry, nullptr, nullptr, nullptr, "icg_ba_slide_resident");
+}
+
+int icg_ba_slide_integrate_resident(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba_slide_window *carry, const icg_ba_slide_integrate *integ,
+                                    const double *noise5, const double *station3) {
+    if (!integ) {
+        set_error("icg_ba_slide_integrate_resident: bad arguments");
+        return ICG_EINVAL;
+    }
+    return slide_body(h, n, next, carry, integ, noise5, station3, "icg_ba_slide_integrate_resident");
 }
 
 // ---- landmark shards over peer memory (transport "p2p")

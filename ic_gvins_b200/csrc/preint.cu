@@ -235,6 +235,80 @@ __global__ void __launch_bounds__(PREINT_WARPS * 32) preint_resident_kernel(Prei
     }
 }
 
+// One warp per window: the aligned GNSS fixes, then the integrated factors in order, so that an ICG_SLIDE_CHAIN factor starts from the state
+// the previous iteration left in st.  Everything goes into the staged value rows; the handle itself is only read.
+__global__ void __launch_bounds__(PREINT_WARPS * 32) preint_slide_kernel(PreintSlide A) {
+    __shared__ double s_m[PREINT_WARPS * SM_WARP];
+    __shared__ signed char s_k[15 * PH_NZ], s_nz[16];
+    phi_pattern(s_k, s_nz);
+    __syncthreads();
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, q = blockIdx.x * PREINT_WARPS + warp;
+    if (q >= A.n) return;
+    double *sm = s_m + warp * SM_WARP;
+    const SlideIntWin W = A.win[q];
+    const size_t base = (size_t) W.win * A.K;
+    // insertNewGnssTimeNode's alignment: blh[c] -= mix[c] * dt / += mix[c] * dt (ic_gvins.cc:836-838, 850-852), with the sign in dt
+    for (int e = lane; e < 3 * W.n_align; e += 32) {
+        const SlideAlign g = A.align[W.align0 + e / 3];
+        const int c = e % 3;
+        double *b = A.val + g.blh + c;
+        *b = __dadd_rn(*b, __dmul_rn(A.mix[(base + g.node) * 9 + c], g.dt));
+    }
+    double nz5[5], stn[3], st[16], iw[3];
+#pragma unroll
+    for (int i = 0; i < 5; i++) nz5[i] = A.noise5[i];
+#pragma unroll
+    for (int i = 0; i < 3; i++) stn[i] = A.station[i];
+#pragma unroll
+    for (int i = 0; i < 16; i++) st[i] = 0;
+    for (int t = 0; t < W.n_item; t++) {
+        const int k = W.item0 + t;
+        const SlideItem it = A.item[k];
+        if (it.src == ICG_SLIDE_ROW) {
+#pragma unroll
+            for (int i = 0; i < 16; i++) st[i] = A.state[it.state + i];
+        } else {
+            // stateFromData (preintegration_base.cc:115-125) of an old node, or of the stateToData(currentState()) st holds (ICG_SLIDE_CHAIN)
+            if (it.src >= 0) {
+                const double *pose = A.pose + 7 * (base + it.src), *mix = A.mix + 9 * (base + it.src);
+#pragma unroll
+                for (int i = 0; i < 7; i++) st[i] = pose[i];
+#pragma unroll
+                for (int i = 0; i < 9; i++) st[7 + i] = mix[i];
+            }
+            const double qx = st[3], qy = st[4], qz = st[5], qw = st[6], qn = sqrt(qx * qx + qy * qy + qz * qz + qw * qw);
+            st[3] = qx / qn, st[4] = qy / qn, st[5] = qz / qn, st[6] = qw / qn;
+        }
+        if (!it.normal) {  // resetState: iewn_ = Earth::iewn(station, p) at the start position (preintegration_earth.cc:305-324)
+            const bam::V3 v = gc::earth_iewn(stn, bam::mk(st[0], st[1], st[2]));
+            iw[0] = v.x, iw[1] = v.y, iw[2] = v.z;
+        }
+        gc::PreintScalar S;
+        gc::preint_begin(S, st, it.normal ? nullptr : iw, it.grav);
+        propagate(S, nz5, A.imu + 7 * (size_t) it.row0, it.nrow, sm, s_k, s_nz, lane);
+        double *blob = A.val + it.blob;
+        int ok = 0;
+        if (lane == 0) ok = gc::imu_sqrt_info(sm + SM_C, blob + ICG_IMU_BLOB_DOUBLES, sm + SM_G) ? 1 : 0;
+        ok = __shfl_sync(0xffffffffu, ok, 0);
+        double *ob = A.out_blob ? A.out_blob + (size_t) ICG_IMU_BLOB_DOUBLES * k : nullptr;
+        write_matrices(sm, blob, lane);
+        if (ob) write_matrices(sm, ob, lane);
+        if (lane == 0) {
+            A.status[k] = ok ? 1 : -1;
+            gc::preint_head(S, st, it.grav, blob, A.ends + 10 * (size_t) k);
+            if (ob) gc::preint_head(S, st, it.grav, ob, nullptr);
+        }
+        // stateToData(currentState()): p, q, v propagated, bg / ba of the start state -- the new node's row and the next CHAIN's start
+        st[0] = S.cur_p.x, st[1] = S.cur_p.y, st[2] = S.cur_p.z, st[3] = S.cur_q.x, st[4] = S.cur_q.y, st[5] = S.cur_q.z, st[6] = S.cur_q.w;
+        st[7] = S.cur_v.x, st[8] = S.cur_v.y, st[9] = S.cur_v.z;
+        if (it.node >= 0 && lane == 0) {
+#pragma unroll
+            for (int i = 0; i < 16; i++) A.val[it.node + i] = st[i];
+        }
+        __syncwarp();  // the next factor's propagate rewrites the shared matrices the lanes have just read
+    }
+}
+
 }  // namespace
 
 cudaError_t preint_batch_launch(const PreintBatch &a, cudaStream_t stream) {
@@ -246,6 +320,12 @@ cudaError_t preint_batch_launch(const PreintBatch &a, cudaStream_t stream) {
 cudaError_t preint_resident_launch(const PreintResident &a, cudaStream_t stream) {
     if (a.n <= 0) return cudaSuccess;
     preint_resident_kernel<<<(a.n + PREINT_WARPS - 1) / PREINT_WARPS, PREINT_WARPS * 32, 0, stream>>>(a);
+    return cudaGetLastError();
+}
+
+cudaError_t preint_slide_launch(const PreintSlide &a, cudaStream_t stream) {
+    if (a.n <= 0) return cudaSuccess;
+    preint_slide_kernel<<<(a.n + PREINT_WARPS - 1) / PREINT_WARPS, PREINT_WARPS * 32, 0, stream>>>(a);
     return cudaGetLastError();
 }
 

@@ -293,16 +293,18 @@ public:
         std::vector<int32_t> node_src, lm_src, f_src, imu_src, gnss_src;
     };
     void slideWindow(const icg_ba_problem &next, const Carry &carry, bool prior_from_marginalization) {
-        auto ptr = [](const std::vector<int32_t> &v, int32_t n, const char *what) -> const int32_t * {
-            if (v.empty()) return nullptr;
-            if (v.size() != (size_t) (n > 0 ? n : 0)) throw std::runtime_error(std::string("WindowSolver::slideWindow: ") + what + " needs one entry per row of next");
-            return v.data();
-        };
-        icg_ba_slide_window c{};
-        c.node_src = ptr(carry.node_src, next.K, "node_src"), c.lm_src = ptr(carry.lm_src, next.L, "lm_src"), c.f_src = ptr(carry.f_src, next.F, "f_src");
-        c.imu_src = ptr(carry.imu_src, next.n_imu, "imu_src"), c.gnss_src = ptr(carry.gnss_src, next.n_gnss, "gnss_src");
+        icg_ba_slide_window c = carryStruct(next, carry);
         c.prior_from_marg = prior_from_marginalization ? 1 : 0;
         check(icg_ba_slide_resident(h_, 1, &next, &c), "icg_ba_slide_resident");
+    }
+    // The same, with the new factors, node states and aligned GNSS fixes that `integrate` names computed on the device from the states this
+    // solver holds, in place of the host parts of addNewTimeNode, removeUnusedTimeNode and insertNewGnssTimeNode (IG/ic_gvins.cc:754-928):
+    // see icg_ba_slide_integrate. Its outputs (status, blob_out, end_state10) are written as that struct names them.
+    void slideWindow(const icg_ba_problem &next, const Carry &carry, bool prior_from_marginalization, icg_ba_slide_integrate &integrate,
+                     const double noise5[5], const double station[3]) {
+        icg_ba_slide_window c = carryStruct(next, carry);
+        c.prior_from_marg = prior_from_marginalization ? 1 : 0;
+        check(icg_ba_slide_integrate_resident(h_, 1, &next, &c, &integrate, noise5, station), "icg_ba_slide_integrate_resident");
     }
     // the two-pass body of gvinsOptimization on the window slideWindow left (nothing is uploaded); results as gvinsOptimization gives them
     void gvinsOptimizationResident(const icg_ba_problem &next, int num_iterations, icg_ba_summary out[2], int32_t culled[2]) {
@@ -311,6 +313,17 @@ public:
     }
 
 private:
+    static icg_ba_slide_window carryStruct(const icg_ba_problem &next, const Carry &carry) {
+        auto ptr = [](const std::vector<int32_t> &v, int32_t n, const char *what) -> const int32_t * {
+            if (v.empty()) return nullptr;
+            if (v.size() != (size_t) (n > 0 ? n : 0)) throw std::runtime_error(std::string("WindowSolver::slideWindow: ") + what + " needs one entry per row of next");
+            return v.data();
+        };
+        icg_ba_slide_window c{};
+        c.node_src = ptr(carry.node_src, next.K, "node_src"), c.lm_src = ptr(carry.lm_src, next.L, "lm_src"), c.f_src = ptr(carry.f_src, next.F, "f_src");
+        c.imu_src = ptr(carry.imu_src, next.n_imu, "imu_src"), c.gnss_src = ptr(carry.gnss_src, next.n_gnss, "gnss_src");
+        return c;
+    }
     template <typename Call>
     Prior marginalize(const icg_ba_problem &problem, int num_marg, Call call) {
         Prior P;

@@ -640,6 +640,55 @@ typedef struct icg_ba_slide_window {
 } icg_ba_slide_window;
 int icg_ba_slide_resident(icg_ba *h, int n_windows, const icg_ba_problem *next, const icg_ba_slide_window *carry);
 /*
+ * icg_ba_slide_resident whose new IMU factors, new node states and aligned GNSS fixes are computed on the device from the states the handle
+ * holds, instead of being preintegrated on the host and read from `next`: the host halves of the time-node edits between two solves,
+ *   GVINS::addNewTimeNode (IG/ic_gvins.cc:897-928)        a new factor from the last node's state (NODE), the new node = its currentState();
+ *   GVINS::removeUnusedTimeNode (:754-789)                 a merged factor: the first interval's start state replayed over the first interval's
+ *                                                         rows followed by the second's without its first row (ROW);
+ *   GVINS::insertNewGnssTimeNode (:791-888)                a fix moved onto a node, blh -= v dt / blh += v dt (alignment); or a node inserted at
+ *                                                         the fix and the later nodes re-created, each interval from the state the previous
+ *                                                         one propagated (NODE, then CHAIN).
+ * Per window, only rows that `carry` marks -1 (or whose carry map is NULL) are read.  For an integrated factor k (joining new nodes k, k + 1):
+ *   start  NODE i (>= 0): old node i's resident pose (q normalised as icg_ba_reintegrate_resident normalises it) and mix;  ICG_SLIDE_CHAIN:
+ *          stateFromData(stateToData(currentState())) of factor k - 1 of the same window, which must be integrated too;  ICG_SLIDE_ROW:
+ *          state16 row k as given (p, q_xyzw, v, bg, ba; not normalised)
+ *   form   normal[k] (NULL: all PreintegrationEarth) and gravity3 row k; the Earth form takes iewn = Earth::iewn(station3, start p) as resetState
+ *          does (preintegration_earth.cc:305-324), the Normal form iewn = 0
+ *   rows   imu rows imu_off[k] .. imu_off[k + 1] - 1 (dt, dtheta[3], dvel[3]), row imu_off[k] the sample at the interval's start; at least one
+ * Its blob and square-root information become new factor k's, as icg_ba_slide_resident would read them from next.imu_blob (the blob is
+ * icg_imu_preintegrate's from the same start state, bit for bit).  A flagged new node j takes pose = (p, q) and mix = (v, bg, ba) of
+ * stateToData(currentState()) of integrated factor j - 1 (bg, ba: its start state's).  An aligned new GNSS fix g takes
+ * blh = next.gnss_blh[g] + dt v(old node), each component rounded on its own (blh - v |dt| bit for bit for dt < 0); its std is next's (the
+ * caller applies the reference's x 1.2).  One warp per window walks the window's integrated factors in order.
+ * Every check of icg_ba_slide_resident and of these arrays (sources and nodes in range, CHAIN after an integrated factor, offsets, flags)
+ * runs before the device is written.  The integration then runs into the slide's staging, the call synchronises and, when an integrated
+ * covariance is not positive definite, returns ICG_EINVAL naming the first such factor (window order, then factor order) with the handle as it
+ * was; the outputs are written either way.  Otherwise the call goes on as icg_ba_slide_resident does (asynchronous from there).
+ * ICG_EUNSUPPORTED on a landmark-sharded handle.
+ */
+#define ICG_SLIDE_CHAIN (-2)
+#define ICG_SLIDE_ROW (-3)
+typedef struct icg_ba_slide_integrate {
+    /* in: per new IMU factor (next.n_imu entries) */
+    const int32_t *imu_from;      /* NULL: nothing integrated in this window.  -1: next.imu_blob row; i >= 0: NODE i; ICG_SLIDE_CHAIN; ICG_SLIDE_ROW */
+    const double *state16;        /* n_imu x 16: the ICG_SLIDE_ROW start states (other rows not read; NULL when there is none) */
+    const double *gravity3;       /* n_imu x 3 */
+    const uint8_t *normal;        /* n_imu: 1 PreintegrationNormal, 0 PreintegrationEarth; NULL: all Earth */
+    const double *imu;            /* rows (dt, dtheta[3], dvel[3]) */
+    const int32_t *imu_off;       /* n_imu + 1 */
+    /* in: per new node (next.K entries), NULL: none */
+    const uint8_t *node_from_imu; /* 1: the node is currentState() of integrated factor j - 1 */
+    /* in: per new GNSS fix (next.n_gnss entries), NULL: none */
+    const int32_t *gnss_node;     /* -1: next.gnss_blh as given; i >= 0: aligned by old node i's velocity */
+    const double *gnss_dt;        /* signed dt of the alignment (the reference's -dt for a fix moved back onto node index - 1) */
+    /* out, each may be NULL */
+    int8_t *status;               /* n_imu: 1 integrated, 0 not integrated, -1 integrated covariance not positive definite */
+    double *blob_out;             /* n_imu x ICG_IMU_BLOB_DOUBLES: written where status != 0 */
+    double *end_state10;          /* n_imu x 10: currentState() p, q_xyzw, v where status != 0 */
+} icg_ba_slide_integrate;
+int icg_ba_slide_integrate_resident(icg_ba *h, int n_windows, const icg_ba_problem *next, const icg_ba_slide_window *carry,
+                                    const icg_ba_slide_integrate *integ, const double *noise5, const double *station3);
+/*
  * Landmark sharding of the window solve across the GPUs of one box (SURVEY.md 8e), over PEER MEMORY (transport "p2p"): every process
  * (one per GPU) uploads the same camera-side problem but only ITS landmarks and their reprojection factors; window w of the batch is
  * owned by rank w mod world.  Every rank STORES its packed reduction operand straight into the owner's inbox over NVLink; the owner sums
