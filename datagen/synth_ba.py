@@ -1,6 +1,6 @@
 """Synthetic sliding-window problems for hot path B (SURVEY.md section 8d, cfg 3 / cfg 4).  Input generator only.
 
-K nodes at 0.5 s spacing on a planar arc (5 m/s, yaw rate 5 deg/s), IMU at 200 Hz with the noise model of
+K nodes at 0.5 s spacing (dt_node) on a planar arc (5 m/s, yaw rate 5 deg/s), IMU at 200 Hz with the noise model of
 config/gvins.yaml:26-31, GNSS on every 2nd node, L landmarks at depth U(5, 60) m with reference frame j mod 5 observed in
 frames r+1 .. min(K-1, r+3+(j mod 6)), pixel noise 0.5 px / f=787, reprojection std 1.5/787, extrinsic of
 config/gvins.yaml:78-79 (free), td = 0 (free).  Initial guess = truth (+) N(0; 0.1 m, 0.5 deg, 0.1 m/s), rho (1+N(0,0.1)).
@@ -84,12 +84,14 @@ def imu_samples(t0, t1, rate, rng, bg, ba, yaw_rate=5.0 * D2R, earth=True):
 
 # ---------------------------------------------------------------------------------------------- problem
 def make_window(preintegrate, K=10, L=300, seed=2024, full_visibility=False, perturb=True, with_marg=False, pixel_noise=0.5, with_priors=False,
-                gnss_every=2, earth=True, n_ref=5):
+                gnss_every=2, earth=True, n_ref=5, dt_node=0.5):
     """n_ref: landmark j is anchored in node j mod n_ref (j mod (K - 1) when K <= n_ref).  A larger n_ref spreads the landmarks over more
     nodes, so fewer of them are marginalized with node 0.  The anchor itself draws no random numbers: the default (5) generates the same
-    arrays as before the keyword existed."""
+    arrays as before the keyword existed.
+    dt_node: time between consecutive nodes (s).  Shorter spacing keeps landmarks in view over more nodes: long tracks.  The default (0.5)
+    generates the same arrays as before the keyword existed."""
     rng = np.random.Generator(np.random.PCG64(seed))
-    dtk, rate = 0.5, 200.0
+    dtk, rate = dt_node, 200.0
     times = np.arange(K) * dtk
     bg_true = rng.normal(0, 20.0 * D2R / 3600.0, 3)
     ba_true = rng.normal(0, 20.0 * 1e-5, 3)

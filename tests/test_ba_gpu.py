@@ -130,6 +130,24 @@ def test_batched_windows_are_independent(olib, solver):
             assert np.array_equal(a[key], b[key]), key
 
 
+def oracle_two_pass(olib, po):
+    """GVINS::gvinsOptimization's 5 + 15 iterations on the oracle, culling on the host between the passes; po is updated in place.
+    Returns the two pass summaries and the mask of removed reprojection factors."""
+    po["gnss_huber"] = 1
+    s1 = oa.ba_solve(olib, po, 5)
+    rc, gc = oa.ba_residual_costs(olib, po)
+    std = po["gnss_std"].reshape(-1, 3)
+    for g in range(po["n_gnss"]):
+        if 2 * gc[g] > 7.815:
+            std[g] *= np.sqrt(2 * gc[g] / 7.815)
+    po["gnss_std"] = std.reshape(-1)
+    out = (2 * rc > 5.991)
+    po["f_active"][out] = 0
+    po["gnss_huber"] = 0
+    s2 = oa.ba_solve(olib, po, 15)
+    return s1, s2, out
+
+
 def test_two_pass_protocol_matches_oracle(olib, solver):
     """GVINS::gvinsOptimization: 5 iterations, chi2 culling (GNSS re-weighting + reprojection removal), 15 iterations."""
     prob, _ = make(olib, K=10, L=300, seed=77)
@@ -140,19 +158,7 @@ def test_two_pass_protocol_matches_oracle(olib, solver):
     prob["gnss_blh"][3:6] += np.array([1.0, -0.8, 0.5])  # a GNSS outlier on the second fix
     pg, po = copy.deepcopy(prob), copy.deepcopy(prob)
     info = solver.gvins_optimization(pg, 20)
-    # the same protocol on the oracle
-    po["gnss_huber"] = 1
-    oa.ba_solve(olib, po, 5)
-    rc, gc = oa.ba_residual_costs(olib, po)
-    std = po["gnss_std"].reshape(-1, 3)
-    for g in range(po["n_gnss"]):
-        if 2 * gc[g] > 7.815:
-            std[g] *= np.sqrt(2 * gc[g] / 7.815)
-    po["gnss_std"] = std.reshape(-1)
-    out = (2 * rc > 5.991)
-    po["f_active"][out] = 0
-    po["gnss_huber"] = 0
-    oa.ba_solve(olib, po, 15)
+    _, _, out = oracle_two_pass(olib, po)
     assert info["reproj_removed"] == int(out.sum()) and out[10] and out[500]
     assert np.array_equal(pg["f_active"], po["f_active"])
     assert rel_err(pg["gnss_std"], po["gnss_std"]) <= 1e-9
@@ -288,18 +294,7 @@ def test_cfg4_two_pass_protocol_matches_oracle(olib, solver_cfg4):
     prob["gnss_blh"][3:6] += np.array([1.0, -0.8, 0.5])
     pg, po = copy.deepcopy(prob), copy.deepcopy(prob)
     info = solver_cfg4.gvins_optimization_batch([pg], 20)[0]
-    po["gnss_huber"] = 1
-    s1 = oa.ba_solve(olib, po, 5)
-    rc, gc = oa.ba_residual_costs(olib, po)
-    std = po["gnss_std"].reshape(-1, 3)
-    for g in range(po["n_gnss"]):
-        if 2 * gc[g] > 7.815:
-            std[g] *= np.sqrt(2 * gc[g] / 7.815)
-    po["gnss_std"] = std.reshape(-1)
-    out = (2 * rc > 5.991)
-    po["f_active"][out] = 0
-    po["gnss_huber"] = 0
-    s2 = oa.ba_solve(olib, po, 15)
+    s1, s2, out = oracle_two_pass(olib, po)
     assert info["pass1"]["iterations"] == s1["iterations"] and info["pass2"]["iterations"] == s2["iterations"]
     assert info["reproj_removed"] == int(out.sum()) and out[10] and out[5000]
     assert np.array_equal(pg["f_active"], po["f_active"])
