@@ -60,6 +60,16 @@ def warp_point(x, y, t: int, W: int, H: int):
     return xr, yr
 
 
+def unwarp_point(x, y, t: int, W: int, H: int):
+    """Inverse of warp_point: the frame-0 pixel coords of the point that appears at (x, y) in frame t."""
+    tx, ty, rot, sc = ego_motion(t)
+    cx, cy = W / 2.0, H / 2.0
+    c, s = math.cos(rot) * sc, math.sin(rot) * sc
+    det = c * c + s * s
+    u, v = x - cx - tx, y - cy - ty
+    return (c * u + s * v) / det + cx, (-s * u + c * v) / det + cy
+
+
 def render_frame(tex: np.ndarray, t: int, W: int, H: int, margin: int = 64) -> np.ndarray:
     """Bilinear resample of the texture under the inverse ego-motion; returns u8 HxW."""
     tx, ty, rot, sc = ego_motion(t)
@@ -106,6 +116,57 @@ def klt_pair(W=1280, H=560, n=300, seed=1234, t=1, noise_px=1.0, clahe=False):
     rng = np.random.Generator(np.random.PCG64(seed + 13 + t))
     init = p1 + rng.normal(0.0, noise_px, size=p1.shape)
     return f0, f1, p0.astype(np.float32), init.astype(np.float32), p1.astype(np.float32)
+
+
+def pyramid_sizes(W: int, H: int, levels: int = 4):
+    """(W_l, H_l) of levels 0 .. levels - 1 of a pyramid built with cv::pyrDown ((n + 1) / 2 per level)."""
+    out = [(W, H)]
+    for _ in range(levels - 1):
+        W, H = (W + 1) // 2, (H + 1) // 2
+        out.append((W, H))
+    return out
+
+
+def lk_levels(W: int, H: int, max_level: int = 3, win: int = 21) -> int:
+    """Levels cv::buildOpticalFlowPyramid builds: it stops at the first level whose width or height is <= win."""
+    n = 1
+    for w, h in pyramid_sizes(W, H, max_level + 1)[1:]:
+        if w <= win or h <= win:
+            break
+        n += 1
+    return n
+
+
+# window origins floor(x 2^-l - 10) of the LK edge rings at level l: low side, and offsets from W_l (H_l) on the high side.  -21 / W_l - 1
+# are the last origins LK tracks at all, -1 / W_l - 23 the last ones whose 24 x 24 template taps (bilinear + Scharr) stay inside the level
+EDGE_LO = (-22, -21, -20, -1, 0, 1, 2)
+EDGE_HI = (-24, -23, -22, -2, -1, 0)
+EDGE_FRACS = (0.0, 0.25, 0.5, 0.999)
+
+
+def edge_rings(W: int, H: int, n_levels: int, rng: np.random.Generator, fracs=EDGE_FRACS, corner_origins=(-21, -1, -23, -1)):
+    """Level-0 points (float32, N x 2) on all four sides of every level l < n_levels: for each edge origin o (EDGE_LO, W_l + EDGE_HI) and
+    fractional part f, the level-l coordinate is o + 10 + f (2^-l is exact, so the level-l origin is exactly o); the other coordinate is
+    uniform over the image.  Plus corner points (two low and two high origins per axis).  fracs=None draws a fresh fractional part per point."""
+    def frac_list():
+        return list(fracs) if fracs is not None else list(rng.uniform(0.0, 1.0, len(EDGE_FRACS)))
+
+    def frac():
+        return float(rng.choice(fracs)) if fracs is not None else float(rng.uniform(0.0, 1.0))
+
+    pts = []
+    for level, (wl, hl) in enumerate(pyramid_sizes(W, H, n_levels)):
+        s = float(1 << level)
+        for axis, (nl, full) in enumerate(((wl, H), (hl, W))):
+            for o in [*EDGE_LO, *(nl + d for d in EDGE_HI)]:
+                for f in frac_list():
+                    c, other = (o + 10 + f) * s, rng.uniform(0.0, full)
+                    pts.append((c, other) if axis == 0 else (other, c))
+        lo, hi = corner_origins[:2], corner_origins[2:]
+        for ox in [*lo, *(wl + d for d in hi)]:
+            for oy in [*lo, *(hl + d for d in hi)]:
+                pts.append(((ox + 10 + frac()) * s, (oy + 10 + frac()) * s))
+    return np.array(pts, np.float32)
 
 
 class KltStream:

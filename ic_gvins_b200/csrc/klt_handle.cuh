@@ -38,6 +38,7 @@ void track_scratch_free(TrackScratch *t);  // track.cu
 
 struct icg_klt {
     int W, H, n_slots, max_pts, device;
+    int n_levels;  // pyramid levels cv::buildOpticalFlowPyramid builds for this size at maxLevel KLT_LEVELS - 1 (<= KLT_LEVELS)
     cudaStream_t stream;
     bool own_stream;
     icg::KltLevel lv[icg::KLT_LEVELS];

@@ -72,8 +72,9 @@ public:
         nextPts.resize(n);
         status.resize(n);
         err.resize(n);
+        // OpenCV's defaults for a criterion the type leaves out: 30 iterations, epsilon 0.01
         const int max_iter = (criteria.type & 1) ? criteria.maxCount : 30;
-        const double eps = (criteria.type & 2) ? criteria.epsilon : 0.0;
+        const double eps = (criteria.type & 2) ? criteria.epsilon : 0.01;
         check(icg_klt_calc_optical_flow_pyr_lk(h_, mat_data(prev), mat_data(next), mat_stride(prev), reinterpret_cast<const float *>(prevPts.data()),
                                                reinterpret_cast<float *>(nextPts.data()), status.data(), err.data(), n, winSize.width, maxLevel, max_iter, eps,
                                                flags),

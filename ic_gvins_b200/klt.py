@@ -146,8 +146,9 @@ class KltTracker:
             q = p.copy()
         status = np.zeros(n, np.uint8)
         err = np.zeros(n, np.float32)
+        # cv::calcOpticalFlowPyrLK's defaults for a criterion the type leaves out: 30 iterations, epsilon 0.01
         max_iter = criteria[1] if criteria[0] & TERM_COUNT else 30
-        eps = criteria[2] if criteria[0] & TERM_EPS else 0.0
+        eps = criteria[2] if criteria[0] & TERM_EPS else 0.01
         check(lib().icg_klt_calc_optical_flow_pyr_lk(self._h, _ptr(prevImg), _ptr(nextImg), self.W, _ptr(p), _ptr(q),
                                                      _ptr(status), _ptr(err), n, winSize[0], maxLevel, max_iter,
                                                      float(eps), flags), "icg_klt_calc_optical_flow_pyr_lk")

@@ -95,7 +95,8 @@ int icg_klt_build_pyramids(icg_klt *h, int first_slot, int count);
  * Batched forward+backward tracking of n_total points, all arrays in DEVICE memory:
  *   slots[2k], slots[2k+1] = (prev slot, next slot) of point k;  prev_xy/init_xy/fwd_xy/bwd_xy: float2 per point.
  * Asynchronous on the handle's stream.  mode 0: forward only (status = raw LK status);
- * mode 1: fused forward+backward+gates (as icg_klt_track_fb).
+ * mode 1: fused forward+backward+gates (as icg_klt_track_fb).  Tracks on the pyramid levels cv::buildOpticalFlowPyramid(winSize 21,
+ * maxLevel 3) builds for the handle's size: it stops at the first level whose width or height is <= 21 (e.g. 320x168: 3 levels, 32x32: 1).
  */
 int icg_klt_track_batch_dev(icg_klt *h, int n_total, const int32_t *dev_slots, const float *dev_prev_xy,
                             const float *dev_init_xy, float *dev_fwd_xy, float *dev_bwd_xy, uint8_t *dev_status,

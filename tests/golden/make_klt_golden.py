@@ -23,9 +23,9 @@ from datagen import synth_klt as synth  # noqa: E402
 CRIT = (cv2.TERM_CRITERIA_COUNT + cv2.TERM_CRITERIA_EPS, 30, 0.01)
 
 
-def lk(a, b, p, init):
+def lk(a, b, p, init, max_level=3, criteria=CRIT, flags=cv2.OPTFLOW_USE_INITIAL_FLOW):
     out, st, err = cv2.calcOpticalFlowPyrLK(a, b, p.reshape(-1, 1, 2), init.reshape(-1, 1, 2).copy(), winSize=(21, 21),
-                                            maxLevel=3, criteria=CRIT, flags=cv2.OPTFLOW_USE_INITIAL_FLOW)
+                                            maxLevel=max_level, criteria=criteria, flags=flags)
     return out.reshape(-1, 2), st.ravel().astype(np.uint8), err.ravel()
 
 

@@ -52,9 +52,16 @@ int main(int argc, char **argv) {
         icg_b200::KltContext klt(W, H);
         klt.calcOpticalFlowPyrLK(A, B, prev, next, st, err, icg_b200::Size(21, 21), 3, icg_b200::TermCriteria(3, 30, 0.01), ICG_OPTFLOW_USE_INITIAL_FLOW);
         klt.trackForwardBackward(A, B, prev, next2, st_fb);
-        std::vector<double> o1, o2;
+        // COUNT-only criteria: OpenCV takes its default epsilon 0.01, so this is the call above
+        std::vector<icg_b200::Point2f> next3(n);
+        for (int k = 0; k < n; k++) next3[k] = {(float) init[2 * k], (float) init[2 * k + 1]};
+        std::vector<uint8_t> st3;
+        std::vector<float> err3;
+        klt.calcOpticalFlowPyrLK(A, B, prev, next3, st3, err3, icg_b200::Size(21, 21), 3, icg_b200::TermCriteria(1, 30, 0.5), ICG_OPTFLOW_USE_INITIAL_FLOW);
+        std::vector<double> o1, o2, o3;
         for (int k = 0; k < n; k++) o1.insert(o1.end(), {next[k].x, next[k].y, (double) st[k]}), o2.insert(o2.end(), {next2[k].x, next2[k].y, (double) st_fb[k]});
-        wr(out, o1), wr(out, o2);
+        for (int k = 0; k < n; k++) o3.insert(o3.end(), {next3[k].x, next3[k].y, (double) st3[k]});
+        wr(out, o1), wr(out, o2), wr(out, o3);
         // ---------------- cv::CLAHE::apply
         icg_b200::Clahe clahe(W, H);
         std::vector<uint8_t> eq(a.size());
@@ -143,13 +150,14 @@ def test_cpp_shims_run_on_the_gpu(oracle, klt_golden):
         r = subprocess.run([exe, fin, fout], capture_output=True, text=True, timeout=300)
         assert r.returncode == 0, (r.returncode, r.stderr)
         with open(fout, "rb") as fh:
-            lk, fb, eq = _rd(fh).reshape(-1, 3), _rd(fh).reshape(-1, 3), _rd(fh)
+            lk, fb, lk_count, eq = _rd(fh).reshape(-1, 3), _rd(fh).reshape(-1, 3), _rd(fh).reshape(-1, 3), _rd(fh)
             r_rep, Ji, Jj, Je, Jr, Jt, r_rep2 = (_rd(fh) for _ in range(7))
             r_imu, I0, I2, I3 = (_rd(fh) for _ in range(4))
             r_gn, Jg = _rd(fh), _rd(fh)
     # KLT vs the cv2 golden vectors
     assert np.array_equal(lk[:, 2].astype(np.uint8), g[name + "_st"])
     assert_px(lk[:, :2].astype(np.float32), g[name + "_fwd"], g[name + "_st"] == 1, name)
+    assert np.array_equal(lk_count, lk)
     assert np.array_equal(fb[:, 2].astype(np.uint8), g[name + "_good"])
     assert_px(fb[:, :2].astype(np.float32), g[name + "_fwd"], g[name + "_good"] == 1, name)
     # CLAHE vs the oracle (bit-exact with cv2)
