@@ -138,6 +138,33 @@ def merge_shard(prob: dict, shard: dict) -> None:
         prob[k][...] = shard[k]
 
 
+def shard_cull_inputs(ci: dict, shard: dict) -> dict:
+    """The culling inputs of one landmark shard (what each rank passes to update_and_cull on a sharded handle) from those of the whole
+    window: the shard's landmarks and their observation lists, `obs_factor` renumbered to the shard's factors (-1 stays -1)."""
+    lo, hi = shard["lm_lo"], shard["lm_hi"]
+    off = np.asarray(ci["obs_off"], np.int32)
+    o0, o1 = int(off[lo]), int(off[hi])
+    out = dict(ci, lm_ref_node=np.array(ci["lm_ref_node"][lo:hi], np.int32), lm_ref_kp=np.array(ci["lm_ref_kp"][lo:hi], np.float32),
+               obs_off=(off[lo:hi + 1] - o0).astype(np.int32), obs_node=np.array(ci["obs_node"][o0:o1], np.int32),
+               obs_kp=np.array(ci["obs_kp"][o0:o1], np.float32))
+    if ci.get("obs_factor") is not None:
+        local = np.full(max(1, int(np.max(shard["f_index"], initial=-1)) + 1), -1, np.int32)
+        local[shard["f_index"]] = np.arange(len(shard["f_index"]), dtype=np.int32)
+        f = np.asarray(ci["obs_factor"][o0:o1], np.int32)
+        out["obs_factor"] = np.where(f >= 0, local[np.clip(f, 0, len(local) - 1)], -1).astype(np.int32)
+    return out
+
+
+def merge_cull_shard(full: dict, shard: dict, shard_out: dict) -> None:
+    """Write one shard's culling results (update_and_cull on a sharded handle) into the whole window's result dict `full`: lm_pw, lm_depth,
+    lm_outlier over the shard's landmark range, obs_outlier over its observations.  Camera outputs and counts are the same on every rank."""
+    lo, hi = shard["lm_lo"], shard["lm_hi"]
+    off = full["obs_off"]
+    for k in ("lm_pw", "lm_depth", "lm_outlier"):
+        full[k][lo:hi] = shard_out[k]
+    full["obs_outlier"][off[lo]:off[hi]] = shard_out["obs_outlier"]
+
+
 def connect_shards(solver: "WindowSolver", rank: int, world: int, transport: str, dist) -> None:
     """Join `solver` to the landmark-shard group of `world` processes (one per GPU) over peer memory (transport "p2p": each rank stores
     its reduction operand into the window owner's buffer over NVLink; the only transport).  `dist` is an initialised torch.distributed
@@ -286,7 +313,9 @@ class WindowSolver:
         update_and_cull returned, with `obs_factor` in each dict; the factor set is then the map after the culling
         (icg_ba_marginalize_resident_culled), node_in_map[w] (K flags) naming the keyframes still in the map (all of them when None).
         Any handle marginalizes (cfg-4 windows included); a window whose marginalized or remained block exceeds 512 rows raises IcgError
-        (ICG_EUNSUPPORTED) before anything runs.  To consume its own prior, a handle of max_K nodes needs max_marg_r >= 15 (max_K - 1) + 7."""
+        (ICG_EUNSUPPORTED) before anything runs.  To consume its own prior, a handle of max_K nodes needs max_marg_r >= 15 (max_K - 1) + 7.
+        On a landmark-sharded handle (resident only) the call is collective: every rank passes its shard dicts (and, with culled=, its own
+        update_and_cull results); window w's prior is returned on rank w mod world, the other ranks get m = r = 0 and empty arrays."""
         if isinstance(problems, dict):
             problems = [problems]
         call = self.marg_prepare(problems, num_marg, want_schur)
@@ -313,7 +342,9 @@ class WindowSolver:
         solved (icg_ba_update_and_cull_resident).  camera: a camera.Camera or CameraStruct; std: reprojection_error_std_.  cull_inputs: one
         dict per window with R_bc (3x3), t_bc, td_bc, estimate_ext, estimate_td, lm_ref_node (L), lm_ref_kp (L x 2), obs_off (L + 1),
         obs_node, obs_kp (x 2) and optionally obs_factor.  Returns one dict per window: the inputs plus R_bc_out, t_bc_out, td_bc_out,
-        ext_accepted, cam_pose (K x 12), lm_pw (L x 3), lm_depth, lm_outlier, obs_outlier and counts (5)."""
+        ext_accepted, cam_pose (K x 12), lm_pw (L x 3), lm_depth, lm_outlier, obs_outlier and counts (5).  On a landmark-sharded handle every
+        rank calls with its shard dicts and shard_cull_inputs(); the counts are the window's totals on every rank, the landmark outputs cover the
+        shard (merge_cull_shard writes them into the whole window's)."""
         if isinstance(problems, dict):
             problems, cull_inputs = [problems], [cull_inputs]
         n = len(problems)

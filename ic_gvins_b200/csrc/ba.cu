@@ -32,6 +32,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <functional>
 #include <string>
 #include <thread>
 #include <vector>
@@ -78,6 +79,7 @@ struct ShardDev {
     int PK, BS, RV;            // packed partial length, step-broadcast stride, reduced-vector stride (doubles)
     double *peer[8];
     size_t off_inbox, off_bcast, off_scal, off_flagA, off_flagB, off_flagC;  // offsets in doubles, identical on every rank
+    size_t off_flagX, off_post, off_exp;  // the post-solve exchanges of a shard group (ba_split.cuh); off_exp: sized by this rank's max_F
     double *redv;              // [NW][RV] owner-side reduced vectors: diag H_vis | g_vis | W phi g_l | cost, sum rho^2, max |g_l|
     int *err;                  // device error word (flag wait timed out)
     double *slm;               // [NW][STEP_SLICES][8] partial sums of ba_step_lm's landmark slices
@@ -1824,6 +1826,19 @@ struct icg_ba {
     size_t slide_cap = 0;
     double *slide_old = nullptr, *fc_alt = nullptr;
     cudaEvent_t slide_ev = nullptr;  // recorded after the staging's H2D
+    // post-solve calls of a shard group (world > 1): integer exchanges so far (slot parity), epoch of the last marginalization export, the
+    // exchange's device word, the export's slot lists, the owner's gathered rows with their tables, and the handle the owner uploads its
+    // gathered windows to (created on first use, recreated when a batch needs more landmarks, factors or windows)
+    unsigned long long xs_calls = 0, exp_epoch = 0;
+    HostDev<int> xs_v, mx_sel, mx_row;
+    HostDev<long long> mx_heads, mx_idx;
+    double *mx_rows = nullptr;
+    size_t mx_rows_cap = 0;
+    icg_ba *mx_h = nullptr;
+    // buffers a shard group's call outgrew.  Freeing synchronises the device, and between handles of one process that would wait for a
+    // peer's kernel spinning on this rank's flags: they are freed when the group is left or the handle destroyed
+    std::vector<void *> retired_d, retired_h;
+    std::vector<icg_ba *> retired_mx;
 };
 
 extern "C" {
@@ -2018,6 +2033,9 @@ void icg_ba_destroy(icg_ba *h) {
     h->marg_c0.release(), h->lm_off.release(), h->lm_perm.release(), h->lm_fidx.release(), h->gnss_node.release();
     h->f_meta_s.release(), h->vb_lm0.release(), h->ref_nrun.release(), h->f_const_s.release(), h->marg_type.release(), h->marg_node.release(), h->f_active.release(), h->scratch.release(), h->st_save.release(), h->cull_counters.release(), h->part_off.release(), h->pair_ro.release(), h->vis_ord.release(), h->npairs.release();
     split_release(h);
+    if (h->mx_h) icg_ba_destroy(h->mx_h);
+    h->xs_v.release(), h->mx_sel.release(), h->mx_row.release(), h->mx_heads.release(), h->mx_idx.release();
+    if (h->mx_rows) cudaFree(h->mx_rows);
     if (h->marg_ready) h->marg_map.release(), h->marg_oJ0.release(), h->marg_oe0.release(), h->marg_oHp.release(), h->marg_obp.release(), h->marg_fmask.release();
     for (double *p : {h->M.H0, h->M.b0, h->M.G1, h->M.V1, h->M.lam1, h->M.Z})
         if (p) cudaFree(p);
@@ -2449,7 +2467,23 @@ static int enqueue_lm(icg_ba *h, int max_num_iterations) {
 }
 
 // ---- split pipeline: host side
+// a buffer outgrown by a call: freed now on a single rank, kept until the group is left in a shard group (icg_ba::retired_d)
+static void retire(icg_ba *h, void *d, void *hp) {
+    if (h->D.world > 1) {
+        if (d) h->retired_d.push_back(d);
+        if (hp) h->retired_h.push_back(hp);
+        return;
+    }
+    if (d) cudaFree(d);
+    if (hp) cudaFreeHost(hp);
+}
+
 static void split_release(icg_ba *h) {
+    if (h->stream) cudaStreamSynchronize(h->stream);
+    for (void *p : h->retired_d) cudaFree(p);
+    for (void *p : h->retired_h) cudaFreeHost(p);
+    for (icg_ba *m : h->retired_mx) icg_ba_destroy(m);
+    h->retired_d.clear(), h->retired_h.clear(), h->retired_mx.clear();
     for (int r = 0; r < 8; r++)
         if (h->ipc_opened[r]) cudaIpcCloseMemHandle(h->ipc_opened[r]), h->ipc_opened[r] = nullptr;
     if (h->xbuf) cudaFree(h->xbuf), h->xbuf = nullptr;
@@ -2459,6 +2493,23 @@ static void split_release(icg_ba *h) {
     if (h->D.S.slm_cnt) cudaFree(h->D.S.slm_cnt), h->D.S.slm_cnt = nullptr;
     if (h->D.Sglobal) cudaFree(h->D.Sglobal), h->D.Sglobal = nullptr;
     h->D.S.split = 0;
+}
+
+// Under lazy module loading (the CUDA 12 default) a kernel is loaded at its first launch, and the load waits for the kernels running in the
+// context.  Ranks driven by one process share the context: a rank's first launch of a kernel would wait for a peer's kernel that spins on
+// this very rank's flags, until the bounded wait gives up.  A group therefore loads every kernel its calls launch when it is set up.
+static int preload_group_kernels() {
+    const void *k[] = {(const void *) ba_accept, (const void *) ba_accept_split, (const void *) ba_chi2_cull, (const void *) ba_cost, (const void *) ba_cost_cam,
+                       (const void *) ba_exchange, (const void *) ba_lin_cam, (const void *) ba_lin_vis, (const void *) ba_marg_export, (const void *) ba_marg_fill,
+                       (const void *) ba_marg_gather, (const void *) ba_marg_heads, (const void *) ba_reduce, (const void *) ba_reset_state,
+                       (const void *) ba_schur_dmma, (const void *) ba_set_gnss_huber, (const void *) ba_signal, (const void *) ba_solve, (const void *) ba_solve_cam,
+                       (const void *) ba_solve_cam_dsm, (const void *) ba_step_lm, (const void *) ba_xflag, (const void *) ba_xsum, (const void *) marg_assemble,
+                       (const void *) marg_finish, (const void *) marg_jacobi, (const void *) marg_jacobi_cluster, (const void *) marg_jacobi_cta,
+                       (const void *) marg_jacobi_pair, (const void *) marg_prepare, (const void *) marg_schur};
+    cudaFuncAttributes a;
+    for (const void *f : k) ICG_CUDA(cudaFuncGetAttributes(&a, f));
+    ICG_CUDA(preload_update_cull());
+    return ICG_OK;
 }
 
 // (re)allocate the exchange buffer of this rank for a group of `world` ranks and switch the handle to the split pipeline.  The layout
@@ -2486,7 +2537,20 @@ static int split_setup(icg_ba *h, int rank, int world) {
     S.off_flagA = off, off += 8;
     S.off_flagB = off, off += (NW + 3) & ~(size_t) 3;
     S.off_flagC = off, off += (NW * G + 3) & ~(size_t) 3;
+    S.off_flagX = off, off += 3 * 8;
+    S.off_post = off, off += 2 * NW * G * SPLIT_SCAL;
+    S.off_exp = off;  // the part every rank lays out alike ends here; the export region follows at this rank's own max_F
+    if (world > 1) off += 2 * NW + NW * (size_t) C.F * MEXP_ROW;
     h->xbuf_doubles = off;
+    h->xs_calls = 0, h->exp_epoch = 0;
+    if (world > 1) {
+        const int rc = preload_group_kernels();
+        if (rc != ICG_OK) return rc;
+        if (!h->xs_v.d && h->xs_v.alloc(16) != ICG_OK) {
+            set_error("split pipeline: allocation of the exchange word failed");
+            return ICG_ENOMEM;
+        }
+    }
     if (cudaMalloc(&h->xbuf, sizeof(double) * off) != cudaSuccess || cudaMalloc(&S.redv, sizeof(double) * NW * S.RV) != cudaSuccess ||
         cudaMalloc(&S.err, sizeof(int) * 4) != cudaSuccess || cudaMalloc(&S.slm, sizeof(double) * NW * STEP_SLICES * 8) != cudaSuccess ||
         cudaMalloc(&S.slm_cnt, sizeof(int) * NW) != cudaSuccess ||
@@ -2806,9 +2870,12 @@ static int marg_grow(icg_ba *h, int n, int max_m, int max_n0) {
 }
 
 // fmask (resident only, may be NULL): per window, the factor set to marginalize in place of the problem's activity (F bytes each); it reaches
-// ba_lin_vis through a copy of the device view, so the handle's own f_active is never written
+// ba_lin_vis through a copy of the device view, so the handle's own f_active is never written.
+// agree (may be NULL): called once the structure is known, with {largest m, largest r, 1 if a window is rejected} of this batch; it returns
+// the values the eigensolver kernels are chosen by (the owner of a shard group's windows takes the group's maxima, so that it runs the
+// kernels an unsharded handle holding the whole batch runs).  It is called on the rejection path too, so that no peer is left waiting.
 static int marginalize_body(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg, icg_ba_prior *out, bool resident,
-                            const uint8_t *const *fmask = nullptr) {
+                            const uint8_t *const *fmask = nullptr, const std::function<int(int *)> *agree = nullptr) {
     if (!h || !problems || !num_marg || !out || n_windows < 1 || n_windows > h->C.NW) {
         set_error("icg_ba_marginalize: bad arguments");
         return ICG_EINVAL;
@@ -2899,6 +2966,10 @@ static int marginalize_body(icg_ba *h, int n_windows, const icg_ba_problem *prob
         o.m = m, o.r = idx - m, o.nblocks = nb;
         // checked before anything is launched: a rejected call leaves the device state of the handle as it was
         if (m > MARG_MAXN || idx - m > MARG_MAXN) {
+            if (agree) {
+                int mx[3] = {0, 0, 1};
+                (*agree)(mx);
+            }
             set_error("icg_ba_marginalize: window %d: %s=%d exceeds the %d rows of the largest eigensolver kernel", w, m > MARG_MAXN ? "m" : "r",
                       m > MARG_MAXN ? m : idx - m, MARG_MAXN);
             return ICG_EUNSUPPORTED;
@@ -2906,6 +2977,17 @@ static int marginalize_body(icg_ba *h, int n_windows, const icg_ba_problem *prob
     }
     int max_m = 0, max_r = 0, max_n0 = 0;
     for (int w = 0; w < n; w++) max_m = std::max(max_m, out[w].m), max_r = std::max(max_r, out[w].r), max_n0 = std::max(max_n0, out[w].m + out[w].r);
+    int sel_m = max_m, sel_r = max_r;  // what the eigensolver kernels are chosen by
+    if (agree) {
+        int mx[3] = {max_m, max_r, 0};
+        rc = (*agree)(mx);
+        if (rc != ICG_OK) return rc;
+        if (mx[2]) {
+            set_error("icg_ba_marginalize_resident: a window owned by another rank of the shard group was rejected (see that rank's error)");
+            return ICG_EUNSUPPORTED;
+        }
+        sel_m = mx[0], sel_r = mx[1];
+    }
     rc = marg_grow(h, n, max_m, max_n0);
     if (rc != ICG_OK) return rc;
     cudaStream_t s = h->stream;
@@ -2969,10 +3051,10 @@ static int marginalize_body(icg_ba *h, int n_windows, const icg_ba_problem *prob
         }
         return ICG_OK;
     };
-    rc = jacobi(0, max_m);
+    rc = jacobi(0, sel_m);
     if (rc != ICG_OK) return rc;
     marg_schur<<<n, MARG_THREADS, 0, s>>>(M);
-    rc = jacobi(1, max_r);
+    rc = jacobi(1, sel_r);
     if (rc != ICG_OK) return rc;
     marg_finish<<<n, MARG_THREADS, 0, s>>>(M);
     marg_prepare<<<(n + 127) / 128, 128, 0, s>>>(D, M, n, 1);
@@ -3030,17 +3112,265 @@ int icg_ba_marginalize(icg_ba *h, int n_windows, const icg_ba_problem *problems,
     return marginalize_body(h, n_windows, problems, num_marg, out, false);
 }
 
+// ---- post-solve calls of a landmark-sharded group (world > 1, ba_split.cuh)
+extern "C++" {
+template <typename T>
+static int hd_reserve(icg_ba *h, HostDev<T> &b, size_t count) {
+    if (b.d && b.n >= count) return ICG_OK;
+    retire(h, b.d, b.h);  // earlier launches may still use the old buffers
+    b.d = b.h = nullptr, b.n = 0;
+    if (b.alloc(std::max<size_t>(16, count + count / 4)) != ICG_OK) {
+        set_error("landmark-sharded post-solve call: staging allocation of %zu elements failed", count);
+        return ICG_ENOMEM;
+    }
+    return ICG_OK;
+}
+}
+
+static int shard_timed_out(icg_ba *h, const char *what) {
+    if (icg_ba_shard_error(h) == 0) return ICG_OK;
+    set_error("%s: a peer exchange of the shard group timed out (a rank did not make the same call)", what);
+    return ICG_ECUDA;
+}
+
+// enqueue the group's integer exchange of v (device; see ba_xsum)
+static int shard_xsum(icg_ba *h, int *v, int stride, int n, int nv, int op) {
+    const unsigned long long epoch = ++h->epoch;
+    const int par = (int) (h->xs_calls++ & 1);
+    ba_xsum<<<1, 256, 0, h->stream>>>(h->C, h->D, v, stride, n, nv, op, par, epoch);
+    ICG_CHECK_LAUNCH();
+    count_launch();
+    return ICG_OK;
+}
+
+// the group's maxima of three host integers
+static int shard_xmax(icg_ba *h, int *v3) {
+    int rc = hd_reserve(h, h->xs_v, 8);
+    if (rc != ICG_OK) return rc;
+    memcpy(h->xs_v.h, v3, 3 * sizeof(int));
+    ICG_CUDA(h->xs_v.up(h->stream, 3));
+    rc = shard_xsum(h, h->xs_v.d, 3, 1, 3, 1);
+    if (rc != ICG_OK) return rc;
+    ICG_CUDA(h->xs_v.down(h->stream, 3));
+    ICG_CUDA(cudaStreamSynchronize(h->stream));
+    rc = shard_timed_out(h, "icg_ba_marginalize_resident");
+    if (rc != ICG_OK) return rc;
+    memcpy(v3, h->xs_v.h, 3 * sizeof(int));
+    return ICG_OK;
+}
+
+// The resident marginalization on a landmark-sharded handle, a collective call: every rank exports the rows of its factors with
+// f_ref < num_marg (ba_marg_export); the owner of window w (w mod world) gathers the world exports of w in rank order -- global landmark
+// order, since the landmarks are block-partitioned and each rank lists its factors landmark by landmark --, packs the gathered windows' integer
+// structure into a handle of its own (nothing of their values goes through the host: ba_marg_fill copies the gathered rows and the shard
+// handle's resident camera side on the device), and runs the single-GPU marginalization there.  That handle packs the
+// gathered window exactly as an unsharded handle packs the marginalized part of the whole window (runs, Gram partials and pairs of the
+// reference nodes < num_marg depend on those landmarks only), so the prior is the unsharded one, bit for bit.
+static int marginalize_sharded(icg_ba *h, int n, const icg_ba_problem *problems, const int32_t *num_marg, icg_ba_prior *out, const uint8_t *const *fmask,
+                               const char *fn) {
+    const BaCaps &C = h->C;
+    const int G = h->D.world, R = h->D.rank;
+    if (!problems || !num_marg || !out || n < 1 || n > C.NW) {
+        set_error("%s: bad arguments", fn);
+        return ICG_EINVAL;
+    }
+    if (h->cur_windows != n) {
+        set_error("%s: the handle holds %d uploaded windows, the call names %d", fn, h->cur_windows, n);
+        return ICG_EINVAL;
+    }
+    for (int r = 0; r < G; r++)
+        if (!h->D.S.peer[r]) {
+            set_error("%s: peer %d is not connected (icg_ba_shard_connect)", fn, r);
+            return ICG_EINVAL;
+        }
+    // every check before anything is launched: a rank that returns here leaves its peers to the bounded waits
+    size_t n_sel = 0;
+    for (int w = 0; w < n; w++) {
+        const icg_ba_problem &p = problems[w];
+        const WinDims &d = h->dims.h[w];
+        const icg_ba_prior &o = out[w];
+        if (p.K != d.K || p.L != d.L || p.F != d.F || (p.F > 0 && (!p.f_lm || !p.f_ref || !p.f_obs))) {
+            set_error("%s: window %d does not describe the uploaded shard (K=%d L=%d F=%d)", fn, w, p.K, p.L, p.F);
+            return ICG_EINVAL;
+        }
+        if (num_marg[w] < 1 || num_marg[w] >= p.K || !o.block_type || !o.block_node || !o.x0 || !o.J0 || !o.e0 || o.rcap < 15 * (p.K - num_marg[w]) + 7) {
+            set_error("%s: window %d: num_marg=%d out of range or output arrays missing / too small (rcap=%d)", fn, w, num_marg[w], o.rcap);
+            return ICG_EINVAL;
+        }
+        for (int f = 0; f < p.F; f++) {
+            if (f > 0 && p.f_lm[f] < p.f_lm[f - 1]) {
+                set_error("%s: window %d factor %d: a landmark-sharded window must list its factors landmark by landmark (f_lm non-decreasing)", fn, w, f);
+                return ICG_EINVAL;
+            }
+            n_sel += p.f_ref[f] < num_marg[w];
+        }
+    }
+    ICG_CUDA(cudaSetDevice(h->device));
+    cudaStream_t s = h->stream;
+    int rc = marg_alloc(h);  // marg_fmask: the culled factor set the export reads
+    if (rc != ICG_OK) return rc;
+    if ((rc = hd_reserve(h, h->mx_sel, n_sel + n + 1)) != ICG_OK) return rc;
+    int *sel = h->mx_sel.h, *sel_off = sel + n_sel;
+    {   // the record slots of the exported factors, in factor order (the inverse of the packing's slot -> factor table)
+        size_t at = 0;
+        std::vector<int> slot_of;
+        for (int w = 0; w < n; w++) {
+            const icg_ba_problem &p = problems[w];
+            slot_of.assign(p.F, 0);
+            const int *fidx = h->lm_fidx.h + (size_t) w * C.F;
+            for (int q = 0; q < p.F; q++) slot_of[fidx[q]] = q;
+            sel_off[w] = (int) at;
+            for (int f = 0; f < p.F; f++)
+                if (p.f_ref[f] < num_marg[w]) sel[at++] = slot_of[f];
+            if (fmask) memcpy(h->marg_fmask.h + (size_t) w * C.F, fmask[w], p.F);
+        }
+        sel_off[n] = (int) at;
+    }
+    ICG_CUDA(h->mx_sel.up(s, n_sel + n + 1));
+    if (fmask) ICG_CUDA(h->marg_fmask.up(s, (size_t) n * C.F));
+    const unsigned long long epoch = ++h->epoch;
+    ba_marg_export<<<n, 128, 0, s>>>(C, h->D, h->mx_sel.d, h->mx_sel.d + n_sel, fmask ? h->marg_fmask.d : nullptr, h->exp_epoch);
+    ba_xflag<<<1, 32, 0, s>>>(h->D, XF_EXPORT, epoch);
+    h->exp_epoch = epoch;
+    count_launch(2);
+    const int n_own = R < n ? (n - R + G - 1) / G : 0;
+    std::vector<int> row0(n_own + 1, 0);
+    if (n_own > 0) {
+        if ((rc = hd_reserve(h, h->mx_heads, 2 * (size_t) n_own * G)) != ICG_OK) return rc;
+        ba_marg_heads<<<1, 256, 0, s>>>(C, h->D, n_own, h->mx_heads.d, epoch);
+        ICG_CUDA(h->mx_heads.down(s, 2 * (size_t) n_own * G));
+        ICG_CUDA(cudaStreamSynchronize(s));
+        if ((rc = shard_timed_out(h, fn)) != ICG_OK) return rc;
+        if ((rc = hd_reserve(h, h->mx_row, (size_t) n_own * G + n_own + 1)) != ICG_OK) return rc;
+        size_t tot = 0;
+        for (int e = 0; e < n_own * G; e++) {
+            if (e % G == 0) row0[e / G] = (int) tot;
+            h->mx_row.h[e] = (int) tot;
+            tot += (size_t) h->mx_heads.h[2 * e + 1];
+        }
+        row0[n_own] = (int) tot;
+        if (tot > (size_t) INT32_MAX / MEXP_ROW) {
+            set_error("%s: %zu gathered factors exceed the gather buffer's index range", fn, tot);
+            return ICG_EINVAL;
+        }
+        if (tot * MEXP_ROW > h->mx_rows_cap) {
+            retire(h, h->mx_rows, nullptr), h->mx_rows = nullptr;
+            h->mx_rows_cap = 0;
+            const size_t cap = (tot + tot / 4) * MEXP_ROW;
+            if (cudaMalloc(&h->mx_rows, sizeof(double) * cap) != cudaSuccess) {
+                set_error("%s: gather buffer allocation of %zu doubles failed", fn, cap);
+                return ICG_ENOMEM;
+            }
+            h->mx_rows_cap = cap;
+        }
+        if ((rc = hd_reserve(h, h->mx_idx, std::max<size_t>(1, tot))) != ICG_OK) return rc;
+        memcpy(h->mx_row.h + (size_t) n_own * G, row0.data(), sizeof(int) * (n_own + 1));
+        ICG_CUDA(h->mx_row.up(s, (size_t) n_own * G + n_own + 1));
+        ba_marg_gather<<<dim3(n_own, G), 256, 0, s>>>(C, h->D, h->mx_heads.d, h->mx_row.d, h->mx_rows);
+        count_launch(2);
+        if (tot) ICG_CUDA(cudaMemcpy2DAsync(h->mx_idx.h, sizeof(long long), h->mx_rows, sizeof(double) * MEXP_ROW, sizeof(long long), tot, cudaMemcpyDeviceToHost, s));
+    }
+    ba_xflag<<<1, 32, 0, s>>>(h->D, XF_DONE, epoch);  // this rank's reads of the exports are enqueued: the exporters may reuse their regions
+    ICG_CHECK_LAUNCH();
+    count_launch();
+    for (int w = 0; w < n; w++)
+        if (w % G != R) out[w].m = out[w].r = out[w].nblocks = 0;
+    h->marg_res_n = 0;  // the sharded slide is not available: no resident prior is kept
+    if (n_own == 0) {
+        int mx[3] = {0, 0, 0};
+        rc = shard_xmax(h, mx);
+        if (rc != ICG_OK) return rc;
+        if (mx[2]) {
+            set_error("%s: a window owned by another rank of the shard group was rejected (see that rank's error)", fn);
+            return ICG_EUNSUPPORTED;
+        }
+        return ICG_OK;
+    }
+    ICG_CUDA(cudaStreamSynchronize(s));
+    if ((rc = shard_timed_out(h, fn)) != ICG_OK) return rc;
+    // the gathered windows, structure on the host (values follow on the device): landmarks renumbered densely in (rank, shard landmark) order
+    std::vector<icg_ba_problem> gp(n_own);
+    std::vector<std::vector<int32_t>> g_lm(n_own), g_ref(n_own), g_obs(n_own);
+    std::vector<std::vector<uint8_t>> g_act(n_own);
+    int max_L = 1, max_F = 1;
+    for (int j = 0; j < n_own; j++) {
+        const int w = R + j * G, F = row0[j + 1] - row0[j];
+        const icg_ba_problem &p = problems[w];
+        g_lm[j].resize(F), g_ref[j].resize(F), g_obs[j].resize(F), g_act[j].resize(F);
+        int L = 0, last_r = -1, last_l = -1;
+        for (int r = 0, i = 0; r < G; r++)
+            for (long long k = 0; k < h->mx_heads.h[2 * ((size_t) j * G + r) + 1]; k++, i++) {
+                const unsigned long long x = (unsigned long long) h->mx_idx.h[row0[j] + i];
+                const int l = (int) (x & 0xffffffffu), hi = (int) (x >> 32), ref = hi & 255, obs = (hi >> 8) & 255;
+                if (r != last_r || l != last_l) L++, last_r = r, last_l = l;
+                if (ref >= num_marg[w] || obs >= p.K) {
+                    set_error("%s: window %d: gathered factor %d names nodes %d / %d (the ranks' windows differ)", fn, w, i, ref, obs);
+                    int mx[3] = {0, 0, 1};
+                    shard_xmax(h, mx);
+                    return ICG_EINVAL;
+                }
+                g_lm[j][i] = L - 1, g_ref[j][i] = ref, g_obs[j][i] = obs, g_act[j][i] = (uint8_t) ((hi >> 16) & 1);
+            }
+        icg_ba_problem &q = gp[j];
+        q = p;
+        q.L = L, q.F = F;
+        q.f_lm = g_lm[j].data(), q.f_ref = g_ref[j].data(), q.f_obs = g_obs[j].data(), q.f_active = g_act[j].data();
+        max_L = std::max(max_L, L), max_F = std::max(max_F, F);
+    }
+    double unread = 0;  // the structure-only packing checks these pointers but reads no value: ba_marg_fill writes them on the device
+    for (auto &q : gp) q.invdepth = &unread, q.f_const = &unread;
+    icg_ba *&mh = h->mx_h;
+    if (mh && (mh->C.NW < n_own || mh->C.L < max_L || mh->C.F < max_F)) {
+        max_L = std::max(max_L, mh->C.L), max_F = std::max(max_F, mh->C.F);
+        h->retired_mx.push_back(mh), mh = nullptr;
+    }
+    if (!mh) {
+        const int nw = std::max(n_own, (C.NW + G - 1) / G);
+        rc = icg_ba_create(&mh, nw, C.K, max_L + max_L / 4, max_F + max_F / 4, C.G, C.R, h->device, (void *) s);
+        if (rc != ICG_OK) {
+            mh = nullptr;
+            int mx[3] = {0, 0, 1};
+            shard_xmax(h, mx);
+            return rc;
+        }
+    }
+    // structure only (landmark positions, record slots, lin_vis runs, Gram partials, pairs; the small camera-side tables): the same packing
+    // icg_ba_upload does, so the sums match an unsharded handle's.  Every value comes from the device: the gathered rows, and the shard
+    // handle's resident camera side (parameters, IMU blobs and square-root information, GNSS, the carried prior's normal equations).
+    rc = pack_windows(mh, n_own, gp.data(), false);
+    if (rc == ICG_OK) rc = upload_structure(mh, n_own);
+    if (rc == ICG_OK) {
+        mh->cur_windows = n_own, mh->marg_res_n = 0;
+        ICG_CUDA(mh->lm_fidx.up(s, (size_t) n_own * mh->C.F));
+        ba_marg_fill<<<n_own, 128, 0, s>>>(mh->C, mh->D, C, h->D, h->mx_rows, h->mx_row.d + (size_t) n_own * G, mh->lm_fidx.d);
+        ICG_CHECK_LAUNCH();
+        count_launch();
+    } else {
+        int mx[3] = {0, 0, 1};
+        shard_xmax(h, mx);
+        return rc;
+    }
+    std::vector<int32_t> nm(n_own);
+    std::vector<icg_ba_prior> po(n_own);
+    for (int j = 0; j < n_own; j++) nm[j] = num_marg[R + j * G], po[j] = out[R + j * G];
+    const std::function<int(int *)> agree = [h](int *mx) { return shard_xmax(h, mx); };
+    rc = marginalize_body(mh, n_own, gp.data(), nm.data(), po.data(), true, nullptr, &agree);
+    for (int j = 0; j < n_own; j++) out[R + j * G].m = po[j].m, out[R + j * G].r = po[j].r, out[R + j * G].nblocks = po[j].nblocks;
+    return rc;
+}
+
 int icg_ba_marginalize_resident(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg, icg_ba_prior *out) {
+    if (h && h->D.world > 1) return marginalize_sharded(h, n_windows, problems, num_marg, out, nullptr, "icg_ba_marginalize_resident");
     return marginalize_body(h, n_windows, problems, num_marg, out, true);
 }
 
 // ---- post-solve map update + outlier culling (ba_cull.cu)
-static int resident_single_rank(icg_ba *h, int n_windows, const icg_ba_problem *problems, const char *what) {
+static int resident_single_rank(icg_ba *h, int n_windows, const icg_ba_problem *problems, const char *what, bool sharded_ok = false) {
     if (!h || !problems || n_windows < 1) {
         set_error("%s: bad arguments", what);
         return ICG_EINVAL;
     }
-    if (h->D.world > 1) {
+    if (h->D.world > 1 && !sharded_ok) {
         set_error("%s: not available on a landmark-sharded handle (icg_ba_shard_leave first)", what);
         return ICG_EUNSUPPORTED;
     }
@@ -3053,7 +3383,7 @@ static int resident_single_rank(icg_ba *h, int n_windows, const icg_ba_problem *
 
 int icg_ba_update_and_cull_resident(icg_ba *h, int n_windows, const icg_ba_problem *problems, const icg_camera *cam, double reprojection_error_std,
                                     icg_ba_cull_window *io) {
-    int rc = resident_single_rank(h, n_windows, problems, "icg_ba_update_and_cull_resident");
+    int rc = resident_single_rank(h, n_windows, problems, "icg_ba_update_and_cull_resident", true);
     if (rc != ICG_OK) return rc;
     if (!cam || !io) {
         set_error("icg_ba_update_and_cull_resident: bad arguments");
@@ -3111,8 +3441,7 @@ int icg_ba_update_and_cull_resident(icg_ba *h, int n_windows, const icg_ba_probl
     cudaStream_t s = h->stream;
     if (at > h->cull_cap) {
         ICG_CUDA(cudaStreamSynchronize(s));
-        if (h->cull_h) cudaFreeHost(h->cull_h), h->cull_h = nullptr;
-        if (h->cull_d) cudaFree(h->cull_d), h->cull_d = nullptr;
+        retire(h, h->cull_d, h->cull_h), h->cull_h = nullptr, h->cull_d = nullptr;
         h->cull_cap = 0;
         const size_t cap = at + at / 4;
         if (cudaMallocHost(&h->cull_h, cap) != cudaSuccess || cudaMalloc(&h->cull_d, cap) != cudaSuccess) {
@@ -3147,8 +3476,13 @@ int icg_ba_update_and_cull_resident(icg_ba *h, int n_windows, const icg_ba_probl
     a.lm_outlier = Dv + o_lmo, a.obs_outlier = Dv + o_obso;
     ICG_CUDA(launch_update_cull(a, n, s));
     count_launch();
+    if (h->D.world > 1) {  // landmark shards: every rank's counters become the window's totals (the other outputs are the camera side or its shard's)
+        rc = shard_xsum(h, (int *) (Dv + o_win + offsetof(CullOut, counts)), (int) (sizeof(CullOut) / sizeof(int)), n, 5, 0);
+        if (rc != ICG_OK) return rc;
+    }
     ICG_CUDA(cudaMemcpyAsync(H + in_bytes, Dv + in_bytes, out_bytes, cudaMemcpyDeviceToHost, s));
     ICG_CUDA(cudaStreamSynchronize(s));
+    if (h->D.world > 1 && (rc = shard_timed_out(h, "icg_ba_update_and_cull_resident")) != ICG_OK) return rc;
     for (int w = 0; w < n; w++) {
         const icg_ba_problem &p = problems[w];
         icg_ba_cull_window &c = io[w];
@@ -3305,7 +3639,7 @@ int icg_ba_reintegrate_resident(icg_ba *h, int n_windows, const icg_ba_problem *
 
 int icg_ba_marginalize_resident_culled(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg,
                                        const icg_ba_cull_window *culled, const uint8_t *const *node_in_map, icg_ba_prior *out) {
-    int rc = resident_single_rank(h, n_windows, problems, "icg_ba_marginalize_resident_culled");
+    int rc = resident_single_rank(h, n_windows, problems, "icg_ba_marginalize_resident_culled", true);
     if (rc != ICG_OK) return rc;
     if (!culled || !node_in_map) {
         set_error("icg_ba_marginalize_resident_culled: bad arguments");
@@ -3343,6 +3677,7 @@ int icg_ba_marginalize_resident_culled(icg_ba *h, int n_windows, const icg_ba_pr
             if (lm_bad[p.f_lm[f]] || !node_in_map[w][p.f_obs[f]]) m[f] = 0;
         mp[w] = m.data();
     }
+    if (h->D.world > 1) return marginalize_sharded(h, n_windows, problems, num_marg, out, mp.data(), "icg_ba_marginalize_resident_culled");
     return marginalize_body(h, n_windows, problems, num_marg, out, true, mp.data());
 }
 
@@ -3734,7 +4069,7 @@ int icg_ba_slide_integrate_resident(icg_ba *h, int n, const icg_ba_problem *next
 
 // ---- landmark shards over peer memory (transport "p2p")
 struct ShardBlob {  // what a rank publishes to the others (ICG_SHARD_BLOB_BYTES)
-    uint64_t magic, pid, ptr, doubles;
+    uint64_t magic, pid, ptr, doubles;  // doubles: the part of the exchange buffer every rank lays out alike (the export region is per rank)
     int32_t rank, world, device, pad;
     cudaIpcMemHandle_t ipc;
 };
@@ -3749,7 +4084,7 @@ int icg_ba_shard_export(icg_ba *h, int rank, int world, uint8_t *blob) {
     if (rc != ICG_OK) return rc;
     ShardBlob b;
     memset(&b, 0, sizeof(b));
-    b.magic = 0x49434753484152ull, b.pid = (uint64_t) getpid(), b.ptr = (uint64_t) (uintptr_t) h->xbuf, b.doubles = h->xbuf_doubles;
+    b.magic = 0x49434753484152ull, b.pid = (uint64_t) getpid(), b.ptr = (uint64_t) (uintptr_t) h->xbuf, b.doubles = h->D.S.off_exp;
     b.rank = rank, b.world = world, b.device = h->device;
     if (world > 1) ICG_CUDA(cudaIpcGetMemHandle(&b.ipc, h->xbuf));
     memset(blob, 0, ICG_SHARD_BLOB_BYTES);
@@ -3767,7 +4102,7 @@ int icg_ba_shard_connect(icg_ba *h, const uint8_t *blobs) {
     for (int r = 0; r < world; r++) {
         ShardBlob b;
         memcpy(&b, blobs + (size_t) r * ICG_SHARD_BLOB_BYTES, sizeof(b));
-        if (b.magic != 0x49434753484152ull || b.rank != r || b.world != world || b.doubles != h->xbuf_doubles) {
+        if (b.magic != 0x49434753484152ull || b.rank != r || b.world != world || b.doubles != h->D.S.off_exp) {
             set_error("icg_ba_shard_connect: blob %d does not describe rank %d of %d with the same window capacity", r, r, world);
             return ICG_EINVAL;
         }

@@ -152,6 +152,11 @@ __global__ void __launch_bounds__(CULL_THREADS) ba_update_cull(CullArgs a) {
 
 }  // namespace
 
+cudaError_t preload_update_cull() {
+    cudaFuncAttributes attr;
+    return cudaFuncGetAttributes(&attr, ba_update_cull);
+}
+
 cudaError_t launch_update_cull(const CullArgs &a, int n_windows, cudaStream_t stream) {
     ba_update_cull<<<n_windows, CULL_THREADS, 0, stream>>>(a);
     return cudaGetLastError();

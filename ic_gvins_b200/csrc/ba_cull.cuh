@@ -39,5 +39,7 @@ struct CullArgs {
 
 // one CTA of CULL_THREADS per window, on `stream`
 cudaError_t launch_update_cull(const CullArgs &a, int n_windows, cudaStream_t stream);
+// loads the kernel into the current context (landmark-shard groups load every kernel up front: ba.cu, preload_group_kernels)
+cudaError_t preload_update_cull();
 
 }  // namespace icg

@@ -1204,4 +1204,133 @@ __global__ void __launch_bounds__(128) ba_accept_split(BaCaps C, BaDev D, unsign
     for (int e = tid; e < dm.L; e += 128) rho[e] = rho_c[e];
 }
 
+// ------------------------------------------------------------------------------------------------ after the solve (shard groups, world > 1)
+// The post-solve calls of a landmark-sharded group use three more regions of the exchange buffer (offsets in ShardDev):
+//   off_flagX  [3][8] u64 epoch flags by source rank: XF_SUM (integer exchange), XF_EXPORT (marginalization rows published), XF_DONE (the
+//              owner has gathered them: the exporter may overwrite its region)
+//   off_post   [2][NW][world][SPLIT_SCAL] slots of the integer exchange, double-buffered by call parity
+//   off_exp    this rank's marginalization export: [NW][2] int64 (first row, row count), then the rows, MEXP_ROW doubles each
+// These kernels only move data and sum or compare integers: no floating-point arithmetic, so FMA contraction cannot change a result.
+constexpr int MEXP_ROW = 16;  // [landmark | f_ref, f_obs, active (int64 bits)] | inverse depth | f_const[14]
+enum { XF_SUM = 0, XF_EXPORT = 1, XF_DONE = 2 };
+
+__device__ __forceinline__ unsigned long long *x_flagX(const BaDev &D, int peer, int kind, int from) {
+    return (unsigned long long *) (D.S.peer[peer] + D.S.off_flagX) + kind * 8 + from;
+}
+
+// release flag `kind` of this rank on every peer: what earlier kernels of the stream stored has been issued
+__global__ void ba_xflag(BaDev D, int kind, unsigned long long epoch) {
+    const int q = threadIdx.x;
+    if (q >= D.world) return;
+    __threadfence_system();
+    st_release_sys(x_flagX(D, q, kind, D.rank), epoch);
+}
+
+// Integer exchange of the group: v[s * stride + k] (s < n <= NW, k < nv <= SPLIT_SCAL) of every rank is stored into slot [s][rank] of every
+// rank; each rank waits for the world flags and replaces v by the rank-order sum (op 0) or maximum (op 1).  Integers below 2^53 are exact
+// as doubles, so the sum is the unsharded count whatever the order.  A slot is rewritten two calls later, after every rank has passed the
+// wait of the call in between (which follows its reads in stream order): parity double-buffering is enough.
+__global__ void __launch_bounds__(256) ba_xsum(BaCaps C, BaDev D, int *v, int stride, int n, int nv, int op, int par, unsigned long long epoch) {
+    const int tid = threadIdx.x;
+    auto slot = [&](int peer, int s, int from) {
+        return D.S.peer[peer] + D.S.off_post + (((size_t) par * C.NW + s) * D.world + from) * SPLIT_SCAL;
+    };
+    for (int e = tid; e < n * nv; e += 256) {
+        const int s = e / nv, k = e - s * nv;
+        const double x = (double) v[(size_t) s * stride + k];
+        for (int q = 0; q < D.world; q++) slot(q, s, D.rank)[k] = x;
+    }
+    __threadfence_system();
+    __syncthreads();
+    if (tid < D.world) {
+        st_release_sys(x_flagX(D, tid, XF_SUM, D.rank), epoch);
+        wait_flag(x_flagX(D, D.rank, XF_SUM, tid), epoch, D.S.err);
+    }
+    __syncthreads();
+    for (int e = tid; e < n * nv; e += 256) {
+        const int s = e / nv, k = e - s * nv;
+        double acc = 0;
+        for (int r = 0; r < D.world; r++) {
+            const double x = __ldcg(slot(D.rank, s, r) + k);
+            acc = op ? (r == 0 ? x : fmax(acc, x)) : acc + x;
+        }
+        v[(size_t) s * stride + k] = (int) acc;
+    }
+}
+
+// Marginalization export (every rank), CTA per window: the record slots sel[sel_off[w] .. sel_off[w + 1]) -- the factors with f_ref < num_marg,
+// in factor order -- become rows sel_off[w] .. of this rank's export region.  `fmask` (by factor id) is the culled factor set, NULL: f_active.
+// Before writing, every owner must have gathered the previous export (XF_DONE >= prev).
+__global__ void __launch_bounds__(128) ba_marg_export(BaCaps C, BaDev D, const int *sel, const int *sel_off, const uint8_t *fmask, unsigned long long prev) {
+    const int w = blockIdx.x, tid = threadIdx.x;
+    if (tid < D.world) wait_flag(x_flagX(D, D.rank, XF_DONE, tid), prev, D.S.err);
+    __syncthreads();
+    double *X = D.S.peer[D.rank] + D.S.off_exp;
+    const int r0 = sel_off[w], nr = sel_off[w + 1] - r0;
+    if (tid == 0) ((long long *) X)[2 * w] = r0, ((long long *) X)[2 * w + 1] = nr;
+    double *rows = X + 2 * (size_t) C.NW + (size_t) r0 * MEXP_ROW;
+    for (int e = tid; e < nr * MEXP_ROW; e += 128) {
+        const int i = e / MEXP_ROW, c = e - i * MEXP_ROW, q = sel[r0 + i];
+        const int *mt = D.f_meta_s + ((size_t) w * C.F + q) * 4;
+        double x;
+        if (c == 0) {
+            const int fid = mt[3];
+            const int act = (fmask ? fmask : D.f_active)[(size_t) w * C.F + fid] != 0;
+            x = __longlong_as_double((long long) (unsigned) mt[0] | ((long long) (mt[1] | (mt[2] << 8) | (act << 16)) << 32));
+        } else if (c == 1) {
+            x = D.rho[(size_t) w * C.L + mt[0]];
+        } else {
+            x = D.f_const_s[((size_t) w * C.F + q) * 14 + c - 2];
+        }
+        rows[e] = x;
+    }
+}
+
+// Owner: wait for the world exports of this epoch and read the (first row, count) of every owned window j (w = rank + j world) from every rank
+__global__ void ba_marg_heads(BaCaps C, BaDev D, int n_own, long long *heads, unsigned long long epoch) {
+    const int tid = threadIdx.x;
+    if (tid < D.world) wait_flag(x_flagX(D, D.rank, XF_EXPORT, tid), epoch, D.S.err);
+    __syncthreads();
+    for (int e = tid; e < n_own * D.world; e += blockDim.x) {
+        const int j = e / D.world, r = e - j * D.world, w = D.rank + j * D.world;
+        const long long *hdr = (const long long *) (D.S.peer[r] + D.S.off_exp);
+        heads[2 * e] = __ldcg(hdr + 2 * w), heads[2 * e + 1] = __ldcg(hdr + 2 * w + 1);
+    }
+}
+
+// Owner, CTA per (owned window j, rank r): peer loads of rank r's rows of window j into dst, at row dst_row[j world + r] (rank order)
+__global__ void __launch_bounds__(256) ba_marg_gather(BaCaps C, BaDev D, const long long *heads, const int *dst_row, double *dst) {
+    const int e0 = blockIdx.x * D.world + blockIdx.y;
+    const long long r0 = heads[2 * e0], nr = heads[2 * e0 + 1];
+    const double *src = D.S.peer[blockIdx.y] + D.S.off_exp + 2 * (size_t) C.NW + (size_t) r0 * MEXP_ROW;
+    double *d = dst + (size_t) dst_row[e0] * MEXP_ROW;
+    for (long long e = threadIdx.x; e < nr * MEXP_ROW; e += 256) d[e] = __ldcg(src + e);
+}
+
+// Owner: the values of the gathered windows in the handle (Cm, Dm) their structure was packed into (window j <- the shard handle's window
+// rank + j world): factor constants by record slot and inverse depths by landmark from the gathered rows, and the shard handle's resident
+// camera side (solved parameters, IMU blobs and square-root information, GNSS fixes and sigmas, the carried prior's H0 / b0 / c0).
+// Cm has the shard handle's K, G and R strides.
+__global__ void __launch_bounds__(128) ba_marg_fill(BaCaps Cm, BaDev Dm, BaCaps C, BaDev D, const double *rows, const int *row0, const int *fidx) {
+    const int j = blockIdx.x, tid = threadIdx.x, w = D.rank + j * D.world;
+    const int F = Dm.dims[j].F, K = D.dims[w].K, ng = D.dims[w].n_gnss, ni = D.dims[w].n_imu, r = D.dims[w].marg_r;
+    for (int e = tid; e < F * 15; e += 128) {
+        const int q = e / 15, c = e - q * 15;
+        const double *row = rows + ((size_t) row0[j] + fidx[(size_t) j * Cm.F + q]) * MEXP_ROW;
+        if (c < 14) Dm.f_const_s[((size_t) j * Cm.F + q) * 14 + c] = row[2 + c];
+        else Dm.rho[(size_t) j * Cm.L + Dm.f_meta_s[((size_t) j * Cm.F + q) * 4]] = row[1];  // every factor of a landmark carries the same value
+    }
+    for (int e = tid; e < K * 7; e += 128) Dm.pose[(size_t) j * Cm.K * 7 + e] = D.pose[(size_t) w * C.K * 7 + e];
+    for (int e = tid; e < K * 9; e += 128) Dm.mix[(size_t) j * Cm.K * 9 + e] = D.mix[(size_t) w * C.K * 9 + e];
+    if (tid < 8) Dm.ext[(size_t) j * 8 + tid] = D.ext[(size_t) w * 8 + tid];
+    for (int e = tid; e < ng * 3; e += 128) Dm.gnss_std[(size_t) j * Cm.G * 3 + e] = D.gnss_std[(size_t) w * C.G * 3 + e];
+    for (int e = tid; e < ng * 3; e += 128) Dm.gnss_blh[(size_t) j * Cm.G * 3 + e] = D.gnss_blh[(size_t) w * C.G * 3 + e];
+    for (int e = tid; e < ni * ICG_IMU_BLOB_DOUBLES; e += 128)
+        Dm.imu_blob[(size_t) j * Cm.K * ICG_IMU_BLOB_DOUBLES + e] = D.imu_blob[(size_t) w * C.K * ICG_IMU_BLOB_DOUBLES + e];
+    for (int e = tid; e < ni * 225; e += 128) Dm.imu_U[(size_t) j * Cm.K * 225 + e] = D.imu_U[(size_t) w * C.K * 225 + e];
+    for (int e = tid; e < r * r; e += 128) Dm.marg_H0[(size_t) j * Cm.R * Cm.R + e] = D.marg_H0[(size_t) w * C.R * C.R + e];
+    for (int e = tid; e < r; e += 128) Dm.marg_b0[(size_t) j * Cm.R + e] = D.marg_b0[(size_t) w * C.R + e];
+    if (tid == 0) Dm.marg_c0[j] = D.marg_c0[w];
+}
+
 }  // namespace icg

@@ -251,6 +251,9 @@ public:
     }
     // The same on the window this solver just optimised, with the factor set of the map after updateAndCull (IG/ic_gvins.cc:1558-1609):
     // culled = that call's io (obs_factor set), node_in_map = K flags, 0 for the keyframes gvinsRemoveAllSecondNewFrame took out of the map.
+    // Both resident forms also run on a landmark-sharded handle: every rank calls with its shard, and the prior is returned on the window's
+    // owner (rank w mod world) only.  Elsewhere m = r = 0, block_type / block_node / J0 / e0 come back empty and x0 keeps its capacity
+    // unwritten, as for any prior (icgvins_b200.h, icg_ba_marginalize_resident).
     Prior marginalization(const icg_ba_problem &problem, int num_marg, const icg_ba_cull_window &culled, const uint8_t *node_in_map) {
         return marginalize(problem, num_marg, [&](const int32_t *nm, icg_ba_prior *o) {
             return icg_ba_marginalize_resident_culled(h_, 1, &problem, nm, &culled, &node_in_map, o);
@@ -259,7 +262,8 @@ public:
 
     // updateParametersFromOptimizer + gvinsOutlierCulling (IG/ic_gvins.cc:1232-1236) on the window this solver just optimised: io carries the
     // observation lists the caller gathered and receives pose_b_c_ / td_b_c_, every node's frame->pose(), every landmark's pos() / depth and
-    // the outlier flags (see icg_ba_cull_window); the caller applies them to its object graph.
+    // the outlier flags (see icg_ba_cull_window); the caller applies them to its object graph.  On a landmark-sharded handle every rank passes
+    // its shard and its landmarks' observation lists; the counts are the window's totals on every rank, the landmark outputs its shard's.
     void updateAndCull(const icg_ba_problem &problem, const icg_camera &camera, double reprojection_error_std, icg_ba_cull_window &io) {
         check(icg_ba_update_and_cull_resident(h_, 1, &problem, &camera, reprojection_error_std, &io), "icg_ba_update_and_cull_resident");
     }

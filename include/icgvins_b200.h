@@ -511,7 +511,8 @@ int icg_ba_sync(icg_ba *h);
  * an unordered_map (implementation-defined) and only permutes rows / columns.
  * Sizes: the device workspace follows the batch (its largest m and m + r), not the handle's max_K / max_L, so any handle marginalizes,
  * cfg-4 windows (max_K = 20, max_L = 2000) included.  A window whose m or r exceeds 512 rows (the largest eigensolver) returns
- * ICG_EUNSUPPORTED naming the window, before anything runs on the device.  Landmark-sharded handles return ICG_EUNSUPPORTED.  The next
+ * ICG_EUNSUPPORTED naming the window, before anything runs on the device.  Landmark-sharded handles return ICG_EUNSUPPORTED here (the
+ * resident forms below run on them).  The next
  * window consumes the prior through icg_ba_problem.marg_r <= max_marg_r: a window of K nodes can need 15 (K - 1) + 7 rows (292 at K = 20).
  */
 typedef struct icg_ba_prior {
@@ -525,7 +526,18 @@ int icg_ba_marginalize(icg_ba *h, int n_windows, const icg_ba_problem *problems,
 /* The same on the windows the handle already holds: gvinsMarginalization runs right after gvinsOptimization on the same window
  * (IG/ic_gvins.cc:560-567 -> 1412), so after icg_ba_gvins_optimization[_end] / icg_ba_solve the device copy already has the optimised
  * parameters, the culled factor set and the re-weighted GNSS sigmas; nothing is packed or uploaded again.  `problems` must be the array
- * of that solve (n_windows equal to the uploaded count; read for the factor structure and x0 only). */
+ * of that solve (n_windows equal to the uploaded count; read for the factor structure and x0 only).
+ * Landmark-sharded handle (world > 1): a COLLECTIVE call.  Every rank calls with its shard problems (what it uploaded) and the same
+ * num_marg; each window must list its factors landmark by landmark (f_lm non-decreasing, as the reference builds them), which is checked
+ * before anything is launched.  Every rank exports the rows of its factors with f_ref < num_marg; the owner of window w (rank w mod world)
+ * gathers them over peer memory in rank order and forms the prior with the single-GPU kernels: out[w] is bit-for-bit what an unsharded
+ * handle holding the same values produces.  out[w] is filled on the owner only; on every other rank out[w].m = r = nblocks = 0 and its
+ * arrays are not written.  No resident prior is kept for a slide (both slides remain unavailable on sharded handles).  A rank that
+ * rejects its arguments leaves its peers to the bounded flag waits: they return ICG_ECUDA (icg_ba_shard_error).
+ * Memory: each rank's export region (max_windows x max_F x 128 bytes, allocated by icg_ba_shard_export), and on an owner a second handle
+ * the gathered windows are marginalized in (ceil(max_windows / world) windows, this handle's max_K / max_gnss / max_marg_r, 1.25 x the
+ * largest gathered window's landmarks and factors; created on the first call, grown when a batch needs more).  Buffers a call outgrows
+ * are freed by icg_ba_shard_leave, the next icg_ba_shard_export or icg_ba_destroy. */
 int icg_ba_marginalize_resident(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg, icg_ba_prior *out);
 /*
  * The rest of GVINS::gvinsOptimization after the second Solve (IG/ic_gvins.cc:1232-1236), on the windows the handle holds:
@@ -568,7 +580,11 @@ typedef struct icg_ba_cull_window {
 } icg_ba_cull_window;
 /* One CTA per window; the observation lists go up in one copy through pinned staging and the outputs come back in one copy; synchronous.
  * `problems` is the array of the solve (n_windows equal to the uploaded count; K and L are read).  The handle's state (parameters,
- * factor activity, GNSS sigmas) is not changed.  ICG_EUNSUPPORTED on a landmark-sharded handle. */
+ * factor activity, GNSS sigmas) is not changed.
+ * Landmark-sharded handle (world > 1): a collective call.  Every rank passes its shard problems and, per window, the observation lists of
+ * its own landmarks in shard order.  cam_pose, the extrinsic outputs and td_bc_out come from the replicated camera side and are the same on
+ * every rank; lm_pw, lm_depth, lm_outlier and obs_outlier cover the caller's shard; counts are the window's totals on every rank (summed
+ * over the ranks through the peer-memory exchange buffer). */
 int icg_ba_update_and_cull_resident(icg_ba *h, int n_windows, const icg_ba_problem *problems, const icg_camera *cam, double reprojection_error_std,
                                     icg_ba_cull_window *io);
 /* icg_ba_marginalize_resident on the map after the culling: reprojection factor f of a landmark anchored in a removed node is marginalized
@@ -576,7 +592,8 @@ int icg_ba_update_and_cull_resident(icg_ba *h, int n_windows, const icg_ba_probl
  * node_in_map[w][f_obs[f]] is set (the keyframes gvinsRemoveAllSecondNewFrame left in the map, IG/ic_gvins.cc:1391-1410): the factor set
  * gvinsMarginalization builds (:1558-1609).  The chi-square activity plays no part (removeReprojectionFactorsByChi2 never marks a feature).
  * culled: the io array of icg_ba_update_and_cull_resident after that call (obs_factor must be set); node_in_map: K bytes per window.  The
- * handle's factor activity is not changed. */
+ * handle's factor activity is not changed.  On a landmark-sharded handle: collective, as icg_ba_marginalize_resident; each rank passes its
+ * own `culled` array (its shard's landmarks, obs_factor naming its shard's factors) and the same node_in_map. */
 int icg_ba_marginalize_resident_culled(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg,
                                        const icg_ba_cull_window *culled, const uint8_t *const *node_in_map, icg_ba_prior *out);
 /*
