@@ -4,6 +4,7 @@ GVINS::gvinsOptimization (solve N/4 -> chi-square culling -> solve N - N/4).  Al
 """
 from __future__ import annotations
 
+import copy
 import ctypes as C
 
 import numpy as np
@@ -163,6 +164,64 @@ def merge_cull_shard(full: dict, shard: dict, shard_out: dict) -> None:
     for k in ("lm_pw", "lm_depth", "lm_outlier"):
         full[k][lo:hi] = shard_out[k]
     full["obs_outlier"][off[lo]:off[hi]] = shard_out["obs_outlier"]
+
+
+def shard_next(nxt: dict, carry: dict, prev_shards, new_rank):
+    """Per-rank shard slides from a whole-window slide.  nxt / carry: the next whole window and its whole-window carry maps (lm_src and f_src
+    name rows of the old whole window); prev_shards: the old window's shards in rank order, with lm_lo / lm_hi / f_index as shard_window gives
+    them; new_rank[l] (L entries): the rank of next landmark l where lm_src[l] < 0, -1 or the old rank where it is carried.  A carried
+    landmark stays on the rank that held it (ValueError when new_rank names another).  Returns (the next whole window reordered
+    rank-major -- each rank's landmarks contiguous, in next's order within the rank, factors landmark by landmark --, its carry maps,
+    [(shard, shard-local carry)] per rank), each shard with lm_lo / lm_hi / f_index into the reordered window, so that shard_cull_inputs
+    and merge_cull_shard keep working.  Every shard owns its arrays: a call that writes one rank's rows in place (reintegrate() writing
+    imu_blob, a solve writing the parameters) changes no other rank's shard and not the returned whole window."""
+    world = len(prev_shards)
+    lm_src, f_src = np.asarray(carry["lm_src"]), np.asarray(carry["f_src"])
+    L = int(nxt["L"])
+    old_rank = np.full(max(1, max(int(s["lm_hi"]) for s in prev_shards)), -1, np.int64)
+    for r, s in enumerate(prev_shards):
+        old_rank[s["lm_lo"]:s["lm_hi"]] = r
+    rank = np.asarray(new_rank, np.int64).copy() if L else np.zeros(0, np.int64)
+    for l in np.nonzero(lm_src >= 0)[0]:
+        r0 = int(old_rank[lm_src[l]])
+        if int(new_rank[l]) not in (-1, r0):
+            raise ValueError(f"landmark {l} is carried from rank {r0} but assigned to rank {int(new_rank[l])}")
+        rank[l] = r0
+    if ((rank < 0) | (rank >= world)).any():
+        raise ValueError("every new landmark needs a rank in [0, world)")
+    order = np.argsort(rank, kind="stable")  # rank-major, next's order within a rank
+    new_of = np.empty(L, np.int64)
+    new_of[order] = np.arange(L)
+    f_lm = np.asarray(nxt["f_lm"], np.int64)
+    fo = np.argsort(new_of[f_lm], kind="stable")  # factors landmark by landmark, next's order within a landmark
+    whole = copy.deepcopy(nxt)
+    whole.update(invdepth=np.asarray(nxt["invdepth"], np.float64)[order].copy(), f_lm=new_of[f_lm][fo].astype(np.int32),
+                 f_ref=np.asarray(nxt["f_ref"])[fo].astype(np.int32), f_obs=np.asarray(nxt["f_obs"])[fo].astype(np.int32),
+                 f_const=np.asarray(nxt["f_const"], np.float64).reshape(-1, 14)[fo].reshape(-1).copy(),
+                 f_active=np.asarray(nxt["f_active"], np.uint8)[fo].copy())
+    wcarry = dict(carry, lm_src=lm_src[order].astype(np.int32), f_src=f_src[fo].astype(np.int32))
+    counts = np.bincount(rank, minlength=world) if L else np.zeros(world, np.int64)
+    out = []
+    for r in range(world):
+        lo = int(counts[:r].sum())
+        hi = lo + int(counts[r])
+        sel = np.nonzero((whole["f_lm"] >= lo) & (whole["f_lm"] < hi))[0]
+        sh = {k: np.array(v, copy=True) if isinstance(v, np.ndarray) else copy.deepcopy(v) for k, v in whole.items()}
+        sh.update(L=hi - lo, F=len(sel), invdepth=whole["invdepth"][lo:hi].copy(), f_lm=(whole["f_lm"][sel] - lo).astype(np.int32),
+                  f_ref=whole["f_ref"][sel].copy(), f_obs=whole["f_obs"][sel].copy(),
+                  f_const=whole["f_const"].reshape(-1, 14)[sel].reshape(-1).copy(), f_active=whole["f_active"][sel].copy(), lm_lo=lo, lm_hi=hi,
+                  f_index=sel)
+        old = prev_shards[r]
+        old_f = np.full(max(1, int(np.max(old["f_index"], initial=-1)) + 1), -1, np.int64)
+        old_f[old["f_index"]] = np.arange(len(old["f_index"]))
+        lsrc = wcarry["lm_src"][lo:hi].astype(np.int64)
+        fsrc = wcarry["f_src"][sel].astype(np.int64)
+        fl = np.where(fsrc >= 0, old_f[np.clip(fsrc, 0, len(old_f) - 1)], -1)
+        if ((fsrc >= 0) & (fl < 0)).any():
+            raise ValueError(f"rank {r}: a carried factor is not in the old shard of its landmark")
+        sc = dict(carry, lm_src=np.where(lsrc >= 0, lsrc - int(old["lm_lo"]), -1).astype(np.int32), f_src=fl.astype(np.int32))
+        out.append((sh, sc))
+    return whole, wcarry, out
 
 
 def connect_shards(solver: "WindowSolver", rank: int, world: int, transport: str, dist) -> None:
@@ -359,6 +418,14 @@ class WindowSolver:
         return outs
 
     def reintegrate(self, problems, noise5, station, imu_rows, reintegrate=None):
+        return self._reintegrate("icg_ba_reintegrate_resident", problems, noise5, station, imu_rows, reintegrate)
+
+    def shard_reintegrate(self, problems, noise5, station, imu_rows, reintegrate=None):
+        """reintegrate() on a landmark-sharded handle (icg_ba_shard_reintegrate_resident), a collective call: every rank passes its shard dicts
+        and the same IMU rows, and every rank reintegrates the same factors, bit for bit."""
+        return self._reintegrate("icg_ba_shard_reintegrate_resident", problems, noise5, station, imu_rows, reintegrate)
+
+    def _reintegrate(self, fn, problems, noise5, station, imu_rows, reintegrate=None):
         """GVINS::doReintegration (IG/ic_gvins.cc:1680-1695) on the windows this handle has just solved (icg_ba_reintegrate_resident).  noise5 =
         gyr_arw, acc_vrw, gyr_bias_std, acc_bias_std, corr_time; station = parameters_->station (the reference leaves it at (0, 0, 0));
         imu_rows[w] = the n_imu row arrays (m_k, 7) of window w's factors (None for a window left alone); reintegrate: per-window flags
@@ -391,18 +458,26 @@ class WindowSolver:
                 io[w].imu, io[w].imu_off = imu.ctypes.data_as(dp), off.ctypes.data_as(ip)
         nz = np.ascontiguousarray(noise5, np.float64)
         stn = np.ascontiguousarray(station, np.float64)
-        rc = lib().icg_ba_reintegrate_resident(self._h, n, arr, vp(nz.ctypes.data), vp(stn.ctypes.data), io)
+        rc = getattr(lib(), fn)(self._h, n, arr, vp(nz.ctypes.data), vp(stn.ctypes.data), io)
         for w, (p, o) in enumerate(zip(problems, outs)):
             o["count"] = int(io[w].count)
             if (o["status"] == 1).any():
                 p["imu_blob"].reshape(-1, IMU_BLOB)[:len(o["status"])][o["status"] == 1] = o["blobs"][o["status"] == 1]
         if rc != 0:
-            err = IcgError(f"icg_ba_reintegrate_resident failed with code {rc}: {lib().icg_last_error().decode('utf-8', 'replace')}")
+            err = IcgError(f"{fn} failed with code {rc}: {lib().icg_last_error().decode('utf-8', 'replace')}")
             err.code, err.results = rc, outs
             raise err
         return outs
 
     def slide(self, next_problems, carry, prior_from_marg=True):
+        self._slide("icg_ba_slide_resident", next_problems, carry, prior_from_marg)
+
+    def shard_slide(self, next_problems, carry, prior_from_marg=True):
+        """slide() on a landmark-sharded handle (icg_ba_shard_slide_resident), a collective call: every rank passes its next shards and their
+        shard-local carry maps (shard_next builds both); window w's prior comes from the last sharded marginalization on its owner."""
+        self._slide("icg_ba_shard_slide_resident", next_problems, carry, prior_from_marg)
+
+    def _slide(self, fn, next_problems, carry, prior_from_marg=True):
         """The next keyframe's windows from the ones this handle holds (icg_ba_slide_resident): rows whose source is carried stay on the device,
         the rest are read from `next_problems` (dicts as upload() takes them; carried value rows may be stale).  carry: one dict per window
         with int32 arrays node_src (K), lm_src (L), f_src (F), imu_src (n_imu), gnss_src (n_gnss) -- old row or -1; a missing key carries
@@ -422,10 +497,18 @@ class WindowSolver:
                 keep.append(a)
                 setattr(cw[w], k, a.ctypes.data_as(ip))
             cw[w].prior_from_marg = 1 if flags[w] else 0
-        check(lib().icg_ba_slide_resident(self._h, n, arr, cw), "icg_ba_slide_resident")
+        check(getattr(lib(), fn)(self._h, n, arr, cw), fn)
         self._keep, self._n = arr, n
 
     def slide_integrate(self, next_problems, carry, integrate, noise5, station=(0.0, 0.0, 0.0), prior_from_marg=True):
+        return self._slide_integrate("icg_ba_slide_integrate_resident", next_problems, carry, integrate, noise5, station, prior_from_marg)
+
+    def shard_slide_integrate(self, next_problems, carry, integrate, noise5, station=(0.0, 0.0, 0.0), prior_from_marg=True):
+        """slide_integrate() on a landmark-sharded handle (icg_ba_shard_slide_integrate_resident), a collective call: as shard_slide, with the
+        same `integrate` dicts on every rank; every rank integrates the same rows from its replicated states."""
+        return self._slide_integrate("icg_ba_shard_slide_integrate_resident", next_problems, carry, integrate, noise5, station, prior_from_marg)
+
+    def _slide_integrate(self, fn, next_problems, carry, integrate, noise5, station=(0.0, 0.0, 0.0), prior_from_marg=True):
         """slide() whose new IMU factors, new node rows and aligned GNSS fixes are computed on the device from the states this handle holds
         (icg_ba_slide_integrate_resident: the host halves of addNewTimeNode, removeUnusedTimeNode and insertNewGnssTimeNode, IG/ic_gvins.cc:754-928).
         Only rows that `carry` leaves to next_problems are read.  integrate: one dict per window (None: nothing integrated) with
@@ -483,9 +566,9 @@ class WindowSolver:
                 iw[w].gnss_node, iw[w].gnss_dt = arg(g["gnss_node"], np.int32, ip), arg(g["gnss_dt"], np.float64, dp)
         nz = np.ascontiguousarray(noise5, np.float64)
         stn = np.ascontiguousarray(station, np.float64)
-        rc = lib().icg_ba_slide_integrate_resident(self._h, n, arr, cw, iw, vp(nz.ctypes.data), vp(stn.ctypes.data))
+        rc = getattr(lib(), fn)(self._h, n, arr, cw, iw, vp(nz.ctypes.data), vp(stn.ctypes.data))
         if rc != 0:
-            err = IcgError(f"icg_ba_slide_integrate_resident failed with code {rc}: {lib().icg_last_error().decode('utf-8', 'replace')}")
+            err = IcgError(f"{fn} failed with code {rc}: {lib().icg_last_error().decode('utf-8', 'replace')}")
             err.code, err.results = rc, outs
             raise err
         self._keep, self._n = arr, n

@@ -1818,8 +1818,11 @@ struct icg_ba {
     unsigned char *reint_h = nullptr, *reint_d = nullptr;
     size_t reint_cap = 0;
     // the last resident marginalization, while its workspace (marg_oJ0 / marg_oe0) is the prior of the windows the handle holds: its window
-    // count (0: none; an upload, a slide or another marginalization clears it) and every window's m, r and number of remained blocks
+    // count (0: none; an upload, a slide or another marginalization clears it) and every window's m, r and number of remained blocks.
+    // marg_res_sharded: it was the sharded resident marginalization of a shard group; the prior of window w is then in the workspace of mx_h
+    // (slot (w - rank) / world) on its owner, and m = r = nblocks = 0 is kept for the windows another rank owns
     int marg_res_n = 0;
+    bool marg_res_sharded = false;
     std::vector<int> marg_res_m, marg_res_r, marg_res_nb;
     // icg_ba_slide_resident: pinned staging and its device twin (grown on demand), the copy of the old value rows, the second f_const_s buffer
     unsigned char *slide_h = nullptr, *slide_d = nullptr;
@@ -2509,6 +2512,8 @@ static int preload_group_kernels() {
     cudaFuncAttributes a;
     for (const void *f : k) ICG_CUDA(cudaFuncGetAttributes(&a, f));
     ICG_CUDA(preload_update_cull());
+    ICG_CUDA(preload_slide());
+    ICG_CUDA(preload_preint_resident());
     return ICG_OK;
 }
 
@@ -3103,7 +3108,7 @@ static int marginalize_body(icg_ba *h, int n_windows, const icg_ba_problem *prob
     if (resident) {  // icg_ba_slide_resident(prior_from_marg = 1) takes this prior from the workspace
         h->marg_res_m.resize(n), h->marg_res_r.resize(n), h->marg_res_nb.resize(n);
         for (int w = 0; w < n; w++) h->marg_res_m[w] = out[w].m, h->marg_res_r[w] = out[w].r, h->marg_res_nb[w] = out[w].nblocks;
-        h->marg_res_n = n;
+        h->marg_res_n = n, h->marg_res_sharded = false;
     }
     return ICG_OK;
 }
@@ -3143,8 +3148,8 @@ static int shard_xsum(icg_ba *h, int *v, int stride, int n, int nv, int op) {
     return ICG_OK;
 }
 
-// the group's maxima of three host integers
-static int shard_xmax(icg_ba *h, int *v3) {
+// the group's maxima of three host integers (fn: the calling entry point, for the timeout's message)
+static int shard_xmax(icg_ba *h, int *v3, const char *fn) {
     int rc = hd_reserve(h, h->xs_v, 8);
     if (rc != ICG_OK) return rc;
     memcpy(h->xs_v.h, v3, 3 * sizeof(int));
@@ -3153,9 +3158,46 @@ static int shard_xmax(icg_ba *h, int *v3) {
     if (rc != ICG_OK) return rc;
     ICG_CUDA(h->xs_v.down(h->stream, 3));
     ICG_CUDA(cudaStreamSynchronize(h->stream));
-    rc = shard_timed_out(h, "icg_ba_marginalize_resident");
+    rc = shard_timed_out(h, fn);
     if (rc != ICG_OK) return rc;
     memcpy(v3, h->xs_v.h, 3 * sizeof(int));
+    return ICG_OK;
+}
+
+// 31-bit fingerprint of the arguments a collective call requires to be the same on every rank (FNV-1a over 64-bit words)
+extern "C++" {
+struct ArgPrint {
+    uint64_t v = 1469598103934665603ull;
+    void bytes(const void *p, size_t n) {
+        const unsigned char *c = (const unsigned char *) p;
+        size_t i = 0;
+        for (uint64_t x; i + 8 <= n; i += 8) memcpy(&x, c + i, 8), v = (v ^ x) * 1099511628211ull;
+        for (; i < n; i++) v = (v ^ c[i]) * 1099511628211ull;
+    }
+    template <typename T>
+    void arr(const T *p, long long count) {
+        if (p && count > 0) bytes(p, sizeof(T) * (size_t) count);
+    }
+    void num(long long x) { bytes(&x, sizeof(x)); }
+    int get() const { return (int) ((v ^ (v >> 31) ^ (v >> 62)) & 0x7fffffff); }
+};
+}
+
+// The agreement of a collective call before any rank writes its device: one exchange of (rejecting rank + 1, +fp, -fp).  ICG_OK when no rank
+// rejected and every rank passed the same fingerprint fp; otherwise ICG_EINVAL on every rank (a rejecting rank keeps its own message).
+static int shard_agree(icg_ba *h, bool rejected, int fp, const char *fn) {
+    int mx[3] = {rejected ? h->D.rank + 1 : 0, rejected ? 0 : fp, rejected ? 0 : -fp};
+    const int rc = shard_xmax(h, mx, fn);
+    if (rc != ICG_OK || rejected) return rc != ICG_OK ? rc : ICG_EINVAL;
+    if (mx[0]) {
+        set_error("%s: rank %d of the shard group rejected the call (see that rank's error); no rank changed its handle", fn, mx[0] - 1);
+        return ICG_EINVAL;
+    }
+    if (mx[1] != -mx[2]) {
+        set_error("%s: the ranks' camera sides differ (node, IMU and GNSS rows and maps, the prior's source and the integration's inputs must be "
+                  "the same on every rank); no rank changed its handle", fn);
+        return ICG_EINVAL;
+    }
     return ICG_OK;
 }
 
@@ -3275,16 +3317,24 @@ static int marginalize_sharded(icg_ba *h, int n, const icg_ba_problem *problems,
     count_launch();
     for (int w = 0; w < n; w++)
         if (w % G != R) out[w].m = out[w].r = out[w].nblocks = 0;
-    h->marg_res_n = 0;  // the sharded slide is not available: no resident prior is kept
+    h->marg_res_n = 0;  // the workspace is about to be overwritten: the sharded slide's prior again only if this call succeeds
+    // on success: the record icg_ba_shard_slide[_integrate]_resident checks (every rank: a sharded resident marginalization of these n
+    // windows; the owner: each owned window's m, r, nblocks)
+    auto record = [&]() {
+        h->marg_res_m.assign(n, 0), h->marg_res_r.assign(n, 0), h->marg_res_nb.assign(n, 0);
+        for (int w = R; w < n; w += G) h->marg_res_m[w] = out[w].m, h->marg_res_r[w] = out[w].r, h->marg_res_nb[w] = out[w].nblocks;
+        h->marg_res_n = n, h->marg_res_sharded = true;
+        return ICG_OK;
+    };
     if (n_own == 0) {
         int mx[3] = {0, 0, 0};
-        rc = shard_xmax(h, mx);
+        rc = shard_xmax(h, mx, fn);
         if (rc != ICG_OK) return rc;
         if (mx[2]) {
             set_error("%s: a window owned by another rank of the shard group was rejected (see that rank's error)", fn);
             return ICG_EUNSUPPORTED;
         }
-        return ICG_OK;
+        return record();
     }
     ICG_CUDA(cudaStreamSynchronize(s));
     if ((rc = shard_timed_out(h, fn)) != ICG_OK) return rc;
@@ -3306,7 +3356,7 @@ static int marginalize_sharded(icg_ba *h, int n, const icg_ba_problem *problems,
                 if (ref >= num_marg[w] || obs >= p.K) {
                     set_error("%s: window %d: gathered factor %d names nodes %d / %d (the ranks' windows differ)", fn, w, i, ref, obs);
                     int mx[3] = {0, 0, 1};
-                    shard_xmax(h, mx);
+                    shard_xmax(h, mx, fn);
                     return ICG_EINVAL;
                 }
                 g_lm[j][i] = L - 1, g_ref[j][i] = ref, g_obs[j][i] = obs, g_act[j][i] = (uint8_t) ((hi >> 16) & 1);
@@ -3330,7 +3380,7 @@ static int marginalize_sharded(icg_ba *h, int n, const icg_ba_problem *problems,
         if (rc != ICG_OK) {
             mh = nullptr;
             int mx[3] = {0, 0, 1};
-            shard_xmax(h, mx);
+            shard_xmax(h, mx, fn);
             return rc;
         }
     }
@@ -3347,16 +3397,16 @@ static int marginalize_sharded(icg_ba *h, int n, const icg_ba_problem *problems,
         count_launch();
     } else {
         int mx[3] = {0, 0, 1};
-        shard_xmax(h, mx);
+        shard_xmax(h, mx, fn);
         return rc;
     }
     std::vector<int32_t> nm(n_own);
     std::vector<icg_ba_prior> po(n_own);
     for (int j = 0; j < n_own; j++) nm[j] = num_marg[R + j * G], po[j] = out[R + j * G];
-    const std::function<int(int *)> agree = [h](int *mx) { return shard_xmax(h, mx); };
+    const std::function<int(int *)> agree = [h, fn](int *mx) { return shard_xmax(h, mx, fn); };
     rc = marginalize_body(mh, n_own, gp.data(), nm.data(), po.data(), true, nullptr, &agree);
     for (int j = 0; j < n_own; j++) out[R + j * G].m = po[j].m, out[R + j * G].r = po[j].r, out[R + j * G].nblocks = po[j].nblocks;
-    return rc;
+    return rc == ICG_OK ? record() : rc;
 }
 
 int icg_ba_marginalize_resident(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg, icg_ba_prior *out) {
@@ -3370,8 +3420,8 @@ static int resident_single_rank(icg_ba *h, int n_windows, const icg_ba_problem *
         set_error("%s: bad arguments", what);
         return ICG_EINVAL;
     }
-    if (h->D.world > 1 && !sharded_ok) {
-        set_error("%s: not available on a landmark-sharded handle (icg_ba_shard_leave first)", what);
+    if (h->D.world > 1 && !sharded_ok) {  // the reintegration and the slides: their collective forms are icg_ba_shard_*
+        set_error("%s: not available on a landmark-sharded handle (the group calls icg_ba_shard_%s; or icg_ba_shard_leave first)", what, what + 7);
         return ICG_EUNSUPPORTED;
     }
     if (h->cur_windows != n_windows) {
@@ -3503,47 +3553,68 @@ int icg_ba_update_and_cull_resident(icg_ba *h, int n_windows, const icg_ba_probl
 }
 
 // ---- doReintegration (IG/ic_gvins.cc:1680-1695) on the resident IMU factors (preint.cu)
-int icg_ba_reintegrate_resident(icg_ba *h, int n_windows, const icg_ba_problem *problems, const double *noise5, const double *station3,
-                                icg_ba_reint_window *io) {
-    int rc = resident_single_rank(h, n_windows, problems, "icg_ba_reintegrate_resident");
-    if (rc != ICG_OK) return rc;
-    if (!noise5 || !station3 || !io) {
-        set_error("icg_ba_reintegrate_resident: bad arguments");
-        return ICG_EINVAL;
-    }
-    const BaCaps &C = h->C;
+// sharded (icg_ba_shard_reintegrate_resident): every rank runs the same reintegration on its replicated states, after the group agreed
+static int reint_body(icg_ba *h, int n_windows, const icg_ba_problem *problems, const double *noise5, const double *station3, icg_ba_reint_window *io,
+                      const char *fn, bool sharded) {
     const int n = n_windows;
     // validation first: nothing is launched on bad input
     size_t n_items = 0, n_rows = 0;
-    for (int w = 0; w < n; w++) {
-        const icg_ba_problem &p = problems[w];
-        const icg_ba_reint_window &c = io[w];
-        if (p.K < 2 || p.K > C.K || p.n_imu < 0 || p.n_imu > p.K - 1) {
-            set_error("icg_ba_reintegrate_resident: window %d: sizes out of range", w);
+    auto validate = [&]() -> int {
+        int rc = resident_single_rank(h, n_windows, problems, fn, sharded);
+        if (rc != ICG_OK) return rc;
+        if (!noise5 || !station3 || !io) {
+            set_error("%s: bad arguments", fn);
             return ICG_EINVAL;
         }
-        if (!c.reintegrate || p.n_imu == 0) continue;
-        if (!c.imu || !c.imu_off || !c.status || !c.blob_out) {
-            set_error("icg_ba_reintegrate_resident: window %d: arrays missing", w);
-            return ICG_EINVAL;
-        }
-        if (c.imu_off[0] < 0) {
-            set_error("icg_ba_reintegrate_resident: window %d: imu_off[0] is negative", w);
-            return ICG_EINVAL;
-        }
-        for (int k = 0; k < p.n_imu; k++)
-            if (c.imu_off[k + 1] - c.imu_off[k] < 1) {
-                set_error("icg_ba_reintegrate_resident: window %d factor %d: imu_off must give every interval at least one row", w, k);
+        for (int w = 0; w < n; w++) {
+            const icg_ba_problem &p = problems[w];
+            const icg_ba_reint_window &c = io[w];
+            if (p.K < 2 || p.K > h->C.K || p.n_imu < 0 || p.n_imu > p.K - 1) {
+                set_error("%s: window %d: sizes out of range", fn, w);
                 return ICG_EINVAL;
             }
-        n_items += p.n_imu, n_rows += (size_t) (c.imu_off[p.n_imu] - c.imu_off[0]);
+            if (!c.reintegrate || p.n_imu == 0) continue;
+            if (!c.imu || !c.imu_off || !c.status || !c.blob_out) {
+                set_error("%s: window %d: arrays missing", fn, w);
+                return ICG_EINVAL;
+            }
+            if (c.imu_off[0] < 0) {
+                set_error("%s: window %d: imu_off[0] is negative", fn, w);
+                return ICG_EINVAL;
+            }
+            for (int k = 0; k < p.n_imu; k++)
+                if (c.imu_off[k + 1] - c.imu_off[k] < 1) {
+                    set_error("%s: window %d factor %d: imu_off must give every interval at least one row", fn, w, k);
+                    return ICG_EINVAL;
+                }
+            n_items += p.n_imu, n_rows += (size_t) (c.imu_off[p.n_imu] - c.imu_off[0]);
+        }
+        if (n_items > INT32_MAX / 8 || n_rows > INT32_MAX / 8) {
+            set_error("%s: too many factors or IMU rows in one call", fn);
+            return ICG_EINVAL;
+        }
+        return ICG_OK;
+    };
+    int rc = validate();
+    if (sharded) {  // every argument is camera side: the sizes, the flags, the rows, noise and station
+        ArgPrint fp;
+        fp.num(n);
+        for (int w = 0; rc == ICG_OK && w < n; w++) {
+            const icg_ba_problem &p = problems[w];
+            const icg_ba_reint_window &c = io[w];
+            const bool on = c.reintegrate && p.n_imu > 0;
+            fp.num(p.K), fp.num(p.n_imu), fp.num(on);
+            if (!on) continue;
+            fp.arr(c.imu_off, p.n_imu + 1);
+            fp.arr(c.imu + 7 * (size_t) c.imu_off[0], 7LL * (c.imu_off[p.n_imu] - c.imu_off[0]));
+        }
+        if (rc == ICG_OK) fp.arr(noise5, 5), fp.arr(station3, 3);
+        rc = shard_agree(h, rc != ICG_OK, fp.get(), fn);
     }
+    if (rc != ICG_OK) return rc;
+    const BaCaps &C = h->C;
     for (int w = 0; w < n; w++) io[w].count = 0;
     if (n_items == 0) return ICG_OK;
-    if (n_items > INT32_MAX / 8 || n_rows > INT32_MAX / 8) {
-        set_error("icg_ba_reintegrate_resident: too many factors or IMU rows in one call");
-        return ICG_EINVAL;
-    }
     // staging: inputs [items | rows | counter (0)] go up in one copy; [counter | status | ends | out_item] come back in one copy, then the
     // status-1 blobs, compacted on the device
     auto al = [](size_t b) { return (b + 15) & ~(size_t) 15; };
@@ -3559,12 +3630,12 @@ int icg_ba_reintegrate_resident(icg_ba *h, int n_windows, const icg_ba_problem *
     cudaStream_t s = h->stream;
     if (at > h->reint_cap) {
         ICG_CUDA(cudaStreamSynchronize(s));
-        if (h->reint_h) cudaFreeHost(h->reint_h), h->reint_h = nullptr;
-        if (h->reint_d) cudaFree(h->reint_d), h->reint_d = nullptr;
+        retire(h, h->reint_d, h->reint_h);  // a shard group keeps it: freeing would wait for a peer's kernel
+        h->reint_h = nullptr, h->reint_d = nullptr;
         h->reint_cap = 0;
         const size_t cap = at + at / 4;
         if (cudaMallocHost(&h->reint_h, cap) != cudaSuccess || cudaMalloc(&h->reint_d, cap) != cudaSuccess) {
-            set_error("icg_ba_reintegrate_resident: staging allocation of %zu bytes failed", cap);
+            set_error("%s: staging allocation of %zu bytes failed", fn, cap);
             return ICG_ENOMEM;
         }
         h->reint_cap = cap;
@@ -3601,7 +3672,7 @@ int icg_ba_reintegrate_resident(icg_ba *h, int n_windows, const icg_ba_problem *
     ICG_CUDA(cudaStreamSynchronize(s));
     const int n_done = *(const int *) (H + o_cnt);
     if (n_done < 0 || (size_t) n_done > n_items) {
-        set_error("icg_ba_reintegrate_resident: inconsistent completion count %d", n_done);
+        set_error("%s: inconsistent completion count %d", fn, n_done);
         return ICG_ECUDA;
     }
     if (n_done > 0) {
@@ -3630,11 +3701,35 @@ int icg_ba_reintegrate_resident(icg_ba *h, int n_windows, const icg_ba_problem *
         }
     }
     if (bad_w >= 0) {
-        set_error("icg_ba_reintegrate_resident: window %d IMU factor %d: the reintegrated covariance is not positive definite (the factor was kept)", bad_w,
-                  bad_k);
+        set_error("%s: window %d IMU factor %d: the reintegrated covariance is not positive definite (the factor was kept)", fn, bad_w, bad_k);
         return ICG_EINVAL;
     }
     return ICG_OK;
+}
+
+int icg_ba_reintegrate_resident(icg_ba *h, int n_windows, const icg_ba_problem *problems, const double *noise5, const double *station3,
+                                icg_ba_reint_window *io) {
+    return reint_body(h, n_windows, problems, noise5, station3, io, "icg_ba_reintegrate_resident", false);
+}
+
+// a collective call of a shard group: the entry points below take the sharded form of their plain counterpart's body
+static int shard_group_only(icg_ba *h, const char *fn, const char *plain) {
+    if (!h) {
+        set_error("%s: bad arguments", fn);
+        return ICG_EINVAL;
+    }
+    if (h->D.world < 2) {
+        set_error("%s: the handle is not in a landmark-shard group (call %s)", fn, plain);
+        return ICG_EINVAL;
+    }
+    return ICG_OK;
+}
+
+int icg_ba_shard_reintegrate_resident(icg_ba *h, int n_windows, const icg_ba_problem *problems, const double *noise5, const double *station3,
+                                      icg_ba_reint_window *io) {
+    const char *fn = "icg_ba_shard_reintegrate_resident";
+    const int rc = shard_group_only(h, fn, "icg_ba_reintegrate_resident");
+    return rc != ICG_OK ? rc : reint_body(h, n_windows, problems, noise5, station3, io, fn, true);
 }
 
 int icg_ba_marginalize_resident_culled(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg,
@@ -3684,29 +3779,65 @@ int icg_ba_marginalize_resident_culled(icg_ba *h, int n_windows, const icg_ba_pr
 // ---- the next keyframe's windows from the resident ones (ba_slide.cu): the structure is packed on the host as icg_ba_upload packs it, the
 //      values of the carried rows never leave the device.  With `integ`, the new factors, node rows and aligned fixes it names are computed on
 //      the device (preint.cu) into the staged value rows before the gather reads them.
+//
+// sharded (icg_ba_shard_slide[_integrate]_resident, a collective call): the same checks, plus landmark-by-landmark factor lists and the owner's
+// check of its own prior; then one agreement of the group (shard_agree: every rank's verdict and a fingerprint of the camera side) before any
+// rank writes its device, and with `integ` a second one on the integration's outcome.  A rank that rejects joins the agreement all the same
+// (fail below), so its peers never wait for it.  The owner of window w forms its prior from the workspace of mx_h; the other ranks get zeros.
 static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba_slide_window *carry, const icg_ba_slide_integrate *integ,
-                      const double *noise5, const double *station3, const char *fn) {
-    int rc = resident_single_rank(h, n, next, fn);
-    if (rc != ICG_OK) return rc;
+                      const double *noise5, const double *station3, const char *fn, bool sharded) {
+    bool joined = false;  // sharded: this rank has joined the agreement of the call
+    std::vector<WinDims> old_dims;
+    std::vector<std::vector<int>> old_slot;
+    // a rejected call leaves the handle as it was: the packing below rewrites the host tables later calls read (dims, which restore_params
+    // uploads, and the slot table of the next slide), so they go back on failure; nothing reaches the device before every check has passed
+    auto fail = [&](int code) {
+        if (!old_dims.empty()) {
+            memcpy(h->dims.h, old_dims.data(), sizeof(WinDims) * n);
+            for (int w = 0; w < n; w++) {
+                int *fidx = h->lm_fidx.h + (size_t) w * h->C.F;
+                for (int f = 0; f < old_dims[w].F; f++) fidx[old_slot[w][f]] = f;
+            }
+        }
+        // sharded: a rank that rejects before the agreement joins it with its rejection, and returns ICG_EINVAL as its peers do (its own
+        // message says why); only a failed exchange (a peer did not make the call) returns that error instead
+        if (sharded && !joined) joined = true, code = shard_agree(h, true, 0, fn);
+        return code;
+    };
+    // a CUDA error before the agreement is this rank's rejection like any other
+    auto cuda_fail = [&](cudaError_t e, const char *what) {
+        set_error("%s: %s failed: %s", fn, what, cudaGetErrorString(e));
+        return fail(ICG_ECUDA);
+    };
+    int rc = resident_single_rank(h, n, next, fn, sharded);
+    if (rc != ICG_OK) return fail(rc);
     if (!carry || (integ && (!noise5 || !station3))) {
         set_error("%s: bad arguments", fn);
-        return ICG_EINVAL;
+        return fail(ICG_EINVAL);
     }
-    ICG_CUDA(cudaSetDevice(h->device));
+    if (cudaError_t e = cudaSetDevice(h->device)) return cuda_fail(e, "cudaSetDevice");
     const BaCaps &C = h->C;
     const size_t NW = C.NW;
+    const int G = h->D.world, R = h->D.rank;
     for (int w = 0; w < n; w++) {
         const icg_ba_problem &p = next[w];
+        if (sharded)
+            for (int f = 1; p.f_lm && f < p.F; f++)
+                if (p.f_lm[f] < p.f_lm[f - 1]) {
+                    set_error("%s: window %d factor %d: a landmark-sharded window must list its factors landmark by landmark (f_lm non-decreasing)", fn, w, f);
+                    return fail(ICG_EINVAL);
+                }
         if (!carry[w].prior_from_marg) continue;
-        if (h->marg_res_n != n) {
-            set_error("%s: window %d takes its prior from the marginalization, but no resident marginalization of these %d windows "
-                      "ran since the last upload or slide", fn, w, n);
-            return ICG_EINVAL;
+        if (h->marg_res_n != n || h->marg_res_sharded != sharded) {
+            set_error("%s: window %d takes its prior from the marginalization, but no %sresident marginalization of these %d windows "
+                      "ran since the last upload or slide", fn, w, sharded ? "sharded " : "", n);
+            return fail(ICG_EINVAL);
         }
+        if (sharded && w % G != R) continue;  // the owner holds the window's m, r and nblocks
         if (h->marg_res_m[w] <= 0 || p.marg_r != h->marg_res_r[w] || p.marg_nblocks != h->marg_res_nb[w]) {
             set_error("%s: window %d: marg_r=%d / marg_nblocks=%d, but the resident marginalization left m=%d, r=%d / nblocks=%d", fn, w,
                       p.marg_r, p.marg_nblocks, h->marg_res_m[w], h->marg_res_r[w], h->marg_res_nb[w]);
-            return ICG_EINVAL;
+            return fail(ICG_EINVAL);
         }
     }
     // the device buffers of the first slide: the old value rows at the handle's strides, the second f_const_s
@@ -3716,26 +3847,16 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
                           cudaMalloc(&h->fc_alt, sizeof(double) * NW * C.F * 14) != cudaSuccess)) {
         if (h->slide_old) cudaFree(h->slide_old), h->slide_old = nullptr;
         set_error("%s: allocation of the slide buffers failed", fn);
-        return ICG_ENOMEM;
+        return fail(ICG_ENOMEM);
     }
     // the old windows: sizes, and every factor's record slot (the inverse of the last packing's slot -> factor table)
-    std::vector<WinDims> old_dims(h->dims.h, h->dims.h + n);
-    std::vector<std::vector<int>> old_slot(n);
+    old_dims.assign(h->dims.h, h->dims.h + n);
+    old_slot.resize(n);
     for (int w = 0; w < n; w++) {
         old_slot[w].resize(old_dims[w].F);
         const int *fidx = h->lm_fidx.h + (size_t) w * C.F;
         for (int q = 0; q < old_dims[w].F; q++) old_slot[w][fidx[q]] = q;
     }
-    // a rejected call leaves the handle as it was: the packing below rewrites the host tables later calls read (dims, which restore_params
-    // uploads, and the slot table of the next slide), so they go back on failure; nothing reaches the device before every check has passed
-    auto fail = [&](int code) {
-        memcpy(h->dims.h, old_dims.data(), sizeof(WinDims) * n);
-        for (int w = 0; w < n; w++) {
-            int *fidx = h->lm_fidx.h + (size_t) w * C.F;
-            for (int f = 0; f < old_dims[w].F; f++) fidx[old_slot[w][f]] = f;
-        }
-        return code;
-    };
     rc = pack_windows(h, n, next, false);
     if (rc != ICG_OK) return fail(rc);
     // the maps: range checks, sizes of the staging
@@ -3767,6 +3888,7 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
         W.node_map = (int) n_map, W.lm_map = W.node_map + p.K, W.slot_map = W.lm_map + p.L, W.imu_map = W.slot_map + p.F, W.gnss_map = W.imu_map + p.n_imu;
         n_map = (size_t) W.gnss_map + p.n_gnss;
         W.r = p.marg_r, W.from_marg = c.prior_from_marg != 0, W.j0 = W.e0 = 0;
+        W.slot = !sharded ? w : w % G == R ? (w - R) / G : -1;
         if (W.r > 0 && !W.from_marg) n_val += (size_t) W.r * W.r + W.r;
         max_elems = std::max(max_elems, SLIDE_NODE * p.K + p.L + 14 * p.F + SLIDE_IMU * p.n_imu + SLIDE_GNSS * p.n_gnss);
         max_r = std::max(max_r, W.r);
@@ -3860,9 +3982,9 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
     }
     cudaStream_t s = h->stream;
     if (total > h->slide_cap) {
-        ICG_CUDA(cudaStreamSynchronize(s));  // an earlier slide's copy may still read the old buffer
-        if (h->slide_h) cudaFreeHost(h->slide_h), h->slide_h = nullptr;
-        if (h->slide_d) cudaFree(h->slide_d), h->slide_d = nullptr;
+        if (cudaError_t e = cudaStreamSynchronize(s)) return cuda_fail(e, "cudaStreamSynchronize");  // an earlier slide's copy may read the old buffer
+        retire(h, h->slide_d, h->slide_h);    // a shard group keeps it: freeing would wait for a peer's kernel
+        h->slide_h = nullptr, h->slide_d = nullptr;
         h->slide_cap = 0;
         const size_t cap = total + total / 4;
         if (cudaMallocHost(&h->slide_h, cap) != cudaSuccess || cudaMalloc(&h->slide_d, cap) != cudaSuccess) {
@@ -3871,9 +3993,11 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
         }
         h->slide_cap = cap;
     } else if (h->slide_ev) {
-        ICG_CUDA(cudaEventSynchronize(h->slide_ev));  // the previous slide's H2D has left the pinned buffer before it is rewritten
+        // the previous slide's H2D has left the pinned buffer before it is rewritten
+        if (cudaError_t e = cudaEventSynchronize(h->slide_ev)) return cuda_fail(e, "cudaEventSynchronize");
     }
-    if (!h->slide_ev) ICG_CUDA(cudaEventCreateWithFlags(&h->slide_ev, cudaEventDisableTiming));
+    if (!h->slide_ev)
+        if (cudaError_t e = cudaEventCreateWithFlags(&h->slide_ev, cudaEventDisableTiming)) return cuda_fail(e, "cudaEventCreateWithFlags");
     int *map = (int *) (h->slide_h + b_map);
     double *val = (double *) (h->slide_h + b_val);
     SlideItem *items = (SlideItem *) (h->slide_h + b_item);
@@ -3977,9 +4101,58 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
                 return fail(rcs[t]);
             }
     }
+    if (sharded) {
+        ArgPrint fp;
+        fp.num(n);
+        if (integ) fp.arr(noise5, 5), fp.arr(station3, 3);
+        for (int w = 0; w < n; w++) {
+            const icg_ba_problem &p = next[w];
+            const icg_ba_slide_window &c = carry[w];
+            const icg_ba_slide_integrate *g = integ ? &integ[w] : nullptr;
+            fp.num(p.K), fp.num(p.n_imu), fp.num(p.n_gnss), fp.num(c.prior_from_marg), fp.num(p.marg_r), fp.num(p.marg_nblocks);
+            // the flags and camera-side values the structure packing reads from next
+            fp.arr(p.ext, 8), fp.num(p.ext_const), fp.num(p.td_const), fp.arr(&p.reproj_std, 1), fp.num(p.reproj_huber), fp.num(p.gnss_huber);
+            fp.num(p.has_imu_error), fp.arr(p.lever, 3), fp.num(p.has_pose_prior), fp.num(p.has_mix_prior);
+            if (p.has_pose_prior) fp.arr(p.pose_prior, 7), fp.arr(p.pose_prior_std, 6);
+            if (p.has_mix_prior) fp.arr(p.mix_prior, 9), fp.arr(p.mix_prior_std, 9);
+            fp.num(!c.node_src), fp.num(!c.imu_src), fp.num(!c.gnss_src);
+            fp.arr(c.node_src, p.K), fp.arr(c.imu_src, p.n_imu), fp.arr(c.gnss_src, p.n_gnss), fp.arr(p.gnss_node, p.n_gnss);
+            for (int k = 0; k < p.K; k++) {
+                if (c.node_src && c.node_src[k] >= 0) continue;
+                if (g && g->node_from_imu && g->node_from_imu[k]) fp.num(-1);
+                else fp.arr(p.pose + 7 * (size_t) k, 7), fp.arr(p.mix + 9 * (size_t) k, 9);
+            }
+            for (int k = 0; k < p.n_imu; k++) {
+                if (c.imu_src && c.imu_src[k] >= 0) continue;
+                const int q = g ? item_of[w][k] : -1;
+                if (q < 0) {
+                    fp.arr(p.imu_blob + (size_t) k * ICG_IMU_BLOB_DOUBLES, ICG_IMU_BLOB_DOUBLES);
+                    continue;
+                }
+                fp.num(g->imu_from[k]), fp.arr(g->gravity3 + 3 * (size_t) k, 3), fp.num(g->normal && g->normal[k]);
+                fp.arr(g->imu + 7 * (size_t) g->imu_off[k], 7LL * (g->imu_off[k + 1] - g->imu_off[k]));
+                if (g->imu_from[k] == ICG_SLIDE_ROW) fp.arr(g->state16 + 16 * (size_t) k, 16);
+            }
+            for (int q = 0; q < p.n_gnss; q++) {
+                if (c.gnss_src && c.gnss_src[q] >= 0) continue;
+                fp.arr(p.gnss_blh + 3 * (size_t) q, 3), fp.arr(p.gnss_std + 3 * (size_t) q, 3);
+                if (g && g->gnss_node) fp.num(g->gnss_node[q]), fp.arr(g->gnss_node[q] >= 0 ? g->gnss_dt + q : nullptr, 1);
+            }
+            if (p.marg_r > 0) {
+                long long nx = 0;
+                for (int b = 0; p.marg_block_type && b < p.marg_nblocks; b++) nx += p.marg_block_type[b] == 1 ? 9 : p.marg_block_type[b] == 3 ? 1 : 7;
+                fp.arr(p.marg_block_type, p.marg_nblocks), fp.arr(p.marg_block_node, p.marg_nblocks), fp.arr(p.marg_x0, nx);
+                if (!c.prior_from_marg) fp.arr(p.marg_J0, (long long) p.marg_r * p.marg_r), fp.arr(p.marg_e0, p.marg_r);
+            }
+        }
+        joined = true;
+        if ((rc = shard_agree(h, false, fp.get(), fn)) != ICG_OK) return fail(rc);
+    }
     memcpy(h->slide_h, wins.data(), sizeof(SlideWin) * n);
     if (integ) {
-        // the device work writes the staging only; a covariance that is not positive definite is known after it, so the call waits for it
+        // the device work writes the staging only; a covariance that is not positive definite is known after it, so the call waits for it.
+        // Sharded: the ranks integrate the same rows from the same states; the outcome is agreed on all the same before the device is written
+        int irc = ICG_OK;
         if (!iwins.empty()) {
             memcpy(h->slide_h + b_iw, iwins.data(), sizeof(SlideIntWin) * iwins.size());
             PreintSlide a;
@@ -3996,14 +4169,14 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
             if (e == cudaSuccess) e = cudaStreamSynchronize(s);
             if (e != cudaSuccess) {
                 set_error("%s: the integration on the device failed: %s", fn, cudaGetErrorString(e));
-                return fail(ICG_ECUDA);
+                irc = ICG_ECUDA;
             }
             count_launch();
         }
         const int8_t *st = (const int8_t *) (h->slide_h + b_status);
         const double *ends = (const double *) (h->slide_h + b_ends), *blobs = (const double *) (h->slide_h + b_blob);
         int bad_w = -1, bad_k = -1;
-        for (int w = 0; w < n; w++) {
+        for (int w = 0; irc == ICG_OK && w < n; w++) {
             const icg_ba_slide_integrate &g = integ[w];
             for (int k = 0; k < next[w].n_imu; k++) {
                 const int q = item_of[w][k];
@@ -4016,8 +4189,10 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
         }
         if (bad_w >= 0) {
             set_error("%s: window %d IMU factor %d: the integrated covariance is not positive definite", fn, bad_w, bad_k);
-            return fail(ICG_EINVAL);
+            irc = ICG_EINVAL;
         }
+        if (sharded) irc = shard_agree(h, irc != ICG_OK, 0, fn);  // a rank's own rejection or a peer's: ICG_EINVAL on every rank
+        if (irc != ICG_OK) return fail(irc);
     }
     // every check has passed: from here on the device is written
     h->marg_res_n = 0;
@@ -4042,7 +4217,8 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
     a.old_pose = old, a.old_mix = old + o_mix, a.old_rho = old + o_rho, a.old_fc = D.f_const_s, a.old_blob = old + o_blob, a.old_U = old + o_U;
     a.old_blh = old + o_blh, a.old_std = old + o_std;
     a.pose = D.pose, a.mix = D.mix, a.rho = D.rho, a.fc = h->fc_alt, a.blob = D.imu_blob, a.U = D.imu_U, a.blh = D.gnss_blh, a.std = D.gnss_std;
-    a.mJ0 = h->M.J0, a.me0 = h->M.e0, a.mrcap = h->M.rcap;
+    const icg_ba *mw = sharded ? h->mx_h : h;  // the marginalization's workspace (sharded: the owner's gather handle; none on a rank owning no window)
+    a.mJ0 = mw ? mw->M.J0 : nullptr, a.me0 = mw ? mw->M.e0 : nullptr, a.mrcap = mw ? mw->M.rcap : 0;
     a.H0 = D.marg_H0, a.b0 = D.marg_b0, a.c0 = D.marg_c0;
     ICG_CUDA(launch_slide(a, n, max_elems, max_r, s));
     count_launch(2);
@@ -4055,7 +4231,7 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
 }
 
 int icg_ba_slide_resident(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba_slide_window *carry) {
-    return slide_body(h, n, next, carry, nullptr, nullptr, nullptr, "icg_ba_slide_resident");
+    return slide_body(h, n, next, carry, nullptr, nullptr, nullptr, "icg_ba_slide_resident", false);
 }
 
 int icg_ba_slide_integrate_resident(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba_slide_window *carry, const icg_ba_slide_integrate *integ,
@@ -4064,7 +4240,26 @@ int icg_ba_slide_integrate_resident(icg_ba *h, int n, const icg_ba_problem *next
         set_error("icg_ba_slide_integrate_resident: bad arguments");
         return ICG_EINVAL;
     }
-    return slide_body(h, n, next, carry, integ, noise5, station3, "icg_ba_slide_integrate_resident");
+    return slide_body(h, n, next, carry, integ, noise5, station3, "icg_ba_slide_integrate_resident", false);
+}
+
+int icg_ba_shard_slide_resident(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba_slide_window *carry) {
+    const char *fn = "icg_ba_shard_slide_resident";
+    const int rc = shard_group_only(h, fn, "icg_ba_slide_resident");
+    return rc != ICG_OK ? rc : slide_body(h, n, next, carry, nullptr, nullptr, nullptr, fn, true);
+}
+
+int icg_ba_shard_slide_integrate_resident(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba_slide_window *carry,
+                                          const icg_ba_slide_integrate *integ, const double *noise5, const double *station3) {
+    const char *fn = "icg_ba_shard_slide_integrate_resident";
+    int rc = shard_group_only(h, fn, "icg_ba_slide_integrate_resident");
+    if (rc != ICG_OK) return rc;
+    if (!integ) {  // still a collective call: the rank joins the agreement with its rejection
+        set_error("%s: bad arguments", fn);
+        shard_agree(h, true, 0, fn);
+        return ICG_EINVAL;
+    }
+    return slide_body(h, n, next, carry, integ, noise5, station3, fn, true);
 }
 
 // ---- landmark shards over peer memory (transport "p2p")

@@ -54,23 +54,32 @@ __global__ void __launch_bounds__(SLIDE_THREADS) ba_slide_prior(SlideArgs a) {
     if (r <= 0) return;
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e > r * r + r) return;
-    const double *J0 = W.from_marg ? a.mJ0 + (size_t) w * a.mrcap * a.mrcap : a.val + W.j0;
-    const double *e0 = W.from_marg ? a.me0 + (size_t) w * a.mrcap : a.val + W.e0;
+    // a window without a source (slot -1) sums nothing: its rows become zeros
+    const bool src = !W.from_marg || W.slot >= 0;
+    const int nk = src ? r : 0;
+    const double *J0 = !W.from_marg ? a.val + W.j0 : src ? a.mJ0 + (size_t) W.slot * a.mrcap * a.mrcap : nullptr;
+    const double *e0 = !W.from_marg ? a.val + W.e0 : src ? a.me0 + (size_t) W.slot * a.mrcap : nullptr;
     double s = 0;
     if (e < r * r) {
         const int i = e / r, j = e % r;
         if (j < i) return;
-        for (int k = 0; k < r; k++) s = __dadd_rn(s, __dmul_rn(J0[(size_t) k * r + i], J0[(size_t) k * r + j]));
+        for (int k = 0; k < nk; k++) s = __dadd_rn(s, __dmul_rn(J0[(size_t) k * r + i], J0[(size_t) k * r + j]));
         double *H0 = a.H0 + (size_t) w * a.R * a.R;
         H0[(size_t) i * r + j] = s, H0[(size_t) j * r + i] = s;
     } else if (e < r * r + r) {
         const int i = e - r * r;
-        for (int k = 0; k < r; k++) s = __dadd_rn(s, __dmul_rn(J0[(size_t) k * r + i], e0[k]));
+        for (int k = 0; k < nk; k++) s = __dadd_rn(s, __dmul_rn(J0[(size_t) k * r + i], e0[k]));
         a.b0[(size_t) w * a.R + i] = s;
     } else {
-        for (int k = 0; k < r; k++) s = __dadd_rn(s, __dmul_rn(e0[k], e0[k]));
+        for (int k = 0; k < nk; k++) s = __dadd_rn(s, __dmul_rn(e0[k], e0[k]));
         a.c0[w] = s;
     }
+}
+
+cudaError_t preload_slide() {
+    cudaFuncAttributes attr;
+    cudaError_t e = cudaFuncGetAttributes(&attr, ba_slide_gather);
+    return e == cudaSuccess ? cudaFuncGetAttributes(&attr, ba_slide_prior) : e;
 }
 
 cudaError_t launch_slide(const SlideArgs &a, int n_windows, int max_elems, int max_r, cudaStream_t stream) {

@@ -18,6 +18,7 @@ struct SlideWin {
     int node_map, lm_map, slot_map, imu_map, gnss_map;  // first entry of each map in SlideArgs::map (slot_map: by record slot)
     int r, from_marg;  // prior rows (0: none); 1: J0 / e0 from the marginalization workspace, 0: staged at j0 / e0
     int j0, e0;        // value offsets of the staged J0 (r x r row-major) and e0 (from_marg = 0)
+    int slot;          // from_marg = 1: the window's slot of the workspace, or -1: no source here (H0, b0, c0 are written as zeros)
 };
 
 struct SlideArgs {
@@ -28,7 +29,7 @@ struct SlideArgs {
     // the old window (copies of the handle's arrays at the same strides; old_fc is the f_const_s buffer the slide swaps out) -> the handle
     const double *old_pose, *old_mix, *old_rho, *old_fc, *old_blob, *old_U, *old_blh, *old_std;
     double *pose, *mix, *rho, *fc, *blob, *U, *blh, *std;
-    // prior: the marginalization workspace (J0 r x r at w mrcap^2, e0 at w mrcap) -> the handle's H0 (r x r at w R^2), b0, c0
+    // prior: the marginalization workspace (J0 r x r at slot mrcap^2, e0 at slot mrcap) -> the handle's H0 (r x r at w R^2), b0, c0
     const double *mJ0, *me0;
     int mrcap;
     double *H0, *b0, *c0;
@@ -38,5 +39,7 @@ struct SlideArgs {
 // c0 = e0.e0 of every window with a prior, in the order of icg_ba_upload's host loop.  Both on `stream`, batched over the windows; max_elems is
 // the largest window's destination doubles of the gather (16 K + L + 14 F + 705 n_imu + 6 n_gnss), max_r its largest prior.
 cudaError_t launch_slide(const SlideArgs &a, int n_windows, int max_elems, int max_r, cudaStream_t stream);
+// loads both kernels (a shard group loads every kernel its calls launch when it is set up)
+cudaError_t preload_slide();
 
 }  // namespace icg

@@ -329,4 +329,10 @@ cudaError_t preint_slide_launch(const PreintSlide &a, cudaStream_t stream) {
     return cudaGetLastError();
 }
 
+cudaError_t preload_preint_resident() {
+    cudaFuncAttributes attr;
+    cudaError_t e = cudaFuncGetAttributes(&attr, preint_resident_kernel);
+    return e == cudaSuccess ? cudaFuncGetAttributes(&attr, preint_slide_kernel) : e;
+}
+
 }  // namespace icg

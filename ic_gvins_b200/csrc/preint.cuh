@@ -75,5 +75,7 @@ struct PreintSlide {
 cudaError_t preint_batch_launch(const PreintBatch &a, cudaStream_t stream);
 cudaError_t preint_resident_launch(const PreintResident &a, cudaStream_t stream);
 cudaError_t preint_slide_launch(const PreintSlide &a, cudaStream_t stream);
+// loads the resident and slide kernels (a shard group loads every kernel its calls launch when it is set up)
+cudaError_t preload_preint_resident();
 
 }  // namespace icg

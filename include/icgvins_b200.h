@@ -614,7 +614,7 @@ int icg_ba_marginalize_resident_culled(icg_ba *h, int n_windows, const icg_ba_pr
  * (unchanged blobs do not).  Synchronous.  `problems` is the array of the solve (n_windows equal to the uploaded count; K and n_imu are
  * read).  ICG_EINVAL before anything is launched when imu_off is not increasing by at least one row per factor; ICG_EINVAL after the call,
  * naming the first such factor, when a reintegrated covariance is not positive definite (status -1: that factor is kept, every other one
- * is processed).  ICG_EUNSUPPORTED on a landmark-sharded handle.
+ * is processed).  ICG_EUNSUPPORTED on a landmark-sharded handle: its group calls icg_ba_shard_reintegrate_resident.
  */
 typedef struct icg_ba_reint_window {
     /* in */
@@ -645,7 +645,7 @@ int icg_ba_reintegrate_resident(icg_ba *h, int n_windows, const icg_ba_problem *
  * (restart included), icg_ba_download / icg_ba_gvins_optimization_end(next) and the resident calls give the same bits.  Every check (map ranges
  * against the old window, the upload's checks of next, a new blob's positive-definite covariance, the prior's origin) runs before the device is
  * written; a rejected call (ICG_EINVAL with a message) leaves the handle as it was.  n_windows must equal the uploaded count.  Asynchronous on the
- * handle's stream.  ICG_EUNSUPPORTED on a landmark-sharded handle.
+ * handle's stream.  ICG_EUNSUPPORTED on a landmark-sharded handle: its group calls icg_ba_shard_slide_resident.
  */
 typedef struct icg_ba_slide_window {
     const int32_t *node_src;  /* next.K: old node whose pose / mix carries over, or -1 (next.pose / next.mix row) */
@@ -682,7 +682,7 @@ int icg_ba_slide_resident(icg_ba *h, int n_windows, const icg_ba_problem *next, 
  * runs before the device is written.  The integration then runs into the slide's staging, the call synchronises and, when an integrated
  * covariance is not positive definite, returns ICG_EINVAL naming the first such factor (window order, then factor order) with the handle as it
  * was; the outputs are written either way.  Otherwise the call goes on as icg_ba_slide_resident does (asynchronous from there).
- * ICG_EUNSUPPORTED on a landmark-sharded handle.
+ * ICG_EUNSUPPORTED on a landmark-sharded handle: its group calls icg_ba_shard_slide_integrate_resident.
  */
 #define ICG_SLIDE_CHAIN (-2)
 #define ICG_SLIDE_ROW (-3)
@@ -706,6 +706,41 @@ typedef struct icg_ba_slide_integrate {
 } icg_ba_slide_integrate;
 int icg_ba_slide_integrate_resident(icg_ba *h, int n_windows, const icg_ba_problem *next, const icg_ba_slide_window *carry,
                                     const icg_ba_slide_integrate *integ, const double *noise5, const double *station3);
+/*
+ * The reintegration and the two slides on a landmark-sharded handle (world > 1): doReintegration (IG/ic_gvins.cc:1680-1695) and the time-node
+ * edits and next window of gvinsOptimization (:754-928, 1697-1837), as icg_ba_reintegrate_resident, icg_ba_slide_resident and
+ * icg_ba_slide_integrate_resident describe them, with the same structs.  Each is a COLLECTIVE call: every rank of the group calls it with its
+ * own shard problems, the same number of times.  On a handle outside a shard group (world == 1) each returns ICG_EINVAL naming its plain call.
+ *   Replicated / shard-local.  node_src, imu_src, gnss_src, prior_from_marg, the camera-side rows read from `next` (new pose / mix rows, new
+ *     blobs, new GNSS rows, gnss_node, the prior's block tables and x0, marg_J0 / marg_e0 when prior_from_marg = 0), noise5, station3, every
+ *     `integ` array and every icg_ba_reint_window must be the same on every rank.  lm_src and f_src name rows of the same rank's old shard (a
+ *     landmark never changes rank across a slide); new landmarks go to whichever rank the caller puts them on.  Every next shard lists its
+ *     factors landmark by landmark (f_lm non-decreasing), as the next sharded marginalization requires; a shard may be empty (L = 0).
+ *   Redundant integration.  The reintegration and the slide's integration run on every rank from its replicated states with the same
+ *     inputs, so every rank writes the same blobs, square-root information and node rows bit for bit; nothing is exchanged for them.
+ *   The prior on its owner.  prior_from_marg = 1: the owner of window w (rank w mod world) forms H0 / b0 / c0 on the device from the J0 / e0
+ *     that the last icg_ba_marginalize_resident[_culled] of the group left in the owner's gather handle.  That call must be the last
+ *     marginalization of the handle, a sharded resident one over the same n_windows with no upload or slide since, and the owner checks
+ *     next.marg_r / marg_nblocks against it.  The other ranks write zeros into that window's prior rows: nothing reads them there
+ *     (ba_lin_cam and ba_cost_cam evaluate the prior factor under the owner gate of the camera-only factors, and the sharded marginalization's
+ *     ba_marg_fill copies the prior from the owner's own handle).  prior_from_marg = 0: every rank forms it from next.marg_J0 / marg_e0, as
+ *     icg_ba_upload does.
+ *   Agreement before any write.  Each rank runs every check of the plain call, the ones above and its owner checks, then joins one integer
+ *     exchange of the group: its verdict and a 31-bit fingerprint of its camera-side arguments.  When any rank rejected, or the fingerprints
+ *     differ, EVERY rank returns ICG_EINVAL with its handle as it was, naming the rejecting rank or saying that the ranks' camera sides differ
+ *     (a rejecting rank keeps its own message; a failed allocation or CUDA call before the agreement is a rejection like any other).
+ *     The integrating slide exchanges its positive-definiteness outcome once more before the device is written.  A rank's own argument error therefore never leaves its peers to the bounded waits of the exchange; only a rank
+ *     that does not make the call does.  The sharded slide synchronises for the agreement (the plain slide stays asynchronous).
+ *   Contract.  After icg_ba_shard_slide[_integrate]_resident the group cannot be told apart from one whose ranks each called icg_ba_upload on
+ *     their next shards with the carried values filled in -- blobs as icg_imu_preintegrate gives them from the same start states, and the
+ *     owner's J0 / e0 as the prior --, for every later call (icg_ba_run_gvins with restart, icg_ba_gvins_optimization_end, the sharded
+ *     culling and marginalizations, the next sharded slide), except for the non-owners' prior rows, which nothing reads.
+ */
+int icg_ba_shard_reintegrate_resident(icg_ba *h, int n_windows, const icg_ba_problem *problems, const double *noise5, const double *station3,
+                                      icg_ba_reint_window *io);
+int icg_ba_shard_slide_resident(icg_ba *h, int n_windows, const icg_ba_problem *next, const icg_ba_slide_window *carry);
+int icg_ba_shard_slide_integrate_resident(icg_ba *h, int n_windows, const icg_ba_problem *next, const icg_ba_slide_window *carry,
+                                          const icg_ba_slide_integrate *integ, const double *noise5, const double *station3);
 /*
  * Landmark sharding of the window solve across the GPUs of one box (SURVEY.md 8e), over PEER MEMORY (transport "p2p"): every process
  * (one per GPU) uploads the same camera-side problem but only ITS landmarks and their reprojection factors; window w of the batch is
