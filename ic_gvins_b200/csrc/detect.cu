@@ -4,9 +4,11 @@
 //     cv::goodFeaturesToTrack(block_image, out, n, 0.01, track_min_pixel_distance_, block_mask)      (:647)
 //     cv::cornerSubPix(block_image, out, Size(5,5), Size(-1,-1), TermCriteria(COUNT+EPS, 20, 0.01))    (:651)
 // for ALL blocks of a frame in one call.  OpenCV is an un-vendored dependency of the reference; the arithmetic restated here
-// (SURVEY.md Appendix A.4 / A.5, float sequences matched bit-for-bit against cv2 4.13.0) is pinned by oracle/detect_ref.c and
-// tests/golden/detect_golden.npz.  ROI semantics as in C++: the Sobel derivative of a block reads the frame's pixels beyond
-// the block edge, the 3x3 covariance box filter reflects at the block edge, getRectSubPix replicates at the block edge.
+// (SURVEY.md Appendix A.4 / A.5: eig maps, corner lists and getRectSubPix patches bit-exact against cv2 4.13.0, sub-pixel positions
+// within 1e-3 px) is pinned by oracle/detect_ref.c and tests/golden/detect_golden.npz, detect_edges_golden.npz.  ROI semantics as in
+// C++: the Sobel derivative of a block reads the frame's pixels beyond the block edge, the 3x3 covariance box filter reflects at the
+// block edge, and cornerSubPix sees the block alone: getRectSubPix replicates at its edges except the top-right corner, and an
+// iterate that leaves the block is discarded.
 //
 // Kernels (all HBM/L2 streaming or tiny):  detect_eig (min-eigenvalue map + masked per-block maximum),
 // detect_nms (threshold, 3x3 non-maximum suppression, candidate list), detect_select (CTA per block: bitonic sort by
@@ -270,18 +272,29 @@ __global__ void __launch_bounds__(128) detect_subpix(DetArgs A, int half_win, in
     int iter = 0;
     float err = 0.f;
     do {
-        // getRectSubPix(src, Size(13, 13), cI, ..., CV_32F): bilinear, replicate at the ROI edge
+        // getRectSubPix(src, Size(13, 13), cI, ..., CV_32F) on the ROI, cv2 4.13.0's float sequence (SURVEY.md A.5): bilinear
+        // inside, a horizontal fma in window rows clamped to the first / last ROI row, edge columns replicated with the vertical weights,
+        // except that window rows above the ROI read column w - 2 at its right edge
         const float cx = cIx - 6.f, cy = cIy - 6.f;
         const int ipx = __float2int_rd(cx), ipy = __float2int_rd(cy);
         const float a = cx - (float) ipx, bq = cy - (float) ipy;
-        const float a11 = (1.f - a) * (1.f - bq), a12 = a * (1.f - bq), a21 = (1.f - a) * bq, a22 = a * bq;
+        const float a11 = (1.f - a) * (1.f - bq), a12 = a * (1.f - bq), a21 = (1.f - a) * bq, a22 = a * bq, b1 = 1.f - bq;
         __syncwarp();
         for (int e = lane; e < 169; e += 32) {
             const int yy = e / 13, xx = e - 13 * yy;
-            const int X0 = min(max(ipx + xx, 0), R.w - 1), X1 = min(max(ipx + xx + 1, 0), R.w - 1);
-            const int Y0 = min(max(ipy + yy, 0), R.h - 1), Y1 = min(max(ipy + yy + 1, 0), R.h - 1);
-            sub[e] = (float) roi[(size_t) Y0 * A.pitch + X0] * a11 + (float) roi[(size_t) Y0 * A.pitch + X1] * a12 + (float) roi[(size_t) Y1 * A.pitch + X0] * a21 +
-                     (float) roi[(size_t) Y1 * A.pitch + X1] * a22;
+            const int x = ipx + xx, y = ipy + yy;
+            const int Y0 = min(max(y, 0), R.h - 1), Y1 = min(max(y + 1, 0), R.h - 1);
+            const uint8_t *r0 = roi + (size_t) Y0 * A.pitch, *r1 = roi + (size_t) Y1 * A.pitch;
+            float v;
+            if (x < 0 || x >= R.w - 1) {
+                const int c = x < 0 ? 0 : (y < 0 ? R.w - 2 : R.w - 1);
+                v = (float) r0[c] * b1 + (float) r1[c] * bq;
+            } else if (Y0 == Y1) {
+                v = __fmaf_rn((float) r0[x + 1], a, (float) r0[x] * (1.f - a));
+            } else {
+                v = ((float) r0[x] * a11 + (float) r0[x + 1] * a12) + ((float) r1[x] * a21 + (float) r1[x + 1] * a22);
+            }
+            sub[e] = v;
         }
         __syncwarp();
         double sa = 0, sb = 0, sc = 0, sb1 = 0, sb2 = 0;
@@ -305,8 +318,8 @@ __global__ void __launch_bounds__(128) detect_subpix(DetArgs A, int half_win, in
         const double scale = 1.0 / det;
         const float nx = (float) ((double) cIx + sc * scale * sb1 - sb * scale * sb2), ny = (float) ((double) cIy - sb * scale * sb1 + sa * scale * sb2);
         err = (nx - cIx) * (nx - cIx) + (ny - cIy) * (ny - cIy);
+        if (nx < 0 || nx >= (float) R.w || ny < 0 || ny >= (float) R.h) break;  // an iterate outside the ROI is discarded
         cIx = nx, cIy = ny;
-        if (cIx < 0 || cIx >= (float) R.w || cIy < 0 || cIy >= (float) R.h) break;
     } while (++iter < max_iter && (double) err > eps2);
     if (fabsf(cIx - cTx) > (float) half_win || fabsf(cIy - cTy) > (float) half_win) cIx = cTx, cIy = cTy;
     if (lane == 0) xy[0] = cIx, xy[1] = cIy;

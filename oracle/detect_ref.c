@@ -7,9 +7,11 @@
  *
  * block_image / block_mask are ROI views of the frame (tracking.cc:644-645).  OpenCV (un-vendored; pinned here to
  * opencv-python-headless 4.13.0) evaluates the Sobel derivative of an ROI with the PARENT image's pixels beyond the ROI
- * edge, but box-filters the (ROI-sized, freshly allocated) covariance image with reflect-101 at the ROI edge, and
- * getRectSubPix replicates at the ROI edge.  This file reproduces exactly that; the float sequences of Sobel
- * (FMA forms below) were matched bit-for-bit against cv2 (tests/golden/make_detect_golden.py, SURVEY.md Appendix A.4/A.5).
+ * edge, but box-filters the (ROI-sized, freshly allocated) covariance image with reflect-101 at the ROI edge;
+ * cornerSubPix samples the ROI alone, through getRectSubPix's edge rule (icgo_rect_subpix: replicate, except at the
+ * top-right corner).  The min-eigenvalue maps and corner lists are bit-exact against cv2 and getRectSubPix patches are
+ * bit-exact; sub-pixel positions agree to 1e-3 px (tests/golden/make_detect_golden.py, make_detect_edges_golden.py,
+ * SURVEY.md Appendix A.4/A.5).
  */
 #include <float.h>
 #include <math.h>
@@ -161,8 +163,41 @@ int icgo_good_features_from_eig(const float *eig_in, int w, int h, const uint8_t
     return n_out;
 }
 
+/* cv::getRectSubPix(src, Size(n, n), (cx, cy), patch, CV_32F) of the w x h u8 image src (row stride `stride`), centres inside
+ * the image.  Window pixel (i, j) samples src at (ipx + j + a, ipy + i + b), (ipx, ipy) = floor of the window's top-left corner
+ * (cx, cy) - (n - 1) / 2 and (a, b) its fraction.  The float sequence below matches cv2 4.13.0 bit for bit, inside the image
+ * and at its edges (tests/golden/make_detect_edges_golden.py):
+ *  - both sample columns x, x + 1 and both sample rows y, y + 1 in the image: (s00 * a11 + s01 * a12) + (s10 * a21 + s11 * a22);
+ *  - window rows above the image or at / below its last row (the row clamped to [0, h - 1]): fmaf(s01, a, s00 * (1 - a));
+ *  - a column left of 0 or at / right of w - 1: (1 - b) * src(c, Y0) + b * src(c, Y1) of one edge column c, which is 0 on the
+ *    left and w - 1 on the right, except in window rows above the image (ipy + i < 0), where cv2 reads column w - 2 on the
+ *    right: it does not replicate at the top-right corner. */
+void icgo_rect_subpix(const uint8_t *src, int w, int h, int stride, float cx, float cy, int n, float *dst) {
+    const float x0 = cx - (n - 1) * 0.5f, y0 = cy - (n - 1) * 0.5f;
+    const int ipx = (int) floorf(x0), ipy = (int) floorf(y0);
+    const float a = x0 - ipx, b = y0 - ipy;
+    const float a11 = (1.f - a) * (1.f - b), a12 = a * (1.f - b), a21 = (1.f - a) * b, a22 = a * b, b1 = 1.f - b, b2 = b;
+    for (int i = 0; i < n; i++) {
+        const int y = ipy + i, Y0 = y < 0 ? 0 : (y > h - 1 ? h - 1 : y), Y1 = y + 1 < 0 ? 0 : (y + 1 > h - 1 ? h - 1 : y + 1);
+        const uint8_t *r0 = src + (size_t) Y0 * stride, *r1 = src + (size_t) Y1 * stride;
+        for (int j = 0; j < n; j++) {
+            const int x = ipx + j;
+            if (x < 0 || x >= w - 1) {
+                const int c = x < 0 ? 0 : (y < 0 ? w - 2 : w - 1);
+                dst[i * n + j] = (float) r0[c] * b1 + (float) r1[c] * b2;
+            } else if (Y0 == Y1) {
+                dst[i * n + j] = fmaf((float) r0[x + 1], a, (float) r0[x] * (1.f - a));
+            } else {
+                dst[i * n + j] = ((float) r0[x] * a11 + (float) r0[x + 1] * a12) + ((float) r1[x] * a21 + (float) r1[x + 1] * a22);
+            }
+        }
+    }
+}
+
 /* cv::cornerSubPix(roi, corners, win (5,5), zeroZone (-1,-1), (COUNT+EPS, max_iter, eps)) on the ROI (x0,y0,w,h):
- * getRectSubPix replicates at the ROI edge.  corners in ROI-local coordinates, refined in place. */
+ * cornerSubPix reads nothing outside its input, so the ROI behaves as a w x h image sampled by icgo_rect_subpix.  An iterate
+ * outside the ROI ends the loop and is discarded: the corner keeps the last iterate inside it.  corners in ROI-local
+ * coordinates, refined in place. */
 void icgo_corner_subpix_roi(const uint8_t *img, int W, int H, int stride, int x0, int y0, int w, int h, float *xy, int n, int half_win, int max_iter, double eps) {
     (void) W, (void) H;
     const int win_w = 2 * half_win + 1, sw = win_w + 2;
@@ -184,19 +219,7 @@ void icgo_corner_subpix_roi(const uint8_t *img, int W, int H, int stride, int x0
         int iter = 0;
         double err = 0;
         do {
-            /* getRectSubPix(src, Size(sw, sw), cI, subpix, CV_32F): bilinear, replicate border; top-left = cI - (sw-1)/2 */
-            float cx = cIx - (sw - 1) * 0.5f, cy = cIy - (sw - 1) * 0.5f;
-            int ipx = (int) floorf(cx), ipy = (int) floorf(cy);
-            float a = cx - ipx, b = cy - ipy;
-            float a11 = (1.f - a) * (1.f - b), a12 = a * (1.f - b), a21 = (1.f - a) * b, a22 = a * b;
-            for (int yy = 0; yy < sw; yy++)
-                for (int xx = 0; xx < sw; xx++) {
-                    int X0 = ipx + xx, Y0 = ipy + yy, X1 = X0 + 1, Y1 = Y0 + 1;
-                    X0 = X0 < 0 ? 0 : (X0 > w - 1 ? w - 1 : X0), X1 = X1 < 0 ? 0 : (X1 > w - 1 ? w - 1 : X1);
-                    Y0 = Y0 < 0 ? 0 : (Y0 > h - 1 ? h - 1 : Y0), Y1 = Y1 < 0 ? 0 : (Y1 > h - 1 ? h - 1 : Y1);
-                    sub[yy * sw + xx] = roi[(size_t) Y0 * stride + X0] * a11 + roi[(size_t) Y0 * stride + X1] * a12 + roi[(size_t) Y1 * stride + X0] * a21 +
-                                        roi[(size_t) Y1 * stride + X1] * a22;
-                }
+            icgo_rect_subpix(roi, w, h, stride, cIx, cIy, sw, sub);
             double A = 0, Bm = 0, Cc = 0, bb1 = 0, bb2 = 0;
             for (int i = 0; i < win_w; i++) {
                 double py = i - half_win;
@@ -216,8 +239,8 @@ void icgo_corner_subpix_roi(const uint8_t *img, int W, int H, int stride, int x0
             double scale = 1.0 / det;
             float nx = (float) (cIx + Cc * scale * bb1 - Bm * scale * bb2), ny = (float) (cIy - Bm * scale * bb1 + A * scale * bb2);
             err = (nx - cIx) * (nx - cIx) + (ny - cIy) * (ny - cIy); /* float arithmetic, as in cornersubpix.cpp */
+            if (nx < 0 || nx >= w || ny < 0 || ny >= h) break;
             cIx = nx, cIy = ny;
-            if (cIx < 0 || cIx >= w || cIy < 0 || cIy >= h) break;
         } while (++iter < max_iter && err > eps2);
         if (fabsf(cIx - cTx) > half_win || fabsf(cIy - cTy) > half_win) cIx = cTx, cIy = cTy;
         xy[2 * p] = cIx, xy[2 * p + 1] = cIy;

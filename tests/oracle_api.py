@@ -165,6 +165,8 @@ def declare_detect(lib):
     lib.icgo_good_features_from_eig.restype = C.c_int
     lib.icgo_corner_subpix_roi.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_double]
     lib.icgo_corner_subpix_roi.restype = None
+    lib.icgo_rect_subpix.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_int, vp]
+    lib.icgo_rect_subpix.restype = None
     lib.icgo_detect_block.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, vp]
     lib.icgo_detect_block.restype = C.c_int
 
@@ -184,7 +186,7 @@ def good_features(lib, img, n, quality, min_dist, mask=None, roi=None):
     roi = roi or (0, 0, W, H)
     eig = min_eig_roi(lib, img, roi)
     x0, y0, w, h = roi
-    out = np.zeros((max(1, n), 2), np.float32)
+    out = np.zeros((w * h, 2), np.float32)  # max_corners <= 0 is unlimited: every pixel can be a corner
     m = None
     if mask is not None:
         m = np.ascontiguousarray(mask)
@@ -202,11 +204,20 @@ def corner_subpix(lib, img, pts, roi=None):
     return p
 
 
+def rect_subpix(lib, img, centre, n=13):
+    """cv2.getRectSubPix(img, (n, n), centre, patchType=CV_32F) of a u8 image."""
+    img = np.ascontiguousarray(img)
+    H, W = img.shape
+    out = np.zeros((n, n), np.float32)
+    lib.icgo_rect_subpix(_p(img), W, H, W, float(centre[0]), float(centre[1]), n, _p(out))
+    return out
+
+
 def detect_block(lib, img, mask, roi, n, quality, min_dist):
     img = np.ascontiguousarray(img)
     H, W = img.shape
     x0, y0, w, h = roi
-    out = np.zeros((max(1, n), 2), np.float32)
+    out = np.zeros((w * h, 2), np.float32)  # as in good_features
     m = np.ascontiguousarray(mask) if mask is not None else None
     cnt = lib.icgo_detect_block(_p(img), _p(m) if m is not None else None, W, H, W, x0, y0, w, h, n, quality, min_dist, _p(out))
     return out[:cnt].copy()
