@@ -139,6 +139,7 @@ def _declare_r2(L: C.CDLL) -> None:
     L.icg_ba_reintegrate_resident.argtypes = [vp, C.c_int, vp, vp, vp, vp]
     L.icg_ba_slide_resident.argtypes = [vp, C.c_int, vp, vp]
     L.icg_ba_slide_integrate_resident.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp]
+    L.icg_ba_slide_vision_resident.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp, vp]
     L.icg_ba_shard_reintegrate_resident.argtypes = [vp, C.c_int, vp, vp, vp, vp]
     L.icg_ba_shard_slide_resident.argtypes = [vp, C.c_int, vp, vp]
     L.icg_ba_shard_slide_integrate_resident.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp]
@@ -159,6 +160,18 @@ class SlideIntegrate(C.Structure):
                 ("status", C.POINTER(C.c_int8)), ("blob_out", f64p), ("end_state10", f64p)]
 
 
+class SlideVision(C.Structure):
+    """ctypes image of `icg_ba_slide_vision` (device pointers as void *)."""
+    _fields_ = [("num_marg", C.c_int32), ("node_in_map", u8p), ("obs_factor", i32p), ("cam", C.c_double * 10), ("node_td", f64p),
+                ("cur_node", C.c_int32), ("n_frames", C.c_int32), ("frame_id", C.POINTER(C.c_int64)), ("frame_node", i32p),
+                ("n_obs", C.c_int32), ("n_in", C.c_int32), ("dev_n", vp), ("obs_src", vp), ("obs_lm", vp), ("obs_node", vp), ("obs_undis_xy", vp),
+                ("obs_vel", vp), ("n_new", C.c_int32), ("dev_new_n", vp), ("new_depth", vp), ("new_vel_ref", vp), ("new_vel_cur", vp),
+                ("new_ref_undis_xy", vp), ("new_cur_undis_xy", vp), ("new_ref_frame_id", vp),
+                ("L", C.c_int32), ("F", C.c_int32), ("nan_dropped", C.c_int32),
+                ("lm_src", i32p), ("f_src", i32p), ("f_lm", i32p), ("f_ref", i32p), ("f_obs", i32p), ("lm_origin", i32p), ("nan_flags", u8p),
+                ("invdepth", f64p), ("f_const", f64p)]
+
+
 # every symbol include/icgvins_b200.h declares (checked by tests/test_abi.py against the header text)
 EXPORTS = [
     "icg_last_error", "icg_version", "icg_launch_count", "icg_launch_count_reset",
@@ -172,5 +185,5 @@ EXPORTS = [
     "icg_geom_find_fundamental_mat_ransac_batch", "icg_klt_track_frames_dev", "icg_klt_track_frame",
     "icg_klt_triangulate_dev", "icg_klt_triangulate",
     "icg_imu_preintegrate", "icg_ba_create", "icg_ba_destroy", "icg_ba_solve", "icg_ba_upload", "icg_ba_run", "icg_ba_download",
-    "icg_ba_sync", "icg_ba_shard_export", "icg_ba_shard_connect", "icg_ba_shard_error", "icg_ba_shard_leave", "icg_ba_gvins_optimization", "icg_ba_run_gvins", "icg_ba_gvins_optimization_begin", "icg_ba_gvins_optimization_end", "icg_ba_residual_costs", "icg_ba_reproj_evaluate", "icg_ba_imu_evaluate", "icg_ba_marginalize", "icg_ba_marginalize_resident", "icg_ba_update_and_cull_resident", "icg_ba_marginalize_resident_culled", "icg_ba_reintegrate_resident", "icg_ba_slide_resident", "icg_ba_slide_integrate_resident", "icg_ba_shard_reintegrate_resident", "icg_ba_shard_slide_resident", "icg_ba_shard_slide_integrate_resident", "icg_ba_gnss_evaluate", "icg_ba_pose_prior_evaluate", "icg_ba_mix_prior_evaluate", "icg_ba_imu_error_evaluate", "icg_ba_marg_factor_evaluate",
+    "icg_ba_sync", "icg_ba_shard_export", "icg_ba_shard_connect", "icg_ba_shard_error", "icg_ba_shard_leave", "icg_ba_gvins_optimization", "icg_ba_run_gvins", "icg_ba_gvins_optimization_begin", "icg_ba_gvins_optimization_end", "icg_ba_residual_costs", "icg_ba_reproj_evaluate", "icg_ba_imu_evaluate", "icg_ba_marginalize", "icg_ba_marginalize_resident", "icg_ba_update_and_cull_resident", "icg_ba_marginalize_resident_culled", "icg_ba_reintegrate_resident", "icg_ba_slide_resident", "icg_ba_slide_integrate_resident", "icg_ba_slide_vision_resident", "icg_ba_shard_reintegrate_resident", "icg_ba_shard_slide_resident", "icg_ba_shard_slide_integrate_resident", "icg_ba_gnss_evaluate", "icg_ba_pose_prior_evaluate", "icg_ba_mix_prior_evaluate", "icg_ba_imu_error_evaluate", "icg_ba_marg_factor_evaluate",
 ]

@@ -250,11 +250,35 @@ def imu_preintegrate(state16, iewn, gravity, noise5, imu):
     return blob, end
 
 
+def _integ_struct(s, g, m, arg):
+    """fill one icg_ba_slide_integrate from an `integrate` dict of WindowSolver.slide_integrate (m = next n_imu)"""
+    from ._lib import u8p
+    if g.get("imu_from") is not None:
+        s.imu_from = arg(g["imu_from"], np.int32, ip)
+        if "imu_off" in g:
+            imu, off = g["imu"], g["imu_off"]
+        else:
+            rows = [np.zeros((0, 7)) if r is None else np.asarray(r, np.float64).reshape(-1, 7) for r in g["imu_rows"]]
+            off = np.zeros(m + 1, np.int32)
+            off[1:] = np.cumsum([len(r) for r in rows])
+            imu = np.concatenate(rows, axis=0) if rows else np.zeros((0, 7))
+        s.imu, s.imu_off = arg(imu, np.float64, dp), arg(off, np.int32, ip)
+        s.gravity3 = arg(np.broadcast_to(np.asarray(g["gravity"], np.float64), (m, 3)), np.float64, dp)
+        s.normal = arg(np.broadcast_to(np.asarray(g.get("normal", False), np.uint8), (m,)), np.uint8, u8p)
+        if g.get("state16") is not None:
+            s.state16 = arg(g["state16"], np.float64, dp)
+    if g.get("node_from_imu") is not None:
+        s.node_from_imu = arg(g["node_from_imu"], np.uint8, u8p)
+    if g.get("gnss_node") is not None:
+        s.gnss_node, s.gnss_dt = arg(g["gnss_node"], np.int32, ip), arg(g["gnss_dt"], np.float64, dp)
+
+
 class WindowSolver:
     """Batched sliding-window solver handle (one per optimization thread / GPU)."""
 
     def __init__(self, max_windows=1, max_K=10, max_L=300, max_F=2700, max_gnss=16, max_marg_r=160, device=0, stream=None):
         self._h = vp()
+        self.max_L, self.max_F = max_L, max_F
         check(lib().icg_ba_create(C.byref(self._h), max_windows, max_K, max_L, max_F, max_gnss, max_marg_r, device,
                                   vp(stream) if stream else None), "icg_ba_create")
 
@@ -544,26 +568,8 @@ class WindowSolver:
             outs.append(o)
             iw[w].status, iw[w].blob_out = o["status"].ctypes.data_as(C.POINTER(C.c_int8)), o["blobs"].ctypes.data_as(dp)
             iw[w].end_state10 = o["end_states"].ctypes.data_as(dp)
-            if not g:
-                continue
-            if g.get("imu_from") is not None:
-                iw[w].imu_from = arg(g["imu_from"], np.int32, ip)
-                if "imu_off" in g:
-                    imu, off = g["imu"], g["imu_off"]
-                else:
-                    rows = [np.zeros((0, 7)) if r is None else np.asarray(r, np.float64).reshape(-1, 7) for r in g["imu_rows"]]
-                    off = np.zeros(m + 1, np.int32)
-                    off[1:] = np.cumsum([len(r) for r in rows])
-                    imu = np.concatenate(rows, axis=0) if rows else np.zeros((0, 7))
-                iw[w].imu, iw[w].imu_off = arg(imu, np.float64, dp), arg(off, np.int32, ip)
-                iw[w].gravity3 = arg(np.broadcast_to(np.asarray(g["gravity"], np.float64), (m, 3)), np.float64, dp)
-                iw[w].normal = arg(np.broadcast_to(np.asarray(g.get("normal", False), np.uint8), (m,)), np.uint8, u8p)
-                if g.get("state16") is not None:
-                    iw[w].state16 = arg(g["state16"], np.float64, dp)
-            if g.get("node_from_imu") is not None:
-                iw[w].node_from_imu = arg(g["node_from_imu"], np.uint8, u8p)
-            if g.get("gnss_node") is not None:
-                iw[w].gnss_node, iw[w].gnss_dt = arg(g["gnss_node"], np.int32, ip), arg(g["gnss_dt"], np.float64, dp)
+            if g:
+                _integ_struct(iw[w], g, m, arg)
         nz = np.ascontiguousarray(noise5, np.float64)
         stn = np.ascontiguousarray(station, np.float64)
         rc = getattr(lib(), fn)(self._h, n, arr, cw, iw, vp(nz.ctypes.data), vp(stn.ctypes.data))
@@ -573,6 +579,105 @@ class WindowSolver:
             raise err
         self._keep, self._n = arr, n
         return outs
+
+    def slide_vision(self, next_problems, carry, vision, integrate=None, noise5=None, station=(0.0, 0.0, 0.0), prior_from_marg=True):
+        """slide() (integrate given: slide_integrate()) whose vision rows are built on the device (icg_ba_slide_vision_resident):
+        addReprojectionParameters + addReprojectionFactors on the culled window this handle holds plus the new keyframes' observations.  The
+        last update_and_cull() of these windows must be current.  next_problems' L, F, invdepth, f_lm / f_ref / f_obs / f_const, f_active and
+        carry's lm_src / f_src are not read; they are written into next_problems / carry (carried f_const rows as NaN, as slide() never reads
+        them).  vision: one dict per window with
+          num_marg, node_in_map (old K), obs_factor (the culling's), camera (camera.Camera or CameraStruct), node_td (next K), cur_node,
+          frames ({frame id: next node}) for the new points' reference frames;
+          tracked observations as DEVICE tensors (torch): obs_lm, obs_node (optional: cur_node), obs_undis_xy (float32 x 2), obs_vel (x 2),
+            obs_src (optional, with n_in) and dev_n (optional int32 device count), n_obs (count, or the list's length with dev_n);
+          new map points as DEVICE tensors: new_depth, new_ref_undis_xy, new_vel_ref, new_ref_frame_id (int64), new_cur_undis_xy,
+            new_vel_cur, n_new and optionally dev_new_n.
+        Returns one dict per window: L, F, nan_dropped, nan_flags (old L + n_new entries first: 1 where a landmark or new point was dropped
+        for a NaN inverse depth), lm_origin (old landmark, or -(j + 1) for new point j), lm_src, f_src, f_lm, f_ref, f_obs, invdepth and f_const (the new factors' rows, f_src = -1;
+        the others zero).  A rejected call raises IcgError with the handle unchanged."""
+        from ._lib import IcgError, SlideIntegrate, SlideVision, SlideWindow
+        from .camera import CameraStruct
+        if integrate is not None and noise5 is None:
+            raise ValueError("slide_vision: integrate needs noise5")
+        n = len(next_problems)
+        flags = [prior_from_marg] * n if np.isscalar(prior_from_marg) else list(prior_from_marg)
+        Lc, Fc = self.max_L, self.max_F
+        outs = []
+        for p, v in zip(next_problems, vision):  # the built rows land here, sized to the handle's capacity until the call returns
+            o = dict(lm_src=np.zeros(Lc, np.int32), lm_origin=np.zeros(Lc, np.int32), nan_flags=np.zeros(Lc + int(v.get("n_new", 0)), np.uint8), f_src=np.zeros(Fc, np.int32), f_lm=np.zeros(Fc, np.int32), f_ref=np.zeros(Fc, np.int32),
+                     f_obs=np.zeros(Fc, np.int32), invdepth=np.zeros(Lc), f_const=np.zeros((Fc, 14)))
+            outs.append(o)
+            p.update(L=0, F=0, invdepth=np.zeros(0), f_lm=np.zeros(0, np.int32), f_ref=np.zeros(0, np.int32), f_obs=np.zeros(0, np.int32),
+                     f_const=np.zeros(0), f_active=np.zeros(0, np.uint8))
+        arr = (BaProblem * n)(*[to_struct(p) for p in next_problems])
+        cw = (SlideWindow * n)()
+        vw = (SlideVision * n)()
+        iw = (SlideIntegrate * n)() if integrate is not None else None
+        keep = []
+
+        def arg(a, dtype, ptr):
+            a = np.ascontiguousarray(a, dtype)
+            keep.append(a)
+            return a.ctypes.data_as(ptr)
+
+        def dev(t):
+            return None if t is None else vp(t.data_ptr() if hasattr(t, "data_ptr") else int(t))
+
+        for w, (p, c, v) in enumerate(zip(next_problems, carry, vision)):
+            for k in ("node_src", "imu_src", "gnss_src"):
+                if c.get(k) is not None:
+                    setattr(cw[w], k, arg(c[k], np.int32, ip))
+            cw[w].prior_from_marg = 1 if flags[w] else 0
+            if iw is not None and integrate[w]:
+                _integ_struct(iw[w], integrate[w], int(p["n_imu"]), arg)
+            s = vw[w]
+            s.num_marg = int(v["num_marg"])
+            s.node_in_map = arg(v["node_in_map"], np.uint8, bp)
+            if v.get("obs_factor") is not None and len(v["obs_factor"]):
+                s.obs_factor = arg(v["obs_factor"], np.int32, ip)
+            cam = v["camera"]
+            cs = cam.c if hasattr(cam, "c") else cam
+            s.cam[:] = [float(getattr(cs, k)) for k, _ in CameraStruct._fields_]
+            s.node_td = arg(v["node_td"], np.float64, dp)
+            s.cur_node = int(v["cur_node"])
+            frames = v.get("frames", {})
+            s.n_frames = len(frames)
+            s.frame_id = arg(np.array(list(frames.keys()), np.int64), np.int64, C.POINTER(C.c_int64))
+            s.frame_node = arg(np.array(list(frames.values()), np.int32), np.int32, ip)
+            s.n_obs, s.n_in = int(v.get("n_obs", 0)), int(v.get("n_in", 0))
+            s.dev_n, s.obs_src, s.obs_lm, s.obs_node = (dev(v.get(k)) for k in ("dev_n", "obs_src", "obs_lm", "obs_node"))
+            s.obs_undis_xy, s.obs_vel = dev(v.get("obs_undis_xy")), dev(v.get("obs_vel"))
+            s.n_new = int(v.get("n_new", 0))
+            s.dev_new_n = dev(v.get("dev_new_n"))
+            s.new_depth, s.new_vel_ref, s.new_vel_cur = (dev(v.get(k)) for k in ("new_depth", "new_vel_ref", "new_vel_cur"))
+            s.new_ref_undis_xy, s.new_cur_undis_xy, s.new_ref_frame_id = (dev(v.get(k)) for k in ("new_ref_undis_xy", "new_cur_undis_xy", "new_ref_frame_id"))
+            o = outs[w]
+            s.lm_src, s.f_src, s.f_lm, s.f_ref, s.f_obs = (o[k].ctypes.data_as(ip) for k in ("lm_src", "f_src", "f_lm", "f_ref", "f_obs"))
+            s.invdepth, s.f_const = o["invdepth"].ctypes.data_as(dp), o["f_const"].ctypes.data_as(dp)
+            s.lm_origin, s.nan_flags = o["lm_origin"].ctypes.data_as(ip), o["nan_flags"].ctypes.data_as(bp)
+        nz = np.ascontiguousarray(noise5 if noise5 is not None else np.zeros(5), np.float64)
+        stn = np.ascontiguousarray(station, np.float64)
+        rc = lib().icg_ba_slide_vision_resident(self._h, n, arr, cw, None if iw is None else iw, vp(nz.ctypes.data) if iw is not None else None,
+                                                vp(stn.ctypes.data) if iw is not None else None, vw)
+        if rc != 0:
+            err = IcgError(f"icg_ba_slide_vision_resident failed with code {rc}: {lib().icg_last_error().decode('utf-8', 'replace')}")
+            err.code = rc
+            raise err
+        res = []
+        for w, (p, c, o) in enumerate(zip(next_problems, carry, outs)):
+            L, F = int(vw[w].L), int(vw[w].F)
+            r = dict(L=L, F=F, nan_dropped=int(vw[w].nan_dropped), lm_src=o["lm_src"][:L].copy(), lm_origin=o["lm_origin"][:L].copy(),
+                     nan_flags=o["nan_flags"], invdepth=o["invdepth"][:L].copy(),
+                     f_src=o["f_src"][:F].copy(), f_lm=o["f_lm"][:F].copy(), f_ref=o["f_ref"][:F].copy(), f_obs=o["f_obs"][:F].copy(),
+                     f_const=o["f_const"][:F].copy())
+            res.append(r)
+            fcn = r["f_const"].copy()
+            fcn[r["f_src"] >= 0] = np.nan
+            p.update(L=L, F=F, invdepth=r["invdepth"].copy(), f_lm=r["f_lm"].copy(), f_ref=r["f_ref"].copy(), f_obs=r["f_obs"].copy(),
+                     f_const=fcn.reshape(-1), f_active=np.ones(F, np.uint8))
+            c["lm_src"], c["f_src"] = r["lm_src"].copy(), r["f_src"].copy()
+        self._keep, self._n = arr, n
+        return res
 
     def gvins_optimization_end(self, problems):
         """icg_ba_gvins_optimization_end after run_gvins(): synchronises, writes the parameters, f_active and gnss_std back into the problem

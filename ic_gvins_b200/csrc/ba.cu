@@ -33,12 +33,14 @@
 
 #include <algorithm>
 #include <functional>
+#include <memory>
 #include <string>
 #include <thread>
 #include <vector>
 
 #include "ba_cull.cuh"
 #include "ba_slide.cuh"
+#include "ba_vision.cuh"
 #include "preint.cuh"
 #include "ba_math.cuh"
 #include "common.cuh"
@@ -1814,6 +1816,15 @@ struct icg_ba {
     // post-solve update + culling: one pinned staging buffer and its device twin, [inputs | outputs], grown on demand
     unsigned char *cull_h = nullptr, *cull_d = nullptr;
     size_t cull_cap = 0;
+    // the last culling, while it is current (icg_ba_slide_vision_resident reads its flags from the staging above): its window count (0: none;
+    // an upload, a slide or a sharded culling clears it), every window's slices and observation count, the staging offsets of its arrays
+    int cull_res_n = 0;
+    std::vector<CullWin> cull_res_win;
+    std::vector<int> cull_res_nobs;
+    size_t cull_res_ref = 0, cull_res_off = 0, cull_res_lmo = 0, cull_res_obso = 0;
+    // icg_ba_slide_vision_resident: pinned staging and its device twin, grown on demand
+    unsigned char *vis_h = nullptr, *vis_d = nullptr;
+    size_t vis_cap = 0;
     // reintegration of the resident IMU factors: the same arrangement, its own buffers
     unsigned char *reint_h = nullptr, *reint_d = nullptr;
     size_t reint_cap = 0;
@@ -1828,6 +1839,9 @@ struct icg_ba {
     unsigned char *slide_h = nullptr, *slide_d = nullptr;
     size_t slide_cap = 0;
     double *slide_old = nullptr, *fc_alt = nullptr;
+    // every landmark's reference row pts0[3] | vel0[3] | td0 (NaN: unknown), 7 doubles at w L + l, and the buffer the next slide writes: set by
+    // icg_ba_upload from the landmark's first factor, carried by every slide, read by icg_ba_slide_vision_resident
+    double *lm_ref = nullptr, *lm_ref_alt = nullptr;
     cudaEvent_t slide_ev = nullptr;  // recorded after the staging's H2D
     // post-solve calls of a shard group (world > 1): integer exchanges so far (slot parity), epoch of the last marginalization export, the
     // exchange's device word, the export's slot lists, the owner's gathered rows with their tables, and the handle the owner uploads its
@@ -1996,6 +2010,8 @@ static int ba_create_body(icg_ba *h, int max_windows, int max_K, int max_L, int 
         rc = dmalloc(h, &fa0, (NW * C.F + 7) / 8 + 1);
         D.f_active_0 = (uint8_t *) fa0;
     }
+    if (rc == ICG_OK) rc = dmalloc(h, &h->lm_ref, NW * C.L * 7);
+    if (rc == ICG_OK) rc = dmalloc(h, &h->lm_ref_alt, NW * C.L * 7);
     if (rc != ICG_OK) return rc;
     // shared-memory budgets
     h->smem_cam = sizeof(double) * ((size_t) C.K * 480 + (size_t) C.G * 24 + 48 + 16 + 2 * (size_t) C.R + 8) + sizeof(int) * (size_t) C.R + 64;
@@ -2048,6 +2064,8 @@ void icg_ba_destroy(icg_ba *h) {
     if (h->reint_d) cudaFree(h->reint_d);
     if (h->slide_h) cudaFreeHost(h->slide_h);
     if (h->slide_d) cudaFree(h->slide_d);
+    if (h->vis_h) cudaFreeHost(h->vis_h);
+    if (h->vis_d) cudaFree(h->vis_d);
     if (h->slide_old) cudaFree(h->slide_old);
     if (h->fc_alt) cudaFree(h->fc_alt);
     if (h->slide_ev) cudaEventDestroy(h->slide_ev);
@@ -2057,6 +2075,34 @@ void icg_ba_destroy(icg_ba *h) {
     if (h->ev_join) cudaEventDestroy(h->ev_join);
     if (h->own_stream && h->stream) cudaStreamDestroy(h->stream);
     delete h;
+}
+
+// Every landmark's reference row (pts0, vel0, td0 of its factors' constants) into out: the old row of the landmark a slide carries (win / map:
+// the slide's staging), otherwise its first factor's (record slot order), otherwise NaN.  One thread per landmark position, blockIdx.y = window.
+__global__ void ba_lm_ref_fill(const WinDims *dims, const SlideWin *win, const int *map, const double *old, const double *fc, const int *lm_off,
+                               const int *lm_perm, double *out, int Lc, int Fc) {
+    const int w = blockIdx.y, L = dims[w].L;
+    const size_t wL = (size_t) w * Lc;
+    for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < L; p += gridDim.x * blockDim.x) {
+        const int l = lm_perm[wL + p], m = win ? map[win[w].lm_map + l] : -1;
+        const int q0 = lm_off[(size_t) w * (Lc + 1) + p], q1 = lm_off[(size_t) w * (Lc + 1) + p + 1];
+        double *r = out + (wL + l) * 7;
+        if (m >= 0) {
+            for (int c = 0; c < 7; c++) r[c] = old[(wL + m) * 7 + c];
+        } else if (q1 > q0) {
+            const double *f = fc + ((size_t) w * Fc + q0) * 14;
+            r[0] = f[0], r[1] = f[1], r[2] = f[2], r[3] = f[6], r[4] = f[7], r[5] = f[8], r[6] = f[12];
+        } else {
+            for (int c = 0; c < 7; c++) r[c] = __longlong_as_double(0x7ff8000000000000LL);
+        }
+    }
+}
+
+static cudaError_t launch_lm_ref_fill(icg_ba *h, int n, const SlideWin *win, const int *map, const double *old, double *out) {
+    const int gx = std::max(1, std::min(8, (h->C.L + 255) / 256));
+    ba_lm_ref_fill<<<dim3(gx, n), 256, 0, h->stream>>>(h->D.dims, win, map, old, h->D.f_const_s, h->D.lm_off, h->D.lm_perm, out, h->C.L, h->C.F);
+    count_launch();
+    return cudaGetLastError();
 }
 
 // Packing of one window into the pinned staging arrays (host side of the seam: what AddParameterBlock / AddResidualBlock do in
@@ -2320,6 +2366,7 @@ int icg_ba_upload(icg_ba *h, int n, const icg_ba_problem *P) {
     ICG_CUDA(cudaSetDevice(h->device));
     const BaCaps &C = h->C;
     h->marg_res_n = 0;  // the marginalization workspace no longer belongs to the windows the handle holds
+    h->cull_res_n = 0;
     int rc = pack_windows(h, n, P, true);
     if (rc != ICG_OK) return rc;
     rc = upload_structure(h, n);
@@ -2330,6 +2377,7 @@ int icg_ba_upload(icg_ba *h, int n, const icg_ba_problem *P) {
     UP(pose, C.K * 7); UP(mix, C.K * 9); UP(rho, C.L); UP(f_const_s, C.F * 14); UP(imu_blob, C.K * ICG_IMU_BLOB_DOUBLES); UP(imu_U, C.K * 225);
     UP(gnss_blh, C.G * 3); UP(gnss_std, C.G * 3); UP(marg_H0, (size_t) C.R * C.R); UP(marg_b0, C.R); UP(marg_c0, 1);
 #undef UP
+    ICG_CUDA(launch_lm_ref_fill(h, n, nullptr, nullptr, nullptr, h->lm_ref));
     rc = keep_pristine(h, n);
     if (rc != ICG_OK) return rc;
     h->cur_windows = n;
@@ -3487,6 +3535,7 @@ int icg_ba_update_and_cull_resident(icg_ba *h, int n_windows, const icg_ba_probl
     const size_t in_bytes = at;
     const size_t o_win = take(sizeof(CullOut) * n), o_pose = take(96 * nK), o_pw = take(24 * nL), o_depth = take(8 * nL), o_lmo = take(nL), o_obso = take(nO);
     const size_t out_bytes = at - in_bytes;
+    h->cull_res_n = 0;  // the staging is rewritten (or replaced) from here
     ICG_CUDA(cudaSetDevice(h->device));
     cudaStream_t s = h->stream;
     if (at > h->cull_cap) {
@@ -3533,6 +3582,11 @@ int icg_ba_update_and_cull_resident(icg_ba *h, int n_windows, const icg_ba_probl
     ICG_CUDA(cudaMemcpyAsync(H + in_bytes, Dv + in_bytes, out_bytes, cudaMemcpyDeviceToHost, s));
     ICG_CUDA(cudaStreamSynchronize(s));
     if (h->D.world > 1 && (rc = shard_timed_out(h, "icg_ba_update_and_cull_resident")) != ICG_OK) return rc;
+    if (h->D.world == 1) {
+        h->cull_res_n = n, h->cull_res_win = win, h->cull_res_nobs.resize(n);
+        for (int w = 0; w < n; w++) h->cull_res_nobs[w] = problems[w].L > 0 ? io[w].obs_off[problems[w].L] : 0;
+        h->cull_res_ref = i_ref, h->cull_res_off = i_off, h->cull_res_lmo = o_lmo, h->cull_res_obso = o_obso;
+    }
     for (int w = 0; w < n; w++) {
         const icg_ba_problem &p = problems[w];
         icg_ba_cull_window &c = io[w];
@@ -3784,8 +3838,9 @@ int icg_ba_marginalize_resident_culled(icg_ba *h, int n_windows, const icg_ba_pr
 // check of its own prior; then one agreement of the group (shard_agree: every rank's verdict and a fingerprint of the camera side) before any
 // rank writes its device, and with `integ` a second one on the integration's outcome.  A rank that rejects joins the agreement all the same
 // (fail below), so its peers never wait for it.  The owner of window w forms its prior from the workspace of mx_h; the other ranks get zeros.
+// lm_ref_built: icg_ba_slide_vision_resident has written the next windows' reference rows into lm_ref_alt already
 static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba_slide_window *carry, const icg_ba_slide_integrate *integ,
-                      const double *noise5, const double *station3, const char *fn, bool sharded) {
+                      const double *noise5, const double *station3, const char *fn, bool sharded, bool lm_ref_built = false) {
     bool joined = false;  // sharded: this rank has joined the agreement of the call
     std::vector<WinDims> old_dims;
     std::vector<std::vector<int>> old_slot;
@@ -4196,6 +4251,7 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
     }
     // every check has passed: from here on the device is written
     h->marg_res_n = 0;
+    h->cull_res_n = 0;
     if (iwins.empty()) ICG_CUDA(cudaMemcpyAsync(h->slide_d, h->slide_h, in_end, cudaMemcpyHostToDevice, s));
     ICG_CUDA(cudaEventRecord(h->slide_ev, s));
     rc = upload_structure(h, n);
@@ -4224,6 +4280,8 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
     count_launch(2);
     std::swap(h->f_const_s.d, h->fc_alt);  // the gathered record constants become the handle's
     D.f_const_s = h->f_const_s.d;
+    if (!lm_ref_built) ICG_CUDA(launch_lm_ref_fill(h, n, a.win, a.map, h->lm_ref, h->lm_ref_alt));
+    std::swap(h->lm_ref, h->lm_ref_alt);
     rc = keep_pristine(h, n);
     if (rc != ICG_OK) return rc;
     h->cur_windows = n;
@@ -4241,6 +4299,158 @@ int icg_ba_slide_integrate_resident(icg_ba *h, int n, const icg_ba_problem *next
         return ICG_EINVAL;
     }
     return slide_body(h, n, next, carry, integ, noise5, station3, "icg_ba_slide_integrate_resident", false);
+}
+
+// the vision half of the next windows built on the device (ba_vision.cu), then the slide of those windows
+int icg_ba_slide_vision_resident(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba_slide_window *carry, const icg_ba_slide_integrate *integ,
+                                 const double *noise5, const double *station3, icg_ba_slide_vision *vis) {
+    static const char *fn = "icg_ba_slide_vision_resident";
+    if (h && h->D.world > 1) {
+        set_error("%s: not available on a landmark-sharded handle", fn);
+        return ICG_EUNSUPPORTED;
+    }
+    int rc = resident_single_rank(h, n, next, fn);
+    if (rc != ICG_OK) return rc;
+    if (!carry || !vis || (integ && (!noise5 || !station3))) {
+        set_error("%s: bad arguments", fn);
+        return ICG_EINVAL;
+    }
+    if (h->cull_res_n != n) {
+        set_error("%s: no culling of these %d windows is current (icg_ba_update_and_cull_resident, with no upload or slide since)", fn, n);
+        return ICG_EINVAL;
+    }
+    ICG_CUDA(cudaSetDevice(h->device));
+    const BaCaps &C = h->C;
+    std::vector<VisWin> wins(n);
+    size_t n_ofac = 0, n_lm = 0, n_f = 0, n_nf = 0, n_scr = 0;
+    for (int w = 0; w < n; w++) {
+        const icg_ba_problem &p = next[w];
+        const icg_ba_slide_vision &v = vis[w];
+        const WinDims &od = h->dims.h[w];
+        const CullWin &cw = h->cull_res_win[w];
+        const int nco = h->cull_res_nobs[w];
+        bool bad = p.K < 2 || p.K > C.K || v.num_marg < 0 || v.num_marg > od.K || !v.node_in_map || !v.node_td || v.cur_node < 0 || v.cur_node >= p.K ||
+                   v.n_frames < 0 || v.n_frames > VIS_MAX_FRAMES || (v.n_frames > 0 && (!v.frame_id || !v.frame_node)) || v.n_obs < 0 || v.n_new < 0 ||
+                   (v.obs_src && v.n_in < 0) || (v.n_obs > 0 && (!v.obs_lm || !v.obs_undis_xy || !v.obs_vel)) ||
+                   (v.n_new > 0 && (!v.new_depth || !v.new_vel_ref || !v.new_vel_cur || !v.new_ref_undis_xy || !v.new_cur_undis_xy || !v.new_ref_frame_id)) ||
+                   (nco > 0 && !v.obs_factor) || cw.K != od.K || cw.L != od.L;
+        for (int e = 0; !bad && e < v.n_frames; e++) bad = v.frame_node[e] < 0 || v.frame_node[e] >= p.K;
+        if (bad) {
+            set_error("%s: window %d: arguments out of range or arrays missing", fn, w);
+            return ICG_EINVAL;
+        }
+        VisWin &W = wins[w];
+        memset(&W, 0, sizeof(W));
+        W.cam = v.cam;
+        memcpy(W.node_td, v.node_td, sizeof(double) * p.K);
+        memset(W.onode, -1, sizeof(W.onode));
+        const int32_t *ns = carry[w].node_src;
+        for (int j = 0; ns && j < p.K; j++)
+            if (ns[j] >= v.num_marg && ns[j] < od.K && v.node_in_map[ns[j]]) W.onode[ns[j]] = (int8_t) j;
+        for (int e = 0; e < v.n_frames; e++) W.frame_id[e] = v.frame_id[e], W.frame_node[e] = v.frame_node[e];
+        W.oK = od.K, W.oL = od.L, W.oF = od.F, W.nK = p.K, W.n_frames = v.n_frames, W.cur_node = v.cur_node;
+        W.cull_lm0 = cw.lm0, W.cull_off0 = cw.off0, W.cull_obs0 = cw.obs0, W.n_cull_obs = nco, W.obs_factor0 = (int) n_ofac;
+        W.n_obs = v.n_obs, W.n_in = v.obs_src ? v.n_in : v.n_obs, W.dev_n = v.dev_n, W.src = v.obs_src, W.obs_node = v.obs_node, W.obs_lm = v.obs_lm;
+        W.obs_xy = v.obs_undis_xy, W.obs_vel = v.obs_vel;
+        W.n_new = v.n_new, W.dev_new_n = v.dev_new_n, W.new_depth = v.new_depth, W.new_vel_ref = v.new_vel_ref, W.new_vel_cur = v.new_vel_cur;
+        W.new_ref_xy = v.new_ref_undis_xy, W.new_cur_xy = v.new_cur_undis_xy, W.new_ref_frame = v.new_ref_frame_id;
+        W.lm_out = (int) n_lm, W.f_out = (int) n_f, W.nf_out = (int) n_nf, W.scr = (int) n_scr;
+        n_ofac += nco, n_lm += (size_t) od.L + v.n_new, n_f += (size_t) od.F + v.n_obs + v.n_new, n_nf += (size_t) v.n_obs + v.n_new;
+        n_scr += (size_t) od.F + 3 * (size_t) od.L + 5 * ((size_t) od.L + v.n_new) + v.n_new;  // ba_vision_build's scratch
+        if (n_ofac >= INT32_MAX / 2 || n_f >= INT32_MAX / 16 || n_scr >= INT32_MAX / 2) {
+            set_error("%s: too many rows in one call", fn);
+            return ICG_EINVAL;
+        }
+    }
+    // staging: inputs [windows | obs_factor], outputs [counts | lm_src | lm_org | f_lm | f_ref | f_obs | f_src | invdepth | new factor rows |
+    // NaN flags], then the kernel's scratch (never copied)
+    auto al = [](size_t b) { return (b + 15) & ~(size_t) 15; };
+    size_t at = 0;
+    auto take = [&](size_t bytes) {
+        const size_t o = at;
+        at += al(bytes);
+        return o;
+    };
+    const size_t b_win = take(sizeof(VisWin) * n), b_ofac = take(4 * n_ofac), in_end = at;
+    const size_t b_cnt = take(4 * VIS_COUNTS * (size_t) n), b_lms = take(4 * n_lm), b_org = take(4 * n_lm), b_flm = take(4 * n_f), b_fref = take(4 * n_f), b_fobs = take(4 * n_f),
+                 b_fsrc = take(4 * n_f), b_invd = take(8 * n_lm), b_fnew = take(112 * n_nf), b_nan = take(n_lm), out_end = at, b_scr = take(4 * n_scr);
+    cudaStream_t s = h->stream;
+    if (at > h->vis_cap) {
+        ICG_CUDA(cudaStreamSynchronize(s));
+        if (h->vis_h) cudaFreeHost(h->vis_h);
+        if (h->vis_d) cudaFree(h->vis_d);
+        h->vis_h = nullptr, h->vis_d = nullptr, h->vis_cap = 0;
+        const size_t cap = at + at / 4;
+        if (cudaMallocHost(&h->vis_h, cap) != cudaSuccess || cudaMalloc(&h->vis_d, cap) != cudaSuccess) {
+            set_error("%s: staging allocation of %zu bytes failed", fn, cap);
+            return ICG_ENOMEM;
+        }
+        h->vis_cap = cap;
+    }
+    unsigned char *H = h->vis_h, *Dv = h->vis_d;
+    memcpy(H + b_win, wins.data(), sizeof(VisWin) * n);
+    for (int w = 0; w < n; w++)
+        if (wins[w].n_cull_obs > 0) memcpy(H + b_ofac + 4 * (size_t) wins[w].obs_factor0, vis[w].obs_factor, 4 * (size_t) wins[w].n_cull_obs);
+    ICG_CUDA(cudaMemcpyAsync(Dv, H, in_end, cudaMemcpyHostToDevice, s));
+    VisArgs a;
+    a.win = (const VisWin *) (Dv + b_win), a.K = C.K, a.L = C.L, a.F = C.F;
+    a.rho = h->D.rho, a.lm_ref = h->lm_ref, a.lm_ref_next = h->lm_ref_alt, a.f_meta_s = h->D.f_meta_s, a.lm_off = h->D.lm_off, a.lm_perm = h->D.lm_perm;
+    a.lm_ref_node = (const int *) (h->cull_d + h->cull_res_ref), a.obs_off = (const int *) (h->cull_d + h->cull_res_off);
+    a.lm_outlier = h->cull_d + h->cull_res_lmo, a.obs_outlier = h->cull_d + h->cull_res_obso, a.obs_factor = (const int *) (Dv + b_ofac);
+    a.counts = (int *) (Dv + b_cnt), a.lm_src = (int *) (Dv + b_lms), a.lm_org = (int *) (Dv + b_org), a.lm_nan = Dv + b_nan, a.f_lm = (int *) (Dv + b_flm), a.f_ref = (int *) (Dv + b_fref);
+    a.f_obs = (int *) (Dv + b_fobs), a.f_src = (int *) (Dv + b_fsrc), a.invdepth = (double *) (Dv + b_invd), a.f_new = (double *) (Dv + b_fnew);
+    a.scratch = (int *) (Dv + b_scr);
+    ICG_CUDA(cudaMemsetAsync(Dv + b_cnt, 0, 4 * VIS_COUNTS * (size_t) n, s));
+    ICG_CUDA(launch_vision(a, n, s));
+    count_launch();
+    ICG_CUDA(cudaMemcpyAsync(H + b_cnt, Dv + b_cnt, out_end - b_cnt, cudaMemcpyDeviceToHost, s));
+    ICG_CUDA(cudaStreamSynchronize(s));
+    // the built windows: every check, then the slide of next with these vision rows
+    static const char *what[] = {"", "obs_factor names no factor of the old window", "a device count is outside its list", "obs_src is out of range",
+                                 "a node is out of range", "obs_lm is out of range", "two observations of one landmark in one node",
+                                 "a reference frame id is not in the frame table", "a landmark whose reference row is unknown takes a new observation"};
+    std::vector<icg_ba_problem> nx(next, next + n);
+    std::vector<icg_ba_slide_window> cr(carry, carry + n);
+    std::vector<std::unique_ptr<double[]>> fc_tmp(n);
+    const int *cnt = (const int *) (H + b_cnt);
+    for (int w = 0; w < n; w++) {
+        const int *c = cnt + VIS_COUNTS * w;
+        if (c[3] != 0) {
+            set_error("%s: window %d: %s (entry %d)", fn, w, c[3] > 0 && c[3] <= VIS_EROW ? what[c[3]] : "?", c[4]);
+            return ICG_EINVAL;
+        }
+        if (c[0] > C.L || c[1] > C.F) {
+            set_error("%s: window %d: the next window has %d landmarks and %d factors, the handle holds %d / %d", fn, w, c[0], c[1], C.L, C.F);
+            return ICG_EINVAL;
+        }
+    }
+    for (int w = 0; w < n; w++) {
+        const int *c = cnt + VIS_COUNTS * w;
+        const VisWin &W = wins[w];
+        icg_ba_slide_vision &v = vis[w];
+        icg_ba_problem &p = nx[w];
+        const int L = c[0], F = c[1];
+        int *lm_src = (int *) (H + b_lms) + W.lm_out, *f_src = (int *) (H + b_fsrc) + W.f_out;
+        p.L = L, p.F = F, p.invdepth = (double *) (H + b_invd) + W.lm_out, p.f_active = nullptr;
+        p.f_lm = (int *) (H + b_flm) + W.f_out, p.f_ref = (int *) (H + b_fref) + W.f_out, p.f_obs = (int *) (H + b_fobs) + W.f_out;
+        double *fc = v.f_const;
+        if (!fc) fc_tmp[w].reset(new double[14 * (size_t) std::max(F, 1)]), fc = fc_tmp[w].get();
+        const double *rows = (const double *) (H + b_fnew) + 14 * (size_t) W.nf_out;
+        for (int f = 0, t = 0; f < F; f++)
+            if (f_src[f] < 0) memcpy(fc + 14 * (size_t) f, rows + 14 * (size_t) t++, 112);
+        p.f_const = fc;
+        cr[w].lm_src = lm_src, cr[w].f_src = f_src;
+        v.L = L, v.F = F, v.nan_dropped = c[5];
+        if (v.lm_src) memcpy(v.lm_src, lm_src, 4 * (size_t) L);
+        if (v.lm_origin) memcpy(v.lm_origin, (int *) (H + b_org) + W.lm_out, 4 * (size_t) L);
+        if (v.nan_flags) memcpy(v.nan_flags, H + b_nan + W.lm_out, (size_t) W.oL + W.n_new);
+        if (v.f_src) memcpy(v.f_src, f_src, 4 * (size_t) F);
+        if (v.f_lm) memcpy(v.f_lm, p.f_lm, 4 * (size_t) F);
+        if (v.f_ref) memcpy(v.f_ref, p.f_ref, 4 * (size_t) F);
+        if (v.f_obs) memcpy(v.f_obs, p.f_obs, 4 * (size_t) F);
+        if (v.invdepth) memcpy(v.invdepth, p.invdepth, 8 * (size_t) L);
+    }
+    return slide_body(h, n, nx.data(), cr.data(), integ, noise5, station3, fn, false, true);
 }
 
 int icg_ba_shard_slide_resident(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba_slide_window *carry) {

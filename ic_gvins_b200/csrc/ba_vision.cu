@@ -1,0 +1,212 @@
+// ba_vision.cu -- the device half of icg_ba_slide_vision_resident (ba_vision.cuh).  One CTA per window: the structure of one window is small
+// (a few thousand landmarks and factors) and windows are independent, as in the slide's gather.  Built with -fmad=false: pixel2cam is a
+// subtract and a divide on the host, and must stay so here.
+#include <cub/block/block_scan.cuh>
+
+#include "ba_vision.cuh"
+#include "geom_core.cuh"
+
+namespace icg {
+
+namespace {
+
+using Scan = cub::BlockScan<int, VIS_THREADS>;
+
+// in-place exclusive prefix sum of a[0 .. n) by the whole CTA (each thread a contiguous chunk, one block scan of the chunk sums); returns the total
+__device__ int block_exscan(int *a, int n, Scan::TempStorage &tmp) {
+    const int chunk = (n + VIS_THREADS - 1) / VIS_THREADS, b = threadIdx.x * chunk, e = min(n, b + chunk);
+    int s = 0;
+    for (int i = b; i < e; i++) s += a[i];
+    int base, total;
+    Scan(tmp).ExclusiveSum(s, base, total);
+    for (int i = b; i < e; i++) {
+        const int v = a[i];
+        a[i] = base, base += v;
+    }
+    __syncthreads();
+    return total;
+}
+
+__device__ void fail(int *cnt, int code, int idx) {
+    if (atomicCAS(cnt + 3, 0, code) == 0) cnt[4] = idx;
+}
+
+__device__ double carried_invdepth(double rho) { return __ddiv_rn(1.0, __ddiv_rn(1.0, rho)); }
+
+__device__ void cam_point(const icg_camera &c, float u, float v, double *p) {
+    gc::pixel2cam(c, u, v, p[0], p[1]);
+    p[2] = 1.0;
+}
+
+}  // namespace
+
+// Rules (include/icgvins_b200.h, icg_ba_slide_vision_resident): landmark l of the old window is carried when it is not a culling outlier, its
+// reference node is usable (in the map, not marginalized, kept by the slide) and 1 / (1 / rho) is not NaN; its old factors survive when their
+// observation is listed by the culling and not an outlier and their observing node is usable; its new observations follow in node order.  New map
+// points follow the carried landmarks in creation order, each with one factor from its reference node to the current node.
+__global__ void __launch_bounds__(VIS_THREADS) ba_vision_build(VisArgs a) {
+    __shared__ Scan::TempStorage tmp;
+    __shared__ int s_nobs, s_nnew;
+    const int w = blockIdx.x, t = threadIdx.x;
+    const VisWin &W = a.win[w];
+    const int oK = W.oK, oL = W.oL, oF = W.oF;
+    int *cnt = a.counts + (size_t) w * VIS_COUNTS;
+    const size_t wL = (size_t) w * a.L, wF = (size_t) w * a.F;
+    const int *meta = a.f_meta_s + wF * 4, *off = a.lm_off + (size_t) w * (a.L + 1), *perm = a.lm_perm + wL;
+    const double *rho = a.rho + wL;
+    const int *ref_node = a.lm_ref_node + W.cull_lm0;
+    const uint8_t *lm_out = a.lm_outlier + W.cull_lm0, *obs_out = a.obs_outlier + W.cull_obs0;
+    const int *ofac = a.obs_factor + W.obs_factor0;
+    if (t == 0) {
+        int n = W.dev_n ? *W.dev_n : W.n_obs, m = W.dev_new_n ? *W.dev_new_n : W.n_new;
+        if (n < 0 || n > W.n_obs) fail(cnt, VIS_ECOUNT, n), n = 0;
+        if (m < 0 || m > W.n_new) fail(cnt, VIS_ECOUNT, m), m = 0;
+        s_nobs = n, s_nnew = m;
+    }
+    // scratch (vis_scratch_ints): fkeep (oF) | pos_of (oL) | mask (oL) | nkeep (oL) | keep, nn, lidx, fbase, nbase (oL + n_new each) | ref node
+    // of each new point (n_new)
+    const int NA = oL + W.n_new;
+    int *fkeep = a.scratch + W.scr, *pos_of = fkeep + oF, *mask = pos_of + oL, *nkeep = mask + oL;
+    int *keep = nkeep + oL, *nn = keep + NA, *lidx = nn + NA, *fbase = lidx + NA, *nbase = fbase + NA, *new_ref = nbase + NA;
+    const double *lref = a.lm_ref + wL * 7;
+    double *lref_next = a.lm_ref_next + wL * 7;
+    uint8_t *lm_nan = a.lm_nan + W.lm_out;
+    for (int q = t; q < oF; q += VIS_THREADS) fkeep[q] = 0;
+    for (int p = t; p < oL; p += VIS_THREADS) pos_of[perm[p]] = p, mask[perm[p]] = 0;
+    __syncthreads();
+    const int nobs = s_nobs, nnew = s_nnew;
+    // 1. flags: the factors the culling's observations keep, the carried landmarks, the new points' reference nodes
+    for (int o = t; o < W.n_cull_obs; o += VIS_THREADS) {
+        const int f = ofac[o];
+        if (f < -1 || f >= oF) fail(cnt, VIS_EOBS_FACTOR, o);
+        else if (f >= 0) fkeep[f] = obs_out[o] == 0;
+    }
+    int nan_drops = 0;
+    for (int l = t; l < oL; l += VIS_THREADS) {
+        const int r = ref_node[l];
+        const bool nan = isnan(carried_invdepth(rho[l]));
+        const bool k = lm_out[l] == 0 && r >= 0 && r < oK && W.onode[r] >= 0;
+        keep[l] = k && !nan;
+        lm_nan[l] = k && nan;
+        nan_drops += k && nan;
+    }
+    for (int j = t; j < NA - oL; j += VIS_THREADS) {
+        keep[oL + j] = 0, lm_nan[oL + j] = 0;
+        if (j >= nnew) {
+            new_ref[j] = -1;
+            continue;
+        }
+        const int64_t id = W.new_ref_frame[j];
+        int node = -1;
+        for (int e = 0; e < W.n_frames; e++)
+            if (W.frame_id[e] == id) node = W.frame_node[e];
+        if (node < 0) fail(cnt, VIS_EFRAME, j);
+        new_ref[j] = node;
+        const bool nan = isnan(__ddiv_rn(1.0, W.new_depth[j]));
+        keep[oL + j] = node >= 0 && !nan;
+        lm_nan[oL + j] = node >= 0 && nan;
+        nan_drops += node >= 0 && nan;
+    }
+    __syncthreads();
+    // the new observations: one bit per (landmark, next node); a second observation of a landmark in one node is an error
+    for (int k = t; k < nobs; k += VIS_THREADS) {
+        const int j = W.src ? W.src[k] : k;
+        if (j < 0 || j >= W.n_in) {
+            fail(cnt, VIS_ESRC, k);
+            continue;
+        }
+        const int l = W.obs_lm[j], node = W.obs_node ? W.obs_node[j] : W.cur_node;
+        if (node < 0 || node >= W.nK) fail(cnt, VIS_ENODE, k);
+        else if (l < -1 || l >= oL) fail(cnt, VIS_ELM, k);
+        else if (l >= 0 && keep[l] && W.onode[ref_node[l]] != node && (atomicOr((unsigned *) mask + l, 1u << node) >> node) & 1u) fail(cnt, VIS_EDUP, k);
+    }
+    __syncthreads();
+    // 2. counts per landmark (factors, new factors) and the three dense numberings
+    for (int i = t; i < NA; i += VIS_THREADS) {
+        int s = 0, m = 0;
+        if (i < oL && keep[i]) {
+            const int p = pos_of[i];
+            for (int q = off[p]; q < off[p + 1]; q++) s += fkeep[meta[4 * q + 3]] && W.onode[meta[4 * q + 2]] >= 0;
+            m = __popc(mask[i]);
+            if (m > 0 && isnan(lref[(size_t) i * 7])) fail(cnt, VIS_EROW, i);
+            nkeep[i] = s;
+        } else if (i >= oL && keep[i]) {
+            m = new_ref[i - oL] != W.cur_node;
+        }
+        nn[i] = m, lidx[i] = keep[i], fbase[i] = s + m, nbase[i] = m;
+    }
+    __syncthreads();
+    const int L = block_exscan(lidx, NA, tmp), F = block_exscan(fbase, NA, tmp), N = block_exscan(nbase, NA, tmp);
+    {
+        int before;
+        Scan(tmp).ExclusiveSum(nan_drops, before, nan_drops);
+    }
+    if (t == 0) cnt[0] = L, cnt[1] = F, cnt[2] = N, cnt[5] = nan_drops;
+    // 3. the rows: carried landmarks and factors, new map points with their factor
+    int *lm_src = a.lm_src + W.lm_out, *lm_org = a.lm_org + W.lm_out, *f_lm = a.f_lm + W.f_out, *f_ref = a.f_ref + W.f_out, *f_obs = a.f_obs + W.f_out, *f_src = a.f_src + W.f_out;
+    double *invd = a.invdepth + W.lm_out, *fnew = a.f_new + (size_t) W.nf_out * 14;
+    for (int i = t; i < NA; i += VIS_THREADS) {
+        if (!keep[i]) continue;
+        const int li = lidx[i];
+        int fo = fbase[i];
+        double *row = li < a.L ? lref_next + (size_t) li * 7 : nullptr;  // a window beyond the handle's capacity is rejected afterwards
+        if (i < oL) {
+            const double v = carried_invdepth(rho[i]);
+            lm_src[li] = v == 0.0 ? -1 : i;  // addReprojectionFactors: 0 -> 1 / MapPoint::DEFAULT_DEPTH, staged as a new row
+            lm_org[li] = i;
+            invd[li] = v == 0.0 ? 0.1 : v;
+            for (int c = 0; row && c < 7; c++) row[c] = lref[(size_t) i * 7 + c];
+            const int p = pos_of[i], r = W.onode[ref_node[i]];
+            for (int q = off[p]; q < off[p + 1]; q++) {
+                const int f = meta[4 * q + 3], ob = W.onode[meta[4 * q + 2]];
+                if (!fkeep[f] || ob < 0) continue;
+                f_lm[fo] = li, f_ref[fo] = r, f_obs[fo] = ob, f_src[fo] = f;
+                fo++;
+            }
+        } else {
+            const int j = i - oL;
+            const double v = __ddiv_rn(1.0, W.new_depth[j]);
+            const int r = new_ref[j];
+            lm_src[li] = -1, lm_org[li] = -(j + 1);
+            invd[li] = v == 0.0 ? 0.1 : v;
+            if (row) {
+                cam_point(W.cam, W.new_ref_xy[2 * j], W.new_ref_xy[2 * j + 1], row);
+                row[3] = W.new_vel_ref[2 * j], row[4] = W.new_vel_ref[2 * j + 1], row[5] = 0.0, row[6] = W.node_td[r];
+            }
+            if (nn[i] == 0) continue;
+            f_lm[fo] = li, f_ref[fo] = r, f_obs[fo] = W.cur_node, f_src[fo] = -1;
+            double *c = fnew + (size_t) nbase[i] * 14;
+            cam_point(W.cam, W.new_ref_xy[2 * j], W.new_ref_xy[2 * j + 1], c);
+            cam_point(W.cam, W.new_cur_xy[2 * j], W.new_cur_xy[2 * j + 1], c + 3);
+            c[6] = W.new_vel_ref[2 * j], c[7] = W.new_vel_ref[2 * j + 1], c[8] = 0.0;
+            c[9] = W.new_vel_cur[2 * j], c[10] = W.new_vel_cur[2 * j + 1], c[11] = 0.0;
+            c[12] = W.node_td[r], c[13] = W.node_td[W.cur_node];
+        }
+    }
+    // the new observations of carried landmarks, after the landmark's surviving old factors, in node order, with the landmark's resident
+    // reference row (pts0, vel0, td0)
+    for (int k = t; k < nobs; k += VIS_THREADS) {
+        const int j = W.src ? W.src[k] : k;
+        if (j < 0 || j >= W.n_in) continue;
+        const int l = W.obs_lm[j], node = W.obs_node ? W.obs_node[j] : W.cur_node;
+        if (node < 0 || node >= W.nK || l < 0 || l >= oL || !keep[l] || W.onode[ref_node[l]] == node) continue;
+        const double *r0 = lref + (size_t) l * 7;
+        if (isnan(r0[0])) continue;
+        const int rank = __popc(mask[l] & ((1u << node) - 1u));
+        const int fo = fbase[l] + nkeep[l] + rank;
+        f_lm[fo] = lidx[l], f_ref[fo] = W.onode[ref_node[l]], f_obs[fo] = node, f_src[fo] = -1;
+        double *c = fnew + (size_t) (nbase[l] + rank) * 14;
+        c[0] = r0[0], c[1] = r0[1], c[2] = r0[2];
+        cam_point(W.cam, W.obs_xy[2 * k], W.obs_xy[2 * k + 1], c + 3);
+        c[6] = r0[3], c[7] = r0[4], c[8] = r0[5];
+        c[9] = W.obs_vel[2 * k], c[10] = W.obs_vel[2 * k + 1], c[11] = 0.0;
+        c[12] = r0[6], c[13] = W.node_td[node];
+    }
+}
+
+cudaError_t launch_vision(const VisArgs &a, int n_windows, cudaStream_t stream) {
+    ba_vision_build<<<n_windows, VIS_THREADS, 0, stream>>>(a);
+    return cudaGetLastError();
+}
+
+}  // namespace icg

@@ -1,0 +1,70 @@
+// ba_vision.cuh -- the vision half of the next window (icg_ba_slide_vision_resident): GVINS::addReprojectionParameters +
+// addReprojectionFactors (IG/ic_gvins.cc:1697-1837) after Map::removeKeyFrame(frame, true) (tracking/map.cc:89-125), built on the device from
+// the culled window the handle holds and the new keyframes' observations.  The interface between the handle (ba.cu: validation, staging,
+// the slide) and the kernel (ba_vision.cu, built without FMA contraction so that pixel2cam is the host's sub-then-divide).
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "../../include/icgvins_b200.h"
+
+namespace icg {
+
+constexpr int VIS_THREADS = 256;
+constexpr int VIS_MAX_NODES = 32;   // = the handle's max_K limit (one bit per node in the per-landmark masks)
+constexpr int VIS_MAX_FRAMES = 64;  // frame id -> node table entries
+
+// one window, as staged.  Old-window arrays are the handle's (capacity-strided) and the last culling's staging; new-keyframe arrays are the
+// caller's DEVICE pointers.  Every output and scratch offset is in elements of its own array.
+struct VisWin {
+    icg_camera cam;
+    double node_td[VIS_MAX_NODES];     // next-window node -> timeDelay()
+    int8_t onode[VIS_MAX_NODES];       // old node -> next node, -1: marginalized, removed or not in the map
+    int64_t frame_id[VIS_MAX_FRAMES];  // frame table of the new map points' reference frames
+    int frame_node[VIS_MAX_FRAMES];
+    int oK, oL, oF, nK, n_frames, cur_node;
+    int cull_lm0, cull_off0, cull_obs0, n_cull_obs;  // the window's slices of the culling's staging
+    int obs_factor0;                                  // first entry of the window's obs_factor in VisArgs::obs_factor
+    // tracked observations: k < count (*dev_n when given, else n_obs), j = src ? src[k] : k (j < n_in); lm = obs_lm[j], node = obs_node[j]
+    // (obs_node NULL: cur_node); undis_xy / vel at k
+    int n_obs, n_in;
+    const int *dev_n, *src, *obs_node, *obs_lm;
+    const float *obs_xy;
+    const double *obs_vel;
+    // new map points: j < count (*dev_new_n when given, else n_new)
+    int n_new;
+    const int *dev_new_n;
+    const double *new_depth, *new_vel_ref, *new_vel_cur;
+    const float *new_ref_xy, *new_cur_xy;
+    const int64_t *new_ref_frame;
+    // bounds: next landmarks Lb = oL + n_new, next factors Fb = oF + n_obs + n_new, new factors Nb = n_obs + n_new
+    int lm_out, f_out, nf_out, scr;  // offsets of the window's output rows (Lb, Fb, Nb) and int scratch
+};
+
+// per window: [L, F, new factors, error code, error index, landmarks dropped for a NaN inverse depth]
+constexpr int VIS_COUNTS = 6;
+enum VisError { VIS_OK = 0, VIS_EOBS_FACTOR = 1, VIS_ECOUNT = 2, VIS_ESRC = 3, VIS_ENODE = 4, VIS_ELM = 5, VIS_EDUP = 6, VIS_EFRAME = 7, VIS_EROW = 8 };
+
+struct VisArgs {
+    const VisWin *win;
+    int K, L, F;  // the handle's capacities (strides of its arrays)
+    // the window the handle holds
+    const double *rho;
+    const int *f_meta_s, *lm_off, *lm_perm;
+    const double *lm_ref;  // per landmark: its reference row pts0[3] | vel0[3] | td0 (NaN: unknown), capacity-strided (7 L per window)
+    // the last culling (its staging)
+    const int *lm_ref_node, *obs_off;
+    const uint8_t *lm_outlier, *obs_outlier;
+    const int *obs_factor;
+    // outputs: counts (VIS_COUNTS per window), per next landmark lm_src, its origin (old landmark, or -(j + 1) for new map point j) and
+    // invdepth, per old landmark and new map point a NaN-drop flag (Lb bytes), per next factor f_lm / f_ref / f_obs / f_src, per new factor
+    // its 14 constants (the new factors in factor order); lm_ref_next: the next window's reference rows (capacity-strided, as lm_ref)
+    int *counts, *lm_src, *lm_org, *f_lm, *f_ref, *f_obs, *f_src;
+    uint8_t *lm_nan;
+    double *invdepth, *f_new, *lm_ref_next;
+    int *scratch;
+};
+
+cudaError_t launch_vision(const VisArgs &a, int n_windows, cudaStream_t stream);
+
+}  // namespace icg

@@ -311,6 +311,23 @@ public:
         c.prior_from_marg = prior_from_marginalization ? 1 : 0;
         check(icg_ba_slide_integrate_resident(h_, 1, &next, &c, &integrate, noise5, station), "icg_ba_slide_integrate_resident");
     }
+    // The same again with the vision half built on the device in place of addReprojectionParameters + addReprojectionFactors
+    // (IG/ic_gvins.cc:1697-1837): see icg_ba_slide_vision.  carry.lm_src / f_src and next's vision rows are not read; integrate may be null
+    // (no IMU row integrated).  The last updateAndCull on this solver must be current.  On return next.L / F and, where `vision` names
+    // output arrays, next's invdepth / f_lm / f_ref / f_obs / f_const point at them (f_active all active), so gvinsOptimizationResident(next)
+    // writes the solved inverse depths there; vision.lm_origin / nan_flags say which MapPoint each row is and which ones to set outliers.
+    void slideVision(icg_ba_problem &next, const Carry &carry, bool prior_from_marginalization, icg_ba_slide_vision &vision,
+                     icg_ba_slide_integrate *integrate = nullptr, const double noise5[5] = nullptr, const double station[3] = nullptr) {
+        icg_ba_slide_window c = carryStruct(next, Carry{carry.node_src, {}, {}, carry.imu_src, carry.gnss_src});
+        c.prior_from_marg = prior_from_marginalization ? 1 : 0;
+        check(icg_ba_slide_vision_resident(h_, 1, &next, &c, integrate, noise5, station, &vision), "icg_ba_slide_vision_resident");
+        next.L = vision.L, next.F = vision.F, next.f_active = nullptr;
+        if (vision.invdepth) next.invdepth = vision.invdepth;
+        if (vision.f_lm) next.f_lm = vision.f_lm;
+        if (vision.f_ref) next.f_ref = vision.f_ref;
+        if (vision.f_obs) next.f_obs = vision.f_obs;
+        if (vision.f_const) next.f_const = vision.f_const;
+    }
     // the two-pass body of gvinsOptimization on the window slideWindow left (nothing is uploaded); results as gvinsOptimization gives them
     void gvinsOptimizationResident(const icg_ba_problem &next, int num_iterations, icg_ba_summary out[2], int32_t culled[2]) {
         check(icg_ba_run_gvins(h_, num_iterations, 0), "icg_ba_run_gvins");

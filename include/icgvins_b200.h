@@ -707,6 +707,78 @@ typedef struct icg_ba_slide_integrate {
 int icg_ba_slide_integrate_resident(icg_ba *h, int n_windows, const icg_ba_problem *next, const icg_ba_slide_window *carry,
                                     const icg_ba_slide_integrate *integ, const double *noise5, const double *station3);
 /*
+ * icg_ba_slide_integrate_resident (integ NULL: icg_ba_slide_resident) whose vision rows are built on the device: GVINS::addReprojectionParameters
+ * + addReprojectionFactors (IG/ic_gvins.cc:1697-1837) on the map after the culling and Map::removeKeyFrame(frame, true) (tracking/map.cc:89-125,
+ * called at :1675), from the culled window the handle holds and the new keyframes' observations.  next.L, F, invdepth, f_lm / f_ref / f_obs /
+ * f_const, f_active and carry.lm_src / f_src are NOT read: the call builds them.  Everything else of next and carry keeps its meaning.
+ * The old window is the one the handle holds; the culling outcome is the last icg_ba_update_and_cull_resident on this handle, which must still be
+ * current (no upload or slide since, the same n_windows): the handle keeps its landmark and observation flags on the device for this call.
+ * Landmarks of the next window:
+ *   carried first, in old order: landmark l is carried when it is not a culling outlier, its reference node (the culling's lm_ref_node) is
+ *     >= num_marg, set in node_in_map and kept by carry.node_src, and its inverse depth 1.0 / (1.0 / rho) is not NaN (a NaN drops it and is counted
+ *     in nan_dropped and flagged in nan_flags: the caller marks the map point an outlier); a 0 becomes 1 / 10 (MapPoint::DEFAULT_DEPTH): its
+ *     row is then staged (lm_src -1) and lm_origin still names the old landmark;
+ *   then the new map points in creation order, invdepth = 1.0 / depth under the same two rules.
+ * Factors, landmark by landmark (f_lm non-decreasing):
+ *   the landmark's surviving old factors in old order: the culling lists the factor's observation (obs_factor) and did not mark it an outlier,
+ *     and its observing node is usable as above (the reference node never observes: the reference skips it).  The chi-square pass's removals
+ *     come back: every factor of the next window is active;
+ *   then its new observations in node order: pts0 / vel0 / td0 from the landmark's reference row, pts1 = pixel2cam(undis_xy) (geom_core, as
+ *     icg_camera_pixel2cam), vel1 = (vx, vy, 0),
+ *     td1 = node_td[node].  An observation of a landmark that is not carried, or in its reference node, is skipped;
+ *   a new map point: one factor from its reference node (frame table) to cur_node, pts = pixel2cam of the two keypoints, vel = (v, 0), td from
+ *     node_td; none when the two nodes are the same.
+ * Reference rows.  The handle keeps every landmark's reference row (pts0, vel0, td0 = pixel2cam(referenceKeypoint()), the reference feature's
+ * velocity, the reference frame's timeDelay()), so that a landmark whose factors were all dropped can still take a new observation:
+ * icg_ba_upload sets it from the landmark's first factor (unknown, NaN, for a landmark uploaded without factors), every slide carries it with
+ * the landmark (a landmark that carry.lm_src names keeps its old row; a new one takes its first factor's), and this call writes a new map
+ * point's from its reference keypoint, velocity and node_td.  A new observation of a landmark whose row is unknown is ICG_EINVAL.
+ * The reference's order is unordered_map iteration (implementation-defined); this order is fixed and only permutes rows.
+ * One CTA per window builds the structure on the device; the counts, the integer structure, the new invdepth rows and the new factors' constants
+ * come back in one copy (one synchronisation), and the call goes on as icg_ba_slide_integrate_resident with that window, every check included.
+ * A rejected call (ICG_EINVAL: max_L / max_F exceeded, a reference frame id missing from the table, a node, landmark or source index out of
+ * range, a count outside its list, two observations of one landmark in one node) leaves the handle as it was.  Afterwards the handle cannot be
+ * told apart from one that called icg_ba_slide_integrate_resident with the same next whose vision rows were built on the host by these rules.
+ * ICG_EUNSUPPORTED on a landmark-sharded handle.
+ */
+typedef struct icg_ba_slide_vision {
+    /* in: the old window */
+    int32_t num_marg;
+    const uint8_t *node_in_map;  /* old K: isKeyFrameInMap after gvinsRemoveAllSecondNewFrame */
+    const int32_t *obs_factor;   /* the culling's observations (its obs_off order): factor of each, -1 for none */
+    /* in: the new keyframes */
+    icg_camera cam;
+    const double *node_td;       /* next.K: frame->timeDelay() */
+    int32_t cur_node;            /* next-window node of the current frame */
+    int32_t n_frames;            /* <= 64 */
+    const int64_t *frame_id;     /* HOST n_frames: frame id -> */
+    const int32_t *frame_node;   /* HOST n_frames:   next-window node */
+    /* tracked map-point observations (DEVICE): k < count (*dev_n when dev_n is not NULL, else n_obs; a count outside [0, n_obs] is an error),
+       j = obs_src ? obs_src[k] : k (< n_in): landmark obs_lm[j] (old landmark, -1: not in the window), node obs_node[j] (NULL: cur_node),
+       undis_xy[2 k] (feat->keyPoint()), vel[2 k]; icg_klt_track_frames_dev's compacted map list plugs in with obs_src = its src and
+       dev_n = dev_n_out + 2 s */
+    int32_t n_obs, n_in;
+    const int32_t *dev_n, *obs_src, *obs_lm, *obs_node;
+    const float *obs_undis_xy;
+    const double *obs_vel;
+    /* new map points (DEVICE, icg_tri_new's arrays at the stream's offset): count *dev_new_n (dev_counts + 5 s + 1) or n_new */
+    int32_t n_new;
+    const int32_t *dev_new_n;
+    const double *new_depth, *new_vel_ref, *new_vel_cur;
+    const float *new_ref_undis_xy, *new_cur_undis_xy;
+    const int64_t *new_ref_frame_id;
+    /* out */
+    int32_t L, F, nan_dropped;
+    int32_t *lm_src, *f_src, *f_lm, *f_ref, *f_obs; /* HOST, each may be NULL: max_L / max_F entries (lm_src / f_src as carry takes them) */
+    int32_t *lm_origin;                             /* HOST or NULL: max_L, every next landmark's origin: old landmark l, or -(j + 1) for new point j */
+    uint8_t *nan_flags;                             /* HOST or NULL: old L + n_new, 1 where the landmark / new point was dropped for a NaN inverse
+                                                       depth (the caller sets that MapPoint an outlier, IG/ic_gvins.cc:1720-1724) */
+    double *invdepth;                               /* HOST or NULL: max_L, the landmarks' inverse depths (carried ones as the slide computes them) */
+    double *f_const;                                /* HOST or NULL: max_F x 14, the rows of the new factors (f_src = -1); carried rows are not written */
+} icg_ba_slide_vision;
+int icg_ba_slide_vision_resident(icg_ba *h, int n_windows, const icg_ba_problem *next, const icg_ba_slide_window *carry,
+                                 const icg_ba_slide_integrate *integ, const double *noise5, const double *station3, icg_ba_slide_vision *vis);
+/*
  * The reintegration and the two slides on a landmark-sharded handle (world > 1): doReintegration (IG/ic_gvins.cc:1680-1695) and the time-node
  * edits and next window of gvinsOptimization (:754-928, 1697-1837), as icg_ba_reintegrate_resident, icg_ba_slide_resident and
  * icg_ba_slide_integrate_resident describe them, with the same structs.  Each is a COLLECTIVE call: every rank of the group calls it with its
