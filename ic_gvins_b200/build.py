@@ -27,6 +27,8 @@ SOURCES = {
     "geom.cu": ["-fmad=false"],         # device versions of the camera model / RANSAC gate / triangulation / IMU propagation (same cores)
     "track.cu": ["-fmad=false"],       # trackMappoint / trackReferenceFrame on the KLT handle (geom_core.cuh arithmetic)
     "ba.cu": [],
+    "ba_handle.cu": [],                # host side of the window solve: handle lifecycle, upload, LM sequences, shard-group plumbing
+    "ba_keyframe.cu": [],              # host side of the resident keyframe cycle: culling, reintegration, marginalization, slides
     "ba_cull.cu": ["-fmad=false"],     # post-solve map update and outlier culling (fixed-order sums, as the numpy restatement)
     "preint.cu": ["-fmad=false"],      # IMU propagation, warp per interval: the sums of geom_core.cuh's preintegrate_core, bit for bit
     "ba_slide.cu": ["-fmad=false"],    # slide to the next window: the prior's normal equations are icg_ba_upload's host sums, bit for bit

@@ -23,23 +23,6 @@
 namespace icg {
 
 constexpr double MARG_EPS = 1e-8;  // MarginalizationInfo::EPS (marginalization_info.h:256)
-constexpr int MARG_THREADS = 512;
-constexpr int MARG_MAP_HDR = 8;    // [m, r, n0, num_marg, ext_col, td_col, -, -] then pose_col[K], mix_col[K], lm_col[L]
-
-struct MargDev {
-    int *map;        // [NW][MARG_MAP_HDR + 2*K + L]
-    int map_stride;
-    double *H0, *b0; // [NW][n0cap^2], [NW][n0cap]
-    double *G1, *V1; // [NW][mcap^2] each: Jacobi workspace of Hmm
-    double *G2, *V2; // [NW][rcap^2] each: Jacobi workspace of Hp
-    double *lam1, *lam2;  // eigenvalues
-    double *Z;       // [NW][mcap * (rcap + 1)]
-    double *Hp, *bp; // [NW][rcap^2], [NW][rcap]
-    double *J0, *e0; // outputs
-    int *flags;      // [NW][4] saved dims flags
-    int n0cap, mcap, rcap;
-};
-
 __global__ void marg_prepare(BaDev D, MargDev M, int n, int restore) {
     const int w = blockIdx.x * blockDim.x + threadIdx.x;
     if (w >= n) return;
@@ -324,7 +307,6 @@ __global__ void __launch_bounds__(MARG_THREADS) marg_jacobi(MargDev M, int which
 // applies the list while CTA 0 already works on the next step (two record slots, one cluster barrier per step).  No L2 round trip sits on
 // the rotation loop any more (the global-memory kernel above pays two per rotation); same rotation formula, ordering and stopping rule, so
 // the decomposition is the same up to rounding.  lambda_i = v_i . g_i is formed by CTA 1 reading G over DSMEM once at the end.
-constexpr int MARG_PAIR_MAXN = 160;  // 160^2 doubles = 204.8 KB per CTA
 __global__ void __launch_bounds__(MARG_THREADS) marg_jacobi_pair(MargDev M, int which) {
     extern __shared__ double sm_mat[];  // CTA 0: G; CTA 1: V   (n x n, column-major), then the two rotation-record slots (CTA 1)
     cg::cluster_group cluster = cg::this_cluster();
@@ -477,8 +459,6 @@ __global__ void __launch_bounds__(MARG_THREADS) marg_jacobi_pair(MargDev M, int 
 // gives m = 15 + its landmarks and r <= 70): ONE CTA per window with G = A V and V both in shared memory, eight lanes per column pair (four pairs
 // per warp share the warp-wide scalar chain; all n/2 pairs of a round-robin step run in one round), one block barrier per step.  Against the
 // cluster-pair kernel: no cluster barrier on the step, and the grid needs half the CTAs.
-constexpr int MARG_CTA_MAXN = 118;     // 2 * 118^2 doubles = 222.8 KB
-constexpr int MARG_CTA_THREADS = 512;  // 64 pair slots >= MARG_CTA_MAXN / 2
 __global__ void __launch_bounds__(MARG_CTA_THREADS) marg_jacobi_cta(MargDev M, int which) {
     extern __shared__ double sm_mat[];  // G | V (n x n each, column-major)
     __shared__ int s_any[2];
@@ -574,14 +554,6 @@ __global__ void __launch_bounds__(MARG_CTA_THREADS) marg_jacobi_cta(MargDev M, i
 //   4. every CTA rotates its own rows of G and V; a block barrier separates them from the next step's partials.
 // The slots are double-buffered by step parity: a slot is rewritten two steps later, after every CTA has passed the barrier that follows its
 // reads, so one cluster barrier per step is enough.  lambda_j = v_j . g_j is summed from rank-ordered per-CTA partials.
-constexpr int MARG_CLUSTER_MAXN = 320;
-constexpr int MARG_CLUSTER_CTAS = 8;                       // portable maximum cluster size
-constexpr int MARG_CLUSTER_THREADS = 640;                  // 160 four-lane groups: one per pair of a step at n = 320
-constexpr int MARG_CLUSTER_SLOT = 3 * (MARG_CLUSTER_MAXN / 2);  // (al, be, ga) per pair
-__host__ __device__ constexpr int marg_cluster_rows(int n) { return (n + MARG_CLUSTER_CTAS - 1) / MARG_CLUSTER_CTAS; }
-__host__ __device__ constexpr size_t marg_cluster_smem(int n) {
-    return sizeof(double) * (2 * (size_t) marg_cluster_rows(n) * n + 2 * (size_t) MARG_CLUSTER_SLOT);
-}
 __global__ void __launch_bounds__(MARG_CLUSTER_THREADS) marg_jacobi_cluster(MargDev M, int which) {
     extern __shared__ double sm_mat[];  // G slice | V slice (n columns of R8 rows each) | partial slots [2][MARG_CLUSTER_SLOT]
     __shared__ int s_any[2];

@@ -29,11 +29,6 @@
 namespace icg {
 namespace cg = cooperative_groups;
 
-constexpr int SPLIT_CLUSTER = 4;      // CTAs per window in ba_solve_cam
-constexpr int SPLIT_HDR = 16;         // header doubles of the step broadcast
-constexpr int SPLIT_SCAL = 8;         // doubles per (window, rank) slot of the scalar exchange
-constexpr int SPLIT_BS_ROWS = 32;     // rows per block of the blocked back-substitution
-
 __device__ __forceinline__ unsigned long long ld_acquire_sys(const unsigned long long *p) {
     unsigned long long v;
     asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
@@ -118,8 +113,6 @@ __global__ void __launch_bounds__(256) ba_reduce(BaCaps C, BaDev D, unsigned lon
         rv[3 * NCV + 2] = m;
     }
 }
-
-__host__ __device__ inline size_t split_S_stride(const BaCaps &C) { return (size_t) (C.N + 1) * (C.N + 2) / 2 + (size_t) C.NS; }
 
 // ------------------------------------------------------------------------------------------------ solve_cam (owner, cluster per window)
 // The camera-side half of ba_solve for systems that do not fit one CTA: S lives packed in global memory (L2-resident, written and read by all
@@ -469,20 +462,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS) ba_solve_cam(BaCaps C, BaDev D,
 // row's contributions to its own partial sums for the columns on the left and pushes the partial sums of the next three tile rows (final by
 // construction: its next own tile row is T - 4) to their owners' inboxes with st.async, each inbox counted by an mbarrier (point to point, no
 // cluster barrier on the chain).
-constexpr int DSM_CL = 4;
-static_assert(SOLVE_THREADS == 256 && DSM_CL == SPLIT_CLUSTER, "ba_solve_cam_dsm: warp r assembles row r of a tile row; one launch geometry for both forms");
 __host__ __device__ inline int dsm_tile_off(int cr, int m) { return m * cr + 2 * m * (m - 1); }  // tiles ahead of local tile row m (T = cr + 4 m)
-__host__ __device__ constexpr int dsm_ntiles(int NR) { return (NR + 7) / 8; }
-__host__ inline size_t dsm_smem_doubles(const BaCaps &C) {
-    const int nt = dsm_ntiles(C.N + 1);
-    int mx = 0;
-    for (int cr = 0; cr < DSM_CL; cr++) {
-        int s = 0;
-        for (int T = cr; T < nt; T += DSM_CL) s += T;
-        mx = s > mx ? s : mx;
-    }
-    return 40 + 8 * (size_t) nt * 8 + 64 + 8 + 8 * DSM_CL + 8 + 8 + (size_t) nt * 64 * 3 + (size_t) mx * 64;
-}
 
 // ---- distributed-shared-memory plumbing: cluster addresses, mbarriers with transaction counts, asynchronous remote stores
 __device__ __forceinline__ unsigned mapa_u32(unsigned addr, unsigned rank) {
@@ -969,7 +949,6 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 1) ba_solve_cam_dsm(BaCaps C, B
 // STEP_SLICES contiguous landmark slices, one CTA each; slice 0 also forms the candidate camera blocks.  The slices' partial sums meet in
 // slot order in the CTA that finishes last (a per-window counter that resets itself): the same bits whatever the arrival order and whatever
 // the batch size.
-constexpr int STEP_SLICES = 4;
 __global__ void __launch_bounds__(SOLVE_THREADS) ba_step_lm(BaCaps C, BaDev D, unsigned long long epoch) {
     extern __shared__ double sm[];
     __shared__ int s_last;
@@ -1211,8 +1190,6 @@ __global__ void __launch_bounds__(128) ba_accept_split(BaCaps C, BaDev D, unsign
 //   off_post   [2][NW][world][SPLIT_SCAL] slots of the integer exchange, double-buffered by call parity
 //   off_exp    this rank's marginalization export: [NW][2] int64 (first row, row count), then the rows, MEXP_ROW doubles each
 // These kernels only move data and sum or compare integers: no floating-point arithmetic, so FMA contraction cannot change a result.
-constexpr int MEXP_ROW = 16;  // [landmark | f_ref, f_obs, active (int64 bits)] | inverse depth | f_const[14]
-enum { XF_SUM = 0, XF_EXPORT = 1, XF_DONE = 2 };
 
 __device__ __forceinline__ unsigned long long *x_flagX(const BaDev &D, int peer, int kind, int from) {
     return (unsigned long long *) (D.S.peer[peer] + D.S.off_flagX) + kind * 8 + from;
