@@ -156,6 +156,21 @@ def shard_cull_inputs(ci: dict, shard: dict) -> dict:
     return out
 
 
+def shard_vision_inputs(vision: dict, shard: dict, cull_shard: dict) -> dict:
+    """The vision inputs of one landmark shard (what each rank passes to shard_slide_vision) from those of the whole window: obs_lm remapped
+    on the device to the shard's old rows (-1 outside [lm_lo, lm_hi)), obs_factor the shard's (shard_cull_inputs' output, `cull_shard`).
+    Every other entry, the new map points included, is the whole window's.  Returns once the remap is done on torch's current stream (the
+    handle reads it on its own)."""
+    lo, hi = int(shard["lm_lo"]), int(shard["lm_hi"])
+    out = dict(vision, obs_factor=cull_shard.get("obs_factor"))
+    lm = vision.get("obs_lm")
+    if lm is not None:
+        import torch
+        out["obs_lm"] = torch.where((lm >= lo) & (lm < hi), lm - lo, torch.full_like(lm, -1))
+        torch.cuda.current_stream(lm.device).synchronize()
+    return out
+
+
 def merge_cull_shard(full: dict, shard: dict, shard_out: dict) -> None:
     """Write one shard's culling results (update_and_cull on a sharded handle) into the whole window's result dict `full`: lm_pw, lm_depth,
     lm_outlier over the shard's landmark range, obs_outlier over its observations.  Camera outputs and counts are the same on every rank."""
@@ -581,6 +596,16 @@ class WindowSolver:
         return outs
 
     def slide_vision(self, next_problems, carry, vision, integrate=None, noise5=None, station=(0.0, 0.0, 0.0), prior_from_marg=True):
+        return self._slide_vision("icg_ba_slide_vision_resident", next_problems, carry, vision, integrate, noise5, station, prior_from_marg)
+
+    def shard_slide_vision(self, next_problems, carry, vision, integrate=None, noise5=None, station=(0.0, 0.0, 0.0), prior_from_marg=True):
+        """slide_vision() on a landmark-sharded handle (icg_ba_shard_slide_vision_resident), a collective call: every rank passes its next shards
+        (camera side as shard_slide takes it), their carry maps (node / IMU / GNSS) and its own vision dicts (shard_vision_inputs); new map
+        point j of window w is built on rank (j + w) % world.  Returns the rank's shard as slide_vision does (lm_src / f_src shard-local,
+        lm_origin: old shard-local landmark or -(j + 1) for global new point j, nan_flags: old shard L + every new point, set on its own rank)."""
+        return self._slide_vision("icg_ba_shard_slide_vision_resident", next_problems, carry, vision, integrate, noise5, station, prior_from_marg)
+
+    def _slide_vision(self, fn, next_problems, carry, vision, integrate=None, noise5=None, station=(0.0, 0.0, 0.0), prior_from_marg=True):
         """slide() (integrate given: slide_integrate()) whose vision rows are built on the device (icg_ba_slide_vision_resident):
         addReprojectionParameters + addReprojectionFactors on the culled window this handle holds plus the new keyframes' observations.  The
         last update_and_cull() of these windows must be current.  next_problems' L, F, invdepth, f_lm / f_ref / f_obs / f_const, f_active and
@@ -598,7 +623,7 @@ class WindowSolver:
         from ._lib import IcgError, SlideIntegrate, SlideVision, SlideWindow
         from .camera import CameraStruct
         if integrate is not None and noise5 is None:
-            raise ValueError("slide_vision: integrate needs noise5")
+            raise ValueError(f"{fn}: integrate needs noise5")
         n = len(next_problems)
         flags = [prior_from_marg] * n if np.isscalar(prior_from_marg) else list(prior_from_marg)
         Lc, Fc = self.max_L, self.max_F
@@ -657,10 +682,10 @@ class WindowSolver:
             s.lm_origin, s.nan_flags = o["lm_origin"].ctypes.data_as(ip), o["nan_flags"].ctypes.data_as(bp)
         nz = np.ascontiguousarray(noise5 if noise5 is not None else np.zeros(5), np.float64)
         stn = np.ascontiguousarray(station, np.float64)
-        rc = lib().icg_ba_slide_vision_resident(self._h, n, arr, cw, None if iw is None else iw, vp(nz.ctypes.data) if iw is not None else None,
-                                                vp(stn.ctypes.data) if iw is not None else None, vw)
+        rc = getattr(lib(), fn)(self._h, n, arr, cw, None if iw is None else iw, vp(nz.ctypes.data) if iw is not None else None,
+                                vp(stn.ctypes.data) if iw is not None else None, vw)
         if rc != 0:
-            err = IcgError(f"icg_ba_slide_vision_resident failed with code {rc}: {lib().icg_last_error().decode('utf-8', 'replace')}")
+            err = IcgError(f"{fn} failed with code {rc}: {lib().icg_last_error().decode('utf-8', 'replace')}")
             err.code = rc
             raise err
         res = []

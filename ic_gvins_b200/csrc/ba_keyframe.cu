@@ -695,9 +695,11 @@ static int shard_group_only(icg_ba *h, const char *fn, const char *plain) {
 // check of its own prior; then one agreement of the group (shard_agree: every rank's verdict and a fingerprint of the camera side) before any
 // rank writes its device, and with `integ` a second one on the integration's outcome.  A rank that rejects joins the agreement all the same
 // (fail below), so its peers never wait for it.  The owner of window w forms its prior from the workspace of mx_h; the other ranks get zeros.
-// lm_ref_built: icg_ba_slide_vision_resident has written the next windows' reference rows into lm_ref_alt already
+// lm_ref_built: vision_body has written the next windows' reference rows into lm_ref_alt already; seed (sharded): vision_body's fingerprint of
+// its own arguments, which the agreement's fingerprint continues
 static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba_slide_window *carry, const icg_ba_slide_integrate *integ,
-                      const double *noise5, const double *station3, const char *fn, bool sharded, bool lm_ref_built = false) {
+                      const double *noise5, const double *station3, const char *fn, bool sharded, bool lm_ref_built = false,
+                      const ArgPrint *seed = nullptr) {
     bool joined = false;  // sharded: this rank has joined the agreement of the call
     std::vector<WinDims> old_dims;
     std::vector<std::vector<int>> old_slot;
@@ -1002,7 +1004,7 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
             }
     }
     if (sharded) {
-        ArgPrint fp;
+        ArgPrint fp = seed ? *seed : ArgPrint();
         fp.num(n);
         if (integ) fp.arr(noise5, 5), fp.arr(station3, 3);
         for (int w = 0; w < n; w++) {
@@ -1133,6 +1135,156 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
     return ICG_OK;
 }
 
+// ---- the vision half of the next windows built on the device (ba_vision.cu), then the slide of those windows (slide_body).
+//
+// sharded (icg_ba_shard_slide_vision_resident, a collective call): each rank builds its next shard from its own old shard, its own culling and
+// its shard-local obs_lm; new map point j of window w is built on rank (j + w) mod world only.  The vision arguments every rank must share and
+// the two counts the kernel read on the device seed slide_body's fingerprint, so the group still agrees once; a rank that rejects before
+// slide_body joins that agreement with its rejection, as slide_body's own checks do.
+static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba_slide_window *carry, const icg_ba_slide_integrate *integ,
+                       const double *noise5, const double *station3, icg_ba_slide_vision *vis, const char *fn, bool sharded) {
+    auto reject = [&](int code) { return sharded ? shard_agree(h, true, 0, fn) : code; };
+    auto cuda_fail = [&](cudaError_t e, const char *what) {
+        set_error("%s: %s failed: %s", fn, what, cudaGetErrorString(e));
+        return reject(ICG_ECUDA);
+    };
+    int rc = resident_single_rank(h, n, next, fn, sharded);
+    if (rc != ICG_OK) return reject(rc);
+    if (!carry || !vis || (integ && (!noise5 || !station3))) {
+        set_error("%s: bad arguments", fn);
+        return reject(ICG_EINVAL);
+    }
+    if (h->cull_res_n != n) {
+        set_error("%s: no culling of these %d windows is current (icg_ba_update_and_cull_resident, with no upload or slide since)", fn, n);
+        return reject(ICG_EINVAL);
+    }
+    if (cudaError_t e = cudaSetDevice(h->device)) return cuda_fail(e, "cudaSetDevice");
+    const BaCaps &C = h->C;
+    std::vector<VisWin> wins(n);
+    ArgPrint fp;  // sharded: what every rank must pass alike, then the counts its kernel read
+    size_t n_ofac = 0, n_lm = 0, n_f = 0, n_nf = 0, n_scr = 0;
+    for (int w = 0; w < n; w++) {
+        const icg_ba_problem &p = next[w];
+        const icg_ba_slide_vision &v = vis[w];
+        const WinDims &od = h->dims.h[w];
+        const CullWin &cw = h->cull_res_win[w];
+        const int nco = h->cull_res_nobs[w];
+        bool bad = p.K < 2 || p.K > C.K || v.num_marg < 0 || v.num_marg > od.K || !v.node_in_map || !v.node_td || v.cur_node < 0 || v.cur_node >= p.K ||
+                   v.n_frames < 0 || v.n_frames > VIS_MAX_FRAMES || (v.n_frames > 0 && (!v.frame_id || !v.frame_node)) || v.n_obs < 0 || v.n_new < 0 ||
+                   (v.obs_src && v.n_in < 0) || (v.n_obs > 0 && (!v.obs_lm || !v.obs_undis_xy || !v.obs_vel)) ||
+                   (v.n_new > 0 && (!v.new_depth || !v.new_vel_ref || !v.new_vel_cur || !v.new_ref_undis_xy || !v.new_cur_undis_xy || !v.new_ref_frame_id)) ||
+                   (nco > 0 && !v.obs_factor) || cw.K != od.K || cw.L != od.L;
+        for (int e = 0; !bad && e < v.n_frames; e++) bad = v.frame_node[e] < 0 || v.frame_node[e] >= p.K;
+        if (bad) {
+            set_error("%s: window %d: arguments out of range or arrays missing", fn, w);
+            return reject(ICG_EINVAL);
+        }
+        if (sharded) {
+            fp.num(v.num_marg), fp.arr(v.node_in_map, od.K), fp.arr(&v.cam, 1), fp.arr(v.node_td, p.K), fp.num(v.cur_node), fp.num(v.n_frames);
+            fp.arr(v.frame_id, v.n_frames), fp.arr(v.frame_node, v.n_frames), fp.num(v.n_obs), fp.num(v.n_new);
+        }
+        VisWin &W = wins[w];
+        memset(&W, 0, sizeof(W));
+        W.cam = v.cam;
+        memcpy(W.node_td, v.node_td, sizeof(double) * p.K);
+        memset(W.onode, -1, sizeof(W.onode));
+        const int32_t *ns = carry[w].node_src;
+        for (int j = 0; ns && j < p.K; j++)
+            if (ns[j] >= v.num_marg && ns[j] < od.K && v.node_in_map[ns[j]]) W.onode[ns[j]] = (int8_t) j;
+        for (int e = 0; e < v.n_frames; e++) W.frame_id[e] = v.frame_id[e], W.frame_node[e] = v.frame_node[e];
+        W.oK = od.K, W.oL = od.L, W.oF = od.F, W.nK = p.K, W.n_frames = v.n_frames, W.cur_node = v.cur_node;
+        W.cull_lm0 = cw.lm0, W.cull_off0 = cw.off0, W.cull_obs0 = cw.obs0, W.n_cull_obs = nco, W.obs_factor0 = (int) n_ofac;
+        W.n_obs = v.n_obs, W.n_in = v.obs_src ? v.n_in : v.n_obs, W.dev_n = v.dev_n, W.src = v.obs_src, W.obs_node = v.obs_node, W.obs_lm = v.obs_lm;
+        W.obs_xy = v.obs_undis_xy, W.obs_vel = v.obs_vel;
+        W.n_new = v.n_new, W.dev_new_n = v.dev_new_n, W.new_depth = v.new_depth, W.new_vel_ref = v.new_vel_ref, W.new_vel_cur = v.new_vel_cur;
+        W.new_ref_xy = v.new_ref_undis_xy, W.new_cur_xy = v.new_cur_undis_xy, W.new_ref_frame = v.new_ref_frame_id;
+        W.lm_out = (int) n_lm, W.f_out = (int) n_f, W.nf_out = (int) n_nf, W.scr = (int) n_scr;
+        n_ofac += nco, n_lm += (size_t) od.L + v.n_new, n_f += (size_t) od.F + v.n_obs + v.n_new, n_nf += (size_t) v.n_obs + v.n_new;
+        n_scr += (size_t) od.F + 3 * (size_t) od.L + 5 * ((size_t) od.L + v.n_new) + v.n_new;  // ba_vision_build's scratch
+        if (n_ofac >= INT32_MAX / 2 || n_f >= INT32_MAX / 16 || n_scr >= INT32_MAX / 2) {
+            set_error("%s: too many rows in one call", fn);
+            return reject(ICG_EINVAL);
+        }
+    }
+    // staging: inputs [windows | obs_factor], outputs [counts | lm_src | lm_org | f_lm | f_ref | f_obs | f_src | invdepth | new factor rows |
+    // NaN flags], then the kernel's scratch (never copied)
+    Layout lay;
+    const size_t b_win = lay.take(sizeof(VisWin) * n), b_ofac = lay.take(4 * n_ofac), in_end = lay.size();
+    const size_t b_cnt = lay.take(4 * VIS_COUNTS * (size_t) n), b_lms = lay.take(4 * n_lm), b_org = lay.take(4 * n_lm), b_flm = lay.take(4 * n_f),
+                 b_fref = lay.take(4 * n_f), b_fobs = lay.take(4 * n_f), b_fsrc = lay.take(4 * n_f), b_invd = lay.take(8 * n_lm), b_fnew = lay.take(112 * n_nf),
+                 b_nan = lay.take(n_lm), out_end = lay.size(), b_scr = lay.take(4 * n_scr);
+    cudaStream_t s = h->stream;
+    if (lay.size() > h->vis.n)
+        if (cudaError_t e = cudaStreamSynchronize(s)) return cuda_fail(e, "cudaStreamSynchronize");
+    if ((rc = hd_reserve(h, h->vis, lay.size(), fn)) != ICG_OK) return reject(rc);
+    unsigned char *H = h->vis.h, *Dv = h->vis.d;
+    memcpy(H + b_win, wins.data(), sizeof(VisWin) * n);
+    for (int w = 0; w < n; w++)
+        if (wins[w].n_cull_obs > 0) memcpy(H + b_ofac + 4 * (size_t) wins[w].obs_factor0, vis[w].obs_factor, 4 * (size_t) wins[w].n_cull_obs);
+    VisArgs a;
+    a.win = (const VisWin *) (Dv + b_win), a.K = C.K, a.L = C.L, a.F = C.F;
+    a.rank = sharded ? h->D.rank : 0, a.world = sharded ? h->D.world : 1;
+    a.rho = h->D.rho, a.lm_ref = h->lm_ref, a.lm_ref_next = h->lm_ref_alt, a.f_meta_s = h->D.f_meta_s, a.lm_off = h->D.lm_off, a.lm_perm = h->D.lm_perm;
+    a.lm_ref_node = (const int *) (h->cull.d + h->cull_res_ref), a.obs_off = (const int *) (h->cull.d + h->cull_res_off);
+    a.lm_outlier = h->cull.d + h->cull_res_lmo, a.obs_outlier = h->cull.d + h->cull_res_obso, a.obs_factor = (const int *) (Dv + b_ofac);
+    a.counts = (int *) (Dv + b_cnt), a.lm_src = (int *) (Dv + b_lms), a.lm_org = (int *) (Dv + b_org), a.lm_nan = Dv + b_nan, a.f_lm = (int *) (Dv + b_flm), a.f_ref = (int *) (Dv + b_fref);
+    a.f_obs = (int *) (Dv + b_fobs), a.f_src = (int *) (Dv + b_fsrc), a.invdepth = (double *) (Dv + b_invd), a.f_new = (double *) (Dv + b_fnew);
+    a.scratch = (int *) (Dv + b_scr);
+    cudaError_t e = cudaMemcpyAsync(Dv, H, in_end, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemsetAsync(Dv + b_cnt, 0, 4 * VIS_COUNTS * (size_t) n, s);
+    if (e == cudaSuccess && (e = launch_vision(a, n, s)) == cudaSuccess) count_launch();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(H + b_cnt, Dv + b_cnt, out_end - b_cnt, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) return cuda_fail(e, "the build on the device");
+    // the built windows: every check, then the slide of next with these vision rows
+    static const char *what[] = {"", "obs_factor names no factor of the old window", "a device count is outside its list", "obs_src is out of range",
+                                 "a node is out of range", "obs_lm is out of range", "two observations of one landmark in one node",
+                                 "a reference frame id is not in the frame table", "a landmark whose reference row is unknown takes a new observation"};
+    std::vector<icg_ba_problem> nx(next, next + n);
+    std::vector<icg_ba_slide_window> cr(carry, carry + n);
+    std::vector<std::unique_ptr<double[]>> fc_tmp(n);
+    const int *cnt = (const int *) (H + b_cnt);
+    for (int w = 0; w < n; w++) {
+        const int *c = cnt + VIS_COUNTS * w;
+        if (c[3] != 0) {
+            set_error("%s: window %d: %s (entry %d)", fn, w, c[3] > 0 && c[3] <= VIS_EROW ? what[c[3]] : "?", c[4]);
+            return reject(ICG_EINVAL);
+        }
+        if (c[0] > C.L || c[1] > C.F) {
+            set_error("%s: window %d: the next window has %d landmarks and %d factors, the handle holds %d / %d", fn, w, c[0], c[1], C.L, C.F);
+            return reject(ICG_EINVAL);
+        }
+        if (sharded) fp.num(c[6]), fp.num(c[7]);
+    }
+    for (int w = 0; w < n; w++) {
+        const int *c = cnt + VIS_COUNTS * w;
+        const VisWin &W = wins[w];
+        icg_ba_slide_vision &v = vis[w];
+        icg_ba_problem &p = nx[w];
+        const int L = c[0], F = c[1];
+        int *lm_src = (int *) (H + b_lms) + W.lm_out, *f_src = (int *) (H + b_fsrc) + W.f_out;
+        p.L = L, p.F = F, p.invdepth = (double *) (H + b_invd) + W.lm_out, p.f_active = nullptr;
+        p.f_lm = (int *) (H + b_flm) + W.f_out, p.f_ref = (int *) (H + b_fref) + W.f_out, p.f_obs = (int *) (H + b_fobs) + W.f_out;
+        double *fc = v.f_const;
+        if (!fc) fc_tmp[w].reset(new double[14 * (size_t) std::max(F, 1)]), fc = fc_tmp[w].get();
+        const double *rows = (const double *) (H + b_fnew) + 14 * (size_t) W.nf_out;
+        for (int f = 0, t = 0; f < F; f++)
+            if (f_src[f] < 0) memcpy(fc + 14 * (size_t) f, rows + 14 * (size_t) t++, 112);
+        p.f_const = fc;
+        cr[w].lm_src = lm_src, cr[w].f_src = f_src;
+        v.L = L, v.F = F, v.nan_dropped = c[5];
+        if (v.lm_src) memcpy(v.lm_src, lm_src, 4 * (size_t) L);
+        if (v.lm_origin) memcpy(v.lm_origin, (int *) (H + b_org) + W.lm_out, 4 * (size_t) L);
+        if (v.nan_flags) memcpy(v.nan_flags, H + b_nan + W.lm_out, (size_t) W.oL + W.n_new);
+        if (v.f_src) memcpy(v.f_src, f_src, 4 * (size_t) F);
+        if (v.f_lm) memcpy(v.f_lm, p.f_lm, 4 * (size_t) F);
+        if (v.f_ref) memcpy(v.f_ref, p.f_ref, 4 * (size_t) F);
+        if (v.f_obs) memcpy(v.f_obs, p.f_obs, 4 * (size_t) F);
+        if (v.invdepth) memcpy(v.invdepth, p.invdepth, 8 * (size_t) L);
+    }
+    return slide_body(h, n, nx.data(), cr.data(), integ, noise5, station3, fn, sharded, true, sharded ? &fp : nullptr);
+}
+
 extern "C" {
 
 int icg_ba_marginalize(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg, icg_ba_prior *out) {
@@ -1233,11 +1385,10 @@ int icg_ba_update_and_cull_resident(icg_ba *h, int n_windows, const icg_ba_probl
     ICG_CUDA(cudaMemcpyAsync(H + in_bytes, Dv + in_bytes, out_bytes, cudaMemcpyDeviceToHost, s));
     ICG_CUDA(cudaStreamSynchronize(s));
     if (h->D.world > 1 && (rc = shard_timed_out(h, "icg_ba_update_and_cull_resident")) != ICG_OK) return rc;
-    if (h->D.world == 1) {
-        h->cull_res_n = n, h->cull_res_win = win, h->cull_res_nobs.resize(n);
-        for (int w = 0; w < n; w++) h->cull_res_nobs[w] = problems[w].L > 0 ? io[w].obs_off[problems[w].L] : 0;
-        h->cull_res_ref = i_ref, h->cull_res_off = i_off, h->cull_res_lmo = o_lmo, h->cull_res_obso = o_obso;
-    }
+    // where the flags sit, for vision_body (sharded: the rank's own shard's)
+    h->cull_res_n = n, h->cull_res_win = win, h->cull_res_nobs.resize(n);
+    for (int w = 0; w < n; w++) h->cull_res_nobs[w] = problems[w].L > 0 ? io[w].obs_off[problems[w].L] : 0;
+    h->cull_res_ref = i_ref, h->cull_res_off = i_off, h->cull_res_lmo = o_lmo, h->cull_res_obso = o_obso;
     for (int w = 0; w < n; w++) {
         const icg_ba_problem &p = problems[w];
         icg_ba_cull_window &c = io[w];
@@ -1326,141 +1477,14 @@ int icg_ba_slide_integrate_resident(icg_ba *h, int n, const icg_ba_problem *next
     return slide_body(h, n, next, carry, integ, noise5, station3, "icg_ba_slide_integrate_resident", false);
 }
 
-// the vision half of the next windows built on the device (ba_vision.cu), then the slide of those windows
 int icg_ba_slide_vision_resident(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba_slide_window *carry, const icg_ba_slide_integrate *integ,
                                  const double *noise5, const double *station3, icg_ba_slide_vision *vis) {
     static const char *fn = "icg_ba_slide_vision_resident";
     if (h && h->D.world > 1) {
-        set_error("%s: not available on a landmark-sharded handle", fn);
+        set_error("%s: not available on a landmark-sharded handle (its group calls icg_ba_shard_slide_vision_resident)", fn);
         return ICG_EUNSUPPORTED;
     }
-    int rc = resident_single_rank(h, n, next, fn);
-    if (rc != ICG_OK) return rc;
-    if (!carry || !vis || (integ && (!noise5 || !station3))) {
-        set_error("%s: bad arguments", fn);
-        return ICG_EINVAL;
-    }
-    if (h->cull_res_n != n) {
-        set_error("%s: no culling of these %d windows is current (icg_ba_update_and_cull_resident, with no upload or slide since)", fn, n);
-        return ICG_EINVAL;
-    }
-    ICG_CUDA(cudaSetDevice(h->device));
-    const BaCaps &C = h->C;
-    std::vector<VisWin> wins(n);
-    size_t n_ofac = 0, n_lm = 0, n_f = 0, n_nf = 0, n_scr = 0;
-    for (int w = 0; w < n; w++) {
-        const icg_ba_problem &p = next[w];
-        const icg_ba_slide_vision &v = vis[w];
-        const WinDims &od = h->dims.h[w];
-        const CullWin &cw = h->cull_res_win[w];
-        const int nco = h->cull_res_nobs[w];
-        bool bad = p.K < 2 || p.K > C.K || v.num_marg < 0 || v.num_marg > od.K || !v.node_in_map || !v.node_td || v.cur_node < 0 || v.cur_node >= p.K ||
-                   v.n_frames < 0 || v.n_frames > VIS_MAX_FRAMES || (v.n_frames > 0 && (!v.frame_id || !v.frame_node)) || v.n_obs < 0 || v.n_new < 0 ||
-                   (v.obs_src && v.n_in < 0) || (v.n_obs > 0 && (!v.obs_lm || !v.obs_undis_xy || !v.obs_vel)) ||
-                   (v.n_new > 0 && (!v.new_depth || !v.new_vel_ref || !v.new_vel_cur || !v.new_ref_undis_xy || !v.new_cur_undis_xy || !v.new_ref_frame_id)) ||
-                   (nco > 0 && !v.obs_factor) || cw.K != od.K || cw.L != od.L;
-        for (int e = 0; !bad && e < v.n_frames; e++) bad = v.frame_node[e] < 0 || v.frame_node[e] >= p.K;
-        if (bad) {
-            set_error("%s: window %d: arguments out of range or arrays missing", fn, w);
-            return ICG_EINVAL;
-        }
-        VisWin &W = wins[w];
-        memset(&W, 0, sizeof(W));
-        W.cam = v.cam;
-        memcpy(W.node_td, v.node_td, sizeof(double) * p.K);
-        memset(W.onode, -1, sizeof(W.onode));
-        const int32_t *ns = carry[w].node_src;
-        for (int j = 0; ns && j < p.K; j++)
-            if (ns[j] >= v.num_marg && ns[j] < od.K && v.node_in_map[ns[j]]) W.onode[ns[j]] = (int8_t) j;
-        for (int e = 0; e < v.n_frames; e++) W.frame_id[e] = v.frame_id[e], W.frame_node[e] = v.frame_node[e];
-        W.oK = od.K, W.oL = od.L, W.oF = od.F, W.nK = p.K, W.n_frames = v.n_frames, W.cur_node = v.cur_node;
-        W.cull_lm0 = cw.lm0, W.cull_off0 = cw.off0, W.cull_obs0 = cw.obs0, W.n_cull_obs = nco, W.obs_factor0 = (int) n_ofac;
-        W.n_obs = v.n_obs, W.n_in = v.obs_src ? v.n_in : v.n_obs, W.dev_n = v.dev_n, W.src = v.obs_src, W.obs_node = v.obs_node, W.obs_lm = v.obs_lm;
-        W.obs_xy = v.obs_undis_xy, W.obs_vel = v.obs_vel;
-        W.n_new = v.n_new, W.dev_new_n = v.dev_new_n, W.new_depth = v.new_depth, W.new_vel_ref = v.new_vel_ref, W.new_vel_cur = v.new_vel_cur;
-        W.new_ref_xy = v.new_ref_undis_xy, W.new_cur_xy = v.new_cur_undis_xy, W.new_ref_frame = v.new_ref_frame_id;
-        W.lm_out = (int) n_lm, W.f_out = (int) n_f, W.nf_out = (int) n_nf, W.scr = (int) n_scr;
-        n_ofac += nco, n_lm += (size_t) od.L + v.n_new, n_f += (size_t) od.F + v.n_obs + v.n_new, n_nf += (size_t) v.n_obs + v.n_new;
-        n_scr += (size_t) od.F + 3 * (size_t) od.L + 5 * ((size_t) od.L + v.n_new) + v.n_new;  // ba_vision_build's scratch
-        if (n_ofac >= INT32_MAX / 2 || n_f >= INT32_MAX / 16 || n_scr >= INT32_MAX / 2) {
-            set_error("%s: too many rows in one call", fn);
-            return ICG_EINVAL;
-        }
-    }
-    // staging: inputs [windows | obs_factor], outputs [counts | lm_src | lm_org | f_lm | f_ref | f_obs | f_src | invdepth | new factor rows |
-    // NaN flags], then the kernel's scratch (never copied)
-    Layout lay;
-    const size_t b_win = lay.take(sizeof(VisWin) * n), b_ofac = lay.take(4 * n_ofac), in_end = lay.size();
-    const size_t b_cnt = lay.take(4 * VIS_COUNTS * (size_t) n), b_lms = lay.take(4 * n_lm), b_org = lay.take(4 * n_lm), b_flm = lay.take(4 * n_f),
-                 b_fref = lay.take(4 * n_f), b_fobs = lay.take(4 * n_f), b_fsrc = lay.take(4 * n_f), b_invd = lay.take(8 * n_lm), b_fnew = lay.take(112 * n_nf),
-                 b_nan = lay.take(n_lm), out_end = lay.size(), b_scr = lay.take(4 * n_scr);
-    cudaStream_t s = h->stream;
-    if (lay.size() > h->vis.n) ICG_CUDA(cudaStreamSynchronize(s));
-    if ((rc = hd_reserve(h, h->vis, lay.size(), fn)) != ICG_OK) return rc;
-    unsigned char *H = h->vis.h, *Dv = h->vis.d;
-    memcpy(H + b_win, wins.data(), sizeof(VisWin) * n);
-    for (int w = 0; w < n; w++)
-        if (wins[w].n_cull_obs > 0) memcpy(H + b_ofac + 4 * (size_t) wins[w].obs_factor0, vis[w].obs_factor, 4 * (size_t) wins[w].n_cull_obs);
-    ICG_CUDA(cudaMemcpyAsync(Dv, H, in_end, cudaMemcpyHostToDevice, s));
-    VisArgs a;
-    a.win = (const VisWin *) (Dv + b_win), a.K = C.K, a.L = C.L, a.F = C.F;
-    a.rho = h->D.rho, a.lm_ref = h->lm_ref, a.lm_ref_next = h->lm_ref_alt, a.f_meta_s = h->D.f_meta_s, a.lm_off = h->D.lm_off, a.lm_perm = h->D.lm_perm;
-    a.lm_ref_node = (const int *) (h->cull.d + h->cull_res_ref), a.obs_off = (const int *) (h->cull.d + h->cull_res_off);
-    a.lm_outlier = h->cull.d + h->cull_res_lmo, a.obs_outlier = h->cull.d + h->cull_res_obso, a.obs_factor = (const int *) (Dv + b_ofac);
-    a.counts = (int *) (Dv + b_cnt), a.lm_src = (int *) (Dv + b_lms), a.lm_org = (int *) (Dv + b_org), a.lm_nan = Dv + b_nan, a.f_lm = (int *) (Dv + b_flm), a.f_ref = (int *) (Dv + b_fref);
-    a.f_obs = (int *) (Dv + b_fobs), a.f_src = (int *) (Dv + b_fsrc), a.invdepth = (double *) (Dv + b_invd), a.f_new = (double *) (Dv + b_fnew);
-    a.scratch = (int *) (Dv + b_scr);
-    ICG_CUDA(cudaMemsetAsync(Dv + b_cnt, 0, 4 * VIS_COUNTS * (size_t) n, s));
-    ICG_CUDA(launch_vision(a, n, s));
-    count_launch();
-    ICG_CUDA(cudaMemcpyAsync(H + b_cnt, Dv + b_cnt, out_end - b_cnt, cudaMemcpyDeviceToHost, s));
-    ICG_CUDA(cudaStreamSynchronize(s));
-    // the built windows: every check, then the slide of next with these vision rows
-    static const char *what[] = {"", "obs_factor names no factor of the old window", "a device count is outside its list", "obs_src is out of range",
-                                 "a node is out of range", "obs_lm is out of range", "two observations of one landmark in one node",
-                                 "a reference frame id is not in the frame table", "a landmark whose reference row is unknown takes a new observation"};
-    std::vector<icg_ba_problem> nx(next, next + n);
-    std::vector<icg_ba_slide_window> cr(carry, carry + n);
-    std::vector<std::unique_ptr<double[]>> fc_tmp(n);
-    const int *cnt = (const int *) (H + b_cnt);
-    for (int w = 0; w < n; w++) {
-        const int *c = cnt + VIS_COUNTS * w;
-        if (c[3] != 0) {
-            set_error("%s: window %d: %s (entry %d)", fn, w, c[3] > 0 && c[3] <= VIS_EROW ? what[c[3]] : "?", c[4]);
-            return ICG_EINVAL;
-        }
-        if (c[0] > C.L || c[1] > C.F) {
-            set_error("%s: window %d: the next window has %d landmarks and %d factors, the handle holds %d / %d", fn, w, c[0], c[1], C.L, C.F);
-            return ICG_EINVAL;
-        }
-    }
-    for (int w = 0; w < n; w++) {
-        const int *c = cnt + VIS_COUNTS * w;
-        const VisWin &W = wins[w];
-        icg_ba_slide_vision &v = vis[w];
-        icg_ba_problem &p = nx[w];
-        const int L = c[0], F = c[1];
-        int *lm_src = (int *) (H + b_lms) + W.lm_out, *f_src = (int *) (H + b_fsrc) + W.f_out;
-        p.L = L, p.F = F, p.invdepth = (double *) (H + b_invd) + W.lm_out, p.f_active = nullptr;
-        p.f_lm = (int *) (H + b_flm) + W.f_out, p.f_ref = (int *) (H + b_fref) + W.f_out, p.f_obs = (int *) (H + b_fobs) + W.f_out;
-        double *fc = v.f_const;
-        if (!fc) fc_tmp[w].reset(new double[14 * (size_t) std::max(F, 1)]), fc = fc_tmp[w].get();
-        const double *rows = (const double *) (H + b_fnew) + 14 * (size_t) W.nf_out;
-        for (int f = 0, t = 0; f < F; f++)
-            if (f_src[f] < 0) memcpy(fc + 14 * (size_t) f, rows + 14 * (size_t) t++, 112);
-        p.f_const = fc;
-        cr[w].lm_src = lm_src, cr[w].f_src = f_src;
-        v.L = L, v.F = F, v.nan_dropped = c[5];
-        if (v.lm_src) memcpy(v.lm_src, lm_src, 4 * (size_t) L);
-        if (v.lm_origin) memcpy(v.lm_origin, (int *) (H + b_org) + W.lm_out, 4 * (size_t) L);
-        if (v.nan_flags) memcpy(v.nan_flags, H + b_nan + W.lm_out, (size_t) W.oL + W.n_new);
-        if (v.f_src) memcpy(v.f_src, f_src, 4 * (size_t) F);
-        if (v.f_lm) memcpy(v.f_lm, p.f_lm, 4 * (size_t) F);
-        if (v.f_ref) memcpy(v.f_ref, p.f_ref, 4 * (size_t) F);
-        if (v.f_obs) memcpy(v.f_obs, p.f_obs, 4 * (size_t) F);
-        if (v.invdepth) memcpy(v.invdepth, p.invdepth, 8 * (size_t) L);
-    }
-    return slide_body(h, n, nx.data(), cr.data(), integ, noise5, station3, fn, false, true);
+    return vision_body(h, n, next, carry, integ, noise5, station3, vis, fn, false);
 }
 
 int icg_ba_shard_slide_resident(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba_slide_window *carry) {
@@ -1480,6 +1504,13 @@ int icg_ba_shard_slide_integrate_resident(icg_ba *h, int n, const icg_ba_problem
         return ICG_EINVAL;
     }
     return slide_body(h, n, next, carry, integ, noise5, station3, fn, true);
+}
+
+int icg_ba_shard_slide_vision_resident(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba_slide_window *carry,
+                                       const icg_ba_slide_integrate *integ, const double *noise5, const double *station3, icg_ba_slide_vision *vis) {
+    const char *fn = "icg_ba_shard_slide_vision_resident";
+    const int rc = shard_group_only(h, fn, "icg_ba_slide_vision_resident");
+    return rc != ICG_OK ? rc : vision_body(h, n, next, carry, integ, noise5, station3, vis, fn, true);
 }
 
 }  // extern "C"

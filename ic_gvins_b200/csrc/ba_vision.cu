@@ -43,7 +43,8 @@ __device__ void cam_point(const icg_camera &c, float u, float v, double *p) {
 // Rules (include/icgvins_b200.h, icg_ba_slide_vision_resident): landmark l of the old window is carried when it is not a culling outlier, its
 // reference node is usable (in the map, not marginalized, kept by the slide) and 1 / (1 / rho) is not NaN; its old factors survive when their
 // observation is listed by the culling and not an outlier and their observing node is usable; its new observations follow in node order.  New map
-// points follow the carried landmarks in creation order, each with one factor from its reference node to the current node.
+// points follow the carried landmarks in creation order, each with one factor from its reference node to the current node.  On a landmark shard
+// the old window is the rank's shard and only the rank's new points are kept; the numbering below is then the shard's.
 __global__ void __launch_bounds__(VIS_THREADS) ba_vision_build(VisArgs a) {
     __shared__ Scan::TempStorage tmp;
     __shared__ int s_nobs, s_nnew;
@@ -59,6 +60,7 @@ __global__ void __launch_bounds__(VIS_THREADS) ba_vision_build(VisArgs a) {
     const int *ofac = a.obs_factor + W.obs_factor0;
     if (t == 0) {
         int n = W.dev_n ? *W.dev_n : W.n_obs, m = W.dev_new_n ? *W.dev_new_n : W.n_new;
+        cnt[6] = n, cnt[7] = m;
         if (n < 0 || n > W.n_obs) fail(cnt, VIS_ECOUNT, n), n = 0;
         if (m < 0 || m > W.n_new) fail(cnt, VIS_ECOUNT, m), m = 0;
         s_nobs = n, s_nnew = m;
@@ -102,10 +104,11 @@ __global__ void __launch_bounds__(VIS_THREADS) ba_vision_build(VisArgs a) {
             if (W.frame_id[e] == id) node = W.frame_node[e];
         if (node < 0) fail(cnt, VIS_EFRAME, j);
         new_ref[j] = node;
-        const bool nan = isnan(__ddiv_rn(1.0, W.new_depth[j]));
-        keep[oL + j] = node >= 0 && !nan;
-        lm_nan[oL + j] = node >= 0 && nan;
-        nan_drops += node >= 0 && nan;
+        // landmark shards: new point j of window w lives on rank (j + w) mod world only (world 1: every point)
+        const bool nan = isnan(__ddiv_rn(1.0, W.new_depth[j])), mine = node >= 0 && (j + w) % a.world == a.rank;
+        keep[oL + j] = mine && !nan;
+        lm_nan[oL + j] = mine && nan;
+        nan_drops += mine && nan;
     }
     __syncthreads();
     // the new observations: one bit per (landmark, next node); a second observation of a landmark in one node is an error

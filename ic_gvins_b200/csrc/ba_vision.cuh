@@ -1,4 +1,4 @@
-// ba_vision.cuh -- the vision half of the next window (icg_ba_slide_vision_resident): GVINS::addReprojectionParameters +
+// ba_vision.cuh -- the vision half of the next window (icg_ba_slide_vision_resident and its sharded form): GVINS::addReprojectionParameters +
 // addReprojectionFactors (IG/ic_gvins.cc:1697-1837) after Map::removeKeyFrame(frame, true) (tracking/map.cc:89-125), built on the device from
 // the culled window the handle holds and the new keyframes' observations.  The interface between the handle (ba.cu: validation, staging,
 // the slide) and the kernel (ba_vision.cu, built without FMA contraction so that pixel2cam is the host's sub-then-divide).
@@ -41,13 +41,15 @@ struct VisWin {
     int lm_out, f_out, nf_out, scr;  // offsets of the window's output rows (Lb, Fb, Nb) and int scratch
 };
 
-// per window: [L, F, new factors, error code, error index, landmarks dropped for a NaN inverse depth]
-constexpr int VIS_COUNTS = 6;
+// per window: [L, F, new factors, error code, error index, landmarks dropped for a NaN inverse depth, the observation count and the new-point
+// count the kernel read (a landmark shard's ranks must read the same)]
+constexpr int VIS_COUNTS = 8;
 enum VisError { VIS_OK = 0, VIS_EOBS_FACTOR = 1, VIS_ECOUNT = 2, VIS_ESRC = 3, VIS_ENODE = 4, VIS_ELM = 5, VIS_EDUP = 6, VIS_EFRAME = 7, VIS_EROW = 8 };
 
 struct VisArgs {
     const VisWin *win;
-    int K, L, F;  // the handle's capacities (strides of its arrays)
+    int K, L, F;      // the handle's capacities (strides of its arrays)
+    int rank, world;  // landmark shards: new map point j of window w is built on rank (j + w) mod world only (one GPU: 0, 1)
     // the window the handle holds
     const double *rho;
     const int *f_meta_s, *lm_off, *lm_perm;

@@ -739,7 +739,7 @@ int icg_ba_slide_integrate_resident(icg_ba *h, int n_windows, const icg_ba_probl
  * A rejected call (ICG_EINVAL: max_L / max_F exceeded, a reference frame id missing from the table, a node, landmark or source index out of
  * range, a count outside its list, two observations of one landmark in one node) leaves the handle as it was.  Afterwards the handle cannot be
  * told apart from one that called icg_ba_slide_integrate_resident with the same next whose vision rows were built on the host by these rules.
- * ICG_EUNSUPPORTED on a landmark-sharded handle.
+ * ICG_EUNSUPPORTED on a landmark-sharded handle: its group calls icg_ba_shard_slide_vision_resident.
  */
 typedef struct icg_ba_slide_vision {
     /* in: the old window */
@@ -813,6 +813,34 @@ int icg_ba_shard_reintegrate_resident(icg_ba *h, int n_windows, const icg_ba_pro
 int icg_ba_shard_slide_resident(icg_ba *h, int n_windows, const icg_ba_problem *next, const icg_ba_slide_window *carry);
 int icg_ba_shard_slide_integrate_resident(icg_ba *h, int n_windows, const icg_ba_problem *next, const icg_ba_slide_window *carry,
                                           const icg_ba_slide_integrate *integ, const double *noise5, const double *station3);
+/*
+ * icg_ba_slide_vision_resident on a landmark-sharded handle: each rank builds its own next shard's landmarks and reprojection factors on the
+ * device, from its own old shard and its own culling, then slides as icg_ba_shard_slide[_integrate]_resident (integ NULL or not), with every
+ * rule above.  A COLLECTIVE call, with the structs of the plain call.
+ *   What each rank passes.  Its own next shard problems and carry maps; next.L, F, f_* and carry.lm_src / f_src are built, not read.
+ *     vis[w].obs_factor is the table the rank's own sharded culling took (shard_cull_inputs' obs_factor); vis[w].obs_lm names rows of the
+ *     rank's own OLD shard, -1 for a map point the rank does not hold.  The lists are otherwise the same on every rank (the same tracked
+ *     observations, the same new map points), and every device array must be readable from the rank's own device.
+ *   Old landmarks.  A carried landmark stays on the rank that held it; each rank applies the plain call's rules to its shard: the carry rule,
+ *     the surviving factors, the new observations in node order.
+ *   New map points.  New point j of window w (creation order) goes to rank (j + w) mod world.  The rule is fixed: the count lives on the
+ *     device, so the caller could not place points itself without a host round trip.
+ *   Order.  Each rank's next shard holds its carried landmarks in old shard order, then its new points in creation order; factors landmark
+ *     by landmark.  The next whole window written rank-major is exactly what icg_ba_slide_vision_resident builds from the merged old window,
+ *     reordered rank-major (new points by the rule above, a carried landmark staged for a zero depth -- lm_src -1, lm_origin >= 0 -- on its
+ *     old rank).
+ *   Outputs, per rank.  L, F, nan_dropped of the rank's shard; lm_src / f_src local to the shard, as carry takes them; lm_origin: the old
+ *     shard-local landmark, or -(j + 1) for global new point j; nan_flags: the old shard's L entries, then all n_new entries, a new point
+ *     flagged on its own rank only (OR the ranks together).
+ *   Agreement.  Each rank folds num_marg, node_in_map, cam, node_td, cur_node, the frame table, n_obs / n_new and the observation and
+ *     new-point counts its build read on the device into the fingerprint of the slide's one agreement.  One rejection on any rank (capacity
+ *     on the rank that received the new points, no current culling, every build error of the plain call) or a fingerprint mismatch makes
+ *     EVERY rank return ICG_EINVAL with its handle as it was.  On a handle outside a shard group: ICG_EINVAL naming
+ *     icg_ba_slide_vision_resident.
+ */
+int icg_ba_shard_slide_vision_resident(icg_ba *h, int n_windows, const icg_ba_problem *next, const icg_ba_slide_window *carry,
+                                       const icg_ba_slide_integrate *integ, const double *noise5, const double *station3,
+                                       icg_ba_slide_vision *vis);
 /*
  * Landmark sharding of the window solve across the GPUs of one box (SURVEY.md 8e), over PEER MEMORY (transport "p2p"): every process
  * (one per GPU) uploads the same camera-side problem but only ITS landmarks and their reprojection factors; window w of the batch is
