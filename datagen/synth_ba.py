@@ -54,16 +54,22 @@ def q_yaw(psi):
 
 
 # ---------------------------------------------------------------------------------------------- trajectory + IMU
-def trajectory(t, speed=5.0, yaw_rate=5.0 * D2R):
+def trajectory(t, speed=5.0, yaw_rate=5.0 * D2R, heave=True):
+    """Planar arc at `speed` (m/s) and `yaw_rate` (rad/s), a straight line when yaw_rate is 0; heave adds the 0.02 m vertical oscillation.
+    speed = yaw_rate = 0 with heave=False is a vehicle standing still."""
     psi = 0.3 + yaw_rate * t
+    z = (0.02 * math.sin(0.5 * t), 0.01 * math.cos(0.5 * t), -0.005 * math.sin(0.5 * t)) if heave else (0.0, 0.0, 0.0)
+    if yaw_rate == 0:
+        p = np.array([speed * t * math.cos(psi), speed * t * math.sin(psi), z[0]])
+        return p, np.array([speed * math.cos(psi), speed * math.sin(psi), z[1]]), np.array([0.0, 0.0, z[2]]), psi
     r = speed / yaw_rate
-    p = np.array([r * (math.sin(psi) - math.sin(0.3)), -r * (math.cos(psi) - math.cos(0.3)), 0.02 * math.sin(0.5 * t)])
-    v = np.array([speed * math.cos(psi), speed * math.sin(psi), 0.01 * math.cos(0.5 * t)])
-    a = np.array([-speed * yaw_rate * math.sin(psi), speed * yaw_rate * math.cos(psi), -0.005 * math.sin(0.5 * t)])
+    p = np.array([r * (math.sin(psi) - math.sin(0.3)), -r * (math.cos(psi) - math.cos(0.3)), z[0]])
+    v = np.array([speed * math.cos(psi), speed * math.sin(psi), z[1]])
+    a = np.array([-speed * yaw_rate * math.sin(psi), speed * yaw_rate * math.cos(psi), z[2]])
     return p, v, a, psi
 
 
-def imu_samples(t0, t1, rate, rng, bg, ba, yaw_rate=5.0 * D2R, earth=True):
+def imu_samples(t0, t1, rate, rng, bg, ba, yaw_rate=5.0 * D2R, earth=True, speed=5.0, heave=True):
     """(n, 7) rows: dt, dtheta[3], dvel[3]; row 0 is the sample AT t0 (imu0 of the preintegration)."""
     n = int(round((t1 - t0) * rate))
     dt = 1.0 / rate
@@ -71,7 +77,7 @@ def imu_samples(t0, t1, rate, rng, bg, ba, yaw_rate=5.0 * D2R, earth=True):
     arw, vrw = NOISE5[0], NOISE5[1]
     for i in range(n + 1):
         tm = t0 + (i - 0.5) * dt  # mid-point of the sampling interval ending at t0 + i dt
-        p, v, a, psi = trajectory(tm)
+        p, v, a, psi = trajectory(tm, speed, yaw_rate, heave)
         R = q_mat(q_yaw(psi))
         iewn = IEWN if earth else np.zeros(3)  # earth = False: the PreintegrationNormal world (no Earth rotation / Coriolis)
         w_b = np.array([0.0, 0.0, yaw_rate]) + R.T @ iewn
@@ -84,12 +90,14 @@ def imu_samples(t0, t1, rate, rng, bg, ba, yaw_rate=5.0 * D2R, earth=True):
 
 # ---------------------------------------------------------------------------------------------- problem
 def make_window(preintegrate, K=10, L=300, seed=2024, full_visibility=False, perturb=True, with_marg=False, pixel_noise=0.5, with_priors=False,
-                gnss_every=2, earth=True, n_ref=5, dt_node=0.5):
+                gnss_every=2, earth=True, n_ref=5, dt_node=0.5, speed=5.0, yaw_rate=5.0 * D2R, heave=True):
     """n_ref: landmark j is anchored in node j mod n_ref (j mod (K - 1) when K <= n_ref).  A larger n_ref spreads the landmarks over more
     nodes, so fewer of them are marginalized with node 0.  The anchor itself draws no random numbers: the default (5) generates the same
     arrays as before the keyword existed.
     dt_node: time between consecutive nodes (s).  Shorter spacing keeps landmarks in view over more nodes: long tracks.  The default (0.5)
-    generates the same arrays as before the keyword existed."""
+    generates the same arrays as before the keyword existed.
+    speed (m/s), yaw_rate (rad/s), heave: the trajectory (see trajectory()); speed = yaw_rate = 0, heave=False is a vehicle standing still,
+    whose landmarks are seen with no parallax.  They draw no random numbers: the defaults generate the same arrays as before they existed."""
     rng = np.random.Generator(np.random.PCG64(seed))
     dtk, rate = dt_node, 200.0
     times = np.arange(K) * dtk
@@ -98,7 +106,7 @@ def make_window(preintegrate, K=10, L=300, seed=2024, full_visibility=False, per
     pose_t = np.zeros((K, 7))
     mix_t = np.zeros((K, 9))
     for k, t in enumerate(times):
-        p, v, _, psi = trajectory(t)
+        p, v, _, psi = trajectory(t, speed, yaw_rate, heave)
         pose_t[k, :3] = p
         pose_t[k, 3:] = q_yaw(psi)
         mix_t[k, :3], mix_t[k, 3:6], mix_t[k, 6:9] = v, bg_true, ba_true
@@ -140,7 +148,7 @@ def make_window(preintegrate, K=10, L=300, seed=2024, full_visibility=False, per
     bg_lin = bg_true + rng.normal(0, 5.0 * D2R / 3600.0, 3)
     ba_lin = ba_true + rng.normal(0, 5.0 * 1e-5, 3)
     for k in range(K - 1):
-        imu = imu_samples(times[k], times[k + 1], rate, rng, bg_true, ba_true, earth=earth)
+        imu = imu_samples(times[k], times[k + 1], rate, rng, bg_true, ba_true, yaw_rate=yaw_rate, earth=earth, speed=speed, heave=heave)
         state16 = np.concatenate([pose_t[k], mix_t[k, :3], bg_lin, ba_lin])
         blob, pn, _ = preintegrate(state16, IEWN if earth else None, GRAVITY, NOISE5, imu)
         blobs[k] = blob

@@ -36,11 +36,14 @@ def make(olib, **kw):
     return synth_ba.make_window(lambda *a: oa.preintegrate(olib, *a), **kw)[0]
 
 
-def compare(g, o, tol_h=5e-6, tol_sqrt=1e-9):
+def compare(g, o, tol_h=5e-6, tol_sqrt=1e-9, sc_floor=0.0):
+    """sc_floor: the smallest column scale.  A window with unobservable directions (a vehicle standing still) has Hp diagonals at rounding
+    level (1e-25); scaled by their own square root, rounding differences look like O(1).  sqrt(EPS) = 1e-4 scales such a column as one at
+    the pseudo-inverse cut, below which the prior keeps nothing of it."""
     assert g["m"] == o["m"] and g["r"] == o["r"]
     assert np.array_equal(g["block_type"], o["block_type"]) and np.array_equal(g["block_node"], o["block_node"])
     assert np.array_equal(g["x0"], o["x0"])
-    sc = np.sqrt(np.abs(np.diag(o["Hp"])))
+    sc = np.maximum(np.sqrt(np.abs(np.diag(o["Hp"]))), sc_floor)
     sc[sc == 0] = 1
     dH = np.abs((g["Hp"] - o["Hp"]) / np.outer(sc, sc)).max()
     db = np.abs((g["bp"] - o["bp"]) / sc).max() / max(1.0, np.abs(o["bp"] / sc).max())
