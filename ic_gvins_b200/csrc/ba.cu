@@ -24,6 +24,7 @@
 //                (panel updates on DMMA), triangular solves, landmark back-substitution, model cost change, candidate x (+) delta
 //   single GPU : lin_vis + lin_cam at the candidate, into the window's second linearisation buffer (its costs are the candidate cost)
 //   cost       : candidate cost (all factors, residuals only) of the split pipeline;   accept : Ceres step acceptance + radius update
+//   ba_lm.cuh  : that trust-region policy (LM diagonal, termination, iteration commit, step decision), shared with ba_split.cuh
 //   ba_marg.cuh: sliding-window marginalization (MarginalizationInfo) on the same device-resident linearisation
 // Kernels only: the host side is ba_handle.cu (lifecycle, the solve) and ba_keyframe.cu (the resident keyframe cycle), through ba_dev.cuh.
 #include <cooperative_groups.h>
@@ -52,6 +53,12 @@ __device__ __forceinline__ int col_pose(int k) { return 6 * k; }
 __device__ __forceinline__ int col_ext(int K) { return 6 * K; }
 __device__ __forceinline__ int col_td(int K) { return 6 * K + 6; }
 __device__ __forceinline__ int col_mix(int K, int k) { return 6 * K + 7 + 9 * k; }
+
+__device__ __forceinline__ double block_sum(double v, double *s_red);
+__device__ __forceinline__ double block_max(double v, double *s_red);
+}  // namespace icg
+#include "ba_lm.cuh"  // the trust-region policy (over the column layout and block_sum above)
+namespace icg {
 
 // ------------------------------------------------------------------------------------------------ lin_vis (+ landmark rows)
 __device__ __forceinline__ int jc_off(int a) { return a < 18 ? (a / 6) * 12 + (a % 6) : 36 + 2 * (a - 18); }  // row 0 offset in a record
@@ -342,8 +349,6 @@ __device__ __forceinline__ double gram2_entry(const BaCaps &C, const BaDev &D, i
 }
 
 // ------------------------------------------------------------------------------------------------ Schur term + reduced camera system
-__device__ __forceinline__ double block_sum(double v, double *s_red);
-__device__ __forceinline__ double block_max(double v, double *s_red);
 __device__ __forceinline__ double *x_inbox(const BaDev &D, int peer, int w, int from);  // ba_split.cuh
 __device__ __forceinline__ int tri_idx(int A, int B, int ncv);
 
@@ -479,7 +484,7 @@ __global__ void __cluster_dims__(BA_SPLIT_W, 1, 1) __launch_bounds__(256) ba_sch
                 if (rr < nr) {
                     const int l = r0 + rr;
                     const double sl = D.scale_l[(size_t) w * C.L + l], hs = sl * sl * hl[l];
-                    ph = sl * sl / (hs + fmin(fmax(hs, 1e-6), 1e32) / radius);
+                    ph = sl * sl / (hs + lm_d2(hs, radius));
                 }
                 sphi[rr] = ph;
             }
@@ -922,12 +927,8 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
         __syncthreads();
         if (tid == 0) st.first = 0;
     }
-    // ---- TrustRegionMinimizer::FinalizeIterationAndCheckIfMinimizerCanContinue
     {
-        int term = 0;
-        if (f_iter >= st.max_iter) term = 1;                                    // NO_CONVERGENCE
-        else if (f_last && gmax_now <= 1e-10) term = 2;                         // gradient tolerance
-        else if (f_last && st.radius <= 1e-32) term = 2;                        // min trust region radius
+        const int term = lm_term(f_iter, st.max_iter, f_last, gmax_now, st.radius);
         if (term) {
             __syncthreads();
             if (tid == 0) st.done = term, st.step_valid = 0;
@@ -956,7 +957,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
     for (int a = tid; a < N; a += SOLVE_THREADS) {
         double h = Hc[(size_t) a * C.NS + a] + (a < NCV ? V[a] : 0.0);
         double hs = s_scale[a] * s_scale[a] * h;
-        s_d2[a] = fmin(fmax(hs, 1e-6), 1e32) / radius;
+        s_d2[a] = lm_d2(hs, radius);
         double gw = a < NCV ? V[2 * NCV + a] : 0.0;
         s_rhs[a] = -s_scale[a] * (s_g[a] - gw);
     }
@@ -1245,7 +1246,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 2) ba_solve(BaCaps C, BaDev D) 
 #pragma unroll
                 for (int u = 0; u < LB; u++) d[u] += (l0 + u < L ? AW[(size_t) (l0 + u) * C.NCA + c] : 0.0) * sx;
             }
-            const double hs = sl * sl * hh, d2 = fmin(fmax(hs, 1e-6), 1e32) / radius, den = hs + d2, sg = sl * gg;
+            const double hs = sl * sl * hh, d2 = lm_d2(hs, radius), den = hs + d2, sg = sl * gg;
             // transposing butterfly: 8 values x 32 lanes -> 1 value per lane in 4 + 2 + 1 + 1 + 1 exchanges (a plain butterfly needs 8 x 5)
             double e4[4], e2[2];
             {
@@ -1387,13 +1388,7 @@ __global__ void __launch_bounds__(128) ba_accept(BaCaps C, BaDev D) {
     const double *R2 = D.red2 + (size_t) w * 4;
     // |x|^2 of the camera-side blocks and of the landmarks
     {
-        const double *pose = D.pose + (size_t) w * C.K * 7, *mix = D.mix + (size_t) w * C.K * 9, *ext = D.ext + (size_t) w * 8;
-        double s = 0;
-        for (int e = tid; e < dm.K * 7; e += 128) s += pose[e] * pose[e];
-        for (int e = tid; e < dm.K * 9; e += 128) s += mix[e] * mix[e];
-        if (tid < 7 && !dm.ext_const) s += ext[tid] * ext[tid];
-        if (tid == 7 && !dm.td_const) s += ext[7] * ext[7];
-        s = block_sum(s, s_red);
+        const double s = lm_cam_sq(C, D, w, dm, s_red);
         double q = 0;  // |rho|^2
         for (int l = tid; l < dm.L; l += 128) q += D.rho[(size_t) w * C.L + l] * D.rho[(size_t) w * C.L + l];
         q = block_sum(q, s_red);
@@ -1419,7 +1414,6 @@ __global__ void __launch_bounds__(128) ba_accept(BaCaps C, BaDev D) {
     }
     __syncthreads();
     if (tid == 0) {
-        s_accept = 0;
         const double mcc = R2[0], sn = R2[1], nfin = R2[2];
         double cand = 0;
         if (st.step_valid) {
@@ -1430,54 +1424,11 @@ __global__ void __launch_bounds__(128) ba_accept(BaCaps C, BaDev D) {
             }
             cand += st.cost_cam[1 - st.lin_buf];
         }
-        if (!st.chol_ok || nfin != 0.0 || !(mcc > 0.0)) {
-            // HandleInvalidStep + LevenbergMarquardtStrategy::StepIsInvalid
-            st.step_valid = 0;
-            st.n_invalid++;
-            if (st.n_invalid >= 5) st.done = 3;  // FAILURE
-            st.radius *= 0.5;
-            st.last_success = 0;
-        } else {
-            st.n_invalid = 0;
-            st.model_cost_change = mcc;
-            st.step_norm = sqrt(sn);
-            st.x_norm = sqrt(s_camsq + s_rhosq);
-            st.cand_cost = cand;
-            // ParameterToleranceReached / FunctionToleranceReached (Ceres trust_region_minimizer.cc)
-            if (st.step_norm <= 1e-8 * (st.x_norm + 1e-8)) {
-                st.done = 2;
-            } else if (fabs(st.x_cost - cand) <= 1e-6 * st.x_cost) {
-                st.done = 2;
-            } else {
-                const double rel = (st.x_cost - cand) / mcc;
-                if (rel > 1e-3) {
-                    s_accept = 1;
-                    st.n_success++;
-                    // LevenbergMarquardtStrategy::StepAccepted
-                    double t = 2.0 * rel - 1.0;
-                    st.radius = fmin(1e16, st.radius / fmax(1.0 / 3.0, 1.0 - t * t * t));
-                    st.decrease_factor = 2.0;
-                    st.last_success = 1;
-                    st.fresh_lin = 1;
-                    st.lin_buf ^= 1;  // the candidate's linearisation is now the one at x
-                } else {
-                    // StepRejected
-                    st.radius = st.radius / st.decrease_factor;
-                    st.decrease_factor *= 2.0;
-                    st.last_success = 0;
-                    st.need_lin = 0;
-                }
-            }
-        }
+        s_accept = lm_decide(st, mcc, sn, nfin, s_camsq + s_rhosq, cand);
+        if (s_accept) st.lin_buf ^= 1;  // the candidate's linearisation is now the one at x
     }
     __syncthreads();
-    if (!s_accept) return;
-    double *pose = D.pose + (size_t) w * C.K * 7, *mix = D.mix + (size_t) w * C.K * 9, *ext = D.ext + (size_t) w * 8, *rho = D.rho + (size_t) w * C.L;
-    const double *pose_c = D.pose_c + (size_t) w * C.K * 7, *mix_c = D.mix_c + (size_t) w * C.K * 9, *ext_c = D.ext_c + (size_t) w * 8, *rho_c = D.rho_c + (size_t) w * C.L;
-    for (int e = tid; e < dm.K * 7; e += 128) pose[e] = pose_c[e];
-    for (int e = tid; e < dm.K * 9; e += 128) mix[e] = mix_c[e];
-    if (tid < 8) ext[tid] = ext_c[tid];
-    for (int e = tid; e < dm.L; e += 128) rho[e] = rho_c[e];
+    if (s_accept) lm_take_cand(C, D, w, dm);
 }
 
 // ------------------------------------------------------------------------------------------------ LM state reset (device side)

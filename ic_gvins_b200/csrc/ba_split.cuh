@@ -114,6 +114,44 @@ __global__ void __launch_bounds__(256) ba_reduce(BaCaps C, BaDev D, unsigned lon
     }
 }
 
+// ------------------------------------------------------------------------------------------------ the owner's solve: what both forms share
+// ba_solve_cam and ba_solve_cam_dsm differ in the factorisation only.  Both snapshot the window's LM state at their start (s0: CTA 0 commits the
+// new state after the first cluster barrier), keep every column vector in each CTA (no DSMEM traffic) and end on CTA 0.  The iteration start
+// (cost and max |g| at x, termination, commit) is spelled out in each kernel from lm_term / lm_begin / split_hdr: as one shared function it
+// changed the register allocation of both kernels.
+
+// column a < N: gradient g, Jacobi scale sc (computed at the first linearisation), LM diagonal d2, right-hand side rh = -sc (g - W phi g_l)
+__device__ __forceinline__ void split_col(const BaCaps &C, const BaDev &D, int w, int NCV, int a, const LmState &s0, double &g, double &sc, double &d2,
+                                          double &rh) {
+    const double *rv = D.S.redv + (size_t) w * D.S.RV;  // [diag H_vis | g_vis | W phi g_l | cost, sum rho^2, max |g_l|]
+    const double gv = lin_gc(C, D, 0, w)[a] + (a < NCV ? rv[NCV + a] : 0.0);
+    const double h = lin_Hc(C, D, 0, w)[(size_t) a * C.NS + a] + (a < NCV ? rv[a] : 0.0);
+    const double sv = s0.first ? 1.0 / (1.0 + sqrt(h)) : D.scale_c[(size_t) w * C.NS + a];
+    g = gv, sc = sv, d2 = lm_d2(sv * sv * h, s0.radius), rh = -sv * (gv - (a < NCV ? rv[2 * NCV + a] : 0.0));
+}
+
+// The header of the step broadcast, the one place its words are written (ba_step_lm reads them):
+// [0] termination (lm_term) | [1] the step is valid | [2] cost at x | [3] max |g| | [4] initial cost | [5] camera part of the model cost change
+__device__ __forceinline__ void split_hdr(double *BC, int term, bool valid, double x_cost, double gmax, double init, double mcc) {
+    BC[0] = (double) term, BC[1] = valid ? 1.0 : 0.0, BC[2] = x_cost, BC[3] = gmax, BC[4] = init, BC[5] = mcc;
+}
+
+// CTA 0, after the factorisation: [header | delta = step' * scale] into every rank's step buffer, then the window's release flag.  x is the
+// solution step' (read only if the factorisation succeeded); nfin counts its non-finite entries.
+__device__ __forceinline__ void split_bcast(const BaDev &D, int w, int N, bool valid, double nfin, const double *x, const double *s_scale, double x_cost,
+                                            double gmax, double init, double mcc, unsigned long long epoch) {
+    const int tid = threadIdx.x;
+    for (int q = 0; q < D.world; q++) {
+        double *BC = x_bcast(D, q, w);
+        if (valid)
+            for (int a = tid; a < N; a += SOLVE_THREADS) BC[SPLIT_HDR + a] = x[a] * s_scale[a];
+        if (tid == 0) split_hdr(BC, 0, valid && nfin == 0.0, x_cost, gmax, init, mcc);
+    }
+    __threadfence_system();
+    __syncthreads();
+    for (int q = tid; q < D.world; q += SOLVE_THREADS) st_release_sys(x_flagB(D, q, w), epoch);
+}
+
 // ------------------------------------------------------------------------------------------------ solve_cam (owner, cluster per window)
 // The camera-side half of ba_solve for systems that do not fit one CTA: S lives packed in global memory (L2-resident, written and read by all
 // CTAs of the cluster between cluster barriers -- cluster.sync orders the global accesses at cluster scope and invalidates L1).
@@ -129,9 +167,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS) ba_solve_cam(BaCaps C, BaDev D,
     const WinDims dm = D.dims[w];
     const int K = dm.K, NCV = 6 * K + 7, N = 15 * K + 7, NR = N + 1;
     const int CT = CL * SOLVE_THREADS, ctid = cr * SOLVE_THREADS + tid, cwarp = ctid >> 5, ncwarps = CT / 32;
-    // snapshot of the LM state (CTA 0 updates it after the first cluster barrier)
-    const int f_first = st.first, f_fresh = st.fresh_lin, f_last = st.last_success, f_iter = st.iter, f_maxit = st.max_iter;
-    const double radius = st.radius, cost_cam = st.cost_cam[0], gmax_old = st.gmax, xcost_old = st.x_cost, init_old = st.initial_cost;
+    const LmState s0 = st;  // snapshot: CTA 0 commits the new state after the first cluster barrier
     double *s_red = sm;                  // 40
     double *s_scale = s_red + 40;        // N
     double *s_g = s_scale + C.NS;        // N
@@ -139,51 +175,27 @@ __global__ void __launch_bounds__(SOLVE_THREADS) ba_solve_cam(BaCaps C, BaDev D,
     double *s_d2 = s_rhs + C.NS;         // N
     double *s_blk = s_d2 + C.NS;         // SPLIT_BS_ROWS x (NS + 1): row block of L for the back-substitution (CTA 0)
     double *S = D.Sglobal + (size_t) (w / D.world) * split_S_stride(C);  // one workspace per OWNED window: packed triangle | pivot reciprocals
-    const double *Hc = lin_Hc(C, D, 0, w), *gcam = lin_gc(C, D, 0, w), *Hs = D.Hs + (size_t) w * C.NS * C.NS;
-    const double *rv = D.S.redv + (size_t) w * D.S.RV;   // [diag H_vis | g_vis | W phi g_l | cost, sum rho^2, max |g_l|]
-    double *scale_c = D.scale_c + (size_t) w * C.NS;
-    // ---- gradient, Jacobi scaling (first linearisation), LM diagonal, rhs: every CTA keeps its own copy (no DSMEM traffic)
-    for (int a = tid; a < N; a += SOLVE_THREADS) {
-        const double g = gcam[a] + (a < NCV ? rv[NCV + a] : 0.0);
-        s_g[a] = g;
-        const double h = Hc[(size_t) a * C.NS + a] + (a < NCV ? rv[a] : 0.0);
-        const double sc = f_first ? 1.0 / (1.0 + sqrt(h)) : scale_c[a];
-        s_scale[a] = sc;
-        const double hs = sc * sc * h;
-        s_d2[a] = fmin(fmax(hs, 1e-6), 1e32) / radius;
-        s_rhs[a] = -sc * (g - (a < NCV ? rv[2 * NCV + a] : 0.0));
-    }
+    const double *Hc = lin_Hc(C, D, 0, w), *Hs = D.Hs + (size_t) w * C.NS * C.NS;
+    for (int a = tid; a < N; a += SOLVE_THREADS) split_col(C, D, w, NCV, a, s0, s_g[a], s_scale[a], s_d2[a], s_rhs[a]);
     __syncthreads();
-    double gmax_now = gmax_old, x_cost = xcost_old;
-    if (f_fresh) {
+    double x_cost = s0.x_cost, gmax = s0.gmax;
+    if (s0.fresh_lin) {
+        const double *rv = D.S.redv + (size_t) w * D.S.RV;
         double gm = 0;
         for (int a = tid; a < N; a += SOLVE_THREADS) gm = fmax(gm, fabs(s_g[a]));
-        gm = fmax(block_max(gm, s_red), rv[3 * NCV + 2]);
-        gmax_now = gm;
-        x_cost = rv[3 * NCV] + cost_cam;
+        gmax = fmax(block_max(gm, s_red), rv[3 * NCV + 2]);
+        x_cost = rv[3 * NCV] + s0.cost_cam[0];
     }
-    int term = 0;
-    if (f_iter >= f_maxit) term = 1;                               // NO_CONVERGENCE
-    else if (f_last && gmax_now <= 1e-10) term = 2;                // gradient tolerance
-    else if (f_last && radius <= 1e-32) term = 2;                  // min trust region radius
+    const int term = lm_term(s0.iter, s0.max_iter, s0.last_success, gmax, s0.radius);
     cluster.sync();  // every CTA has read the state it needs
-    if (cr == 0 && tid == 0) {
-        st.x_cost = x_cost, st.gmax = gmax_now;
-        if (f_first) st.initial_cost = x_cost;
-        st.fresh_lin = 0, st.first = 0, st.need_lin = 0;
-        if (term) st.done = term, st.step_valid = 0;
-        else st.iter = f_iter + 1;
-    }
-    if (cr == 0 && f_first)
-        for (int a = tid; a < N; a += SOLVE_THREADS) scale_c[a] = s_scale[a];
-    double *BC = nullptr;
-    if (term) {
-        // broadcast the termination (header only) and leave
+    if (cr == 0 && tid == 0) lm_begin(st, x_cost, gmax, s0.first ? x_cost : s0.initial_cost, term);
+    if (cr == 0 && s0.first)
+        for (int a = tid; a < N; a += SOLVE_THREADS) D.scale_c[(size_t) w * C.NS + a] = s_scale[a];
+    if (term) {  // broadcast the termination (header only) and leave
         if (cr == 0) {
             __syncthreads();
             for (int q = tid; q < D.world; q += SOLVE_THREADS) {
-                BC = x_bcast(D, q, w);
-                BC[0] = (double) term, BC[1] = 0.0, BC[2] = x_cost, BC[3] = gmax_now, BC[4] = f_first ? x_cost : init_old, BC[5] = 0.0;
+                split_hdr(x_bcast(D, q, w), term, false, x_cost, gmax, s0.first ? x_cost : s0.initial_cost, 0.0);
                 __threadfence_system();
                 st_release_sys(x_flagB(D, q, w), epoch);
             }
@@ -416,7 +428,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS) ba_solve_cam(BaCaps C, BaDev D,
             __syncthreads();
         }
     }
-    // ---- camera part of the model cost change, broadcast of [header | delta = step' * scale]
+    // ---- camera part of the model cost change (-1/2 step'.g' + 1/2 step'.D^2 step'), broadcast of [header | delta]
     double part = 0;
     bool finite = true;
     if (valid)
@@ -427,17 +439,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS) ba_solve_cam(BaCaps C, BaDev D,
         }
     const double mcc = block_sum(part, s_red);
     const double nfin = block_sum(finite ? 0.0 : 1.0, s_red);
-    for (int q = 0; q < D.world; q++) {
-        BC = x_bcast(D, q, w);
-        if (valid)
-            for (int a = tid; a < N; a += SOLVE_THREADS) BC[SPLIT_HDR + a] = y[a] * s_scale[a];
-        if (tid == 0) {
-            BC[0] = 0.0, BC[1] = (valid && nfin == 0.0) ? 1.0 : 0.0, BC[2] = x_cost, BC[3] = gmax_now, BC[4] = f_first ? x_cost : init_old, BC[5] = mcc;
-        }
-    }
-    __threadfence_system();
-    __syncthreads();
-    for (int q = tid; q < D.world; q += SOLVE_THREADS) st_release_sys(x_flagB(D, q, w), epoch);
+    split_bcast(D, w, N, valid, nfin, y, s_scale, x_cost, gmax, s0.first ? x_cost : s0.initial_cost, mcc, epoch);
 }
 
 // ------------------------------------------------------------------------------------------------ solve_cam, distributed-shared-memory form
@@ -515,8 +517,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 1) ba_solve_cam_dsm(BaCaps C, B
     const int ntc = dsm_ntiles(C.N + 1), VL = ntc * 8;   // capacity: tiles per side, vector length
     const int nt = dsm_ntiles(NR), npan = (N + 7) / 8;   // this window: tile rows (incl. the rhs row), column panels
     const int Tn = N >> 3, rn = N & 7;                   // tile row / row in the tile of the augmented right-hand-side row
-    const int f_first = st.first, f_fresh = st.fresh_lin, f_last = st.last_success, f_iter = st.iter, f_maxit = st.max_iter;
-    const double radius = st.radius, cost_cam = st.cost_cam[0], gmax_old = st.gmax, xcost_old = st.x_cost, init_old = st.initial_cost;
+    const LmState s0 = st;  // snapshot: CTA 0 commits the new state after the first cluster barrier
     double *s_red = sm;                       // 40
     double *s_scale = s_red + 40;             // VL each
     double *s_g = s_scale + VL;
@@ -535,20 +536,10 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 1) ba_solve_cam_dsm(BaCaps C, B
     double *s_dg = s_xT + 16;                 // [ntc][64] replicated diagonal tiles
     double *s_P = s_dg + (size_t) ntc * 64;   // [2][ntc][64] panel column, by panel parity
     double *s_tiles = s_P + (size_t) 2 * ntc * 64;
-    const double *Hc = lin_Hc(C, D, 0, w), *gcam = lin_gc(C, D, 0, w), *Hs = D.Hs + (size_t) w * C.NS * C.NS;
-    const double *rv = D.S.redv + (size_t) w * D.S.RV;   // [diag H_vis | g_vis | W phi g_l | cost, sum rho^2, max |g_l|]
-    double *scale_c = D.scale_c + (size_t) w * C.NS;
-    // ---- gradient, Jacobi scaling (first linearisation), LM diagonal, rhs: every CTA keeps its own copy
-    for (int a = tid; a < VL; a += SOLVE_THREADS) {
+    const double *Hc = lin_Hc(C, D, 0, w), *Hs = D.Hs + (size_t) w * C.NS * C.NS;
+    for (int a = tid; a < VL; a += SOLVE_THREADS) {  // zero beyond N
         double g = 0, sc = 0, d2 = 0, rh = 0;
-        if (a < N) {
-            g = gcam[a] + (a < NCV ? rv[NCV + a] : 0.0);
-            const double h = Hc[(size_t) a * C.NS + a] + (a < NCV ? rv[a] : 0.0);
-            sc = f_first ? 1.0 / (1.0 + sqrt(h)) : scale_c[a];
-            const double hs = sc * sc * h;
-            d2 = fmin(fmax(hs, 1e-6), 1e32) / radius;
-            rh = -sc * (g - (a < NCV ? rv[2 * NCV + a] : 0.0));
-        }
+        if (a < N) split_col(C, D, w, NCV, a, s0, g, sc, d2, rh);
         s_g[a] = g, s_scale[a] = sc, s_d2[a] = d2, s_rhs[a] = rh;
         s_y[a] = 0, s_contrib[a] = 0, s_x[a] = 0, s_dinv[a] = 0;
     }
@@ -559,35 +550,24 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 1) ba_solve_cam_dsm(BaCaps C, B
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
-    double gmax_now = gmax_old, x_cost = xcost_old;
-    if (f_fresh) {
+    double x_cost = s0.x_cost, gmax = s0.gmax;
+    if (s0.fresh_lin) {
+        const double *rv = D.S.redv + (size_t) w * D.S.RV;
         double gm = 0;
         for (int a = tid; a < N; a += SOLVE_THREADS) gm = fmax(gm, fabs(s_g[a]));
-        gm = fmax(block_max(gm, s_red), rv[3 * NCV + 2]);
-        gmax_now = gm;
-        x_cost = rv[3 * NCV] + cost_cam;
+        gmax = fmax(block_max(gm, s_red), rv[3 * NCV + 2]);
+        x_cost = rv[3 * NCV] + s0.cost_cam[0];
     }
-    int term = 0;
-    if (f_iter >= f_maxit) term = 1;                               // NO_CONVERGENCE
-    else if (f_last && gmax_now <= 1e-10) term = 2;                // gradient tolerance
-    else if (f_last && radius <= 1e-32) term = 2;                  // min trust region radius
+    const int term = lm_term(s0.iter, s0.max_iter, s0.last_success, gmax, s0.radius);
     cluster.sync();  // every CTA has read the state it needs (and is running: its shared memory and barriers may be used from now on)
-    if (cr == 0 && tid == 0) {
-        st.x_cost = x_cost, st.gmax = gmax_now;
-        if (f_first) st.initial_cost = x_cost;
-        st.fresh_lin = 0, st.first = 0, st.need_lin = 0;
-        if (term) st.done = term, st.step_valid = 0;
-        else st.iter = f_iter + 1;
-    }
-    if (cr == 0 && f_first)
-        for (int a = tid; a < N; a += SOLVE_THREADS) scale_c[a] = s_scale[a];
-    double *BC = nullptr;
-    if (term) {
+    if (cr == 0 && tid == 0) lm_begin(st, x_cost, gmax, s0.first ? x_cost : s0.initial_cost, term);
+    if (cr == 0 && s0.first)
+        for (int a = tid; a < N; a += SOLVE_THREADS) D.scale_c[(size_t) w * C.NS + a] = s_scale[a];
+    if (term) {  // broadcast the termination (header only) and leave
         if (cr == 0) {
             __syncthreads();
             for (int q = tid; q < D.world; q += SOLVE_THREADS) {
-                BC = x_bcast(D, q, w);
-                BC[0] = (double) term, BC[1] = 0.0, BC[2] = x_cost, BC[3] = gmax_now, BC[4] = f_first ? x_cost : init_old, BC[5] = 0.0;
+                split_hdr(x_bcast(D, q, w), term, false, x_cost, gmax, s0.first ? x_cost : s0.initial_cost, 0.0);
                 __threadfence_system();
                 st_release_sys(x_flagB(D, q, w), epoch);
             }
@@ -920,7 +900,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 1) ba_solve_cam_dsm(BaCaps C, B
     cluster.sync();  // the solution has landed on CTA 0; no CTA leaves while its shared memory may still be written
     DSM_CLK(5, tb0)  // backward substitution
     if (cr != 0) return;
-    // ---- camera part of the model cost change, broadcast of [header | delta = step' * scale]
+    // ---- camera part of the model cost change (-1/2 step'.g' + 1/2 step'.D^2 step'), broadcast of [header | delta]
     double part = 0;
     bool finite = true;
     if (valid)
@@ -931,17 +911,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS, 1) ba_solve_cam_dsm(BaCaps C, B
         }
     const double mcc = block_sum(part, s_red);
     const double nfin = block_sum(finite ? 0.0 : 1.0, s_red);
-    for (int q = 0; q < D.world; q++) {
-        BC = x_bcast(D, q, w);
-        if (valid)
-            for (int a = tid; a < N; a += SOLVE_THREADS) BC[SPLIT_HDR + a] = s_x[a] * s_scale[a];
-        if (tid == 0) {
-            BC[0] = 0.0, BC[1] = (valid && nfin == 0.0) ? 1.0 : 0.0, BC[2] = x_cost, BC[3] = gmax_now, BC[4] = f_first ? x_cost : init_old, BC[5] = mcc;
-        }
-    }
-    __threadfence_system();
-    __syncthreads();
-    for (int q = tid; q < D.world; q += SOLVE_THREADS) st_release_sys(x_flagB(D, q, w), epoch);
+    split_bcast(D, w, N, valid, nfin, s_x, s_scale, x_cost, gmax, s0.first ? x_cost : s0.initial_cost, mcc, epoch);
 }
 
 // ------------------------------------------------------------------------------------------------ step_lm (every rank, STEP_SLICES CTAs per window)
@@ -965,14 +935,9 @@ __global__ void __launch_bounds__(SOLVE_THREADS) ba_step_lm(BaCaps C, BaDev D, u
     const double *BC = x_bcast(D, D.rank, w);
     if (tid == 0) wait_flag(x_flagB(D, D.rank, w), epoch, D.S.err);
     __syncthreads();
-    const int term = (int) __ldcg(BC + 0), valid = (int) __ldcg(BC + 1);
+    const int term = (int) __ldcg(BC + 0), valid = (int) __ldcg(BC + 1);  // the header: split_hdr
     double *R3 = D.red2 + (size_t) w * 4;
-    if (!owner && tid == 0 && sl_id == 0) {  // mirror what the owner's solve did to the LM state
-        st.x_cost = __ldcg(BC + 2), st.gmax = __ldcg(BC + 3), st.initial_cost = __ldcg(BC + 4);
-        st.fresh_lin = 0, st.first = 0, st.need_lin = 0;
-        if (term) st.done = term, st.step_valid = 0;
-        else st.iter = st.iter + 1;
-    }
+    if (!owner && tid == 0 && sl_id == 0) lm_begin(st, __ldcg(BC + 2), __ldcg(BC + 3), __ldcg(BC + 4), term);  // the owner's commit
     if (term) return;
     if (!valid) {
         if (tid == 0 && sl_id == 0) {
@@ -1014,7 +979,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS) ba_step_lm(BaCaps C, BaDev D, u
             }
             if (lane < LB && l0 + lane < lend) {
                 const int l = l0 + lane;
-                const double sl = scale_l[l], hs = sl * sl * hl[l], d2 = fmin(fmax(hs, 1e-6), 1e32) / radius;
+                const double sl = scale_l[l], hs = sl * sl * hl[l], d2 = lm_d2(hs, radius);
                 const double sp = (-sl * gl[l] - sl * mine) / (hs + d2);
                 finite = finite && isfinite(sp);
                 step_l[l] = sp;
@@ -1120,67 +1085,21 @@ __global__ void __launch_bounds__(128) ba_accept_split(BaCaps C, BaDev D, unsign
     const WinDims dm = D.dims[w];
     if (tid < D.world) wait_flag(x_flagC(D, D.rank, w, tid), epoch, D.S.err);
     {
-        const double *pose = D.pose + (size_t) w * C.K * 7, *mix = D.mix + (size_t) w * C.K * 9, *ext = D.ext + (size_t) w * 8;
-        double s = 0;
-        for (int e = tid; e < dm.K * 7; e += 128) s += pose[e] * pose[e];
-        for (int e = tid; e < dm.K * 9; e += 128) s += mix[e] * mix[e];
-        if (tid < 7 && !dm.ext_const) s += ext[tid] * ext[tid];
-        if (tid == 7 && !dm.td_const) s += ext[7] * ext[7];
-        s = block_sum(s, s_red);
+        const double s = lm_cam_sq(C, D, w, dm, s_red);
         if (tid == 0) s_camsq = s;
     }
     __syncthreads();
     if (tid == 0) {
-        s_accept = 0;
         double mcc = 0, sn = 0, nfin = 0, cand = 0, rho2 = 0;
         for (int r = 0; r < D.world; r++) {  // fixed rank order on every rank
             const double *s = x_scal(D, D.rank, w, r);
             mcc += __ldcg(s + 0), sn += __ldcg(s + 1), nfin += __ldcg(s + 2), cand += __ldcg(s + 3), rho2 += __ldcg(s + 4);
         }
-        if (!st.chol_ok || nfin != 0.0 || !(mcc > 0.0)) {
-            st.step_valid = 0;
-            st.n_invalid++;
-            if (st.n_invalid >= 5) st.done = 3;
-            st.radius *= 0.5;
-            st.last_success = 0;
-        } else {
-            st.n_invalid = 0;
-            st.model_cost_change = mcc;
-            st.step_norm = sqrt(sn);
-            st.x_norm = sqrt(s_camsq + rho2);
-            st.cand_cost = cand;
-            if (st.step_norm <= 1e-8 * (st.x_norm + 1e-8)) {
-                st.done = 2;
-            } else if (fabs(st.x_cost - cand) <= 1e-6 * st.x_cost) {
-                st.done = 2;
-            } else {
-                const double rel = (st.x_cost - cand) / mcc;
-                if (rel > 1e-3) {
-                    s_accept = 1;
-                    st.n_success++;
-                    const double t = 2.0 * rel - 1.0;
-                    st.radius = fmin(1e16, st.radius / fmax(1.0 / 3.0, 1.0 - t * t * t));
-                    st.decrease_factor = 2.0;
-                    st.last_success = 1;
-                    st.need_lin = 1;
-                    st.fresh_lin = 1;
-                } else {
-                    st.radius = st.radius / st.decrease_factor;
-                    st.decrease_factor *= 2.0;
-                    st.last_success = 0;
-                    st.need_lin = 0;
-                }
-            }
-        }
+        s_accept = lm_decide(st, mcc, sn, nfin, s_camsq + rho2, cand);
+        if (s_accept) st.need_lin = 1;  // x moved: the next attempt linearises it
     }
     __syncthreads();
-    if (!s_accept) return;
-    double *pose = D.pose + (size_t) w * C.K * 7, *mix = D.mix + (size_t) w * C.K * 9, *ext = D.ext + (size_t) w * 8, *rho = D.rho + (size_t) w * C.L;
-    const double *pose_c = D.pose_c + (size_t) w * C.K * 7, *mix_c = D.mix_c + (size_t) w * C.K * 9, *ext_c = D.ext_c + (size_t) w * 8, *rho_c = D.rho_c + (size_t) w * C.L;
-    for (int e = tid; e < dm.K * 7; e += 128) pose[e] = pose_c[e];
-    for (int e = tid; e < dm.K * 9; e += 128) mix[e] = mix_c[e];
-    if (tid < 8) ext[tid] = ext_c[tid];
-    for (int e = tid; e < dm.L; e += 128) rho[e] = rho_c[e];
+    if (s_accept) lm_take_cand(C, D, w, dm);
 }
 
 // ------------------------------------------------------------------------------------------------ after the solve (shard groups, world > 1)
