@@ -69,12 +69,14 @@ def trajectory(t, speed=5.0, yaw_rate=5.0 * D2R, heave=True):
     return p, v, a, psi
 
 
-def imu_samples(t0, t1, rate, rng, bg, ba, yaw_rate=5.0 * D2R, earth=True, speed=5.0, heave=True):
-    """(n, 7) rows: dt, dtheta[3], dvel[3]; row 0 is the sample AT t0 (imu0 of the preintegration)."""
+def imu_samples(t0, t1, rate, rng, bg, ba, yaw_rate=5.0 * D2R, earth=True, speed=5.0, heave=True, noise_scale=1.0):
+    """(n, 7) rows: dt, dtheta[3], dvel[3]; row 0 is the sample AT t0 (imu0 of the preintegration).
+    noise_scale multiplies the white noise; 0 gives noise-free increments.  The same random numbers are drawn whatever its value, and the
+    default (1) generates the same arrays as before the keyword existed."""
     n = int(round((t1 - t0) * rate))
     dt = 1.0 / rate
     out = np.zeros((n + 1, 7))
-    arw, vrw = NOISE5[0], NOISE5[1]
+    arw, vrw = NOISE5[0] * noise_scale, NOISE5[1] * noise_scale
     for i in range(n + 1):
         tm = t0 + (i - 0.5) * dt  # mid-point of the sampling interval ending at t0 + i dt
         p, v, a, psi = trajectory(tm, speed, yaw_rate, heave)
