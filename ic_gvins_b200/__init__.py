@@ -10,6 +10,8 @@ Host-side mirror (Python, over ctypes) of the reference call sites:
   ba.WindowSolver (.solve / .gvins_optimization / .marginalize)
                                                 <- GVINS::gvinsOptimization + ceres::Solver::Solve (ic_gvins.cc:1130-1239),
                                                    MarginalizationInfo::marginalization via gvinsMarginalization (:1412-1640)
+  ins.InsWindow                                 <- ins_window_: runFusion's mechanization, redoInsMechanization, getCameraPoseFromInsWindow
+                                                   (ic_gvins.cc:249-293, misc.cc:30-286) for B streams on the device
 The product path is the CUDA library only; importing this package never touches oracle/.
 """
 from ._lib import IcgError, LIB_PATH, lib  # noqa: F401

@@ -144,6 +144,20 @@ def _declare_r2(L: C.CDLL) -> None:
     L.icg_ba_shard_slide_resident.argtypes = [vp, C.c_int, vp, vp]
     L.icg_ba_shard_slide_integrate_resident.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp]
     L.icg_ba_shard_slide_vision_resident.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp, vp]
+    # ---- INS windows
+    L.icg_ins_create.argtypes = [C.POINTER(vp), C.c_int, C.c_int, C.c_int, vp]
+    L.icg_ins_destroy.argtypes = [vp]
+    L.icg_ins_destroy.restype = None
+    L.icg_ins_push.argtypes = [vp, C.c_int, vp, vp, vp]
+    L.icg_ins_redo.argtypes = [vp, C.c_int, vp, vp, vp, C.c_int, vp]
+    L.icg_ins_camera_pose.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp]
+    L.icg_ins_window.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp]
+    L.icg_ins_sync.argtypes = [vp]
+
+
+class InsConfig(C.Structure):
+    """ctypes image of `icg_ins_config`."""
+    _fields_ = [("with_earth", C.c_int32), ("gravity", C.c_double * 3), ("iewn", C.c_double * 3)]
 
 
 class SlideWindow(C.Structure):
@@ -187,4 +201,5 @@ EXPORTS = [
     "icg_klt_triangulate_dev", "icg_klt_triangulate",
     "icg_imu_preintegrate", "icg_ba_create", "icg_ba_destroy", "icg_ba_solve", "icg_ba_upload", "icg_ba_run", "icg_ba_download",
     "icg_ba_sync", "icg_ba_shard_export", "icg_ba_shard_connect", "icg_ba_shard_error", "icg_ba_shard_leave", "icg_ba_gvins_optimization", "icg_ba_run_gvins", "icg_ba_gvins_optimization_begin", "icg_ba_gvins_optimization_end", "icg_ba_residual_costs", "icg_ba_reproj_evaluate", "icg_ba_imu_evaluate", "icg_ba_marginalize", "icg_ba_marginalize_resident", "icg_ba_update_and_cull_resident", "icg_ba_marginalize_resident_culled", "icg_ba_reintegrate_resident", "icg_ba_slide_resident", "icg_ba_slide_integrate_resident", "icg_ba_slide_vision_resident", "icg_ba_shard_reintegrate_resident", "icg_ba_shard_slide_resident", "icg_ba_shard_slide_integrate_resident", "icg_ba_shard_slide_vision_resident", "icg_ba_gnss_evaluate", "icg_ba_pose_prior_evaluate", "icg_ba_mix_prior_evaluate", "icg_ba_imu_error_evaluate", "icg_ba_marg_factor_evaluate",
+    "icg_ins_create", "icg_ins_destroy", "icg_ins_push", "icg_ins_redo", "icg_ins_camera_pose", "icg_ins_window", "icg_ins_sync",
 ]

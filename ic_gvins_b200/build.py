@@ -33,6 +33,7 @@ SOURCES = {
     "preint.cu": ["-fmad=false"],      # IMU propagation, warp per interval: the sums of geom_core.cuh's preintegrate_core, bit for bit
     "ba_slide.cu": ["-fmad=false"],    # slide to the next window: the prior's normal equations are icg_ba_upload's host sums, bit for bit
     "ba_vision.cu": ["-fmad=false"],   # the next window's vision rows: pixel2cam as the host computes it (subtract, then divide)
+    "ins.cu": ["-fmad=false"],         # INS windows: insMechanization in geom_core.cuh's operation order, as preint.cu runs it
 }
 
 

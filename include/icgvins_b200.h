@@ -890,6 +890,53 @@ int icg_ba_imu_error_evaluate(icg_ba *h, const double *mix, double *residuals, d
 int icg_ba_marg_factor_evaluate(icg_ba *h, int r, int nblocks, const int32_t *block_type, const double *const *parameters, const double *x0,
                                 const double *J0, const double *e0, double *residuals, double **jacobians);
 
+/* ===================================================================================================== *
+ *  INS windows: the per-stream IMU recurrence that gives every frame its prior camera pose
+ * ===================================================================================================== */
+/* One handle holds max_streams INS windows (GVINS::ins_window_, IG/ic_gvins.h), each a ring of `capacity` entries on the device.  An entry
+ * is one IMU row (time, dt, dtheta[3], dvel[3]) and the state after it (time, p[3], q_xyzw[4], v[3], bg[3], ba[3]).  The handle mirrors each
+ * stream's count, last sample time and "mechanized" flag on the host, so every check of icg_ins_push runs before the device is written.
+ * A stream is "mechanized" from its first icg_ins_redo with status 1 on (GVINS::gvinsInitialization followed by the redo at
+ * IG/ic_gvins.cc:301-306 and :683); before that its pushes take runFusion's initialization path.
+ * capacity is in [1000, 65536]: 1000 = MAXIMUM_INS_NUMBER (IG/ic_gvins.h:124), the most an unmechanized window holds; up to 65537 entries the
+ * binary search of getInsWindowIndex (misc.cc:30-65) ends within the 16 halvings its `counts++ > 15` cap allows, so the cap never triggers. */
+typedef struct icg_ins icg_ins;
+typedef struct icg_ins_config { /* integration_config_ (IG/ic_gvins.cc:99-106, 675-678), one per stream */
+    int32_t with_earth;         /* iswithearth: the Earth form of insMechanization (Coriolis, gravity, Earth rotation) or the Normal form */
+    double gravity[3];          /* (0, 0, g) */
+    double iewn[3];             /* Earth::iewn(origin, p) set at initialization; unused when with_earth == 0 */
+} icg_ins_config;
+int icg_ins_create(icg_ins **h, int max_streams, int capacity, int device, void *stream);
+void icg_ins_destroy(icg_ins *h);
+/* runFusion's per-sample step (IG/ic_gvins.cc:249-293) for streams 0 .. n_streams-1: rows off[s] .. off[s+1]-1 of imu (HOST, 8 doubles per
+ * row: time, dt, dtheta[3], dvel[3]) belong to stream s, cfg (HOST) holds n_streams configurations.
+ *   mechanized stream: each row is insMechanization(imu_pre = the window's last row, imu_cur = the row) (misc.cc:151-206) from the window's
+ *                      last state, and the state is stored with the row (:284-286);
+ *   otherwise:         the row is appended with a zero state and the window keeps its newest 1000 rows (:288-293).
+ * The reference redoes instead of mechanizing the one sample that arrives while isoptimized_ is set (:272-280).  A push followed by
+ * icg_ins_redo gives the same window, because the redo rewrites every state from its index on.
+ * ICG_EINVAL, before anything is launched and with every window unchanged: a row time not greater than the stream's previous one, or a
+ * mechanized stream that would exceed capacity (the reference's window only shrinks at a redo).  Asynchronous. */
+int icg_ins_push(icg_ins *h, int n_streams, const icg_ins_config *cfg, const int32_t *off, const double *imu);
+/* redoInsMechanization (misc.cc:208-261) of streams 0 .. n_streams-1 from state17 (HOST, n x 17: time, p, q_xyzw, v, bg, ba =
+ * statedatalist_.back(); q is normalised as stateFromData does, preintegration_base.cc:115-125).  redo (HOST, n; NULL: all) selects streams.
+ * The window is re-mechanized from getInsWindowIndex(state time) with isNeedInterpolation's four cases (:229-242; MINIMUM_TIME_INTERVAL =
+ * 1e-4), then index - reserved entries are dropped from the front when index >= reserved (:253-260; the reference's reserved_ins_num_ is 2,
+ * IG/ic_gvins.cc:82).  status (HOST, n): 1 redone, 0 not selected, -1 index == 0 (the reference logs and leaves the window unchanged).
+ * Synchronous. */
+int icg_ins_redo(icg_ins *h, int n_streams, const icg_ins_config *cfg, const uint8_t *redo, const double *state17, int reserved, int8_t *status);
+/* getCameraPoseFromInsWindow (misc.cc:67-108; called at IG/ic_gvins.cc:527-533) of streams 0 .. n_streams-1 at stamp[s] = frame->stamp()
+ * + td (HOST), with pose_b_c (HOST, n x 12: R row-major, t).  dev_pose (DEVICE, n x 12): Pose::R row-major, Pose::t, as icg_track_frame
+ * takes them.  host_pose (HOST or NULL: then the call is asynchronous and nothing is copied back) receives the same values.  found (HOST when
+ * host_pose is given, else DEVICE, or NULL): 1 interpolated, 0 outside the window (the back state's pose, the reference's `false`), -1 the
+ * window was never mechanized (pose not written). */
+int icg_ins_camera_pose(icg_ins *h, int n_streams, const double *stamp, const double *pose_b_c, double *dev_pose, double *host_pose,
+                        int32_t *found);
+/* One stream's window, oldest first (tests, and the navigation output of ins_window_.back(), IG/ic_gvins.cc:382-389): *count receives the
+ * window's size, the first min(count, cap) entries go to imu8 (HOST, cap x 8) and state17 (HOST, cap x 17).  Synchronous. */
+int icg_ins_window(icg_ins *h, int stream, int cap, int32_t *count, double *imu8, double *state17);
+int icg_ins_sync(icg_ins *h);
+
 #ifdef __cplusplus
 }
 #endif
