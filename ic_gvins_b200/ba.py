@@ -756,13 +756,14 @@ class WindowSolver:
         return out
 
     # -- single-factor Evaluate (Ceres CostFunction contract), computed on the device
-    def reproj_evaluate(self, pose0, pose1, ext, invdepth, td, const14, std, want_jac=True):
+    def reproj_evaluate(self, pose0, pose1, ext, invdepth, td, const14, std, want_jac=True, frames=False):
+        """frames=True: the node-frame form of ba_lin_vis / ba_cost (icg_ba_reproj_evaluate_frames)"""
         a = [np.ascontiguousarray(x, np.float64) for x in (pose0, pose1, ext, np.atleast_1d(invdepth), np.atleast_1d(td), const14)]
         r = np.zeros(2)
         Js = [np.zeros((2, 7)), np.zeros((2, 7)), np.zeros((2, 7)), np.zeros((2, 1)), np.zeros((2, 1))]
         jp = (vp * 5)(*[vp(j.ctypes.data) for j in Js])
-        check(lib().icg_ba_reproj_evaluate(self._h, *[vp(x.ctypes.data) for x in a], float(std), vp(r.ctypes.data),
-                                           jp if want_jac else None), "icg_ba_reproj_evaluate")
+        name = "icg_ba_reproj_evaluate_frames" if frames else "icg_ba_reproj_evaluate"
+        check(getattr(lib(), name)(self._h, *[vp(x.ctypes.data) for x in a], float(std), vp(r.ctypes.data), jp if want_jac else None), name)
         return r, Js
 
     def gnss_evaluate(self, pose, blh, std3, lever):

@@ -1500,9 +1500,16 @@ __global__ void ba_residual_costs_kernel(BaCaps C, BaDev D, double *reproj_cost,
     }
 }
 
-__global__ void ba_reproj_eval_kernel(const double *in /* 7+7+8+1+1+14+1 */, double *out /* 2 + 14+14+14+2+2 */) {
+// frames != 0: the node-frame form ba_lin_vis and ba_cost run (node_frame of both poses and the extrinsic, then reproj_eval_frames)
+__global__ void ba_reproj_eval_kernel(const double *in /* 7+7+8+1+1+14+1 */, double *out /* 2 + 14+14+14+2+2 */, int frames) {
     double r[2], Ji[12], Jj[12], Je[12], Jr[2], Jt[2];
-    reproj_eval(in, in + 7, in + 14, in[22], in[23], in + 24, 1.0 / in[38], true, r, Ji, Jj, Je, Jr, Jt);
+    if (frames) {
+        double Fi[NODE_FRAME_LD], Fj[NODE_FRAME_LD], Fe[NODE_FRAME_LD];
+        node_frame(in, Fi), node_frame(in + 7, Fj), node_frame(in + 14, Fe);
+        reproj_eval_frames(Fi, Fj, Fe, in[22], in[23], in + 24, 1.0 / in[38], true, r, Ji, Jj, Je, Jr, Jt);
+    } else {
+        reproj_eval(in, in + 7, in + 14, in[22], in[23], in + 24, 1.0 / in[38], true, r, Ji, Jj, Je, Jr, Jt);
+    }
     out[0] = r[0], out[1] = r[1];
     double *o = out + 2;
     const double *src[3] = {Ji, Jj, Je};

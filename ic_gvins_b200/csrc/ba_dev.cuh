@@ -165,7 +165,7 @@ __global__ void ba_reset_state(BaDev D, LmState *save, int n, int max_iter);
 __global__ void ba_chi2_cull(BaCaps C, BaDev D, int *counters);
 __global__ void ba_set_gnss_huber(BaDev D, int n, int v);
 __global__ void ba_residual_costs_kernel(BaCaps C, BaDev D, double *reproj_cost, double *gnss_cost);
-__global__ void ba_reproj_eval_kernel(const double *in, double *out);
+__global__ void ba_reproj_eval_kernel(const double *in, double *out, int frames);
 __global__ void ba_imu_eval_kernel(const double *blob, const double *U, const double *x, double *out);
 __global__ void ba_small_factor_eval_kernel(int kind, const double *in, double *out);
 __global__ void ba_marg_factor_eval_kernel(const double *in, double *out);

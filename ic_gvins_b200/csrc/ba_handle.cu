@@ -1142,10 +1142,10 @@ int icg_ba_residual_costs(icg_ba *h, const icg_ba_problem *problem, double *repr
     return ICG_OK;
 }
 
-int icg_ba_reproj_evaluate(icg_ba *h, const double *pose0, const double *pose1, const double *ext, const double *invdepth, const double *td,
-                           const double *c14, double std_, double *residuals, double **jacobians) {
+static int reproj_evaluate(icg_ba *h, const char *name, int frames, const double *pose0, const double *pose1, const double *ext, const double *invdepth,
+                           const double *td, const double *c14, double std_, double *residuals, double **jacobians) {
     if (!h || !pose0 || !pose1 || !ext || !invdepth || !td || !c14 || !residuals) {
-        set_error("icg_ba_reproj_evaluate: bad arguments");
+        set_error("%s: bad arguments", name);
         return ICG_EINVAL;
     }
     ICG_CUDA(cudaSetDevice(h->device));
@@ -1155,7 +1155,7 @@ int icg_ba_reproj_evaluate(icg_ba *h, const double *pose0, const double *pose1, 
     memcpy(in + 24, c14, 112);
     in[38] = std_;
     ICG_CUDA(cudaMemcpyAsync(h->scratch.d, in, sizeof(double) * 40, cudaMemcpyHostToDevice, h->stream));
-    ba_reproj_eval_kernel<<<1, 1, 0, h->stream>>>(h->scratch.d, h->scratch.d + 64);
+    ba_reproj_eval_kernel<<<1, 1, 0, h->stream>>>(h->scratch.d, h->scratch.d + 64, frames);
     count_launch();
     ICG_CUDA(cudaMemcpyAsync(h->scratch.h + 64, h->scratch.d + 64, sizeof(double) * 48, cudaMemcpyDeviceToHost, h->stream));
     ICG_CUDA(cudaStreamSynchronize(h->stream));
@@ -1168,6 +1168,16 @@ int icg_ba_reproj_evaluate(icg_ba *h, const double *pose0, const double *pose1, 
         if (jacobians[4]) jacobians[4][0] = o[46], jacobians[4][1] = o[47];
     }
     return ICG_OK;
+}
+
+int icg_ba_reproj_evaluate(icg_ba *h, const double *pose0, const double *pose1, const double *ext, const double *invdepth, const double *td,
+                           const double *c14, double std_, double *residuals, double **jacobians) {
+    return reproj_evaluate(h, "icg_ba_reproj_evaluate", 0, pose0, pose1, ext, invdepth, td, c14, std_, residuals, jacobians);
+}
+
+int icg_ba_reproj_evaluate_frames(icg_ba *h, const double *pose0, const double *pose1, const double *ext, const double *invdepth, const double *td,
+                                  const double *c14, double std_, double *residuals, double **jacobians) {
+    return reproj_evaluate(h, "icg_ba_reproj_evaluate_frames", 1, pose0, pose1, ext, invdepth, td, c14, std_, residuals, jacobians);
 }
 
 int icg_ba_imu_evaluate(icg_ba *h, const double *blob, const double *pose0, const double *mix0, const double *pose1, const double *mix1,

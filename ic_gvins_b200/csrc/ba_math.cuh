@@ -154,7 +154,8 @@ BAM_HD void reproj_eval(const double *pi, const double *pj, const double *ext, d
     V3 pts0 = mk(c[0], c[1], c[2]), pts1 = mk(c[3], c[4], c[5]), vel0 = mk(c[6], c[7], c[8]), vel1 = mk(c[9], c[10], c[11]);
     // FP64 division is ~20 instructions on this part and the reference's form has 15 of them per factor (x / depth, the Eigen inverse() of two
     // quaternions = conjugate / squaredNorm per component, two projections, the reduce matrix): one reciprocal per distinct divisor instead
-    // (4 divisions); each quotient differs from the divided form by at most 1.5 ulp, far inside the 1e-12 parity bar of the factor tests.
+    // (4 divisions); each quotient differs from the divided form by at most 1.5 ulp, inside the per-entry first-order rounding bound that
+    // tests/test_factor_edges_gpu.py holds this function to.
     V3 pts_0_td = pts0 - (td - c[12]) * vel0;
     V3 pts_1_td = pts1 - (td - c[13]) * vel1;
     const double inv_id0 = 1.0 / id0;
@@ -198,8 +199,10 @@ BAM_HD void reproj_eval(const double *pi, const double *pj, const double *ext, d
 // its reference node, its observing node and the extrinsic -- K + 1 distinct rotations per window against ~2700 factors -- so the CTA
 // builds them once (node_frame: R = toRotationMatrix(q) row-major | p) and the factor does matrix-vector products: four of them replace the
 // reference's quaternion sandwich products and the two quaternion inverses, and the Jacobian rows use the same matrices.  For the unit
-// quaternions PoseParameterization::Plus maintains, q v q^-1 = R(q) v and q^-1 v q = R(q)^T v up to rounding (the factor tests hold this
-// form to the oracle's quaternion form at 1e-12).  About 40 % fewer FP64 instructions per factor than reproj_eval.
+// quaternions PoseParameterization::Plus maintains, q v q^-1 = R(q) v and q^-1 v q = R(q)^T v up to rounding (tests/test_factor_edges_gpu.py
+// holds this form, through icg_ba_reproj_evaluate_frames, to a high-precision restatement of the reference's quaternion form entry by entry
+// at a first-order rounding bound, with quaternions up to 4 ulp per component off the unit sphere).  About 40 % fewer FP64 instructions per
+// factor than reproj_eval.
 constexpr int NODE_FRAME_LD = 13;  // 9 + 3, padded to an odd length (shared-memory banks)
 BAM_HD void node_frame(const double *pose7, double *F) {
     const M3 R = qmat(pose_q(pose7));

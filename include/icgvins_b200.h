@@ -870,6 +870,10 @@ int icg_ba_residual_costs(icg_ba *h, const icg_ba_problem *problem, double *repr
  * residuals[2]; jacobians row-major 2x7, 2x7, 2x7, 2x1, 2x1 (any may be NULL).  Computed on the device. */
 int icg_ba_reproj_evaluate(icg_ba *h, const double *pose0, const double *pose1, const double *ext, const double *invdepth,
                            const double *td, const double *f_const14, double std, double *residuals, double **jacobians);
+/* The same factor in the node-frame form ba_lin_vis and ba_cost run: R = toRotationMatrix(q) of both poses and the extrinsic (node_frame),
+ * R^T in place of each quaternion inverse (reproj_eval_frames).  Same arguments and outputs as icg_ba_reproj_evaluate. */
+int icg_ba_reproj_evaluate_frames(icg_ba *h, const double *pose0, const double *pose1, const double *ext, const double *invdepth,
+                                  const double *td, const double *f_const14, double std, double *residuals, double **jacobians);
 /* PreintegrationFactor::Evaluate (IG/preintegration/preintegration_factor.h:45): residuals[15], jacobians 15x7,15x9,15x7,15x9 */
 int icg_ba_imu_evaluate(icg_ba *h, const double *imu_blob, const double *pose0, const double *mix0, const double *pose1,
                         const double *mix1, double *residuals, double **jacobians);

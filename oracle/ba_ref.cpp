@@ -672,6 +672,46 @@ inline void huber(double s, double rho[3]) {
     }
 }
 
+// The loss as the solver applies it to one residual block: no loss, cost = 0.5 |r|^2; HuberLoss(1.0), cost = 0.5 rho(|r|^2) and the
+// Corrector (ceres corrector.cc; the reference's own copy: factors/residual_block_info.h:59-87) on the residuals and on every non-null
+// global Jacobian J[i] (nres x gsize[i], row-major).
+void apply_loss(bool hub, int nres, double *r, int nb, double *const *J, const int *gsize, double &cost) {
+    double sq = 0;
+    for (int k = 0; k < nres; k++) sq += r[k] * r[k];
+    if (!hub) {
+        cost = 0.5 * sq;
+        return;
+    }
+    double rho[3];
+    huber(sq, rho);
+    cost = 0.5 * rho[0];
+    const double sqrt_rho1 = std::sqrt(rho[1]);
+    double residual_scaling, alpha_sq_norm;
+    if (sq == 0.0 || rho[2] <= 0.0) {
+        residual_scaling = sqrt_rho1;
+        alpha_sq_norm    = 0.0;
+    } else {
+        const double D     = 1.0 + 2.0 * sq * rho[2] / rho[1];
+        const double alpha = 1.0 - std::sqrt(D);
+        residual_scaling   = sqrt_rho1 / (1 - alpha);
+        alpha_sq_norm      = alpha / sq;
+    }
+    for (int i = 0; J && i < nb; i++) {
+        if (!J[i]) continue;
+        const int gs = gsize[i];
+        if (alpha_sq_norm == 0.0) {
+            for (int e = 0; e < nres * gs; e++) J[i][e] *= sqrt_rho1;
+        } else {
+            for (int c = 0; c < gs; c++) {
+                double rtj = 0;
+                for (int k = 0; k < nres; k++) rtj += r[k] * J[i][(size_t) k * gs + c];
+                for (int k = 0; k < nres; k++) J[i][(size_t) k * gs + c] = sqrt_rho1 * (J[i][(size_t) k * gs + c] - alpha_sq_norm * r[k] * rtj);
+            }
+        }
+    }
+    for (int k = 0; k < nres; k++) r[k] *= residual_scaling;
+}
+
 struct EvalBlock {  // one residual block's corrected residuals + local Jacobians
     int nres;
     std::vector<double> r;
@@ -700,43 +740,10 @@ void evaluate_block(const Program &P, const Residual &R, bool want_jac, EvalBloc
         }
     }
     R.cost->Evaluate(params.data(), E.r.data(), want_jac ? jp.data() : nullptr);
-    double sq = 0;
-    for (double v : E.r) sq += v * v;
-    if (!R.huber) {
-        E.cost = 0.5 * sq;
-    } else {
-        double rho[3];
-        huber(sq, rho);
-        E.cost = 0.5 * rho[0];
-        // Corrector (ceres corrector.cc; the reference's own copy: factors/residual_block_info.h:59-87)
-        const double sqrt_rho1 = std::sqrt(rho[1]);
-        double residual_scaling, alpha_sq_norm;
-        if (sq == 0.0 || rho[2] <= 0.0) {
-            residual_scaling = sqrt_rho1;
-            alpha_sq_norm    = 0.0;
-        } else {
-            const double D     = 1.0 + 2.0 * sq * rho[2] / rho[1];
-            const double alpha = 1.0 - std::sqrt(D);
-            residual_scaling   = sqrt_rho1 / (1 - alpha);
-            alpha_sq_norm      = alpha / sq;
-        }
-        if (want_jac) {
-            for (int i = 0; i < nb; i++) {
-                if (!jp[i]) continue;
-                const int gs = P.blocks[R.blocks[i]].gsize;
-                if (alpha_sq_norm == 0.0) {
-                    for (auto &v : Jg[i]) v *= sqrt_rho1;
-                } else {
-                    for (int c = 0; c < gs; c++) {
-                        double rtj = 0;
-                        for (int k = 0; k < nres; k++) rtj += E.r[k] * Jg[i][(size_t) k * gs + c];
-                        for (int k = 0; k < nres; k++) Jg[i][(size_t) k * gs + c] = sqrt_rho1 * (Jg[i][(size_t) k * gs + c] - alpha_sq_norm * E.r[k] * rtj);
-                    }
-                }
-            }
-        }
-        for (auto &v : E.r) v *= residual_scaling;
-    }
+    static thread_local std::vector<int> gs;
+    gs.resize(nb);
+    for (int i = 0; i < nb; i++) gs[i] = P.blocks[R.blocks[i]].gsize;
+    apply_loss(R.huber, nres, E.r.data(), nb, want_jac ? jp.data() : nullptr, gs.data(), E.cost);
     if (want_jac) {
         E.J.resize(nb);
         for (int i = 0; i < nb; i++) {
@@ -1516,6 +1523,24 @@ int icgo_gnss_eval(const double *pose, const double *blh, const double *std3, co
     const double *params[1] = {pose};
     double *Jp[1] = {J};
     f.Evaluate(params, r, J ? Jp : nullptr);
+    return 0;
+}
+
+// The same factors with the loss the solver applies (huber = 0: none), through apply_loss: corrected residuals and global Jacobians, and
+// the block's cost (evaluate_block's arithmetic)
+int icgo_reproj_eval_loss(const double *pose0, const double *pose1, const double *ext, const double *invdepth, const double *td, const double *c,
+                          double std_, int huber, double *r, double **J, double *cost) {
+    icgo_reproj_eval(pose0, pose1, ext, invdepth, td, c, std_, r, J);
+    const int gs[5] = {7, 7, 7, 1, 1};
+    apply_loss(huber != 0, 2, r, 5, J, gs, *cost);
+    return 0;
+}
+
+int icgo_gnss_eval_loss(const double *pose, const double *blh, const double *std3, const double *lever, int huber, double *r, double *J, double *cost) {
+    icgo_gnss_eval(pose, blh, std3, lever, r, J);
+    const int gs[1] = {7};
+    double *Jp[1] = {J};
+    apply_loss(huber != 0, 3, r, 1, J ? Jp : nullptr, gs, *cost);
     return 0;
 }
 

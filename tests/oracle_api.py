@@ -64,6 +64,8 @@ def declare_ba(lib):
     lib.icgo_imu_eval.argtypes = [vp, vp, C.c_int, vp, vp, vp, vp, vp, vp]
     lib.icgo_gnss_eval.argtypes = [vp, vp, vp, vp, vp, vp]
     lib.icgo_pose_prior_eval.argtypes = [vp, vp, vp, vp, vp]
+    lib.icgo_reproj_eval_loss.argtypes = [vp, vp, vp, vp, vp, vp, C.c_double, C.c_int, vp, vp, vp]
+    lib.icgo_gnss_eval_loss.argtypes = [vp, vp, vp, vp, C.c_int, vp, vp, vp]
     lib.icgo_pose_plus.argtypes = [vp, vp, vp]
     lib.icgo_pose_plus.restype = None
     lib.icgo_ba_marginalize.argtypes = [C.POINTER(BaProblem), vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp]
@@ -148,6 +150,23 @@ def imu_eval(lib, blob, pn, pose0, mix0, pose1, mix1, want_jac=True):
     jp = (vp * 4)(*[vp(j.ctypes.data) for j in Js])
     lib.icgo_imu_eval(_p(a[0]), _p(a[1]), a[1].size // 4, _p(a[2]), _p(a[3]), _p(a[4]), _p(a[5]), _p(r), jp if want_jac else None)
     return r, Js
+
+
+def reproj_eval_loss(lib, pose0, pose1, ext, rho, td, c14, std, huber):
+    """ReprojectionFactor with the loss the solver applies (evaluate_block's apply_loss): corrected r, global Jacobians, cost"""
+    a = [np.ascontiguousarray(x, np.float64) for x in (pose0, pose1, ext, np.atleast_1d(rho), np.atleast_1d(td), c14)]
+    r, cost = np.zeros(2), np.zeros(1)
+    Js = [np.zeros((2, 7)), np.zeros((2, 7)), np.zeros((2, 7)), np.zeros((2, 1)), np.zeros((2, 1))]
+    jp = (vp * 5)(*[vp(j.ctypes.data) for j in Js])
+    lib.icgo_reproj_eval_loss(*[_p(x) for x in a], float(std), int(huber), _p(r), jp, _p(cost))
+    return r, Js, float(cost[0])
+
+
+def gnss_eval_loss(lib, pose, blh, std3, lever, huber):
+    a = [np.ascontiguousarray(x, np.float64) for x in (pose, blh, std3, lever)]
+    r, J, cost = np.zeros(3), np.zeros((3, 7)), np.zeros(1)
+    lib.icgo_gnss_eval_loss(*[_p(x) for x in a], int(huber), _p(r), _p(J), _p(cost))
+    return r, J, float(cost[0])
 
 
 def pose_plus(lib, x, d):
