@@ -154,11 +154,27 @@ def _declare_r2(L: C.CDLL) -> None:
     L.icg_ins_camera_pose.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp]
     L.icg_ins_window.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp]
     L.icg_ins_sync.argtypes = [vp]
+    L.icg_ins_gins_initialize.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp, C.c_int, vp]
 
 
 class InsConfig(C.Structure):
     """ctypes image of `icg_ins_config`."""
     _fields_ = [("with_earth", C.c_int32), ("gravity", C.c_double * 3), ("iewn", C.c_double * 3)]
+
+
+class GinsInit(C.Structure):
+    """ctypes image of `icg_gins_init`."""
+    _fields_ = [("gnss_time", C.c_double), ("gnss_blh", C.c_double * 3), ("gnss_std", C.c_double * 3),
+                ("last_time", C.c_double), ("last_blh", C.c_double * 3), ("last_std", C.c_double * 3),
+                ("last_yaw_valid", C.c_int32), ("last_yaw", C.c_double), ("origin_blh", C.c_double * 3), ("gravity", C.c_double),
+                ("antlever", C.c_double * 3), ("imudatarate", C.c_double)]
+
+
+class GinsInitOut(C.Structure):
+    """ctypes image of `icg_gins_init_out`."""
+    _fields_ = [("status", C.c_int32), ("has_zero_velocity", C.c_int32), ("bg", C.c_double * 3), ("initatt", C.c_double * 3),
+                ("state17", C.c_double * 34), ("pose_prior", C.c_double * 7), ("pose_prior_std", C.c_double * 6), ("mix_prior", C.c_double * 9),
+                ("mix_prior_std", C.c_double * 9), ("imu_blob", C.c_double * 480), ("n_series", C.c_int32)]
 
 
 class SlideWindow(C.Structure):
@@ -202,5 +218,5 @@ EXPORTS = [
     "icg_klt_triangulate_dev", "icg_klt_triangulate",
     "icg_imu_preintegrate", "icg_ba_create", "icg_ba_destroy", "icg_ba_solve", "icg_ba_upload", "icg_ba_run", "icg_ba_download",
     "icg_ba_sync", "icg_ba_shard_export", "icg_ba_shard_connect", "icg_ba_shard_error", "icg_ba_shard_leave", "icg_ba_gvins_optimization", "icg_ba_run_gvins", "icg_ba_gvins_optimization_begin", "icg_ba_gvins_optimization_end", "icg_ba_residual_costs", "icg_ba_reproj_evaluate", "icg_ba_reproj_evaluate_frames", "icg_ba_imu_evaluate", "icg_ba_marginalize", "icg_ba_marginalize_resident", "icg_ba_update_and_cull_resident", "icg_ba_marginalize_resident_culled", "icg_ba_reintegrate_resident", "icg_ba_slide_resident", "icg_ba_slide_integrate_resident", "icg_ba_slide_vision_resident", "icg_ba_shard_reintegrate_resident", "icg_ba_shard_slide_resident", "icg_ba_shard_slide_integrate_resident", "icg_ba_shard_slide_vision_resident", "icg_ba_gnss_evaluate", "icg_ba_pose_prior_evaluate", "icg_ba_mix_prior_evaluate", "icg_ba_imu_error_evaluate", "icg_ba_marg_factor_evaluate",
-    "icg_ins_create", "icg_ins_destroy", "icg_ins_push", "icg_ins_redo", "icg_ins_camera_pose", "icg_ins_window", "icg_ins_sync",
+    "icg_ins_create", "icg_ins_destroy", "icg_ins_push", "icg_ins_redo", "icg_ins_gins_initialize", "icg_ins_camera_pose", "icg_ins_window", "icg_ins_sync",
 ]

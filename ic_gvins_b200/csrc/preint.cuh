@@ -72,7 +72,23 @@ struct PreintSlide {
     double *out_blob;               // per item x ICG_IMU_BLOB_DOUBLES, or NULL
 };
 
+// icg_ins_gins_initialize (ins.cu): the first GNSS time node's factor of each stream gvinsInitialization initialized, from its state17[0]
+// as a slide's ICG_SLIDE_ROW item starts (stateFromData's q.normalize() added, as for an old node), into blob and end_state10
+struct PreintGins {
+    int n;                      // streams
+    const int32_t *status;      // DEVICE, all below too: per stream; only status 1 is integrated
+    const double *state17;      // per stream: time, p, q_xyzw, v, bg, ba
+    const double *gravity;      // per stream: g, the preintegration's gravity (0, 0, g)
+    const int32_t *earth;       // per stream: PreintegrationEarth (iewn = Earth::iewn(station, p)) or PreintegrationNormal
+    const double *imu;          // per stream: rows (dt, dtheta[3], dvel[3]), max_rows apart
+    const int32_t *nrow;
+    int max_rows;
+    double noise5[5], station[3];
+    double *blob, *ends;        // per stream x ICG_IMU_BLOB_DOUBLES, x 10
+};
+
 cudaError_t preint_batch_launch(const PreintBatch &a, cudaStream_t stream);
+cudaError_t preint_gins_launch(const PreintGins &a, cudaStream_t stream);
 cudaError_t preint_resident_launch(const PreintResident &a, cudaStream_t stream);
 cudaError_t preint_slide_launch(const PreintSlide &a, cudaStream_t stream);
 // loads the resident and slide kernels (a shard group loads every kernel its calls launch when it is set up)

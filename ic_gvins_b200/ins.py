@@ -2,14 +2,18 @@
 redo (MISC::redoInsMechanization, misc.cc:208-261) and each frame's prior camera pose (MISC::getCameraPoseFromInsWindow, misc.cc:67-108).
 
 Rows are (time, dt, dtheta[3], dvel[3]); states are (time, p[3], q_xyzw[4], v[3], bg[3], ba[3]); poses are (R row-major, t), 12 doubles.
-A configuration is a dict {"with_earth": bool, "gravity": (3,), "iewn": (3,)} or a list of them, one per stream."""
+A configuration is a dict {"with_earth": bool, "gravity": (3,), "iewn": (3,)} or a list of them, one per stream.
+
+InsWindow.gins_initialize is GVINS::gvinsInitialization (ic_gvins.cc:584-692) for B streams: an initialization input is a dict with the
+fields of icg_gins_init (gnss_time, gnss_blh, last_time, last_blh, last_yaw_valid, last_yaw, origin_blh, gravity, antlever, imudatarate;
+gnss_std / last_std optional)."""
 from __future__ import annotations
 
 import ctypes as C
 
 import numpy as np
 
-from ._lib import InsConfig, check, lib, vp
+from ._lib import GinsInit, GinsInitOut, InsConfig, check, lib, vp
 
 RESERVED_INS_NUM = 2  # GVINS::reserved_ins_num_ (ic_gvins.cc:82)
 
@@ -65,6 +69,34 @@ class InsWindow:
         check(lib().icg_ins_redo(self._h, n, _configs(cfg, n), vp(sel.ctypes.data) if sel is not None else None, vp(st.ctypes.data), int(reserved),
                                  vp(status.ctypes.data)), "icg_ins_redo")
         return status
+
+    def gins_initialize(self, inits, cfg, noise5, station3=(0.0, 0.0, 0.0), sel=None, reserved: int = RESERVED_INS_NUM):
+        """gvinsInitialization of the selected streams (sel: n flags, None: all).  Returns (out, cfg): out is a dict of numpy arrays over the
+        n streams -- status (1 initialized, 0 not selected, -1 .. -5 as icg_ins_gins_initialize), has_zero_velocity, bg (n, 3), initatt (n, 3),
+        state17 (n, 2, 17), pose_prior (n, 7), pose_prior_std (n, 6), mix_prior (n, 9), mix_prior_std (n, 9), imu_blob (n, 480), n_series --
+        and cfg the configurations as the call left them (gravity and, in the Earth form, iewn set where status == 1)."""
+        n = len(inits)
+        c = _configs(cfg, n)
+        arr = (GinsInit * max(n, 1))()
+        for s, g in enumerate(inits):
+            a = arr[s]
+            for k in ("gnss_time", "last_time", "last_yaw", "gravity", "imudatarate"):
+                setattr(a, k, float(g.get(k, 0.0)))
+            a.last_yaw_valid = 1 if g.get("last_yaw_valid", False) else 0
+            for k in ("gnss_blh", "gnss_std", "last_blh", "last_std", "origin_blh", "antlever"):
+                getattr(a, k)[:] = [float(x) for x in g.get(k, (0.0, 0.0, 0.0))]
+        res = (GinsInitOut * max(n, 1))()
+        nz = np.ascontiguousarray(np.asarray(noise5, np.float64).reshape(5))
+        stn = np.ascontiguousarray(np.asarray(station3, np.float64).reshape(3))
+        sl = None if sel is None else np.ascontiguousarray(np.asarray(sel, np.uint8).reshape(n))
+        check(lib().icg_ins_gins_initialize(self._h, n, c, vp(sl.ctypes.data) if sl is not None else None, arr, vp(nz.ctypes.data),
+                                            vp(stn.ctypes.data), int(reserved), res), "icg_ins_gins_initialize")
+        out = {k: np.array([getattr(res[s], k) for s in range(n)], np.int32) for k in ("status", "has_zero_velocity", "n_series")}
+        for k, shape in (("bg", (3,)), ("initatt", (3,)), ("state17", (2, 17)), ("pose_prior", (7,)), ("pose_prior_std", (6,)),
+                         ("mix_prior", (9,)), ("mix_prior_std", (9,)), ("imu_blob", (480,))):
+            out[k] = np.array([np.ctypeslib.as_array(getattr(res[s], k)) for s in range(n)], np.float64).reshape((n,) + shape)
+        cfg_out = [{"with_earth": bool(c[s].with_earth), "gravity": tuple(c[s].gravity), "iewn": tuple(c[s].iewn)} for s in range(n)]
+        return out, cfg_out
 
     def camera_pose(self, stamp, pose_b_c, dev_pose=None):
         """Prior camera poses at stamp (n,) with pose_b_c (n x 12 or one 12-vector for all).  dev_pose: a torch float64 CUDA tensor (n, 12)
