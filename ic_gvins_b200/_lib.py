@@ -155,6 +155,11 @@ def _declare_r2(L: C.CDLL) -> None:
     L.icg_ins_window.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp]
     L.icg_ins_sync.argtypes = [vp]
     L.icg_ins_gins_initialize.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp, C.c_int, vp]
+    # ---- the window solver's IMU sample store, filled from the INS windows
+    L.icg_ba_imu_samples_from_ins.argtypes = [vp, vp, C.c_int, vp]
+    L.icg_ba_slide_ins_resident.argtypes = [vp, vp, C.c_int, vp, vp, vp, vp, vp, vp]
+    L.icg_ba_reintegrate_stored_resident.argtypes = [vp, C.c_int, vp, vp, vp, vp]
+    L.icg_ba_imu_samples.argtypes = [vp, C.c_int, C.c_int, vp, vp]
 
 
 class InsConfig(C.Structure):
@@ -192,6 +197,16 @@ class SlideIntegrate(C.Structure):
                 ("status", C.POINTER(C.c_int8)), ("blob_out", f64p), ("end_state10", f64p)]
 
 
+class InsCut(C.Structure):
+    """ctypes image of `icg_ba_ins_cut`."""
+    _fields_ = [("stream", C.c_int32), ("node_time", f64p)]
+
+
+class SlideIns(C.Structure):
+    """ctypes image of `icg_ba_slide_ins`."""
+    _fields_ = [("integ", SlideIntegrate), ("stream", C.c_int32), ("node_time", f64p), ("merge_src", i32p), ("n_rows", i32p)]
+
+
 class SlideVision(C.Structure):
     """ctypes image of `icg_ba_slide_vision` (device pointers as void *)."""
     _fields_ = [("num_marg", C.c_int32), ("node_in_map", u8p), ("obs_factor", i32p), ("cam", C.c_double * 10), ("node_td", f64p),
@@ -219,4 +234,5 @@ EXPORTS = [
     "icg_imu_preintegrate", "icg_ba_create", "icg_ba_destroy", "icg_ba_solve", "icg_ba_upload", "icg_ba_run", "icg_ba_download",
     "icg_ba_sync", "icg_ba_shard_export", "icg_ba_shard_connect", "icg_ba_shard_error", "icg_ba_shard_leave", "icg_ba_gvins_optimization", "icg_ba_run_gvins", "icg_ba_gvins_optimization_begin", "icg_ba_gvins_optimization_end", "icg_ba_residual_costs", "icg_ba_reproj_evaluate", "icg_ba_reproj_evaluate_frames", "icg_ba_imu_evaluate", "icg_ba_marginalize", "icg_ba_marginalize_resident", "icg_ba_update_and_cull_resident", "icg_ba_marginalize_resident_culled", "icg_ba_reintegrate_resident", "icg_ba_slide_resident", "icg_ba_slide_integrate_resident", "icg_ba_slide_vision_resident", "icg_ba_shard_reintegrate_resident", "icg_ba_shard_slide_resident", "icg_ba_shard_slide_integrate_resident", "icg_ba_shard_slide_vision_resident", "icg_ba_gnss_evaluate", "icg_ba_pose_prior_evaluate", "icg_ba_mix_prior_evaluate", "icg_ba_imu_error_evaluate", "icg_ba_marg_factor_evaluate",
     "icg_ins_create", "icg_ins_destroy", "icg_ins_push", "icg_ins_redo", "icg_ins_gins_initialize", "icg_ins_camera_pose", "icg_ins_window", "icg_ins_sync",
+    "icg_ba_imu_samples_from_ins", "icg_ba_slide_ins_resident", "icg_ba_reintegrate_stored_resident", "icg_ba_imu_samples",
 ]

@@ -265,19 +265,22 @@ def imu_preintegrate(state16, iewn, gravity, noise5, imu):
     return blob, end
 
 
-def _integ_struct(s, g, m, arg):
-    """fill one icg_ba_slide_integrate from an `integrate` dict of WindowSolver.slide_integrate (m = next n_imu)"""
+def _integ_struct(s, g, m, arg, with_rows=True):
+    """fill one icg_ba_slide_integrate from an `integrate` dict of WindowSolver.slide_integrate (m = next n_imu; with_rows False: imu /
+    imu_off stay NULL, the rows come from the device)"""
     from ._lib import u8p
     if g.get("imu_from") is not None:
         s.imu_from = arg(g["imu_from"], np.int32, ip)
-        if "imu_off" in g:
-            imu, off = g["imu"], g["imu_off"]
+        if not with_rows:
+            pass
+        elif "imu_off" in g:
+            s.imu, s.imu_off = arg(g["imu"], np.float64, dp), arg(g["imu_off"], np.int32, ip)
         else:
             rows = [np.zeros((0, 7)) if r is None else np.asarray(r, np.float64).reshape(-1, 7) for r in g["imu_rows"]]
             off = np.zeros(m + 1, np.int32)
             off[1:] = np.cumsum([len(r) for r in rows])
             imu = np.concatenate(rows, axis=0) if rows else np.zeros((0, 7))
-        s.imu, s.imu_off = arg(imu, np.float64, dp), arg(off, np.int32, ip)
+            s.imu, s.imu_off = arg(imu, np.float64, dp), arg(off, np.int32, ip)
         s.gravity3 = arg(np.broadcast_to(np.asarray(g["gravity"], np.float64), (m, 3)), np.float64, dp)
         s.normal = arg(np.broadcast_to(np.asarray(g.get("normal", False), np.uint8), (m,)), np.uint8, u8p)
         if g.get("state16") is not None:
@@ -293,7 +296,7 @@ class WindowSolver:
 
     def __init__(self, max_windows=1, max_K=10, max_L=300, max_F=2700, max_gnss=16, max_marg_r=160, device=0, stream=None):
         self._h = vp()
-        self.max_L, self.max_F = max_L, max_F
+        self.max_L, self.max_F, self.max_K = max_L, max_F, max_K
         check(lib().icg_ba_create(C.byref(self._h), max_windows, max_K, max_L, max_F, max_gnss, max_marg_r, device,
                                   vp(stream) if stream else None), "icg_ba_create")
 
@@ -464,7 +467,14 @@ class WindowSolver:
         and the same IMU rows, and every rank reintegrates the same factors, bit for bit."""
         return self._reintegrate("icg_ba_shard_reintegrate_resident", problems, noise5, station, imu_rows, reintegrate)
 
-    def _reintegrate(self, fn, problems, noise5, station, imu_rows, reintegrate=None):
+    def reintegrate_stored(self, problems, noise5, station=(0.0, 0.0, 0.0), reintegrate=None):
+        """reintegrate() with every factor's rows from the handle's sample store (icg_ba_reintegrate_stored_resident): filled by
+        imu_samples_from_ins() or slide_ins(), and not replaced by an upload or another slide since."""
+        if isinstance(problems, dict):
+            problems = [problems]
+        return self._reintegrate("icg_ba_reintegrate_stored_resident", problems, noise5, station, [None] * len(problems), reintegrate, stored=True)
+
+    def _reintegrate(self, fn, problems, noise5, station, imu_rows, reintegrate=None, stored=False):
         """GVINS::doReintegration (IG/ic_gvins.cc:1680-1695) on the windows this handle has just solved (icg_ba_reintegrate_resident).  noise5 =
         gyr_arw, acc_vrw, gyr_bias_std, acc_bias_std, corr_time; station = parameters_->station (the reference leaves it at (0, 0, 0));
         imu_rows[w] = the n_imu row arrays (m_k, 7) of window w's factors (None for a window left alone); reintegrate: per-window flags
@@ -488,7 +498,7 @@ class WindowSolver:
             io[w].reintegrate = flags[w] if m > 0 else 0
             io[w].status, io[w].blob_out = o["status"].ctypes.data_as(C.POINTER(C.c_int8)), o["blobs"].ctypes.data_as(dp)
             io[w].end_state10 = o["end_states"].ctypes.data_as(dp)
-            if io[w].reintegrate:
+            if io[w].reintegrate and not stored:
                 rows = [np.asarray(x, np.float64).reshape(-1, 7) for x in imu_rows[w]]
                 off = np.zeros(m + 1, np.int32)
                 off[1:] = np.cumsum([len(x) for x in rows])
@@ -595,6 +605,112 @@ class WindowSolver:
         self._keep, self._n = arr, n
         return outs
 
+    def imu_samples_from_ins(self, ins, streams, node_times) -> None:
+        """Seeds the handle's IMU sample store (icg_ba_imu_samples_from_ins): factor k of resident window w gets getImuSeriesFromTo(
+        node_times[w][k], node_times[w][k + 1]) cut from stream streams[w] of `ins` (an ins.InsWindow on this handle's device).  Call it right
+        after the upload of windows whose INS windows still cover their spans."""
+        from ._lib import InsCut
+        n = len(streams)
+        cut = (InsCut * n)()
+        keep = []
+        for w in range(n):
+            t = np.ascontiguousarray(node_times[w], np.float64)
+            keep.append(t)
+            cut[w].stream, cut[w].node_time = int(streams[w]), t.ctypes.data_as(dp)
+        check(lib().icg_ba_imu_samples_from_ins(self._h, ins._h, n, cut), "icg_ba_imu_samples_from_ins")
+
+    def imu_samples(self, w: int):
+        """The stored rows of resident window w (icg_ba_imu_samples): a list with one (m, 7) array per IMU factor, None for a factor without
+        samples."""
+        # the call writes the window's n_imu + 1 offsets: room for the most a window of this handle holds, the rest left at a sentinel
+        off = np.full(self.max_K + 1, np.iinfo(np.int32).min, np.int32)
+        check(lib().icg_ba_imu_samples(self._h, int(w), 0, vp(off.ctypes.data), None), "icg_ba_imu_samples")
+        m = int(np.nonzero(off != np.iinfo(np.int32).min)[0][-1])
+        total = int(off[m])
+        rows = np.zeros((total, 7))
+        if total:
+            check(lib().icg_ba_imu_samples(self._h, int(w), total, vp(off.ctypes.data), vp(rows.ctypes.data)), "icg_ba_imu_samples")
+        out = []
+        for k in range(m):
+            if off[k] < 0:
+                out.append(None)
+                continue
+            end = next((int(off[j]) for j in range(k + 1, m + 1) if off[j] >= 0), total)
+            out.append(rows[off[k]:end].copy())
+        return out
+
+    def slide_ins(self, next_problems, carry, integrate, ins, streams, node_times, merge_src, noise5, station=(0.0, 0.0, 0.0), vision=None,
+                  prior_from_marg=True):
+        """slide_integrate() (vision given: slide_vision() with `integrate`) whose integrated factors' rows come from the device
+        (icg_ba_slide_ins_resident): NODE / SLIDE_CHAIN factor k of window w is cut from stream streams[w] of `ins` over node_times[w][k] ..
+        node_times[w][k + 1] (next K entries); a SLIDE_ROW factor k is old factors merge_src[w][k] and merge_src[w][k] + 1 of the sample store;
+        carried factors keep their stored rows.  `integrate` dicts as slide_integrate takes them, without imu_rows / imu / imu_off.  Returns
+        slide_integrate()'s dicts (vision: slide_vision()'s), each with n_rows (every new factor's stored rows, -1: none).  Status -2 marks a
+        factor whose interval the INS window cannot serve (the call raises IcgError, the handle unchanged)."""
+        from ._lib import IcgError, SlideIns, SlideIntegrate
+        fn = "icg_ba_slide_ins_resident"
+        n = len(next_problems)
+        keep = []
+        n_rows = [np.full(int(p["n_imu"]), -1, np.int32) for p in next_problems]
+        statuses = [np.zeros(int(p["n_imu"]), np.int8) for p in next_problems]
+        blobs = [np.zeros((int(p["n_imu"]), IMU_BLOB)) for p in next_problems]
+        ends = [np.zeros((int(p["n_imu"]), 10)) for p in next_problems]
+
+        def arg(a, dtype, ptr):
+            a = np.ascontiguousarray(a, dtype)
+            keep.append(a)
+            return a.ctypes.data_as(ptr)
+
+        def call(arr, cw, iw, nz, stn, vw):
+            io = (SlideIns * n)()
+            for w, p in enumerate(next_problems):
+                m = int(p["n_imu"])
+                if iw is not None:
+                    io[w].integ = iw[w]
+                elif integrate is not None and integrate[w]:
+                    _integ_struct(io[w].integ, integrate[w], m, arg, with_rows=False)
+                g = io[w].integ
+                g.status, g.blob_out = statuses[w].ctypes.data_as(C.POINTER(C.c_int8)), blobs[w].ctypes.data_as(dp)
+                g.end_state10 = ends[w].ctypes.data_as(dp)
+                io[w].stream = int(streams[w])
+                if node_times[w] is not None:
+                    io[w].node_time = arg(node_times[w], np.float64, dp)
+                if merge_src is not None and merge_src[w] is not None:
+                    io[w].merge_src = arg(merge_src[w], np.int32, ip)
+                io[w].n_rows = n_rows[w].ctypes.data_as(ip)
+            return lib().icg_ba_slide_ins_resident(self._h, ins._h, n, arr, cw, io, vp(nz.ctypes.data), vp(stn.ctypes.data), vw)
+
+        def results():
+            return [dict(status=statuses[w], blobs=blobs[w], end_states=ends[w], n_rows=n_rows[w]) for w in range(n)]
+
+        if vision is not None:
+            try:
+                res = self._slide_vision(fn, next_problems, carry, vision, integrate, noise5, station, prior_from_marg, call=call)
+            except IcgError as e:
+                e.results = results()
+                raise
+            for w, r in enumerate(res):
+                r.update(results()[w])
+            return res
+        from ._lib import SlideWindow
+        flags = [prior_from_marg] * n if np.isscalar(prior_from_marg) else list(prior_from_marg)
+        arr = (BaProblem * n)(*[to_struct(p) for p in next_problems])
+        cw = (SlideWindow * n)()
+        for w, c in enumerate(carry):
+            for k in ("node_src", "lm_src", "f_src", "imu_src", "gnss_src"):
+                if c.get(k) is not None:
+                    setattr(cw[w], k, arg(c[k], np.int32, ip))
+            cw[w].prior_from_marg = 1 if flags[w] else 0
+        nz = np.ascontiguousarray(noise5, np.float64)
+        stn = np.ascontiguousarray(station, np.float64)
+        rc = call(arr, cw, None, nz, stn, None)
+        if rc != 0:
+            err = IcgError(f"{fn} failed with code {rc}: {lib().icg_last_error().decode('utf-8', 'replace')}")
+            err.code, err.results = rc, results()
+            raise err
+        self._keep, self._n = arr, n
+        return results()
+
     def slide_vision(self, next_problems, carry, vision, integrate=None, noise5=None, station=(0.0, 0.0, 0.0), prior_from_marg=True):
         return self._slide_vision("icg_ba_slide_vision_resident", next_problems, carry, vision, integrate, noise5, station, prior_from_marg)
 
@@ -605,7 +721,8 @@ class WindowSolver:
         lm_origin: old shard-local landmark or -(j + 1) for global new point j, nan_flags: old shard L + every new point, set on its own rank)."""
         return self._slide_vision("icg_ba_shard_slide_vision_resident", next_problems, carry, vision, integrate, noise5, station, prior_from_marg)
 
-    def _slide_vision(self, fn, next_problems, carry, vision, integrate=None, noise5=None, station=(0.0, 0.0, 0.0), prior_from_marg=True):
+    def _slide_vision(self, fn, next_problems, carry, vision, integrate=None, noise5=None, station=(0.0, 0.0, 0.0), prior_from_marg=True,
+                      call=None):
         """slide() (integrate given: slide_integrate()) whose vision rows are built on the device (icg_ba_slide_vision_resident):
         addReprojectionParameters + addReprojectionFactors on the culled window this handle holds plus the new keyframes' observations.  The
         last update_and_cull() of these windows must be current.  next_problems' L, F, invdepth, f_lm / f_ref / f_obs / f_const, f_active and
@@ -654,7 +771,7 @@ class WindowSolver:
                     setattr(cw[w], k, arg(c[k], np.int32, ip))
             cw[w].prior_from_marg = 1 if flags[w] else 0
             if iw is not None and integrate[w]:
-                _integ_struct(iw[w], integrate[w], int(p["n_imu"]), arg)
+                _integ_struct(iw[w], integrate[w], int(p["n_imu"]), arg, with_rows=call is None)
             s = vw[w]
             s.num_marg = int(v["num_marg"])
             s.node_in_map = arg(v["node_in_map"], np.uint8, bp)
@@ -682,8 +799,11 @@ class WindowSolver:
             s.lm_origin, s.nan_flags = o["lm_origin"].ctypes.data_as(ip), o["nan_flags"].ctypes.data_as(bp)
         nz = np.ascontiguousarray(noise5 if noise5 is not None else np.zeros(5), np.float64)
         stn = np.ascontiguousarray(station, np.float64)
-        rc = getattr(lib(), fn)(self._h, n, arr, cw, None if iw is None else iw, vp(nz.ctypes.data) if iw is not None else None,
-                                vp(stn.ctypes.data) if iw is not None else None, vw)
+        if call is not None:  # slide_ins: the INS form of the call, from the same structs
+            rc = call(arr, cw, iw, nz, stn, vw)
+        else:
+            rc = getattr(lib(), fn)(self._h, n, arr, cw, None if iw is None else iw, vp(nz.ctypes.data) if iw is not None else None,
+                                    vp(stn.ctypes.data) if iw is not None else None, vw)
         if rc != 0:
             err = IcgError(f"{fn} failed with code {rc}: {lib().icg_last_error().decode('utf-8', 'replace')}")
             err.code = rc

@@ -864,6 +864,9 @@ void icg_ba_destroy(icg_ba *h) {
     for (double *p : {h->M.H0, h->M.b0, h->M.G1, h->M.V1, h->M.lam1, h->M.Z})
         if (p) cudaFree(p);
     if (h->slide_old) cudaFree(h->slide_old);
+    for (double *p : {h->store_d[0], h->store_d[1], h->cut_rows})
+        if (p) cudaFree(p);
+    if (h->ins_ev) cudaEventDestroy(h->ins_ev);
     if (h->fc_alt) cudaFree(h->fc_alt);
     if (h->slide_ev) cudaEventDestroy(h->slide_ev);
     for (void *p : h->dev_only) cudaFree(p);
@@ -884,6 +887,7 @@ int icg_ba_upload(icg_ba *h, int n, const icg_ba_problem *P) {
     const BaCaps &C = h->C;
     h->marg_res_n = 0;  // the marginalization workspace no longer belongs to the windows the handle holds
     h->cull_res_n = 0;
+    h->store_valid = false;  // the IMU factors are next's now, without samples
     int rc = pack_windows(h, n, P, true);
     if (rc != ICG_OK) return rc;
     rc = upload_structure(h, n);

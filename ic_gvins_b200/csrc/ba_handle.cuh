@@ -129,6 +129,18 @@ struct icg_ba {
     // icg_ba_upload from the landmark's first factor, carried by every slide, read by icg_ba_slide_vision_resident
     double *lm_ref = nullptr, *lm_ref_alt = nullptr;
     cudaEvent_t slide_ev = nullptr;  // recorded after the staging's H2D
+    // every IMU factor's samples (imu_buffer_), filled from the INS windows by icg_ba_imu_samples_from_ins / icg_ba_slide_ins_resident.  Rows
+    // (dt, dtheta[3], dvel[3]) window after window, factor after factor, in store_d[store_cur]; a call builds the next store in the other
+    // buffer and swaps only when it commits.  Valid while no upload or other slide has replaced the windows' structure since the last fill
+    double *store_d[2] = {nullptr, nullptr};
+    size_t store_cap[2] = {0, 0};  // rows
+    int store_cur = 0;
+    bool store_valid = false;
+    std::vector<std::vector<int>> store_row0, store_nrow;  // per window and factor: first row, row count (-1: the factor has no samples)
+    HostDev<unsigned char> store_stage;                    // [cut jobs | row counts | statuses | gather segments], grown on demand
+    double *cut_rows = nullptr;                            // the series cut out of the INS windows, before the gather
+    size_t cut_cap = 0;                                    // rows
+    cudaEvent_t ins_ev = nullptr;                          // recorded on the INS handle's stream, waited on by this one
     // post-solve calls of a shard group (world > 1): integer exchanges so far (slot parity), epoch of the last marginalization export, the
     // exchange's device word, the export's slot lists, the owner's gathered rows with their tables, and the handle the owner uploads its
     // gathered windows to (created on first use, recreated when a batch needs more landmarks, factors or windows)

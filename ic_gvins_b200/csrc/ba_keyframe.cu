@@ -8,6 +8,7 @@
 
 #include "ba_handle.cuh"
 #include "ba_vision.cuh"
+#include "ins_handle.cuh"
 #include "preint.cuh"
 
 using namespace icg;
@@ -534,10 +535,18 @@ static int resident_single_rank(icg_ba *h, int n_windows, const icg_ba_problem *
     return ICG_OK;
 }
 
+// Every IMU factor's rows already on the device (the handle's sample store, or the next one a slide builds): factor k of window w is rows
+// row0[w][k] .. + nrow[w][k] of d (nrow -1: no samples)
+struct FactorRows {
+    const double *d;
+    const std::vector<std::vector<int>> &row0, &nrow;
+};
+
 // ---- doReintegration (IG/ic_gvins.cc:1680-1695) on the resident IMU factors (preint.cu)
+// fr: the rows are the store's (icg_ba_reintegrate_stored_resident), io's imu / imu_off are not read
 // sharded (icg_ba_shard_reintegrate_resident): every rank runs the same reintegration on its replicated states, after the group agreed
 static int reint_body(icg_ba *h, int n_windows, const icg_ba_problem *problems, const double *noise5, const double *station3, icg_ba_reint_window *io,
-                      const char *fn, bool sharded) {
+                      const char *fn, bool sharded, const FactorRows *fr = nullptr) {
     const int n = n_windows;
     // validation first: nothing is launched on bad input
     size_t n_items = 0, n_rows = 0;
@@ -556,9 +565,18 @@ static int reint_body(icg_ba *h, int n_windows, const icg_ba_problem *problems, 
                 return ICG_EINVAL;
             }
             if (!c.reintegrate || p.n_imu == 0) continue;
-            if (!c.imu || !c.imu_off || !c.status || !c.blob_out) {
+            if ((!fr && (!c.imu || !c.imu_off)) || !c.status || !c.blob_out) {
                 set_error("%s: window %d: arrays missing", fn, w);
                 return ICG_EINVAL;
+            }
+            if (fr) {
+                for (int k = 0; k < p.n_imu; k++)
+                    if (k >= (int) fr->nrow[w].size() || fr->nrow[w][k] < 1) {
+                        set_error("%s: window %d IMU factor %d has no samples in the store", fn, w, k);
+                        return ICG_EINVAL;
+                    }
+                n_items += p.n_imu;
+                continue;
             }
             if (c.imu_off[0] < 0) {
                 set_error("%s: window %d: imu_off[0] is negative", fn, w);
@@ -617,6 +635,10 @@ static int reint_body(icg_ba *h, int n_windows, const icg_ba_problem *problems, 
             const icg_ba_reint_window &c = io[w];
             if (!c.reintegrate || p.n_imu == 0) continue;
             first[w] = (int) it;
+            if (fr) {
+                for (int k = 0; k < p.n_imu; k++, it++) items[it] = ReintItem{w, k, fr->row0[w][k], fr->nrow[w][k]};
+                continue;
+            }
             const int r0 = c.imu_off[0], nr = c.imu_off[p.n_imu] - r0;
             memcpy(H + i_rows + 56 * row, c.imu + 7 * (size_t) r0, 56 * (size_t) nr);
             for (int k = 0; k < p.n_imu; k++, it++)
@@ -627,7 +649,7 @@ static int reint_body(icg_ba *h, int n_windows, const icg_ba_problem *problems, 
     *(int *) (H + o_cnt) = 0;
     ICG_CUDA(cudaMemcpyAsync(Dv, H, o_status, cudaMemcpyHostToDevice, s));
     PreintResident a;
-    a.n = (int) n_items, a.item = (const ReintItem *) (Dv + i_item), a.imu = (const double *) (Dv + i_rows);
+    a.n = (int) n_items, a.item = (const ReintItem *) (Dv + i_item), a.imu = fr ? fr->d : (const double *) (Dv + i_rows);
     a.pose = h->D.pose, a.mix = h->D.mix, a.blob = h->D.imu_blob, a.U = h->D.imu_U, a.K = C.K;
     for (int k = 0; k < 5; k++) a.noise5[k] = noise5[k];
     for (int k = 0; k < 3; k++) a.station[k] = station3[k];
@@ -696,10 +718,11 @@ static int shard_group_only(icg_ba *h, const char *fn, const char *plain) {
 // rank writes its device, and with `integ` a second one on the integration's outcome.  A rank that rejects joins the agreement all the same
 // (fail below), so its peers never wait for it.  The owner of window w forms its prior from the workspace of mx_h; the other ranks get zeros.
 // lm_ref_built: vision_body has written the next windows' reference rows into lm_ref_alt already; seed (sharded): vision_body's fingerprint of
-// its own arguments, which the agreement's fingerprint continues
+// its own arguments, which the agreement's fingerprint continues; fr (icg_ba_slide_ins_resident): the integrated factors' rows are the next
+// sample store's, integ's imu / imu_off are not read
 static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba_slide_window *carry, const icg_ba_slide_integrate *integ,
                       const double *noise5, const double *station3, const char *fn, bool sharded, bool lm_ref_built = false,
-                      const ArgPrint *seed = nullptr) {
+                      const ArgPrint *seed = nullptr, const FactorRows *fr = nullptr) {
     bool joined = false;  // sharded: this rank has joined the agreement of the call
     std::vector<WinDims> old_dims;
     std::vector<std::vector<int>> old_slot;
@@ -834,16 +857,16 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
                 set_error("%s: window %d: imu_from[%d] is ICG_SLIDE_CHAIN, but no integrated factor precedes it", fn, w, k);
                 return fail(ICG_EINVAL);
             }
-            if (!g.gravity3 || !g.imu || !g.imu_off || (src == ICG_SLIDE_ROW && !g.state16)) {
+            if (!g.gravity3 || (!fr && (!g.imu || !g.imu_off)) || (src == ICG_SLIDE_ROW && !g.state16)) {
                 set_error("%s: window %d: arrays missing", fn, w);
                 return fail(ICG_EINVAL);
             }
-            if (g.imu_off[k] < 0 || (long long) g.imu_off[k + 1] - g.imu_off[k] < 1) {
+            if (fr ? fr->nrow[w][k] < 1 : g.imu_off[k] < 0 || (long long) g.imu_off[k + 1] - g.imu_off[k] < 1) {
                 set_error("%s: window %d factor %d: imu_off must give every integrated interval at least one row", fn, w, k);
                 return fail(ICG_EINVAL);
             }
             io[k] = (int) n_item++;
-            n_row += (size_t) (g.imu_off[k + 1] - g.imu_off[k]);
+            if (!fr) n_row += (size_t) (g.imu_off[k + 1] - g.imu_off[k]);
             n_state += src == ICG_SLIDE_ROW;
         }
         for (int j = 0; g.node_from_imu && j < p.K; j++) {
@@ -947,12 +970,17 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
             }
             if (g && item_of[w][k] >= 0) {
                 SlideItem &it = items[item_of[w][k]];
-                const int r0 = g->imu_off[k], nr = g->imu_off[k + 1] - r0;
-                it.src = g->imu_from[k], it.row0 = (int) row_at, it.nrow = nr, it.state = -1, it.blob = vo, it.node = node_at[k + 1];
+                it.src = g->imu_from[k], it.state = -1, it.blob = vo, it.node = node_at[k + 1];
                 it.normal = g->normal && g->normal[k] ? 1 : 0;
                 for (int i = 0; i < 3; i++) it.grav[i] = g->gravity3[3 * (size_t) k + i];
-                memcpy(rows + 7 * row_at, g->imu + 7 * (size_t) r0, 56 * (size_t) nr);
-                row_at += nr;
+                if (fr) {
+                    it.row0 = fr->row0[w][k], it.nrow = fr->nrow[w][k];
+                } else {
+                    const int r0 = g->imu_off[k], nr = g->imu_off[k + 1] - r0;
+                    it.row0 = (int) row_at, it.nrow = nr;
+                    memcpy(rows + 7 * row_at, g->imu + 7 * (size_t) r0, 56 * (size_t) nr);
+                    row_at += nr;
+                }
                 if (it.src == ICG_SLIDE_ROW) {
                     memcpy(states + 16 * state_at, g->state16 + 16 * (size_t) k, 128);
                     it.state = (int) (16 * state_at++);
@@ -1059,7 +1087,7 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
             memcpy(h->slide.h + b_iw, iwins.data(), sizeof(SlideIntWin) * iwins.size());
             PreintSlide a;
             a.n = (int) iwins.size(), a.win = (const SlideIntWin *) (h->slide.d + b_iw), a.item = (const SlideItem *) (h->slide.d + b_item);
-            a.align = (const SlideAlign *) (h->slide.d + b_align), a.imu = (const double *) (h->slide.d + b_rows);
+            a.align = (const SlideAlign *) (h->slide.d + b_align), a.imu = fr ? fr->d : (const double *) (h->slide.d + b_rows);
             a.state = (const double *) (h->slide.d + b_state), a.pose = h->D.pose, a.mix = h->D.mix, a.K = C.K, a.val = (double *) (h->slide.d + b_val);
             for (int k = 0; k < 5; k++) a.noise5[k] = noise5[k];
             for (int k = 0; k < 3; k++) a.station[k] = station3[k];
@@ -1099,6 +1127,7 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
     // every check has passed: from here on the device is written
     h->marg_res_n = 0;
     h->cull_res_n = 0;
+    h->store_valid = false;  // icg_ba_slide_ins_resident sets it again when it commits its store
     if (iwins.empty()) ICG_CUDA(cudaMemcpyAsync(h->slide.d, h->slide.h, in_end, cudaMemcpyHostToDevice, s));
     ICG_CUDA(cudaEventRecord(h->slide_ev, s));
     rc = upload_structure(h, n);
@@ -1142,7 +1171,8 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
 // the two counts the kernel read on the device seed slide_body's fingerprint, so the group still agrees once; a rank that rejects before
 // slide_body joins that agreement with its rejection, as slide_body's own checks do.
 static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba_slide_window *carry, const icg_ba_slide_integrate *integ,
-                       const double *noise5, const double *station3, icg_ba_slide_vision *vis, const char *fn, bool sharded) {
+                       const double *noise5, const double *station3, icg_ba_slide_vision *vis, const char *fn, bool sharded,
+                       const FactorRows *fr = nullptr) {
     auto reject = [&](int code) { return sharded ? shard_agree(h, true, 0, fn) : code; };
     auto cuda_fail = [&](cudaError_t e, const char *what) {
         set_error("%s: %s failed: %s", fn, what, cudaGetErrorString(e));
@@ -1282,8 +1312,182 @@ static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_b
         if (v.f_obs) memcpy(v.f_obs, p.f_obs, 4 * (size_t) F);
         if (v.invdepth) memcpy(v.invdepth, p.invdepth, 8 * (size_t) L);
     }
-    return slide_body(h, n, nx.data(), cr.data(), integ, noise5, station3, fn, sharded, true, sharded ? &fp : nullptr);
+    return slide_body(h, n, nx.data(), cr.data(), integ, noise5, station3, fn, sharded, true, sharded ? &fp : nullptr, fr);
 }
+
+// ---- the per-factor IMU sample store (icg_ba_imu_samples_from_ins, icg_ba_slide_ins_resident, icg_ba_reintegrate_stored_resident)
+struct StoreSeg {  // rows src_row .. + n of the cut rows (src 0) or of the current store (src 1) to row dst of the next store
+    int src, row, dst, n;
+};
+
+// one segment per warp, the lanes over its doubles
+__global__ void __launch_bounds__(128) ba_store_gather_kernel(int n_seg, const StoreSeg *seg, const double *cut, const double *cur, double *next) {
+    const int g = blockIdx.x * 4 + (threadIdx.x >> 5);
+    if (g >= n_seg) return;
+    const StoreSeg S = seg[g];
+    const double *src = (S.src ? cur : cut) + 7 * (size_t) S.row;
+    double *dst = next + 7 * (size_t) S.dst;
+    for (int i = threadIdx.x & 31; i < 7 * S.n; i += 32) dst[i] = src[i];
+}
+
+enum { STORE_NONE, STORE_CUT, STORE_OLD, STORE_MERGE };
+struct StoreSrc {  // where a factor of the next store takes its rows from
+    int kind;      // STORE_CUT: getImuSeriesFromTo(t0, t1) of INS stream `stream`; STORE_OLD: old factor a's rows; STORE_MERGE: old factor a's
+    int a, stream; // rows, then old factor a + 1's without its first (removeUnusedTimeNode's addNewImu loop); STORE_NONE: no samples
+    double t0, t1;
+};
+
+static int grow_rows(double *&d, size_t &cap, size_t rows, cudaStream_t s, const char *fn) {
+    if (rows <= cap) return ICG_OK;
+    ICG_CUDA(cudaStreamSynchronize(s));
+    if (d) cudaFree(d);
+    d = nullptr, cap = 0;
+    const size_t c = std::max<size_t>(64, rows + rows / 4);
+    if (cudaMalloc(&d, 56 * c) != cudaSuccess) {
+        set_error("%s: allocation of %zu IMU rows failed", fn, c);
+        return ICG_ENOMEM;
+    }
+    cap = c;
+    return ICG_OK;
+}
+
+// The next store from src (per window and factor) into store_d[1 - store_cur] and its tables into row0 / nrow; the current store, its
+// tables and the INS windows are not changed.  The cut runs on this handle's stream after the work queued on the INS handle's stream, and
+// has completed when this returns.  Jobs the INS windows cannot serve are listed in bad (window, factor), with ICG_EINVAL naming the first.
+static int store_build(icg_ba *h, const icg_ins *ins, const std::vector<std::vector<StoreSrc>> &src, const char *fn, std::vector<std::vector<int>> &row0,
+                       std::vector<std::vector<int>> &nrow, std::vector<std::pair<int, int>> &bad) {
+    const int n = (int) src.size();
+    std::vector<InsCutJob> jobs;
+    std::vector<std::pair<int, int>> job_of;
+    size_t cut_rows = 0, n_fac = 0;
+    for (int w = 0; w < n; w++)
+        for (int k = 0; k < (int) src[w].size(); k++) {
+            n_fac++;
+            const StoreSrc &q = src[w][k];
+            if (q.kind != STORE_CUT) continue;
+            jobs.push_back(InsCutJob{q.t0, q.t1, q.stream, ins->head[q.stream], ins->count[q.stream], (int) std::min<size_t>(cut_rows, INT32_MAX)});
+            job_of.push_back({w, k});
+            cut_rows += (size_t) ins->count[q.stream] + 2;  // getImuSeriesFromTo's bound
+        }
+    if (cut_rows >= (size_t) INT32_MAX / 8 || n_fac >= (size_t) INT32_MAX / 8) {
+        set_error("%s: too many IMU rows in one call", fn);
+        return ICG_EINVAL;
+    }
+    const size_t nj = jobs.size();
+    Layout lay;
+    const size_t b_job = lay.take(sizeof(InsCutJob) * nj), b_n = lay.take(4 * nj), b_st = lay.take(4 * nj), b_seg = lay.take(sizeof(StoreSeg) * 2 * n_fac);
+    cudaStream_t s = h->stream;
+    int rc = hd_reserve(h, h->store_stage, lay.size(), fn);  // every call of the store synchronises before it returns: the old one is idle
+    if (rc != ICG_OK) return rc;
+    if ((rc = grow_rows(h->cut_rows, h->cut_cap, cut_rows, s, fn)) != ICG_OK) return rc;
+    unsigned char *H = h->store_stage.h, *Dv = h->store_stage.d;
+    const int32_t *got_n = (const int32_t *) (H + b_n), *got_st = (const int32_t *) (H + b_st);
+    if (nj > 0) {
+        memcpy(H + b_job, jobs.data(), sizeof(InsCutJob) * nj);
+        ICG_CUDA(cudaMemcpyAsync(Dv, H, b_n, cudaMemcpyHostToDevice, s));
+        if (!h->ins_ev) ICG_CUDA(cudaEventCreateWithFlags(&h->ins_ev, cudaEventDisableTiming));
+        ICG_CUDA(cudaEventRecord(h->ins_ev, ins->stream));  // the pushes and redos queued on the INS handle come first
+        ICG_CUDA(cudaStreamWaitEvent(s, h->ins_ev, 0));
+        ICG_CUDA(ins_cut_launch(ins, (int) nj, (const InsCutJob *) Dv, h->cut_rows, (int32_t *) (Dv + b_n), (int32_t *) (Dv + b_st), s));
+        ICG_CUDA(cudaMemcpyAsync(H + b_n, Dv + b_n, b_seg - b_n, cudaMemcpyDeviceToHost, s));
+        ICG_CUDA(cudaStreamSynchronize(s));
+        for (size_t q = 0; q < nj; q++)
+            if (got_st[q] != 1) bad.push_back(job_of[q]);
+        if (!bad.empty()) {
+            const InsCutJob &J = jobs[std::find(job_of.begin(), job_of.end(), bad[0]) - job_of.begin()];
+            set_error("%s: window %d IMU factor %d: the INS window of stream %d cannot serve the interval %.17g .. %.17g", fn, bad[0].first,
+                      bad[0].second, J.stream, J.t0, J.t1);
+            return ICG_EINVAL;
+        }
+    }
+    // the next store's layout, window after window, factor after factor
+    std::vector<StoreSeg> segs;
+    row0.assign(n, {}), nrow.assign(n, {});
+    size_t total = 0, q = 0;
+    for (int w = 0; w < n; w++) {
+        row0[w].assign(src[w].size(), -1), nrow[w].assign(src[w].size(), -1);
+        for (int k = 0; k < (int) src[w].size(); k++) {
+            const StoreSrc &f = src[w][k];
+            const int at = (int) total;
+            int m = -1;
+            if (f.kind == STORE_CUT) {
+                m = got_n[q];
+                segs.push_back(StoreSeg{0, jobs[q++].out, at, m});
+            } else if (f.kind == STORE_OLD && h->store_nrow[w][f.a] >= 0) {
+                m = h->store_nrow[w][f.a];
+                segs.push_back(StoreSeg{1, h->store_row0[w][f.a], at, m});
+            } else if (f.kind == STORE_MERGE) {
+                const int na = h->store_nrow[w][f.a], nb = h->store_nrow[w][f.a + 1];
+                segs.push_back(StoreSeg{1, h->store_row0[w][f.a], at, na});
+                if (nb > 1) segs.push_back(StoreSeg{1, h->store_row0[w][f.a + 1] + 1, at + na, nb - 1});
+                m = na + nb - 1;
+            }
+            if (m < 0) continue;
+            row0[w][k] = at, nrow[w][k] = m;
+            total += (size_t) m;
+        }
+    }
+    if (total >= (size_t) INT32_MAX / 8) {
+        set_error("%s: too many IMU rows in one call", fn);
+        return ICG_EINVAL;
+    }
+    const int nx = 1 - h->store_cur;
+    if ((rc = grow_rows(h->store_d[nx], h->store_cap[nx], total, s, fn)) != ICG_OK) return rc;
+    if (segs.empty()) return ICG_OK;
+    memcpy(H + b_seg, segs.data(), sizeof(StoreSeg) * segs.size());
+    ICG_CUDA(cudaMemcpyAsync(Dv + b_seg, H + b_seg, sizeof(StoreSeg) * segs.size(), cudaMemcpyHostToDevice, s));
+    ba_store_gather_kernel<<<(unsigned) ((segs.size() + 3) / 4), 128, 0, s>>>((int) segs.size(), (const StoreSeg *) (Dv + b_seg), h->cut_rows,
+                                                                             h->store_d[h->store_cur], h->store_d[nx]);
+    ICG_CHECK_LAUNCH();
+    count_launch();
+    return ICG_OK;
+}
+
+static void store_commit(icg_ba *h, std::vector<std::vector<int>> &row0, std::vector<std::vector<int>> &nrow) {
+    h->store_cur = 1 - h->store_cur;
+    h->store_row0.swap(row0), h->store_nrow.swap(nrow);
+    h->store_valid = true;
+}
+
+// the checks every call that cuts from the INS windows shares
+static int store_ins_ok(icg_ba *h, const icg_ins *ins, int n_windows, const char *fn) {
+    if (!h || !ins || n_windows < 1) {
+        set_error("%s: bad arguments", fn);
+        return ICG_EINVAL;
+    }
+    if (h->D.world > 1) {
+        set_error("%s: not available on a landmark-sharded handle", fn);
+        return ICG_EUNSUPPORTED;
+    }
+    if (ins->device != h->device) {
+        set_error("%s: the INS windows are on device %d, the solver on device %d", fn, ins->device, h->device);
+        return ICG_EINVAL;
+    }
+    if (h->cur_windows != n_windows) {
+        set_error("%s: the handle holds %d uploaded windows, the call names %d", fn, h->cur_windows, n_windows);
+        return ICG_EINVAL;
+    }
+    return ICG_OK;
+}
+
+// stream in range and mechanized, K node times increasing
+static int cut_window_ok(const icg_ins *ins, int w, int stream, const double *node_time, int K, const char *fn) {
+    if (stream < 0 || stream >= ins->max_streams || !ins->mech[stream]) {
+        set_error("%s: window %d: INS stream %d is out of range or not mechanized", fn, w, stream);
+        return ICG_EINVAL;
+    }
+    if (!node_time) {
+        set_error("%s: window %d: arrays missing", fn, w);
+        return ICG_EINVAL;
+    }
+    for (int j = 0; j + 1 < K; j++)
+        if (!(node_time[j] < node_time[j + 1])) {
+            set_error("%s: window %d: node_time[%d] = %.17g is not less than node_time[%d] = %.17g", fn, w, j, node_time[j], j + 1, node_time[j + 1]);
+            return ICG_EINVAL;
+        }
+    return ICG_OK;
+}
+
 
 extern "C" {
 
@@ -1511,6 +1715,160 @@ int icg_ba_shard_slide_vision_resident(icg_ba *h, int n, const icg_ba_problem *n
     const char *fn = "icg_ba_shard_slide_vision_resident";
     const int rc = shard_group_only(h, fn, "icg_ba_slide_vision_resident");
     return rc != ICG_OK ? rc : vision_body(h, n, next, carry, integ, noise5, station3, vis, fn, true);
+}
+
+int icg_ba_imu_samples_from_ins(icg_ba *h, icg_ins *ins, int n_windows, const icg_ba_ins_cut *cut) {
+    static const char *fn = "icg_ba_imu_samples_from_ins";
+    int rc = store_ins_ok(h, ins, n_windows, fn);
+    if (rc != ICG_OK) return rc;
+    if (!cut) {
+        set_error("%s: bad arguments", fn);
+        return ICG_EINVAL;
+    }
+    std::vector<std::vector<StoreSrc>> src(n_windows);
+    for (int w = 0; w < n_windows; w++) {
+        const WinDims &d = h->dims.h[w];
+        if ((rc = cut_window_ok(ins, w, cut[w].stream, cut[w].node_time, d.K, fn)) != ICG_OK) return rc;
+        for (int k = 0; k < d.n_imu; k++) src[w].push_back(StoreSrc{STORE_CUT, 0, cut[w].stream, cut[w].node_time[k], cut[w].node_time[k + 1]});
+    }
+    ICG_CUDA(cudaSetDevice(h->device));
+    std::vector<std::vector<int>> row0, nrow;
+    std::vector<std::pair<int, int>> bad;
+    if ((rc = store_build(h, ins, src, fn, row0, nrow, bad)) != ICG_OK) return rc;
+    ICG_CUDA(cudaStreamSynchronize(h->stream));
+    store_commit(h, row0, nrow);
+    return ICG_OK;
+}
+
+int icg_ba_slide_ins_resident(icg_ba *h, icg_ins *ins, int n_windows, const icg_ba_problem *next, const icg_ba_slide_window *carry,
+                              const icg_ba_slide_ins *io, const double *noise5, const double *station3, icg_ba_slide_vision *vis) {
+    static const char *fn = "icg_ba_slide_ins_resident";
+    int rc = store_ins_ok(h, ins, n_windows, fn);
+    if (rc != ICG_OK) return rc;
+    if (!next || !carry || !io || !noise5 || !station3) {
+        set_error("%s: bad arguments", fn);
+        return ICG_EINVAL;
+    }
+    // each new factor's rows: carried, cut from the INS window, merged from two old factors, or none (a blob read from next)
+    std::vector<std::vector<StoreSrc>> src(n_windows);
+    for (int w = 0; w < n_windows; w++) {
+        const icg_ba_problem &p = next[w];
+        const icg_ba_slide_window &c = carry[w];
+        const icg_ba_slide_ins &g = io[w];
+        const int on = h->dims.h[w].n_imu;
+        if (g.integ.imu || g.integ.imu_off) {
+            set_error("%s: window %d: integ.imu and integ.imu_off must be NULL (the rows are cut from the INS window)", fn, w);
+            return ICG_EINVAL;
+        }
+        if (p.K < 2 || p.K > h->C.K || p.n_imu < 0 || p.n_imu > p.K - 1) {
+            set_error("%s: window %d: sizes out of range", fn, w);
+            return ICG_EINVAL;
+        }
+        bool cuts = false;
+        for (int k = 0; k < p.n_imu; k++) {
+            StoreSrc f = {STORE_NONE, 0, g.stream, 0, 0};
+            const int from = g.integ.imu_from ? g.integ.imu_from[k] : -1;
+            if (c.imu_src && c.imu_src[k] >= 0) {
+                if (c.imu_src[k] >= on) {
+                    set_error("%s: window %d: imu_src[%d] = %d is out of range of the old window (%d)", fn, w, k, c.imu_src[k], on);
+                    return ICG_EINVAL;
+                }
+                if (h->store_valid) f.kind = STORE_OLD, f.a = c.imu_src[k];
+            } else if (from == ICG_SLIDE_ROW) {
+                const int a = g.merge_src ? g.merge_src[k] : -1;
+                if (a < 0 || a + 1 >= on || !h->store_valid || h->store_nrow[w][a] < 1 || h->store_nrow[w][a + 1] < 1) {
+                    set_error("%s: window %d factor %d: merge_src must name old factors a and a + 1 that both hold samples", fn, w, k);
+                    return ICG_EINVAL;
+                }
+                f.kind = STORE_MERGE, f.a = a;
+            } else if (from >= 0 || from == ICG_SLIDE_CHAIN) {
+                f.kind = STORE_CUT, cuts = true;
+            } else if (from != -1) {
+                set_error("%s: window %d: imu_from[%d] = %d is not a source", fn, w, k, from);
+                return ICG_EINVAL;
+            }
+            src[w].push_back(f);
+        }
+        if (cuts && (rc = cut_window_ok(ins, w, g.stream, g.node_time, p.K, fn)) != ICG_OK) return rc;
+        for (int k = 0; k < p.n_imu; k++)
+            if (src[w][k].kind == STORE_CUT) src[w][k].t0 = g.node_time[k], src[w][k].t1 = g.node_time[k + 1];
+    }
+    ICG_CUDA(cudaSetDevice(h->device));
+    std::vector<std::vector<int>> row0, nrow;
+    std::vector<std::pair<int, int>> bad;
+    rc = store_build(h, ins, src, fn, row0, nrow, bad);
+    if (!bad.empty()) {  // status -2 where the INS window cannot serve the interval
+        for (int w = 0; w < n_windows; w++)
+            if (io[w].integ.status) memset(io[w].integ.status, 0, (size_t) next[w].n_imu);
+        for (const auto &b : bad)
+            if (io[b.first].integ.status) io[b.first].integ.status[b.second] = -2;
+    }
+    if (rc != ICG_OK) return rc;
+    std::vector<icg_ba_slide_integrate> integ(n_windows);
+    for (int w = 0; w < n_windows; w++) integ[w] = io[w].integ;
+    const FactorRows fr = {h->store_d[1 - h->store_cur], row0, nrow};
+    rc = vis ? vision_body(h, n_windows, next, carry, integ.data(), noise5, station3, vis, fn, false, &fr)
+             : slide_body(h, n_windows, next, carry, integ.data(), noise5, station3, fn, false, false, nullptr, &fr);
+    if (rc != ICG_OK) return rc;
+    ICG_CUDA(cudaStreamSynchronize(h->stream));
+    for (int w = 0; w < n_windows; w++)
+        if (io[w].n_rows) memcpy(io[w].n_rows, nrow[w].data(), sizeof(int) * nrow[w].size());
+    store_commit(h, row0, nrow);
+    return ICG_OK;
+}
+
+int icg_ba_reintegrate_stored_resident(icg_ba *h, int n_windows, const icg_ba_problem *problems, const double *noise5, const double *station3,
+                                       icg_ba_reint_window *io) {
+    static const char *fn = "icg_ba_reintegrate_stored_resident";
+    int rc = resident_single_rank(h, n_windows, problems, fn);
+    if (rc != ICG_OK) return rc;
+    if (!io) {
+        set_error("%s: bad arguments", fn);
+        return ICG_EINVAL;
+    }
+    if (!h->store_valid) {
+        set_error("%s: the handle holds no IMU samples (an upload or a slide other than icg_ba_slide_ins_resident replaced the windows since "
+                  "the last icg_ba_imu_samples_from_ins)", fn);
+        return ICG_EINVAL;
+    }
+    for (int w = 0; w < n_windows; w++)
+        if (io[w].imu || io[w].imu_off) {
+            set_error("%s: window %d: imu and imu_off must be NULL (the rows are the store's)", fn, w);
+            return ICG_EINVAL;
+        }
+    const FactorRows fr = {h->store_d[h->store_cur], h->store_row0, h->store_nrow};
+    return reint_body(h, n_windows, problems, noise5, station3, io, fn, false, &fr);
+}
+
+int icg_ba_imu_samples(icg_ba *h, int window, int cap_rows, int32_t *off, double *rows) {
+    static const char *fn = "icg_ba_imu_samples";
+    if (!h || window < 0 || window >= h->cur_windows || cap_rows < 0 || !off || (cap_rows > 0 && !rows)) {
+        set_error("%s: bad arguments", fn);
+        return ICG_EINVAL;
+    }
+    if (h->D.world > 1) {
+        set_error("%s: not available on a landmark-sharded handle", fn);
+        return ICG_EUNSUPPORTED;
+    }
+    if (!h->store_valid) {
+        set_error("%s: the handle holds no IMU samples", fn);
+        return ICG_EINVAL;
+    }
+    const std::vector<int> &r0 = h->store_row0[window], &nr = h->store_nrow[window];
+    int first = -1, total = 0;
+    for (size_t k = 0; k < nr.size(); k++) {
+        off[k] = nr[k] < 0 ? -1 : total;
+        if (nr[k] < 0) continue;
+        if (first < 0) first = r0[k];
+        total += nr[k];
+    }
+    off[nr.size()] = total;
+    const int m = std::min(total, cap_rows);
+    if (m == 0) return ICG_OK;
+    ICG_CUDA(cudaSetDevice(h->device));
+    ICG_CUDA(cudaMemcpyAsync(rows, h->store_d[h->store_cur] + 7 * (size_t) first, 56 * (size_t) m, cudaMemcpyDeviceToHost, h->stream));
+    ICG_CUDA(cudaStreamSynchronize(h->stream));
+    return ICG_OK;
 }
 
 }  // extern "C"

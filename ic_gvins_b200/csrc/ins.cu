@@ -17,6 +17,7 @@
 
 #include "common.cuh"
 #include "geom_core.cuh"
+#include "ins_handle.cuh"
 #include "preint.cuh"
 
 using namespace icg;
@@ -216,6 +217,68 @@ __device__ __forceinline__ void series_row(double *dst, const double *row8) {  /
     for (int k = 1; k < INS_ROW; k++) dst[k - 1] = row8[k];
 }
 
+// MISC::getImuSeriesFromTo(start, end) (misc.cc:307-361) of window J in two halves.  series_ends, on one lane: both indices, the
+// isNeedInterpolation cases at each end with imuInterpolation's split, written to ser (rows of 7); n = 0 when the window cannot serve the
+// interval (getInsWindowIndex 0 at either end, or an empty series).  series_middle, on the warp: the middle rows (:337-340) between them.
+// The last row's time becomes `end` (:357-358); the rows carry no time, and the preintegration does not read it.
+struct SeriesCut {
+    int n, m0, nm, nh;  // rows; first middle entry, middle rows, rows before them
+};
+
+__device__ SeriesCut series_ends(const double *I, const InsJob &J, int cap, double start, double end, double *ser) {
+    SeriesCut c = {0, 0, 0, 0};
+    const int is = window_index(I, J, cap, start), ie = window_index(I, J, cap, end);
+    if (!is || !ie) return c;
+    const double *a0 = I + INS_ROW * ring(J, cap, is - 1), *a1 = I + INS_ROW * ring(J, cap, is);
+    const double *b0 = I + INS_ROW * ring(J, cap, ie - 1), *b1 = I + INS_ROW * ring(J, cap, ie);
+    double part[INS_ROW], rest[INS_ROW];
+    const int sa = need_interpolation(a0, a1, start);
+    if (sa == -1) {
+        series_row(ser, a0), series_row(ser + 7, a1), c.nh = 2;
+    } else if (sa == 1) {
+        series_row(ser, a1), c.nh = 1;
+    } else if (sa == 2) {
+        imu_interpolation(a1, start, part, rest);
+        series_row(ser, part), series_row(ser + 7, rest), c.nh = 2;
+    }
+    c.m0 = is + 1, c.nm = ie - 1 - c.m0 > 0 ? ie - 1 - c.m0 : 0;
+    double *tail = ser + 7 * (c.nh + c.nm);
+    int nt = 0;
+    const int sb = need_interpolation(b0, b1, end);
+    if (sb == -1) {
+        series_row(tail, b0), nt = 1;
+    } else if (sb == 1) {
+        series_row(tail, b0), series_row(tail + 7, b1), nt = 2;
+    } else if (sb == 2) {
+        imu_interpolation(b1, end, part, rest);
+        series_row(tail, b0), series_row(tail + 7, part), nt = 2;
+    }
+    c.n = c.nh + c.nm + nt;
+    return c;
+}
+
+__device__ __forceinline__ void series_middle(const double *I, const InsJob &J, int cap, const SeriesCut &c, double *ser) {
+    for (int k = threadIdx.x & 31; k < c.nm; k += 32) series_row(ser + 7 * (c.nh + k), I + INS_ROW * ring(J, cap, c.m0 + k));
+}
+
+// the series of each (stream, start, end) job, one warp per job (ins_handle.cuh)
+__global__ void __launch_bounds__(32 * INS_WARPS) ins_cut_kernel(int n_jobs, int cap, const InsCutJob *jobs, const double *imu, double *rows,
+                                                                int32_t *n_rows, int32_t *status) {
+    const int lane = threadIdx.x & 31, j = blockIdx.x * INS_WARPS + (threadIdx.x >> 5);
+    if (j >= n_jobs) return;
+    const InsCutJob q = jobs[j];
+    InsJob J = {};
+    J.head = q.head, J.count = q.count;
+    const double *I = imu + (size_t) q.stream * cap * INS_ROW;
+    double *ser = rows + 7 * (size_t) q.out;
+    SeriesCut c = {0, 0, 0, 0};
+    if (lane == 0) c = series_ends(I, J, cap, q.t0, q.t1, ser);
+    c.n = __shfl_sync(0xffffffffu, c.n, 0), c.m0 = __shfl_sync(0xffffffffu, c.m0, 0);
+    c.nm = __shfl_sync(0xffffffffu, c.nm, 0), c.nh = __shfl_sync(0xffffffffu, c.nh, 0);
+    if (c.n > 0) series_middle(I, J, cap, c, ser);
+    if (lane == 0) n_rows[j] = c.n, status[j] = c.n > 0 ? 1 : -5;
+}
+
 // gvinsInitialization up to and including the redo; series (INS_SERIES_MAX x 7 per stream) receives getImuSeriesFromTo(last_time,
 // gnss_time) of the window the redo leaves.  The series only reads rows, which the redo does not change, so it and every status are decided
 // before the window is written.
@@ -285,33 +348,9 @@ __global__ void __launch_bounds__(32 * INS_WARPS) ins_gins_init_kernel(int n_str
             const int index = window_index(I, J, cap, G.last_time);
             drop = index >= reserved ? index - reserved : 0;
             J2.head = (J.head + drop) % cap, J2.count = J.count - drop;
-            const int is = index ? window_index(I, J2, cap, G.last_time) : 0, ie = index ? window_index(I, J2, cap, G.gnss_time) : 0;
-            if (is && ie) {
-                const double *a0 = I + INS_ROW * ring(J2, cap, is - 1), *a1 = I + INS_ROW * ring(J2, cap, is);
-                const double *b0 = I + INS_ROW * ring(J2, cap, ie - 1), *b1 = I + INS_ROW * ring(J2, cap, ie);
-                double part[INS_ROW], rest[INS_ROW];
-                const int sa = need_interpolation(a0, a1, G.last_time);
-                if (sa == -1) {
-                    series_row(ser, a0), series_row(ser + 7, a1), nh = 2;
-                } else if (sa == 1) {
-                    series_row(ser, a1), nh = 1;
-                } else if (sa == 2) {
-                    imu_interpolation(a1, G.last_time, part, rest);
-                    series_row(ser, part), series_row(ser + 7, rest), nh = 2;
-                }
-                m0 = is + 1, nm = ie - 1 - m0 > 0 ? ie - 1 - m0 : 0;
-                double *tail = ser + 7 * (nh + nm);
-                int nt = 0;
-                const int sb = need_interpolation(b0, b1, G.gnss_time);
-                if (sb == -1) {
-                    series_row(tail, b0), nt = 1;
-                } else if (sb == 1) {
-                    series_row(tail, b0), series_row(tail + 7, b1), nt = 2;
-                } else if (sb == 2) {
-                    imu_interpolation(b1, G.gnss_time, part, rest);
-                    series_row(tail, b0), series_row(tail + 7, part), nt = 2;
-                }
-                n_ser = nh + nm + nt;  // the last row's time becomes gnss_time (:357-358); the preintegration does not read it
+            if (index) {
+                const SeriesCut c = series_ends(I, J2, cap, G.last_time, G.gnss_time, ser);
+                n_ser = c.n, m0 = c.m0, nm = c.nm, nh = c.nh;
             }
             status = n_ser > 0 ? 1 : -5;
         }
@@ -332,11 +371,10 @@ __global__ void __launch_bounds__(32 * INS_WARPS) ins_gins_init_kernel(int n_str
     }
     __syncwarp();
     if (info[w][0] != 1) return;
-    const int m0 = info[w][1], nm = info[w][2], nh = info[w][3];
+    const SeriesCut c = {0, info[w][1], info[w][2], info[w][3]};
     InsJob J2 = J;
     J2.head = (J.head + info[w][4]) % cap, J2.count = J.count - info[w][4];
-    // the middle rows of the series (misc.cc:337-340), on the pruned window
-    for (int k = lane; k < nm; k += 32) series_row(ser + 7 * (nh + k), I + INS_ROW * ring(J2, cap, m0 + k));
+    series_middle(I, J2, cap, c, ser);  // on the pruned window
     // the redo of :682-683 from that state, with integration_config_ as it now is
     J.grav[0] = 0, J.grav[1] = 0, J.grav[2] = G.gravity;
     if (J.earth)
@@ -397,25 +435,13 @@ __global__ void ins_pose_kernel(int n_streams, int cap, const InsJob *jobs, cons
 
 }  // namespace
 
-struct icg_ins {
-    int device, max_streams, capacity;
-    cudaStream_t stream;
-    bool own_stream;
-    double *d_imu = nullptr, *d_st = nullptr;
-    // the host mirror
-    std::vector<int32_t> head, count;
-    std::vector<uint8_t> mech, seen;
-    std::vector<double> last_time;
-    // gvinsInitialization's function statics, one set per stream: bg[3], initatt[3]; is_has_zero_velocity
-    std::vector<double> init_slot6;
-    std::vector<int32_t> init_zv;
-    double *d_series = nullptr;  // max_streams x INS_SERIES_MAX x 7, the first GNSS interval's rows (allocated by the first initialization)
-    // per-call staging [jobs | doubles | ints], pinned and device, grown on demand; the asynchronous calls' copies complete at stage_ev
-    uint8_t *h_stage = nullptr, *d_stage = nullptr;
-    size_t stage_bytes = 0;
-    cudaEvent_t stage_ev = nullptr;
-    bool stage_pending = false;
-};
+cudaError_t icg::ins_cut_launch(const icg_ins *h, int n_jobs, const InsCutJob *jobs, double *rows, int32_t *n_rows, int32_t *status,
+                                cudaStream_t stream) {
+    if (n_jobs <= 0) return cudaSuccess;
+    ins_cut_kernel<<<(n_jobs + INS_WARPS - 1) / INS_WARPS, 32 * INS_WARPS, 0, stream>>>(n_jobs, h->capacity, jobs, h->d_imu, rows, n_rows, status);
+    count_launch();
+    return cudaGetLastError();
+}
 
 static int ins_stage(icg_ins *h, size_t bytes) {
     if (h->stage_pending) ICG_CUDA(cudaEventSynchronize(h->stage_ev));

@@ -217,6 +217,48 @@ private:
 // The window solve seam: what GVINS::gvinsOptimization hands to ceres::Solver::Solve (IG/ic_gvins.cc:1130-1239).
 // Any max_K / max_L marginalizes (a block beyond 512 rows throws ICG_EUNSUPPORTED); to consume its own prior the handle needs
 // max_marg_r >= 15 (max_K - 1) + 7, e.g. 292 for a 20-keyframe window.
+// ins_window_ of GVINS (IG/ic_gvins.cc:249-293) for a set of streams on the device: the per-sample mechanization, the post-solve redo
+// (MISC::redoInsMechanization), the prior camera pose and gvinsInitialization (see the icg_ins_* calls).  WindowSolver cuts its factors' IMU
+// series out of these windows (imuSamplesFromIns, the INS form of slideWindow).
+class InsWindows {
+public:
+    explicit InsWindows(int max_streams, int capacity = 1000, int device = 0) {
+        check(icg_ins_create(&h_, max_streams, capacity, device, nullptr), "icg_ins_create");
+    }
+    ~InsWindows() { icg_ins_destroy(h_); }
+    InsWindows(const InsWindows &) = delete;
+    InsWindows &operator=(const InsWindows &) = delete;
+
+    // runFusion's IMU step: rows (time, dt, dtheta[3], dvel[3]) of stream s are imu[off[s] .. off[s + 1])
+    void push(int n_streams, const icg_ins_config *cfg, const int32_t *off, const double *imu) {
+        check(icg_ins_push(h_, n_streams, cfg, off, imu), "icg_ins_push");
+    }
+    // redoInsMechanization from state17 (n x 17) of the streams redo selects (nullptr: all); status per stream (1, 0, -1)
+    void redo(int n_streams, const icg_ins_config *cfg, const uint8_t *redo, const double *state17, int reserved, int8_t *status) {
+        check(icg_ins_redo(h_, n_streams, cfg, redo, state17, reserved, status), "icg_ins_redo");
+    }
+    // getCameraPoseFromInsWindow at stamp[s] (see icg_ins_camera_pose)
+    void cameraPose(int n_streams, const double *stamp, const double *pose_b_c, double *dev_pose, double *host_pose, int32_t *found) {
+        check(icg_ins_camera_pose(h_, n_streams, stamp, pose_b_c, dev_pose, host_pose, found), "icg_ins_camera_pose");
+    }
+    // gvinsInitialization of the selected streams (see icg_ins_gins_initialize)
+    void ginsInitialize(int n_streams, icg_ins_config *cfg, const uint8_t *sel, const icg_gins_init *in, const double noise5[5],
+                        const double station[3], int reserved, icg_gins_init_out *out) {
+        check(icg_ins_gins_initialize(h_, n_streams, cfg, sel, in, noise5, station, reserved, out), "icg_ins_gins_initialize");
+    }
+    // one stream's window, oldest first: rows (count x 8) and states (count x 17)
+    void window(int stream, std::vector<double> &imu8, std::vector<double> &state17) {
+        int32_t count = 0;
+        check(icg_ins_window(h_, stream, 0, &count, nullptr, nullptr), "icg_ins_window");
+        imu8.resize(8 * (size_t) count), state17.resize(17 * (size_t) count);
+        check(icg_ins_window(h_, stream, count, &count, imu8.data(), state17.data()), "icg_ins_window");
+    }
+    icg_ins *handle() const { return h_; }
+
+private:
+    icg_ins *h_ = nullptr;
+};
+
 class WindowSolver {
 public:
     WindowSolver(int max_K, int max_L, int max_F, int max_gnss = 16, int max_marg_r = 160, int device = 0) {
@@ -327,6 +369,47 @@ public:
         if (vision.f_ref) next.f_ref = vision.f_ref;
         if (vision.f_obs) next.f_obs = vision.f_obs;
         if (vision.f_const) next.f_const = vision.f_const;
+    }
+    // Every IMU factor's imu_buffer_ kept on the device, cut from `ins` (icg_ba_imu_samples_from_ins): factor k of the window this solver
+    // holds is getImuSeriesFromTo(timelist[k], timelist[k + 1]) of stream `stream`.  Right after the upload of a window whose INS window still
+    // covers it (the GINS window of gvinsInitializationOptimization: before the next redo).
+    void imuSamplesFromIns(InsWindows &ins, int32_t stream, const std::vector<double> &timelist) {
+        const icg_ba_ins_cut cut = {stream, timelist.data()};
+        check(icg_ba_imu_samples_from_ins(h_, ins.handle(), 1, &cut), "icg_ba_imu_samples_from_ins");
+    }
+    // slideWindow(next, carry, prior, integrate, ...) whose integrated factors' rows come from the device (icg_ba_slide_ins_resident): NODE
+    // and ICG_SLIDE_CHAIN factors cut from stream `stream` of `ins` over the next timelist_ (next.K times), ICG_SLIDE_ROW factor k merged
+    // from stored factors merge_src[k] and merge_src[k] + 1 (an empty vector: no ROW factor), carried factors keep their rows.
+    // integrate.imu / imu_off must be null.  n_rows (optional): every new factor's stored rows, -1 for none.
+    void slideWindow(const icg_ba_problem &next, const Carry &carry, bool prior_from_marginalization, icg_ba_slide_integrate &integrate,
+                     InsWindows &ins, int32_t stream, const std::vector<double> &timelist, const std::vector<int32_t> &merge_src,
+                     const double noise5[5], const double station[3], std::vector<int32_t> *n_rows = nullptr) {
+        icg_ba_slide_window c = carryStruct(next, carry);
+        c.prior_from_marg = prior_from_marginalization ? 1 : 0;
+        if (timelist.size() != (size_t) (next.K > 0 ? next.K : 0)) throw std::runtime_error("WindowSolver::slideWindow: timelist needs next.K times");
+        icg_ba_slide_ins io{};
+        io.integ = integrate, io.stream = stream, io.node_time = timelist.data(), io.merge_src = merge_src.empty() ? nullptr : merge_src.data();
+        if (n_rows) n_rows->assign(next.n_imu > 0 ? next.n_imu : 0, -1), io.n_rows = n_rows->data();
+        check(icg_ba_slide_ins_resident(h_, ins.handle(), 1, &next, &c, &io, noise5, station, nullptr), "icg_ba_slide_ins_resident");
+    }
+    // doReintegration from the stored rows (icg_ba_reintegrate_stored_resident): as the other doReintegration, without the host's rows
+    int doReintegration(const icg_ba_problem &problem, const double noise5[5], const double station[3], std::vector<int8_t> &status,
+                        std::vector<double> &blobs, std::vector<double> *end_states = nullptr) {
+        const size_t m = problem.n_imu > 0 ? (size_t) problem.n_imu : 0;
+        status.assign(m, 0);
+        blobs.resize(m * ICG_IMU_BLOB_DOUBLES);
+        if (end_states) end_states->assign(10 * m, 0.0);
+        icg_ba_reint_window io{};
+        io.reintegrate = 1, io.status = status.data(), io.blob_out = blobs.data(), io.end_state10 = end_states ? end_states->data() : nullptr;
+        check(icg_ba_reintegrate_stored_resident(h_, 1, &problem, noise5, station, &io), "icg_ba_reintegrate_stored_resident");
+        return io.count;
+    }
+    // the stored rows of the window (icg_ba_imu_samples): off (n_imu + 1; -1 for a factor without samples) and rows (7 per row)
+    void imuSamples(int n_imu, std::vector<int32_t> &off, std::vector<double> &rows) {
+        off.assign((size_t) n_imu + 1, 0);
+        check(icg_ba_imu_samples(h_, 0, 0, off.data(), nullptr), "icg_ba_imu_samples");
+        rows.resize(7 * (size_t) off[n_imu]);
+        check(icg_ba_imu_samples(h_, 0, off[n_imu], off.data(), rows.data()), "icg_ba_imu_samples");
     }
     // the two-pass body of gvinsOptimization on the window slideWindow left (nothing is uploaded); results as gvinsOptimization gives them
     void gvinsOptimizationResident(const icg_ba_problem &next, int num_iterations, icg_ba_summary out[2], int32_t culled[2]) {

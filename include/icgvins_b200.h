@@ -983,6 +983,68 @@ int icg_ins_camera_pose(icg_ins *h, int n_streams, const double *stamp, const do
 int icg_ins_window(icg_ins *h, int stream, int cap, int32_t *count, double *imu8, double *state17);
 int icg_ins_sync(icg_ins *h);
 
+/* ===================================================================================================== *
+ *  Every IMU factor's samples on the device: the window solver's sample store, filled from the INS windows
+ * ===================================================================================================== */
+/*
+ * The reference keeps each factor's imu_buffer_ (PreintegrationBase) from the moment its interval is cut, MISC::getImuSeriesFromTo (misc.cc:
+ * 307-361) on ins_window_, for two later readers: the merge of removeUnusedTimeNode (IG/ic_gvins.cc:754-789) and doReintegration (:1680-1695).
+ * An icg_ba handle keeps the same rows on the device, per resident window and factor, so that a caller whose samples live in icg_ins windows
+ * needs no host copy of them.  The store is filled only by the two calls below that cut from the INS windows; icg_ba_upload and every other
+ * slide replace the factors and leave the handle without samples (bookkeeping only).  A call builds the next store in a second buffer and
+ * swaps only when it commits, so a rejected call leaves the store as it was.
+ * The series cut is getImuSeriesFromTo(start, end) exactly (both getInsWindowIndex, the four isNeedInterpolation cases at each end with
+ * MINIMUM_TIME_INTERVAL = 1e-4, imuInterpolation's split, the middle rows), on the window as the INS handle holds it when the call runs.  An
+ * interval the window cannot serve -- getInsWindowIndex 0 at either end, or an empty series, the rule of icg_ins_gins_initialize's status -5
+ * -- is refused.
+ * Ordering.  The solver's stream waits for an event recorded on the INS handle's stream (pushes and redos queued before the call are seen), and
+ * each call synchronises before it returns, so a later icg_ins_push / icg_ins_redo cannot overwrite rows it reads.  The two handles must be on
+ * one device.  Every check (streams in range and mechanized, node_time increasing, merge_src in range with both sources holding samples, the
+ * NULL rows) runs before anything is written; a rejected call leaves the handle, its store and the INS windows as they were.
+ * Landmark-sharded handles: ICG_EUNSUPPORTED for all four calls.
+ */
+typedef struct icg_ba_ins_cut {
+    int32_t stream;          /* the window's INS stream */
+    const double *node_time; /* next.K: timelist_; factor k is getImuSeriesFromTo(node_time[k], node_time[k + 1]) */
+} icg_ba_ins_cut;
+/* Seeds the store of n_windows (the uploaded count) resident windows: every IMU factor k of window w from cut[w].  Call it right after the
+ * upload of a window whose INS window still covers the window's span.  After icg_ins_gins_initialize and the upload of the K = 2 GINS window
+ * (gvinsInitializationOptimization), that is before the next icg_ins_redo, which prunes the first interval out of the INS window.  Synchronous. */
+int icg_ba_imu_samples_from_ins(icg_ba *h, icg_ins *ins, int n_windows, const icg_ba_ins_cut *cut);
+/* icg_ba_slide_integrate_resident (vis NULL) or icg_ba_slide_vision_resident (vis given, its vision build exactly) whose integrated factors'
+ * rows come from the device.  Per new IMU factor k of window w:
+ *   NODE / ICG_SLIDE_CHAIN     getImuSeriesFromTo(node_time[k], node_time[k + 1]) cut from INS stream `stream` (addNewTimeNode, :897-928;
+ *                              the re-created tail of insertNewGnssTimeNode, :791-888);
+ *   ICG_SLIDE_ROW              old factor merge_src[k]'s stored rows, then old factor merge_src[k] + 1's without its first row
+ *                              (removeUnusedTimeNode's addNewImu loop);
+ *   carried (imu_src >= 0)     its stored rows carry over (none when the handle holds no samples);
+ *   read from next.imu_blob    no samples.
+ * Everything after the rows is icg_ba_slide_integrate_resident's path, on the same kernels; the handle is bit for bit the one that call leaves
+ * when it is given the same rows from the host.  integ.imu / imu_off must be NULL; its other fields keep their meaning.  An interval the INS
+ * window cannot serve: ICG_EINVAL naming the window and factor, integ.status -2 there (0 elsewhere), and the handle, its store and the INS
+ * windows as they were.  Order of the checks: the call's own (streams, node_time, merge_src, the NULL rows) run first, then the cut (into
+ * staging only, one launch and one synchronisation), then every check of icg_ba_slide_integrate_resident / icg_ba_slide_vision_resident;
+ * so an interval the window cannot serve is reported ahead of those, and a call they reject has run the cut.  Nothing the handle, its store
+ * or the INS windows hold is written before every check has passed.  Synchronous. */
+typedef struct icg_ba_slide_ins {
+    icg_ba_slide_integrate integ; /* imu / imu_off NULL */
+    int32_t stream;               /* the window's INS stream (read when a factor is cut) */
+    const double *node_time;      /* next.K: the next window's timelist_ (read when a factor is cut) */
+    const int32_t *merge_src;     /* next.n_imu: read for ICG_SLIDE_ROW factors */
+    int32_t *n_rows;              /* out, next.n_imu or NULL: every new factor's stored rows, -1 for none */
+} icg_ba_slide_ins;
+int icg_ba_slide_ins_resident(icg_ba *h, icg_ins *ins, int n_windows, const icg_ba_problem *next, const icg_ba_slide_window *carry,
+                              const icg_ba_slide_ins *io, const double *noise5, const double *station3, icg_ba_slide_vision *vis);
+/* icg_ba_reintegrate_resident with every factor's rows from the store: io[w].imu / imu_off must be NULL.  The same gate, replay and
+ * replacement on the same kernel; a window with reintegrate = 1 that holds a factor without samples is refused before any launch, as is a
+ * handle without a store.  The stored rows do not change (the reference's imu_buffer_ does not either).  Synchronous. */
+int icg_ba_reintegrate_stored_resident(icg_ba *h, int n_windows, const icg_ba_problem *problems, const double *noise5, const double *station3,
+                                       icg_ba_reint_window *io);
+/* Download of one resident window's stored rows (HOST): off (n_imu + 1): factor k's first row in rows, or -1 for a factor without samples;
+ * off[n_imu] = the window's rows.  A factor's rows run to the next non-negative offset.  The first min(total, cap_rows) rows go to rows
+ * (cap_rows x 7).  Synchronous. */
+int icg_ba_imu_samples(icg_ba *h, int window, int cap_rows, int32_t *off, double *rows);
+
 #ifdef __cplusplus
 }
 #endif
