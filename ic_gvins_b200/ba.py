@@ -80,7 +80,7 @@ def cull_struct(prob: dict, ci: dict) -> CullWindow:
         a = np.ascontiguousarray(ci[k], dtype=dt)
         ci[k] = a
         setattr(s, k, a.ctypes.data_as(pt) if a.size else pt())
-    n_obs = int(ci["obs_off"][L]) if L > 0 else 0
+    n_obs = int(ci["obs_off"][L]) if L > 0 and ci.get("obs_off") is not None else len(ci.get("obs_outlier", ()))
     ci.update(cam_pose=np.zeros((K, 12)), lm_pw=np.zeros((L, 3)), lm_depth=np.zeros(L), lm_outlier=np.zeros(L, np.uint8), obs_outlier=np.zeros(n_obs, np.uint8))
     s.cam_pose, s.lm_pw, s.lm_depth = (ci[k].ctypes.data_as(dp) for k in ("cam_pose", "lm_pw", "lm_depth"))
     s.lm_outlier, s.obs_outlier = ci["lm_outlier"].ctypes.data_as(bp), ci["obs_outlier"].ctypes.data_as(bp)
@@ -457,6 +457,50 @@ class WindowSolver:
         for c, s in zip(outs, cw):
             c.update(R_bc_out=np.array(s.R_bc_out[:]).reshape(3, 3), t_bc_out=np.array(s.t_bc_out[:]), td_bc_out=s.td_bc_out, ext_accepted=s.ext_accepted,
                      counts=np.array(s.counts[:], np.int32))
+        return outs
+
+    def update_and_cull_built(self, problems, camera, std, ext_inputs):
+        """update_and_cull() on the observation lists the last slide_vision() built on the device (icg_ba_update_and_cull_built): nothing
+        but the extrinsic inputs goes up.  ext_inputs: one dict per window with R_bc (3x3), t_bc, td_bc, estimate_ext, estimate_td.  Returns
+        update_and_cull()'s dicts with the list keys the culling walked filled in (lm_ref_node, lm_ref_kp, obs_off, obs_node, obs_kp,
+        obs_factor, and n_obs), so that marginalize(culled=...) takes them unchanged; slide_vision() may then omit obs_factor, and
+        marginalize(culled=...) takes dicts without the four integer lists (the culling's own are used)."""
+        from ._lib import CullLists
+        if isinstance(problems, dict):
+            problems, ext_inputs = [problems], [ext_inputs]
+        n = len(problems)
+        arr = (BaProblem * n)(*[to_struct(p) for p in problems])
+        outs, cw, cl = [], (CullWindow * n)(), (CullLists * n)()
+        cap = self.max_L + self.max_F
+        for w, (p, e) in enumerate(zip(problems, ext_inputs)):
+            K, L = int(p["K"]), int(p["L"])
+            o = {k: e[k] for k in ("R_bc", "t_bc", "td_bc", "estimate_ext", "estimate_td") if k in e}
+            o.update(lm_ref_node=np.zeros(L, np.int32), obs_off=np.zeros(L + 1, np.int32), obs_node=np.zeros(cap, np.int32), obs_factor=np.zeros(cap, np.int32),
+                     lm_ref_kp=np.zeros((L, 2), np.float32), obs_kp=np.zeros((cap, 2), np.float32), cam_pose=np.zeros((K, 12)), lm_pw=np.zeros((L, 3)),
+                     lm_depth=np.zeros(L), lm_outlier=np.zeros(L, np.uint8), obs_outlier=np.zeros(cap, np.uint8))
+            outs.append(o)
+            s = cw[w]
+            for k, v in zip(("R_bc", "t_bc"), (np.asarray(e["R_bc"], np.float64).reshape(-1), np.asarray(e["t_bc"], np.float64).reshape(-1))):
+                getattr(s, k)[:] = [float(x) for x in v]
+            s.td_bc, s.estimate_ext, s.estimate_td = float(e.get("td_bc", 0.0)), int(e.get("estimate_ext", 1)), int(e.get("estimate_td", 1))
+            s.cam_pose, s.lm_pw, s.lm_depth = (o[k].ctypes.data_as(dp) for k in ("cam_pose", "lm_pw", "lm_depth"))
+            s.lm_outlier, s.obs_outlier = o["lm_outlier"].ctypes.data_as(bp), o["obs_outlier"].ctypes.data_as(bp)
+            for k in ("lm_ref_node", "obs_off", "obs_node", "obs_factor"):
+                setattr(cl[w], k, o[k].ctypes.data_as(ip))
+            cl[w].lm_ref_kp, cl[w].obs_kp = o["lm_ref_kp"].ctypes.data_as(fp), o["obs_kp"].ctypes.data_as(fp)
+        cam = camera.c if hasattr(camera, "c") else camera
+        rc = lib().icg_ba_update_and_cull_built(self._h, n, arr, C.byref(cam), float(std), cw, cl)
+        if rc != 0:
+            from ._lib import IcgError
+            err = IcgError(f"icg_ba_update_and_cull_built failed with code {rc}: {lib().icg_last_error().decode('utf-8', 'replace')}")
+            err.code = rc
+            raise err
+        for o, s, c in zip(outs, cw, cl):
+            no = int(c.n_obs)
+            for k in ("obs_node", "obs_factor", "obs_kp", "obs_outlier"):
+                o[k] = o[k][:no].copy()
+            o.update(n_obs=no, R_bc_out=np.array(s.R_bc_out[:]).reshape(3, 3), t_bc_out=np.array(s.t_bc_out[:]), td_bc_out=s.td_bc_out,
+                     ext_accepted=s.ext_accepted, counts=np.array(s.counts[:], np.int32))
         return outs
 
     def reintegrate(self, problems, noise5, station, imu_rows, reintegrate=None):

@@ -887,6 +887,7 @@ int icg_ba_upload(icg_ba *h, int n, const icg_ba_problem *P) {
     const BaCaps &C = h->C;
     h->marg_res_n = 0;  // the marginalization workspace no longer belongs to the windows the handle holds
     h->cull_res_n = 0;
+    h->lists_n = 0;
     h->store_valid = false;  // the IMU factors are next's now, without samples
     int rc = pack_windows(h, n, P, true);
     if (rc != ICG_OK) return rc;
@@ -1037,6 +1038,7 @@ int icg_ba_shard_export(icg_ba *h, int rank, int world, uint8_t *blob) {
     }
     int rc = split_setup(h, rank, world);
     if (rc != ICG_OK) return rc;
+    h->lists_n = 0;  // built culling lists are a single-GPU handle's
     ShardBlob b;
     memset(&b, 0, sizeof(b));
     b.magic = 0x49434753484152ull, b.pid = (uint64_t) getpid(), b.ptr = (uint64_t) (uintptr_t) h->xbuf, b.doubles = h->D.S.off_exp;

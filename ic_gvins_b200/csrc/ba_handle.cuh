@@ -107,12 +107,30 @@ struct icg_ba {
     HostDev<double> marg_oJ0, marg_oe0, marg_oHp, marg_obp;
     HostDev<uint8_t> marg_fmask;  // factor set of icg_ba_marginalize_resident_culled (ba_lin_vis reads it in place of f_active)
     HostDev<unsigned char> cull;  // post-solve update + culling: staging [inputs | outputs], grown on demand
-    // the last culling, while it is current (icg_ba_slide_vision_resident reads its flags from the staging above): its window count (0: none;
-    // an upload, a slide or a sharded culling clears it), every window's slices and observation count, the staging offsets of its arrays
+    // the last culling, while it is current (icg_ba_slide_vision_resident reads its lists and flags on the device): its window count (0: none;
+    // an upload, a slide or a sharded culling clears it), every window's slices and observation count, and where its arrays are: the lists
+    // in the culling's staging (host lists) or in the current built lists, the flags in the culling's staging.  cull_res_fac: the built
+    // lists' obs_factor (NULL after a host-list culling, whose obs_factor comes with the slide); cull_res_h*: the built lists' host copies
     int cull_res_n = 0;
     std::vector<icg::CullWin> cull_res_win;
     std::vector<int> cull_res_nobs;
-    size_t cull_res_ref = 0, cull_res_off = 0, cull_res_lmo = 0, cull_res_obso = 0;
+    const int *cull_res_ref = nullptr, *cull_res_off = nullptr, *cull_res_node = nullptr, *cull_res_fac = nullptr;
+    const float *cull_res_rkp = nullptr, *cull_res_kp = nullptr;
+    const uint8_t *cull_res_lmo = nullptr, *cull_res_obso = nullptr;
+    const int *cull_res_href = nullptr, *cull_res_hoff = nullptr, *cull_res_hnode = nullptr, *cull_res_hfac = nullptr;
+    // the next culling's lists, built by icg_ba_slide_vision_resident into lists[lists_cur ^ 1] and current from its commit until an upload,
+    // any other slide or a shard export (lists_n: their window count, 0: none).  Each buffer is [lm_ref_node | obs_off | obs_node | obs_factor |
+    // lm_ref_kp | obs_kp] at lists_at; window w's slices are lists_win[w] (lm0, off0, obs0, K, L) with lists_nobs[w] entries, the arrays sized
+    // by the slide's bounds (lists_nL landmarks, lists_nO observations)
+    struct ListAt {
+        size_t ref, off, node, fac, rkp, kp, end;
+    };
+    HostDev<unsigned char> lists[2];
+    ListAt lists_at[2] = {};
+    int lists_cur = 0, lists_n = 0;
+    size_t lists_nL = 0, lists_nO = 0;
+    std::vector<icg::CullWin> lists_win;
+    std::vector<int> lists_nobs;
     HostDev<unsigned char> vis;    // icg_ba_slide_vision_resident's staging, grown on demand
     HostDev<unsigned char> reint;  // the reintegration's staging, grown on demand
     // the last resident marginalization, while its workspace (marg_oJ0 / marg_oe0) is the prior of the windows the handle holds: its window

@@ -1127,6 +1127,7 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
     // every check has passed: from here on the device is written
     h->marg_res_n = 0;
     h->cull_res_n = 0;
+    h->lists_n = 0;          // icg_ba_slide_vision_resident makes the lists it built current when this returns
     h->store_valid = false;  // icg_ba_slide_ins_resident sets it again when it commits its store
     if (iwins.empty()) ICG_CUDA(cudaMemcpyAsync(h->slide.d, h->slide.h, in_end, cudaMemcpyHostToDevice, s));
     ICG_CUDA(cudaEventRecord(h->slide_ev, s));
@@ -1191,8 +1192,9 @@ static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_b
     if (cudaError_t e = cudaSetDevice(h->device)) return cuda_fail(e, "cudaSetDevice");
     const BaCaps &C = h->C;
     std::vector<VisWin> wins(n);
+    std::vector<long long> ofac_at(n, -1);  // the window's first entry in the staged obs_factor, -1: the built lists' (vis[w].obs_factor NULL)
     ArgPrint fp;  // sharded: what every rank must pass alike, then the counts its kernel read
-    size_t n_ofac = 0, n_lm = 0, n_f = 0, n_nf = 0, n_scr = 0;
+    size_t n_ofac = 0, n_lm = 0, n_f = 0, n_nf = 0, n_scr = 0, n_lo = 0;
     for (int w = 0; w < n; w++) {
         const icg_ba_problem &p = next[w];
         const icg_ba_slide_vision &v = vis[w];
@@ -1203,7 +1205,7 @@ static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_b
                    v.n_frames < 0 || v.n_frames > VIS_MAX_FRAMES || (v.n_frames > 0 && (!v.frame_id || !v.frame_node)) || v.n_obs < 0 || v.n_new < 0 ||
                    (v.obs_src && v.n_in < 0) || (v.n_obs > 0 && (!v.obs_lm || !v.obs_undis_xy || !v.obs_vel)) ||
                    (v.n_new > 0 && (!v.new_depth || !v.new_vel_ref || !v.new_vel_cur || !v.new_ref_undis_xy || !v.new_cur_undis_xy || !v.new_ref_frame_id)) ||
-                   (nco > 0 && !v.obs_factor) || cw.K != od.K || cw.L != od.L;
+                   (nco > 0 && !v.obs_factor && !h->cull_res_fac) || cw.K != od.K || cw.L != od.L;
         for (int e = 0; !bad && e < v.n_frames; e++) bad = v.frame_node[e] < 0 || v.frame_node[e] >= p.K;
         if (bad) {
             set_error("%s: window %d: arguments out of range or arrays missing", fn, w);
@@ -1223,15 +1225,17 @@ static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_b
             if (ns[j] >= v.num_marg && ns[j] < od.K && v.node_in_map[ns[j]]) W.onode[ns[j]] = (int8_t) j;
         for (int e = 0; e < v.n_frames; e++) W.frame_id[e] = v.frame_id[e], W.frame_node[e] = v.frame_node[e];
         W.oK = od.K, W.oL = od.L, W.oF = od.F, W.nK = p.K, W.n_frames = v.n_frames, W.cur_node = v.cur_node;
-        W.cull_lm0 = cw.lm0, W.cull_off0 = cw.off0, W.cull_obs0 = cw.obs0, W.n_cull_obs = nco, W.obs_factor0 = (int) n_ofac;
+        W.cull_lm0 = cw.lm0, W.cull_off0 = cw.off0, W.cull_obs0 = cw.obs0, W.n_cull_obs = nco;
+        if (v.obs_factor) ofac_at[w] = (long long) n_ofac, n_ofac += nco;
         W.n_obs = v.n_obs, W.n_in = v.obs_src ? v.n_in : v.n_obs, W.dev_n = v.dev_n, W.src = v.obs_src, W.obs_node = v.obs_node, W.obs_lm = v.obs_lm;
         W.obs_xy = v.obs_undis_xy, W.obs_vel = v.obs_vel;
         W.n_new = v.n_new, W.dev_new_n = v.dev_new_n, W.new_depth = v.new_depth, W.new_vel_ref = v.new_vel_ref, W.new_vel_cur = v.new_vel_cur;
         W.new_ref_xy = v.new_ref_undis_xy, W.new_cur_xy = v.new_cur_undis_xy, W.new_ref_frame = v.new_ref_frame_id;
-        W.lm_out = (int) n_lm, W.f_out = (int) n_f, W.nf_out = (int) n_nf, W.scr = (int) n_scr;
-        n_ofac += nco, n_lm += (size_t) od.L + v.n_new, n_f += (size_t) od.F + v.n_obs + v.n_new, n_nf += (size_t) v.n_obs + v.n_new;
+        W.lm_out = (int) n_lm, W.f_out = (int) n_f, W.nf_out = (int) n_nf, W.scr = (int) n_scr, W.lst_obs = (int) n_lo;
+        n_lm += (size_t) od.L + v.n_new, n_f += (size_t) od.F + v.n_obs + v.n_new, n_nf += (size_t) v.n_obs + v.n_new;
         n_scr += (size_t) od.F + 3 * (size_t) od.L + 5 * ((size_t) od.L + v.n_new) + v.n_new;  // ba_vision_build's scratch
-        if (n_ofac >= INT32_MAX / 2 || n_f >= INT32_MAX / 16 || n_scr >= INT32_MAX / 2) {
+        if (!sharded) n_scr += (size_t) od.F + od.L + v.n_new, n_lo += (size_t) nco + v.n_obs + 2 * (size_t) v.n_new;  // and the lists'
+        if (n_ofac >= INT32_MAX / 2 || n_f >= INT32_MAX / 16 || n_scr >= INT32_MAX / 2 || n_lo >= INT32_MAX / 4) {
             set_error("%s: too many rows in one call", fn);
             return reject(ICG_EINVAL);
         }
@@ -1247,19 +1251,33 @@ static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_b
     if (lay.size() > h->vis.n)
         if (cudaError_t e = cudaStreamSynchronize(s)) return cuda_fail(e, "cudaStreamSynchronize");
     if ((rc = hd_reserve(h, h->vis, lay.size(), fn)) != ICG_OK) return reject(rc);
+    // one GPU: the next culling's lists go to the buffer that is not current
+    const int nb = h->lists_cur ^ 1;
+    icg_ba::ListAt at{};
+    if (!sharded) {
+        Layout ll;
+        at.ref = ll.take(4 * n_lm), at.off = ll.take(4 * (n_lm + n)), at.node = ll.take(4 * n_lo), at.fac = ll.take(4 * n_lo);
+        at.rkp = ll.take(8 * n_lm), at.kp = ll.take(8 * n_lo), at.end = ll.size();
+        if ((rc = hd_reserve(h, h->lists[nb], at.end, fn)) != ICG_OK) return reject(rc);
+    }
     unsigned char *H = h->vis.h, *Dv = h->vis.d;
+    for (int w = 0; w < n; w++) {
+        wins[w].obs_factor = ofac_at[w] >= 0 ? (const int *) (Dv + b_ofac) + ofac_at[w] : h->cull_res_fac + h->cull_res_win[w].obs0;
+        if (ofac_at[w] >= 0 && wins[w].n_cull_obs > 0) memcpy(H + b_ofac + 4 * (size_t) ofac_at[w], vis[w].obs_factor, 4 * (size_t) wins[w].n_cull_obs);
+    }
     memcpy(H + b_win, wins.data(), sizeof(VisWin) * n);
-    for (int w = 0; w < n; w++)
-        if (wins[w].n_cull_obs > 0) memcpy(H + b_ofac + 4 * (size_t) wins[w].obs_factor0, vis[w].obs_factor, 4 * (size_t) wins[w].n_cull_obs);
     VisArgs a;
     a.win = (const VisWin *) (Dv + b_win), a.K = C.K, a.L = C.L, a.F = C.F;
     a.rank = sharded ? h->D.rank : 0, a.world = sharded ? h->D.world : 1;
     a.rho = h->D.rho, a.lm_ref = h->lm_ref, a.lm_ref_next = h->lm_ref_alt, a.f_meta_s = h->D.f_meta_s, a.lm_off = h->D.lm_off, a.lm_perm = h->D.lm_perm;
-    a.lm_ref_node = (const int *) (h->cull.d + h->cull_res_ref), a.obs_off = (const int *) (h->cull.d + h->cull_res_off);
-    a.lm_outlier = h->cull.d + h->cull_res_lmo, a.obs_outlier = h->cull.d + h->cull_res_obso, a.obs_factor = (const int *) (Dv + b_ofac);
+    a.lm_ref_node = h->cull_res_ref, a.obs_off = h->cull_res_off, a.obs_node = h->cull_res_node, a.lm_ref_kp = h->cull_res_rkp, a.obs_kp = h->cull_res_kp;
+    a.lm_outlier = h->cull_res_lmo, a.obs_outlier = h->cull_res_obso;
     a.counts = (int *) (Dv + b_cnt), a.lm_src = (int *) (Dv + b_lms), a.lm_org = (int *) (Dv + b_org), a.lm_nan = Dv + b_nan, a.f_lm = (int *) (Dv + b_flm), a.f_ref = (int *) (Dv + b_fref);
     a.f_obs = (int *) (Dv + b_fobs), a.f_src = (int *) (Dv + b_fsrc), a.invdepth = (double *) (Dv + b_invd), a.f_new = (double *) (Dv + b_fnew);
     a.scratch = (int *) (Dv + b_scr);
+    unsigned char *Dl = sharded ? nullptr : h->lists[nb].d;
+    a.l_ref = Dl ? (int *) (Dl + at.ref) : nullptr, a.l_off = Dl ? (int *) (Dl + at.off) : nullptr, a.l_node = Dl ? (int *) (Dl + at.node) : nullptr;
+    a.l_fac = Dl ? (int *) (Dl + at.fac) : nullptr, a.l_rkp = Dl ? (float *) (Dl + at.rkp) : nullptr, a.l_kp = Dl ? (float *) (Dl + at.kp) : nullptr;
     cudaError_t e = cudaMemcpyAsync(Dv, H, in_end, cudaMemcpyHostToDevice, s);
     if (e == cudaSuccess) e = cudaMemsetAsync(Dv + b_cnt, 0, 4 * VIS_COUNTS * (size_t) n, s);
     if (e == cudaSuccess && (e = launch_vision(a, n, s)) == cudaSuccess) count_launch();
@@ -1312,7 +1330,17 @@ static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_b
         if (v.f_obs) memcpy(v.f_obs, p.f_obs, 4 * (size_t) F);
         if (v.invdepth) memcpy(v.invdepth, p.invdepth, 8 * (size_t) L);
     }
-    return slide_body(h, n, nx.data(), cr.data(), integ, noise5, station3, fn, sharded, true, sharded ? &fp : nullptr, fr);
+    std::vector<CullWin> lw(n);
+    std::vector<int> lnobs(n);
+    for (int w = 0; w < n; w++) {
+        const int *c = cnt + VIS_COUNTS * w;
+        lw[w].K = next[w].K, lw[w].L = c[0], lw[w].lm0 = wins[w].lm_out, lw[w].off0 = wins[w].lm_out + w, lw[w].obs0 = wins[w].lst_obs, lnobs[w] = c[8];
+    }
+    rc = slide_body(h, n, nx.data(), cr.data(), integ, noise5, station3, fn, sharded, true, sharded ? &fp : nullptr, fr);
+    if (rc != ICG_OK || sharded) return rc;
+    h->lists_cur = nb, h->lists_at[nb] = at, h->lists_n = n, h->lists_nL = n_lm, h->lists_nO = n_lo;
+    h->lists_win = std::move(lw), h->lists_nobs = std::move(lnobs);
+    return ICG_OK;
 }
 
 // ---- the per-factor IMU sample store (icg_ba_imu_samples_from_ins, icg_ba_slide_ins_resident, icg_ba_reintegrate_stored_resident)
@@ -1489,64 +1517,22 @@ static int cut_window_ok(const icg_ins *ins, int w, int stream, const double *no
 }
 
 
-extern "C" {
-
-int icg_ba_marginalize(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg, icg_ba_prior *out) {
-    return marginalize_body(h, n_windows, problems, num_marg, out, false);
-}
-
-int icg_ba_marginalize_resident(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg, icg_ba_prior *out) {
-    if (h && h->D.world > 1) return marginalize_sharded(h, n_windows, problems, num_marg, out, nullptr, "icg_ba_marginalize_resident");
-    return marginalize_body(h, n_windows, problems, num_marg, out, true);
-}
-
-int icg_ba_update_and_cull_resident(icg_ba *h, int n_windows, const icg_ba_problem *problems, const icg_camera *cam, double reprojection_error_std,
-                                    icg_ba_cull_window *io) {
-    int rc = resident_single_rank(h, n_windows, problems, "icg_ba_update_and_cull_resident", true);
-    if (rc != ICG_OK) return rc;
-    if (!cam || !io) {
-        set_error("icg_ba_update_and_cull_resident: bad arguments");
-        return ICG_EINVAL;
-    }
+// ---- the culling (ba_cull.cu) of both entries: staging [windows | host lists] in, [windows | cam_pose | lm_pw | lm_depth | lm_outlier |
+//      obs_outlier] out, one launch, one synchronisation, the outputs into io.  win[w]'s slices index the lists and the outputs alike.
+//      built: the lists the last vision slide built (lists_nL landmarks, lists_nO observations); NULL: io's host lists, staged here.
+//      Records where the culling's lists and flags sit for icg_ba_slide_vision_resident.
+struct CullSrc {
+    const int *ref, *off, *node, *fac;
+    const float *rkp, *kp;
+};
+static int cull_run(icg_ba *h, int n, const icg_ba_problem *problems, const icg_camera *cam, double std, icg_ba_cull_window *io,
+                    const std::vector<CullWin> &win, const std::vector<int> &nobs, size_t nL, size_t nO, size_t nK, const CullSrc *built,
+                    const char *fn) {
     const BaCaps &C = h->C;
-    const int n = n_windows;
-    // layout of the staging buffer: inputs [windows | lm_ref_node | obs_off | obs_node | lm_ref_kp | obs_kp], then outputs
-    // [windows | cam_pose | lm_pw | lm_depth | lm_outlier | obs_outlier], every array 16-byte aligned
-    std::vector<CullWin> win(n);
-    size_t nL = 0, nO = 0, nK = 0;
-    for (int w = 0; w < n; w++) {
-        const icg_ba_problem &p = problems[w];
-        const icg_ba_cull_window &c = io[w];
-        if (p.K < 2 || p.K > C.K || p.L < 0 || p.L > C.L || !c.cam_pose ||
-            (p.L > 0 && (!c.lm_ref_node || !c.lm_ref_kp || !c.obs_off || !c.lm_pw || !c.lm_depth || !c.lm_outlier))) {
-            set_error("icg_ba_update_and_cull_resident: window %d: sizes out of range or arrays missing", w);
-            return ICG_EINVAL;
-        }
-        const int no = p.L > 0 ? c.obs_off[p.L] : 0;
-        if (p.L > 0 && (c.obs_off[0] != 0 || no < 0 || no > INT32_MAX - (int64_t) nO || (no > 0 && (!c.obs_node || !c.obs_kp || !c.obs_outlier)))) {
-            set_error("icg_ba_update_and_cull_resident: window %d: obs_off must start at 0 and observation arrays must be given", w);
-            return ICG_EINVAL;
-        }
-        for (int l = 0; l < p.L; l++) {
-            if (c.obs_off[l + 1] < c.obs_off[l] || c.lm_ref_node[l] < 0 || c.lm_ref_node[l] >= p.K) {
-                set_error("icg_ba_update_and_cull_resident: window %d landmark %d: obs_off not monotone or reference node out of range", w, l);
-                return ICG_EINVAL;
-            }
-        }
-        for (int o = 0; o < no; o++)
-            if (c.obs_node[o] < 0 || c.obs_node[o] >= p.K) {
-                set_error("icg_ba_update_and_cull_resident: window %d observation %d: node %d out of range", w, o, c.obs_node[o]);
-                return ICG_EINVAL;
-            }
-        CullWin &W = win[w];
-        memcpy(W.R_bc, c.R_bc, sizeof(W.R_bc)), memcpy(W.t_bc, c.t_bc, sizeof(W.t_bc));
-        W.td_bc = c.td_bc, W.K = p.K, W.L = p.L, W.estimate_ext = c.estimate_ext != 0, W.estimate_td = c.estimate_td != 0;
-        W.lm0 = (int) nL, W.off0 = (int) (nL + w), W.obs0 = (int) nO, W.node0 = (int) nK;
-        nL += p.L, nO += no, nK += p.K;
-    }
+    const size_t sL = built ? 0 : nL, sO = built ? 0 : nO;  // the host lists' staging
     Layout lay;
-    const size_t i_win = lay.take(sizeof(CullWin) * n), i_ref = lay.take(4 * nL), i_off = lay.take(4 * (nL + n)), i_node = lay.take(4 * nO),
-                 i_rkp = lay.take(8 * nL), i_kp = lay.take(8 * nO);
+    const size_t i_win = lay.take(sizeof(CullWin) * n), i_ref = lay.take(4 * sL), i_off = lay.take(4 * (sL + (built ? 0 : n))), i_node = lay.take(4 * sO),
+                 i_rkp = lay.take(8 * sL), i_kp = lay.take(8 * sO);
     const size_t in_bytes = lay.size();
     const size_t o_win = lay.take(sizeof(CullOut) * n), o_pose = lay.take(96 * nK), o_pw = lay.take(24 * nL), o_depth = lay.take(8 * nL),
                  o_lmo = lay.take(nL), o_obso = lay.take(nO);
@@ -1555,10 +1541,11 @@ int icg_ba_update_and_cull_resident(icg_ba *h, int n_windows, const icg_ba_probl
     ICG_CUDA(cudaSetDevice(h->device));
     cudaStream_t s = h->stream;
     if (lay.size() > h->cull.n) ICG_CUDA(cudaStreamSynchronize(s));
-    if ((rc = hd_reserve(h, h->cull, lay.size(), "icg_ba_update_and_cull_resident")) != ICG_OK) return rc;
+    int rc = hd_reserve(h, h->cull, lay.size(), fn);
+    if (rc != ICG_OK) return rc;
     unsigned char *H = h->cull.h, *Dv = h->cull.d;
     memcpy(H + i_win, win.data(), sizeof(CullWin) * n);
-    for (int w = 0; w < n; w++) {
+    for (int w = 0; !built && w < n; w++) {
         const icg_ba_problem &p = problems[w];
         const icg_ba_cull_window &c = io[w];
         const CullWin &W = win[w];
@@ -1573,11 +1560,13 @@ int icg_ba_update_and_cull_resident(icg_ba *h, int n_windows, const icg_ba_probl
         if (no > 0) memcpy(H + i_node + 4 * (size_t) W.obs0, c.obs_node, 4 * (size_t) no), memcpy(H + i_kp + 8 * (size_t) W.obs0, c.obs_kp, 8 * (size_t) no);
     }
     ICG_CUDA(cudaMemcpyAsync(Dv, H, in_bytes, cudaMemcpyHostToDevice, s));
+    const CullSrc src = built ? *built
+                              : CullSrc{(const int *) (Dv + i_ref), (const int *) (Dv + i_off), (const int *) (Dv + i_node), nullptr,
+                                        (const float *) (Dv + i_rkp), (const float *) (Dv + i_kp)};
     CullArgs a;
-    a.cam = *cam, a.std = reprojection_error_std;
+    a.cam = *cam, a.std = std;
     a.pose = h->D.pose, a.ext = h->D.ext, a.rho = h->D.rho, a.pose_stride = C.K * 7, a.rho_stride = C.L;
-    a.win = (const CullWin *) (Dv + i_win), a.lm_ref_node = (const int *) (Dv + i_ref), a.obs_off = (const int *) (Dv + i_off);
-    a.obs_node = (const int *) (Dv + i_node), a.lm_ref_kp = (const float *) (Dv + i_rkp), a.obs_kp = (const float *) (Dv + i_kp);
+    a.win = (const CullWin *) (Dv + i_win), a.lm_ref_node = src.ref, a.obs_off = src.off, a.obs_node = src.node, a.lm_ref_kp = src.rkp, a.obs_kp = src.kp;
     a.out = (CullOut *) (Dv + o_win), a.cam_pose = (double *) (Dv + o_pose), a.lm_pw = (double *) (Dv + o_pw), a.lm_depth = (double *) (Dv + o_depth);
     a.lm_outlier = Dv + o_lmo, a.obs_outlier = Dv + o_obso;
     ICG_CUDA(launch_update_cull(a, n, s));
@@ -1588,11 +1577,12 @@ int icg_ba_update_and_cull_resident(icg_ba *h, int n_windows, const icg_ba_probl
     }
     ICG_CUDA(cudaMemcpyAsync(H + in_bytes, Dv + in_bytes, out_bytes, cudaMemcpyDeviceToHost, s));
     ICG_CUDA(cudaStreamSynchronize(s));
-    if (h->D.world > 1 && (rc = shard_timed_out(h, "icg_ba_update_and_cull_resident")) != ICG_OK) return rc;
-    // where the flags sit, for vision_body (sharded: the rank's own shard's)
-    h->cull_res_n = n, h->cull_res_win = win, h->cull_res_nobs.resize(n);
-    for (int w = 0; w < n; w++) h->cull_res_nobs[w] = problems[w].L > 0 ? io[w].obs_off[problems[w].L] : 0;
-    h->cull_res_ref = i_ref, h->cull_res_off = i_off, h->cull_res_lmo = o_lmo, h->cull_res_obso = o_obso;
+    if (h->D.world > 1 && (rc = shard_timed_out(h, fn)) != ICG_OK) return rc;
+    // where the lists and flags sit, for vision_body (sharded: the rank's own shard's)
+    h->cull_res_n = n, h->cull_res_win = win, h->cull_res_nobs = nobs;
+    h->cull_res_ref = src.ref, h->cull_res_off = src.off, h->cull_res_node = src.node, h->cull_res_fac = src.fac;
+    h->cull_res_rkp = src.rkp, h->cull_res_kp = src.kp, h->cull_res_lmo = Dv + o_lmo, h->cull_res_obso = Dv + o_obso;
+    h->cull_res_href = h->cull_res_hoff = h->cull_res_hnode = h->cull_res_hfac = nullptr;
     for (int w = 0; w < n; w++) {
         const icg_ba_problem &p = problems[w];
         icg_ba_cull_window &c = io[w];
@@ -1603,11 +1593,147 @@ int icg_ba_update_and_cull_resident(icg_ba *h, int n_windows, const icg_ba_probl
         memcpy(c.counts, O.counts, sizeof(c.counts));
         memcpy(c.cam_pose, H + o_pose + 96 * (size_t) W.node0, 96 * (size_t) p.K);
         if (p.L == 0) continue;
-        const int no = c.obs_off[p.L];
         memcpy(c.lm_pw, H + o_pw + 24 * (size_t) W.lm0, 24 * (size_t) p.L);
         memcpy(c.lm_depth, H + o_depth + 8 * (size_t) W.lm0, 8 * (size_t) p.L);
         memcpy(c.lm_outlier, H + o_lmo + W.lm0, p.L);
-        if (no > 0) memcpy(c.obs_outlier, H + o_obso + W.obs0, no);
+        if (nobs[w] > 0) memcpy(c.obs_outlier, H + o_obso + W.obs0, nobs[w]);
+    }
+    return ICG_OK;
+}
+
+extern "C" {
+
+int icg_ba_marginalize(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg, icg_ba_prior *out) {
+    return marginalize_body(h, n_windows, problems, num_marg, out, false);
+}
+
+int icg_ba_marginalize_resident(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg, icg_ba_prior *out) {
+    if (h && h->D.world > 1) return marginalize_sharded(h, n_windows, problems, num_marg, out, nullptr, "icg_ba_marginalize_resident");
+    return marginalize_body(h, n_windows, problems, num_marg, out, true);
+}
+
+int icg_ba_update_and_cull_resident(icg_ba *h, int n_windows, const icg_ba_problem *problems, const icg_camera *cam, double reprojection_error_std,
+                                    icg_ba_cull_window *io) {
+    static const char *fn = "icg_ba_update_and_cull_resident";
+    int rc = resident_single_rank(h, n_windows, problems, fn, true);
+    if (rc != ICG_OK) return rc;
+    if (!cam || !io) {
+        set_error("%s: bad arguments", fn);
+        return ICG_EINVAL;
+    }
+    const BaCaps &C = h->C;
+    const int n = n_windows;
+    std::vector<CullWin> win(n);
+    std::vector<int> nobs(n);
+    size_t nL = 0, nO = 0, nK = 0;
+    for (int w = 0; w < n; w++) {
+        const icg_ba_problem &p = problems[w];
+        const icg_ba_cull_window &c = io[w];
+        if (p.K < 2 || p.K > C.K || p.L < 0 || p.L > C.L || !c.cam_pose ||
+            (p.L > 0 && (!c.lm_ref_node || !c.lm_ref_kp || !c.obs_off || !c.lm_pw || !c.lm_depth || !c.lm_outlier))) {
+            set_error("%s: window %d: sizes out of range or arrays missing", fn, w);
+            return ICG_EINVAL;
+        }
+        const int no = p.L > 0 ? c.obs_off[p.L] : 0;
+        if (p.L > 0 && (c.obs_off[0] != 0 || no < 0 || no > INT32_MAX - (int64_t) nO || (no > 0 && (!c.obs_node || !c.obs_kp || !c.obs_outlier)))) {
+            set_error("%s: window %d: obs_off must start at 0 and observation arrays must be given", fn, w);
+            return ICG_EINVAL;
+        }
+        for (int l = 0; l < p.L; l++) {
+            if (c.obs_off[l + 1] < c.obs_off[l] || c.lm_ref_node[l] < 0 || c.lm_ref_node[l] >= p.K) {
+                set_error("%s: window %d landmark %d: obs_off not monotone or reference node out of range", fn, w, l);
+                return ICG_EINVAL;
+            }
+        }
+        for (int o = 0; o < no; o++)
+            if (c.obs_node[o] < 0 || c.obs_node[o] >= p.K) {
+                set_error("%s: window %d observation %d: node %d out of range", fn, w, o, c.obs_node[o]);
+                return ICG_EINVAL;
+            }
+        CullWin &W = win[w];
+        memcpy(W.R_bc, c.R_bc, sizeof(W.R_bc)), memcpy(W.t_bc, c.t_bc, sizeof(W.t_bc));
+        W.td_bc = c.td_bc, W.K = p.K, W.L = p.L, W.estimate_ext = c.estimate_ext != 0, W.estimate_td = c.estimate_td != 0;
+        W.lm0 = (int) nL, W.off0 = (int) (nL + w), W.obs0 = (int) nO, W.node0 = (int) nK;
+        nobs[w] = no;
+        nL += p.L, nO += no, nK += p.K;
+    }
+    return cull_run(h, n, problems, cam, reprojection_error_std, io, win, nobs, nL, nO, nK, nullptr, fn);
+}
+
+int icg_ba_update_and_cull_built(icg_ba *h, int n_windows, const icg_ba_problem *problems, const icg_camera *cam, double reprojection_error_std,
+                                 icg_ba_cull_window *io, icg_ba_cull_lists *lists) {
+    static const char *fn = "icg_ba_update_and_cull_built";
+    if (h && h->D.world > 1) {
+        set_error("%s: not available on a landmark-sharded handle (its lists would be shard-local)", fn);
+        return ICG_EUNSUPPORTED;
+    }
+    // lists_n is 0 or the uploaded count, so a call over another window count fails here already
+    int rc = resident_single_rank(h, n_windows, problems, fn);
+    if (rc != ICG_OK) return rc;
+    const int n = n_windows;
+    if (!cam || !io) {
+        set_error("%s: bad arguments", fn);
+        return ICG_EINVAL;
+    }
+    if (h->lists_n != n) {
+        set_error("%s: no built lists of these %d windows are current (icg_ba_slide_vision_resident, with no upload or other slide since)", fn, n);
+        return ICG_EINVAL;
+    }
+    const BaCaps &C = h->C;
+    std::vector<CullWin> win(n);
+    size_t nK = 0;
+    for (int w = 0; w < n; w++) {
+        const icg_ba_problem &p = problems[w];
+        const icg_ba_cull_window &c = io[w];
+        const CullWin &lw = h->lists_win[w];
+        const int no = h->lists_nobs[w];
+        // the caller's observation arrays hold max_L + max_F entries: lists not shaped as the reference builds them (an entry listed twice
+        // in the host lists the slide carried) can be longer
+        if (no > C.L + C.F) {
+            set_error("%s: window %d: the built lists hold %d observations, more than max_L + max_F = %d", fn, w, no, C.L + C.F);
+            return ICG_EINVAL;
+        }
+        if (p.K != lw.K || p.L != lw.L || p.K > C.K || !c.cam_pose || (p.L > 0 && (!c.lm_pw || !c.lm_depth || !c.lm_outlier)) || (no > 0 && !c.obs_outlier)) {
+            set_error("%s: window %d: sizes differ from the built lists' (K %d, L %d) or arrays missing", fn, w, lw.K, lw.L);
+            return ICG_EINVAL;
+        }
+        if (c.lm_ref_node || c.lm_ref_kp || c.obs_off || c.obs_node || c.obs_kp || c.obs_factor) {
+            set_error("%s: window %d: the lists are the built ones; their inputs must be NULL", fn, w);
+            return ICG_EINVAL;
+        }
+        CullWin &W = win[w];
+        memcpy(W.R_bc, c.R_bc, sizeof(W.R_bc)), memcpy(W.t_bc, c.t_bc, sizeof(W.t_bc));
+        W.td_bc = c.td_bc, W.K = p.K, W.L = p.L, W.estimate_ext = c.estimate_ext != 0, W.estimate_td = c.estimate_td != 0;
+        W.lm0 = lw.lm0, W.off0 = lw.off0, W.obs0 = lw.obs0, W.node0 = (int) nK;
+        nK += p.K;
+    }
+    bool want_kp = false;
+    for (int w = 0; lists && w < n; w++) want_kp = want_kp || lists[w].lm_ref_kp || lists[w].obs_kp;
+    HostDev<unsigned char> &lb = h->lists[h->lists_cur];
+    const icg_ba::ListAt &at = h->lists_at[h->lists_cur];
+    const CullSrc src{(const int *) (lb.d + at.ref), (const int *) (lb.d + at.off), (const int *) (lb.d + at.node), (const int *) (lb.d + at.fac),
+                      (const float *) (lb.d + at.rkp), (const float *) (lb.d + at.kp)};
+    rc = cull_run(h, n, problems, cam, reprojection_error_std, io, win, h->lists_nobs, h->lists_nL, h->lists_nO, nK, &src, fn);
+    if (rc != ICG_OK) return rc;
+    // the integer lists on the host (icg_ba_marginalize_resident_culled's NULL lists read them there) and, when asked for, the keypoints
+    h->cull_res_n = 0;
+    ICG_CUDA(cudaMemcpyAsync(lb.h, lb.d, at.rkp, cudaMemcpyDeviceToHost, h->stream));
+    if (want_kp) ICG_CUDA(cudaMemcpyAsync(lb.h + at.rkp, lb.d + at.rkp, at.end - at.rkp, cudaMemcpyDeviceToHost, h->stream));
+    ICG_CUDA(cudaStreamSynchronize(h->stream));
+    h->cull_res_n = n;
+    h->cull_res_href = (const int *) (lb.h + at.ref), h->cull_res_hoff = (const int *) (lb.h + at.off), h->cull_res_hnode = (const int *) (lb.h + at.node);
+    h->cull_res_hfac = (const int *) (lb.h + at.fac);
+    for (int w = 0; lists && w < n; w++) {
+        const int L = problems[w].L, no = h->lists_nobs[w];
+        const CullWin &W = win[w];
+        icg_ba_cull_lists &o = lists[w];
+        o.n_obs = no;
+        if (o.lm_ref_node) memcpy(o.lm_ref_node, lb.h + at.ref + 4 * (size_t) W.lm0, 4 * (size_t) L);
+        if (o.obs_off) memcpy(o.obs_off, lb.h + at.off + 4 * (size_t) W.off0, 4 * ((size_t) L + 1));
+        if (o.obs_node) memcpy(o.obs_node, lb.h + at.node + 4 * (size_t) W.obs0, 4 * (size_t) no);
+        if (o.obs_factor) memcpy(o.obs_factor, lb.h + at.fac + 4 * (size_t) W.obs0, 4 * (size_t) no);
+        if (o.lm_ref_kp) memcpy(o.lm_ref_kp, lb.h + at.rkp + 8 * (size_t) W.lm0, 8 * (size_t) L);
+        if (o.obs_kp) memcpy(o.obs_kp, lb.h + at.kp + 8 * (size_t) W.obs0, 8 * (size_t) no);
     }
     return ICG_OK;
 }
@@ -1636,9 +1762,24 @@ int icg_ba_marginalize_resident_culled(icg_ba *h, int n_windows, const icg_ba_pr
     // of marginalize_body, which reads the factor set on the host as well
     std::vector<std::vector<uint8_t>> masks(n_windows);
     std::vector<const uint8_t *> mp(n_windows);
+    // a NULL list after a built culling is that culling's own (its host copy)
+    const bool built = h->cull_res_n == n_windows && h->cull_res_href;
     for (int w = 0; w < n_windows; w++) {
         const icg_ba_problem &p = problems[w];
-        const icg_ba_cull_window &c = culled[w];
+        icg_ba_cull_window c = culled[w];
+        if (!c.lm_ref_node || !c.obs_off || !c.obs_node || !c.obs_factor) {
+            const CullWin *bw = built ? &h->cull_res_win[w] : nullptr;
+            if (p.L > 0 && (!bw || bw->L != p.L || bw->K != p.K)) {
+                set_error("icg_ba_marginalize_resident_culled: window %d: lists missing, and no built culling of these windows is current", w);
+                return ICG_EINVAL;
+            }
+            if (bw) {
+                if (!c.lm_ref_node) c.lm_ref_node = h->cull_res_href + bw->lm0;
+                if (!c.obs_off) c.obs_off = h->cull_res_hoff + bw->off0;
+                if (!c.obs_node) c.obs_node = h->cull_res_hnode + bw->obs0;
+                if (!c.obs_factor) c.obs_factor = h->cull_res_hfac + bw->obs0;
+            }
+        }
         if (!node_in_map[w] || (p.L > 0 && (!c.lm_ref_node || !c.obs_off || !c.lm_outlier)) || p.K > h->C.K || p.L > h->C.L || p.F > h->C.F ||
             (p.L > 0 && c.obs_off[p.L] > 0 && (!c.obs_node || !c.obs_factor || !c.obs_outlier))) {
             set_error("icg_ba_marginalize_resident_culled: window %d: arrays missing", w);

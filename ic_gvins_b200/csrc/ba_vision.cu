@@ -38,13 +38,25 @@ __device__ void cam_point(const icg_camera &c, float u, float v, double *p) {
     p[2] = 1.0;
 }
 
+// an entry of the last culling's list is kept in the next one (step 4): not flagged, in a next node, naming a carried factor or, with no
+// factor, in the landmark's reference node
+__device__ __forceinline__ bool listed(int f, int k, uint8_t flagged, int8_t next_node, int ref, int oF, const int *fmap) {
+    if (flagged != 0 || next_node < 0) return false;
+    return f >= 0 ? f < oF && fmap[f] >= 0 : f == -1 && k == ref;
+}
+
+__device__ __forceinline__ void list_entry(int *node, int *fac, float *kp, int e, int nd, int f, const float *xy) {
+    node[e] = nd, fac[e] = f, kp[2 * e] = xy[0], kp[2 * e + 1] = xy[1];
+}
+
 }  // namespace
 
 // Rules (include/icgvins_b200.h, icg_ba_slide_vision_resident): landmark l of the old window is carried when it is not a culling outlier, its
 // reference node is usable (in the map, not marginalized, kept by the slide) and 1 / (1 / rho) is not NaN; its old factors survive when their
 // observation is listed by the culling and not an outlier and their observing node is usable; its new observations follow in node order.  New map
 // points follow the carried landmarks in creation order, each with one factor from its reference node to the current node.  On a landmark shard
-// the old window is the rank's shard and only the rank's new points are kept; the numbering below is then the shard's.
+// the old window is the rank's shard and only the rank's new points are kept; the numbering below is then the shard's.  On one GPU the kernel
+// then writes the next culling's lists (step 4, the list rule of icg_ba_update_and_cull_built).
 __global__ void __launch_bounds__(VIS_THREADS) ba_vision_build(VisArgs a) {
     __shared__ Scan::TempStorage tmp;
     __shared__ int s_nobs, s_nnew;
@@ -57,7 +69,7 @@ __global__ void __launch_bounds__(VIS_THREADS) ba_vision_build(VisArgs a) {
     const double *rho = a.rho + wL;
     const int *ref_node = a.lm_ref_node + W.cull_lm0;
     const uint8_t *lm_out = a.lm_outlier + W.cull_lm0, *obs_out = a.obs_outlier + W.cull_obs0;
-    const int *ofac = a.obs_factor + W.obs_factor0;
+    const int *ofac = W.obs_factor;
     if (t == 0) {
         int n = W.dev_n ? *W.dev_n : W.n_obs, m = W.dev_new_n ? *W.dev_new_n : W.n_new;
         cnt[6] = n, cnt[7] = m;
@@ -66,14 +78,17 @@ __global__ void __launch_bounds__(VIS_THREADS) ba_vision_build(VisArgs a) {
         s_nobs = n, s_nnew = m;
     }
     // scratch (vis_scratch_ints): fkeep (oF) | pos_of (oL) | mask (oL) | nkeep (oL) | keep, nn, lidx, fbase, nbase (oL + n_new each) | ref node
-    // of each new point (n_new)
+    // of each new point (n_new); with the lists: | next factor row of each old factor, -1: dropped (oF) | list entries per landmark (oL + n_new)
     const int NA = oL + W.n_new;
     int *fkeep = a.scratch + W.scr, *pos_of = fkeep + oF, *mask = pos_of + oL, *nkeep = mask + oL;
     int *keep = nkeep + oL, *nn = keep + NA, *lidx = nn + NA, *fbase = lidx + NA, *nbase = fbase + NA, *new_ref = nbase + NA;
     const double *lref = a.lm_ref + wL * 7;
     double *lref_next = a.lm_ref_next + wL * 7;
     uint8_t *lm_nan = a.lm_nan + W.lm_out;
-    for (int q = t; q < oF; q += VIS_THREADS) fkeep[q] = 0;
+    for (int q = t; q < oF; q += VIS_THREADS) {
+        fkeep[q] = 0;
+        if (a.l_off) new_ref[W.n_new + q] = -1;  // fmap, step 4
+    }
     for (int p = t; p < oL; p += VIS_THREADS) pos_of[perm[p]] = p, mask[perm[p]] = 0;
     __syncthreads();
     const int nobs = s_nobs, nnew = s_nnew;
@@ -164,6 +179,7 @@ __global__ void __launch_bounds__(VIS_THREADS) ba_vision_build(VisArgs a) {
                 const int f = meta[4 * q + 3], ob = W.onode[meta[4 * q + 2]];
                 if (!fkeep[f] || ob < 0) continue;
                 f_lm[fo] = li, f_ref[fo] = r, f_obs[fo] = ob, f_src[fo] = f;
+                if (a.l_off) new_ref[W.n_new + f] = fo;
                 fo++;
             }
         } else {
@@ -204,6 +220,59 @@ __global__ void __launch_bounds__(VIS_THREADS) ba_vision_build(VisArgs a) {
         c[6] = r0[3], c[7] = r0[4], c[8] = r0[5];
         c[9] = W.obs_vel[2 * k], c[10] = W.obs_vel[2 * k + 1], c[11] = 0.0;
         c[12] = r0[6], c[13] = W.node_td[node];
+    }
+    if (!a.l_off) return;
+    __syncthreads();
+    const int *fmap = new_ref + W.n_new;
+    int *lcnt = new_ref + W.n_new + oF;
+    // 4. the next culling's lists, landmark by landmark in next-row order: a carried landmark's entries of the last culling's list that are not
+    // flagged, lie in a next node and name a carried factor (or no factor, in the reference node), then its new observations in node order;
+    // a new map point's creation observation (when it has a factor) and its reference observation
+    const int *ooff = a.obs_off + W.cull_off0, *o_node = a.obs_node + W.cull_obs0;
+    const float *o_kp = a.obs_kp + 2 * (size_t) W.cull_obs0, *o_rkp = a.lm_ref_kp + 2 * (size_t) W.cull_lm0;
+    for (int i = t; i < NA; i += VIS_THREADS) {
+        int c = 0;
+        if (i < oL && keep[i]) {
+            const int r = ref_node[i];
+            for (int o = ooff[i]; o < ooff[i + 1]; o++) c += listed(ofac[o], o_node[o], obs_out[o], W.onode[o_node[o]], r, oF, fmap);
+            c += nn[i];
+        } else if (keep[i]) {
+            c = 1 + nn[i];
+        }
+        lcnt[i] = c;
+    }
+    __syncthreads();
+    const int n_list = block_exscan(lcnt, NA, tmp);
+    int *l_ref = a.l_ref + W.lm_out, *l_off = a.l_off + W.lm_out + w, *l_node = a.l_node + W.lst_obs, *l_fac = a.l_fac + W.lst_obs;
+    float *l_rkp = a.l_rkp + 2 * (size_t) W.lm_out, *l_kp = a.l_kp + 2 * (size_t) W.lst_obs;
+    if (t == 0) cnt[8] = n_list, l_off[L] = n_list;
+    for (int i = t; i < NA; i += VIS_THREADS) {
+        if (!keep[i]) continue;
+        const int li = lidx[i];
+        int e = lcnt[i];
+        l_off[li] = e;
+        if (i < oL) {
+            const int r = ref_node[i];
+            l_ref[li] = W.onode[r], l_rkp[2 * li] = o_rkp[2 * i], l_rkp[2 * li + 1] = o_rkp[2 * i + 1];
+            for (int o = ooff[i]; o < ooff[i + 1]; o++)
+                if (listed(ofac[o], o_node[o], obs_out[o], W.onode[o_node[o]], r, oF, fmap))
+                    list_entry(l_node, l_fac, l_kp, e++, W.onode[o_node[o]], ofac[o] >= 0 ? fmap[ofac[o]] : -1, o_kp + 2 * o);
+        } else {
+            const int j = i - oL;
+            l_ref[li] = new_ref[j], l_rkp[2 * li] = W.new_ref_xy[2 * j], l_rkp[2 * li + 1] = W.new_ref_xy[2 * j + 1];
+            if (nn[i]) list_entry(l_node, l_fac, l_kp, e++, W.cur_node, fbase[i], W.new_cur_xy + 2 * j);
+            list_entry(l_node, l_fac, l_kp, e, new_ref[j], -1, W.new_ref_xy + 2 * j);
+        }
+    }
+    // a carried landmark's new observations end its list (its segment ends where the next one's starts)
+    for (int k = t; k < nobs; k += VIS_THREADS) {
+        const int j = W.src ? W.src[k] : k;
+        if (j < 0 || j >= W.n_in) continue;
+        const int l = W.obs_lm[j], node = W.obs_node ? W.obs_node[j] : W.cur_node;
+        if (node < 0 || node >= W.nK || l < 0 || l >= oL || !keep[l] || W.onode[ref_node[l]] == node || isnan(lref[(size_t) l * 7])) continue;
+        const int rank = __popc(mask[l] & ((1u << node) - 1u));
+        const int end = l + 1 < NA ? lcnt[l + 1] : n_list;
+        list_entry(l_node, l_fac, l_kp, end - nn[l] + rank, node, fbase[l] + nkeep[l] + rank, W.obs_xy + 2 * k);
     }
 }
 

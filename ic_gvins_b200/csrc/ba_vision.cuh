@@ -23,8 +23,8 @@ struct VisWin {
     int64_t frame_id[VIS_MAX_FRAMES];  // frame table of the new map points' reference frames
     int frame_node[VIS_MAX_FRAMES];
     int oK, oL, oF, nK, n_frames, cur_node;
-    int cull_lm0, cull_off0, cull_obs0, n_cull_obs;  // the window's slices of the culling's staging
-    int obs_factor0;                                  // first entry of the window's obs_factor in VisArgs::obs_factor
+    int cull_lm0, cull_off0, cull_obs0, n_cull_obs;  // the window's slices of the last culling's lists and flags
+    const int *obs_factor;                            // the window's obs_factor (n_cull_obs entries): the caller's, staged, or the built lists'
     // tracked observations: k < count (*dev_n when given, else n_obs), j = src ? src[k] : k (j < n_in); lm = obs_lm[j], node = obs_node[j]
     // (obs_node NULL: cur_node); undis_xy / vel at k
     int n_obs, n_in;
@@ -39,11 +39,12 @@ struct VisWin {
     const int64_t *new_ref_frame;
     // bounds: next landmarks Lb = oL + n_new, next factors Fb = oF + n_obs + n_new, new factors Nb = n_obs + n_new
     int lm_out, f_out, nf_out, scr;  // offsets of the window's output rows (Lb, Fb, Nb) and int scratch
+    int lst_obs;                     // the next culling's lists: first entry of the window's observations (Ob = n_cull_obs + n_obs + 2 n_new)
 };
 
 // per window: [L, F, new factors, error code, error index, landmarks dropped for a NaN inverse depth, the observation count and the new-point
-// count the kernel read (a landmark shard's ranks must read the same)]
-constexpr int VIS_COUNTS = 8;
+// count the kernel read (a landmark shard's ranks must read the same), the entries of the next culling's lists (0 when they are not emitted)]
+constexpr int VIS_COUNTS = 9;
 enum VisError { VIS_OK = 0, VIS_EOBS_FACTOR = 1, VIS_ECOUNT = 2, VIS_ESRC = 3, VIS_ENODE = 4, VIS_ELM = 5, VIS_EDUP = 6, VIS_EFRAME = 7, VIS_EROW = 8 };
 
 struct VisArgs {
@@ -54,10 +55,10 @@ struct VisArgs {
     const double *rho;
     const int *f_meta_s, *lm_off, *lm_perm;
     const double *lm_ref;  // per landmark: its reference row pts0[3] | vel0[3] | td0 (NaN: unknown), capacity-strided (7 L per window)
-    // the last culling (its staging)
-    const int *lm_ref_node, *obs_off;
+    // the last culling: its lists (the host lists it staged, or the lists the last slide built) and its flags
+    const int *lm_ref_node, *obs_off, *obs_node;
+    const float *lm_ref_kp, *obs_kp;
     const uint8_t *lm_outlier, *obs_outlier;
-    const int *obs_factor;
     // outputs: counts (VIS_COUNTS per window), per next landmark lm_src, its origin (old landmark, or -(j + 1) for new map point j) and
     // invdepth, per old landmark and new map point a NaN-drop flag (Lb bytes), per next factor f_lm / f_ref / f_obs / f_src, per new factor
     // its 14 constants (the new factors in factor order); lm_ref_next: the next window's reference rows (capacity-strided, as lm_ref)
@@ -65,6 +66,10 @@ struct VisArgs {
     uint8_t *lm_nan;
     double *invdepth, *f_new, *lm_ref_next;
     int *scratch;
+    // the next culling's lists (NULL: not emitted; landmark shards never emit them).  Per window, in next-landmark order: l_ref / l_rkp at
+    // lm_out (Lb), l_off at lm_out + w (Lb + 1), l_node / l_fac / l_kp at lst_obs (Ob); keypoints 2 floats each
+    int *l_ref, *l_off, *l_node, *l_fac;
+    float *l_rkp, *l_kp;
 };
 
 cudaError_t launch_vision(const VisArgs &a, int n_windows, cudaStream_t stream);

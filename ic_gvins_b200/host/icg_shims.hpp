@@ -309,6 +309,14 @@ public:
     void updateAndCull(const icg_ba_problem &problem, const icg_camera &camera, double reprojection_error_std, icg_ba_cull_window &io) {
         check(icg_ba_update_and_cull_resident(h_, 1, &problem, &camera, reprojection_error_std, &io), "icg_ba_update_and_cull_resident");
     }
+    // The same on the observation lists the last slideVision built on the device (icg_ba_update_and_cull_built): io's list inputs stay NULL,
+    // its outputs are updateAndCull's with obs_outlier indexed by the built list, and `lists` (may be null; each array may be NULL) receives
+    // that list, so that the caller maps each flag to its Feature through (landmark, obs_node).  marginalization(problem, num_marg, io,
+    // node_in_map) and the next slideVision (vision.obs_factor NULL) then use the culling's own lists.  Single-GPU solvers only.
+    void updateAndCullBuilt(const icg_ba_problem &problem, const icg_camera &camera, double reprojection_error_std, icg_ba_cull_window &io,
+                            icg_ba_cull_lists *lists = nullptr) {
+        check(icg_ba_update_and_cull_built(h_, 1, &problem, &camera, reprojection_error_std, &io, lists), "icg_ba_update_and_cull_built");
+    }
 
     // GVINS::doReintegration (IG/ic_gvins.cc:1680-1695) on the window this solver just optimised, as gvinsOptimization calls it while the
     // window is not full (:1223-1227).  imu = the rows (dt, dtheta[3], dvel[3]) of every factor's imu_buffer_, imu_off = n_imu + 1 offsets

@@ -591,11 +591,47 @@ int icg_ba_update_and_cull_resident(icg_ba *h, int n_windows, const icg_ba_probl
  * iff its landmark is not a culling outlier, neither its observation nor the landmark's reference observation is a feature outlier, and
  * node_in_map[w][f_obs[f]] is set (the keyframes gvinsRemoveAllSecondNewFrame left in the map, IG/ic_gvins.cc:1391-1410): the factor set
  * gvinsMarginalization builds (:1558-1609).  The chi-square activity plays no part (removeReprojectionFactorsByChi2 never marks a feature).
- * culled: the io array of icg_ba_update_and_cull_resident after that call (obs_factor must be set); node_in_map: K bytes per window.  The
+ * culled: the io array of icg_ba_update_and_cull_resident after that call (obs_factor must be set); node_in_map: K bytes per window.  After
+ * icg_ba_update_and_cull_built, culled's lm_ref_node, obs_off, obs_node and obs_factor may be NULL: each NULL one is that culling's own list
+ * (the handle keeps a host copy; ICG_EINVAL when no built culling of these windows is current).  The
  * handle's factor activity is not changed.  On a landmark-sharded handle: collective, as icg_ba_marginalize_resident; each rank passes its
  * own `culled` array (its shard's landmarks, obs_factor naming its shard's factors) and the same node_in_map. */
 int icg_ba_marginalize_resident_culled(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg,
                                        const icg_ba_cull_window *culled, const uint8_t *const *node_in_map, icg_ba_prior *out);
+/*
+ * icg_ba_update_and_cull_resident on the observation lists the last icg_ba_slide_vision_resident built on the device, so that no list crosses
+ * PCIe.  The reference only appends to MapPoint::observations_ (tracking.cc:437 a tracked frame, :771 then :778 a new point's current and
+ * reference frames), its walk only skips entries (:1061-1069: outlier features, frames not in the map) and a landmark's reference never
+ * changes.  So the next culling's list of a landmark is the last one's without the dropped entries, plus the new keyframes' observations.
+ * The list rule.  The slide writes the next window's lists landmark by landmark in next-window row order:
+ *   a carried landmark: the entries of the last culling's list for it, in their old order, that were not flagged (obs_outlier 0), whose node
+ *     maps to a next node, and that name a factor the slide carries (renumbered to its next row) or name none (-1) and lie in the landmark's
+ *     reference node; then its new observations in node order (their new factor rows, nodes and obs_undis_xy);
+ *   new map point j: its creation observation (cur_node, its factor, new_cur_undis_xy[j]), then its reference observation (its reference
+ *     node, -1, new_ref_undis_xy[j]); when the two nodes are the same the slide builds no factor and only the reference entry is written;
+ *   lm_ref_node: the old reference node through the slide's node map, or the new point's frame-table node; lm_ref_kp: the old one, or
+ *     new_ref_undis_xy[j].  Nodes and factors are next-window ones.
+ * For lists shaped as the reference builds them each entry is the one reference observation of its landmark or names exactly one factor, so
+ * n_obs = L + F of the window.
+ * The built lists are current from a successful icg_ba_slide_vision_resident (or the vision form of icg_ba_slide_ins_resident) until the
+ * next upload, any other slide or a shard export; a rejected slide leaves the previous ones current.  After this call they are the last
+ * culling's lists: icg_ba_marginalize_resident_culled and the next vision slide may then take NULL lists (obs_factor NULL) and use them.
+ * io[w]: R_bc, t_bc, td_bc, estimate_ext and estimate_td are read, the list inputs must be NULL; the outputs are icg_ba_update_and_cull_resident's,
+ * obs_outlier indexed by the built list and max_L + max_F long (the caller cannot know n_obs before the call; the host maps flags to its
+ * features through (landmark, obs_node)).  lists: NULL, or per window the lists the culling walked, copied to the caller's HOST arrays (each may
+ * be NULL).  The kernel and its arithmetic are the host-list call's.
+ * ICG_EINVAL, with the handle unchanged: no built lists of these n_windows are current, problems[w].K / L differ from the built window's, or
+ * a window's built lists hold more than max_L + max_F observations (possible only when the host lists they grew from were not shaped as the
+ * reference builds them, e.g. an entry listed twice).
+ * ICG_EUNSUPPORTED on a landmark-sharded handle.  Synchronous.
+ */
+typedef struct icg_ba_cull_lists { /* out, HOST, each may be NULL: the lists the culling walked, in its order */
+    int32_t n_obs;                 /* L + F for lists shaped as the reference builds them */
+    int32_t *lm_ref_node, *obs_off, *obs_node, *obs_factor; /* L, L + 1, max_L + max_F, max_L + max_F */
+    float *lm_ref_kp, *obs_kp;                               /* L x 2, (max_L + max_F) x 2 */
+} icg_ba_cull_lists;
+int icg_ba_update_and_cull_built(icg_ba *h, int n_windows, const icg_ba_problem *problems, const icg_camera *cam, double reprojection_error_std,
+                                 icg_ba_cull_window *io, icg_ba_cull_lists *lists);
 /*
  * GVINS::doReintegration (IG/ic_gvins.cc:1680-1695), which gvinsOptimization runs after the second Solve while the window is not full
  * (:1223-1227), on the IMU factors the handle holds.  For factor k of a window (joining nodes k and k + 1):
@@ -734,6 +770,7 @@ int icg_ba_slide_integrate_resident(icg_ba *h, int n_windows, const icg_ba_probl
  * the landmark (a landmark that carry.lm_src names keeps its old row; a new one takes its first factor's), and this call writes a new map
  * point's from its reference keypoint, velocity and node_td.  A new observation of a landmark whose row is unknown is ICG_EINVAL.
  * The reference's order is unordered_map iteration (implementation-defined); this order is fixed and only permutes rows.
+ * On a single-GPU handle the same kernel writes the next culling's lists (icg_ba_update_and_cull_built).
  * One CTA per window builds the structure on the device; the counts, the integer structure, the new invdepth rows and the new factors' constants
  * come back in one copy (one synchronisation), and the call goes on as icg_ba_slide_integrate_resident with that window, every check included.
  * A rejected call (ICG_EINVAL: max_L / max_F exceeded, a reference frame id missing from the table, a node, landmark or source index out of
@@ -745,7 +782,8 @@ typedef struct icg_ba_slide_vision {
     /* in: the old window */
     int32_t num_marg;
     const uint8_t *node_in_map;  /* old K: isKeyFrameInMap after gvinsRemoveAllSecondNewFrame */
-    const int32_t *obs_factor;   /* the culling's observations (its obs_off order): factor of each, -1 for none */
+    const int32_t *obs_factor;   /* the culling's observations (its obs_off order): factor of each, -1 for none; NULL after
+                                    icg_ba_update_and_cull_built: the built lists' */
     /* in: the new keyframes */
     icg_camera cam;
     const double *node_td;       /* next.K: frame->timeDelay() */
