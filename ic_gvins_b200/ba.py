@@ -360,6 +360,26 @@ class WindowSolver:
     def sync(self):
         check(lib().icg_ba_sync(self._h), "icg_ba_sync")
 
+    def peek_linearization(self, w: int) -> dict:
+        """Window w's system as the last linearisation and Schur complement left it (icg_ba_peek_linearization; a test read-out).  Mp: a
+        dict (reference node, observing node) -> packed upper 20x20; A_W: (L, 6K + 8) by landmark id; Hs: (NCV, NCV) lower triangle."""
+        from ._lib import Linearization
+        K, L, F = self.max_K, max(1, self.max_L), max(1, self.max_F)
+        NCV, N, PM = 6 * K + 7, 15 * K + 7, K * (K - 1)
+        a = dict(pair_ro=np.zeros(PM, np.int32), Mp=np.zeros(PM * 210), A_W=np.zeros(L * (NCV + 1)), h_l=np.zeros(L), g_l=np.zeros(L),
+                 H_c=np.zeros(N * N), g_c=np.zeros(N), costf=np.zeros(F), scale_l=np.zeros(L), Hs=np.zeros(NCV * NCV), visv=np.zeros(3 * NCV))
+        s = Linearization()
+        for name, arr in a.items():
+            setattr(s, name, arr.ctypes.data_as(C.POINTER(C.c_int32 if arr.dtype == np.int32 else C.c_double)))
+        check(lib().icg_ba_peek_linearization(self._h, w, C.byref(s)), "icg_ba_peek_linearization")
+        K, L, F, P = s.K, s.L, s.F, s.n_pairs
+        NCV, N = 6 * K + 7, 15 * K + 7
+        ro, Mp = a["pair_ro"][:P], a["Mp"][:P * 210].reshape(P, 210)
+        return dict(K=K, L=L, F=F, lin_buf=s.lin_buf, radius=s.radius, Mp={(int(v) >> 8, int(v) & 255): Mp[p].copy() for p, v in enumerate(ro)},
+                    A_W=a["A_W"][:L * (NCV + 1)].reshape(L, NCV + 1), h_l=a["h_l"][:L], g_l=a["g_l"][:L], scale_l=a["scale_l"][:L],
+                    H_c=a["H_c"][:N * N].reshape(N, N), g_c=a["g_c"][:N], costf=a["costf"][:F], Hs=a["Hs"][:NCV * NCV].reshape(NCV, NCV),
+                    visv=a["visv"][:3 * NCV].reshape(3, NCV))
+
     def residual_costs(self, prob):
         s = to_struct(prob)
         rc = np.zeros(prob["F"])

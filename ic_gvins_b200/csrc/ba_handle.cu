@@ -524,6 +524,7 @@ static int pack_window(icg_ba *h, int w, const icg_ba_problem &p, bool values, s
 // pack_window over n windows.  Per-window packing is independent (disjoint slices of the pinned staging arrays): spread it over a few host
 // threads -- it is memcpy-bound (about 0.4 MB per cfg-3 window) and sits inside the end-to-end path of every keyframe
 int pack_windows(icg_ba *h, int n, const icg_ba_problem *P, bool values) {
+    h->lin_ready = false;  // an upload or a slide replaces the windows
     const int nthreads = std::max(1, std::min({n / 4, 16, (int) std::thread::hardware_concurrency()}));
     std::vector<int> rcs(nthreads, ICG_OK);
     std::vector<std::string> errs(nthreads);
@@ -704,6 +705,7 @@ static int enqueue_lm(icg_ba *h, int max_num_iterations) {
         count_launch();
     }
     ICG_CHECK_LAUNCH();
+    h->lin_ready = true;
     return ICG_OK;
 }
 
@@ -1121,6 +1123,62 @@ int icg_ba_sync(icg_ba *h) {
     ICG_CUDA(cudaSetDevice(h->device));
     ICG_CUDA(cudaStreamSynchronize(h->stream));
     prof_collect(h);
+    return ICG_OK;
+}
+
+int icg_ba_peek_linearization(icg_ba *h, int w, icg_ba_linearization *out) {
+    static const char *fn = "icg_ba_peek_linearization";
+    if (!h || !out || w < 0 || w >= h->cur_windows) {
+        set_error("%s: bad arguments", fn);
+        return ICG_EINVAL;
+    }
+    if (h->D.S.split) {
+        set_error("%s: the split pipeline drives this handle; its reduced system is not kept in Hs", fn);
+        return ICG_EUNSUPPORTED;
+    }
+    if (!h->lin_ready) {
+        set_error("%s: no icg_ba_run / icg_ba_run_gvins since the windows were uploaded or last changed", fn);
+        return ICG_EINVAL;
+    }
+    ICG_CUDA(cudaSetDevice(h->device));
+    ICG_CUDA(cudaStreamSynchronize(h->stream_cam));
+    ICG_CUDA(cudaStreamSynchronize(h->stream));
+    const BaCaps &C = h->C;
+    const BaDev &D = h->D;
+    WinDims dm;
+    LmState st;
+    int P = 0;
+    ICG_CUDA(cudaMemcpy(&dm, D.dims + w, sizeof(dm), cudaMemcpyDeviceToHost));
+    ICG_CUDA(cudaMemcpy(&st, D.st + w, sizeof(st), cudaMemcpyDeviceToHost));
+    ICG_CUDA(cudaMemcpy(&P, D.npairs + w, sizeof(int), cudaMemcpyDeviceToHost));
+    const int b = st.lin_buf;
+    if (b < 0 || b > 1 || !D.Mp[b]) {
+        set_error("%s: window %d has no linearisation buffer %d", fn, w, b);
+        return ICG_EINVAL;
+    }
+    out->K = dm.K, out->L = dm.L, out->F = dm.F, out->n_pairs = P, out->lin_buf = b, out->radius = st.radius;
+    const size_t K = dm.K, L = dm.L, NCV = 6 * K + 7, N = 15 * K + 7, PM = (size_t) C.K * (C.K - 1), d = sizeof(double);
+    // a NULL destination is skipped.  get: n contiguous doubles; get2d: rows of cols doubles at a source row stride of ld doubles
+    auto get = [&](double *dst, const double *src, size_t n) -> cudaError_t {
+        return dst && n ? cudaMemcpy(dst, src, n * d, cudaMemcpyDeviceToHost) : cudaSuccess;
+    };
+    auto get2d = [&](double *dst, const double *src, size_t rows, size_t cols, size_t ld) -> cudaError_t {
+        return dst && rows ? cudaMemcpy2D(dst, cols * d, src, ld * d, cols * d, rows, cudaMemcpyDeviceToHost) : cudaSuccess;
+    };
+    if (out->pair_ro && P) ICG_CUDA(cudaMemcpy(out->pair_ro, D.pair_ro + w * PM, sizeof(int) * P, cudaMemcpyDeviceToHost));
+    ICG_CUDA(get(out->Mp, D.Mp[b] + w * PM * 210, (size_t) P * 210));
+    ICG_CUDA(get2d(out->A_W, D.AW[b] + (size_t) w * C.LP * C.NCA, L, NCV + 1, C.NCA));
+    ICG_CUDA(get(out->h_l, D.hl[b] + (size_t) w * C.L, L));
+    ICG_CUDA(get(out->g_l, D.gl[b] + (size_t) w * C.L, L));
+    ICG_CUDA(get(out->scale_l, D.scale_l + (size_t) w * C.L, L));
+    ICG_CUDA(get2d(out->H_c, D.Hc[b] + (size_t) w * C.NS * C.NS, N, N, C.NS));
+    ICG_CUDA(get(out->g_c, D.gc[b] + (size_t) w * C.NS, N));
+    ICG_CUDA(get(out->costf, D.costf[b] + (size_t) w * C.F, dm.F));
+    ICG_CUDA(get2d(out->Hs, D.Hs + (size_t) w * C.NS * C.NS, NCV, NCV, C.NS));
+    ICG_CUDA(get(out->visv, D.visv + (size_t) w * 3 * C.NCV, 3 * NCV));
+    if (out->Hs)
+        for (size_t i = 0; i < NCV; i++)
+            for (size_t j = i + 1; j < NCV; j++) out->Hs[i * NCV + j] = 0.0;
     return ICG_OK;
 }
 

@@ -67,6 +67,9 @@ struct icg_ba {
     size_t smem_cam, smem_solve, smem_schur;
     int ld_schur;
     int use_global_S;
+    // the linearisation buffers hold the system of the windows the handle holds, as the last single-GPU LM sequence left it: set when
+    // icg_ba_run / icg_ba_run_gvins enqueue one, cleared by every call that changes the windows after it (icg_ba_peek_linearization reads it)
+    bool lin_ready = false;
     HostDev<icg::WinDims> dims;
     HostDev<icg::LmState> st;
     HostDev<double> pose, mix, ext, rho, imu_blob, imu_U, gnss_blh, gnss_std, lever, pose_prior, pose_prior_sinfo, mix_prior, mix_prior_std, marg_x0,

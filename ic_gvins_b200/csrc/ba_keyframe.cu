@@ -109,6 +109,7 @@ static int marginalize_body(icg_ba *h, int n_windows, const icg_ba_problem *prob
     }
     int rc = ICG_OK;
     h->marg_res_n = 0;  // the workspace is about to be overwritten: it is the resident prior again only if this call is resident and succeeds
+    h->lin_ready = false;  // its linearisation takes the buffer the window uses
     if (resident) {
         // the windows of the last upload / solve are still on the device (parameters at their optimised values, factor activity and GNSS
         // weights as the two-pass solve left them): `problems` is read for the structure and for x0 only
@@ -655,6 +656,7 @@ static int reint_body(icg_ba *h, int n_windows, const icg_ba_problem *problems, 
     for (int k = 0; k < 3; k++) a.station[k] = station3[k];
     a.status = (int8_t *) (Dv + o_status), a.ends = (double *) (Dv + o_ends), a.out_blob = (double *) (Dv + o_blob), a.out_item = (int *) (Dv + o_item);
     a.counter = (int *) (Dv + o_cnt);
+    h->lin_ready = false;  // the reintegrated factors are not those of the last linearisation
     ICG_CUDA(preint_resident_launch(a, s));
     count_launch();
     ICG_CUDA(cudaMemcpyAsync(H + o_cnt, Dv + o_cnt, o_blob - o_cnt, cudaMemcpyDeviceToHost, s));
@@ -1538,6 +1540,7 @@ static int cull_run(icg_ba *h, int n, const icg_ba_problem *problems, const icg_
                  o_lmo = lay.take(nL), o_obso = lay.take(nO);
     const size_t out_bytes = lay.size() - in_bytes;
     h->cull_res_n = 0;  // the staging is rewritten (or replaced) from here
+    h->lin_ready = false;  // parameters and factor activity change
     ICG_CUDA(cudaSetDevice(h->device));
     cudaStream_t s = h->stream;
     if (lay.size() > h->cull.n) ICG_CUDA(cudaStreamSynchronize(s));

@@ -1083,6 +1083,33 @@ int icg_ba_reintegrate_stored_resident(icg_ba *h, int n_windows, const icg_ba_pr
  * (cap_rows x 7).  Synchronous. */
 int icg_ba_imu_samples(icg_ba *h, int window, int cap_rows, int32_t *off, double *rows);
 
+/*
+ * Read-out of one window's system for tests: what the linearisation kernels and the Schur kernel left in the linearisation buffer the
+ * window uses now (LmState::lin_buf), copied to the host in the window's own sizes (K, L, F of the upload; NCV = 6K + 7, N = 15K + 7, columns
+ * [pose 6K | extrinsic 6 | td 1 | mix 9K]).  After icg_ba_run(h, 0, 1) this is the system at the uploaded parameters: one linearisation and one
+ * Schur complement.  Synchronises the handle's streams; changes nothing on the device.  Every array pointer may be NULL (not copied).
+ * ICG_EINVAL when no icg_ba_run / icg_ba_run_gvins has run since the windows were uploaded, slid, reintegrated, culled or marginalized (the
+ * buffers would not hold their system).  ICG_EUNSUPPORTED on a handle the split pipeline drives (max_K >= 15 or a landmark-shard group), whose
+ * reduced system is not kept in Hs.
+ */
+typedef struct icg_ba_linearization {
+    int32_t K, L, F;   /* out: the window's sizes (arrays at the handle's capacities always suffice) */
+    int32_t n_pairs;   /* out: (reference node, observing node) pairs of the window */
+    int32_t lin_buf;   /* out: the linearisation buffer read */
+    double radius;     /* out: the trust-region radius the Schur complement was formed at */
+    int32_t *pair_ro;  /* [K (K - 1)]: pair p = (reference node << 8 | observing node), pairs ordered by (reference, observing) */
+    double *Mp;        /* [K (K - 1)][210]: pair p's Gram matrix of [J_ref pose 6 | J_obs pose 6 | J_ext 6 | J_td | r], packed upper, row-major */
+    double *A_W;       /* [L][NCV + 1]: by landmark id, w_l = sum_f J_f^T j_rho,f over the NCV vision columns, then g_l */
+    double *h_l, *g_l; /* [L]: sum_f j_rho,f^T j_rho,f and sum_f j_rho,f^T r_f */
+    double *H_c;       /* [N][N]: the camera-only factors' J^T J (full) */
+    double *g_c;       /* [N]: their J^T r */
+    double *costf;     /* [F]: per reprojection factor (by factor id) the cost with its loss, 0 for an inactive factor */
+    double *scale_l;   /* [L]: the landmark's Jacobi scaling 1 / (1 + sqrt(h_l)) of the solve's first linearisation */
+    double *Hs;        /* [NCV][NCV]: H_c + H_vis - sum_l phi_l w_l w_l^T, lower triangle (entries above the diagonal set to 0) */
+    double *visv;      /* [3 NCV]: diag H_vis | g_vis | sum_l phi_l w_l g_l */
+} icg_ba_linearization;
+int icg_ba_peek_linearization(icg_ba *h, int window, icg_ba_linearization *out);
+
 #ifdef __cplusplus
 }
 #endif
