@@ -138,6 +138,7 @@ def _declare_r2(L: C.CDLL) -> None:
     L.icg_ba_update_and_cull_resident.argtypes = [vp, C.c_int, vp, vp, C.c_double, vp]
     L.icg_ba_marginalize_resident_culled.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp]
     L.icg_ba_update_and_cull_built.argtypes = [vp, C.c_int, vp, vp, C.c_double, vp, vp]
+    L.icg_ba_shard_update_and_cull_built.argtypes = [vp, C.c_int, vp, vp, C.c_double, vp, vp]
     L.icg_ba_reintegrate_resident.argtypes = [vp, C.c_int, vp, vp, vp, vp]
     L.icg_ba_slide_resident.argtypes = [vp, C.c_int, vp, vp]
     L.icg_ba_slide_integrate_resident.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp]
@@ -249,5 +250,5 @@ EXPORTS = [
     "icg_ba_sync", "icg_ba_shard_export", "icg_ba_shard_connect", "icg_ba_shard_error", "icg_ba_shard_leave", "icg_ba_gvins_optimization", "icg_ba_run_gvins", "icg_ba_gvins_optimization_begin", "icg_ba_gvins_optimization_end", "icg_ba_residual_costs", "icg_ba_reproj_evaluate", "icg_ba_reproj_evaluate_frames", "icg_ba_imu_evaluate", "icg_ba_marginalize", "icg_ba_marginalize_resident", "icg_ba_update_and_cull_resident", "icg_ba_marginalize_resident_culled", "icg_ba_reintegrate_resident", "icg_ba_slide_resident", "icg_ba_slide_integrate_resident", "icg_ba_slide_vision_resident", "icg_ba_shard_reintegrate_resident", "icg_ba_shard_slide_resident", "icg_ba_shard_slide_integrate_resident", "icg_ba_shard_slide_vision_resident", "icg_ba_gnss_evaluate", "icg_ba_pose_prior_evaluate", "icg_ba_mix_prior_evaluate", "icg_ba_imu_error_evaluate", "icg_ba_marg_factor_evaluate",
     "icg_ins_create", "icg_ins_destroy", "icg_ins_push", "icg_ins_redo", "icg_ins_gins_initialize", "icg_ins_camera_pose", "icg_ins_window", "icg_ins_sync",
     "icg_ba_imu_samples_from_ins", "icg_ba_slide_ins_resident", "icg_ba_reintegrate_stored_resident", "icg_ba_imu_samples",
-    "icg_ba_update_and_cull_built", "icg_ba_peek_linearization",
+    "icg_ba_update_and_cull_built", "icg_ba_shard_update_and_cull_built", "icg_ba_peek_linearization",
 ]

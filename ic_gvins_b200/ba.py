@@ -485,6 +485,20 @@ class WindowSolver:
         update_and_cull()'s dicts with the list keys the culling walked filled in (lm_ref_node, lm_ref_kp, obs_off, obs_node, obs_kp,
         obs_factor, and n_obs), so that marginalize(culled=...) takes them unchanged; slide_vision() may then omit obs_factor, and
         marginalize(culled=...) takes dicts without the four integer lists (the culling's own are used)."""
+        return self._cull_built("icg_ba_update_and_cull_built", problems, camera, std, ext_inputs)
+
+    def shard_update_and_cull_built(self, problems, camera, std, ext_inputs):
+        """update_and_cull_built() on a landmark-sharded handle (icg_ba_shard_update_and_cull_built), a collective call: every rank passes its
+        shard dicts and the same ext_inputs, and culls on the lists its last shard_slide_vision() built.  Returns the rank's dicts as the sharded
+        update_and_cull() does (landmark outputs over the shard, counts the window's totals) with the rank's shard-local lists, without
+        obs_factor: marginalize(culled=...) and shard_vision_inputs() / shard_slide_vision() take them unchanged, and each rank's own culling
+        supplies obs_factor.  A rejection on any rank raises IcgError on every rank, with every handle unchanged."""
+        outs = self._cull_built("icg_ba_shard_update_and_cull_built", problems, camera, std, ext_inputs)
+        for o in outs:
+            o.pop("obs_factor")
+        return outs
+
+    def _cull_built(self, fn, problems, camera, std, ext_inputs):
         from ._lib import CullLists
         if isinstance(problems, dict):
             problems, ext_inputs = [problems], [ext_inputs]
@@ -509,10 +523,10 @@ class WindowSolver:
                 setattr(cl[w], k, o[k].ctypes.data_as(ip))
             cl[w].lm_ref_kp, cl[w].obs_kp = o["lm_ref_kp"].ctypes.data_as(fp), o["obs_kp"].ctypes.data_as(fp)
         cam = camera.c if hasattr(camera, "c") else camera
-        rc = lib().icg_ba_update_and_cull_built(self._h, n, arr, C.byref(cam), float(std), cw, cl)
+        rc = getattr(lib(), fn)(self._h, n, arr, C.byref(cam), float(std), cw, cl)
         if rc != 0:
             from ._lib import IcgError
-            err = IcgError(f"icg_ba_update_and_cull_built failed with code {rc}: {lib().icg_last_error().decode('utf-8', 'replace')}")
+            err = IcgError(f"{fn} failed with code {rc}: {lib().icg_last_error().decode('utf-8', 'replace')}")
             err.code = rc
             raise err
         for o, s, c in zip(outs, cw, cl):

@@ -1040,7 +1040,7 @@ int icg_ba_shard_export(icg_ba *h, int rank, int world, uint8_t *blob) {
     }
     int rc = split_setup(h, rank, world);
     if (rc != ICG_OK) return rc;
-    h->lists_n = 0;  // built culling lists are a single-GPU handle's
+    h->lists_n = 0;  // joining a group ends the built culling lists
     ShardBlob b;
     memset(&b, 0, sizeof(b));
     b.magic = 0x49434753484152ull, b.pid = (uint64_t) getpid(), b.ptr = (uint64_t) (uintptr_t) h->xbuf, b.doubles = h->D.S.off_exp;

@@ -121,8 +121,9 @@ struct icg_ba {
     const float *cull_res_rkp = nullptr, *cull_res_kp = nullptr;
     const uint8_t *cull_res_lmo = nullptr, *cull_res_obso = nullptr;
     const int *cull_res_href = nullptr, *cull_res_hoff = nullptr, *cull_res_hnode = nullptr, *cull_res_hfac = nullptr;
-    // the next culling's lists, built by icg_ba_slide_vision_resident into lists[lists_cur ^ 1] and current from its commit until an upload,
-    // any other slide or a shard export (lists_n: their window count, 0: none).  Each buffer is [lm_ref_node | obs_off | obs_node | obs_factor |
+    // the next culling's lists, built by icg_ba_slide_vision_resident (sharded: icg_ba_shard_slide_vision_resident, the rank's next shard's)
+    // into lists[lists_cur ^ 1] and current from its commit until an upload, any other slide or a shard export (lists_n: their window count,
+    // 0: none).  Each buffer is [lm_ref_node | obs_off | obs_node | obs_factor |
     // lm_ref_kp | obs_kp] at lists_at; window w's slices are lists_win[w] (lm0, off0, obs0, K, L) with lists_nobs[w] entries, the arrays sized
     // by the slide's bounds (lists_nL landmarks, lists_nO observations)
     struct ListAt {

@@ -1172,7 +1172,8 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
 // sharded (icg_ba_shard_slide_vision_resident, a collective call): each rank builds its next shard from its own old shard, its own culling and
 // its shard-local obs_lm; new map point j of window w is built on rank (j + w) mod world only.  The vision arguments every rank must share and
 // the two counts the kernel read on the device seed slide_body's fingerprint, so the group still agrees once; a rank that rejects before
-// slide_body joins that agreement with its rejection, as slide_body's own checks do.
+// slide_body joins that agreement with its rejection, as slide_body's own checks do.  The kernel also writes the next culling's lists (the
+// rank's next shard's, sharded); they become current only when slide_body has committed.
 static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba_slide_window *carry, const icg_ba_slide_integrate *integ,
                        const double *noise5, const double *station3, icg_ba_slide_vision *vis, const char *fn, bool sharded,
                        const FactorRows *fr = nullptr) {
@@ -1236,7 +1237,7 @@ static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_b
         W.lm_out = (int) n_lm, W.f_out = (int) n_f, W.nf_out = (int) n_nf, W.scr = (int) n_scr, W.lst_obs = (int) n_lo;
         n_lm += (size_t) od.L + v.n_new, n_f += (size_t) od.F + v.n_obs + v.n_new, n_nf += (size_t) v.n_obs + v.n_new;
         n_scr += (size_t) od.F + 3 * (size_t) od.L + 5 * ((size_t) od.L + v.n_new) + v.n_new;  // ba_vision_build's scratch
-        if (!sharded) n_scr += (size_t) od.F + od.L + v.n_new, n_lo += (size_t) nco + v.n_obs + 2 * (size_t) v.n_new;  // and the lists'
+        n_scr += (size_t) od.F + od.L + v.n_new, n_lo += (size_t) nco + v.n_obs + 2 * (size_t) v.n_new;  // and the lists'
         if (n_ofac >= INT32_MAX / 2 || n_f >= INT32_MAX / 16 || n_scr >= INT32_MAX / 2 || n_lo >= INT32_MAX / 4) {
             set_error("%s: too many rows in one call", fn);
             return reject(ICG_EINVAL);
@@ -1253,10 +1254,10 @@ static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_b
     if (lay.size() > h->vis.n)
         if (cudaError_t e = cudaStreamSynchronize(s)) return cuda_fail(e, "cudaStreamSynchronize");
     if ((rc = hd_reserve(h, h->vis, lay.size(), fn)) != ICG_OK) return reject(rc);
-    // one GPU: the next culling's lists go to the buffer that is not current
+    // the next culling's lists (sharded: the rank's next shard's) go to the buffer that is not current
     const int nb = h->lists_cur ^ 1;
     icg_ba::ListAt at{};
-    if (!sharded) {
+    {
         Layout ll;
         at.ref = ll.take(4 * n_lm), at.off = ll.take(4 * (n_lm + n)), at.node = ll.take(4 * n_lo), at.fac = ll.take(4 * n_lo);
         at.rkp = ll.take(8 * n_lm), at.kp = ll.take(8 * n_lo), at.end = ll.size();
@@ -1277,9 +1278,9 @@ static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_b
     a.counts = (int *) (Dv + b_cnt), a.lm_src = (int *) (Dv + b_lms), a.lm_org = (int *) (Dv + b_org), a.lm_nan = Dv + b_nan, a.f_lm = (int *) (Dv + b_flm), a.f_ref = (int *) (Dv + b_fref);
     a.f_obs = (int *) (Dv + b_fobs), a.f_src = (int *) (Dv + b_fsrc), a.invdepth = (double *) (Dv + b_invd), a.f_new = (double *) (Dv + b_fnew);
     a.scratch = (int *) (Dv + b_scr);
-    unsigned char *Dl = sharded ? nullptr : h->lists[nb].d;
-    a.l_ref = Dl ? (int *) (Dl + at.ref) : nullptr, a.l_off = Dl ? (int *) (Dl + at.off) : nullptr, a.l_node = Dl ? (int *) (Dl + at.node) : nullptr;
-    a.l_fac = Dl ? (int *) (Dl + at.fac) : nullptr, a.l_rkp = Dl ? (float *) (Dl + at.rkp) : nullptr, a.l_kp = Dl ? (float *) (Dl + at.kp) : nullptr;
+    unsigned char *Dl = h->lists[nb].d;
+    a.l_ref = (int *) (Dl + at.ref), a.l_off = (int *) (Dl + at.off), a.l_node = (int *) (Dl + at.node), a.l_fac = (int *) (Dl + at.fac);
+    a.l_rkp = (float *) (Dl + at.rkp), a.l_kp = (float *) (Dl + at.kp);
     cudaError_t e = cudaMemcpyAsync(Dv, H, in_end, cudaMemcpyHostToDevice, s);
     if (e == cudaSuccess) e = cudaMemsetAsync(Dv + b_cnt, 0, 4 * VIS_COUNTS * (size_t) n, s);
     if (e == cudaSuccess && (e = launch_vision(a, n, s)) == cudaSuccess) count_launch();
@@ -1339,7 +1340,7 @@ static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_b
         lw[w].K = next[w].K, lw[w].L = c[0], lw[w].lm0 = wins[w].lm_out, lw[w].off0 = wins[w].lm_out + w, lw[w].obs0 = wins[w].lst_obs, lnobs[w] = c[8];
     }
     rc = slide_body(h, n, nx.data(), cr.data(), integ, noise5, station3, fn, sharded, true, sharded ? &fp : nullptr, fr);
-    if (rc != ICG_OK || sharded) return rc;
+    if (rc != ICG_OK) return rc;  // sharded: the group's agreement inside slide_body has committed every rank's slide, or none
     h->lists_cur = nb, h->lists_at[nb] = at, h->lists_n = n, h->lists_nL = n_lm, h->lists_nO = n_lo;
     h->lists_win = std::move(lw), h->lists_nobs = std::move(lnobs);
     return ICG_OK;
@@ -1604,6 +1605,88 @@ static int cull_run(icg_ba *h, int n, const icg_ba_problem *problems, const icg_
     return ICG_OK;
 }
 
+// ---- the culling on the lists the last vision slide built (icg_ba_update_and_cull_built and its collective form).  sharded
+//      (icg_ba_shard_update_and_cull_built): each rank's lists are its shard's; every rank runs the checks of the plain call, then the group
+//      agrees once (every rank's verdict and a fingerprint of what every rank must pass alike) before cull_run writes anything or exchanges
+//      its counters, so that a rejection on any rank leaves every handle as it was, the last culling included.
+static int cull_built_body(icg_ba *h, int n, const icg_ba_problem *problems, const icg_camera *cam, double reprojection_error_std,
+                           icg_ba_cull_window *io, icg_ba_cull_lists *lists, const char *fn, bool sharded) {
+    auto reject = [&](int code) { return sharded ? shard_agree(h, true, 0, fn) : code; };
+    // lists_n is 0 or the uploaded count, so a call over another window count fails here already
+    int rc = resident_single_rank(h, n, problems, fn, sharded);
+    if (rc != ICG_OK) return reject(rc);
+    if (!cam || !io) {
+        set_error("%s: bad arguments", fn);
+        return reject(ICG_EINVAL);
+    }
+    if (h->lists_n != n) {
+        set_error("%s: no built lists of these %d windows are current (%s, with no upload or other slide since)", fn, n,
+                  sharded ? "icg_ba_shard_slide_vision_resident" : "icg_ba_slide_vision_resident");
+        return reject(ICG_EINVAL);
+    }
+    const BaCaps &C = h->C;
+    std::vector<CullWin> win(n);
+    size_t nK = 0;
+    ArgPrint fp;  // sharded: the camera side, which every rank must pass alike
+    fp.num(n), fp.arr(cam, 1), fp.arr(&reprojection_error_std, 1);
+    for (int w = 0; w < n; w++) {
+        const icg_ba_problem &p = problems[w];
+        const icg_ba_cull_window &c = io[w];
+        const CullWin &lw = h->lists_win[w];
+        const int no = h->lists_nobs[w];
+        // the caller's observation arrays hold max_L + max_F entries: lists not shaped as the reference builds them (an entry listed twice
+        // in the host lists the slide carried) can be longer
+        if (no > C.L + C.F) {
+            set_error("%s: window %d: the built lists hold %d observations, more than max_L + max_F = %d", fn, w, no, C.L + C.F);
+            return reject(ICG_EINVAL);
+        }
+        if (p.K != lw.K || p.L != lw.L || p.K > C.K || !c.cam_pose || (p.L > 0 && (!c.lm_pw || !c.lm_depth || !c.lm_outlier)) || (no > 0 && !c.obs_outlier)) {
+            set_error("%s: window %d: sizes differ from the built lists' (K %d, L %d) or arrays missing", fn, w, lw.K, lw.L);
+            return reject(ICG_EINVAL);
+        }
+        if (c.lm_ref_node || c.lm_ref_kp || c.obs_off || c.obs_node || c.obs_kp || c.obs_factor) {
+            set_error("%s: window %d: the lists are the built ones; their inputs must be NULL", fn, w);
+            return reject(ICG_EINVAL);
+        }
+        CullWin &W = win[w];
+        memcpy(W.R_bc, c.R_bc, sizeof(W.R_bc)), memcpy(W.t_bc, c.t_bc, sizeof(W.t_bc));
+        W.td_bc = c.td_bc, W.K = p.K, W.L = p.L, W.estimate_ext = c.estimate_ext != 0, W.estimate_td = c.estimate_td != 0;
+        W.lm0 = lw.lm0, W.off0 = lw.off0, W.obs0 = lw.obs0, W.node0 = (int) nK;
+        nK += p.K;
+        fp.num(p.K), fp.arr(c.R_bc, 9), fp.arr(c.t_bc, 3), fp.arr(&c.td_bc, 1), fp.num(W.estimate_ext), fp.num(W.estimate_td);
+    }
+    if (sharded && (rc = shard_agree(h, false, fp.get(), fn)) != ICG_OK) return rc;
+    bool want_kp = false;
+    for (int w = 0; lists && w < n; w++) want_kp = want_kp || lists[w].lm_ref_kp || lists[w].obs_kp;
+    HostDev<unsigned char> &lb = h->lists[h->lists_cur];
+    const icg_ba::ListAt &at = h->lists_at[h->lists_cur];
+    const CullSrc src{(const int *) (lb.d + at.ref), (const int *) (lb.d + at.off), (const int *) (lb.d + at.node), (const int *) (lb.d + at.fac),
+                      (const float *) (lb.d + at.rkp), (const float *) (lb.d + at.kp)};
+    rc = cull_run(h, n, problems, cam, reprojection_error_std, io, win, h->lists_nobs, h->lists_nL, h->lists_nO, nK, &src, fn);
+    if (rc != ICG_OK) return rc;
+    // the integer lists on the host (icg_ba_marginalize_resident_culled's NULL lists read them there) and, when asked for, the keypoints
+    h->cull_res_n = 0;
+    ICG_CUDA(cudaMemcpyAsync(lb.h, lb.d, at.rkp, cudaMemcpyDeviceToHost, h->stream));
+    if (want_kp) ICG_CUDA(cudaMemcpyAsync(lb.h + at.rkp, lb.d + at.rkp, at.end - at.rkp, cudaMemcpyDeviceToHost, h->stream));
+    ICG_CUDA(cudaStreamSynchronize(h->stream));
+    h->cull_res_n = n;
+    h->cull_res_href = (const int *) (lb.h + at.ref), h->cull_res_hoff = (const int *) (lb.h + at.off), h->cull_res_hnode = (const int *) (lb.h + at.node);
+    h->cull_res_hfac = (const int *) (lb.h + at.fac);
+    for (int w = 0; lists && w < n; w++) {
+        const int L = problems[w].L, no = h->lists_nobs[w];
+        const CullWin &W = win[w];
+        icg_ba_cull_lists &o = lists[w];
+        o.n_obs = no;
+        if (o.lm_ref_node) memcpy(o.lm_ref_node, lb.h + at.ref + 4 * (size_t) W.lm0, 4 * (size_t) L);
+        if (o.obs_off) memcpy(o.obs_off, lb.h + at.off + 4 * (size_t) W.off0, 4 * ((size_t) L + 1));
+        if (o.obs_node) memcpy(o.obs_node, lb.h + at.node + 4 * (size_t) W.obs0, 4 * (size_t) no);
+        if (o.obs_factor) memcpy(o.obs_factor, lb.h + at.fac + 4 * (size_t) W.obs0, 4 * (size_t) no);
+        if (o.lm_ref_kp) memcpy(o.lm_ref_kp, lb.h + at.rkp + 8 * (size_t) W.lm0, 8 * (size_t) L);
+        if (o.obs_kp) memcpy(o.obs_kp, lb.h + at.kp + 8 * (size_t) W.obs0, 8 * (size_t) no);
+    }
+    return ICG_OK;
+}
+
 extern "C" {
 
 int icg_ba_marginalize(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg, icg_ba_prior *out) {
@@ -1667,80 +1750,18 @@ int icg_ba_update_and_cull_built(icg_ba *h, int n_windows, const icg_ba_problem 
                                  icg_ba_cull_window *io, icg_ba_cull_lists *lists) {
     static const char *fn = "icg_ba_update_and_cull_built";
     if (h && h->D.world > 1) {
-        set_error("%s: not available on a landmark-sharded handle (its lists would be shard-local)", fn);
+        set_error("%s: not available on a landmark-sharded handle (its group calls icg_ba_shard_update_and_cull_built)", fn);
         return ICG_EUNSUPPORTED;
     }
-    // lists_n is 0 or the uploaded count, so a call over another window count fails here already
-    int rc = resident_single_rank(h, n_windows, problems, fn);
-    if (rc != ICG_OK) return rc;
-    const int n = n_windows;
-    if (!cam || !io) {
-        set_error("%s: bad arguments", fn);
-        return ICG_EINVAL;
-    }
-    if (h->lists_n != n) {
-        set_error("%s: no built lists of these %d windows are current (icg_ba_slide_vision_resident, with no upload or other slide since)", fn, n);
-        return ICG_EINVAL;
-    }
-    const BaCaps &C = h->C;
-    std::vector<CullWin> win(n);
-    size_t nK = 0;
-    for (int w = 0; w < n; w++) {
-        const icg_ba_problem &p = problems[w];
-        const icg_ba_cull_window &c = io[w];
-        const CullWin &lw = h->lists_win[w];
-        const int no = h->lists_nobs[w];
-        // the caller's observation arrays hold max_L + max_F entries: lists not shaped as the reference builds them (an entry listed twice
-        // in the host lists the slide carried) can be longer
-        if (no > C.L + C.F) {
-            set_error("%s: window %d: the built lists hold %d observations, more than max_L + max_F = %d", fn, w, no, C.L + C.F);
-            return ICG_EINVAL;
-        }
-        if (p.K != lw.K || p.L != lw.L || p.K > C.K || !c.cam_pose || (p.L > 0 && (!c.lm_pw || !c.lm_depth || !c.lm_outlier)) || (no > 0 && !c.obs_outlier)) {
-            set_error("%s: window %d: sizes differ from the built lists' (K %d, L %d) or arrays missing", fn, w, lw.K, lw.L);
-            return ICG_EINVAL;
-        }
-        if (c.lm_ref_node || c.lm_ref_kp || c.obs_off || c.obs_node || c.obs_kp || c.obs_factor) {
-            set_error("%s: window %d: the lists are the built ones; their inputs must be NULL", fn, w);
-            return ICG_EINVAL;
-        }
-        CullWin &W = win[w];
-        memcpy(W.R_bc, c.R_bc, sizeof(W.R_bc)), memcpy(W.t_bc, c.t_bc, sizeof(W.t_bc));
-        W.td_bc = c.td_bc, W.K = p.K, W.L = p.L, W.estimate_ext = c.estimate_ext != 0, W.estimate_td = c.estimate_td != 0;
-        W.lm0 = lw.lm0, W.off0 = lw.off0, W.obs0 = lw.obs0, W.node0 = (int) nK;
-        nK += p.K;
-    }
-    bool want_kp = false;
-    for (int w = 0; lists && w < n; w++) want_kp = want_kp || lists[w].lm_ref_kp || lists[w].obs_kp;
-    HostDev<unsigned char> &lb = h->lists[h->lists_cur];
-    const icg_ba::ListAt &at = h->lists_at[h->lists_cur];
-    const CullSrc src{(const int *) (lb.d + at.ref), (const int *) (lb.d + at.off), (const int *) (lb.d + at.node), (const int *) (lb.d + at.fac),
-                      (const float *) (lb.d + at.rkp), (const float *) (lb.d + at.kp)};
-    rc = cull_run(h, n, problems, cam, reprojection_error_std, io, win, h->lists_nobs, h->lists_nL, h->lists_nO, nK, &src, fn);
-    if (rc != ICG_OK) return rc;
-    // the integer lists on the host (icg_ba_marginalize_resident_culled's NULL lists read them there) and, when asked for, the keypoints
-    h->cull_res_n = 0;
-    ICG_CUDA(cudaMemcpyAsync(lb.h, lb.d, at.rkp, cudaMemcpyDeviceToHost, h->stream));
-    if (want_kp) ICG_CUDA(cudaMemcpyAsync(lb.h + at.rkp, lb.d + at.rkp, at.end - at.rkp, cudaMemcpyDeviceToHost, h->stream));
-    ICG_CUDA(cudaStreamSynchronize(h->stream));
-    h->cull_res_n = n;
-    h->cull_res_href = (const int *) (lb.h + at.ref), h->cull_res_hoff = (const int *) (lb.h + at.off), h->cull_res_hnode = (const int *) (lb.h + at.node);
-    h->cull_res_hfac = (const int *) (lb.h + at.fac);
-    for (int w = 0; lists && w < n; w++) {
-        const int L = problems[w].L, no = h->lists_nobs[w];
-        const CullWin &W = win[w];
-        icg_ba_cull_lists &o = lists[w];
-        o.n_obs = no;
-        if (o.lm_ref_node) memcpy(o.lm_ref_node, lb.h + at.ref + 4 * (size_t) W.lm0, 4 * (size_t) L);
-        if (o.obs_off) memcpy(o.obs_off, lb.h + at.off + 4 * (size_t) W.off0, 4 * ((size_t) L + 1));
-        if (o.obs_node) memcpy(o.obs_node, lb.h + at.node + 4 * (size_t) W.obs0, 4 * (size_t) no);
-        if (o.obs_factor) memcpy(o.obs_factor, lb.h + at.fac + 4 * (size_t) W.obs0, 4 * (size_t) no);
-        if (o.lm_ref_kp) memcpy(o.lm_ref_kp, lb.h + at.rkp + 8 * (size_t) W.lm0, 8 * (size_t) L);
-        if (o.obs_kp) memcpy(o.obs_kp, lb.h + at.kp + 8 * (size_t) W.obs0, 8 * (size_t) no);
-    }
-    return ICG_OK;
+    return cull_built_body(h, n_windows, problems, cam, reprojection_error_std, io, lists, fn, false);
 }
 
+int icg_ba_shard_update_and_cull_built(icg_ba *h, int n_windows, const icg_ba_problem *problems, const icg_camera *cam, double reprojection_error_std,
+                                       icg_ba_cull_window *io, icg_ba_cull_lists *lists) {
+    const char *fn = "icg_ba_shard_update_and_cull_built";
+    const int rc = shard_group_only(h, fn, "icg_ba_update_and_cull_built");
+    return rc != ICG_OK ? rc : cull_built_body(h, n_windows, problems, cam, reprojection_error_std, io, lists, fn, true);
+}
 int icg_ba_reintegrate_resident(icg_ba *h, int n_windows, const icg_ba_problem *problems, const double *noise5, const double *station3,
                                 icg_ba_reint_window *io) {
     return reint_body(h, n_windows, problems, noise5, station3, io, "icg_ba_reintegrate_resident", false);

@@ -55,8 +55,10 @@ __device__ __forceinline__ void list_entry(int *node, int *fac, float *kp, int e
 // reference node is usable (in the map, not marginalized, kept by the slide) and 1 / (1 / rho) is not NaN; its old factors survive when their
 // observation is listed by the culling and not an outlier and their observing node is usable; its new observations follow in node order.  New map
 // points follow the carried landmarks in creation order, each with one factor from its reference node to the current node.  On a landmark shard
-// the old window is the rank's shard and only the rank's new points are kept; the numbering below is then the shard's.  On one GPU the kernel
-// then writes the next culling's lists (step 4, the list rule of icg_ba_update_and_cull_built).
+// the old window is the rank's shard and only the rank's new points are kept; the numbering below is then the shard's.  The kernel then writes
+// the next culling's lists (step 4, the list rule of icg_ba_update_and_cull_built).  The rule is local to each landmark, so on a shard step 4
+// needs nothing else: keep covers the rank's carried landmarks and its own new points, fmap maps its old shard factors to next shard rows,
+// and node indices are the replicated camera side's.
 __global__ void __launch_bounds__(VIS_THREADS) ba_vision_build(VisArgs a) {
     __shared__ Scan::TempStorage tmp;
     __shared__ int s_nobs, s_nnew;

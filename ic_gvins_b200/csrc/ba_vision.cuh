@@ -66,8 +66,9 @@ struct VisArgs {
     uint8_t *lm_nan;
     double *invdepth, *f_new, *lm_ref_next;
     int *scratch;
-    // the next culling's lists (NULL: not emitted; landmark shards never emit them).  Per window, in next-landmark order: l_ref / l_rkp at
-    // lm_out (Lb), l_off at lm_out + w (Lb + 1), l_node / l_fac / l_kp at lst_obs (Ob); keypoints 2 floats each
+    // the next culling's lists (NULL: not emitted); on a landmark shard the rank's next shard's, in its numbering.  Per window, in
+    // next-landmark order: l_ref / l_rkp at lm_out (Lb), l_off at lm_out + w (Lb + 1), l_node / l_fac / l_kp at lst_obs (Ob); keypoints 2
+    // floats each
     int *l_ref, *l_off, *l_node, *l_fac;
     float *l_rkp, *l_kp;
 };

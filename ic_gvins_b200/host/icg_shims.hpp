@@ -317,6 +317,13 @@ public:
                             icg_ba_cull_lists *lists = nullptr) {
         check(icg_ba_update_and_cull_built(h_, 1, &problem, &camera, reprojection_error_std, &io, lists), "icg_ba_update_and_cull_built");
     }
+    // updateAndCullBuilt on a landmark-sharded solver, a collective call of its group (icg_ba_shard_update_and_cull_built): every rank passes
+    // its shard problem and the same extrinsic inputs, and culls on the lists its last sharded slideVision built; the outputs are
+    // updateAndCull's on a shard, `lists` the rank's shard-local lists.  A rejection on any rank throws on every rank, no solver changed.
+    void shardUpdateAndCullBuilt(const icg_ba_problem &problem, const icg_camera &camera, double reprojection_error_std, icg_ba_cull_window &io,
+                                 icg_ba_cull_lists *lists = nullptr) {
+        check(icg_ba_shard_update_and_cull_built(h_, 1, &problem, &camera, reprojection_error_std, &io, lists), "icg_ba_shard_update_and_cull_built");
+    }
 
     // GVINS::doReintegration (IG/ic_gvins.cc:1680-1695) on the window this solver just optimised, as gvinsOptimization calls it while the
     // window is not full (:1223-1227).  imu = the rows (dt, dtheta[3], dvel[3]) of every factor's imu_buffer_, imu_off = n_imu + 1 offsets

@@ -592,7 +592,7 @@ int icg_ba_update_and_cull_resident(icg_ba *h, int n_windows, const icg_ba_probl
  * node_in_map[w][f_obs[f]] is set (the keyframes gvinsRemoveAllSecondNewFrame left in the map, IG/ic_gvins.cc:1391-1410): the factor set
  * gvinsMarginalization builds (:1558-1609).  The chi-square activity plays no part (removeReprojectionFactorsByChi2 never marks a feature).
  * culled: the io array of icg_ba_update_and_cull_resident after that call (obs_factor must be set); node_in_map: K bytes per window.  After
- * icg_ba_update_and_cull_built, culled's lm_ref_node, obs_off, obs_node and obs_factor may be NULL: each NULL one is that culling's own list
+ * icg_ba_update_and_cull_built (on a shard group icg_ba_shard_update_and_cull_built), culled's lm_ref_node, obs_off, obs_node and obs_factor may be NULL: each NULL one is that culling's own list
  * (the handle keeps a host copy; ICG_EINVAL when no built culling of these windows is current).  The
  * handle's factor activity is not changed.  On a landmark-sharded handle: collective, as icg_ba_marginalize_resident; each rank passes its
  * own `culled` array (its shard's landmarks, obs_factor naming its shard's factors) and the same node_in_map. */
@@ -623,7 +623,7 @@ int icg_ba_marginalize_resident_culled(icg_ba *h, int n_windows, const icg_ba_pr
  * ICG_EINVAL, with the handle unchanged: no built lists of these n_windows are current, problems[w].K / L differ from the built window's, or
  * a window's built lists hold more than max_L + max_F observations (possible only when the host lists they grew from were not shaped as the
  * reference builds them, e.g. an entry listed twice).
- * ICG_EUNSUPPORTED on a landmark-sharded handle.  Synchronous.
+ * ICG_EUNSUPPORTED on a landmark-sharded handle: its group calls icg_ba_shard_update_and_cull_built.  Synchronous.
  */
 typedef struct icg_ba_cull_lists { /* out, HOST, each may be NULL: the lists the culling walked, in its order */
     int32_t n_obs;                 /* L + F for lists shaped as the reference builds them */
@@ -632,6 +632,29 @@ typedef struct icg_ba_cull_lists { /* out, HOST, each may be NULL: the lists the
 } icg_ba_cull_lists;
 int icg_ba_update_and_cull_built(icg_ba *h, int n_windows, const icg_ba_problem *problems, const icg_camera *cam, double reprojection_error_std,
                                  icg_ba_cull_window *io, icg_ba_cull_lists *lists);
+/*
+ * icg_ba_update_and_cull_built on a landmark-sharded handle (world > 1), with the same arguments: the culling on the lists the group's last
+ * icg_ba_shard_slide_vision_resident built on each rank, so that a sharded host neither walks mappoint->observations() nor cuts and uploads
+ * the lists.  A COLLECTIVE call.
+ *   Lists.  Each rank's built lists are its next shard's, in shard numbering: the list rule above applied to the rank's carried landmarks (the
+ *     entries of its own last culling's lists) and to its own new map points (new point j of window w on rank (j + w) mod world), factors
+ *     the shard's rows, nodes the replicated camera side's.  Written rank-major with the factors mapped to the whole window's, they are the
+ *     lists icg_ba_update_and_cull_built would walk on the merged window.  They are current, and end, under the plain call's rules; a shard
+ *     export ends them.
+ *   What each rank passes.  Its shard problems, and per window the extrinsic inputs (R_bc, t_bc, td_bc, estimate_ext, estimate_td) with the
+ *     list inputs NULL.  n_windows, cam, reprojection_error_std, and per window K and the extrinsic inputs must be the same on every rank.
+ *   Agreement first.  Each rank runs every check of the plain call, then joins one integer exchange of the group: its verdict and a 31-bit
+ *     fingerprint of the arguments above.  When any rank rejected, or the fingerprints differ, EVERY rank returns ICG_EINVAL with its handle as
+ *     it was (the last culling stays current); nothing has been written and no counter exchanged.
+ *   Outputs, per rank, as the sharded icg_ba_update_and_cull_resident gives them: cam_pose, the extrinsic outputs and td_bc_out the same on
+ *     every rank; lm_pw, lm_depth, lm_outlier and obs_outlier over the rank's shard (obs_outlier indexed by its built list); counts the
+ *     window's totals.  lists: the rank's shard-local lists.
+ *   Afterwards, on the group, icg_ba_marginalize_resident_culled takes NULL lists and icg_ba_shard_slide_vision_resident a NULL obs_factor,
+ *     each rank's being its own culling's.
+ * On a handle outside a shard group (world == 1): ICG_EINVAL naming icg_ba_update_and_cull_built.  Synchronous.
+ */
+int icg_ba_shard_update_and_cull_built(icg_ba *h, int n_windows, const icg_ba_problem *problems, const icg_camera *cam, double reprojection_error_std,
+                                       icg_ba_cull_window *io, icg_ba_cull_lists *lists);
 /*
  * GVINS::doReintegration (IG/ic_gvins.cc:1680-1695), which gvinsOptimization runs after the second Solve while the window is not full
  * (:1223-1227), on the IMU factors the handle holds.  For factor k of a window (joining nodes k and k + 1):
@@ -770,7 +793,7 @@ int icg_ba_slide_integrate_resident(icg_ba *h, int n_windows, const icg_ba_probl
  * the landmark (a landmark that carry.lm_src names keeps its old row; a new one takes its first factor's), and this call writes a new map
  * point's from its reference keypoint, velocity and node_td.  A new observation of a landmark whose row is unknown is ICG_EINVAL.
  * The reference's order is unordered_map iteration (implementation-defined); this order is fixed and only permutes rows.
- * On a single-GPU handle the same kernel writes the next culling's lists (icg_ba_update_and_cull_built).
+ * The same kernel writes the next culling's lists (icg_ba_update_and_cull_built; on a shard group icg_ba_shard_update_and_cull_built).
  * One CTA per window builds the structure on the device; the counts, the integer structure, the new invdepth rows and the new factors' constants
  * come back in one copy (one synchronisation), and the call goes on as icg_ba_slide_integrate_resident with that window, every check included.
  * A rejected call (ICG_EINVAL: max_L / max_F exceeded, a reference frame id missing from the table, a node, landmark or source index out of
@@ -783,7 +806,7 @@ typedef struct icg_ba_slide_vision {
     int32_t num_marg;
     const uint8_t *node_in_map;  /* old K: isKeyFrameInMap after gvinsRemoveAllSecondNewFrame */
     const int32_t *obs_factor;   /* the culling's observations (its obs_off order): factor of each, -1 for none; NULL after
-                                    icg_ba_update_and_cull_built: the built lists' */
+                                    icg_ba_update_and_cull_built or icg_ba_shard_update_and_cull_built: the built lists' */
     /* in: the new keyframes */
     icg_camera cam;
     const double *node_td;       /* next.K: frame->timeDelay() */
@@ -856,7 +879,8 @@ int icg_ba_shard_slide_integrate_resident(icg_ba *h, int n_windows, const icg_ba
  * device, from its own old shard and its own culling, then slides as icg_ba_shard_slide[_integrate]_resident (integ NULL or not), with every
  * rule above.  A COLLECTIVE call, with the structs of the plain call.
  *   What each rank passes.  Its own next shard problems and carry maps; next.L, F, f_* and carry.lm_src / f_src are built, not read.
- *     vis[w].obs_factor is the table the rank's own sharded culling took (shard_cull_inputs' obs_factor); vis[w].obs_lm names rows of the
+ *     vis[w].obs_factor is the table the rank's own sharded culling took (shard_cull_inputs' obs_factor), or NULL after
+ *     icg_ba_shard_update_and_cull_built (the rank's built lists'); vis[w].obs_lm names rows of the
  *     rank's own OLD shard, -1 for a map point the rank does not hold.  The lists are otherwise the same on every rank (the same tracked
  *     observations, the same new map points), and every device array must be readable from the rank's own device.
  *   Old landmarks.  A carried landmark stays on the rank that held it; each rank applies the plain call's rules to its shard: the carry rule,
