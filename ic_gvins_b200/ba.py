@@ -9,71 +9,35 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import check, lib, vp
+from ._lib import (BaPrior, BaProblem, BaSummary, CullLists, CullWindow, InsCut, Linearization, ReintWindow, SlideIns, SlideIntegrate, SlideVision,
+                   SlideWindow, check, f32p, f64p, i8p, i32p, i64p, lib, u8p, vp)
+from .camera import CameraStruct
 
 IMU_BLOB = 480
-dp = C.POINTER(C.c_double)
-ip = C.POINTER(C.c_int32)
-bp = C.POINTER(C.c_uint8)
+
+_CULL_IN = dict(lm_ref_node=(np.int32, i32p), lm_ref_kp=(np.float32, f32p), obs_off=(np.int32, i32p), obs_node=(np.int32, i32p),
+                obs_kp=(np.float32, f32p), obs_factor=(np.int32, i32p))
 
 
-class BaProblem(C.Structure):
-    """ctypes image of `icg_ba_problem` (include/icgvins_b200.h)."""
-    _fields_ = [
-        ("K", C.c_int32), ("L", C.c_int32), ("F", C.c_int32),
-        ("pose", dp), ("mix", dp), ("ext", dp), ("invdepth", dp),
-        ("ext_const", C.c_int32), ("td_const", C.c_int32),
-        ("f_lm", ip), ("f_ref", ip), ("f_obs", ip), ("f_const", dp), ("f_active", bp),
-        ("reproj_std", C.c_double), ("reproj_huber", C.c_int32),
-        ("n_imu", C.c_int32), ("imu_blob", dp), ("has_imu_error", C.c_int32),
-        ("has_pose_prior", C.c_int32), ("pose_prior", dp), ("pose_prior_std", dp),
-        ("has_mix_prior", C.c_int32), ("mix_prior", dp), ("mix_prior_std", dp),
-        ("n_gnss", C.c_int32), ("gnss_node", ip), ("gnss_blh", dp), ("gnss_std", dp), ("lever", C.c_double * 3),
-        ("gnss_huber", C.c_int32),
-        ("marg_r", C.c_int32), ("marg_nblocks", C.c_int32), ("marg_block_type", ip), ("marg_block_node", ip),
-        ("marg_x0", dp), ("marg_J0", dp), ("marg_e0", dp),
-    ]
+def _cull_ext(s: CullWindow, ci: dict) -> None:
+    """The extrinsic inputs of one icg_ba_cull_window from those of `ci` (R_bc, t_bc; td_bc, estimate_ext, estimate_td default 0, 1, 1)."""
+    for k in ("R_bc", "t_bc"):
+        getattr(s, k)[:] = [float(x) for x in np.asarray(ci[k], np.float64).reshape(-1)]
+    s.td_bc, s.estimate_ext, s.estimate_td = float(ci.get("td_bc", 0.0)), int(ci.get("estimate_ext", 1)), int(ci.get("estimate_td", 1))
 
 
-class BaPrior(C.Structure):
-    """ctypes image of `icg_ba_prior`."""
-    _fields_ = [("m", C.c_int32), ("r", C.c_int32), ("nblocks", C.c_int32), ("rcap", C.c_int32), ("block_type", ip), ("block_node", ip),
-                ("x0", dp), ("J0", dp), ("e0", dp), ("Hp", dp), ("bp", dp)]
-
-
-class BaSummary(C.Structure):
-    _fields_ = [("iterations", C.c_int32), ("num_successful_steps", C.c_int32), ("termination", C.c_int32), ("reserved", C.c_int32),
-                ("initial_cost", C.c_double), ("final_cost", C.c_double), ("final_radius", C.c_double)]
-
-
-fp = C.POINTER(C.c_float)
-
-
-class CullWindow(C.Structure):
-    """ctypes image of `icg_ba_cull_window`."""
-    _fields_ = [("R_bc", C.c_double * 9), ("t_bc", C.c_double * 3), ("td_bc", C.c_double), ("estimate_ext", C.c_int32), ("estimate_td", C.c_int32),
-                ("lm_ref_node", ip), ("lm_ref_kp", fp), ("obs_off", ip), ("obs_node", ip), ("obs_kp", fp), ("obs_factor", ip),
-                ("R_bc_out", C.c_double * 9), ("t_bc_out", C.c_double * 3), ("td_bc_out", C.c_double), ("ext_accepted", C.c_int32),
-                ("cam_pose", dp), ("lm_pw", dp), ("lm_depth", dp), ("lm_outlier", bp), ("obs_outlier", bp), ("counts", C.c_int32 * 5)]
-
-
-class ReintWindow(C.Structure):
-    """ctypes image of `icg_ba_reint_window`."""
-    _fields_ = [("reintegrate", C.c_int32), ("imu", dp), ("imu_off", ip), ("status", C.POINTER(C.c_int8)), ("blob_out", dp), ("end_state10", dp),
-                ("count", C.c_int32)]
-
-
-_CULL_IN = dict(lm_ref_node=(np.int32, ip), lm_ref_kp=(np.float32, fp), obs_off=(np.int32, ip), obs_node=(np.int32, ip), obs_kp=(np.float32, fp),
-                obs_factor=(np.int32, ip))
+def _cull_outputs(s: CullWindow, ci: dict, K: int, L: int, n_obs: int) -> None:
+    """Add the culling's output arrays to `ci` and point `s` at them."""
+    ci.update(cam_pose=np.zeros((K, 12)), lm_pw=np.zeros((L, 3)), lm_depth=np.zeros(L), lm_outlier=np.zeros(L, np.uint8), obs_outlier=np.zeros(n_obs, np.uint8))
+    s.cam_pose, s.lm_pw, s.lm_depth = (ci[k].ctypes.data_as(f64p) for k in ("cam_pose", "lm_pw", "lm_depth"))
+    s.lm_outlier, s.obs_outlier = ci["lm_outlier"].ctypes.data_as(u8p), ci["obs_outlier"].ctypes.data_as(u8p)
 
 
 def cull_struct(prob: dict, ci: dict) -> CullWindow:
     """The icg_ba_cull_window of one window over the arrays of `ci` (made contiguous in place; output arrays are added to it)."""
     s = CullWindow()
-    K, L = int(prob["K"]), int(prob["L"])
-    for k, v in zip(("R_bc", "t_bc"), (np.asarray(ci["R_bc"], np.float64).reshape(-1), np.asarray(ci["t_bc"], np.float64).reshape(-1))):
-        getattr(s, k)[:] = [float(x) for x in v]
-    s.td_bc, s.estimate_ext, s.estimate_td = float(ci.get("td_bc", 0.0)), int(ci.get("estimate_ext", 1)), int(ci.get("estimate_td", 1))
+    L = int(prob["L"])
+    _cull_ext(s, ci)
     for k, (dt, pt) in _CULL_IN.items():
         if ci.get(k) is None:
             continue
@@ -81,9 +45,7 @@ def cull_struct(prob: dict, ci: dict) -> CullWindow:
         ci[k] = a
         setattr(s, k, a.ctypes.data_as(pt) if a.size else pt())
     n_obs = int(ci["obs_off"][L]) if L > 0 and ci.get("obs_off") is not None else len(ci.get("obs_outlier", ()))
-    ci.update(cam_pose=np.zeros((K, 12)), lm_pw=np.zeros((L, 3)), lm_depth=np.zeros(L), lm_outlier=np.zeros(L, np.uint8), obs_outlier=np.zeros(n_obs, np.uint8))
-    s.cam_pose, s.lm_pw, s.lm_depth = (ci[k].ctypes.data_as(dp) for k in ("cam_pose", "lm_pw", "lm_depth"))
-    s.lm_outlier, s.obs_outlier = ci["lm_outlier"].ctypes.data_as(bp), ci["obs_outlier"].ctypes.data_as(bp)
+    _cull_outputs(s, ci, int(prob["K"]), L, n_obs)
     return s
 
 
@@ -91,6 +53,7 @@ _ARR = dict(pose=np.float64, mix=np.float64, ext=np.float64, invdepth=np.float64
             f_const=np.float64, f_active=np.uint8, imu_blob=np.float64, pose_prior=np.float64, pose_prior_std=np.float64,
             mix_prior=np.float64, mix_prior_std=np.float64, gnss_node=np.int32, gnss_blh=np.float64, gnss_std=np.float64,
             marg_block_type=np.int32, marg_block_node=np.int32, marg_x0=np.float64, marg_J0=np.float64, marg_e0=np.float64)
+_PTR = {np.float64: f64p, np.int32: i32p, np.uint8: u8p}
 _SCAL = ["K", "L", "F", "ext_const", "td_const", "reproj_std", "reproj_huber", "n_imu", "has_imu_error", "has_pose_prior",
          "has_mix_prior", "n_gnss", "gnss_huber", "marg_r", "marg_nblocks"]
 
@@ -102,7 +65,7 @@ def to_struct(prob: dict) -> BaProblem:
     for k, dt in _ARR.items():
         a = np.ascontiguousarray(prob[k], dtype=dt)
         prob[k] = a
-        ptr_t = dp if dt == np.float64 else ip if dt == np.int32 else bp
+        ptr_t = _PTR[dt]
         setattr(s, k, a.ctypes.data_as(ptr_t) if a.size else ptr_t())
     for k in _SCAL:
         setattr(s, k, prob[k])
@@ -265,30 +228,162 @@ def imu_preintegrate(state16, iewn, gravity, noise5, imu):
     return blob, end
 
 
-def _integ_struct(s, g, m, arg, with_rows=True):
+def _arg(keep: list, a, dtype, ptr):
+    """`a` as a contiguous `dtype` array, cast to `ptr`.  The array goes into `keep`, which the caller holds until the C call returns."""
+    a = np.ascontiguousarray(a, dtype)
+    keep.append(a)
+    return a.ctypes.data_as(ptr)
+
+
+def _problems(problems):
+    """The icg_ba_problem array over the problem dicts (to_struct: their arrays are made contiguous in place)."""
+    return (BaProblem * len(problems))(*[to_struct(p) for p in problems])
+
+
+def _summary(s: BaSummary) -> dict:
+    return dict(iterations=s.iterations, num_successful_steps=s.num_successful_steps, termination=s.termination,
+                initial_cost=s.initial_cost, final_cost=s.final_cost, final_radius=s.final_radius)
+
+
+def _two_pass(summ, culled, n: int) -> list:
+    """One gvinsOptimization result per window from the two summaries and two counts per window of icg_ba_gvins_optimization[_end]."""
+    return [dict(pass1=_summary(summ[2 * w]), pass2=_summary(summ[2 * w + 1]), reproj_removed=culled[2 * w], gnss_reweighted=culled[2 * w + 1])
+            for w in range(n)]
+
+
+def _flags(flag, n: int) -> list:
+    """Per-window 0 / 1 flags from one flag for all n windows or one per window."""
+    return [1 if f else 0 for f in ([flag] * n if np.isscalar(flag) else flag)]
+
+
+def _cam(camera) -> CameraStruct:
+    """The icg_camera of a camera.Camera or CameraStruct."""
+    return camera.c if hasattr(camera, "c") else camera
+
+
+_CARRY = ("node_src", "lm_src", "f_src", "imu_src", "gnss_src")
+_VISION_CARRY = ("node_src", "imu_src", "gnss_src")  # a vision slide builds lm_src / f_src itself
+
+
+def _slide_carry(carry, n: int, prior_from_marg, keep: list, keys=_CARRY):
+    """The icg_ba_slide_window array of n windows from their carry dicts: the maps of `keys` a dict holds (a missing or None map carries
+    nothing of its kind) and the prior_from_marg flag (one, or one per window)."""
+    cw = (SlideWindow * n)()
+    for w, (c, f) in enumerate(zip(carry, _flags(prior_from_marg, n))):
+        for k in keys:
+            if c.get(k) is not None:
+                setattr(cw[w], k, _arg(keep, c[k], np.int32, i32p))
+        cw[w].prior_from_marg = f
+    return cw
+
+
+def _noise_station(noise5, station, keep: list):
+    """The noise5 and station3 pointers of a reintegration or an integrating slide (noise5 None: zeros)."""
+    return _arg(keep, np.zeros(5) if noise5 is None else noise5, np.float64, vp), _arg(keep, station, np.float64, vp)
+
+
+def _imu_rows(rows, m: int):
+    """The rows (n x 7) and offsets (m + 1) of m factors from one (k, 7) row array per factor, None for a factor without rows."""
+    rows = [np.zeros((0, 7)) if r is None else np.asarray(r, np.float64).reshape(-1, 7) for r in rows]
+    off = np.zeros(m + 1, np.int32)
+    off[1:] = np.cumsum([len(r) for r in rows])
+    return (np.concatenate(rows, axis=0) if rows else np.zeros((0, 7))), off
+
+
+def _point_outputs(s, o: dict) -> None:
+    """Point an icg_ba_slide_integrate or icg_ba_reint_window at the status, blobs and end_states arrays of `o`."""
+    s.status, s.blob_out, s.end_state10 = o["status"].ctypes.data_as(i8p), o["blobs"].ctypes.data_as(f64p), o["end_states"].ctypes.data_as(f64p)
+
+
+def _integ_struct(s, g, m, keep, with_rows=True):
     """fill one icg_ba_slide_integrate from an `integrate` dict of WindowSolver.slide_integrate (m = next n_imu; with_rows False: imu /
     imu_off stay NULL, the rows come from the device)"""
-    from ._lib import u8p
     if g.get("imu_from") is not None:
-        s.imu_from = arg(g["imu_from"], np.int32, ip)
+        s.imu_from = _arg(keep, g["imu_from"], np.int32, i32p)
         if not with_rows:
             pass
         elif "imu_off" in g:
-            s.imu, s.imu_off = arg(g["imu"], np.float64, dp), arg(g["imu_off"], np.int32, ip)
+            s.imu, s.imu_off = _arg(keep, g["imu"], np.float64, f64p), _arg(keep, g["imu_off"], np.int32, i32p)
         else:
-            rows = [np.zeros((0, 7)) if r is None else np.asarray(r, np.float64).reshape(-1, 7) for r in g["imu_rows"]]
-            off = np.zeros(m + 1, np.int32)
-            off[1:] = np.cumsum([len(r) for r in rows])
-            imu = np.concatenate(rows, axis=0) if rows else np.zeros((0, 7))
-            s.imu, s.imu_off = arg(imu, np.float64, dp), arg(off, np.int32, ip)
-        s.gravity3 = arg(np.broadcast_to(np.asarray(g["gravity"], np.float64), (m, 3)), np.float64, dp)
-        s.normal = arg(np.broadcast_to(np.asarray(g.get("normal", False), np.uint8), (m,)), np.uint8, u8p)
+            imu, off = _imu_rows(g["imu_rows"], m)
+            s.imu, s.imu_off = _arg(keep, imu, np.float64, f64p), _arg(keep, off, np.int32, i32p)
+        s.gravity3 = _arg(keep, np.broadcast_to(np.asarray(g["gravity"], np.float64), (m, 3)), np.float64, f64p)
+        s.normal = _arg(keep, np.broadcast_to(np.asarray(g.get("normal", False), np.uint8), (m,)), np.uint8, u8p)
         if g.get("state16") is not None:
-            s.state16 = arg(g["state16"], np.float64, dp)
+            s.state16 = _arg(keep, g["state16"], np.float64, f64p)
     if g.get("node_from_imu") is not None:
-        s.node_from_imu = arg(g["node_from_imu"], np.uint8, u8p)
+        s.node_from_imu = _arg(keep, g["node_from_imu"], np.uint8, u8p)
     if g.get("gnss_node") is not None:
-        s.gnss_node, s.gnss_dt = arg(g["gnss_node"], np.int32, ip), arg(g["gnss_dt"], np.float64, dp)
+        s.gnss_node, s.gnss_dt = _arg(keep, g["gnss_node"], np.int32, i32p), _arg(keep, g["gnss_dt"], np.float64, f64p)
+
+
+def _integ_array(next_problems, integrate, keep: list):
+    """The icg_ba_slide_integrate array of the `integrate` dicts (a None entry integrates nothing in its window)."""
+    iw = (SlideIntegrate * len(next_problems))()
+    for w, (p, g) in enumerate(zip(next_problems, integrate)):
+        if g:
+            _integ_struct(iw[w], g, int(p["n_imu"]), keep)
+    return iw
+
+
+def _dev(t):
+    return None if t is None else vp(t.data_ptr() if hasattr(t, "data_ptr") else int(t))
+
+
+def _vision_struct(next_problems, vision, Lc: int, Fc: int, keep: list):
+    """The icg_ba_slide_vision array of the `vision` dicts (WindowSolver.slide_vision) and the host rows the call builds into, sized to a
+    handle of Lc landmarks and Fc factors.  Empties the vision rows of next_problems, which the call does not read."""
+    vw = (SlideVision * len(next_problems))()
+    outs = []
+    for w, (p, v) in enumerate(zip(next_problems, vision)):
+        o = dict(lm_src=np.zeros(Lc, np.int32), lm_origin=np.zeros(Lc, np.int32), nan_flags=np.zeros(Lc + int(v.get("n_new", 0)), np.uint8), f_src=np.zeros(Fc, np.int32), f_lm=np.zeros(Fc, np.int32), f_ref=np.zeros(Fc, np.int32),
+                 f_obs=np.zeros(Fc, np.int32), invdepth=np.zeros(Lc), f_const=np.zeros((Fc, 14)))
+        outs.append(o)
+        p.update(L=0, F=0, invdepth=np.zeros(0), f_lm=np.zeros(0, np.int32), f_ref=np.zeros(0, np.int32), f_obs=np.zeros(0, np.int32),
+                 f_const=np.zeros(0), f_active=np.zeros(0, np.uint8))
+        s = vw[w]
+        s.num_marg = int(v["num_marg"])
+        s.node_in_map = _arg(keep, v["node_in_map"], np.uint8, u8p)
+        if v.get("obs_factor") is not None and len(v["obs_factor"]):
+            s.obs_factor = _arg(keep, v["obs_factor"], np.int32, i32p)
+        cs = _cam(v["camera"])
+        s.cam[:] = [float(getattr(cs, k)) for k, _ in CameraStruct._fields_]
+        s.node_td = _arg(keep, v["node_td"], np.float64, f64p)
+        s.cur_node = int(v["cur_node"])
+        frames = v.get("frames", {})
+        s.n_frames = len(frames)
+        s.frame_id = _arg(keep, np.array(list(frames.keys()), np.int64), np.int64, i64p)
+        s.frame_node = _arg(keep, np.array(list(frames.values()), np.int32), np.int32, i32p)
+        s.n_obs, s.n_in = int(v.get("n_obs", 0)), int(v.get("n_in", 0))
+        s.dev_n, s.obs_src, s.obs_lm, s.obs_node = (_dev(v.get(k)) for k in ("dev_n", "obs_src", "obs_lm", "obs_node"))
+        s.obs_undis_xy, s.obs_vel = _dev(v.get("obs_undis_xy")), _dev(v.get("obs_vel"))
+        s.n_new = int(v.get("n_new", 0))
+        s.dev_new_n = _dev(v.get("dev_new_n"))
+        s.new_depth, s.new_vel_ref, s.new_vel_cur = (_dev(v.get(k)) for k in ("new_depth", "new_vel_ref", "new_vel_cur"))
+        s.new_ref_undis_xy, s.new_cur_undis_xy, s.new_ref_frame_id = (_dev(v.get(k)) for k in ("new_ref_undis_xy", "new_cur_undis_xy", "new_ref_frame_id"))
+        s.lm_src, s.f_src, s.f_lm, s.f_ref, s.f_obs = (o[k].ctypes.data_as(i32p) for k in ("lm_src", "f_src", "f_lm", "f_ref", "f_obs"))
+        s.invdepth, s.f_const = o["invdepth"].ctypes.data_as(f64p), o["f_const"].ctypes.data_as(f64p)
+        s.lm_origin, s.nan_flags = o["lm_origin"].ctypes.data_as(i32p), o["nan_flags"].ctypes.data_as(u8p)
+    return vw, outs
+
+
+def _vision_results(next_problems, carry, vw, outs) -> list:
+    """slide_vision()'s dicts from the rows a successful call built; writes the built window into next_problems and its lm_src / f_src
+    into carry."""
+    res = []
+    for w, (p, c, o) in enumerate(zip(next_problems, carry, outs)):
+        L, F = int(vw[w].L), int(vw[w].F)
+        r = dict(L=L, F=F, nan_dropped=int(vw[w].nan_dropped), lm_src=o["lm_src"][:L].copy(), lm_origin=o["lm_origin"][:L].copy(),
+                 nan_flags=o["nan_flags"], invdepth=o["invdepth"][:L].copy(),
+                 f_src=o["f_src"][:F].copy(), f_lm=o["f_lm"][:F].copy(), f_ref=o["f_ref"][:F].copy(), f_obs=o["f_obs"][:F].copy(),
+                 f_const=o["f_const"][:F].copy())
+        res.append(r)
+        fcn = r["f_const"].copy()
+        fcn[r["f_src"] >= 0] = np.nan
+        p.update(L=L, F=F, invdepth=r["invdepth"].copy(), f_lm=r["f_lm"].copy(), f_ref=r["f_ref"].copy(), f_obs=r["f_obs"].copy(),
+                 f_const=fcn.reshape(-1), f_active=np.ones(F, np.uint8))
+        c["lm_src"], c["f_src"] = r["lm_src"].copy(), r["f_src"].copy()
+    return res
 
 
 class WindowSolver:
@@ -332,11 +427,10 @@ class WindowSolver:
         if isinstance(problems, dict):
             problems = [problems]
         n = len(problems)
-        arr = (BaProblem * n)(*[to_struct(p) for p in problems])
+        arr = _problems(problems)
         summ = (BaSummary * n)()
         check(lib().icg_ba_solve(self._h, n, arr, max_num_iterations, summ), "icg_ba_solve")
-        return [dict(iterations=s.iterations, num_successful_steps=s.num_successful_steps, termination=s.termination,
-                     initial_cost=s.initial_cost, final_cost=s.final_cost, final_radius=s.final_radius) for s in summ]
+        return [_summary(s) for s in summ]
 
     def solve_structs(self, arr, n, max_num_iterations, summ):
         check(lib().icg_ba_solve(self._h, n, arr, max_num_iterations, summ), "icg_ba_solve")
@@ -344,7 +438,7 @@ class WindowSolver:
     # -- device-resident stages
     def upload(self, problems):
         n = len(problems)
-        self._keep = (BaProblem * n)(*[to_struct(p) for p in problems])
+        self._keep = _problems(problems)
         self._n = n
         check(lib().icg_ba_upload(self._h, n, self._keep), "icg_ba_upload")
 
@@ -354,8 +448,7 @@ class WindowSolver:
     def download(self, write_back: bool = True):
         summ = (BaSummary * self._n)()
         check(lib().icg_ba_download(self._h, self._n, self._keep if write_back else None, summ), "icg_ba_download")
-        return [dict(iterations=s.iterations, num_successful_steps=s.num_successful_steps, termination=s.termination,
-                     initial_cost=s.initial_cost, final_cost=s.final_cost, final_radius=s.final_radius) for s in summ]
+        return [_summary(s) for s in summ]
 
     def sync(self):
         check(lib().icg_ba_sync(self._h), "icg_ba_sync")
@@ -363,14 +456,13 @@ class WindowSolver:
     def peek_linearization(self, w: int) -> dict:
         """Window w's system as the last linearisation and Schur complement left it (icg_ba_peek_linearization; a test read-out).  Mp: a
         dict (reference node, observing node) -> packed upper 20x20; A_W: (L, 6K + 8) by landmark id; Hs: (NCV, NCV) lower triangle."""
-        from ._lib import Linearization
         K, L, F = self.max_K, max(1, self.max_L), max(1, self.max_F)
         NCV, N, PM = 6 * K + 7, 15 * K + 7, K * (K - 1)
         a = dict(pair_ro=np.zeros(PM, np.int32), Mp=np.zeros(PM * 210), A_W=np.zeros(L * (NCV + 1)), h_l=np.zeros(L), g_l=np.zeros(L),
                  H_c=np.zeros(N * N), g_c=np.zeros(N), costf=np.zeros(F), scale_l=np.zeros(L), Hs=np.zeros(NCV * NCV), visv=np.zeros(3 * NCV))
         s = Linearization()
         for name, arr in a.items():
-            setattr(s, name, arr.ctypes.data_as(C.POINTER(C.c_int32 if arr.dtype == np.int32 else C.c_double)))
+            setattr(s, name, arr.ctypes.data_as(i32p if arr.dtype == np.int32 else f64p))
         check(lib().icg_ba_peek_linearization(self._h, w, C.byref(s)), "icg_ba_peek_linearization")
         K, L, F, P = s.K, s.L, s.F, s.n_pairs
         NCV, N = 6 * K + 7, 15 * K + 7
@@ -391,14 +483,11 @@ class WindowSolver:
     def gvins_optimization_batch(self, problems, num_iterations=20):
         """GVINS::gvinsOptimization on a list of windows in one device-resident call (icg_ba_gvins_optimization)."""
         n = len(problems)
-        arr = (BaProblem * n)(*[to_struct(p) for p in problems])
+        arr = _problems(problems)
         summ = (BaSummary * (2 * n))()
         culled = (C.c_int32 * (2 * n))()
         check(lib().icg_ba_gvins_optimization(self._h, n, arr, num_iterations, summ, culled), "icg_ba_gvins_optimization")
-        f = lambda s: dict(iterations=s.iterations, num_successful_steps=s.num_successful_steps, termination=s.termination,
-                           initial_cost=s.initial_cost, final_cost=s.final_cost, final_radius=s.final_radius)
-        return [dict(pass1=f(summ[2 * w]), pass2=f(summ[2 * w + 1]), reproj_removed=culled[2 * w], gnss_reweighted=culled[2 * w + 1])
-                for w in range(n)]
+        return _two_pass(summ, culled, n)
 
     def run_gvins(self, num_iterations: int = 20, restart: bool = False):
         check(lib().icg_ba_run_gvins(self._h, num_iterations, 1 if restart else 0), "icg_ba_run_gvins")
@@ -452,7 +541,7 @@ class WindowSolver:
             cw = (CullWindow * len(problems))(*[cull_struct(p, c) for p, c in zip(problems, keep)])
             for w, (c, k) in enumerate(zip(culled, keep)):  # the culling's flags, as that call returned them
                 k["flags"] = [np.ascontiguousarray(c["lm_outlier"], np.uint8), np.ascontiguousarray(c["obs_outlier"], np.uint8)]
-                cw[w].lm_outlier, cw[w].obs_outlier = (a.ctypes.data_as(bp) for a in k["flags"])
+                cw[w].lm_outlier, cw[w].obs_outlier = (a.ctypes.data_as(u8p) for a in k["flags"])
             ptrs = (vp * len(nim))(*[vp(m.ctypes.data) for m in nim])
             check(lib().icg_ba_marginalize_resident_culled(self._h, call["n"], call["arr"], vp(call["nm"].ctypes.data), cw, ptrs, call["pri"]),
                   "icg_ba_marginalize_resident_culled")
@@ -469,11 +558,10 @@ class WindowSolver:
         if isinstance(problems, dict):
             problems, cull_inputs = [problems], [cull_inputs]
         n = len(problems)
-        arr = (BaProblem * n)(*[to_struct(p) for p in problems])
+        arr = _problems(problems)
         outs = [dict(c) for c in cull_inputs]
         cw = (CullWindow * n)(*[cull_struct(p, c) for p, c in zip(problems, outs)])
-        cam = camera.c if hasattr(camera, "c") else camera
-        check(lib().icg_ba_update_and_cull_resident(self._h, n, arr, C.byref(cam), float(std), cw), "icg_ba_update_and_cull_resident")
+        check(lib().icg_ba_update_and_cull_resident(self._h, n, arr, C.byref(_cam(camera)), float(std), cw), "icg_ba_update_and_cull_resident")
         for c, s in zip(outs, cw):
             c.update(R_bc_out=np.array(s.R_bc_out[:]).reshape(3, 3), t_bc_out=np.array(s.t_bc_out[:]), td_bc_out=s.td_bc_out, ext_accepted=s.ext_accepted,
                      counts=np.array(s.counts[:], np.int32))
@@ -499,36 +587,24 @@ class WindowSolver:
         return outs
 
     def _cull_built(self, fn, problems, camera, std, ext_inputs):
-        from ._lib import CullLists
         if isinstance(problems, dict):
             problems, ext_inputs = [problems], [ext_inputs]
         n = len(problems)
-        arr = (BaProblem * n)(*[to_struct(p) for p in problems])
+        arr = _problems(problems)
         outs, cw, cl = [], (CullWindow * n)(), (CullLists * n)()
         cap = self.max_L + self.max_F
         for w, (p, e) in enumerate(zip(problems, ext_inputs)):
             K, L = int(p["K"]), int(p["L"])
             o = {k: e[k] for k in ("R_bc", "t_bc", "td_bc", "estimate_ext", "estimate_td") if k in e}
             o.update(lm_ref_node=np.zeros(L, np.int32), obs_off=np.zeros(L + 1, np.int32), obs_node=np.zeros(cap, np.int32), obs_factor=np.zeros(cap, np.int32),
-                     lm_ref_kp=np.zeros((L, 2), np.float32), obs_kp=np.zeros((cap, 2), np.float32), cam_pose=np.zeros((K, 12)), lm_pw=np.zeros((L, 3)),
-                     lm_depth=np.zeros(L), lm_outlier=np.zeros(L, np.uint8), obs_outlier=np.zeros(cap, np.uint8))
+                     lm_ref_kp=np.zeros((L, 2), np.float32), obs_kp=np.zeros((cap, 2), np.float32))
             outs.append(o)
-            s = cw[w]
-            for k, v in zip(("R_bc", "t_bc"), (np.asarray(e["R_bc"], np.float64).reshape(-1), np.asarray(e["t_bc"], np.float64).reshape(-1))):
-                getattr(s, k)[:] = [float(x) for x in v]
-            s.td_bc, s.estimate_ext, s.estimate_td = float(e.get("td_bc", 0.0)), int(e.get("estimate_ext", 1)), int(e.get("estimate_td", 1))
-            s.cam_pose, s.lm_pw, s.lm_depth = (o[k].ctypes.data_as(dp) for k in ("cam_pose", "lm_pw", "lm_depth"))
-            s.lm_outlier, s.obs_outlier = o["lm_outlier"].ctypes.data_as(bp), o["obs_outlier"].ctypes.data_as(bp)
+            _cull_ext(cw[w], e)
+            _cull_outputs(cw[w], o, K, L, cap)
             for k in ("lm_ref_node", "obs_off", "obs_node", "obs_factor"):
-                setattr(cl[w], k, o[k].ctypes.data_as(ip))
-            cl[w].lm_ref_kp, cl[w].obs_kp = o["lm_ref_kp"].ctypes.data_as(fp), o["obs_kp"].ctypes.data_as(fp)
-        cam = camera.c if hasattr(camera, "c") else camera
-        rc = getattr(lib(), fn)(self._h, n, arr, C.byref(cam), float(std), cw, cl)
-        if rc != 0:
-            from ._lib import IcgError
-            err = IcgError(f"{fn} failed with code {rc}: {lib().icg_last_error().decode('utf-8', 'replace')}")
-            err.code = rc
-            raise err
+                setattr(cl[w], k, o[k].ctypes.data_as(i32p))
+            cl[w].lm_ref_kp, cl[w].obs_kp = o["lm_ref_kp"].ctypes.data_as(f32p), o["obs_kp"].ctypes.data_as(f32p)
+        check(getattr(lib(), fn)(self._h, n, arr, C.byref(_cam(camera)), float(std), cw, cl), fn)
         for o, s, c in zip(outs, cw, cl):
             no = int(c.n_obs)
             for k in ("obs_node", "obs_factor", "obs_kp", "obs_outlier"):
@@ -560,12 +636,11 @@ class WindowSolver:
         end_states (n_imu x 10, zero where the gate was closed) and blobs (n_imu x 480: the window's blobs with the reintegrated ones
         replaced).  The reintegrated blobs are written into problem["imu_blob"], as the reference mutates preintegrationlist_.  A factor with
         status -1 raises IcgError after the call; the exception's `results` holds the dicts."""
-        from ._lib import IcgError
         if isinstance(problems, dict):
             problems, imu_rows = [problems], [imu_rows]
         n = len(problems)
-        flags = [1] * n if reintegrate is None else [int(bool(x)) for x in reintegrate]
-        arr = (BaProblem * n)(*[to_struct(p) for p in problems])
+        flags = _flags(True if reintegrate is None else reintegrate, n)
+        arr = _problems(problems)
         io = (ReintWindow * n)()
         outs, keep = [], []
         for w, p in enumerate(problems):
@@ -574,26 +649,17 @@ class WindowSolver:
                      blobs=np.array(np.asarray(p["imu_blob"], np.float64)[:m * IMU_BLOB].reshape(m, IMU_BLOB), copy=True))
             outs.append(o)
             io[w].reintegrate = flags[w] if m > 0 else 0
-            io[w].status, io[w].blob_out = o["status"].ctypes.data_as(C.POINTER(C.c_int8)), o["blobs"].ctypes.data_as(dp)
-            io[w].end_state10 = o["end_states"].ctypes.data_as(dp)
+            _point_outputs(io[w], o)
             if io[w].reintegrate and not stored:
-                rows = [np.asarray(x, np.float64).reshape(-1, 7) for x in imu_rows[w]]
-                off = np.zeros(m + 1, np.int32)
-                off[1:] = np.cumsum([len(x) for x in rows])
-                imu = np.ascontiguousarray(np.concatenate(rows, axis=0)) if rows else np.zeros((0, 7))
-                keep.append((imu, off))
-                io[w].imu, io[w].imu_off = imu.ctypes.data_as(dp), off.ctypes.data_as(ip)
-        nz = np.ascontiguousarray(noise5, np.float64)
-        stn = np.ascontiguousarray(station, np.float64)
-        rc = getattr(lib(), fn)(self._h, n, arr, vp(nz.ctypes.data), vp(stn.ctypes.data), io)
+                imu, off = _imu_rows(imu_rows[w], m)
+                io[w].imu, io[w].imu_off = _arg(keep, imu, np.float64, f64p), _arg(keep, off, np.int32, i32p)
+        nz, stn = _noise_station(noise5, station, keep)
+        rc = getattr(lib(), fn)(self._h, n, arr, nz, stn, io)
         for w, (p, o) in enumerate(zip(problems, outs)):
             o["count"] = int(io[w].count)
             if (o["status"] == 1).any():
                 p["imu_blob"].reshape(-1, IMU_BLOB)[:len(o["status"])][o["status"] == 1] = o["blobs"][o["status"] == 1]
-        if rc != 0:
-            err = IcgError(f"{fn} failed with code {rc}: {lib().icg_last_error().decode('utf-8', 'replace')}")
-            err.code, err.results = rc, outs
-            raise err
+        check(rc, fn, outs)
         return outs
 
     def slide(self, next_problems, carry, prior_from_marg=True):
@@ -610,20 +676,9 @@ class WindowSolver:
         with int32 arrays node_src (K), lm_src (L), f_src (F), imu_src (n_imu), gnss_src (n_gnss) -- old row or -1; a missing key carries
         nothing of that kind.  prior_from_marg (one flag, or one per window): the prior is the one the last resident marginalization left.
         Follow with run_gvins() and gvins_optimization_end(next_problems)."""
-        from ._lib import SlideWindow
         n = len(next_problems)
-        flags = [prior_from_marg] * n if np.isscalar(prior_from_marg) else list(prior_from_marg)
-        arr = (BaProblem * n)(*[to_struct(p) for p in next_problems])
-        cw = (SlideWindow * n)()
         keep = []
-        for w, c in enumerate(carry):
-            for k in ("node_src", "lm_src", "f_src", "imu_src", "gnss_src"):
-                if c.get(k) is None:
-                    continue
-                a = np.ascontiguousarray(c[k], np.int32)
-                keep.append(a)
-                setattr(cw[w], k, a.ctypes.data_as(ip))
-            cw[w].prior_from_marg = 1 if flags[w] else 0
+        arr, cw = _problems(next_problems), _slide_carry(carry, n, prior_from_marg, keep)
         check(getattr(lib(), fn)(self._h, n, arr, cw), fn)
         self._keep, self._n = arr, n
 
@@ -648,38 +703,17 @@ class WindowSolver:
         noise5 = gyr_arw, acc_vrw, gyr_bias_std, acc_bias_std, corr_time; station = parameters_->station.  Returns one dict per window: status
         (n_imu int8: 1 integrated, 0 not, -1 not positive definite), blobs (n_imu x 480) and end_states (n_imu x 10), zero where status is 0.
         A rejected call raises IcgError with the handle unchanged; after the integration its `results` holds the dicts."""
-        from ._lib import IcgError, SlideIntegrate, SlideWindow, u8p
         n = len(next_problems)
-        flags = [prior_from_marg] * n if np.isscalar(prior_from_marg) else list(prior_from_marg)
-        arr = (BaProblem * n)(*[to_struct(p) for p in next_problems])
-        cw = (SlideWindow * n)()
-        iw = (SlideIntegrate * n)()
-        keep, outs = [], []
-
-        def arg(a, dtype, ptr):
-            a = np.ascontiguousarray(a, dtype)
-            keep.append(a)
-            return a.ctypes.data_as(ptr)
-
-        for w, (p, c, g) in enumerate(zip(next_problems, carry, integrate)):
-            for k in ("node_src", "lm_src", "f_src", "imu_src", "gnss_src"):
-                if c.get(k) is not None:
-                    setattr(cw[w], k, arg(c[k], np.int32, ip))
-            cw[w].prior_from_marg = 1 if flags[w] else 0
+        keep = []
+        arr, cw = _problems(next_problems), _slide_carry(carry, n, prior_from_marg, keep)
+        iw = _integ_array(next_problems, integrate, keep)
+        outs = []
+        for w, p in enumerate(next_problems):
             m = int(p["n_imu"])
-            o = dict(status=np.zeros(m, np.int8), blobs=np.zeros((m, IMU_BLOB)), end_states=np.zeros((m, 10)))
-            outs.append(o)
-            iw[w].status, iw[w].blob_out = o["status"].ctypes.data_as(C.POINTER(C.c_int8)), o["blobs"].ctypes.data_as(dp)
-            iw[w].end_state10 = o["end_states"].ctypes.data_as(dp)
-            if g:
-                _integ_struct(iw[w], g, m, arg)
-        nz = np.ascontiguousarray(noise5, np.float64)
-        stn = np.ascontiguousarray(station, np.float64)
-        rc = getattr(lib(), fn)(self._h, n, arr, cw, iw, vp(nz.ctypes.data), vp(stn.ctypes.data))
-        if rc != 0:
-            err = IcgError(f"{fn} failed with code {rc}: {lib().icg_last_error().decode('utf-8', 'replace')}")
-            err.code, err.results = rc, outs
-            raise err
+            outs.append(dict(status=np.zeros(m, np.int8), blobs=np.zeros((m, IMU_BLOB)), end_states=np.zeros((m, 10))))
+            _point_outputs(iw[w], outs[w])
+        nz, stn = _noise_station(noise5, station, keep)
+        check(getattr(lib(), fn)(self._h, n, arr, cw, iw, nz, stn), fn, outs)
         self._keep, self._n = arr, n
         return outs
 
@@ -687,14 +721,11 @@ class WindowSolver:
         """Seeds the handle's IMU sample store (icg_ba_imu_samples_from_ins): factor k of resident window w gets getImuSeriesFromTo(
         node_times[w][k], node_times[w][k + 1]) cut from stream streams[w] of `ins` (an ins.InsWindow on this handle's device).  Call it right
         after the upload of windows whose INS windows still cover their spans."""
-        from ._lib import InsCut
         n = len(streams)
         cut = (InsCut * n)()
         keep = []
         for w in range(n):
-            t = np.ascontiguousarray(node_times[w], np.float64)
-            keep.append(t)
-            cut[w].stream, cut[w].node_time = int(streams[w]), t.ctypes.data_as(dp)
+            cut[w].stream, cut[w].node_time = int(streams[w]), _arg(keep, node_times[w], np.float64, f64p)
         check(lib().icg_ba_imu_samples_from_ins(self._h, ins._h, n, cut), "icg_ba_imu_samples_from_ins")
 
     def imu_samples(self, w: int):
@@ -725,69 +756,34 @@ class WindowSolver:
         carried factors keep their stored rows.  `integrate` dicts as slide_integrate takes them, without imu_rows / imu / imu_off.  Returns
         slide_integrate()'s dicts (vision: slide_vision()'s), each with n_rows (every new factor's stored rows, -1: none).  Status -2 marks a
         factor whose interval the INS window cannot serve (the call raises IcgError, the handle unchanged)."""
-        from ._lib import IcgError, SlideIns, SlideIntegrate
         fn = "icg_ba_slide_ins_resident"
+        if vision is not None and integrate is not None and noise5 is None:
+            raise ValueError(f"{fn}: integrate needs noise5")
         n = len(next_problems)
         keep = []
-        n_rows = [np.full(int(p["n_imu"]), -1, np.int32) for p in next_problems]
-        statuses = [np.zeros(int(p["n_imu"]), np.int8) for p in next_problems]
-        blobs = [np.zeros((int(p["n_imu"]), IMU_BLOB)) for p in next_problems]
-        ends = [np.zeros((int(p["n_imu"]), 10)) for p in next_problems]
-
-        def arg(a, dtype, ptr):
-            a = np.ascontiguousarray(a, dtype)
-            keep.append(a)
-            return a.ctypes.data_as(ptr)
-
-        def call(arr, cw, iw, nz, stn, vw):
-            io = (SlideIns * n)()
-            for w, p in enumerate(next_problems):
-                m = int(p["n_imu"])
-                if iw is not None:
-                    io[w].integ = iw[w]
-                elif integrate is not None and integrate[w]:
-                    _integ_struct(io[w].integ, integrate[w], m, arg, with_rows=False)
-                g = io[w].integ
-                g.status, g.blob_out = statuses[w].ctypes.data_as(C.POINTER(C.c_int8)), blobs[w].ctypes.data_as(dp)
-                g.end_state10 = ends[w].ctypes.data_as(dp)
-                io[w].stream = int(streams[w])
-                if node_times[w] is not None:
-                    io[w].node_time = arg(node_times[w], np.float64, dp)
-                if merge_src is not None and merge_src[w] is not None:
-                    io[w].merge_src = arg(merge_src[w], np.int32, ip)
-                io[w].n_rows = n_rows[w].ctypes.data_as(ip)
-            return lib().icg_ba_slide_ins_resident(self._h, ins._h, n, arr, cw, io, vp(nz.ctypes.data), vp(stn.ctypes.data), vw)
-
-        def results():
-            return [dict(status=statuses[w], blobs=blobs[w], end_states=ends[w], n_rows=n_rows[w]) for w in range(n)]
-
+        vw, built = (None, None) if vision is None else _vision_struct(next_problems, vision, self.max_L, self.max_F, keep)
+        arr = _problems(next_problems)
+        cw = _slide_carry(carry, n, prior_from_marg, keep, _CARRY if vision is None else _VISION_CARRY)
+        io = (SlideIns * n)()
+        outs = []
+        for w, p in enumerate(next_problems):
+            m = int(p["n_imu"])
+            outs.append(dict(status=np.zeros(m, np.int8), blobs=np.zeros((m, IMU_BLOB)), end_states=np.zeros((m, 10)), n_rows=np.full(m, -1, np.int32)))
+            if integrate is not None and integrate[w]:
+                _integ_struct(io[w].integ, integrate[w], m, keep, with_rows=False)
+            _point_outputs(io[w].integ, outs[w])
+            io[w].stream = int(streams[w])
+            if node_times[w] is not None:
+                io[w].node_time = _arg(keep, node_times[w], np.float64, f64p)
+            if merge_src is not None and merge_src[w] is not None:
+                io[w].merge_src = _arg(keep, merge_src[w], np.int32, i32p)
+            io[w].n_rows = outs[w]["n_rows"].ctypes.data_as(i32p)
+        nz, stn = _noise_station(noise5, station, keep)
+        check(lib().icg_ba_slide_ins_resident(self._h, ins._h, n, arr, cw, io, nz, stn, vw), fn, outs)
         if vision is not None:
-            try:
-                res = self._slide_vision(fn, next_problems, carry, vision, integrate, noise5, station, prior_from_marg, call=call)
-            except IcgError as e:
-                e.results = results()
-                raise
-            for w, r in enumerate(res):
-                r.update(results()[w])
-            return res
-        from ._lib import SlideWindow
-        flags = [prior_from_marg] * n if np.isscalar(prior_from_marg) else list(prior_from_marg)
-        arr = (BaProblem * n)(*[to_struct(p) for p in next_problems])
-        cw = (SlideWindow * n)()
-        for w, c in enumerate(carry):
-            for k in ("node_src", "lm_src", "f_src", "imu_src", "gnss_src"):
-                if c.get(k) is not None:
-                    setattr(cw[w], k, arg(c[k], np.int32, ip))
-            cw[w].prior_from_marg = 1 if flags[w] else 0
-        nz = np.ascontiguousarray(noise5, np.float64)
-        stn = np.ascontiguousarray(station, np.float64)
-        rc = call(arr, cw, None, nz, stn, None)
-        if rc != 0:
-            err = IcgError(f"{fn} failed with code {rc}: {lib().icg_last_error().decode('utf-8', 'replace')}")
-            err.code, err.results = rc, results()
-            raise err
+            outs = [dict(r, **o) for r, o in zip(_vision_results(next_problems, carry, vw, built), outs)]
         self._keep, self._n = arr, n
-        return results()
+        return outs
 
     def slide_vision(self, next_problems, carry, vision, integrate=None, noise5=None, station=(0.0, 0.0, 0.0), prior_from_marg=True):
         return self._slide_vision("icg_ba_slide_vision_resident", next_problems, carry, vision, integrate, noise5, station, prior_from_marg)
@@ -799,8 +795,7 @@ class WindowSolver:
         lm_origin: old shard-local landmark or -(j + 1) for global new point j, nan_flags: old shard L + every new point, set on its own rank)."""
         return self._slide_vision("icg_ba_shard_slide_vision_resident", next_problems, carry, vision, integrate, noise5, station, prior_from_marg)
 
-    def _slide_vision(self, fn, next_problems, carry, vision, integrate=None, noise5=None, station=(0.0, 0.0, 0.0), prior_from_marg=True,
-                      call=None):
+    def _slide_vision(self, fn, next_problems, carry, vision, integrate=None, noise5=None, station=(0.0, 0.0, 0.0), prior_from_marg=True):
         """slide() (integrate given: slide_integrate()) whose vision rows are built on the device (icg_ba_slide_vision_resident):
         addReprojectionParameters + addReprojectionFactors on the culled window this handle holds plus the new keyframes' observations.  The
         last update_and_cull() of these windows must be current.  next_problems' L, F, invdepth, f_lm / f_ref / f_obs / f_const, f_active and
@@ -815,90 +810,18 @@ class WindowSolver:
         Returns one dict per window: L, F, nan_dropped, nan_flags (old L + n_new entries first: 1 where a landmark or new point was dropped
         for a NaN inverse depth), lm_origin (old landmark, or -(j + 1) for new point j), lm_src, f_src, f_lm, f_ref, f_obs, invdepth and f_const (the new factors' rows, f_src = -1;
         the others zero).  A rejected call raises IcgError with the handle unchanged."""
-        from ._lib import IcgError, SlideIntegrate, SlideVision, SlideWindow
-        from .camera import CameraStruct
         if integrate is not None and noise5 is None:
             raise ValueError(f"{fn}: integrate needs noise5")
         n = len(next_problems)
-        flags = [prior_from_marg] * n if np.isscalar(prior_from_marg) else list(prior_from_marg)
-        Lc, Fc = self.max_L, self.max_F
-        outs = []
-        for p, v in zip(next_problems, vision):  # the built rows land here, sized to the handle's capacity until the call returns
-            o = dict(lm_src=np.zeros(Lc, np.int32), lm_origin=np.zeros(Lc, np.int32), nan_flags=np.zeros(Lc + int(v.get("n_new", 0)), np.uint8), f_src=np.zeros(Fc, np.int32), f_lm=np.zeros(Fc, np.int32), f_ref=np.zeros(Fc, np.int32),
-                     f_obs=np.zeros(Fc, np.int32), invdepth=np.zeros(Lc), f_const=np.zeros((Fc, 14)))
-            outs.append(o)
-            p.update(L=0, F=0, invdepth=np.zeros(0), f_lm=np.zeros(0, np.int32), f_ref=np.zeros(0, np.int32), f_obs=np.zeros(0, np.int32),
-                     f_const=np.zeros(0), f_active=np.zeros(0, np.uint8))
-        arr = (BaProblem * n)(*[to_struct(p) for p in next_problems])
-        cw = (SlideWindow * n)()
-        vw = (SlideVision * n)()
-        iw = (SlideIntegrate * n)() if integrate is not None else None
         keep = []
-
-        def arg(a, dtype, ptr):
-            a = np.ascontiguousarray(a, dtype)
-            keep.append(a)
-            return a.ctypes.data_as(ptr)
-
-        def dev(t):
-            return None if t is None else vp(t.data_ptr() if hasattr(t, "data_ptr") else int(t))
-
-        for w, (p, c, v) in enumerate(zip(next_problems, carry, vision)):
-            for k in ("node_src", "imu_src", "gnss_src"):
-                if c.get(k) is not None:
-                    setattr(cw[w], k, arg(c[k], np.int32, ip))
-            cw[w].prior_from_marg = 1 if flags[w] else 0
-            if iw is not None and integrate[w]:
-                _integ_struct(iw[w], integrate[w], int(p["n_imu"]), arg, with_rows=call is None)
-            s = vw[w]
-            s.num_marg = int(v["num_marg"])
-            s.node_in_map = arg(v["node_in_map"], np.uint8, bp)
-            if v.get("obs_factor") is not None and len(v["obs_factor"]):
-                s.obs_factor = arg(v["obs_factor"], np.int32, ip)
-            cam = v["camera"]
-            cs = cam.c if hasattr(cam, "c") else cam
-            s.cam[:] = [float(getattr(cs, k)) for k, _ in CameraStruct._fields_]
-            s.node_td = arg(v["node_td"], np.float64, dp)
-            s.cur_node = int(v["cur_node"])
-            frames = v.get("frames", {})
-            s.n_frames = len(frames)
-            s.frame_id = arg(np.array(list(frames.keys()), np.int64), np.int64, C.POINTER(C.c_int64))
-            s.frame_node = arg(np.array(list(frames.values()), np.int32), np.int32, ip)
-            s.n_obs, s.n_in = int(v.get("n_obs", 0)), int(v.get("n_in", 0))
-            s.dev_n, s.obs_src, s.obs_lm, s.obs_node = (dev(v.get(k)) for k in ("dev_n", "obs_src", "obs_lm", "obs_node"))
-            s.obs_undis_xy, s.obs_vel = dev(v.get("obs_undis_xy")), dev(v.get("obs_vel"))
-            s.n_new = int(v.get("n_new", 0))
-            s.dev_new_n = dev(v.get("dev_new_n"))
-            s.new_depth, s.new_vel_ref, s.new_vel_cur = (dev(v.get(k)) for k in ("new_depth", "new_vel_ref", "new_vel_cur"))
-            s.new_ref_undis_xy, s.new_cur_undis_xy, s.new_ref_frame_id = (dev(v.get(k)) for k in ("new_ref_undis_xy", "new_cur_undis_xy", "new_ref_frame_id"))
-            o = outs[w]
-            s.lm_src, s.f_src, s.f_lm, s.f_ref, s.f_obs = (o[k].ctypes.data_as(ip) for k in ("lm_src", "f_src", "f_lm", "f_ref", "f_obs"))
-            s.invdepth, s.f_const = o["invdepth"].ctypes.data_as(dp), o["f_const"].ctypes.data_as(dp)
-            s.lm_origin, s.nan_flags = o["lm_origin"].ctypes.data_as(ip), o["nan_flags"].ctypes.data_as(bp)
-        nz = np.ascontiguousarray(noise5 if noise5 is not None else np.zeros(5), np.float64)
-        stn = np.ascontiguousarray(station, np.float64)
-        if call is not None:  # slide_ins: the INS form of the call, from the same structs
-            rc = call(arr, cw, iw, nz, stn, vw)
-        else:
-            rc = getattr(lib(), fn)(self._h, n, arr, cw, None if iw is None else iw, vp(nz.ctypes.data) if iw is not None else None,
-                                    vp(stn.ctypes.data) if iw is not None else None, vw)
-        if rc != 0:
-            err = IcgError(f"{fn} failed with code {rc}: {lib().icg_last_error().decode('utf-8', 'replace')}")
-            err.code = rc
-            raise err
-        res = []
-        for w, (p, c, o) in enumerate(zip(next_problems, carry, outs)):
-            L, F = int(vw[w].L), int(vw[w].F)
-            r = dict(L=L, F=F, nan_dropped=int(vw[w].nan_dropped), lm_src=o["lm_src"][:L].copy(), lm_origin=o["lm_origin"][:L].copy(),
-                     nan_flags=o["nan_flags"], invdepth=o["invdepth"][:L].copy(),
-                     f_src=o["f_src"][:F].copy(), f_lm=o["f_lm"][:F].copy(), f_ref=o["f_ref"][:F].copy(), f_obs=o["f_obs"][:F].copy(),
-                     f_const=o["f_const"][:F].copy())
-            res.append(r)
-            fcn = r["f_const"].copy()
-            fcn[r["f_src"] >= 0] = np.nan
-            p.update(L=L, F=F, invdepth=r["invdepth"].copy(), f_lm=r["f_lm"].copy(), f_ref=r["f_ref"].copy(), f_obs=r["f_obs"].copy(),
-                     f_const=fcn.reshape(-1), f_active=np.ones(F, np.uint8))
-            c["lm_src"], c["f_src"] = r["lm_src"].copy(), r["f_src"].copy()
+        vw, built = _vision_struct(next_problems, vision, self.max_L, self.max_F, keep)
+        arr, cw = _problems(next_problems), _slide_carry(carry, n, prior_from_marg, keep, _VISION_CARRY)
+        iw, nz, stn = None, None, None
+        if integrate is not None:
+            iw = _integ_array(next_problems, integrate, keep)
+            nz, stn = _noise_station(noise5, station, keep)
+        check(getattr(lib(), fn)(self._h, n, arr, cw, iw, nz, stn, vw), fn)
+        res = _vision_results(next_problems, carry, vw, built)
         self._keep, self._n = arr, n
         return res
 
@@ -906,21 +829,18 @@ class WindowSolver:
         """icg_ba_gvins_optimization_end after run_gvins(): synchronises, writes the parameters, f_active and gnss_std back into the problem
         dicts and returns the two-pass results in the layout of gvins_optimization_batch."""
         n = len(problems)
-        arr = (BaProblem * n)(*[to_struct(p) for p in problems])
+        arr = _problems(problems)
         summ = (BaSummary * (2 * n))()
         culled = (C.c_int32 * (2 * n))()
         check(lib().icg_ba_gvins_optimization_end(self._h, n, arr, summ, culled), "icg_ba_gvins_optimization_end")
-        f = lambda s: dict(iterations=s.iterations, num_successful_steps=s.num_successful_steps, termination=s.termination,
-                           initial_cost=s.initial_cost, final_cost=s.final_cost, final_radius=s.final_radius)
-        return [dict(pass1=f(summ[2 * w]), pass2=f(summ[2 * w + 1]), reproj_removed=culled[2 * w], gnss_reweighted=culled[2 * w + 1])
-                for w in range(n)]
+        return _two_pass(summ, culled, n)
 
     def marg_prepare(self, problems, num_marg=1, want_schur=True):
         """The argument block of one icg_ba_marginalize call (struct array over the problems' host arrays + caller-allocated output arrays):
         what a C++ caller keeps alive across keyframes.  marg_run issues the call, marg_collect turns the outputs into dicts."""
         n = len(problems)
         nm = np.full(n, num_marg, np.int32) if np.isscalar(num_marg) else np.ascontiguousarray(num_marg, np.int32)
-        arr = (BaProblem * n)(*[to_struct(p) for p in problems])
+        arr = _problems(problems)
         pri = (BaPrior * n)()
         bufs = []
         for w, p in enumerate(problems):
@@ -931,10 +851,10 @@ class WindowSolver:
                 b.update(Hp=np.zeros(rcap * rcap), bp=np.zeros(rcap))
             bufs.append(b)
             pri[w].rcap = rcap
-            pri[w].block_type, pri[w].block_node = b["bt"].ctypes.data_as(ip), b["bn"].ctypes.data_as(ip)
-            pri[w].x0, pri[w].J0, pri[w].e0 = b["x0"].ctypes.data_as(dp), b["J0"].ctypes.data_as(dp), b["e0"].ctypes.data_as(dp)
+            pri[w].block_type, pri[w].block_node = b["bt"].ctypes.data_as(i32p), b["bn"].ctypes.data_as(i32p)
+            pri[w].x0, pri[w].J0, pri[w].e0 = b["x0"].ctypes.data_as(f64p), b["J0"].ctypes.data_as(f64p), b["e0"].ctypes.data_as(f64p)
             if want_schur:
-                pri[w].Hp, pri[w].bp = b["Hp"].ctypes.data_as(dp), b["bp"].ctypes.data_as(dp)
+                pri[w].Hp, pri[w].bp = b["Hp"].ctypes.data_as(f64p), b["bp"].ctypes.data_as(f64p)
         return dict(n=n, nm=nm, arr=arr, pri=pri, bufs=bufs, want_schur=want_schur, problems=problems)
 
     def marg_run(self, call, resident=False):

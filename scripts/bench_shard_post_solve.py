@@ -45,9 +45,8 @@ def main():
         raise SystemExit("bench_shard_post_solve.py: no CUDA device; the product path has no CPU fallback")
     from datagen import synth_ba
     import ctypes as C
-    from ic_gvins_b200._lib import check, lib
-    from ic_gvins_b200.ba import BaProblem, BaSummary, CullWindow, WindowSolver, cull_struct, imu_preintegrate, merge_shard, shard_cull_inputs, \
-        shard_window, to_struct, vp
+    from ic_gvins_b200._lib import BaProblem, BaSummary, CullWindow, check, lib, vp
+    from ic_gvins_b200.ba import WindowSolver, cull_struct, imu_preintegrate, merge_shard, shard_cull_inputs, shard_window, to_struct
     from ic_gvins_b200.camera import Camera
     from tests.test_post_solve_gpu import CAMD, STD, cull_inputs
 

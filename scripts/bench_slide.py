@@ -89,8 +89,8 @@ def main():
     import ctypes as C
 
     from datagen.slide_window import build_next
-    from ic_gvins_b200._lib import SlideWindow, check, lib
-    from ic_gvins_b200.ba import BaProblem, BaSummary, WindowSolver, to_struct
+    from ic_gvins_b200._lib import BaProblem, BaSummary, SlideWindow, check, lib
+    from ic_gvins_b200.ba import WindowSolver, to_struct
     K, L, R, n_ref, iters = (20, 2000, 292, 20, 12) if args.cfg4 else (10, 300, 160, 0, 20)
     B = args.windows or (128 if args.cfg4 else 296)
     dev = torch.device("cuda:0")

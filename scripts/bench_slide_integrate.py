@@ -55,8 +55,8 @@ def main():
         raise SystemExit("bench_slide_integrate.py: no CUDA device; the product path has no CPU fallback")
     from datagen import synth_ba
     from datagen.slide_window import build_next
-    from ic_gvins_b200._lib import SlideIntegrate, SlideWindow, check, lib, u8p
-    from ic_gvins_b200.ba import BaProblem, WindowSolver, imu_preintegrate, to_struct
+    from ic_gvins_b200._lib import BaProblem, SlideIntegrate, SlideWindow, check, lib, u8p
+    from ic_gvins_b200.ba import WindowSolver, imu_preintegrate, to_struct
     B, K, L, iters = args.windows, 10, 300, 20
     dev = torch.device("cuda:0")
     cs = torch.cuda.Stream(dev)

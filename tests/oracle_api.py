@@ -56,7 +56,7 @@ def track_fb(lib, a, b, p, init):
 
 # ------------------------------------------------------------------------------------------------ BA oracle
 def declare_ba(lib):
-    from ic_gvins_b200.ba import BaProblem, BaSummary
+    from ic_gvins_b200._lib import BaProblem, BaSummary
     lib.icgo_ba_solve.argtypes = [C.POINTER(BaProblem), vp, vp, C.c_int, C.c_int, C.POINTER(BaSummary)]
     lib.icgo_ba_residual_costs.argtypes = [C.POINTER(BaProblem), vp, vp]
     lib.icgo_preintegrate.argtypes = [vp, vp, vp, vp, vp, C.c_int, vp, vp, vp]
@@ -88,7 +88,8 @@ def preintegrate(lib, state16, iewn, gravity, noise5, imu):
 
 
 def ba_solve(lib, prob, max_iter, num_threads=1):
-    from ic_gvins_b200.ba import BaSummary, to_struct
+    from ic_gvins_b200._lib import BaSummary
+    from ic_gvins_b200.ba import to_struct
     s = to_struct(prob)
     pn = np.ascontiguousarray(prob["pn"], np.float64)
     off = np.ascontiguousarray(prob["pn_off"], np.int32)

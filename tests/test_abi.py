@@ -27,6 +27,19 @@ def test_library_exports_every_declared_symbol():
     assert set(_lib.EXPORTS) == set(names), (set(_lib.EXPORTS) ^ set(names))
 
 
+def test_argtypes_match_header_prototypes():
+    """Every entry of _lib.ABI has as many argtypes as its prototype in include/icgvins_b200.h has parameters (a missing or extra argtype
+    shifts every later argument without an error)."""
+    from ic_gvins_b200 import _lib
+    text = open(os.path.join(ROOT, "include", "icgvins_b200.h")).read()
+    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
+    protos = {name: 0 if params.strip() in ("", "void") else params.count(",") + 1
+              for name, params in re.findall(r"\b(icg_[a-z0-9_]+)\s*\(([^()]*)\)\s*;", text)}
+    assert set(protos) == set(_lib.ABI), set(protos) ^ set(_lib.ABI)
+    wrong = {name: (len(argtypes), protos[name]) for name, (argtypes, _) in _lib.ABI.items() if len(argtypes) != protos[name]}
+    assert not wrong, wrong
+
+
 def test_no_cpu_fallback_without_gpu():
     """Without a CUDA device every create() must fail loudly (ICG_ENODEVICE), never fall back to the oracle."""
     import torch

@@ -309,8 +309,8 @@ def test_chain_solve_redo_pose_track(oracle):
 
     import torch
 
-    from ic_gvins_b200._lib import lib
-    from ic_gvins_b200.ba import BaProblem, WindowSolver, to_struct
+    from ic_gvins_b200._lib import BaProblem, lib
+    from ic_gvins_b200.ba import WindowSolver, to_struct
     from ic_gvins_b200.klt import KltTracker
     from datagen import synth_ba
     from datagen import synth_klt as synth

@@ -164,8 +164,8 @@ def test_split_pipeline_cfg4_window(olib, cam):
 
 
 def _download(s, probs):
-    from ic_gvins_b200._lib import check, lib
-    from ic_gvins_b200.ba import BaProblem, BaSummary, to_struct
+    from ic_gvins_b200._lib import BaProblem, BaSummary, check, lib
+    from ic_gvins_b200.ba import to_struct
     cp = [copy.deepcopy(p) for p in probs]
     arr = (BaProblem * len(cp))(*[to_struct(p) for p in cp])
     summ = (BaSummary * len(cp))()

@@ -283,8 +283,8 @@ def test_zero_noise_rejects_every_factor_and_keeps_the_handle(olib):
 
 
 def test_bad_imu_off_is_refused_before_any_launch(olib):
-    from ic_gvins_b200._lib import lib
-    from ic_gvins_b200.ba import BaProblem, ReintWindow, to_struct
+    from ic_gvins_b200._lib import BaProblem, ReintWindow, lib
+    from ic_gvins_b200.ba import to_struct
     prob, rows = window(olib, 510)
     s = solver_for([prob])
     try:

@@ -249,8 +249,8 @@ def test_contract(olib):
         # non-NULL list inputs on rank 0: rejected before the agreement, every handle unchanged (the NULL lists below are this culling's)
         def rank_lists(r):
             import ctypes as C
-            from ic_gvins_b200._lib import CullLists, lib
-            from ic_gvins_b200.ba import BaProblem, CullWindow, cull_struct, to_struct
+            from ic_gvins_b200._lib import BaProblem, CullLists, CullWindow, lib
+            from ic_gvins_b200.ba import cull_struct, to_struct
             arr = (BaProblem * n)(*[to_struct(p) for p in na[r]])
             keep = [dict(e, obs_factor=np.zeros(3, np.int32)) if (r, w) == (0, 1) else dict(e) for w, e in enumerate(exts)]
             cw = (CullWindow * n)(*[cull_struct(p, ci) for p, ci in zip(na[r], keep)])

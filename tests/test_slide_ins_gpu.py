@@ -318,8 +318,8 @@ def test_abi_rejections_and_sharded_handles(olib):
     stream's INS window stay as they were"""
     import ctypes as C
     from ic_gvins_b200 import IcgError
-    from ic_gvins_b200._lib import SlideIns, SlideWindow, lib
-    from ic_gvins_b200.ba import BaProblem, ReintWindow, to_struct
+    from ic_gvins_b200._lib import BaProblem, ReintWindow, SlideIns, SlideWindow, lib
+    from ic_gvins_b200.ba import to_struct
     p = make(olib, seed=1001, K=8, L=120)
     s1, s2 = solved_pair(p, K=10)
     d, o = ins_pair(2)
