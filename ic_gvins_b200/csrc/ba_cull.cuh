@@ -20,6 +20,10 @@ struct CullWin {  // one window's inputs, as staged
     int obs0;  // first observation of the window in the staged observation arrays
     int node0; // first node of the window in cam_pose
 };
+struct CullSrc {  // where the culling's lists sit: lm_ref_node, obs_off, obs_node, obs_factor, lm_ref_kp, obs_kp
+    const int *ref, *off, *node, *fac;
+    const float *rkp, *kp;
+};
 struct CullOut {  // one window's scalar outputs
     double R_bc[9], t_bc[3], td_bc;
     int ext_accepted, counts[5];

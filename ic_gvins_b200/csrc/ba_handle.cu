@@ -866,7 +866,7 @@ void icg_ba_destroy(icg_ba *h) {
     for (double *p : {h->M.H0, h->M.b0, h->M.G1, h->M.V1, h->M.lam1, h->M.Z})
         if (p) cudaFree(p);
     if (h->slide_old) cudaFree(h->slide_old);
-    for (double *p : {h->store_d[0], h->store_d[1], h->cut_rows})
+    for (double *p : {h->store.d[0], h->store.d[1], h->store.cut})
         if (p) cudaFree(p);
     if (h->ins_ev) cudaEventDestroy(h->ins_ev);
     if (h->fc_alt) cudaFree(h->fc_alt);
@@ -887,10 +887,7 @@ int icg_ba_upload(icg_ba *h, int n, const icg_ba_problem *P) {
     }
     ICG_CUDA(cudaSetDevice(h->device));
     const BaCaps &C = h->C;
-    h->marg_res_n = 0;  // the marginalization workspace no longer belongs to the windows the handle holds
-    h->cull_res_n = 0;
-    h->lists_n = 0;
-    h->store_valid = false;  // the IMU factors are next's now, without samples
+    h->end_results();
     int rc = pack_windows(h, n, P, true);
     if (rc != ICG_OK) return rc;
     rc = upload_structure(h, n);
@@ -1040,7 +1037,7 @@ int icg_ba_shard_export(icg_ba *h, int rank, int world, uint8_t *blob) {
     }
     int rc = split_setup(h, rank, world);
     if (rc != ICG_OK) return rc;
-    h->lists_n = 0;  // joining a group ends the built culling lists
+    h->built.n = 0;  // joining a group ends the built culling lists
     ShardBlob b;
     memset(&b, 0, sizeof(b));
     b.magic = 0x49434753484152ull, b.pid = (uint64_t) getpid(), b.ptr = (uint64_t) (uintptr_t) h->xbuf, b.doubles = h->D.S.off_exp;

@@ -67,9 +67,6 @@ struct icg_ba {
     size_t smem_cam, smem_solve, smem_schur;
     int ld_schur;
     int use_global_S;
-    // the linearisation buffers hold the system of the windows the handle holds, as the last single-GPU LM sequence left it: set when
-    // icg_ba_run / icg_ba_run_gvins enqueue one, cleared by every call that changes the windows after it (icg_ba_peek_linearization reads it)
-    bool lin_ready = false;
     HostDev<icg::WinDims> dims;
     HostDev<icg::LmState> st;
     HostDev<double> pose, mix, ext, rho, imu_blob, imu_U, gnss_blh, gnss_std, lever, pose_prior, pose_prior_sinfo, mix_prior, mix_prior_std, marg_x0,
@@ -109,41 +106,68 @@ struct icg_ba {
     HostDev<int> marg_map;
     HostDev<double> marg_oJ0, marg_oe0, marg_oHp, marg_obp;
     HostDev<uint8_t> marg_fmask;  // factor set of icg_ba_marginalize_resident_culled (ba_lin_vis reads it in place of f_active)
-    HostDev<unsigned char> cull;  // post-solve update + culling: staging [inputs | outputs], grown on demand
-    // the last culling, while it is current (icg_ba_slide_vision_resident reads its lists and flags on the device): its window count (0: none;
-    // an upload, a slide or a sharded culling clears it), every window's slices and observation count, and where its arrays are: the lists
-    // in the culling's staging (host lists) or in the current built lists, the flags in the culling's staging.  cull_res_fac: the built
-    // lists' obs_factor (NULL after a host-list culling, whose obs_factor comes with the slide); cull_res_h*: the built lists' host copies
-    int cull_res_n = 0;
-    std::vector<icg::CullWin> cull_res_win;
-    std::vector<int> cull_res_nobs;
-    const int *cull_res_ref = nullptr, *cull_res_off = nullptr, *cull_res_node = nullptr, *cull_res_fac = nullptr;
-    const float *cull_res_rkp = nullptr, *cull_res_kp = nullptr;
-    const uint8_t *cull_res_lmo = nullptr, *cull_res_obso = nullptr;
-    const int *cull_res_href = nullptr, *cull_res_hoff = nullptr, *cull_res_hnode = nullptr, *cull_res_hfac = nullptr;
-    // the next culling's lists, built by icg_ba_slide_vision_resident (sharded: icg_ba_shard_slide_vision_resident, the rank's next shard's)
-    // into lists[lists_cur ^ 1] and current from its commit until an upload, any other slide or a shard export (lists_n: their window count,
-    // 0: none).  Each buffer is [lm_ref_node | obs_off | obs_node | obs_factor |
-    // lm_ref_kp | obs_kp] at lists_at; window w's slices are lists_win[w] (lm0, off0, obs0, K, L) with lists_nobs[w] entries, the arrays sized
-    // by the slide's bounds (lists_nL landmarks, lists_nO observations)
-    struct ListAt {
-        size_t ref, off, node, fac, rkp, kp, end;
-    };
-    HostDev<unsigned char> lists[2];
-    ListAt lists_at[2] = {};
-    int lists_cur = 0, lists_n = 0;
-    size_t lists_nL = 0, lists_nO = 0;
-    std::vector<icg::CullWin> lists_win;
-    std::vector<int> lists_nobs;
+    HostDev<unsigned char> cull;   // post-solve update + culling: staging [inputs | outputs], grown on demand
     HostDev<unsigned char> vis;    // icg_ba_slide_vision_resident's staging, grown on demand
     HostDev<unsigned char> reint;  // the reintegration's staging, grown on demand
-    // the last resident marginalization, while its workspace (marg_oJ0 / marg_oe0) is the prior of the windows the handle holds: its window
-    // count (0: none; an upload, a slide or another marginalization clears it) and every window's m, r and number of remained blocks.
-    // marg_res_sharded: it was the sharded resident marginalization of a shard group; the prior of window w is then in the workspace of mx_h
-    // (slot (w - rank) / world) on its owner, and m = r = nblocks = 0 is kept for the windows another rank owns
-    int marg_res_n = 0;
-    bool marg_res_sharded = false;
-    std::vector<int> marg_res_m, marg_res_r, marg_res_nb;
+    // ---- the keyframe cycle's results, each current from its one writer until it ends; a call rejected before that point leaves it as it
+    //      was.  "Replaced": end_results, which icg_ba_upload calls after its argument check, and every slide once all its checks have passed
+    void end_results() { culled.n = 0, built.n = 0, prior.n = 0, store.valid = false; }
+    // the linearisation buffers hold the last single-GPU LM sequence's system (icg_ba_peek_linearization): made current by icg_ba_run /
+    // icg_ba_run_gvins; ended by pack_windows (an upload, a slide) and at the start of every culling, marginalization and reintegration launch
+    bool lin_ready = false;
+    // the last culling (sharded: of the rank's shard; icg_ba_slide_vision_resident, icg_ba_marginalize_resident_culled): made current by a
+    // successful cull_run; ended at cull_run's start and when replaced.  Window w's slices: win[w], nobs[w] observations.  Lists: dev (the
+    // culling's staging with fac NULL, or the built lists), host (the built lists' host copies, else NULL); flags: the culling's staging
+    struct CullResult {
+        int n = 0;  // windows (0: none)
+        std::vector<icg::CullWin> win;
+        std::vector<int> nobs;
+        icg::CullSrc dev{};
+        const uint8_t *lm_outlier = nullptr, *obs_outlier = nullptr;
+        icg::CullSrc host{};
+    } culled;
+    // the next culling's lists, built by icg_ba_slide_vision_resident (sharded: the rank's next shard's) into buf[cur ^ 1]: made current at
+    // the end of vision_body, after its slide's commit; ended when replaced and by a shard export.  Each buffer is [lm_ref_node | obs_off |
+    // obs_node | obs_factor | lm_ref_kp | obs_kp] at at[], sized by the slide's bounds (nL landmarks, nO observations); window w's slices are
+    // win[w], with nobs[w] entries.  dev() / host(): the current buffer's lists / their host copies (a culling on them writes those)
+    struct BuiltLists {
+        struct At { size_t ref, off, node, fac, rkp, kp, end; };
+        HostDev<unsigned char> buf[2];
+        At at[2] = {};
+        int cur = 0, n = 0;  // n: windows (0: none)
+        size_t nL = 0, nO = 0;
+        std::vector<icg::CullWin> win;
+        std::vector<int> nobs;
+        icg::CullSrc dev() const { return slices(buf[cur].d); }
+        icg::CullSrc host() const { return slices(buf[cur].h); }
+        icg::CullSrc slices(const unsigned char *p) const {
+            const At &a = at[cur];
+            return {(const int *) (p + a.ref), (const int *) (p + a.off), (const int *) (p + a.node), (const int *) (p + a.fac),
+                    (const float *) (p + a.rkp), (const float *) (p + a.kp)};
+        }
+    } built;
+    // the last resident marginalization, while its workspace (marg_oJ0 / marg_oe0) is the prior of the windows the handle holds (a slide's
+    // prior_from_marg reads it): made current by prior_commit; ended by every marginalization before it writes the workspace, and when
+    // replaced.  m, r, nb: every window's m, r and remained blocks.  sharded: a shard group's; window w's prior is then in the workspace of
+    // mx_h (slot (w - rank) / world) on its owner, and the windows another rank owns keep m = r = nb = 0
+    struct ResidentPrior {
+        int n = 0;  // windows (0: none)
+        bool sharded = false;
+        std::vector<int> m, r, nb;
+    } prior;
+    // every IMU factor's samples (imu_buffer_): rows (dt, dtheta[3], dvel[3]) window after window, factor after factor, in d[cur].  store_build
+    // cuts the next store from the INS windows into the other buffer; store_commit makes it current when icg_ba_imu_samples_from_ins or
+    // icg_ba_slide_ins_resident (after its slide) commits.  Ended when replaced
+    struct SampleStore {
+        double *d[2] = {nullptr, nullptr};
+        size_t cap[2] = {0, 0};  // rows
+        int cur = 0;
+        bool valid = false;
+        std::vector<std::vector<int>> row0, nrow;  // per window and factor: first row, row count (-1: the factor has no samples)
+        HostDev<unsigned char> stage;              // [cut jobs | row counts | statuses | gather segments], grown on demand
+        double *cut = nullptr;                     // the series cut out of the INS windows, before the gather
+        size_t cut_cap = 0;                        // rows
+    } store;
     // icg_ba_slide_resident: staging (grown on demand), the copy of the old value rows, the second f_const_s buffer
     HostDev<unsigned char> slide;
     double *slide_old = nullptr, *fc_alt = nullptr;
@@ -151,18 +175,7 @@ struct icg_ba {
     // icg_ba_upload from the landmark's first factor, carried by every slide, read by icg_ba_slide_vision_resident
     double *lm_ref = nullptr, *lm_ref_alt = nullptr;
     cudaEvent_t slide_ev = nullptr;  // recorded after the staging's H2D
-    // every IMU factor's samples (imu_buffer_), filled from the INS windows by icg_ba_imu_samples_from_ins / icg_ba_slide_ins_resident.  Rows
-    // (dt, dtheta[3], dvel[3]) window after window, factor after factor, in store_d[store_cur]; a call builds the next store in the other
-    // buffer and swaps only when it commits.  Valid while no upload or other slide has replaced the windows' structure since the last fill
-    double *store_d[2] = {nullptr, nullptr};
-    size_t store_cap[2] = {0, 0};  // rows
-    int store_cur = 0;
-    bool store_valid = false;
-    std::vector<std::vector<int>> store_row0, store_nrow;  // per window and factor: first row, row count (-1: the factor has no samples)
-    HostDev<unsigned char> store_stage;                    // [cut jobs | row counts | statuses | gather segments], grown on demand
-    double *cut_rows = nullptr;                            // the series cut out of the INS windows, before the gather
-    size_t cut_cap = 0;                                    // rows
-    cudaEvent_t ins_ev = nullptr;                          // recorded on the INS handle's stream, waited on by this one
+    cudaEvent_t ins_ev = nullptr;    // recorded on the INS handle's stream, waited on by this one (the sample store's cuts)
     // post-solve calls of a shard group (world > 1): integer exchanges so far (slot parity), epoch of the last marginalization export, the
     // exchange's device word, the export's slot lists, the owner's gathered rows with their tables, and the handle the owner uploads its
     // gathered windows to (created on first use, recreated when a batch needs more landmarks, factors or windows)

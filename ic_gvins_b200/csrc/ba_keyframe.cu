@@ -92,6 +92,14 @@ static int marg_grow(icg_ba *h, int n, int max_m, int max_n0) {
     return ICG_OK;
 }
 
+// a resident marginalization succeeded: its record of windows first, first + step, ... (step > 1: those a shard group's rank owns)
+static void prior_commit(icg_ba *h, int n, const icg_ba_prior *out, int first, int step) {
+    icg_ba::ResidentPrior &P = h->prior;
+    P.m.assign(n, 0), P.r.assign(n, 0), P.nb.assign(n, 0);
+    for (int w = first; w < n; w += step) P.m[w] = out[w].m, P.r[w] = out[w].r, P.nb[w] = out[w].nblocks;
+    P.n = n, P.sharded = step > 1;
+}
+
 // fmask (resident only, may be NULL): per window, the factor set to marginalize in place of the problem's activity (F bytes each); it reaches
 // ba_lin_vis through a copy of the device view, so the handle's own f_active is never written.
 // agree (may be NULL): called once the structure is known, with {largest m, largest r, 1 if a window is rejected} of this batch; it returns
@@ -108,7 +116,7 @@ static int marginalize_body(icg_ba *h, int n_windows, const icg_ba_problem *prob
         return ICG_EUNSUPPORTED;
     }
     int rc = ICG_OK;
-    h->marg_res_n = 0;  // the workspace is about to be overwritten: it is the resident prior again only if this call is resident and succeeds
+    h->prior.n = 0;  // the workspace is about to be overwritten: it is the resident prior again only if this call is resident and succeeds
     h->lin_ready = false;  // its linearisation takes the buffer the window uses
     if (resident) {
         // the windows of the last upload / solve are still on the device (parameters at their optimised values, factor activity and GNSS
@@ -306,11 +314,7 @@ static int marginalize_body(icg_ba *h, int n_windows, const icg_ba_problem *prob
         worker(0);
         for (auto &x : th) x.join();
     }
-    if (resident) {  // icg_ba_slide_resident(prior_from_marg = 1) takes this prior from the workspace
-        h->marg_res_m.resize(n), h->marg_res_r.resize(n), h->marg_res_nb.resize(n);
-        for (int w = 0; w < n; w++) h->marg_res_m[w] = out[w].m, h->marg_res_r[w] = out[w].r, h->marg_res_nb[w] = out[w].nblocks;
-        h->marg_res_n = n, h->marg_res_sharded = false;
-    }
+    if (resident) prior_commit(h, n, out, 0, 1);  // icg_ba_slide_resident(prior_from_marg = 1) takes this prior from the workspace
     return ICG_OK;
 }
 
@@ -430,15 +434,10 @@ static int marginalize_sharded(icg_ba *h, int n, const icg_ba_problem *problems,
     count_launch();
     for (int w = 0; w < n; w++)
         if (w % G != R) out[w].m = out[w].r = out[w].nblocks = 0;
-    h->marg_res_n = 0;  // the workspace is about to be overwritten: the sharded slide's prior again only if this call succeeds
+    h->prior.n = 0;  // the workspace is about to be overwritten: the sharded slide's prior again only if this call succeeds
     // on success: the record icg_ba_shard_slide[_integrate]_resident checks (every rank: a sharded resident marginalization of these n
     // windows; the owner: each owned window's m, r, nblocks)
-    auto record = [&]() {
-        h->marg_res_m.assign(n, 0), h->marg_res_r.assign(n, 0), h->marg_res_nb.assign(n, 0);
-        for (int w = R; w < n; w += G) h->marg_res_m[w] = out[w].m, h->marg_res_r[w] = out[w].r, h->marg_res_nb[w] = out[w].nblocks;
-        h->marg_res_n = n, h->marg_res_sharded = true;
-        return ICG_OK;
-    };
+    auto record = [&]() { prior_commit(h, n, out, R, G); return ICG_OK; };
     // an owner that fails from here joins the group's agreement on the eigensolver sizes with a rejection, so that no peer waits for it
     auto reject = [&](int code) {
         int mx[3] = {0, 0, 1};
@@ -505,7 +504,7 @@ static int marginalize_sharded(icg_ba *h, int n, const icg_ba_problem *problems,
     rc = pack_windows(mh, n_own, gp.data(), false);
     if (rc == ICG_OK) rc = upload_structure(mh, n_own);
     if (rc != ICG_OK) return reject(rc);
-    mh->cur_windows = n_own, mh->marg_res_n = 0;
+    mh->cur_windows = n_own, mh->end_results();
     ICG_CUDA(mh->lm_fidx.up(s, (size_t) n_own * mh->C.F));
     ba_marg_fill<<<n_own, 128, 0, s>>>(mh->C, mh->D, C, h->D, h->mx_rows, h->mx_row.d + (size_t) n_own * G, mh->lm_fidx.d);
     ICG_CHECK_LAUNCH();
@@ -767,15 +766,15 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
                     return fail(ICG_EINVAL);
                 }
         if (!carry[w].prior_from_marg) continue;
-        if (h->marg_res_n != n || h->marg_res_sharded != sharded) {
+        if (h->prior.n != n || h->prior.sharded != sharded) {
             set_error("%s: window %d takes its prior from the marginalization, but no %sresident marginalization of these %d windows "
                       "ran since the last upload or slide", fn, w, sharded ? "sharded " : "", n);
             return fail(ICG_EINVAL);
         }
         if (sharded && w % G != R) continue;  // the owner holds the window's m, r and nblocks
-        if (h->marg_res_m[w] <= 0 || p.marg_r != h->marg_res_r[w] || p.marg_nblocks != h->marg_res_nb[w]) {
+        if (h->prior.m[w] <= 0 || p.marg_r != h->prior.r[w] || p.marg_nblocks != h->prior.nb[w]) {
             set_error("%s: window %d: marg_r=%d / marg_nblocks=%d, but the resident marginalization left m=%d, r=%d / nblocks=%d", fn, w,
-                      p.marg_r, p.marg_nblocks, h->marg_res_m[w], h->marg_res_r[w], h->marg_res_nb[w]);
+                      p.marg_r, p.marg_nblocks, h->prior.m[w], h->prior.r[w], h->prior.nb[w]);
             return fail(ICG_EINVAL);
         }
     }
@@ -1127,10 +1126,7 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
         if (irc != ICG_OK) return fail(irc);
     }
     // every check has passed: from here on the device is written
-    h->marg_res_n = 0;
-    h->cull_res_n = 0;
-    h->lists_n = 0;          // icg_ba_slide_vision_resident makes the lists it built current when this returns
-    h->store_valid = false;  // icg_ba_slide_ins_resident sets it again when it commits its store
+    h->end_results();
     if (iwins.empty()) ICG_CUDA(cudaMemcpyAsync(h->slide.d, h->slide.h, in_end, cudaMemcpyHostToDevice, s));
     ICG_CUDA(cudaEventRecord(h->slide_ev, s));
     rc = upload_structure(h, n);
@@ -1188,7 +1184,8 @@ static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_b
         set_error("%s: bad arguments", fn);
         return reject(ICG_EINVAL);
     }
-    if (h->cull_res_n != n) {
+    const icg_ba::CullResult &cul = h->culled;
+    if (cul.n != n) {
         set_error("%s: no culling of these %d windows is current (icg_ba_update_and_cull_resident, with no upload or slide since)", fn, n);
         return reject(ICG_EINVAL);
     }
@@ -1202,13 +1199,13 @@ static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_b
         const icg_ba_problem &p = next[w];
         const icg_ba_slide_vision &v = vis[w];
         const WinDims &od = h->dims.h[w];
-        const CullWin &cw = h->cull_res_win[w];
-        const int nco = h->cull_res_nobs[w];
+        const CullWin &cw = cul.win[w];
+        const int nco = cul.nobs[w];
         bool bad = p.K < 2 || p.K > C.K || v.num_marg < 0 || v.num_marg > od.K || !v.node_in_map || !v.node_td || v.cur_node < 0 || v.cur_node >= p.K ||
                    v.n_frames < 0 || v.n_frames > VIS_MAX_FRAMES || (v.n_frames > 0 && (!v.frame_id || !v.frame_node)) || v.n_obs < 0 || v.n_new < 0 ||
                    (v.obs_src && v.n_in < 0) || (v.n_obs > 0 && (!v.obs_lm || !v.obs_undis_xy || !v.obs_vel)) ||
                    (v.n_new > 0 && (!v.new_depth || !v.new_vel_ref || !v.new_vel_cur || !v.new_ref_undis_xy || !v.new_cur_undis_xy || !v.new_ref_frame_id)) ||
-                   (nco > 0 && !v.obs_factor && !h->cull_res_fac) || cw.K != od.K || cw.L != od.L;
+                   (nco > 0 && !v.obs_factor && !cul.dev.fac) || cw.K != od.K || cw.L != od.L;
         for (int e = 0; !bad && e < v.n_frames; e++) bad = v.frame_node[e] < 0 || v.frame_node[e] >= p.K;
         if (bad) {
             set_error("%s: window %d: arguments out of range or arrays missing", fn, w);
@@ -1255,17 +1252,17 @@ static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_b
         if (cudaError_t e = cudaStreamSynchronize(s)) return cuda_fail(e, "cudaStreamSynchronize");
     if ((rc = hd_reserve(h, h->vis, lay.size(), fn)) != ICG_OK) return reject(rc);
     // the next culling's lists (sharded: the rank's next shard's) go to the buffer that is not current
-    const int nb = h->lists_cur ^ 1;
-    icg_ba::ListAt at{};
+    const int nb = h->built.cur ^ 1;
+    icg_ba::BuiltLists::At at{};
     {
         Layout ll;
         at.ref = ll.take(4 * n_lm), at.off = ll.take(4 * (n_lm + n)), at.node = ll.take(4 * n_lo), at.fac = ll.take(4 * n_lo);
         at.rkp = ll.take(8 * n_lm), at.kp = ll.take(8 * n_lo), at.end = ll.size();
-        if ((rc = hd_reserve(h, h->lists[nb], at.end, fn)) != ICG_OK) return reject(rc);
+        if ((rc = hd_reserve(h, h->built.buf[nb], at.end, fn)) != ICG_OK) return reject(rc);
     }
     unsigned char *H = h->vis.h, *Dv = h->vis.d;
     for (int w = 0; w < n; w++) {
-        wins[w].obs_factor = ofac_at[w] >= 0 ? (const int *) (Dv + b_ofac) + ofac_at[w] : h->cull_res_fac + h->cull_res_win[w].obs0;
+        wins[w].obs_factor = ofac_at[w] >= 0 ? (const int *) (Dv + b_ofac) + ofac_at[w] : cul.dev.fac + cul.win[w].obs0;
         if (ofac_at[w] >= 0 && wins[w].n_cull_obs > 0) memcpy(H + b_ofac + 4 * (size_t) ofac_at[w], vis[w].obs_factor, 4 * (size_t) wins[w].n_cull_obs);
     }
     memcpy(H + b_win, wins.data(), sizeof(VisWin) * n);
@@ -1273,12 +1270,12 @@ static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_b
     a.win = (const VisWin *) (Dv + b_win), a.K = C.K, a.L = C.L, a.F = C.F;
     a.rank = sharded ? h->D.rank : 0, a.world = sharded ? h->D.world : 1;
     a.rho = h->D.rho, a.lm_ref = h->lm_ref, a.lm_ref_next = h->lm_ref_alt, a.f_meta_s = h->D.f_meta_s, a.lm_off = h->D.lm_off, a.lm_perm = h->D.lm_perm;
-    a.lm_ref_node = h->cull_res_ref, a.obs_off = h->cull_res_off, a.obs_node = h->cull_res_node, a.lm_ref_kp = h->cull_res_rkp, a.obs_kp = h->cull_res_kp;
-    a.lm_outlier = h->cull_res_lmo, a.obs_outlier = h->cull_res_obso;
+    a.lm_ref_node = cul.dev.ref, a.obs_off = cul.dev.off, a.obs_node = cul.dev.node, a.lm_ref_kp = cul.dev.rkp, a.obs_kp = cul.dev.kp;
+    a.lm_outlier = cul.lm_outlier, a.obs_outlier = cul.obs_outlier;
     a.counts = (int *) (Dv + b_cnt), a.lm_src = (int *) (Dv + b_lms), a.lm_org = (int *) (Dv + b_org), a.lm_nan = Dv + b_nan, a.f_lm = (int *) (Dv + b_flm), a.f_ref = (int *) (Dv + b_fref);
     a.f_obs = (int *) (Dv + b_fobs), a.f_src = (int *) (Dv + b_fsrc), a.invdepth = (double *) (Dv + b_invd), a.f_new = (double *) (Dv + b_fnew);
     a.scratch = (int *) (Dv + b_scr);
-    unsigned char *Dl = h->lists[nb].d;
+    unsigned char *Dl = h->built.buf[nb].d;
     a.l_ref = (int *) (Dl + at.ref), a.l_off = (int *) (Dl + at.off), a.l_node = (int *) (Dl + at.node), a.l_fac = (int *) (Dl + at.fac);
     a.l_rkp = (float *) (Dl + at.rkp), a.l_kp = (float *) (Dl + at.kp);
     cudaError_t e = cudaMemcpyAsync(Dv, H, in_end, cudaMemcpyHostToDevice, s);
@@ -1341,8 +1338,8 @@ static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_b
     }
     rc = slide_body(h, n, nx.data(), cr.data(), integ, noise5, station3, fn, sharded, true, sharded ? &fp : nullptr, fr);
     if (rc != ICG_OK) return rc;  // sharded: the group's agreement inside slide_body has committed every rank's slide, or none
-    h->lists_cur = nb, h->lists_at[nb] = at, h->lists_n = n, h->lists_nL = n_lm, h->lists_nO = n_lo;
-    h->lists_win = std::move(lw), h->lists_nobs = std::move(lnobs);
+    icg_ba::BuiltLists &B = h->built;
+    B.cur = nb, B.at[nb] = at, B.n = n, B.nL = n_lm, B.nO = n_lo, B.win = std::move(lw), B.nobs = std::move(lnobs);
     return ICG_OK;
 }
 
@@ -1382,11 +1379,12 @@ static int grow_rows(double *&d, size_t &cap, size_t rows, cudaStream_t s, const
     return ICG_OK;
 }
 
-// The next store from src (per window and factor) into store_d[1 - store_cur] and its tables into row0 / nrow; the current store, its
-// tables and the INS windows are not changed.  The cut runs on this handle's stream after the work queued on the INS handle's stream, and
-// has completed when this returns.  Jobs the INS windows cannot serve are listed in bad (window, factor), with ICG_EINVAL naming the first.
+// The next store from src (per window and factor) into d[1 - cur] and its tables into row0 / nrow; the current store, its tables and the
+// INS windows are not changed.  The cut runs on this handle's stream after the work queued on the INS handle's stream, and has completed
+// when this returns.  Jobs the INS windows cannot serve are listed in bad (window, factor), with ICG_EINVAL naming the first.
 static int store_build(icg_ba *h, const icg_ins *ins, const std::vector<std::vector<StoreSrc>> &src, const char *fn, std::vector<std::vector<int>> &row0,
                        std::vector<std::vector<int>> &nrow, std::vector<std::pair<int, int>> &bad) {
+    icg_ba::SampleStore &S = h->store;
     const int n = (int) src.size();
     std::vector<InsCutJob> jobs;
     std::vector<std::pair<int, int>> job_of;
@@ -1408,10 +1406,10 @@ static int store_build(icg_ba *h, const icg_ins *ins, const std::vector<std::vec
     Layout lay;
     const size_t b_job = lay.take(sizeof(InsCutJob) * nj), b_n = lay.take(4 * nj), b_st = lay.take(4 * nj), b_seg = lay.take(sizeof(StoreSeg) * 2 * n_fac);
     cudaStream_t s = h->stream;
-    int rc = hd_reserve(h, h->store_stage, lay.size(), fn);  // every call of the store synchronises before it returns: the old one is idle
+    int rc = hd_reserve(h, S.stage, lay.size(), fn);  // every call of the store synchronises before it returns: the old one is idle
     if (rc != ICG_OK) return rc;
-    if ((rc = grow_rows(h->cut_rows, h->cut_cap, cut_rows, s, fn)) != ICG_OK) return rc;
-    unsigned char *H = h->store_stage.h, *Dv = h->store_stage.d;
+    if ((rc = grow_rows(S.cut, S.cut_cap, cut_rows, s, fn)) != ICG_OK) return rc;
+    unsigned char *H = S.stage.h, *Dv = S.stage.d;
     const int32_t *got_n = (const int32_t *) (H + b_n), *got_st = (const int32_t *) (H + b_st);
     if (nj > 0) {
         memcpy(H + b_job, jobs.data(), sizeof(InsCutJob) * nj);
@@ -1419,7 +1417,7 @@ static int store_build(icg_ba *h, const icg_ins *ins, const std::vector<std::vec
         if (!h->ins_ev) ICG_CUDA(cudaEventCreateWithFlags(&h->ins_ev, cudaEventDisableTiming));
         ICG_CUDA(cudaEventRecord(h->ins_ev, ins->stream));  // the pushes and redos queued on the INS handle come first
         ICG_CUDA(cudaStreamWaitEvent(s, h->ins_ev, 0));
-        ICG_CUDA(ins_cut_launch(ins, (int) nj, (const InsCutJob *) Dv, h->cut_rows, (int32_t *) (Dv + b_n), (int32_t *) (Dv + b_st), s));
+        ICG_CUDA(ins_cut_launch(ins, (int) nj, (const InsCutJob *) Dv, S.cut, (int32_t *) (Dv + b_n), (int32_t *) (Dv + b_st), s));
         ICG_CUDA(cudaMemcpyAsync(H + b_n, Dv + b_n, b_seg - b_n, cudaMemcpyDeviceToHost, s));
         ICG_CUDA(cudaStreamSynchronize(s));
         for (size_t q = 0; q < nj; q++)
@@ -1444,13 +1442,13 @@ static int store_build(icg_ba *h, const icg_ins *ins, const std::vector<std::vec
             if (f.kind == STORE_CUT) {
                 m = got_n[q];
                 segs.push_back(StoreSeg{0, jobs[q++].out, at, m});
-            } else if (f.kind == STORE_OLD && h->store_nrow[w][f.a] >= 0) {
-                m = h->store_nrow[w][f.a];
-                segs.push_back(StoreSeg{1, h->store_row0[w][f.a], at, m});
+            } else if (f.kind == STORE_OLD && S.nrow[w][f.a] >= 0) {
+                m = S.nrow[w][f.a];
+                segs.push_back(StoreSeg{1, S.row0[w][f.a], at, m});
             } else if (f.kind == STORE_MERGE) {
-                const int na = h->store_nrow[w][f.a], nb = h->store_nrow[w][f.a + 1];
-                segs.push_back(StoreSeg{1, h->store_row0[w][f.a], at, na});
-                if (nb > 1) segs.push_back(StoreSeg{1, h->store_row0[w][f.a + 1] + 1, at + na, nb - 1});
+                const int na = S.nrow[w][f.a], nb = S.nrow[w][f.a + 1];
+                segs.push_back(StoreSeg{1, S.row0[w][f.a], at, na});
+                if (nb > 1) segs.push_back(StoreSeg{1, S.row0[w][f.a + 1] + 1, at + na, nb - 1});
                 m = na + nb - 1;
             }
             if (m < 0) continue;
@@ -1462,22 +1460,22 @@ static int store_build(icg_ba *h, const icg_ins *ins, const std::vector<std::vec
         set_error("%s: too many IMU rows in one call", fn);
         return ICG_EINVAL;
     }
-    const int nx = 1 - h->store_cur;
-    if ((rc = grow_rows(h->store_d[nx], h->store_cap[nx], total, s, fn)) != ICG_OK) return rc;
+    const int nx = 1 - S.cur;
+    if ((rc = grow_rows(S.d[nx], S.cap[nx], total, s, fn)) != ICG_OK) return rc;
     if (segs.empty()) return ICG_OK;
     memcpy(H + b_seg, segs.data(), sizeof(StoreSeg) * segs.size());
     ICG_CUDA(cudaMemcpyAsync(Dv + b_seg, H + b_seg, sizeof(StoreSeg) * segs.size(), cudaMemcpyHostToDevice, s));
-    ba_store_gather_kernel<<<(unsigned) ((segs.size() + 3) / 4), 128, 0, s>>>((int) segs.size(), (const StoreSeg *) (Dv + b_seg), h->cut_rows,
-                                                                             h->store_d[h->store_cur], h->store_d[nx]);
+    ba_store_gather_kernel<<<(unsigned) ((segs.size() + 3) / 4), 128, 0, s>>>((int) segs.size(), (const StoreSeg *) (Dv + b_seg), S.cut, S.d[S.cur],
+                                                                             S.d[nx]);
     ICG_CHECK_LAUNCH();
     count_launch();
     return ICG_OK;
 }
 
 static void store_commit(icg_ba *h, std::vector<std::vector<int>> &row0, std::vector<std::vector<int>> &nrow) {
-    h->store_cur = 1 - h->store_cur;
-    h->store_row0.swap(row0), h->store_nrow.swap(nrow);
-    h->store_valid = true;
+    h->store.cur = 1 - h->store.cur;
+    h->store.row0.swap(row0), h->store.nrow.swap(nrow);
+    h->store.valid = true;
 }
 
 // the checks every call that cuts from the INS windows shares
@@ -1522,15 +1520,11 @@ static int cut_window_ok(const icg_ins *ins, int w, int stream, const double *no
 
 // ---- the culling (ba_cull.cu) of both entries: staging [windows | host lists] in, [windows | cam_pose | lm_pw | lm_depth | lm_outlier |
 //      obs_outlier] out, one launch, one synchronisation, the outputs into io.  win[w]'s slices index the lists and the outputs alike.
-//      built: the lists the last vision slide built (lists_nL landmarks, lists_nO observations); NULL: io's host lists, staged here.
-//      Records where the culling's lists and flags sit for icg_ba_slide_vision_resident.
-struct CullSrc {
-    const int *ref, *off, *node, *fac;
-    const float *rkp, *kp;
-};
+//      built: the current built lists (nL landmarks, nO observations), copied back to the host with the outputs (with their keypoints
+//      when want_kp); NULL: io's host lists, staged here.  Makes the culling current.
 static int cull_run(icg_ba *h, int n, const icg_ba_problem *problems, const icg_camera *cam, double std, icg_ba_cull_window *io,
-                    const std::vector<CullWin> &win, const std::vector<int> &nobs, size_t nL, size_t nO, size_t nK, const CullSrc *built,
-                    const char *fn) {
+                    const std::vector<CullWin> &win, const std::vector<int> &nobs, size_t nL, size_t nO, size_t nK,
+                    const icg_ba::BuiltLists *built, bool want_kp, const char *fn) {
     const BaCaps &C = h->C;
     const size_t sL = built ? 0 : nL, sO = built ? 0 : nO;  // the host lists' staging
     Layout lay;
@@ -1540,7 +1534,7 @@ static int cull_run(icg_ba *h, int n, const icg_ba_problem *problems, const icg_
     const size_t o_win = lay.take(sizeof(CullOut) * n), o_pose = lay.take(96 * nK), o_pw = lay.take(24 * nL), o_depth = lay.take(8 * nL),
                  o_lmo = lay.take(nL), o_obso = lay.take(nO);
     const size_t out_bytes = lay.size() - in_bytes;
-    h->cull_res_n = 0;  // the staging is rewritten (or replaced) from here
+    h->culled.n = 0;  // the staging is rewritten (or replaced) from here
     h->lin_ready = false;  // parameters and factor activity change
     ICG_CUDA(cudaSetDevice(h->device));
     cudaStream_t s = h->stream;
@@ -1564,7 +1558,7 @@ static int cull_run(icg_ba *h, int n, const icg_ba_problem *problems, const icg_
         if (no > 0) memcpy(H + i_node + 4 * (size_t) W.obs0, c.obs_node, 4 * (size_t) no), memcpy(H + i_kp + 8 * (size_t) W.obs0, c.obs_kp, 8 * (size_t) no);
     }
     ICG_CUDA(cudaMemcpyAsync(Dv, H, in_bytes, cudaMemcpyHostToDevice, s));
-    const CullSrc src = built ? *built
+    const CullSrc src = built ? built->dev()
                               : CullSrc{(const int *) (Dv + i_ref), (const int *) (Dv + i_off), (const int *) (Dv + i_node), nullptr,
                                         (const float *) (Dv + i_rkp), (const float *) (Dv + i_kp)};
     CullArgs a;
@@ -1580,13 +1574,14 @@ static int cull_run(icg_ba *h, int n, const icg_ba_problem *problems, const icg_
         if (rc != ICG_OK) return rc;
     }
     ICG_CUDA(cudaMemcpyAsync(H + in_bytes, Dv + in_bytes, out_bytes, cudaMemcpyDeviceToHost, s));
+    if (built) {  // the integer lists on the host (icg_ba_marginalize_resident_culled's NULL lists read them there), the keypoints if asked
+        const HostDev<unsigned char> &lb = built->buf[built->cur];
+        const icg_ba::BuiltLists::At &at = built->at[built->cur];
+        ICG_CUDA(cudaMemcpyAsync(lb.h, lb.d, want_kp ? at.end : at.rkp, cudaMemcpyDeviceToHost, s));
+    }
     ICG_CUDA(cudaStreamSynchronize(s));
     if (h->D.world > 1 && (rc = shard_timed_out(h, fn)) != ICG_OK) return rc;
-    // where the lists and flags sit, for vision_body (sharded: the rank's own shard's)
-    h->cull_res_n = n, h->cull_res_win = win, h->cull_res_nobs = nobs;
-    h->cull_res_ref = src.ref, h->cull_res_off = src.off, h->cull_res_node = src.node, h->cull_res_fac = src.fac;
-    h->cull_res_rkp = src.rkp, h->cull_res_kp = src.kp, h->cull_res_lmo = Dv + o_lmo, h->cull_res_obso = Dv + o_obso;
-    h->cull_res_href = h->cull_res_hoff = h->cull_res_hnode = h->cull_res_hfac = nullptr;
+    h->culled = {n, win, nobs, src, Dv + o_lmo, Dv + o_obso, built ? built->host() : CullSrc{}};
     for (int w = 0; w < n; w++) {
         const icg_ba_problem &p = problems[w];
         icg_ba_cull_window &c = io[w];
@@ -1612,14 +1607,14 @@ static int cull_run(icg_ba *h, int n, const icg_ba_problem *problems, const icg_
 static int cull_built_body(icg_ba *h, int n, const icg_ba_problem *problems, const icg_camera *cam, double reprojection_error_std,
                            icg_ba_cull_window *io, icg_ba_cull_lists *lists, const char *fn, bool sharded) {
     auto reject = [&](int code) { return sharded ? shard_agree(h, true, 0, fn) : code; };
-    // lists_n is 0 or the uploaded count, so a call over another window count fails here already
+    // built.n is 0 or the uploaded count, so a call over another window count fails here already
     int rc = resident_single_rank(h, n, problems, fn, sharded);
     if (rc != ICG_OK) return reject(rc);
     if (!cam || !io) {
         set_error("%s: bad arguments", fn);
         return reject(ICG_EINVAL);
     }
-    if (h->lists_n != n) {
+    if (h->built.n != n) {
         set_error("%s: no built lists of these %d windows are current (%s, with no upload or other slide since)", fn, n,
                   sharded ? "icg_ba_shard_slide_vision_resident" : "icg_ba_slide_vision_resident");
         return reject(ICG_EINVAL);
@@ -1632,8 +1627,8 @@ static int cull_built_body(icg_ba *h, int n, const icg_ba_problem *problems, con
     for (int w = 0; w < n; w++) {
         const icg_ba_problem &p = problems[w];
         const icg_ba_cull_window &c = io[w];
-        const CullWin &lw = h->lists_win[w];
-        const int no = h->lists_nobs[w];
+        const CullWin &lw = h->built.win[w];
+        const int no = h->built.nobs[w];
         // the caller's observation arrays hold max_L + max_F entries: lists not shaped as the reference builds them (an entry listed twice
         // in the host lists the slide carried) can be longer
         if (no > C.L + C.F) {
@@ -1658,31 +1653,21 @@ static int cull_built_body(icg_ba *h, int n, const icg_ba_problem *problems, con
     if (sharded && (rc = shard_agree(h, false, fp.get(), fn)) != ICG_OK) return rc;
     bool want_kp = false;
     for (int w = 0; lists && w < n; w++) want_kp = want_kp || lists[w].lm_ref_kp || lists[w].obs_kp;
-    HostDev<unsigned char> &lb = h->lists[h->lists_cur];
-    const icg_ba::ListAt &at = h->lists_at[h->lists_cur];
-    const CullSrc src{(const int *) (lb.d + at.ref), (const int *) (lb.d + at.off), (const int *) (lb.d + at.node), (const int *) (lb.d + at.fac),
-                      (const float *) (lb.d + at.rkp), (const float *) (lb.d + at.kp)};
-    rc = cull_run(h, n, problems, cam, reprojection_error_std, io, win, h->lists_nobs, h->lists_nL, h->lists_nO, nK, &src, fn);
+    const icg_ba::BuiltLists &B = h->built;
+    rc = cull_run(h, n, problems, cam, reprojection_error_std, io, win, B.nobs, B.nL, B.nO, nK, &B, want_kp, fn);
     if (rc != ICG_OK) return rc;
-    // the integer lists on the host (icg_ba_marginalize_resident_culled's NULL lists read them there) and, when asked for, the keypoints
-    h->cull_res_n = 0;
-    ICG_CUDA(cudaMemcpyAsync(lb.h, lb.d, at.rkp, cudaMemcpyDeviceToHost, h->stream));
-    if (want_kp) ICG_CUDA(cudaMemcpyAsync(lb.h + at.rkp, lb.d + at.rkp, at.end - at.rkp, cudaMemcpyDeviceToHost, h->stream));
-    ICG_CUDA(cudaStreamSynchronize(h->stream));
-    h->cull_res_n = n;
-    h->cull_res_href = (const int *) (lb.h + at.ref), h->cull_res_hoff = (const int *) (lb.h + at.off), h->cull_res_hnode = (const int *) (lb.h + at.node);
-    h->cull_res_hfac = (const int *) (lb.h + at.fac);
+    const CullSrc hl = B.host();
     for (int w = 0; lists && w < n; w++) {
-        const int L = problems[w].L, no = h->lists_nobs[w];
+        const int L = problems[w].L, no = B.nobs[w];
         const CullWin &W = win[w];
         icg_ba_cull_lists &o = lists[w];
         o.n_obs = no;
-        if (o.lm_ref_node) memcpy(o.lm_ref_node, lb.h + at.ref + 4 * (size_t) W.lm0, 4 * (size_t) L);
-        if (o.obs_off) memcpy(o.obs_off, lb.h + at.off + 4 * (size_t) W.off0, 4 * ((size_t) L + 1));
-        if (o.obs_node) memcpy(o.obs_node, lb.h + at.node + 4 * (size_t) W.obs0, 4 * (size_t) no);
-        if (o.obs_factor) memcpy(o.obs_factor, lb.h + at.fac + 4 * (size_t) W.obs0, 4 * (size_t) no);
-        if (o.lm_ref_kp) memcpy(o.lm_ref_kp, lb.h + at.rkp + 8 * (size_t) W.lm0, 8 * (size_t) L);
-        if (o.obs_kp) memcpy(o.obs_kp, lb.h + at.kp + 8 * (size_t) W.obs0, 8 * (size_t) no);
+        if (o.lm_ref_node) memcpy(o.lm_ref_node, hl.ref + W.lm0, 4 * (size_t) L);
+        if (o.obs_off) memcpy(o.obs_off, hl.off + W.off0, 4 * ((size_t) L + 1));
+        if (o.obs_node) memcpy(o.obs_node, hl.node + W.obs0, 4 * (size_t) no);
+        if (o.obs_factor) memcpy(o.obs_factor, hl.fac + W.obs0, 4 * (size_t) no);
+        if (o.lm_ref_kp) memcpy(o.lm_ref_kp, hl.rkp + 2 * (size_t) W.lm0, 8 * (size_t) L);
+        if (o.obs_kp) memcpy(o.obs_kp, hl.kp + 2 * (size_t) W.obs0, 8 * (size_t) no);
     }
     return ICG_OK;
 }
@@ -1743,7 +1728,7 @@ int icg_ba_update_and_cull_resident(icg_ba *h, int n_windows, const icg_ba_probl
         nobs[w] = no;
         nL += p.L, nO += no, nK += p.K;
     }
-    return cull_run(h, n, problems, cam, reprojection_error_std, io, win, nobs, nL, nO, nK, nullptr, fn);
+    return cull_run(h, n, problems, cam, reprojection_error_std, io, win, nobs, nL, nO, nK, nullptr, false, fn);
 }
 
 int icg_ba_update_and_cull_built(icg_ba *h, int n_windows, const icg_ba_problem *problems, const icg_camera *cam, double reprojection_error_std,
@@ -1787,21 +1772,22 @@ int icg_ba_marginalize_resident_culled(icg_ba *h, int n_windows, const icg_ba_pr
     std::vector<std::vector<uint8_t>> masks(n_windows);
     std::vector<const uint8_t *> mp(n_windows);
     // a NULL list after a built culling is that culling's own (its host copy)
-    const bool built = h->cull_res_n == n_windows && h->cull_res_href;
+    const icg_ba::CullResult &cul = h->culled;
+    const bool built = cul.n == n_windows && cul.host.ref;
     for (int w = 0; w < n_windows; w++) {
         const icg_ba_problem &p = problems[w];
         icg_ba_cull_window c = culled[w];
         if (!c.lm_ref_node || !c.obs_off || !c.obs_node || !c.obs_factor) {
-            const CullWin *bw = built ? &h->cull_res_win[w] : nullptr;
+            const CullWin *bw = built ? &cul.win[w] : nullptr;
             if (p.L > 0 && (!bw || bw->L != p.L || bw->K != p.K)) {
                 set_error("icg_ba_marginalize_resident_culled: window %d: lists missing, and no built culling of these windows is current", w);
                 return ICG_EINVAL;
             }
             if (bw) {
-                if (!c.lm_ref_node) c.lm_ref_node = h->cull_res_href + bw->lm0;
-                if (!c.obs_off) c.obs_off = h->cull_res_hoff + bw->off0;
-                if (!c.obs_node) c.obs_node = h->cull_res_hnode + bw->obs0;
-                if (!c.obs_factor) c.obs_factor = h->cull_res_hfac + bw->obs0;
+                if (!c.lm_ref_node) c.lm_ref_node = cul.host.ref + bw->lm0;
+                if (!c.obs_off) c.obs_off = cul.host.off + bw->off0;
+                if (!c.obs_node) c.obs_node = cul.host.node + bw->obs0;
+                if (!c.obs_factor) c.obs_factor = cul.host.fac + bw->obs0;
             }
         }
         if (!node_in_map[w] || (p.L > 0 && (!c.lm_ref_node || !c.obs_off || !c.lm_outlier)) || p.K > h->C.K || p.L > h->C.L || p.F > h->C.F ||
@@ -1938,10 +1924,10 @@ int icg_ba_slide_ins_resident(icg_ba *h, icg_ins *ins, int n_windows, const icg_
                     set_error("%s: window %d: imu_src[%d] = %d is out of range of the old window (%d)", fn, w, k, c.imu_src[k], on);
                     return ICG_EINVAL;
                 }
-                if (h->store_valid) f.kind = STORE_OLD, f.a = c.imu_src[k];
+                if (h->store.valid) f.kind = STORE_OLD, f.a = c.imu_src[k];
             } else if (from == ICG_SLIDE_ROW) {
                 const int a = g.merge_src ? g.merge_src[k] : -1;
-                if (a < 0 || a + 1 >= on || !h->store_valid || h->store_nrow[w][a] < 1 || h->store_nrow[w][a + 1] < 1) {
+                if (a < 0 || a + 1 >= on || !h->store.valid || h->store.nrow[w][a] < 1 || h->store.nrow[w][a + 1] < 1) {
                     set_error("%s: window %d factor %d: merge_src must name old factors a and a + 1 that both hold samples", fn, w, k);
                     return ICG_EINVAL;
                 }
@@ -1971,7 +1957,7 @@ int icg_ba_slide_ins_resident(icg_ba *h, icg_ins *ins, int n_windows, const icg_
     if (rc != ICG_OK) return rc;
     std::vector<icg_ba_slide_integrate> integ(n_windows);
     for (int w = 0; w < n_windows; w++) integ[w] = io[w].integ;
-    const FactorRows fr = {h->store_d[1 - h->store_cur], row0, nrow};
+    const FactorRows fr = {h->store.d[1 - h->store.cur], row0, nrow};
     rc = vis ? vision_body(h, n_windows, next, carry, integ.data(), noise5, station3, vis, fn, false, &fr)
              : slide_body(h, n_windows, next, carry, integ.data(), noise5, station3, fn, false, false, nullptr, &fr);
     if (rc != ICG_OK) return rc;
@@ -1991,7 +1977,7 @@ int icg_ba_reintegrate_stored_resident(icg_ba *h, int n_windows, const icg_ba_pr
         set_error("%s: bad arguments", fn);
         return ICG_EINVAL;
     }
-    if (!h->store_valid) {
+    if (!h->store.valid) {
         set_error("%s: the handle holds no IMU samples (an upload or a slide other than icg_ba_slide_ins_resident replaced the windows since "
                   "the last icg_ba_imu_samples_from_ins)", fn);
         return ICG_EINVAL;
@@ -2001,7 +1987,7 @@ int icg_ba_reintegrate_stored_resident(icg_ba *h, int n_windows, const icg_ba_pr
             set_error("%s: window %d: imu and imu_off must be NULL (the rows are the store's)", fn, w);
             return ICG_EINVAL;
         }
-    const FactorRows fr = {h->store_d[h->store_cur], h->store_row0, h->store_nrow};
+    const FactorRows fr = {h->store.d[h->store.cur], h->store.row0, h->store.nrow};
     return reint_body(h, n_windows, problems, noise5, station3, io, fn, false, &fr);
 }
 
@@ -2015,11 +2001,11 @@ int icg_ba_imu_samples(icg_ba *h, int window, int cap_rows, int32_t *off, double
         set_error("%s: not available on a landmark-sharded handle", fn);
         return ICG_EUNSUPPORTED;
     }
-    if (!h->store_valid) {
+    if (!h->store.valid) {
         set_error("%s: the handle holds no IMU samples", fn);
         return ICG_EINVAL;
     }
-    const std::vector<int> &r0 = h->store_row0[window], &nr = h->store_nrow[window];
+    const std::vector<int> &r0 = h->store.row0[window], &nr = h->store.nrow[window];
     int first = -1, total = 0;
     for (size_t k = 0; k < nr.size(); k++) {
         off[k] = nr[k] < 0 ? -1 : total;
@@ -2031,7 +2017,7 @@ int icg_ba_imu_samples(icg_ba *h, int window, int cap_rows, int32_t *off, double
     const int m = std::min(total, cap_rows);
     if (m == 0) return ICG_OK;
     ICG_CUDA(cudaSetDevice(h->device));
-    ICG_CUDA(cudaMemcpyAsync(rows, h->store_d[h->store_cur] + 7 * (size_t) first, 56 * (size_t) m, cudaMemcpyDeviceToHost, h->stream));
+    ICG_CUDA(cudaMemcpyAsync(rows, h->store.d[h->store.cur] + 7 * (size_t) first, 56 * (size_t) m, cudaMemcpyDeviceToHost, h->stream));
     ICG_CUDA(cudaStreamSynchronize(h->stream));
     return ICG_OK;
 }
