@@ -98,6 +98,7 @@ ABI = {
     "icg_ba_marginalize": ([vp, c_int, vp, vp, vp], c_int),
     "icg_ba_marginalize_resident": ([vp, c_int, vp, vp, vp], c_int),
     "icg_ba_peek_linearization": ([vp, c_int, vp], c_int),
+    "icg_ba_peek_structure": ([vp, c_int, vp], c_int),
     # ---- window solver: landmark-shard group
     "icg_ba_shard_export": ([vp, c_int, c_int, vp], c_int),
     "icg_ba_shard_connect": ([vp, vp], c_int),
@@ -264,6 +265,13 @@ class Linearization(C.Structure):
     """ctypes image of `icg_ba_linearization`."""
     _fields_ = [("K", C.c_int32), ("L", C.c_int32), ("F", C.c_int32), ("n_pairs", C.c_int32), ("lin_buf", C.c_int32), ("radius", C.c_double), ("pair_ro", i32p), ("Mp", f64p), ("A_W", f64p),
                 ("h_l", f64p), ("g_l", f64p), ("H_c", f64p), ("g_c", f64p), ("costf", f64p), ("scale_l", f64p), ("Hs", f64p), ("visv", f64p)]
+
+
+class Structure(C.Structure):
+    """ctypes image of `icg_ba_structure`."""
+    _fields_ = [("K", C.c_int32), ("L", C.c_int32), ("F", C.c_int32), ("n_runs", C.c_int32), ("npairs", C.c_int32), ("lm_perm", i32p),
+                ("lm_off", i32p), ("f_meta_s", i32p), ("vb_lm0", i32p), ("ref_nrun", i32p), ("part_off", i32p), ("pair_ro", i32p),
+                ("vis_ord", i32p), ("f_active", u8p)]
 
 
 class InsConfig(C.Structure):

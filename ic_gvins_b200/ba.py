@@ -9,7 +9,7 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import (BaPrior, BaProblem, BaSummary, CullLists, CullWindow, InsCut, Linearization, ReintWindow, SlideIns, SlideIntegrate, SlideVision,
+from ._lib import (BaPrior, BaProblem, BaSummary, CullLists, CullWindow, InsCut, Linearization, ReintWindow, SlideIns, SlideIntegrate, SlideVision, Structure,
                    SlideWindow, check, f32p, f64p, i8p, i32p, i64p, lib, u8p, vp)
 from .camera import CameraStruct
 
@@ -330,14 +330,22 @@ def _dev(t):
     return None if t is None else vp(t.data_ptr() if hasattr(t, "data_ptr") else int(t))
 
 
-def _vision_struct(next_problems, vision, Lc: int, Fc: int, keep: list):
+_LEAN_ROWS = ("lm_src", "lm_origin", "f_src", "f_lm", "f_ref", "f_obs")
+
+
+def _vision_struct(next_problems, vision, Lc: int, Fc: int, keep: list, rows: bool = True):
     """The icg_ba_slide_vision array of the `vision` dicts (WindowSolver.slide_vision) and the host rows the call builds into, sized to a
-    handle of Lc landmarks and Fc factors.  Empties the vision rows of next_problems, which the call does not read."""
+    handle of Lc landmarks and Fc factors (rows False: no invdepth / f_const, which the call then leaves on the device).  Empties the vision
+    rows of next_problems, which the call does not read."""
     vw = (SlideVision * len(next_problems))()
     outs = []
     for w, (p, v) in enumerate(zip(next_problems, vision)):
-        o = dict(lm_src=np.zeros(Lc, np.int32), lm_origin=np.zeros(Lc, np.int32), nan_flags=np.zeros(Lc + int(v.get("n_new", 0)), np.uint8), f_src=np.zeros(Fc, np.int32), f_lm=np.zeros(Fc, np.int32), f_ref=np.zeros(Fc, np.int32),
-                 f_obs=np.zeros(Fc, np.int32), invdepth=np.zeros(Lc), f_const=np.zeros((Fc, 14)))
+        if rows:
+            o = dict(lm_src=np.zeros(Lc, np.int32), lm_origin=np.zeros(Lc, np.int32), nan_flags=np.zeros(Lc + int(v.get("n_new", 0)), np.uint8), f_src=np.zeros(Fc, np.int32), f_lm=np.zeros(Fc, np.int32), f_ref=np.zeros(Fc, np.int32),
+                     f_obs=np.zeros(Fc, np.int32), invdepth=np.zeros(Lc), f_const=np.zeros((Fc, 14)))
+        else:
+            o = {k: np.empty(Fc if k.startswith("f_") else Lc, np.int32) for k in _LEAN_ROWS}
+            o["nan_flags"] = np.zeros(Lc + int(v.get("n_new", 0)), np.uint8)
         outs.append(o)
         p.update(L=0, F=0, invdepth=np.zeros(0), f_lm=np.zeros(0, np.int32), f_ref=np.zeros(0, np.int32), f_obs=np.zeros(0, np.int32),
                  f_const=np.zeros(0), f_active=np.zeros(0, np.uint8))
@@ -362,7 +370,8 @@ def _vision_struct(next_problems, vision, Lc: int, Fc: int, keep: list):
         s.new_depth, s.new_vel_ref, s.new_vel_cur = (_dev(v.get(k)) for k in ("new_depth", "new_vel_ref", "new_vel_cur"))
         s.new_ref_undis_xy, s.new_cur_undis_xy, s.new_ref_frame_id = (_dev(v.get(k)) for k in ("new_ref_undis_xy", "new_cur_undis_xy", "new_ref_frame_id"))
         s.lm_src, s.f_src, s.f_lm, s.f_ref, s.f_obs = (o[k].ctypes.data_as(i32p) for k in ("lm_src", "f_src", "f_lm", "f_ref", "f_obs"))
-        s.invdepth, s.f_const = o["invdepth"].ctypes.data_as(f64p), o["f_const"].ctypes.data_as(f64p)
+        if rows:
+            s.invdepth, s.f_const = o["invdepth"].ctypes.data_as(f64p), o["f_const"].ctypes.data_as(f64p)
         s.lm_origin, s.nan_flags = o["lm_origin"].ctypes.data_as(i32p), o["nan_flags"].ctypes.data_as(u8p)
     return vw, outs
 
@@ -373,6 +382,13 @@ def _vision_results(next_problems, carry, vw, outs) -> list:
     res = []
     for w, (p, c, o) in enumerate(zip(next_problems, carry, outs)):
         L, F = int(vw[w].L), int(vw[w].F)
+        if "f_const" not in o:
+            # rows=False: what the rest of the keyframe cycle reads on the host.  invdepth is the buffer a later download fills
+            r = dict(L=L, F=F, nan_dropped=int(vw[w].nan_dropped), nan_flags=o["nan_flags"], **{k: o[k][:F if k.startswith("f_") else L] for k in _LEAN_ROWS})
+            res.append(r)
+            p.update(L=L, F=F, invdepth=np.zeros(L), f_lm=r["f_lm"], f_ref=r["f_ref"], f_obs=r["f_obs"], f_const=np.zeros(0), f_active=np.ones(F, np.uint8))
+            c["lm_src"], c["f_src"] = r["lm_src"], r["f_src"]
+            continue
         r = dict(L=L, F=F, nan_dropped=int(vw[w].nan_dropped), lm_src=o["lm_src"][:L].copy(), lm_origin=o["lm_origin"][:L].copy(),
                  nan_flags=o["nan_flags"], invdepth=o["invdepth"][:L].copy(),
                  f_src=o["f_src"][:F].copy(), f_lm=o["f_lm"][:F].copy(), f_ref=o["f_ref"][:F].copy(), f_obs=o["f_obs"][:F].copy(),
@@ -471,6 +487,23 @@ class WindowSolver:
                     A_W=a["A_W"][:L * (NCV + 1)].reshape(L, NCV + 1), h_l=a["h_l"][:L], g_l=a["g_l"][:L], scale_l=a["scale_l"][:L],
                     H_c=a["H_c"][:N * N].reshape(N, N), g_c=a["g_c"][:N], costf=a["costf"][:F], Hs=a["Hs"][:NCV * NCV].reshape(NCV, NCV),
                     visv=a["visv"][:3 * NCV].reshape(3, NCV))
+
+    def peek_structure(self, w: int) -> dict:
+        """Window w's structure tables (icg_ba_peek_structure; a test read-out), in the window's sizes: lm_perm, lm_off, f_meta_s (F x 4),
+        vb_lm0 (runs + 1), ref_nrun, part_off, pair_ro, vis_ord, npairs, f_active."""
+        K, L, F = self.max_K, self.max_L, self.max_F
+        PM = K * (K - 1)
+        a = dict(lm_perm=np.zeros(L, np.int32), lm_off=np.zeros(L + 1, np.int32), f_meta_s=np.zeros(4 * F, np.int32), vb_lm0=np.zeros(L + F + 2, np.int32),
+                 ref_nrun=np.zeros(K, np.int32), part_off=np.zeros(PM + 1, np.int32), pair_ro=np.zeros(PM, np.int32), vis_ord=np.zeros(F, np.int32),
+                 f_active=np.zeros(F, np.uint8))
+        s = Structure()
+        for name, arr in a.items():
+            setattr(s, name, arr.ctypes.data_as(u8p if arr.dtype == np.uint8 else i32p))
+        check(lib().icg_ba_peek_structure(self._h, w, C.byref(s)), "icg_ba_peek_structure")
+        L, F, R, P = s.L, s.F, s.n_runs, s.npairs
+        return dict(lm_perm=a["lm_perm"][:L], lm_off=a["lm_off"][:L + 1], f_meta_s=a["f_meta_s"][:4 * F].reshape(F, 4), vb_lm0=a["vb_lm0"][:R + 1],
+                    ref_nrun=a["ref_nrun"][:s.K], part_off=a["part_off"][:P + 1], pair_ro=a["pair_ro"][:P], vis_ord=a["vis_ord"][:F],
+                    npairs=np.array([P]), f_active=a["f_active"][:F])
 
     def residual_costs(self, prob):
         s = to_struct(prob)
@@ -785,17 +818,18 @@ class WindowSolver:
         self._keep, self._n = arr, n
         return outs
 
-    def slide_vision(self, next_problems, carry, vision, integrate=None, noise5=None, station=(0.0, 0.0, 0.0), prior_from_marg=True):
-        return self._slide_vision("icg_ba_slide_vision_resident", next_problems, carry, vision, integrate, noise5, station, prior_from_marg)
+    def slide_vision(self, next_problems, carry, vision, integrate=None, noise5=None, station=(0.0, 0.0, 0.0), prior_from_marg=True, rows=True):
+        return self._slide_vision("icg_ba_slide_vision_resident", next_problems, carry, vision, integrate, noise5, station, prior_from_marg, rows)
 
-    def shard_slide_vision(self, next_problems, carry, vision, integrate=None, noise5=None, station=(0.0, 0.0, 0.0), prior_from_marg=True):
+    def shard_slide_vision(self, next_problems, carry, vision, integrate=None, noise5=None, station=(0.0, 0.0, 0.0), prior_from_marg=True,
+                           rows=True):
         """slide_vision() on a landmark-sharded handle (icg_ba_shard_slide_vision_resident), a collective call: every rank passes its next shards
         (camera side as shard_slide takes it), their carry maps (node / IMU / GNSS) and its own vision dicts (shard_vision_inputs); new map
         point j of window w is built on rank (j + w) % world.  Returns the rank's shard as slide_vision does (lm_src / f_src shard-local,
         lm_origin: old shard-local landmark or -(j + 1) for global new point j, nan_flags: old shard L + every new point, set on its own rank)."""
-        return self._slide_vision("icg_ba_shard_slide_vision_resident", next_problems, carry, vision, integrate, noise5, station, prior_from_marg)
+        return self._slide_vision("icg_ba_shard_slide_vision_resident", next_problems, carry, vision, integrate, noise5, station, prior_from_marg, rows)
 
-    def _slide_vision(self, fn, next_problems, carry, vision, integrate=None, noise5=None, station=(0.0, 0.0, 0.0), prior_from_marg=True):
+    def _slide_vision(self, fn, next_problems, carry, vision, integrate=None, noise5=None, station=(0.0, 0.0, 0.0), prior_from_marg=True, rows=True):
         """slide() (integrate given: slide_integrate()) whose vision rows are built on the device (icg_ba_slide_vision_resident):
         addReprojectionParameters + addReprojectionFactors on the culled window this handle holds plus the new keyframes' observations.  The
         last update_and_cull() of these windows must be current.  next_problems' L, F, invdepth, f_lm / f_ref / f_obs / f_const, f_active and
@@ -809,12 +843,15 @@ class WindowSolver:
             new_vel_cur, n_new and optionally dev_new_n.
         Returns one dict per window: L, F, nan_dropped, nan_flags (old L + n_new entries first: 1 where a landmark or new point was dropped
         for a NaN inverse depth), lm_origin (old landmark, or -(j + 1) for new point j), lm_src, f_src, f_lm, f_ref, f_obs, invdepth and f_const (the new factors' rows, f_src = -1;
-        the others zero).  A rejected call raises IcgError with the handle unchanged."""
+        the others zero).  rows=False returns only what the rest of the keyframe cycle reads on the host (L, F, nan_dropped, nan_flags,
+        lm_origin, lm_src, f_src, f_lm, f_ref, f_obs, sized to L and F): the inverse depths and factor constants stay on the device, and
+        next_problems gets f_const empty and invdepth as a buffer for the next download.  A rejected call raises IcgError with the handle
+        unchanged."""
         if integrate is not None and noise5 is None:
             raise ValueError(f"{fn}: integrate needs noise5")
         n = len(next_problems)
         keep = []
-        vw, built = _vision_struct(next_problems, vision, self.max_L, self.max_F, keep)
+        vw, built = _vision_struct(next_problems, vision, self.max_L, self.max_F, keep, rows)
         arr, cw = _problems(next_problems), _slide_carry(carry, n, prior_from_marg, keep, _VISION_CARRY)
         iw, nz, stn = None, None, None
         if integrate is not None:

@@ -8,6 +8,7 @@
 
 #include "ba_cull.cuh"
 #include "ba_dev.cuh"
+#include "ba_vision.cuh"
 #include "geom_core.cuh"
 
 // ---- IMU sqrt information  U = LLT(cov^-1).matrixL().transpose(): the shared core of geom_core.cuh, so that the reintegration kernel
@@ -171,6 +172,9 @@ struct icg_ba {
     // icg_ba_slide_resident: staging (grown on demand), the copy of the old value rows, the second f_const_s buffer
     HostDev<unsigned char> slide;
     double *slide_old = nullptr, *fc_alt = nullptr;
+    // icg_ba_slide_vision_resident: the structure tables ba_pack_structure writes (one allocation at f_meta_s, the handle's capacities and
+    // strides), copied into the handle's when the slide commits
+    icg::PackTables pack{};
     // every landmark's reference row pts0[3] | vel0[3] | td0 (NaN: unknown), 7 doubles at w L + l, and the buffer the next slide writes: set by
     // icg_ba_upload from the landmark's first factor, carried by every slide, read by icg_ba_slide_vision_resident
     double *lm_ref = nullptr, *lm_ref_alt = nullptr;
@@ -207,8 +211,8 @@ struct ClusterLaunch {
 // ---- shared by ba_handle.cu and ba_keyframe.cu
 int dmalloc(icg_ba *h, double **p, size_t n);
 cudaError_t launch_lm_ref_fill(icg_ba *h, int n, const icg::SlideWin *win, const int *map, const double *old, double *out);
-int pack_windows(icg_ba *h, int n, const icg_ba_problem *P, bool values);
-int upload_structure(icg_ba *h, int n);
+int pack_windows(icg_ba *h, int n, const icg_ba_problem *P, bool values, bool vision = true);
+int upload_structure(icg_ba *h, int n, bool vision = true);
 int keep_pristine(icg_ba *h, int n);
 void retire(icg_ba *h, void *d, void *hp);
 // shard groups (world > 1, ba_split.cuh); fn: the calling entry point, for the error messages

@@ -710,6 +710,16 @@ static int shard_group_only(icg_ba *h, const char *fn, const char *plain) {
     return ICG_OK;
 }
 
+// What vision_body hands slide_body for windows built on the device: the outcome of ba_pack_structure (a rejection is reported where the
+// host packing would report it), and the maps and rows the gather reads there (PackArgs::map)
+struct VisSlide {
+    int rc = ICG_OK;
+    std::string err;
+    const int *map = nullptr;
+    const double *invdepth = nullptr, *f_new = nullptr;
+    std::vector<int> lm_at, slot_at;  // per window: its first landmark / record-slot entry of map
+};
+
 // ---- the next keyframe's windows from the resident ones (ba_slide.cu): the structure is packed on the host as icg_ba_upload packs it, the
 //      values of the carried rows never leave the device.  With `integ`, the new factors, node rows and aligned fixes it names are computed on
 //      the device (preint.cu) into the staged value rows before the gather reads them.
@@ -718,11 +728,12 @@ static int shard_group_only(icg_ba *h, const char *fn, const char *plain) {
 // check of its own prior; then one agreement of the group (shard_agree: every rank's verdict and a fingerprint of the camera side) before any
 // rank writes its device, and with `integ` a second one on the integration's outcome.  A rank that rejects joins the agreement all the same
 // (fail below), so its peers never wait for it.  The owner of window w forms its prior from the workspace of mx_h; the other ranks get zeros.
-// lm_ref_built: vision_body has written the next windows' reference rows into lm_ref_alt already; seed (sharded): vision_body's fingerprint of
+// vs: the windows vision_body built, whose vision structure ba_pack_structure packed into h->pack and whose new vision rows the gather reads
+// on the device (vision_body has also written their reference rows into lm_ref_alt); seed (sharded): vision_body's fingerprint of
 // its own arguments, which the agreement's fingerprint continues; fr (icg_ba_slide_ins_resident): the integrated factors' rows are the next
 // sample store's, integ's imu / imu_off are not read
 static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba_slide_window *carry, const icg_ba_slide_integrate *integ,
-                      const double *noise5, const double *station3, const char *fn, bool sharded, bool lm_ref_built = false,
+                      const double *noise5, const double *station3, const char *fn, bool sharded, const VisSlide *vs = nullptr,
                       const ArgPrint *seed = nullptr, const FactorRows *fr = nullptr) {
     bool joined = false;  // sharded: this rank has joined the agreement of the call
     std::vector<WinDims> old_dims;
@@ -732,7 +743,7 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
     auto fail = [&](int code) {
         if (!old_dims.empty()) {
             memcpy(h->dims.h, old_dims.data(), sizeof(WinDims) * n);
-            for (int w = 0; w < n; w++) {
+            for (int w = 0; w < (int) old_slot.size(); w++) {
                 int *fidx = h->lm_fidx.h + (size_t) w * h->C.F;
                 for (int f = 0; f < old_dims[w].F; f++) fidx[old_slot[w][f]] = f;
             }
@@ -759,6 +770,7 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
     const int G = h->D.world, R = h->D.rank;
     for (int w = 0; w < n; w++) {
         const icg_ba_problem &p = next[w];
+        // (the vision build lists each landmark's factors together, landmarks in order: next's f_lm is NULL there)
         if (sharded)
             for (int f = 1; p.f_lm && f < p.F; f++)
                 if (p.f_lm[f] < p.f_lm[f - 1]) {
@@ -787,15 +799,17 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
         set_error("%s: allocation of the slide buffers failed", fn);
         return fail(ICG_ENOMEM);
     }
-    // the old windows: sizes, and every factor's record slot (the inverse of the last packing's slot -> factor table)
+    // the old windows: sizes, and every factor's record slot (the inverse of the last packing's slot -> factor table; built windows: the
+    // device's slot maps)
     old_dims.assign(h->dims.h, h->dims.h + n);
-    old_slot.resize(n);
-    for (int w = 0; w < n; w++) {
+    old_slot.resize(vs ? 0 : n);
+    for (int w = 0; w < (int) old_slot.size(); w++) {
         old_slot[w].resize(old_dims[w].F);
         const int *fidx = h->lm_fidx.h + (size_t) w * C.F;
         for (int q = 0; q < old_dims[w].F; q++) old_slot[w][fidx[q]] = q;
     }
-    rc = pack_windows(h, n, next, false);
+    rc = pack_windows(h, n, next, false, !vs);
+    if (rc == ICG_OK && vs && vs->rc != ICG_OK) set_error("%s", vs->err.c_str()), rc = vs->rc;
     if (rc != ICG_OK) return fail(rc);
     // the maps: range checks, sizes of the staging
     std::vector<SlideWin> wins(n);
@@ -811,7 +825,7 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
         static const char *names[5] = {"node_src", "lm_src", "f_src", "imu_src", "gnss_src"};
         vbase[w] = n_val;
         for (int t = 0; t < 5; t++)
-            for (int i = 0; maps[t] && i < cnt[t]; i++) {
+            for (int i = 0; maps[t] && i < cnt[t] && !(vs && (t == 1 || t == 2)); i++) {
                 if (maps[t][i] < -1 || maps[t][i] >= lim[t]) {
                     set_error("%s: window %d: %s[%d] = %d is out of range of the old window (%d)", fn, w, names[t], i, maps[t][i], lim[t]);
                     return fail(ICG_EINVAL);
@@ -820,10 +834,15 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
                 n_val += width[t];
             }
         for (int t = 0; t < 5; t++)
-            if (!maps[t]) n_val += (size_t) width[t] * cnt[t];
+            if (!maps[t] && !(vs && (t == 1 || t == 2))) n_val += (size_t) width[t] * cnt[t];
         SlideWin &W = wins[w];
         W.K = p.K, W.L = p.L, W.F = p.F, W.n_imu = p.n_imu, W.n_gnss = p.n_gnss;
-        W.node_map = (int) n_map, W.lm_map = W.node_map + p.K, W.slot_map = W.lm_map + p.L, W.imu_map = W.slot_map + p.F, W.gnss_map = W.imu_map + p.n_imu;
+        if (vs) {
+            W.vis = 1, W.lm_map = vs->lm_at[w], W.slot_map = vs->slot_at[w];
+            W.node_map = (int) n_map, W.imu_map = W.node_map + p.K, W.gnss_map = W.imu_map + p.n_imu;
+        } else {
+            W.node_map = (int) n_map, W.lm_map = W.node_map + p.K, W.slot_map = W.lm_map + p.L, W.imu_map = W.slot_map + p.F, W.gnss_map = W.imu_map + p.n_imu;
+        }
         n_map = (size_t) W.gnss_map + p.n_gnss;
         W.r = p.marg_r, W.from_marg = c.prior_from_marg != 0, W.j0 = W.e0 = 0;
         W.slot = !sharded ? w : w % G == R ? (w - R) / G : -1;
@@ -957,9 +976,9 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
             map[W.node_map + k] = stage(p.pose + 7 * (size_t) k, 7);
             stage(p.mix + 9 * (size_t) k, 9);
         }
-        for (int l = 0; l < p.L; l++) map[W.lm_map + l] = c.lm_src && c.lm_src[l] >= 0 ? c.lm_src[l] : stage(p.invdepth + l, 1);
+        for (int l = 0; !vs && l < p.L; l++) map[W.lm_map + l] = c.lm_src && c.lm_src[l] >= 0 ? c.lm_src[l] : stage(p.invdepth + l, 1);
         const int *fidx = h->lm_fidx.h + (size_t) w * C.F;  // the new packing's slot -> factor table
-        for (int q = 0; q < p.F; q++) {
+        for (int q = 0; !vs && q < p.F; q++) {
             const int f = fidx[q];
             map[W.slot_map + q] = c.f_src && c.f_src[f] >= 0 ? old_slot[w][c.f_src[f]] : stage(p.f_const + 14 * (size_t) f, 14);
         }
@@ -1129,9 +1148,24 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
     h->end_results();
     if (iwins.empty()) ICG_CUDA(cudaMemcpyAsync(h->slide.d, h->slide.h, in_end, cudaMemcpyHostToDevice, s));
     ICG_CUDA(cudaEventRecord(h->slide_ev, s));
-    rc = upload_structure(h, n);
+    rc = upload_structure(h, n, !vs);
     if (rc != ICG_OK) return rc;
     BaDev &D = h->D;
+    if (vs) {
+        const size_t nn = (size_t) n, PM = (size_t) C.K * (C.K - 1);
+        const PackTables &T = h->pack;
+        auto take = [&](void *dst, const void *src, size_t bytes) { return cudaMemcpyAsync(dst, src, nn * bytes, cudaMemcpyDeviceToDevice, s); };
+        ICG_CUDA(take(D.f_meta_s, T.f_meta_s, 16 * (size_t) C.F));
+        ICG_CUDA(take(D.vb_lm0, T.vb_lm0, 4 * (size_t) C.NVB));
+        ICG_CUDA(take(D.lm_off, T.lm_off, 4 * ((size_t) C.L + 1)));
+        ICG_CUDA(take(D.lm_perm, T.lm_perm, 4 * (size_t) C.L));
+        ICG_CUDA(take(D.ref_nrun, T.ref_nrun, 4 * (size_t) C.K));
+        ICG_CUDA(take(D.part_off, T.part_off, 4 * (PM + 1)));
+        ICG_CUDA(take(D.pair_ro, T.pair_ro, 4 * PM));
+        ICG_CUDA(take(D.vis_ord, T.vis_ord, 4 * (size_t) C.F));
+        ICG_CUDA(take(D.npairs, T.npairs, 4));
+        ICG_CUDA(take(D.f_active, T.f_active, C.F));
+    }
     double *old = h->slide_old;
     const size_t nn = (size_t) n;
     auto d2d = [&](double *dst, const double *src, size_t count) { return cudaMemcpyAsync(dst, src, sizeof(double) * count, cudaMemcpyDeviceToDevice, s); };
@@ -1144,6 +1178,7 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
     ICG_CUDA(d2d(old + o_std, D.gnss_std, nn * C.G * 3));
     SlideArgs a;
     a.win = (const SlideWin *) h->slide.d, a.map = (const int *) (h->slide.d + b_map), a.val = (const double *) (h->slide.d + b_val);
+    a.vmap = vs ? vs->map : nullptr, a.vlm = vs ? vs->invdepth : nullptr, a.vfc = vs ? vs->f_new : nullptr;
     a.K = C.K, a.L = C.L, a.F = C.F, a.G = C.G, a.R = C.R;
     a.old_pose = old, a.old_mix = old + o_mix, a.old_rho = old + o_rho, a.old_fc = D.f_const_s, a.old_blob = old + o_blob, a.old_U = old + o_U;
     a.old_blh = old + o_blh, a.old_std = old + o_std;
@@ -1155,7 +1190,7 @@ static int slide_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba
     count_launch(2);
     std::swap(h->f_const_s.d, h->fc_alt);  // the gathered record constants become the handle's
     D.f_const_s = h->f_const_s.d;
-    if (!lm_ref_built) ICG_CUDA(launch_lm_ref_fill(h, n, a.win, a.map, h->lm_ref, h->lm_ref_alt));
+    if (!vs) ICG_CUDA(launch_lm_ref_fill(h, n, a.win, a.map, h->lm_ref, h->lm_ref_alt));
     std::swap(h->lm_ref, h->lm_ref_alt);
     rc = keep_pristine(h, n);
     if (rc != ICG_OK) return rc;
@@ -1194,7 +1229,7 @@ static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_b
     std::vector<VisWin> wins(n);
     std::vector<long long> ofac_at(n, -1);  // the window's first entry in the staged obs_factor, -1: the built lists' (vis[w].obs_factor NULL)
     ArgPrint fp;  // sharded: what every rank must pass alike, then the counts its kernel read
-    size_t n_ofac = 0, n_lm = 0, n_f = 0, n_nf = 0, n_scr = 0, n_lo = 0;
+    size_t n_ofac = 0, n_lm = 0, n_f = 0, n_nf = 0, n_scr = 0, n_lo = 0, n_pscr = 0;
     for (int w = 0; w < n; w++) {
         const icg_ba_problem &p = next[w];
         const icg_ba_slide_vision &v = vis[w];
@@ -1231,26 +1266,43 @@ static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_b
         W.obs_xy = v.obs_undis_xy, W.obs_vel = v.obs_vel;
         W.n_new = v.n_new, W.dev_new_n = v.dev_new_n, W.new_depth = v.new_depth, W.new_vel_ref = v.new_vel_ref, W.new_vel_cur = v.new_vel_cur;
         W.new_ref_xy = v.new_ref_undis_xy, W.new_cur_xy = v.new_cur_undis_xy, W.new_ref_frame = v.new_ref_frame_id;
-        W.lm_out = (int) n_lm, W.f_out = (int) n_f, W.nf_out = (int) n_nf, W.scr = (int) n_scr, W.lst_obs = (int) n_lo;
+        W.lm_out = (int) n_lm, W.f_out = (int) n_f, W.nf_out = (int) n_nf, W.scr = (int) n_scr, W.lst_obs = (int) n_lo, W.pscr = (int) n_pscr;
+        n_pscr += 5 * ((size_t) od.L + v.n_new) + 2 * (size_t) od.F + v.n_obs + v.n_new + C.NVB;  // ba_pack_structure's
         n_lm += (size_t) od.L + v.n_new, n_f += (size_t) od.F + v.n_obs + v.n_new, n_nf += (size_t) v.n_obs + v.n_new;
         n_scr += (size_t) od.F + 3 * (size_t) od.L + 5 * ((size_t) od.L + v.n_new) + v.n_new;  // ba_vision_build's scratch
         n_scr += (size_t) od.F + od.L + v.n_new, n_lo += (size_t) nco + v.n_obs + 2 * (size_t) v.n_new;  // and the lists'
-        if (n_ofac >= INT32_MAX / 2 || n_f >= INT32_MAX / 16 || n_scr >= INT32_MAX / 2 || n_lo >= INT32_MAX / 4) {
+        if (n_ofac >= INT32_MAX / 2 || n_f >= INT32_MAX / 16 || n_scr >= INT32_MAX / 2 || n_lo >= INT32_MAX / 4 || n_pscr >= INT32_MAX / 2) {
             set_error("%s: too many rows in one call", fn);
             return reject(ICG_EINVAL);
         }
     }
-    // staging: inputs [windows | obs_factor], outputs [counts | lm_src | lm_org | f_lm | f_ref | f_obs | f_src | invdepth | new factor rows |
-    // NaN flags], then the kernel's scratch (never copied)
+    // staging: inputs [windows | obs_factor], outputs [counts | slot -> factor tables] (always copied back), [lm_src | lm_org | f_lm | f_ref |
+    // f_obs | f_src | invdepth | new factor rows | NaN flags] (each copied back when a caller asks for it), then the slide's maps and the
+    // kernels' scratch (never copied)
     Layout lay;
     const size_t b_win = lay.take(sizeof(VisWin) * n), b_ofac = lay.take(4 * n_ofac), in_end = lay.size();
-    const size_t b_cnt = lay.take(4 * VIS_COUNTS * (size_t) n), b_lms = lay.take(4 * n_lm), b_org = lay.take(4 * n_lm), b_flm = lay.take(4 * n_f),
-                 b_fref = lay.take(4 * n_f), b_fobs = lay.take(4 * n_f), b_fsrc = lay.take(4 * n_f), b_invd = lay.take(8 * n_lm), b_fnew = lay.take(112 * n_nf),
-                 b_nan = lay.take(n_lm), out_end = lay.size(), b_scr = lay.take(4 * n_scr);
+    const size_t b_cnt = lay.take(4 * VIS_COUNTS * (size_t) n), b_fidx = lay.take(4 * n_f), cnt_end = lay.end;
+    const size_t b_lms = lay.take(4 * n_lm), b_org = lay.take(4 * n_lm), b_flm = lay.take(4 * n_f), b_fref = lay.take(4 * n_f), b_fobs = lay.take(4 * n_f),
+                 b_fsrc = lay.take(4 * n_f), b_invd = lay.take(8 * n_lm), b_fnew = lay.take(112 * n_nf), b_nan = lay.take(n_lm);
+    const size_t b_map = lay.take(4 * (n_lm + n_f)), b_scr = lay.take(4 * n_scr), b_pscr = lay.take(4 * n_pscr);
     cudaStream_t s = h->stream;
     if (lay.size() > h->vis.n)
         if (cudaError_t e = cudaStreamSynchronize(s)) return cuda_fail(e, "cudaStreamSynchronize");
     if ((rc = hd_reserve(h, h->vis, lay.size(), fn)) != ICG_OK) return reject(rc);
+    // the packed tables' buffer, at the handle's capacities (the first call allocates it)
+    PackTables &T = h->pack;
+    if (!T.f_meta_s) {
+        const size_t NW = C.NW, PM = (size_t) C.K * (C.K - 1);
+        const size_t ints = NW * (4 * (size_t) C.F + C.NVB + 2 * (size_t) C.L + 1 + C.K + 2 * PM + 1 + C.F + 1);
+        if (cudaMalloc(&T.f_meta_s, 4 * ints + NW * C.F) != cudaSuccess) {
+            T.f_meta_s = nullptr;
+            set_error("%s: allocation of the packed structure tables failed", fn);
+            return reject(ICG_ENOMEM);
+        }
+        T.vb_lm0 = T.f_meta_s + NW * 4 * C.F, T.lm_off = T.vb_lm0 + NW * C.NVB, T.lm_perm = T.lm_off + NW * (C.L + 1), T.ref_nrun = T.lm_perm + NW * C.L;
+        T.part_off = T.ref_nrun + NW * C.K, T.pair_ro = T.part_off + NW * (PM + 1), T.vis_ord = T.pair_ro + NW * PM, T.npairs = T.vis_ord + NW * C.F;
+        T.f_active = (uint8_t *) (T.npairs + NW);
+    }
     // the next culling's lists (sharded: the rank's next shard's) go to the buffer that is not current
     const int nb = h->built.cur ^ 1;
     icg_ba::BuiltLists::At at{};
@@ -1278,10 +1330,26 @@ static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_b
     unsigned char *Dl = h->built.buf[nb].d;
     a.l_ref = (int *) (Dl + at.ref), a.l_off = (int *) (Dl + at.off), a.l_node = (int *) (Dl + at.node), a.l_fac = (int *) (Dl + at.fac);
     a.l_rkp = (float *) (Dl + at.rkp), a.l_kp = (float *) (Dl + at.kp);
+    PackArgs pa;
+    pa.win = a.win, pa.K = C.K, pa.L = C.L, pa.F = C.F, pa.NVB = C.NVB, pa.counts = a.counts;
+    pa.lm_src = a.lm_src, pa.f_lm = a.f_lm, pa.f_ref = a.f_ref, pa.f_obs = a.f_obs, pa.f_src = a.f_src, pa.old_meta = h->D.f_meta_s, pa.out = T;
+    pa.fidx = (int *) (Dv + b_fidx), pa.map = (int *) (Dv + b_map), pa.nL = (int) n_lm, pa.scratch = (int *) (Dv + b_pscr);
+    // the rows a caller asks for come back; the rest stay on the device, where the slide reads them
+    bool want[9] = {};
+    for (int w = 0; w < n; w++) {
+        const icg_ba_slide_vision &v = vis[w];
+        const bool wv[9] = {v.lm_src != nullptr, v.lm_origin != nullptr, v.f_lm != nullptr, v.f_ref != nullptr, v.f_obs != nullptr,
+                            v.f_src != nullptr || v.f_const != nullptr, v.invdepth != nullptr, v.f_const != nullptr, v.nan_flags != nullptr};
+        for (int i = 0; i < 9; i++) want[i] = want[i] || wv[i];
+    }
+    const size_t row_at[10] = {b_lms, b_org, b_flm, b_fref, b_fobs, b_fsrc, b_invd, b_fnew, b_nan, b_nan + n_lm};
     cudaError_t e = cudaMemcpyAsync(Dv, H, in_end, cudaMemcpyHostToDevice, s);
     if (e == cudaSuccess) e = cudaMemsetAsync(Dv + b_cnt, 0, 4 * VIS_COUNTS * (size_t) n, s);
     if (e == cudaSuccess && (e = launch_vision(a, n, s)) == cudaSuccess) count_launch();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(H + b_cnt, Dv + b_cnt, out_end - b_cnt, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess && (e = launch_pack(pa, n, s)) == cudaSuccess) count_launch();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(H + b_cnt, Dv + b_cnt, cnt_end - b_cnt, cudaMemcpyDeviceToHost, s);
+    for (int i = 0; i < 9; i++)
+        if (e == cudaSuccess && want[i]) e = cudaMemcpyAsync(H + row_at[i], Dv + row_at[i], row_at[i + 1] - row_at[i], cudaMemcpyDeviceToHost, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
     if (e != cudaSuccess) return cuda_fail(e, "the build on the device");
     // the built windows: every check, then the slide of next with these vision rows
@@ -1290,11 +1358,22 @@ static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_b
                                  "a reference frame id is not in the frame table", "a landmark whose reference row is unknown takes a new observation"};
     std::vector<icg_ba_problem> nx(next, next + n);
     std::vector<icg_ba_slide_window> cr(carry, carry + n);
-    std::vector<std::unique_ptr<double[]>> fc_tmp(n);
+    VisSlide vs;
+    vs.map = pa.map, vs.invdepth = a.invdepth, vs.f_new = a.f_new;
+    vs.lm_at.resize(n), vs.slot_at.resize(n);
     const int *cnt = (const int *) (H + b_cnt);
     for (int w = 0; w < n; w++) {
         const int *c = cnt + VIS_COUNTS * w;
-        if (c[3] != 0) {
+        if (c[3] >= VIS_EPACK_DUP) {
+            // the host packing's checks: reported as icg_ba_upload's packing reports them, at the point of the slide where it runs
+            if (vs.rc != ICG_OK) continue;
+            char eb[256];
+            if (c[3] == VIS_EPACK_DUP)
+                snprintf(eb, sizeof(eb), "icg_ba_upload: window %d factor %d: landmark %d has two reference nodes or two observations in node %d", w, c[4], c[9], c[10]);
+            else
+                snprintf(eb, sizeof(eb), "icg_ba_upload: window %d: landmark %d has more than 128 factors or the run table overflows", w, c[4]);
+            vs.rc = ICG_EINVAL, vs.err = eb;
+        } else if (c[3] != 0) {
             set_error("%s: window %d: %s (entry %d)", fn, w, c[3] > 0 && c[3] <= VIS_EROW ? what[c[3]] : "?", c[4]);
             return reject(ICG_EINVAL);
         }
@@ -1310,25 +1389,25 @@ static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_b
         icg_ba_slide_vision &v = vis[w];
         icg_ba_problem &p = nx[w];
         const int L = c[0], F = c[1];
-        int *lm_src = (int *) (H + b_lms) + W.lm_out, *f_src = (int *) (H + b_fsrc) + W.f_out;
-        p.L = L, p.F = F, p.invdepth = (double *) (H + b_invd) + W.lm_out, p.f_active = nullptr;
-        p.f_lm = (int *) (H + b_flm) + W.f_out, p.f_ref = (int *) (H + b_fref) + W.f_out, p.f_obs = (int *) (H + b_fobs) + W.f_out;
-        double *fc = v.f_const;
-        if (!fc) fc_tmp[w].reset(new double[14 * (size_t) std::max(F, 1)]), fc = fc_tmp[w].get();
-        const double *rows = (const double *) (H + b_fnew) + 14 * (size_t) W.nf_out;
-        for (int f = 0, t = 0; f < F; f++)
-            if (f_src[f] < 0) memcpy(fc + 14 * (size_t) f, rows + 14 * (size_t) t++, 112);
-        p.f_const = fc;
-        cr[w].lm_src = lm_src, cr[w].f_src = f_src;
+        // the vision half of the next window stays on the device: slide_body reads sizes only
+        p.L = L, p.F = F, p.invdepth = nullptr, p.f_active = nullptr, p.f_lm = p.f_ref = p.f_obs = nullptr, p.f_const = nullptr;
+        cr[w].lm_src = cr[w].f_src = nullptr;
+        vs.lm_at[w] = W.lm_out, vs.slot_at[w] = (int) n_lm + W.f_out;
         v.L = L, v.F = F, v.nan_dropped = c[5];
-        if (v.lm_src) memcpy(v.lm_src, lm_src, 4 * (size_t) L);
+        const int *f_src = (const int *) (H + b_fsrc) + W.f_out;
+        if (v.f_const) {
+            const double *rows = (const double *) (H + b_fnew) + 14 * (size_t) W.nf_out;
+            for (int f = 0, t = 0; f < F; f++)
+                if (f_src[f] < 0) memcpy(v.f_const + 14 * (size_t) f, rows + 14 * (size_t) t++, 112);
+        }
+        if (v.lm_src) memcpy(v.lm_src, (int *) (H + b_lms) + W.lm_out, 4 * (size_t) L);
         if (v.lm_origin) memcpy(v.lm_origin, (int *) (H + b_org) + W.lm_out, 4 * (size_t) L);
         if (v.nan_flags) memcpy(v.nan_flags, H + b_nan + W.lm_out, (size_t) W.oL + W.n_new);
         if (v.f_src) memcpy(v.f_src, f_src, 4 * (size_t) F);
-        if (v.f_lm) memcpy(v.f_lm, p.f_lm, 4 * (size_t) F);
-        if (v.f_ref) memcpy(v.f_ref, p.f_ref, 4 * (size_t) F);
-        if (v.f_obs) memcpy(v.f_obs, p.f_obs, 4 * (size_t) F);
-        if (v.invdepth) memcpy(v.invdepth, p.invdepth, 8 * (size_t) L);
+        if (v.f_lm) memcpy(v.f_lm, (int *) (H + b_flm) + W.f_out, 4 * (size_t) F);
+        if (v.f_ref) memcpy(v.f_ref, (int *) (H + b_fref) + W.f_out, 4 * (size_t) F);
+        if (v.f_obs) memcpy(v.f_obs, (int *) (H + b_fobs) + W.f_out, 4 * (size_t) F);
+        if (v.invdepth) memcpy(v.invdepth, (double *) (H + b_invd) + W.lm_out, 8 * (size_t) L);
     }
     std::vector<CullWin> lw(n);
     std::vector<int> lnobs(n);
@@ -1336,8 +1415,11 @@ static int vision_body(icg_ba *h, int n, const icg_ba_problem *next, const icg_b
         const int *c = cnt + VIS_COUNTS * w;
         lw[w].K = next[w].K, lw[w].L = c[0], lw[w].lm0 = wins[w].lm_out, lw[w].off0 = wins[w].lm_out + w, lw[w].obs0 = wins[w].lst_obs, lnobs[w] = c[8];
     }
-    rc = slide_body(h, n, nx.data(), cr.data(), integ, noise5, station3, fn, sharded, true, sharded ? &fp : nullptr, fr);
+    rc = slide_body(h, n, nx.data(), cr.data(), integ, noise5, station3, fn, sharded, &vs, sharded ? &fp : nullptr, fr);
     if (rc != ICG_OK) return rc;  // sharded: the group's agreement inside slide_body has committed every rank's slide, or none
+    // the host's copy of the slot -> factor tables (the next plain slide's old slots, the sharded marginalization's export)
+    for (int w = 0; w < n; w++)
+        memcpy(h->lm_fidx.h + (size_t) w * C.F, (const int *) (H + b_fidx) + wins[w].f_out, 4 * (size_t) h->dims.h[w].F);
     icg_ba::BuiltLists &B = h->built;
     B.cur = nb, B.at[nb] = at, B.n = n, B.nL = n_lm, B.nO = n_lo, B.win = std::move(lw), B.nobs = std::move(lnobs);
     return ICG_OK;
@@ -1959,7 +2041,7 @@ int icg_ba_slide_ins_resident(icg_ba *h, icg_ins *ins, int n_windows, const icg_
     for (int w = 0; w < n_windows; w++) integ[w] = io[w].integ;
     const FactorRows fr = {h->store.d[1 - h->store.cur], row0, nrow};
     rc = vis ? vision_body(h, n_windows, next, carry, integ.data(), noise5, station3, vis, fn, false, &fr)
-             : slide_body(h, n_windows, next, carry, integ.data(), noise5, station3, fn, false, false, nullptr, &fr);
+             : slide_body(h, n_windows, next, carry, integ.data(), noise5, station3, fn, false, nullptr, nullptr, &fr);
     if (rc != ICG_OK) return rc;
     ICG_CUDA(cudaStreamSynchronize(h->stream));
     for (int w = 0; w < n_windows; w++)

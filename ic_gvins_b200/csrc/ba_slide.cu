@@ -23,11 +23,11 @@ __global__ void __launch_bounds__(SLIDE_THREADS) ba_slide_gather(SlideArgs a) {
                 a.mix[(wK + k) * 9 + c - 7] = m >= 0 ? a.old_mix[(wK + m) * 9 + c - 7] : a.val[-(m + 1) + c];
         } else if (e < n1) {
             // updateParametersFromOptimizer stores depth = 1 / invdepth, the next addReprojectionParameters invdepth = 1 / depth
-            const int l = e - n0, m = a.map[W.lm_map + l];
-            a.rho[wL + l] = m >= 0 ? __ddiv_rn(1.0, __ddiv_rn(1.0, a.old_rho[wL + m])) : a.val[-(m + 1)];
+            const int l = e - n0, m = (W.vis ? a.vmap : a.map)[W.lm_map + l];
+            a.rho[wL + l] = m >= 0 ? __ddiv_rn(1.0, __ddiv_rn(1.0, a.old_rho[wL + m])) : (W.vis ? a.vlm : a.val)[-(m + 1)];
         } else if (e < n2) {
-            const int q = (e - n1) / 14, c = (e - n1) % 14, m = a.map[W.slot_map + q];
-            a.fc[(wF + q) * 14 + c] = m >= 0 ? a.old_fc[(wF + m) * 14 + c] : a.val[-(m + 1) + c];
+            const int q = (e - n1) / 14, c = (e - n1) % 14, m = (W.vis ? a.vmap : a.map)[W.slot_map + q];
+            a.fc[(wF + q) * 14 + c] = m >= 0 ? a.old_fc[(wF + m) * 14 + c] : (W.vis ? a.vfc : a.val)[-(m + 1) + c];
         } else if (e < n3) {
             const int k = (e - n2) / SLIDE_IMU, c = (e - n2) % SLIDE_IMU, m = a.map[W.imu_map + k];
             if (c < 480)

@@ -19,12 +19,15 @@ struct SlideWin {
     int r, from_marg;  // prior rows (0: none); 1: J0 / e0 from the marginalization workspace, 0: staged at j0 / e0
     int j0, e0;        // value offsets of the staged J0 (r x r row-major) and e0 (from_marg = 0)
     int slot;          // from_marg = 1: the window's slot of the workspace, or -1: no source here (H0, b0, c0 are written as zeros)
+    int vis;           // 1: lm_map / slot_map are in SlideArgs::vmap, their rows m < 0 start at -(m + 1) of vlm / vfc (the vision build's)
 };
 
 struct SlideArgs {
     const SlideWin *win;
     const int *map;
     const double *val;
+    const int *vmap;          // vision windows: landmark and record-slot maps written on the device (ba_pack_structure)
+    const double *vlm, *vfc;  // and the rows their entries m < 0 name: the built inverse depths, the new factors' constants
     int K, L, F, G, R;  // capacities: the handle's arrays are strided by them per window
     // the old window (copies of the handle's arrays at the same strides; old_fc is the f_const_s buffer the slide swaps out) -> the handle
     const double *old_pose, *old_mix, *old_rho, *old_fc, *old_blob, *old_U, *old_blh, *old_std;

@@ -283,4 +283,200 @@ cudaError_t launch_vision(const VisArgs &a, int n_windows, cudaStream_t stream) 
     return cudaGetLastError();
 }
 
+// pack_window's tables (ba_handle.cu) of one built window, in its orders.  Landmark positions: a stable counting sort by reference node (no
+// factor: last), placed by warp 0 in id order, 32 landmarks a step (__match_any_sync ranks the lanes of one key).  Record slots: factor order
+// within each landmark, placed by warp 0 the same way.  lin_vis runs: the greedy scan is sequential, one thread (L <= max_L steps).  Pairs in
+// key order ref K + obs; a run's Gram partials and its slots ordered by observing node: a warp per run, lane k for observing node k.
+constexpr int NO_FACTOR = 0x7fffffff;
+
+__global__ void __launch_bounds__(VIS_THREADS) ba_pack_structure(PackArgs a) {
+    __shared__ Scan::TempStorage tmp;
+    __shared__ int s_pair[VIS_MAX_NODES * VIS_MAX_NODES];  // (ref K + obs) -> pair, -1: none
+    __shared__ int s_part[VIS_MAX_NODES * VIS_MAX_NODES];  // pair -> its partials, then its first partial
+    __shared__ int s_bin[VIS_MAX_NODES + 1];
+    __shared__ int s_bad, s_nrun;
+    const int w = blockIdx.x, t = threadIdx.x, lane = t & 31;
+    const VisWin &W = a.win[w];
+    int *cnt = a.counts + (size_t) w * VIS_COUNTS;
+    const int L = cnt[0], F = cnt[1], K = W.nK;
+    if (cnt[3] != 0 || L > a.L || F > a.F) return;
+    const int *flm = a.f_lm + W.f_out, *fref = a.f_ref + W.f_out, *fobs = a.f_obs + W.f_out, *fsrc = a.f_src + W.f_out, *lms = a.lm_src + W.lm_out;
+    const size_t wL = (size_t) w * a.L, wF = (size_t) w * a.F, PM = (size_t) a.K * (a.K - 1);
+    const PackTables &T = a.out;
+    int *perm = T.lm_perm + wL, *off = T.lm_off + w * (a.L + 1), *meta = T.f_meta_s + wF * 4, *vb = T.vb_lm0 + (size_t) w * a.NVB;
+    int *nrun_of = T.ref_nrun + (size_t) w * a.K, *poff = T.part_off + w * (PM + 1), *pro = T.pair_ro + w * PM, *ord = T.vis_ord + wF;
+    uint8_t *act = T.f_active + wF;
+    int *fidx = a.fidx + W.f_out, *lmap = a.map + W.lm_out, *smap = a.map + a.nL + W.f_out;
+    // scratch: factors per landmark, first factor per landmark, position of each landmark, reference key by position (K: no factor), cursor
+    // per landmark (K by id first), new-factor rank (F), old slot of each old factor (oF), observing nodes of each run (NVB)
+    int *nf = a.scratch + W.pscr, *first = nf + L, *pos_of = first + L, *key = pos_of + L, *cur = key + L, *newt = cur + L, *oslot = newt + F,
+        *seen = oslot + W.oF;
+    const int *ometa = a.old_meta + wF * 4;
+    __syncthreads();  // every thread has read cnt before any writes it
+    for (int l = t; l < L; l += VIS_THREADS) nf[l] = 0, first[l] = NO_FACTOR;
+    for (int i = t; i < K * K; i += VIS_THREADS) s_pair[i] = -1;
+    for (int i = t; i <= K; i += VIS_THREADS) s_bin[i] = 0;
+    for (int i = t; i < a.K; i += VIS_THREADS) nrun_of[i] = 0;
+    for (int q = t; q < W.oF; q += VIS_THREADS) oslot[ometa[4 * q + 3]] = q;
+    if (t == 0) s_bad = NO_FACTOR;
+    __syncthreads();
+    for (int f = t; f < F; f += VIS_THREADS) {
+        const int l = flm[f];
+        atomicAdd(nf + l, 1), atomicMin(first + l, f);
+        s_pair[fref[f] * K + fobs[f]] = 0;
+        act[f] = 1;
+        newt[f] = fsrc[f] < 0;
+    }
+    for (int l = t; l < L; l += VIS_THREADS) lmap[l] = lms[l] >= 0 ? lms[l] : -(W.lm_out + l + 1);
+    __syncthreads();
+    // 1. landmark positions: by reference node, stable by id, landmarks without factors last
+    for (int l = t; l < L; l += VIS_THREADS) {
+        const int k = nf[l] ? fref[first[l]] : K;
+        cur[l] = k;
+        atomicAdd(s_bin + k, 1);
+    }
+    __syncthreads();
+    if (t == 0)
+        for (int k = 0, s = 0; k <= K; k++) {
+            const int c = s_bin[k];
+            s_bin[k] = s, s += c;
+        }
+    __syncthreads();
+    if (t < 32) {
+        for (int b = 0; b < L; b += 32) {
+            const int l = b + lane, k = l < L ? cur[l] : -1;
+            const unsigned peers = __match_any_sync(~0u, k), below = peers & ((1u << lane) - 1u);
+            if (l < L) {
+                const int p = s_bin[k] + __popc(below);
+                perm[p] = l, pos_of[l] = p, key[p] = k;
+            }
+            __syncwarp();
+            if (l < L && below == 0) s_bin[k] += __popc(peers);
+            __syncwarp();
+        }
+    }
+    __syncthreads();
+    // 2. CSR by position, and the rank of every new factor among the new factors (its row of f_new)
+    for (int p = t; p < L; p += VIS_THREADS) off[p] = nf[perm[p]];
+    __syncthreads();
+    block_exscan(off, L, tmp);
+    block_exscan(newt, F, tmp);
+    if (t == 0) off[L] = F;
+    for (int l = t; l < L; l += VIS_THREADS) cur[l] = off[pos_of[l]];
+    __syncthreads();
+    // 3. record slots in factor order within each landmark; the slot's row of the slide (old slot, or the new factor's constants)
+    if (t < 32) {
+        for (int b = 0; b < F; b += 32) {
+            const int f = b + lane, l = f < F ? flm[f] : -1;
+            const unsigned peers = __match_any_sync(~0u, l), below = peers & ((1u << lane) - 1u);
+            if (f < F) {
+                const int q = cur[l] + __popc(below);
+                meta[4 * q] = l, meta[4 * q + 1] = fref[f], meta[4 * q + 2] = fobs[f], meta[4 * q + 3] = f;
+                fidx[q] = f;
+                smap[q] = fsrc[f] >= 0 ? oslot[fsrc[f]] : -(14 * (W.nf_out + newt[f]) + 1);
+            }
+            __syncwarp();
+            if (f < F && below == 0) cur[l] += __popc(peers);
+            __syncwarp();
+        }
+    }
+    __syncthreads();
+    // a landmark has one reference node and at most one observation per node: the first factor that breaks it, in factor order
+    for (int p = t; p < L; p += VIS_THREADS) {
+        unsigned obs = 0u;
+        for (int q = off[p]; q < off[p + 1]; q++) {
+            const int o = meta[4 * q + 2];
+            if (meta[4 * q + 1] != key[p] || (obs >> o) & 1u) {
+                atomicMin(&s_bad, meta[4 * q + 3]);
+                break;
+            }
+            obs |= 1u << o;
+        }
+    }
+    __syncthreads();
+    if (s_bad != NO_FACTOR) {
+        if (t == 0) cnt[3] = VIS_EPACK_DUP, cnt[4] = s_bad, cnt[9] = flm[s_bad], cnt[10] = fobs[s_bad];
+        return;
+    }
+    // 4. lin_vis runs: whole landmarks of one reference node, <= 128 record slots each
+    if (t == 0) {
+        int nrun = 0, l0 = 0, err = 0;
+        while (l0 < L) {
+            const int ref = key[l0];
+            int l1 = l0;
+            while (l1 < L && key[l1] == ref && off[l1 + 1] - off[l0] <= 128) l1++;
+            if (l1 == l0 || nrun >= a.NVB - 2) {
+                err = l1 == l0 ? VIS_EPACK_LM128 : VIS_EPACK_RUNS;
+                break;
+            }
+            if (ref < K) nrun_of[ref]++;
+            vb[nrun++] = l0;
+            l0 = l1;
+        }
+        if (err) {
+            cnt[3] = err, cnt[4] = perm[l0];
+            nrun = -1;
+        } else {
+            vb[nrun] = L, vb[a.NVB - 1] = nrun;
+        }
+        s_nrun = nrun;
+    }
+    // 5. pairs in key order
+    const int KK = K * K;
+    {
+        const int chunk = (KK + VIS_THREADS - 1) / VIS_THREADS, b = t * chunk, e = min(KK, b + chunk);
+        int c = 0;
+        for (int i = b; i < e; i++) c += s_pair[i] == 0;
+        int base, P;
+        Scan(tmp).ExclusiveSum(c, base, P);
+        for (int i = b; i < e; i++)
+            if (s_pair[i] == 0) s_pair[i] = base, pro[base] = ((i / K) << 8) | (i % K), base++;
+        for (int i = t; i < P; i += VIS_THREADS) s_part[i] = 0;
+        if (t == 0) T.npairs[w] = P;
+    }
+    __syncthreads();
+    const int nrun = s_nrun;
+    if (nrun < 0) return;
+    // 6. each run's observing nodes; a pair's partials: one per run of its reference node that observes from its node
+    for (int r = t; r < nrun; r += VIS_THREADS) {
+        unsigned s = 0u;
+        for (int q = off[vb[r]]; q < off[vb[r + 1]]; q++) s |= 1u << meta[4 * q + 2];
+        seen[r] = (int) s;
+        const int ref = key[vb[r]];
+        for (unsigned m = s; m; m &= m - 1) atomicAdd(s_part + s_pair[ref * K + __ffs(m) - 1], 1);
+    }
+    __syncthreads();
+    {
+        const int P = T.npairs[w], total = block_exscan(s_part, P, tmp);
+        for (int i = t; i < P; i += VIS_THREADS) poff[i] = s_part[i];
+        if (t == 0) poff[P] = total;
+    }
+    __syncthreads();
+    // 7. vis_ord: warp per run, lane k counts the run's slots observed from node k; their Gram partial is the pair's first plus the earlier
+    // runs of the same reference node that observe from k
+    for (int r = t >> 5; r < nrun; r += VIS_THREADS / 32) {
+        const int q0 = off[vb[r]], q1 = off[vb[r + 1]];
+        if (q0 == q1) continue;
+        const int ref = meta[4 * q0 + 1];
+        int c = 0;
+        for (int q = q0; q < q1; q++) c += meta[4 * q + 2] == lane;
+        int incl = c;
+        for (int d = 1; d < 32; d <<= 1) {
+            const int v = __shfl_up_sync(~0u, incl, d);
+            if (lane >= d) incl += v;
+        }
+        int at = q0 + incl - c;
+        if (c == 0) continue;
+        int pidx = s_part[s_pair[ref * K + lane]];
+        for (int r2 = r - 1; r2 >= 0 && key[vb[r2]] == ref; r2--) pidx += (seen[r2] >> lane) & 1;
+        for (int q = q0; q < q1; q++)
+            if (meta[4 * q + 2] == lane) ord[at++] = (q - q0) | (pidx << 8);
+    }
+}
+
+cudaError_t launch_pack(const PackArgs &a, int n_windows, cudaStream_t stream) {
+    ba_pack_structure<<<n_windows, VIS_THREADS, 0, stream>>>(a);
+    return cudaGetLastError();
+}
+
 }  // namespace icg

@@ -40,12 +40,20 @@ struct VisWin {
     // bounds: next landmarks Lb = oL + n_new, next factors Fb = oF + n_obs + n_new, new factors Nb = n_obs + n_new
     int lm_out, f_out, nf_out, scr;  // offsets of the window's output rows (Lb, Fb, Nb) and int scratch
     int lst_obs;                     // the next culling's lists: first entry of the window's observations (Ob = n_cull_obs + n_obs + 2 n_new)
+    int pscr;                        // ba_pack_structure's int scratch (5 Lb + Fb + oF + NVB)
 };
 
 // per window: [L, F, new factors, error code, error index, landmarks dropped for a NaN inverse depth, the observation count and the new-point
-// count the kernel read (a landmark shard's ranks must read the same), the entries of the next culling's lists (0 when they are not emitted)]
-constexpr int VIS_COUNTS = 9;
-enum VisError { VIS_OK = 0, VIS_EOBS_FACTOR = 1, VIS_ECOUNT = 2, VIS_ESRC = 3, VIS_ENODE = 4, VIS_ELM = 5, VIS_EDUP = 6, VIS_EFRAME = 7, VIS_EROW = 8 };
+// count the kernel read (a landmark shard's ranks must read the same), the entries of the next culling's lists (0 when they are not emitted),
+// the landmark and observing node of a VIS_EPACK_DUP factor]
+constexpr int VIS_COUNTS = 11;
+// VIS_EPACK_*: ba_pack_structure's rejections, the checks of icg_ba_upload's packing the build does not make (error index: the factor of a
+// landmark with two reference nodes or two observations in one node; the landmark that starts a run of more than 128 factors or that the run
+// table has no room for)
+enum VisError {
+    VIS_OK = 0, VIS_EOBS_FACTOR = 1, VIS_ECOUNT = 2, VIS_ESRC = 3, VIS_ENODE = 4, VIS_ELM = 5, VIS_EDUP = 6, VIS_EFRAME = 7, VIS_EROW = 8,
+    VIS_EPACK_DUP = 9, VIS_EPACK_LM128 = 10, VIS_EPACK_RUNS = 11
+};
 
 struct VisArgs {
     const VisWin *win;
@@ -74,5 +82,30 @@ struct VisArgs {
 };
 
 cudaError_t launch_vision(const VisArgs &a, int n_windows, cudaStream_t stream);
+
+// The structure tables of the built windows, as icg_ba_upload packs them (ba_handle.cu, pack_window), into second buffers at the handle's
+// strides.  The slide makes them the handle's once every check has passed.
+struct PackTables {
+    int *f_meta_s, *vb_lm0, *lm_off, *lm_perm, *ref_nrun, *part_off, *pair_ro, *vis_ord, *npairs;
+    uint8_t *f_active;
+};
+
+struct PackArgs {
+    const VisWin *win;
+    int K, L, F, NVB;   // the handle's capacities and run-table stride
+    int *counts;        // ba_vision_build's (L, F and its error code are read; a packing error is written there)
+    const int *lm_src, *f_lm, *f_ref, *f_obs, *f_src;  // ba_vision_build's rows
+    const int *old_meta;                                // the handle's f_meta_s: the old window's slot -> factor table
+    PackTables out;
+    // per window: the slot -> factor table at f_out (the host's copy); the slide's maps, landmarks at lm_out, record slots at nL + f_out:
+    // m >= 0 the old landmark / slot carried, m < 0 the row at -(m + 1) of ba_vision_build's invdepth / f_new (doubles)
+    int *fidx, *map;
+    int nL;
+    int *scratch;
+};
+
+// ba_pack_structure, one CTA per window, after ba_vision_build on the same stream; a window the build rejected or that exceeds the handle is
+// skipped
+cudaError_t launch_pack(const PackArgs &a, int n_windows, cudaStream_t stream);
 
 }  // namespace icg

@@ -1134,6 +1134,26 @@ typedef struct icg_ba_linearization {
 } icg_ba_linearization;
 int icg_ba_peek_linearization(icg_ba *h, int window, icg_ba_linearization *out);
 
+/*
+ * Read-out of one window's structure tables for tests: the integer tables icg_ba_upload packs (or icg_ba_slide_vision_resident packs on the
+ * device), in the window's own sizes.  Synchronises the handle's stream; changes nothing.  Every array pointer may be NULL (not copied).
+ */
+typedef struct icg_ba_structure {
+    int32_t K, L, F;    /* out: the window's sizes */
+    int32_t n_runs;     /* out: lin_vis runs */
+    int32_t npairs;     /* out: (reference node, observing node) pairs */
+    int32_t *lm_perm;   /* [L]: landmark id at each position (by reference node, stable by id, landmarks without factors last) */
+    int32_t *lm_off;    /* [L + 1]: CSR of the record slots by landmark position */
+    int32_t *f_meta_s;  /* [F][4]: per record slot (landmark, reference node, observing node, factor id): column 3 is the slot -> factor table */
+    int32_t *vb_lm0;    /* [n_runs + 1]: first landmark position of every run, then L */
+    int32_t *ref_nrun;  /* [K]: runs per reference node */
+    int32_t *part_off;  /* [npairs + 1]: CSR of the Gram partials by pair (in run order within a pair) */
+    int32_t *pair_ro;   /* [npairs]: reference node << 8 | observing node, in key order */
+    int32_t *vis_ord;   /* [F]: each run's slots ordered by observing node (stable): run-local slot | partial << 8 */
+    uint8_t *f_active;  /* [F]: by factor id */
+} icg_ba_structure;
+int icg_ba_peek_structure(icg_ba *h, int window, icg_ba_structure *out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -2,7 +2,9 @@
 
   host rows : icg_ba_slide_resident with the vision rows already built on the host (the restatement in tests/slide_vision_oracle.py builds
               them; that build is numpy and is not timed: a C++ integrator's own graph walk takes its place)
-  device    : icg_ba_slide_vision_resident from the same culled windows and the same new keyframe observations in device memory
+  device    : icg_ba_slide_vision_resident from the same culled windows and the same new keyframe observations in device memory, through the
+              default binding (every built row back on the host, capacity-sized arrays)
+  lean      : the same call through slide_vision(rows=False): only what the rest of the keyframe cycle reads on the host comes back
 
 Per repetition the handle is restored outside the timed region (upload, solve, culling, culled marginalization).  Wall time from the call to a
 device synchronise (CUDA events around it too), the kernel's time from torch.profiler in a separate pass, and the bytes each path moves
@@ -142,13 +144,13 @@ def main():
     def host():
         s.slide([copy.deepcopy(x[2]) for x in cases], [x[3] for x in cases], True)
 
-    def device():
-        s.slide_vision([copy.deepcopy(x[0]) for x in cases], [copy.deepcopy(x[1]) for x in cases], [x[4] for x in cases])
+    def device(rows=True):
+        s.slide_vision([copy.deepcopy(x[0]) for x in cases], [copy.deepcopy(x[1]) for x in cases], [x[4] for x in cases], rows=rows)
 
-    times = {"host_rows": [], "device": []}
-    ev = {"host_rows": [], "device": []}
+    times = {"host_rows": [], "device": [], "lean": []}
+    ev = {"host_rows": [], "device": [], "lean": []}
     for rep in range(args.reps + 1):
-        for name, fn in (("host_rows", host), ("device", device)):
+        for name, fn in (("host_rows", host), ("device", device), ("lean", lambda: device(False))):
             restore()
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             t0 = time.perf_counter()
@@ -164,16 +166,31 @@ def main():
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         device()
         torch.cuda.synchronize()
-    kern = {e.key: e.device_time_total / max(1, e.count) / 1e3 for e in prof.key_averages() if "ba_vision_build" in e.key or "ba_lm_ref_fill" in e.key}
+    kern = {e.key: e.device_time_total / max(1, e.count) / 1e3 for e in prof.key_averages()
+            if any(k in e.key for k in ("ba_vision_build", "ba_pack_structure", "ba_slide_gather", "ba_lm_ref_fill"))}
+    # bytes from the shapes.  The vision call copies back per window [counts | slot -> factor table (bound Fb = F + n_obs + n_new)] and each row
+    # array a caller asks for at its bound (Lb = L + n_new landmarks, Fb factors, n_obs + n_new new factor rows); the host-rows slide uploads
+    # the structure tables at the handle's capacities, which the vision call writes on the device
+    Lb = sum(p["L"] + nn for p, nn in zip(solved, [len(x[4]["new_depth"]) for x in cases]))
+    Fb = sum(p["F"] for p in solved) + n_obs_tot + n_new_tot
+    Nb = n_obs_tot + n_new_tot
+    counts = 4 * 11 * B
+    d2h_lean = counts + 4 * Fb + 4 * (2 * Lb + 4 * Fb) + Lb
+    d2h_default = d2h_lean + 8 * Lb + 112 * Nb
+    Kc, Lc, Fc = K, L + 64, F
+    nvb = (Fc + 127 - Kc) // (128 - Kc) + Lc // 128 + 4 + Kc
+    PM = Kc * (Kc - 1)
+    h2d_tables = B * (16 * Fc + 4 * nvb + 4 * (Lc + 1) + 4 * Lc + 4 * Kc + 4 * (PM + 1) + 4 * PM + 4 * Fc + 4 + Fc)
     F_tot = sum(x[5]["F"] for x in cases)
     L_tot = sum(x[5]["L"] for x in cases)
     new_f = sum(int((x[5]["f_src"] < 0).sum()) for x in cases)
     out = dict(metric=f"slide_vision cfg-{args.cfg}", windows=B, gpu=gpu, power_limit_w=plim, reps=args.reps,
                host_rows_ms_median=statistics.median(times["host_rows"]), device_ms_median=statistics.median(times["device"]),
-               host_rows_event_ms_median=statistics.median(ev["host_rows"]), device_event_ms_median=statistics.median(ev["device"]),
+               lean_ms_median=statistics.median(times["lean"]), host_rows_event_ms_median=statistics.median(ev["host_rows"]),
+               device_event_ms_median=statistics.median(ev["device"]), lean_event_ms_median=statistics.median(ev["lean"]),
                kernel_ms=kern, tracked_obs=n_obs_tot, new_points=n_new_tot, next_L=L_tot, next_F=F_tot, new_factors=new_f,
                bytes_h2d_vision_inputs=int(4 * sum(len(x[4]["obs_factor"]) for x in cases)),
-               bytes_d2h_structure=int(4 * (2 * L_tot + 4 * F_tot) + 8 * L_tot + 112 * (n_obs_tot + n_new_tot)),
+               bytes_d2h_device=int(d2h_default), bytes_d2h_lean=int(d2h_lean), bytes_h2d_structure_tables_host_rows=int(h2d_tables),
                bytes_h2d_host_rows_vision=int(8 * (L_tot - sum(int((x[5]["lm_src"] >= 0).sum()) for x in cases)) + 112 * new_f))
     print(json.dumps(out))
 
