@@ -109,6 +109,7 @@ ABI = {
     "icg_ba_update_and_cull_built": ([vp, c_int, vp, vp, c_double, vp, vp], c_int),
     "icg_ba_shard_update_and_cull_built": ([vp, c_int, vp, vp, c_double, vp, vp], c_int),
     "icg_ba_marginalize_resident_culled": ([vp, c_int, vp, vp, vp, vp, vp], c_int),
+    "icg_ba_marginalize_built": ([vp, c_int, vp, vp, vp, vp], c_int),
     "icg_ba_reintegrate_resident": ([vp, c_int, vp, vp, vp, vp], c_int),
     "icg_ba_shard_reintegrate_resident": ([vp, c_int, vp, vp, vp, vp], c_int),
     "icg_ba_slide_resident": ([vp, c_int, vp, vp], c_int),

@@ -580,6 +580,21 @@ class WindowSolver:
                   "icg_ba_marginalize_resident_culled")
         return self.marg_collect(call)
 
+    def marginalize_built(self, problems, num_marg=1, node_in_map=None, want_schur=True):
+        """marginalize(resident=True, culled=...) after update_and_cull_built(), with the factor set and the column map built on the device
+        (icg_ba_marginalize_built): the problem dicts need their camera side only (f_lm, f_ref, f_obs, f_active and invdepth may be empty).
+        node_in_map[w] (K flags) names the keyframes still in the map (all of them when None).  Returns marginalize()'s dicts, bit for bit the
+        ones marginalize(resident=True, culled=...) returns on the same culling; single-GPU handles only."""
+        if isinstance(problems, dict):
+            problems = [problems]
+        if node_in_map is None:
+            node_in_map = [np.ones(p["K"], np.uint8) for p in problems]
+        call = self.marg_prepare(problems, num_marg, want_schur)
+        nim = [np.ascontiguousarray(m, np.uint8) for m in node_in_map]
+        ptrs = (vp * len(nim))(*[vp(m.ctypes.data) for m in nim])
+        check(lib().icg_ba_marginalize_built(self._h, call["n"], call["arr"], vp(call["nm"].ctypes.data), ptrs, call["pri"]), "icg_ba_marginalize_built")
+        return self.marg_collect(call)
+
     def update_and_cull(self, problems, camera, std, cull_inputs):
         """updateParametersFromOptimizer + gvinsOutlierCulling (IG/ic_gvins.cc:1299-1389, 1035-1128) on the windows this handle has just
         solved (icg_ba_update_and_cull_resident).  camera: a camera.Camera or CameraStruct; std: reprojection_error_std_.  cull_inputs: one

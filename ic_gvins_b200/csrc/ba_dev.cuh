@@ -141,6 +141,26 @@ struct MargDev {
     int n0cap, mcap, rcap;
 };
 
+// marg_select_built (icg_ba_marginalize_built): the factor set and the column map from the built culling, on the device.  MargSelWin: one
+// window as the host stages it (the built lists' slices, num_marg, node_in_map and the camera side's touched blocks); out: per window
+// MARG_SEL_HDR + 2 max_K ints [m, r, nblocks, invalid observations, -, -, -, -] then the remained blocks, type | node << 2 each
+constexpr int MARG_SEL_HDR = 8;
+constexpr int MARG_SEL_THREADS = 256;
+struct MargSelWin {
+    int lm0, off0, obs0, num_marg;  // CullWin's slices of the built lists and the culling's flags
+    int ext, td;                    // the previous prior's block table names ext / td
+    uint8_t tp[BA_MAX_NODES], tm[BA_MAX_NODES];  // pose / mix blocks the camera-side factors touch
+    uint8_t in_map[BA_MAX_NODES];                // node_in_map
+};
+struct MargSelArgs {
+    const MargSelWin *win;
+    const int *ref, *off, *node, *fac;  // the built lists (CullSrc)
+    const uint8_t *lm_outlier, *obs_outlier;
+    uint8_t *fmask;  // [NW][F] the factor set, by factor id
+    int *ftab;       // [NW][F] scratch: landmark * BA_MAX_NODES + observing node, by factor id
+    int *out;        // [n][MARG_SEL_HDR + 2 K]
+};
+
 constexpr int MARG_PAIR_MAXN = 160;  // 160^2 doubles = 204.8 KB per CTA
 constexpr int MARG_CTA_MAXN = 118;     // 2 * 118^2 doubles = 222.8 KB
 constexpr int MARG_CTA_THREADS = 512;  // 64 pair slots >= MARG_CTA_MAXN / 2
@@ -187,6 +207,7 @@ __global__ void ba_marg_gather(BaCaps C, BaDev D, const long long *heads, const 
 __global__ void ba_marg_fill(BaCaps Cm, BaDev Dm, BaCaps C, BaDev D, const double *rows, const int *row0, const int *fidx);
 
 __global__ void marg_prepare(BaDev D, MargDev M, int n, int restore);
+__global__ void marg_select_built(BaCaps C, BaDev D, MargDev M, MargSelArgs a);
 __global__ void marg_assemble(BaCaps C, BaDev D, MargDev M);
 __global__ void marg_jacobi(MargDev M, int which);
 __global__ void marg_jacobi_pair(MargDev M, int which);

@@ -107,6 +107,8 @@ struct icg_ba {
     HostDev<int> marg_map;
     HostDev<double> marg_oJ0, marg_oe0, marg_oHp, marg_obp;
     HostDev<uint8_t> marg_fmask;  // factor set of icg_ba_marginalize_resident_culled (ba_lin_vis reads it in place of f_active)
+    HostDev<unsigned char> marg_sel;  // icg_ba_marginalize_built's staging [MargSelWin | headers and block tables], grown on demand
+    int *marg_ftab = nullptr;         // its device scratch (marg_select_built: NW x max_F ints), allocated on first use
     HostDev<unsigned char> cull;   // post-solve update + culling: staging [inputs | outputs], grown on demand
     HostDev<unsigned char> vis;    // icg_ba_slide_vision_resident's staging, grown on demand
     HostDev<unsigned char> reint;  // the reintegration's staging, grown on demand

@@ -100,6 +100,32 @@ static void prior_commit(icg_ba *h, int n, const icg_ba_prior *out, int first, i
     P.n = n, P.sharded = step > 1;
 }
 
+// The blocks the camera-side factors of the marginalization touch (MarginalizationInfo::addResidualBlockInfo, marginalization_info.h:103-121):
+// the preintegration factors k < num_marg (factor k joins node k and node k + 1), GNSS at the removed nodes, the first-window priors and the
+// previous prior's blocks.  tp / tm: K flags each, set (never cleared) here; ext / td: the previous prior names them
+static void marg_camera_touched(const icg_ba_problem &p, int nm, char *tp, char *tm, bool *ext, bool *td) {
+    for (int k = 0; k < nm && k < p.n_imu; k++) tp[k] = tm[k] = tp[k + 1] = tm[k + 1] = 1;
+    for (int g = 0; g < p.n_gnss; g++)
+        if (p.gnss_node[g] < nm) tp[p.gnss_node[g]] = 1;
+    if (p.has_pose_prior) tp[0] = 1;
+    if (p.has_mix_prior) tm[0] = 1;
+    for (int b = 0; b < p.marg_nblocks && p.marg_r > 0; b++) {
+        const int t = p.marg_block_type[b], nd = p.marg_block_node[b];
+        if (t == 0) tp[nd] = 1;
+        else if (t == 1) tm[nd] = 1;
+        else if (t == 2) *ext = true;
+        else *td = true;
+    }
+}
+
+// num_marg and the output arrays of window w (every entry point checks them before anything is written)
+static bool marg_out_ok(const icg_ba_problem &p, int nm, const icg_ba_prior &o) {
+    return nm >= 1 && nm < p.K && o.block_type && o.block_node && o.x0 && o.J0 && o.e0 && o.rcap >= 15 * (p.K - nm) + 7;
+}
+
+static int marg_solve(icg_ba *h, int n, const icg_ba_problem *problems, const int32_t *num_marg, icg_ba_prior *out, bool resident,
+                      const uint8_t *const *fmask, const std::function<int(int *)> *agree, bool dev_structure);
+
 // fmask (resident only, may be NULL): per window, the factor set to marginalize in place of the problem's activity (F bytes each); it reaches
 // ba_lin_vis through a copy of the device view, so the handle's own f_active is never written.
 // agree (may be NULL): called once the structure is known, with {largest m, largest r, 1 if a window is rejected} of this batch; it returns
@@ -142,7 +168,7 @@ static int marginalize_body(icg_ba *h, int n_windows, const icg_ba_problem *prob
         const icg_ba_problem &p = problems[w];
         const int nm = num_marg[w];
         icg_ba_prior &o = out[w];
-        if (nm < 1 || nm >= p.K || !o.block_type || !o.block_node || !o.x0 || !o.J0 || !o.e0 || o.rcap < 15 * (p.K - nm) + 7) {
+        if (!marg_out_ok(p, nm, o)) {
             set_error("icg_ba_marginalize: window %d: num_marg=%d out of range or output arrays missing / too small (rcap=%d)", w, nm, o.rcap);
             return ICG_EINVAL;
         }
@@ -161,18 +187,7 @@ static int marginalize_body(icg_ba *h, int n_windows, const icg_ba_problem *prob
         // marginalization_info.h:103-121): removed nodes without any factor get no columns
         for (int f = 0; f < p.F; f++)
             if (!(act && !act[f]) && p.f_ref[f] < nm) tp[p.f_ref[f]] = 1;
-        for (int k = 0; k < nm && k < p.n_imu; k++) tp[k] = tm[k] = tp[k + 1] = tm[k + 1] = 1;  // factor k joins node k and node k + 1
-        for (int g = 0; g < p.n_gnss; g++)
-            if (p.gnss_node[g] < nm) tp[p.gnss_node[g]] = 1;
-        if (p.has_pose_prior) tp[0] = 1;
-        if (p.has_mix_prior) tm[0] = 1;
-        for (int b = 0; b < p.marg_nblocks && p.marg_r > 0; b++) {
-            const int t = p.marg_block_type[b], nd = p.marg_block_node[b];
-            if (t == 0) tp[nd] = 1;
-            else if (t == 1) tm[nd] = 1;
-            else if (t == 2) has_ext = true;
-            else has_td = true;
-        }
+        marg_camera_touched(p, nm, tp.data(), tm.data(), &has_ext, &has_td);
         int idx = 0;
         for (int k = 0; k < C.K; k++) pose_col[k] = mix_col[k] = -1;
         for (int k = 0; k < nm; k++) {
@@ -207,6 +222,18 @@ static int marginalize_body(icg_ba *h, int n_windows, const icg_ba_problem *prob
             return ICG_EUNSUPPORTED;
         }
     }
+    return marg_solve(h, n, problems, num_marg, out, resident, fmask, agree, false);
+}
+
+// The launch sequence of every marginalization once the batch's structure is known: out[w]'s m, r, nblocks and block tables, and the column
+// map -- in marg_map's host half (and the factor set in marg_fmask's when fmask is given), uploaded here, or already on the device
+// (dev_structure: marg_select_built wrote both).  Then the eigensolver kernels the batch's largest blocks select, the prior's D2H and the
+// write-back into out, x0 from problems' camera side.
+static int marg_solve(icg_ba *h, int n, const icg_ba_problem *problems, const int32_t *num_marg, icg_ba_prior *out, bool resident,
+                      const uint8_t *const *fmask, const std::function<int(int *)> *agree, bool dev_structure) {
+    const BaCaps &C = h->C;
+    MargDev &M = h->M;
+    int rc = ICG_OK;
     int max_m = 0, max_r = 0, max_n0 = 0;
     for (int w = 0; w < n; w++) max_m = std::max(max_m, out[w].m), max_r = std::max(max_r, out[w].r), max_n0 = std::max(max_n0, out[w].m + out[w].r);
     int sel_m = max_m, sel_r = max_r;  // what the eigensolver kernels are chosen by
@@ -231,10 +258,10 @@ static int marginalize_body(icg_ba *h, int n_windows, const icg_ba_problem *prob
         h->marg_cluster_ok = cudaOccupancyMaxActiveClusters(&nclusters, marg_jacobi_cluster, &L.cfg) == cudaSuccess && nclusters > 0 ? 1 : 0;
         cudaGetLastError();  // a refused query is an answer (the global kernel takes those blocks), not an error of this call
     }
-    ICG_CUDA(h->marg_map.up(s, (size_t) n * M.map_stride));
+    if (!dev_structure) ICG_CUDA(h->marg_map.up(s, (size_t) n * M.map_stride));
     BaDev D = h->D;
-    if (fmask) {
-        ICG_CUDA(h->marg_fmask.up(s, (size_t) n * C.F));
+    if (fmask || dev_structure) {
+        if (!dev_structure) ICG_CUDA(h->marg_fmask.up(s, (size_t) n * C.F));
         D.f_active = h->marg_fmask.d;
     }
     const size_t smem = sizeof(double) * (8 * 480 + 2 * (size_t) C.R) + sizeof(int) * (size_t) C.R + 64;
@@ -1899,6 +1926,111 @@ int icg_ba_marginalize_resident_culled(icg_ba *h, int n_windows, const icg_ba_pr
     }
     if (h->D.world > 1) return marginalize_sharded(h, n_windows, problems, num_marg, out, mp.data(), "icg_ba_marginalize_resident_culled");
     return marginalize_body(h, n_windows, problems, num_marg, out, true, mp.data());
+}
+
+int icg_ba_marginalize_built(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg, const uint8_t *const *node_in_map,
+                             icg_ba_prior *out) {
+    static const char *fn = "icg_ba_marginalize_built";
+    if (h && h->D.world > 1) {
+        set_error("%s: not available on a landmark-sharded handle (its group marginalizes with icg_ba_marginalize_resident_culled and NULL lists "
+                  "after icg_ba_shard_update_and_cull_built)", fn);
+        return ICG_EUNSUPPORTED;
+    }
+    int rc = resident_single_rank(h, n_windows, problems, fn);
+    if (rc != ICG_OK) return rc;
+    if (!num_marg || !node_in_map || !out) {
+        set_error("%s: bad arguments", fn);
+        return ICG_EINVAL;
+    }
+    const icg_ba::CullResult &cul = h->culled;
+    if (cul.n != n_windows) {
+        set_error("%s: no culling of these %d windows is current (icg_ba_update_and_cull_built, with no upload or slide since)", fn, n_windows);
+        return ICG_EINVAL;
+    }
+    if (!cul.host.ref) {
+        set_error("%s: the current culling walked host lists (icg_ba_update_and_cull_resident); this call needs a culling on the built lists "
+                  "(icg_ba_update_and_cull_built)", fn);
+        return ICG_EINVAL;
+    }
+    const BaCaps &C = h->C;
+    const int n = n_windows;
+    for (int w = 0; w < n; w++) {
+        const icg_ba_problem &p = problems[w];
+        const CullWin &W = cul.win[w];
+        if (p.K != W.K || p.L != W.L || !node_in_map[w]) {
+            set_error("%s: window %d: sizes differ from the culled window's (K %d, L %d) or node_in_map missing", fn, w, W.K, W.L);
+            return ICG_EINVAL;
+        }
+        if (!marg_out_ok(p, num_marg[w], out[w])) {
+            set_error("%s: window %d: num_marg=%d out of range or output arrays missing / too small (rcap=%d)", fn, w, num_marg[w], out[w].rcap);
+            return ICG_EINVAL;
+        }
+    }
+    ICG_CUDA(cudaSetDevice(h->device));
+    if ((rc = marg_alloc(h)) != ICG_OK) return rc;
+    if (!h->marg_ftab) {
+        if (cudaMalloc(&h->marg_ftab, sizeof(int) * (size_t) C.NW * std::max(1, C.F)) != cudaSuccess) {
+            h->marg_ftab = nullptr;
+            set_error("%s: scratch allocation failed", fn);
+            return ICG_ENOMEM;
+        }
+        h->dev_only.push_back(h->marg_ftab);
+    }
+    // staging [MargSelWin x n | per window MARG_SEL_HDR + 2 max_K ints out]: the camera side up, the headers and block tables down
+    const int so = MARG_SEL_HDR + 2 * C.K;
+    Layout lay;
+    const size_t i_win = lay.take(sizeof(MargSelWin) * n), i_out = lay.take(sizeof(int) * (size_t) n * so);
+    if ((rc = hd_reserve(h, h->marg_sel, lay.size(), fn)) != ICG_OK) return rc;
+    unsigned char *H = h->marg_sel.h, *Dv = h->marg_sel.d;
+    for (int w = 0; w < n; w++) {
+        const icg_ba_problem &p = problems[w];
+        const CullWin &cw = cul.win[w];
+        MargSelWin &W = ((MargSelWin *) (H + i_win))[w];
+        memset(&W, 0, sizeof(W));
+        W.lm0 = cw.lm0, W.off0 = cw.off0, W.obs0 = cw.obs0, W.num_marg = num_marg[w];
+        char tp[BA_MAX_NODES] = {}, tm[BA_MAX_NODES] = {};
+        bool ext = false, td = false;
+        marg_camera_touched(p, num_marg[w], tp, tm, &ext, &td);
+        for (int k = 0; k < p.K; k++) W.tp[k] = tp[k], W.tm[k] = tm[k], W.in_map[k] = node_in_map[w][k] != 0;
+        W.ext = ext, W.td = td;
+    }
+    cudaStream_t s = h->stream;
+    ICG_CUDA(cudaMemcpyAsync(Dv + i_win, H + i_win, sizeof(MargSelWin) * n, cudaMemcpyHostToDevice, s));
+    MargSelArgs a;
+    a.win = (const MargSelWin *) (Dv + i_win);
+    a.ref = cul.dev.ref, a.off = cul.dev.off, a.node = cul.dev.node, a.fac = cul.dev.fac;
+    a.lm_outlier = cul.lm_outlier, a.obs_outlier = cul.obs_outlier;
+    a.fmask = h->marg_fmask.d, a.ftab = h->marg_ftab, a.out = (int *) (Dv + i_out);
+    marg_select_built<<<n, MARG_SEL_THREADS, 0, s>>>(C, h->D, h->M, a);
+    ICG_CHECK_LAUNCH();
+    count_launch();
+    ICG_CUDA(cudaMemcpyAsync(H + i_out, Dv + i_out, sizeof(int) * (size_t) n * so, cudaMemcpyDeviceToHost, s));
+    ICG_CUDA(cudaStreamSynchronize(s));
+    // every check before the marginalization kernels: a rejected call leaves the culling, the built lists and the resident prior current
+    const int *hdr = (const int *) (H + i_out);
+    for (int w = 0; w < n; w++)
+        if (hdr[(size_t) w * so + 3] > 0) {
+            set_error("%s: window %d: %d observations of the built lists name a factor outside [-1, F) or one of another landmark or node", fn, w,
+                      hdr[(size_t) w * so + 3]);
+            return ICG_EINVAL;
+        }
+    for (int w = 0; w < n; w++) {
+        const int *o = hdr + (size_t) w * so, m = o[0], r = o[1];
+        if (m > MARG_MAXN || r > MARG_MAXN) {
+            set_error("%s: window %d: %s=%d exceeds the %d rows of the largest eigensolver kernel", fn, w, m > MARG_MAXN ? "m" : "r", m > MARG_MAXN ? m : r,
+                      MARG_MAXN);
+            return ICG_EUNSUPPORTED;
+        }
+    }
+    for (int w = 0; w < n; w++) {
+        const int *o = hdr + (size_t) w * so;
+        icg_ba_prior &q = out[w];
+        q.m = o[0], q.r = o[1], q.nblocks = o[2];
+        for (int b = 0; b < q.nblocks; b++) q.block_type[b] = o[MARG_SEL_HDR + b] & 3, q.block_node[b] = o[MARG_SEL_HDR + b] >> 2;
+    }
+    h->prior.n = 0;  // the workspace is about to be overwritten
+    h->lin_ready = false;  // the linearisation takes the buffer the window uses
+    return marg_solve(h, n, problems, num_marg, out, true, nullptr, nullptr, true);
 }
 
 int icg_ba_slide_resident(icg_ba *h, int n, const icg_ba_problem *next, const icg_ba_slide_window *carry) {

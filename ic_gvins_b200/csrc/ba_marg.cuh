@@ -40,6 +40,118 @@ __global__ void marg_prepare(BaDev D, MargDev M, int n, int restore) {
     }
 }
 
+// The structure of icg_ba_marginalize_built, one CTA per window: the factor set gvinsMarginalization builds from the culling (IG/ic_gvins.cc:
+// 1558-1609) into a.fmask, and updateParameterBlocksIndex's column map (marginalization_info.h:228-251) into M.map, from the slot table, the
+// built lists and the culling's flags -- the rules of the host loops of icg_ba_marginalize_resident_culled and marginalize_body (ba_keyframe.cu):
+//   a landmark is bad when lm_outlier is set or an outlier observation lies in its reference node; an outlier observation drops its factor;
+//   a factor of a bad landmark or observed at a node out of the map drops; every other factor is in the set (the chi-square activity plays
+//   no part).  Touched: the landmark, observing and reference node of every factor in the set with f_ref < num_marg, OR the camera side's
+//   flags the host staged.  Columns [pose_k, mix_k (k < num_marg), touched landmarks ascending | pose_k, mix_k (k >= num_marg), ext, td].
+// An observation whose factor is outside [-1, F) or is not a factor of its landmark and node is counted in out[3] (the host then rejects
+// the call).  lm_col serves as the landmark flags first: 1 bad, 2 touched (a touched landmark is never bad: its factors are in the set).
+__global__ void __launch_bounds__(MARG_SEL_THREADS) marg_select_built(BaCaps C, BaDev D, MargDev M, MargSelArgs a) {
+    __shared__ int s_tp[BA_MAX_NODES], s_tm[BA_MAX_NODES], s_warp[MARG_SEL_THREADS / 32], s_bad, s_vis, s_base;
+    const int w = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const WinDims dm = D.dims[w];
+    const MargSelWin &W = a.win[w];
+    const int K = dm.K, L = dm.L, F = dm.F, nm = W.num_marg;
+    int *map = M.map + (size_t) w * M.map_stride;
+    int *pose_col = map + MARG_MAP_HDR, *mix_col = pose_col + C.K, *lm_col = mix_col + C.K;
+    uint8_t *mask = a.fmask + (size_t) w * C.F;
+    int *ftab = a.ftab + (size_t) w * C.F;
+    const int4 *meta = (const int4 *) D.f_meta_s + (size_t) w * C.F;  // (landmark, reference node, observing node, factor id) per slot
+    const int *off = a.off + W.off0;
+    for (int f = tid; f < F; f += blockDim.x) mask[f] = 1;
+    for (int q = tid; q < F; q += blockDim.x) {
+        const int4 mt = meta[q];
+        ftab[mt.w] = mt.x * BA_MAX_NODES + mt.z;
+    }
+    for (int l = tid; l < C.L; l += blockDim.x) lm_col[l] = l < L && a.lm_outlier[W.lm0 + l] ? 1 : 0;
+    for (int k = tid; k < BA_MAX_NODES; k += blockDim.x) s_tp[k] = k < K && W.tp[k], s_tm[k] = k < K && W.tm[k];
+    if (tid == 0) s_bad = 0, s_vis = 0;
+    __syncthreads();
+    // the observations, landmark by landmark (a thread owns its landmark's flag and the factors of its observations)
+    for (int l = tid; l < L; l += blockDim.x) {
+        const int ref = a.ref[W.lm0 + l], ob = W.obs0 + off[l], oe = W.obs0 + off[l + 1];
+        int bad = 0, invalid = 0;
+        for (int o = ob; o < oe; o++) {
+            const int f = a.fac[o], k = a.node[o];
+            if (f < -1 || f >= F || (f >= 0 && ftab[f] != l * BA_MAX_NODES + k)) {
+                invalid++;
+                continue;
+            }
+            if (!a.obs_outlier[o]) continue;
+            if (k == ref) bad = 1;
+            if (f >= 0) mask[f] = 0;
+        }
+        if (bad) lm_col[l] = 1;
+        if (invalid) atomicAdd(&s_bad, invalid);
+    }
+    __syncthreads();
+    for (int q = tid; q < F; q += blockDim.x) {
+        const int4 mt = meta[q];
+        if (lm_col[mt.x] == 1 || !W.in_map[mt.z]) mask[mt.w] = 0;
+    }
+    __syncthreads();
+    // touched blocks (every writer of an entry stores the same value)
+    for (int q = tid; q < F; q += blockDim.x) {
+        const int4 mt = meta[q];
+        if (!mask[mt.w] || mt.y >= nm) continue;
+        lm_col[mt.x] = 2, s_tp[mt.z] = 1, s_tp[mt.y] = 1, s_vis = 1;
+    }
+    __syncthreads();
+    if (tid == 0) {
+        int idx = 0;
+        for (int k = 0; k < nm; k++) {
+            if (s_tp[k]) idx += 6;
+            if (s_tm[k]) idx += 9;
+        }
+        s_base = idx;
+    }
+    __syncthreads();
+    // landmark columns: an exclusive prefix count of the touched landmarks in ascending id, chunk by chunk
+    for (int l0 = 0; l0 < C.L; l0 += blockDim.x) {
+        const int l = l0 + tid;
+        const int t = l < L && lm_col[l] == 2;
+        int incl = t;
+        for (int d = 1; d < 32; d <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, incl, d);
+            if (lane >= d) incl += y;
+        }
+        if (lane == 31) s_warp[warp] = incl;
+        __syncthreads();
+        int before = s_base;
+        for (int v = 0; v < warp; v++) before += s_warp[v];
+        if (l < C.L) lm_col[l] = t ? before + incl - 1 : -1;
+        __syncthreads();
+        if (tid == blockDim.x - 1) s_base = before + incl;
+        __syncthreads();
+    }
+    if (tid != 0) return;
+    int idx = 0;
+    for (int k = 0; k < C.K; k++) pose_col[k] = mix_col[k] = -1;
+    for (int k = 0; k < nm; k++) {
+        if (s_tp[k]) pose_col[k] = idx, idx += 6;
+        if (s_tm[k]) mix_col[k] = idx, idx += 9;
+    }
+    idx = s_base;
+    const int m = idx;
+    int *out = a.out + (size_t) w * (MARG_SEL_HDR + 2 * C.K), *blk = out + MARG_SEL_HDR;
+    int nb = 0;
+    for (int k = nm; k < K; k++) {
+        if (s_tp[k]) pose_col[k] = idx, idx += 6, blk[nb++] = 0 | (k - nm) << 2;
+        if (s_tm[k]) mix_col[k] = idx, idx += 9, blk[nb++] = 1 | (k - nm) << 2;
+    }
+    int ext_col = -1, td_col = -1;
+    if (W.ext || s_vis) ext_col = idx, idx += 6, blk[nb++] = 2;
+    if (W.td || s_vis) td_col = idx, idx += 1, blk[nb++] = 3;
+    // a reprojection factor always carries ext and td columns; give them (unused) columns when only camera factors exist
+    if (ext_col < 0) ext_col = 0;
+    if (td_col < 0) td_col = 0;
+    map[0] = m, map[1] = idx - m, map[2] = idx, map[3] = nm, map[4] = ext_col, map[5] = td_col, map[6] = map[7] = 0;
+    out[0] = m, out[1] = idx - m, out[2] = nb, out[3] = s_bad, out[4] = out[5] = out[6] = out[7] = 0;
+}
+
 // H0, b0 of constructEquation.  One CTA per window; every stage has one writer per entry, stages are separated by barriers.
 __global__ void __launch_bounds__(256) marg_assemble(BaCaps C, BaDev D, MargDev M) {
     extern __shared__ double smem[];

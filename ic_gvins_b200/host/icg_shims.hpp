@@ -301,6 +301,11 @@ public:
             return icg_ba_marginalize_resident_culled(h_, 1, &problem, nm, &culled, &node_in_map, o);
         });
     }
+    // The same after updateAndCullBuilt, with the factor set and the column map built on the device (icg_ba_marginalize_built): problem needs
+    // its camera side only (f_lm / f_ref / f_obs / f_active / invdepth may be NULL), node_in_map = K flags.  Single-GPU solvers only.
+    Prior marginalizeBuilt(const icg_ba_problem &problem, int num_marg, const uint8_t *node_in_map) {
+        return marginalize(problem, num_marg, [&](const int32_t *nm, icg_ba_prior *o) { return icg_ba_marginalize_built(h_, 1, &problem, nm, &node_in_map, o); });
+    }
 
     // updateParametersFromOptimizer + gvinsOutlierCulling (IG/ic_gvins.cc:1232-1236) on the window this solver just optimised: io carries the
     // observation lists the caller gathered and receives pose_b_c_ / td_b_c_, every node's frame->pose(), every landmark's pos() / depth and

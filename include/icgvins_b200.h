@@ -599,6 +599,26 @@ int icg_ba_update_and_cull_resident(icg_ba *h, int n_windows, const icg_ba_probl
 int icg_ba_marginalize_resident_culled(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg,
                                        const icg_ba_cull_window *culled, const uint8_t *const *node_in_map, icg_ba_prior *out);
 /*
+ * icg_ba_marginalize_resident_culled on the current icg_ba_update_and_cull_built culling of these n_windows, with its factor set and column
+ * map built on the device (marg_select_built) from the handle's slot table, the built lists and the culling's flags, so that no landmark- or
+ * factor-sized array is read on the host or crosses PCIe: the host holds only the camera side of its windows.
+ * problems[w]: K, L, the camera side (n_imu, GNSS nodes, the first-window priors, the previous prior's block table) and pose / mix / ext
+ * (x0 is copied from them); invdepth, f_lm, f_ref, f_obs, f_const and f_active are not read and may be NULL.  node_in_map: K bytes per
+ * window.  Up: one 120-byte record per window (the built lists' offsets, num_marg, node_in_map and the blocks the camera-side factors
+ * touch); down: 8 + 2 max_K ints per window (m, r and the remained block table), one synchronisation, then the launches and the prior's
+ * copies of icg_ba_marginalize_resident_culled.
+ * Outputs: those of icg_ba_marginalize_resident_culled on the same culling, bit for bit (the same factor set, the same columns, the same
+ * eigensolver kernels); the prior becomes the resident one, so that a slide with prior_from_marg consumes it.  Synchronous.
+ * ICG_EINVAL, with the handle unchanged (the culling, the built lists and the last resident prior stay current): no icg_ba_update_and_cull_built
+ * culling of these n_windows is current (none, a host-list culling, or an upload or slide since), n_windows is not the uploaded count,
+ * problems[w].K / L differ from the culled window's, num_marg or the output arrays as icg_ba_marginalize rejects them, or an observation of
+ * the built lists names a factor outside [-1, F) or one of another landmark or node.
+ * ICG_EUNSUPPORTED, the handle unchanged: a marginalized or remained block above 512 rows; a landmark-sharded handle (its group marginalizes
+ * with icg_ba_marginalize_resident_culled and NULL lists after icg_ba_shard_update_and_cull_built).
+ */
+int icg_ba_marginalize_built(icg_ba *h, int n_windows, const icg_ba_problem *problems, const int32_t *num_marg, const uint8_t *const *node_in_map,
+                             icg_ba_prior *out);
+/*
  * icg_ba_update_and_cull_resident on the observation lists the last icg_ba_slide_vision_resident built on the device, so that no list crosses
  * PCIe.  The reference only appends to MapPoint::observations_ (tracking.cc:437 a tracked frame, :771 then :778 a new point's current and
  * reference frames), its walk only skips entries (:1061-1069: outlier features, frames not in the map) and a landmark's reference never
